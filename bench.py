@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py -- k-mers/s scanned by the hetmers hot path on B200 (BASELINE.json metric).
+"""bench.py -- k-mers/s scanned by the hetmers hot path on an H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            our CUDA path
   python bench.py --impl reference ...                     the reference's own C hetmers on host cores
+  python bench.py ... --dump-outputs DIR                   also write the last timed step's plot to DIR/plot.npy
 
 A "step" is one full scan (pass 1 + degree exchange + pass 2 + plot reduce = T_scan of SURVEY.md
 §8d) of one synthetic FastK table.  Workload = BASELINE.json configs[1]: synthetic diploid k=31
@@ -17,13 +18,14 @@ N x 2e8 k-mers, every rank holds a replica and scans a contiguous 1/N index rang
          both kernels + plot D2H
   roofline   dominant kernel (runscan_kernel): it reads every entry once, TBYTE = 10 B/k-mer at k=31
              (the official whole-scan figure of SURVEY §8d, A = 2*TBYTE+2 = 22 B/k-mer over T_scan, is
-             reported next to it as roofline.whole_scan), against MEASURED_PEAKS.json hbm_gbs
+             reported next to it as roofline.whole_scan), against MEASURED_PEAKS.json hbm_gbs when present,
+             else the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s)
   parity     hard gates (non-zero exit): the timed table's plot == the plot of the independent direct
              passes; N > 1: the sharded plot == a one-GPU scan of the same table on rank 0; the .smu
              of our executable == the reference binary's on the same files
   cpu_baseline  the reference C hetmers (oracle/_ref/hetmers; else the oracle port) on the host
              cores, on the SAME table files our executable reads (e2e_exec)
-Inputs (1.9 GB table + 0.27 GB bucket index per 2e8 k-mers) exceed the 126 MB L2, so no flush is
+Inputs (1.9 GB table + 0.27 GB bucket index per 2e8 k-mers) exceed the H100's 50 MB L2, so no flush is
 needed between timed iterations.
 """
 import argparse
@@ -45,7 +47,7 @@ UNIT = "k-mers/s"
 
 
 def _baseline_metric():
-    """the metric string of BASELINE.json (the driver compares against it), else a local default"""
+    """the metric string of BASELINE.json, else a local default"""
     try:
         return json.load(open(os.path.join(ROOT, "BASELINE.json")))["metric"]
     except Exception:
@@ -65,6 +67,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="target CPU time of the baseline sample")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the plot of the last timed step to DIR/plot.npy (float64)")
     return ap.parse_args()
 
 
@@ -76,7 +80,7 @@ def workload_name(n_gpus):
 # ------------------------------------------------------------------------------ clocks ------
 
 class ClockSampler:
-    """SM clock + throttle reasons during the timed region (pynvml; B200_PROFILING.md recipe)."""
+    """SM clock + throttle reasons during the timed region (pynvml)."""
 
     def __init__(self, index=0, period=0.05):
         self.samples, self.reasons, self.max_mhz = [], set(), None
@@ -176,7 +180,7 @@ def time_reference(table, nels, threads, runs=1):
 
 def cpu_sample_size(args, threads):
     # reference arm: survey anchor ~0.45e6 k-mers/s per thread at k=31 (SURVEY.md §6), but the reference stops
-    # scaling near 8-9e6 k-mers/s (measured: 7.8e6/s at -T64 on a B200 host); bounded by the GPU workload
+    # scaling near 8-9e6 k-mers/s at -T64; bounded by the GPU workload
     n = min(0.45e6 * threads, 9e6) * args.cpu_seconds
     return int(max(2e6, min(n, args.nels)))
 
@@ -186,7 +190,7 @@ def bench_config(world):
     in the line's `run` object; the reference arm's bounded sample in `cpu_baseline.sample`)"""
     return {"workload": workload_name(world), "k": K, "ploidy": PLOIDY, "het": HET, "cov": COV, "L": LCUT, "seed": SEED,
             "target_nels_per_gpu": 2e8,
-            "l2": "inputs (>= 1.9 GB table + bucket index per GPU) exceed the 126 MB L2; no flush between iterations"}
+            "l2": "inputs (>= 1.9 GB table + bucket index per GPU) exceed the 50 MB L2; no flush between iterations"}
 
 
 def run_reference_arm(args):
@@ -232,22 +236,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def measured_traffic(kernel, nels, grid):
-    """dram bytes per launch of `kernel` from the committed ncu --set full capture (profiles/traffic.json),
-    scaled per k-mer.  The record names the launch shape it was captured with: a record of another shape
-    (entries per CTA) is refused rather than quoted."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        j = json.load(open(p))[kernel]
-        if grid is not None and j.get("entries_per_cta") is not None and \
-                abs(nels / grid - j["entries_per_cta"]) > 0.02 * j["entries_per_cta"]:
-            return None
-        return float(j["dram_bytes_per_kmer"]) * nels
-    except Exception:
-        return None
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def run_ours(args):
@@ -336,6 +325,8 @@ def run_ours(args):
         ms_total = ev0.elapsed_time(ev1)
         ms_p1 = sum(a.elapsed_time(b) for a, b in p1) / args.steps
         timed_plot = plot.clone()
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, timed_plot)
         # keep the sampler alive over the e2e region too (more samples under load)
         e2e = None
         if multi:
@@ -387,7 +378,6 @@ def run_ours(args):
     kbytes = TBYTE if path == "symm" else ALGO_BYTES_PER_KMER
     achieved = kbytes * per_launch / (ms_p1 * 1e-3) / 1e9
     whole = ALGO_BYTES_PER_KMER * nels / world / (ms_step * 1e-3) / 1e9
-    grid = (per_launch + 2047) // 2048 if path == "symm" else None
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "u64", "data": "synthetic",
@@ -399,7 +389,6 @@ def run_ours(args):
             "roofline": {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": peak,
                          "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_kmer": kbytes, "ms_per_launch": ms_p1,
-                         "traffic": measured_traffic(kname, per_launch, grid),
                          "note": (kname + " reads every entry (8 B key + 2 B count) exactly once; the second kernel "
                                   "reads candidate records only.  whole_scan = SURVEY §8d's official 22 B/k-mer over T_scan"
                                   if path == "symm" else "22 B/k-mer = SURVEY §8d (two passes)"),
@@ -434,6 +423,16 @@ def run_ours(args):
     if not ok:
         sys.stderr.write("bench.py: PARITY GATE FAILED -- see the \"parity\" object of the JSON line\n")
         sys.exit(3)
+
+
+def dump_outputs(d, plot):
+    """what a caller of the timed scan receives: the int64 plot[1001][501] of (count sum, min count) cells,
+    stored as float64 (exact: every cell is below 2^53)"""
+    import numpy as np
+    from smudgeplot_b200 import _lib
+    os.makedirs(d, exist_ok=True)
+    a = plot.reshape(_lib.SMAX + 1, _lib.PLOT_W).cpu().numpy()
+    np.save(os.path.join(d, "plot.npy"), a.astype(np.float64))
 
 
 def cpu_baseline(args, dev, keys, cnt, timed_plot):

@@ -1,15 +1,15 @@
 /*******************************************************************************************
- * hetmers_b200.h -- C ABI of libhetmers_b200.so, the B200 (sm_100a) implementation of
+ * hetmers_b200.h -- C ABI of libhetmers_b200.so, the H100 (sm_90a) implementation of
  * smudgeplot's `hetmers` hot path.
  *
  * The reference has NO in-process API for this path: its boundary is the `hetmers` executable
- * spawned by smudgeplot's CLI (/root/reference/src/smudgeplot/cli.py:57-72,348-361) and the
+ * spawned by smudgeplot's CLI (src/smudgeplot/cli.py:57-72,348-361) and the
  * whole computation lives in src/lib/PloidyPlot.c + the Kmer_Stream part of src/lib/libfastk.c.
  * The drop-in therefore is our own `hetmers` executable (smudgeplot_b200/host/hetmers_main.c,
  * plain C); this header is the thin layer between that C host (or any FFI: ctypes, cgo, JNI)
  * and the CUDA kernels.  Plain pointers and sizes only; no torch / C++ types.
  *
- * Every entry point names the reference code it replaces (file:line under /root/reference).
+ * Every entry point names the reference code it replaces (file:line in the reference smudgeplot repository).
  * All functions return 0 on success and a negative HM_E* code on failure; hm_last_error()
  * gives the message (thread-local).  There is NO CPU fallback anywhere behind this ABI.
  *

@@ -1,4 +1,4 @@
-"""smudgeplot_b200 -- B200 (sm_100a) implementation of smudgeplot's `hetmers` hot path.
+"""smudgeplot_b200 -- H100 (sm_90a) implementation of smudgeplot's `hetmers` hot path.
 
 The product is native: `lib/libhetmers_b200.so` (CUDA kernels + C ABI, include/hetmers_b200.h) and
 the drop-in executables `bin/hetmers` / `bin/extract_kmer_pairs` (plain C host).  The Python in

@@ -1,10 +1,10 @@
 /*******************************************************************************************
- * hm_kernels.cu -- CUDA kernels (sm_100a) + layer-A entry points of include/hetmers_b200.h.
+ * hm_kernels.cu -- CUDA kernels (sm_90a) + layer-A entry points of include/hetmers_b200.h.
  *
  * One-substitution neighbour search over a sorted, device-resident k-mer table.
  * Integer / memory-bound work: no tensor cores (see DESIGN.md §5 for the roofline).
  *
- * What replaces what (reference file:line under /root/reference/src/lib):
+ * What replaces what (reference file:line under smudgeplot's src/lib):
  *   unpack_records_{tma_,}kernel  Next_Kmer_Entry + Current_Entry   libfastk.c:1159-1176,:1230-1269
  *   bucket_index_kernel     stub index + GoTo_Kmer_Entry       libfastk.c:1320-1409
  *   filter_build_kernel     (none: the merge's "no head has this suffix", PloidyPlot.c:618-643)
@@ -182,7 +182,7 @@ __device__ __forceinline__ int warp_upper_bound_index(const int64_t *__restrict_
  * order, so a tile resolves its prefixes together: every NON-EMPTY bucket that starts inside the tile marks
  * its first record (the tile spans ~90 buckets at 2e8 k-mers: one coalesced pass over that slice of the
  * index), and a max-scan over the 1024 marks hands every record the last bucket that started at or before
- * it.  (One global-memory bisection per record, ~7 dependent loads each, held the kernel at 17 % of HBM.) */
+ * it.  (One global-memory bisection per record would cost ~7 dependent loads each.)                        */
 __global__ void __launch_bounds__(256)
 unpack_records_tma_kernel(const uint8_t *__restrict__ rec, int64_t first,
                           const int64_t *__restrict__ index, int ixlen, int ibyte, int hbyte,
@@ -380,15 +380,16 @@ int hm_build_filter_range(const uint64_t *d_keys, int filter_bits, uint32_t *d_f
                           int64_t i0, int64_t i1, void *stream);
 
 extern "C" int hm_pick_filter_bits(int64_t n)
-{ /* 45..90 filter bits per entry: measured optimum at 2e8 entries is 43..86 (7.6-8.0 ms), 21 costs
-   * +11 % (more survivors), 172 costs +50 % (filter traffic = #probed (position, base) pairs x
-   * filter size: every probe column streams the whole bitmap once)                              */
+{ /* 23..45 filter bits per entry: fewer let more candidates survive to the bucket look-up, more cost
+   * filter traffic (= #probed (position, base) pairs x filter size: every probe column streams the
+   * whole bitmap once).  Pass 1 at 2e8 entries on one H100 SXM (400 W): 2^33 bits (43 per entry)
+   * 14.6 ms, 2^34 17.4 ms, 2^35 26.3 ms                                                          */
   int lg = 0;                                  /* round(log2 n) */
   while (lg < 62 && ((int64_t) 1 << (lg+1)) <= n)
     lg += 1;
   if (lg < 61 && (double) n > 1.41421356 * (double) ((int64_t) 1 << lg))
     lg += 1;
-  int fb = lg+6;
+  int fb = lg+5;
   if (fb < HM_FILTER_MIN_BITS) fb = HM_FILTER_MIN_BITS;
   if (fb > HM_FILTER_MAX_BITS) fb = HM_FILTER_MAX_BITS;
   return fb;
@@ -428,9 +429,8 @@ int hm_build_filter_range(const uint64_t *d_keys, int filter_bits, uint32_t *d_f
 #ifndef P1_GRID_PER_SM
 #define P1_GRID_PER_SM 1024      /* CTAs launched per SM, started in table order, each striding over a few
                                   * groups of 8 chunks.  Few persistent CTAs drift apart and lose the L2
-                                  * reuse of filter sectors between neighbours: 6/SM 8.77 ms, 32/SM 7.65,
-                                  * 96/SM 7.12, 256/SM 6.87, 1024/SM 6.78; one CTA per 8 chunks (no stride)
-                                  * is slower again (~7.3 ms) (2e8 entries)                              */
+                                  * reuse of filter sectors between neighbours: pass 1 at 2e8 entries on
+                                  * one H100 SXM (400 W) 25.9 ms at 32/SM, 21.4 at 256/SM, 17.4 at 1024/SM */
 #endif
 #ifndef P1_MINBLOCKS
 #define P1_MINBLOCKS 6          /* resident CTAs per SM the register budget must allow (40 regs, no spills) */
@@ -553,8 +553,6 @@ pass1_filter_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restric
               if (pmax > kmer-1) pmax = kmer-1;
             }
         }
-      /* (prefetching the next chunk's keys here was measured slower: 8.3 vs 7.5 ms) */
-
       /* ---- low positions: filter probes, branch-free ----
        * candidate = x with base p replaced by c in {1,2,3}; it is wanted iff it is > x (c above
        * the current base).  Survivor bits are shifted into two 32-bit masks in probe order:
@@ -726,7 +724,7 @@ template <typename IdxT, int F, int KW>
 static cudaError_t launch_pass1(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                 const void *bucket, int bits, const uint32_t *filter, int kmer,
                                 int64_t lo, int64_t hi, const DegView &dv, void *up, cudaStream_t st)
-{ int dev = 0, sms = 148;
+{ int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t nchunks = (hi-lo+31)>>5;
@@ -839,7 +837,7 @@ pass2_plot_kernel(const uint16_t *__restrict__ cnt, const DegView dv,
           if (j[u] != IdxNone<IdxT>::value)
             { const uint8_t *pj = (const uint8_t *) deg_words(dv,(int64_t) j[u]);
               if (pj != (const uint8_t *) dv.self)
-                { /* partner owned by another GPU: a ~2 us NVLink round trip.  Park the pair in this
+                { /* partner owned by another GPU: an NVLink round trip.  Park the pair in this
                    * CTA's slice of the defer list; pass2_deferred_kernel resolves all of them with
                    * every remote load in flight at once (inline only when the slice is full)      */
                   unsigned at = dv.defer_cap > 0 ? atomicAdd(&s_defer,1u) : 0xffffffffu;
@@ -906,7 +904,7 @@ extern "C" int hm_k_pass2_plot(const uint16_t *d_cnt, const uint8_t *d_deg, cons
     return hm_set_error(HM_EINVAL,"pass2: bad range");
   if (hi == lo)
     return HM_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   size_t smem = (size_t) P2_TS*P2_TM*sizeof(uint32_t);
@@ -1004,7 +1002,7 @@ extern "C" int hm_k_pass2_extract(const uint64_t *d_keys, const uint64_t *d_keys
     return hm_set_error(HM_EINVAL,"extract: bad range or capacity");
   if (hi == lo)
     return HM_OK;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = (hi-lo+255)/256;
@@ -1045,7 +1043,7 @@ extern "C" int hm_k_min_count(const uint16_t *d_cnt, int64_t frst, int64_t last,
 { if (last <= frst)
     return HM_OK;
   int64_t want = (last-frst+255)/256;
-  int     grid = (int) (want < 148*8 ? want : 148*8);
+  int     grid = (int) (want < 132*8 ? want : 132*8);
   min_count_kernel<<<grid,256,0,(cudaStream_t) stream>>>(d_cnt,frst,last,d_min);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess)

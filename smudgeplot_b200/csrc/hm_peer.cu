@@ -165,7 +165,7 @@ int hm_peer_sum_deg(uint8_t **deg, const int64_t *lo, const int64_t *hi, const i
       if (w0 >= w1) continue;
       HM_CUDA(cudaSetDevice(dev[g]));
       int64_t want = ((w1-w0)/4+255)/256;
-      int     grid = (int) (want < 148*4 ? (want > 0 ? want : 1) : 148*4);
+      int     grid = (int) (want < 132*4 ? (want > 0 ? want : 1) : 132*4);
       peer_sum_deg_kernel<<<grid,256,0,st[g]>>>(P,n,w0,w1);
       cudaError_t e = cudaGetLastError();
       if (e != cudaSuccess) return hm_cuda_fail(e,"peer_sum_deg_kernel");

@@ -6,7 +6,8 @@
  *   hm_scan_examine  trimmed? / symmetric? decisions of examine_table (PloidyPlot.c:1167-1230)
  *   hm_scan_run      pass 1 -> (degree exchange when >1 GPU) -> pass 2 -> plot D2H  ("T_scan")
  *
- * Every device holds a full replica of the table (180 GB HBM3e holds 16e9 k=31 entries); work is
+ * Every device holds a full replica of the table (the symmetric scan needs ~13.4 B per k=31 entry, so
+ * an 80 GB H100 holds ~6e9 entries with its work area); work is
  * sharded by contiguous index range [lo_g, hi_g).  With one GPU there is no exchange at all.
  * With several GPUs in this single process the loader gathers the shards over NVLink peer
  * copies and foreign degree bytes are reached through the owner's array (remote atomics / loads
@@ -86,7 +87,7 @@ int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
 /* Device allocations of a one-GPU scan come from the device's stream-ordered memory pool with a
  * release threshold of "never": a second hm_scan_create in the same process (bench e2e leg, a
  * service handling many tables) reuses the memory instead of paying cudaMalloc / cudaFree of
- * several GB every call (measured: ~20 ms of a 61 ms call).  Multi-GPU scans keep cudaMalloc:
+ * several GB every call.  Multi-GPU scans keep cudaMalloc:
  * their arrays are mapped by the peers.  HETMERS_NO_POOL=1 disables the pool.                  */
 #define POOL_MAX 32
 typedef struct { void *p[POOL_MAX]; int n, enabled; } PoolReg;
@@ -157,7 +158,7 @@ extern "C" void hm_scan_destroy(hm_scan *s)
 }
 
 /* ---- host-side staging for pageable sources (mmap'ed part files) -------------------------
- * cudaMemcpyAsync from pageable memory is staged by the driver on one thread (~3-6 GB/s).  The
+ * cudaMemcpyAsync from pageable memory is staged by the driver on one thread.  The
  * executable's table lives in the page cache, so the loader copies each chunk into a pinned
  * buffer with a few host threads (this is what the reference's -T is for on the host side) while
  * the previous chunk is in flight to the GPU.                                                   */

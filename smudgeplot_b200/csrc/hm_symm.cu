@@ -56,8 +56,9 @@
 #define RS_SCANCAP RS_HALO                     /* longest run half scanned linearly               */
 #define RS_LONGRUN 32                          /* dense kernel: runs of more entries go to runs_kernel */
 #ifndef RS_MINBLOCKS
-#define RS_MINBLOCKS 6                         /* resident CTAs per SM the register budget must allow (40 regs;
-                                                *   4: 1.18 ms, 5: 1.07, 6 with 30 KB of shared memory: 0.99)     */
+#define RS_MINBLOCKS 5                         /* resident CTAs per SM the register budget must allow (48 regs, no
+                                                *   spills).  runscan_kernel at 2e8 entries on one H100 SXM (400 W):
+                                                *   4: 1.18 ms, 5: 1.12, 6 (40 regs): 1.14                          */
 #endif
 #ifndef RS_STAGE
 #define RS_STAGE   384                         /* candidate records staged per CTA before they leave (a 2048-entry
@@ -197,7 +198,7 @@ extern "C" int hm_k_symm_fingerprint(const uint64_t *d_keys, const uint64_t *d_k
   if (i1 <= i0)
     return HM_OK;
   int64_t want = (i1-i0+255)/256;
-  int     grid = (int) (want < 148*16 ? want : 148*16);
+  int     grid = (int) (want < 132*16 ? want : 132*16);
   if (kmer <= 32)
     symm_fingerprint_kernel<1><<<grid,256,0,(cudaStream_t) stream>>>
         (d_keys,NULL,d_cnt,i0,i1,kmer,seed[0],seed[1],(unsigned long long *) d_acc);
@@ -233,14 +234,13 @@ extern "C" void hm_symm_seeds(uint64_t seed[2])
 extern "C" int hm_symm_plan(int64_t n, int64_t range, int kmer, int n_seg, hm_symm_layout *out)
 { if (out == NULL || n < 0 || range < 0 || range > n || n_seg < 1 || n_seg > HM_MAX_SHARDS)
     return hm_set_error(HM_EINVAL,"hm_symm_plan: bad arguments");
-  int bits = 2;                                  /* Bloom bits per table entry (S is ~1/6 of the table; two bits set per
-                                                  *   element): 50 MB at 2e8 entries, kept in L2 by an access-policy
-                                                  *   window (bloom_window).  Without the window its inserts miss L2 in
-                                                  *   pass 1 (+0.55 ms) and 1 bit per entry is the better choice        */
-  if (n_seg > 1)                                 /* several GPUs: all segments together are far beyond L2 and have to
-                                                  *   cross NVLink between the kernels (0.95 ms of a 4.6 ms scan at 8
-                                                  *   GPUs with 2 bits): half the filter, a few more exact checks      */
-    bits = 1;
+  int bits = 1;                                  /* Bloom bits per table entry (S is ~1/6 of the table; two bits set per
+                                                  *   element): 25 MB at 2e8 entries, which the access-policy window
+                                                  *   (bloom_window) can keep in the H100's 50 MB L2.  2 bits (50 MB) halve
+                                                  *   the exact checks of pass 2 but no longer fit: on one H100 SXM
+                                                  *   (400 W) pass 1 took 2.98 ms with 2 bits against 1.53 ms with 1,
+                                                  *   pass 2 0.75 against 0.81 ms.  Several GPUs: the segments also cross
+                                                  *   NVLink between the kernels, one more reason to keep them small     */
   const char *e = getenv("HETMERS_BLOOM_BITS");
   if (e != NULL && atoi(e) >= 1 && atoi(e) <= 64)
     bits = atoi(e);
@@ -552,9 +552,9 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
 
 /* Pass 1.  83 % of the entries of a genome-sized table are alone in their run (no other entry shares
  * their first k/2 bases) and 15 % sit in a run of exactly two -- almost always the two alleles of one
- * heterozygous site.  The kernel is bound by instruction issue and by the latency of its few serial
- * phases, not by bytes (55 warp instructions per 32 entries is all a B200 can issue while HBM delivers
- * them), so the common cases are loop-free and, once the tile has landed, every WARP works on its own
+ * heterozygous site.  The kernel is limited by instruction issue and by the latency of its few serial
+ * phases as much as by bytes (an H100 SXM issues about 100 warp instructions per 32 entries in the time
+ * its 3.35 TB/s deliver them), so the common cases are loop-free and, once the tile has landed, every WARP works on its own
  * 256 entries without any CTA barrier:
  *   1. adjacency bits: eq[i] = slots i, i+1 belong to one run (one ballot per 32 slots; a warp computes
  *      the ten words it needs itself and keeps them one per lane)
@@ -565,11 +565,10 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
  *      takes them one per thread afterwards
  *   5. candidate records and run heads are staged in shared memory; the LAST warp to finish moves
  *      them out with one global atomic per CTA and list (one per record, or per warp, on the one
- *      list counter serialises in L2: 9.2 ms for 1.8e7 records)
- * (Scanning every entry's run in place cost 436 warp instructions per 32 entries at 34 % lane
- * utilisation; per-entry classification with predicated list writes 163; CTA-wide task lists with a
- * barrier per phase 117, but 57 % of the stall samples at those barriers; longer runs handled by
- * single lanes of every warp in place: slower again.)                                               */
+ *      list counter serialises in L2)
+ * (The alternatives -- every entry scanning its run in place, per-entry classification with predicated
+ * list writes, CTA-wide task lists with a barrier per phase, longer runs handled by single lanes of
+ * every warp in place -- need more instructions, leave more lanes idle or wait at the barriers.)      */
 template <typename IdxT, int KW>
 __global__ void __launch_bounds__(RS_THREADS,RS_MINBLOCKS)
 runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
@@ -785,9 +784,8 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
  * partner; after a barrier every entry of the tile reads its own counts: Bloom insert if it has an
  * upper partner, candidate record if it and its single partner have one partner each.  All pairs of a
  * run are compared exactly once, the comparisons are spread evenly over the lanes, and the cost grows
- * with the run length instead of falling off a cliff (the one-thread-per-run kernel took 9.2 ms per
- * 2.5e8 entries at 2e9 k-mers, 377 ms per 6.25e8 at 5e9).  Runs of more than RS_LONGRUN entries are
- * listed for runs_kernel as before.                                                                   */
+ * with the run length instead of falling off a cliff as one thread per run does.  Runs of more than
+ * RS_LONGRUN entries are listed for runs_kernel as before.                                            */
 template <typename IdxT, int KW>
 __global__ void __launch_bounds__(RS_THREADS,RS_MINBLOCKS)
 runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
@@ -1055,8 +1053,7 @@ template <typename IdxT, int KW>
 static cudaError_t launch_runs(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                const void *bucket, int bits, int kmer, int64_t lo, int64_t hi,
                                const SymmView &W, cudaStream_t st)
-{ /* (building the Bloom filter from the record list in a kernel of its own instead of inside runscan_kernel
-   *  was measured slower: +0.15 ms)                                                                        */
+{ /* (the Bloom filter is filled inside runscan_kernel: a kernel of its own would read the records once more) */
   int64_t want = ((hi-lo)/64+255)/256;                        /* ~1 run of three or more per 60 entries: a thread each */
   int     grid = (int) (want < 0x7fffffff ? (want > 0 ? want : 1) : 0x7fffffff);
   runs_kernel<IdxT,KW><<<grid,256,0,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,lo,hi,W);
@@ -1330,7 +1327,7 @@ static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo,
                                   unsigned long long *plot, int64_t range, cudaStream_t st)
 { static int configured[64] = {0};                            /* per instantiation */
   size_t smem = (size_t) RV_TS*RV_TM*sizeof(uint32_t);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (dev >= 64 || !configured[dev])
     { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);

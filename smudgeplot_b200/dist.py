@@ -69,8 +69,8 @@ def gather_table(local_keys: torch.Tensor, local_cnt: torch.Tensor, group=None, 
                  local_lo: torch.Tensor | None = None, out_lo: torch.Tensor | None = None):
     """Assemble the full sorted table on every rank from per-rank shards (shard r = rank r's
     slice of the key space, so concatenation in rank order is the sorted table): the shards are evened
-    out by small point-to-point copies and then ONE all-gather per array moves everything (round 1 did
-    3 x world sequential broadcasts: 45 ms of a 95 ms end-to-end step at 8 GPUs).
+    out by small point-to-point copies and then ONE all-gather per array moves everything (instead of
+    3 x world sequential broadcasts).
     -> (keys_full, cnt_full, lo, hi) with [lo,hi) this rank's index range; with `local_lo` (second
     key word, k > 32) -> (keys_full, cnt_full, lo, hi, keys_lo_full).
     `out` buffers are used in place when they have room for world*ceil(total/world) elements."""
@@ -147,8 +147,7 @@ def balanced_offsets(keys_full: torch.Tensor, world: int, depth: int = 3, per_ca
     Only neighbours y > x are probed, so an entry with base b at position p has 3-b candidates
     there ('a' three, 't' none) -- each ~3 % of an entry's cost.  For the first `depth` bases that
     number is the same for whole stretches of the sorted table, so shards cut by count are
-    systematically uneven (measured at 8 GPUs: 9.8 vs 8.3 ms with equal counts; 9.4 vs 8.7 ms when
-    only the first base is weighted).  The table is split into the 4^depth prefix classes, each
+    systematically uneven.  The table is split into the 4^depth prefix classes, each
     weighted by its candidate count, and the cuts are placed on the cumulative weight."""
     n = keys_full.numel()
     if world <= 1:

@@ -1,6 +1,6 @@
 """FastK ``.ktab`` table files: host-side reader and writer (numpy only).
 
-Layout as the reference reads it (``/root/reference/src/lib/libfastk.c:786-908`` Open_Kmer_Stream,
+Layout as the reference reads it (``src/lib/libfastk.c:786-908`` of smudgeplot, Open_Kmer_Stream,
 ``:1230-1269`` Current_Entry; SURVEY.md Appendix A), all little-endian host ints:
 
 * stub ``<dir>/<root>.ktab``: ``int32 kmer, nparts, minval, ibyte`` then

@@ -3,7 +3,7 @@
 Reference interface (the only one this path has): ``smudgeplot hetmers -L <cutoff> -t <threads>
 -o <prefix> [--verbose] [-tmp <dir>] <FastK_Table>`` builds ``["-o<o>", "-e<L>", "-T<t>", ("-v"),
 ("-P<tmp>" iff tmp != "."), infile]`` and spawns the ``hetmers`` binary
-(/root/reference/src/smudgeplot/cli.py:57-72, 348-361).  `hetmers_args` + `run_hetmers` reproduce
+(smudgeplot's src/smudgeplot/cli.py:57-72, 348-361).  `hetmers_args` + `run_hetmers` reproduce
 exactly that against OUR executable (smudgeplot_b200/bin/hetmers); `scan_table` / `Scan` are the
 in-process route through the same C ABI (include/hetmers_b200.h layer B) for callers that already
 hold the table in host memory.  Everything computes on the GPU; there is no fallback.

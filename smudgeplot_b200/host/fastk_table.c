@@ -2,7 +2,7 @@
  * fastk_table.c -- layer C of include/hetmers_b200.h: FastK .ktab stub/part parser and the
  * .smu writer.  Plain C host code, no CUDA.
  *
- * Restates what Open_Kmer_Stream does with the files (/root/reference/src/lib/libfastk.c
+ * Restates what Open_Kmer_Stream does with the files (smudgeplot's src/lib/libfastk.c
  * :786-908): stub = int32 kmer,nparts,minval,ibyte + int64 index[1<<(8*ibyte)]; hidden part
  * files ".<root>.ktab.<p>" = int32 kmer, int64 n, then n records of kbyte-ibyte+2 bytes.
  * Unlike the reference (1024-entry read() buffers, :749-784) the part payloads are mapped whole

@@ -1,11 +1,11 @@
 /*******************************************************************************************
  * hetmers_main.c -- the drop-in `hetmers` executable (plain C host; all compute is CUDA behind
  * include/hetmers_b200.h).  Same process boundary as the reference binary that smudgeplot's CLI
- * spawns (/root/reference/src/smudgeplot/cli.py:57-72,348-361):
+ * spawns (smudgeplot's src/smudgeplot/cli.py:57-72,348-361):
  *
  *     hetmers [-v] [-T<int(4)>] [-P<dir(/tmp)>] [-o<output>] [-e<int(4)>] <source>[.ktab]
  *
- * mirrors main() of /root/reference/src/lib/PloidyPlot.c:1232-1630: argv grammar and messages
+ * mirrors main() of smudgeplot's src/lib/PloidyPlot.c:1232-1630: argv grammar and messages
  * (gene_core.h:32-56 ARG_* macros), default output root, the "Found het-table" prompt, the
  * trimmed/symmetric examination (un-conditioned tables are trimmed / symmetrised on the GPU;
  * HETMERS_EXTERNAL_CONDITIONING=1 restores the reference's shell-outs to FastK's Logex/Symmex/Fastrm), the verbose

@@ -1,11 +1,11 @@
 #!/usr/bin/env python3
 """Regenerate tests/golden/: seeded synthetic FastK tables + the .smu the UNMODIFIED reference
-`hetmers` (oracle/_ref/hetmers, built from /root/reference by oracle/Makefile) writes for them.
+`hetmers` (oracle/_ref/hetmers, built from the reference sources by oracle/Makefile) writes for them.
 
 The reference ships no golden vectors for this path (SURVEY.md §4), so these files ARE the pin:
 tests/test_oracle.py requires oracle/hetmers_oracle.c to reproduce each .smu byte for byte, and
-the -m gpu tests require the CUDA path to do the same.  Run from the repo root, in the build
-container (needs /root/reference):   python tests/golden/make_golden.py
+the -m gpu tests require the CUDA path to do the same.  Run from the repo root once oracle/_ref/ is
+built:   python tests/golden/make_golden.py
 """
 import json
 import os
@@ -67,7 +67,7 @@ def run_ref(table, out, e, threads=4):
 
 def main():
     if not os.path.exists(REF):
-        sys.exit("oracle/_ref/hetmers missing: run `make -C oracle` where /root/reference exists")
+        sys.exit("oracle/_ref/hetmers missing: run `make -C oracle REF=<reference checkout>`")
     meta = {}
     for name, c in CASES.items():
         d = os.path.join(HERE, name)

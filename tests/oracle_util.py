@@ -49,6 +49,43 @@ def run_ref_extract(table: str, sma: str, out_root: str, ethresh: int, threads: 
                           capture_output=True, text=True)
 
 
+REF_RUNS = os.path.join(ROOT, "tests", "golden", "reference_runs")
+
+
+def reference_run_name(kind: str, k: int, seed: int) -> str:
+    return f"{kind}_k{k}_s{seed}.smu"
+
+
+def reference_smu(kind: str, k: int, seed: int) -> str:
+    """the .smu the reference binary wrote for a seeded test table (tests/golden/make_reference_runs.py)"""
+    with open(os.path.join(REF_RUNS, reference_run_name(kind, k, seed))) as f:
+        return f.read()
+
+
+def reference_pair_digests(k: int, seed: int):
+    import json
+    with open(os.path.join(REF_RUNS, "extract.json")) as f:
+        return json.load(f)[f"k{k}_s{seed}"]
+
+
+def pair_digests(pairs):
+    """{label: [number of lines, SHA-256 of the sorted lines]} of sorted_pair_files()"""
+    import hashlib
+    return {lab: [len(lines), hashlib.sha256("".join(ln + "\n" for ln in lines).encode()).hexdigest()]
+            for lab, lines in pairs.items()}
+
+
+def first_pair_difference(got, want) -> str:
+    """the first smudge whose sorted pair lines differ, with line counts and the first differing line"""
+    for lab in sorted(set(got) | set(want)):
+        a, b = got.get(lab, []), want.get(lab, [])
+        if a != b:
+            i = next((j for j, (x, y) in enumerate(zip(a, b)) if x != y), min(len(a), len(b)))
+            return (f"smudge {lab}: {len(a)} lines, expected {len(b)}; first difference at sorted line {i}: "
+                    f"{a[i] if i < len(a) else '<end>'!r} != {b[i] if i < len(b) else '<end>'!r}")
+    return "no difference"
+
+
 def sorted_pair_files(out_root: str):
     """{label: sorted lines} of every <out_root>.<a>A<b>B.txt (the reference's line order depends on its
     thread schedule, so pair lists are compared as sorted multisets)"""

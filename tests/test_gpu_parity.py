@@ -1,8 +1,8 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Everything goes through the C ABI of
+"""GPU parity tests (run with -m gpu on an H100).  Everything goes through the C ABI of
 libhetmers_b200.so (in-process via ctypes, or through the drop-in `hetmers` executable) and is
 compared bit for bit with (a) the golden .smu files written by the unmodified reference binary,
-(b) the oracle on seeded tables, (c) the reference binary itself when oracle/_ref/hetmers is
-present, and (d) size-independent properties at BASELINE.json's full size."""
+(b) the oracle on seeded tables, (c) what the reference binary wrote for larger seeded tables
+(tests/golden/reference_runs/), and (d) size-independent properties at BASELINE.json's full size."""
 import os
 import shutil
 import subprocess
@@ -89,29 +89,39 @@ def test_extract_executable_reproduces_reference_pair_lists(name, golden_meta, t
     assert ou.sorted_pair_files(out) == _golden_pairs(name)
 
 
-@pytest.mark.parametrize("k,G,ploidy,seed,L", [(31, 400000, 3, 41, 12), (40, 150000, 2, 42, 4)])
+EXTRACT_CASES = [(31, 400000, 3, 41, 12), (40, 150000, 2, 42, 4)]   # k, G, ploidy, seed, L
+
+
+def write_labelled_sma(plot, sma):
+    """label three quarters of the plot's pixels with smudges (by (sum + min) mod 4) and write them as a
+    .sma; -> (pixel -> 1-based smudge index map, smudge names in index order)"""
+    s_idx, m_idx = np.nonzero(plot[:, :_lib.FMAX] > 0)
+    pix = np.zeros((_lib.SMAX + 1, _lib.PLOT_W), dtype=np.uint16)
+    labels = ["1A1B", "2A1B", "2A2B"]
+    order = []
+    with open(sma, "w") as f:
+        f.write("covB\tcovA\tfreq\tsmudge\n")
+        for s, m in zip(s_idx.tolist(), m_idx.tolist()):
+            lab = (s + m) % 4
+            if lab < 3:
+                if labels[lab] not in order:
+                    order.append(labels[lab])
+                pix[s, m] = order.index(labels[lab]) + 1
+                f.write(f"{m}\t{s - m}\t{plot[s, m]}\t{labels[lab]}\n")
+    return pix, order
+
+
+@pytest.mark.parametrize("k,G,ploidy,seed,L", EXTRACT_CASES)
 def test_extract_matches_reference_binary_and_inprocess_list(k, G, ploidy, seed, L, tmp_path):
     """bigger seeded table: our extract_kmer_pairs vs the reference's (sorted lines), and the
     in-process pair list (hm_scan_extract) vs the files"""
     keys, cnt = synth.synth_table(k, G, ploidy, 0.02, 20 * ploidy, L, seed, device="cuda")
     name = str(tmp_path / "t")
     kt = synth.write_table(name, k, keys, cnt, ibyte=3, nparts=3)
+    sma = str(tmp_path / "ann.sma")
     with hetmers.Scan(kt) as sc:
         plot, _ = sc.run()
-        s_idx, m_idx = np.nonzero(plot[:, :_lib.FMAX] > 0)
-        pix = np.zeros((_lib.SMAX + 1, _lib.PLOT_W), dtype=np.uint16)
-        labels = ["1A1B", "2A1B", "2A2B"]
-        sma = str(tmp_path / "ann.sma")
-        with open(sma, "w") as f:
-            f.write("covB\tcovA\tfreq\tsmudge\n")
-            order = []
-            for s, m in zip(s_idx.tolist(), m_idx.tolist()):
-                lab = (s + m) % 4
-                if lab < 3:
-                    if labels[lab] not in order:
-                        order.append(labels[lab])
-                    pix[s, m] = order.index(labels[lab]) + 1
-                    f.write(f"{m}\t{s - m}\t{plot[s, m]}\t{labels[lab]}\n")
+        pix, order = write_labelled_sma(plot, sma)
         rec = sc.extract(pix)
     assert len(rec) == int(plot[pix > 0].sum())                       # one record per labelled isolated pair
     out = str(tmp_path / "kp")
@@ -122,17 +132,16 @@ def test_extract_matches_reference_binary_and_inprocess_list(k, G, ploidy, seed,
     def fmt(r):
         bases = [((int(r["key_hi"]) if p < 32 else int(r["key_lo"])) >> (62 - 2 * (p & 31))) & 3 for p in range(k)]
         return "".join(f"({dna[b]}/{dna[int(r['alt'])]})" if p == int(r["pos"]) else dna[b] for p, b in enumerate(bases))
-    mine = {}
     for r in rec[:: max(1, len(rec) // 2000)]:                        # spot-check the in-process records
         assert fmt(r) in ours[order[int(r["smudge"]) - 1]]
-    if ou.have_ref_extract():
-        rr = ou.run_ref_extract(name, sma, str(tmp_path / "ref"), L, threads=min(os.cpu_count() or 4, 64))
-        assert rr.returncode == 0, rr.stderr
-        assert ou.sorted_pair_files(str(tmp_path / "ref")) == ours
-    else:
+    want = ou.reference_pair_digests(k, seed)                            # the reference binary's lists
+    if ou.pair_digests(ours) != want:
+        # only digests are stored: let the oracle (pinned to the reference's lists by test_oracle.py) show
+        # which lines differ
         assert ou.oracle_extract(name, L, sma, str(tmp_path / "ora")) == 0
-        assert ou.sorted_pair_files(str(tmp_path / "ora")) == ours
-    del mine
+        ora = ou.sorted_pair_files(str(tmp_path / "ora"))
+        assert ou.pair_digests(ora) == want, "the oracle's pair lists differ from the stored reference digests too"
+        pytest.fail(ou.first_pair_difference(ours, ora))
 
 
 # ------------------------------------------------------------------ conditioning verdicts ----
@@ -154,6 +163,19 @@ def test_examine_table_decisions(name, verdict, tool, golden_meta, tmp_path):
     if shutil.which(tool) is None:
         want = c["stderr_tail"][0].replace("/root/repo/tests/golden", GOLDEN)
         assert want in r.stderr                                         # "hetmers: Command '...' failed"
+
+
+def canonical_mask(keys, ku, k):
+    """x <= rc(x) for every key of a synth_table() (torch keys, their uint64 view ku)"""
+    import torch
+    if k > 32:
+        rh, rl = synth.revcomp_long(keys[:, 0].contiguous(), keys[:, 1].contiguous(), k)
+        rcb = fastk.keys_u64_to_bytes(torch.stack([rh, rl], 1).numpy().view(np.uint64), k)
+    else:
+        rcb = fastk.keys_u64_to_bytes(synth.revcomp_left(keys, k).numpy().view(np.uint64), k)
+    kb = fastk.keys_u64_to_bytes(ku, k)
+    w = kb.shape[1]
+    return kb.view(f"S{w}").reshape(-1) <= rcb.view(f"S{w}").reshape(-1)
 
 
 def _condition_numpy(ku, cn, k, L, trim, symm):
@@ -182,8 +204,11 @@ def _condition_numpy(ku, cn, k, L, trim, symm):
     return ku, cn
 
 
-@pytest.mark.parametrize("k,G,ploidy,seed,L", [(21, 60000, 2, 31, 6), (31, 80000, 3, 32, 12), (32, 50000, 2, 33, 5),
-                                               (40, 50000, 2, 34, 6), (12, 30000, 2, 35, 12)])
+CONDITIONING_CASES = [(21, 60000, 2, 31, 6), (31, 80000, 3, 32, 12), (32, 50000, 2, 33, 5),   # k, G, ploidy, seed, L
+                      (40, 50000, 2, 34, 6), (12, 30000, 2, 35, 12)]
+
+
+@pytest.mark.parametrize("k,G,ploidy,seed,L", CONDITIONING_CASES)
 def test_gpu_conditioning_of_canonical_untrimmed_table(k, G, ploidy, seed, L, tmp_path):
     """a FastK-style table (canonical k-mers only, every count >= 1) is trimmed and symmetrised on
     the GPU; the .smu must equal what the REFERENCE binary writes for the table conditioned by the
@@ -191,15 +216,7 @@ def test_gpu_conditioning_of_canonical_untrimmed_table(k, G, ploidy, seed, L, tm
     keys, cnt = synth.synth_table(k, G, ploidy, 0.02, 40, 1, seed)          # untrimmed: counts from 1
     ku = synth.keys_to_u64_numpy(keys)
     cn = cnt.numpy().astype(np.uint16)
-    import torch
-    if k > 32:
-        rh, rl = synth.revcomp_long(keys[:, 0].contiguous(), keys[:, 1].contiguous(), k)
-        rcb = fastk.keys_u64_to_bytes(torch.stack([rh, rl], 1).numpy().view(np.uint64), k)
-    else:
-        rcb = fastk.keys_u64_to_bytes(synth.revcomp_left(keys, k).numpy().view(np.uint64), k)
-    kb = fastk.keys_u64_to_bytes(ku, k)
-    w = kb.shape[1]
-    canon = kb.view(f"S{w}").reshape(-1) <= rcb.view(f"S{w}").reshape(-1)   # x <= rc(x)
+    canon = canonical_mask(keys, ku, k)
     raw = str(tmp_path / "raw")
     fastk.write_ktab(raw, k, ku[canon], cn[canon], ibyte=3, nparts=3)
     out = str(tmp_path / "gpu")
@@ -212,16 +229,7 @@ def test_gpu_conditioning_of_canonical_untrimmed_table(k, G, ploidy, seed, L, tm
                         "\n  Starting to count covariant pairs\n"
                         "\n  Count complete, outputting table\n")
     ck, cc = _condition_numpy(ku[canon], cn[canon], k, L, True, True)
-    cond = str(tmp_path / "cond")
-    fastk.write_ktab(cond, k, ck, cc, ibyte=3, nparts=2)
-    if ou.have_ref():
-        rr = ou.run_ref(cond, str(tmp_path / "ref"), L, threads=4, verbose=True)
-        assert rr.returncode == 0 and "trimmed and symmetric" in rr.stderr, rr.stderr
-        want = open(str(tmp_path / "ref.smu")).read()
-    else:
-        rc, trim, symm, _ = ou.oracle_file(cond, L, str(tmp_path / "ora.smu"))
-        assert (rc, trim, symm) == (0, 1, 1)
-        want = open(str(tmp_path / "ora.smu")).read()
+    want = ou.reference_smu("conditioned", k, seed)                    # the reference binary on (ck, cc)
     assert open(out + ".smu").read() == want and len(want) > 0
     # in-process route + the conditioned table itself
     with hetmers.Scan(fastk.read_ktab(raw)) as sc:
@@ -335,7 +343,7 @@ def test_result_independent_of_bucket_bits_and_work_split():
 
 @pytest.mark.parametrize("k", [31, 40])
 def test_64bit_offset_kernels_match_32bit(k):
-    """tables with >= 2^32 entries (BASELINE configs[4]: 5e9) use uint64 bucket offsets / partner
+    """tables with >= 2^32 entries (BASELINE configs[4]: 4.4e9) use uint64 bucket offsets / partner
     indices; force those kernel instantiations on a small table and compare with the uint32 ones"""
     import torch
     from smudgeplot_b200.device import DeviceTable
@@ -390,7 +398,7 @@ def test_long_kmer_work_split_and_filter_widths():
     assert bool((pos >= 0).all())                       # symmetric table: every reverse complement is found
 
 
-@pytest.mark.parametrize("k,target,ploidy,het,cov,L,seed,ref_threads", [
+MEDIUM_CASES = [  # k, target, ploidy, het, cov, L, seed, -T of the reference run (0: all cores up to 64)
     (21, 1_000_000, 2, 0.01, 40, 4, 1, 1),        # BASELINE configs[0]: reference C hetmers on 1 CPU thread
     (31, 20_000_000, 2, 0.01, 40, 12, 2, 0),      # configs[1] at 1/10 of the bench size
     (31, 30_000_000, 4, 0.01, 40, 12, 3, 0),      # stand-in for configs[2] (the real S. cerevisiae table needs
@@ -398,7 +406,10 @@ def test_long_kmer_work_split_and_filter_widths():
     (31, 12_000_000, 3, 0.01, 60, 12, 4, 0),      # configs[3] parameters (triploid cov 60) at reduced size
     (31, 12_000_000, 4, 0.02, 80, 10, 5, 0),      # configs[4] parameters (tetraploid het 2% cov 80, L=10), reduced
     (40, 5_000_000, 2, 0.01, 40, 4, 6, 0),        # FastK's default k=40: two-word keys against the reference
-])
+]
+
+
+@pytest.mark.parametrize("k,target,ploidy,het,cov,L,seed,ref_threads", MEDIUM_CASES)
 def test_medium_table_matches_reference_binary(k, target, ploidy, het, cov, L, seed, ref_threads, tmp_path):
     G = synth.calibrate_G(k, target, ploidy, het, cov, L)
     keys, cnt = synth.synth_table(k, G, ploidy, het, cov, L, seed, device="cuda")
@@ -408,14 +419,7 @@ def test_medium_table_matches_reference_binary(k, target, ploidy, het, cov, L, s
     out = str(tmp_path / "gpu")
     hetmers.run_hetmers(name, o=out, L=L, t=4)
     got = open(out + ".smu").read()
-    if ou.have_ref():
-        r = ou.run_ref(name, str(tmp_path / "ref"), L, threads=ref_threads or min(os.cpu_count() or 4, 64))
-        assert r.returncode == 0, r.stderr
-        want = open(str(tmp_path / "ref.smu")).read()
-    else:
-        rc, *_ = ou.oracle_file(name, L, str(tmp_path / "ora.smu"))
-        assert rc == 0
-        want = open(str(tmp_path / "ora.smu")).read()
+    want = ou.reference_smu("medium", k, seed)                         # the reference binary on this table
     assert got == want and len(got) > 0
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests of the strand-symmetric scan (csrc/hm_symm.cu; run with -m gpu on the B200 box).
+"""GPU parity tests of the strand-symmetric scan (csrc/hm_symm.cu; run with -m gpu on an H100).
 The symmetric scan must give the reference's plot on every symmetric table (goldens written by the
 unmodified reference binary, the oracle on seeded / dense / long-run tables), the fingerprint must send
 every table that is not symmetric to the direct passes, and the sharded form (several GPUs) must not

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Profiling driver: one seeded bench-workload table on cuda:0, a few device-resident scans.
-Meant to be wrapped in ncu (see profiles/README.md); prints per-kernel CUDA-event times itself."""
+Meant to be wrapped in a profiler such as ncu; prints per-kernel CUDA-event times itself."""
 import argparse
 import os
 import sys
