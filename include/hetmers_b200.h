@@ -296,6 +296,42 @@ int  hm_scan_is_symmetric(const hm_scan *s);
 /* the pair list of extract_kmer_pairs (runs the direct passes first if the last run did not) for a pixel->smudge map (host
  * uint16[HM_PLOT_CELLS]); *out is malloc'ed (caller frees), sorted by (smudge, k-mer).          */
 int  hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out);
+/* ---- device budget and the streamed symmetric scan (DESIGN.md §4c) --------------------------------
+ * hm_scan_create computes the bytes the in-core scan would allocate per GPU (table arrays, bucket index,
+ * plot, fingerprint, hm_symm_plan(...).bytes).  When they exceed the device budget the scan is STREAMED:
+ * nothing is loaded at create time, and every hm_scan_run passes the table through one GPU in run-aligned
+ * chunks, keeping only the Bloom filter, the candidate records and the S list (keys with an upper
+ * partner) resident.  A streamed scan needs the table strand-symmetric (else HM_EUNSUPPORTED after the
+ * pass) and reads the host table again on every run: the hm_host_table given to hm_scan_create (its
+ * buffers or descriptors) must stay valid until hm_scan_destroy.  Streamed scans refuse what needs the
+ * whole table resident (HM_EUNSUPPORTED): hm_scan_condition, hm_scan_extract, hm_scan_download and
+ * hm_scan_run_path(HM_PATH_DIRECT); hm_scan_examine streams.  Several GPUs are not streamed over.
+ * HETMERS_STREAM=1 streams one-GPU scans whatever their size (the budget then only sizes the chunks);
+ * HETMERS_STREAM_CHUNK=<entries> caps the chunk length below what the budget allows.                */
+
+/* device bytes a scan may hold per GPU; 0 (default) = what cudaMemGetInfo reports free at
+ * hm_scan_create (plus the idle part of the memory pool) minus HM_BUDGET_RESERVE.  The executable passes
+ * HETMERS_DEVICE_BUDGET=<bytes> here.                                                               */
+#define HM_BUDGET_RESERVE (1ll << 30)
+void hm_set_device_budget(int64_t bytes);
+
+typedef struct hm_stream_layout            /* what hm_stream_plan chooses for a table under a budget      */
+  { int64_t budget;
+    int64_t chunk;                          /* entries per chunk buffer (grows if a run is longer)        */
+    int64_t fixed_bytes;                    /* stub index, plot, fingerprint, header + Bloom filter        */
+    int64_t chunk_bytes;                    /* two chunk buffers, their bucket index, run list, staging    */
+    int64_t list_bytes;                     /* left for the resident candidate records and S list          */
+    int64_t chunk_list_bytes;               /* list room one chunk may need at most                        */
+  } hm_stream_layout;
+
+/* the streamed scan's plan for n entries of k-mer length kmer (ibyte: the table's stub-index bytes);
+ * fixed + chunk + list bytes <= budget, chunk is monotone in the budget; HM_ENOMEM if the budget cannot
+ * hold one chunk                                                                                     */
+int  hm_stream_plan(int64_t n, int kmer, int ibyte, int64_t budget, hm_stream_layout *out);
+/* 1 if the scan is streamed, else 0.  *device_bytes: the most device memory the scan held per GPU (in
+ * core: what it allocates); *chunks: chunks of the last run (0 in core).  Either pointer may be NULL.  */
+int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks);
+
 /* one call: create + run + destroy (what bench.py's e2e leg times) */
 int  hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,
                      int64_t *plot, hm_scan_stats *stats);

@@ -24,7 +24,7 @@ ABI_SYMBOLS = [
     "hm_scan_create", "hm_prewarm", "hm_set_io_threads", "hm_scan_destroy", "hm_scan_examine", "hm_scan_condition", "hm_scan_run", "hm_hetmers_host",
     "hm_scan_run_path", "hm_scan_is_symmetric", "hm_symm_plan", "hm_symm_seeds", "hm_k_symm_fingerprint", "hm_k_symm_runscan", "hm_k_symm_runs", "hm_k_symm_resolve",
     "hm_symm_status", "hm_symm_align_cut",
-    "hm_scan_download", "hm_table_open", "hm_table_close", "hm_table_view", "hm_write_smu",
+    "hm_scan_download", "hm_set_device_budget", "hm_stream_plan", "hm_scan_residency", "hm_table_open", "hm_table_close", "hm_table_view", "hm_write_smu",
 ]
 
 
@@ -59,6 +59,15 @@ class SymmShards(C.Structure):
 
 
 SYMM_ASYMMETRIC, SYMM_OVERFLOW = 1, 2
+
+
+class StreamLayout(C.Structure):
+    """hm_stream_layout: what the streamed scan plans for a table under a device budget"""
+    _fields_ = [("budget", C.c_int64), ("chunk", C.c_int64), ("fixed_bytes", C.c_int64), ("chunk_bytes", C.c_int64),
+                ("list_bytes", C.c_int64), ("chunk_list_bytes", C.c_int64)]
+
+
+BUDGET_RESERVE = 1 << 30
 
 
 class PairRec(C.Structure):
@@ -141,6 +150,10 @@ def lib():
     L.hm_scan_extract.argtypes = [vp, vp, C.POINTER(C.POINTER(PairRec)), C.POINTER(i64)]
     L.hm_hetmers_host.argtypes = [C.POINTER(HostTable), C.POINTER(i32), i32, vp, C.POINTER(ScanStats)]
     L.hm_scan_download.argtypes = [vp, vp, vp, vp, vp]
+    L.hm_set_device_budget.argtypes = [i64]
+    L.hm_set_device_budget.restype = None
+    L.hm_stream_plan.argtypes = [i64, i32, i32, i64, C.POINTER(StreamLayout)]
+    L.hm_scan_residency.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     L.hm_table_open.argtypes = [C.c_char_p, C.POINTER(vp)]
     L.hm_table_close.argtypes = [vp]
     L.hm_table_close.restype = None

@@ -241,3 +241,67 @@ int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
   *pn = n;
   return HM_OK;
 }
+
+static int64_t sort_pairs_tmp(int64_t n)
+{ size_t need = 0;
+  cub::DeviceRadixSort::SortPairs(NULL,need,(const uint64_t *) NULL,(uint64_t *) NULL,(const uint64_t *) NULL,
+                                  (uint64_t *) NULL,n,0,64);
+  return (int64_t) need;
+}
+
+/* Device bytes a conditioning call borrows besides the caller's table of n entries: the larger of the
+ * trim stage (flags + one n-entry copy) and the symmetrise stage (two 2n-entry tables, sort indices for
+ * two-word keys, flags), plus CUB's temporary storage.  hm_scan_condition checks it against the budget
+ * before it touches anything.                                                                        */
+int64_t hm_condition_bytes(int kmer, int64_t n, int do_trim, int do_symm)
+{ const int64_t ent = 8 + (kmer > 32 ? 8 : 0) + 2;
+  int64_t trim = 0, symm = 0;
+  if (do_trim)
+    trim = n + ent*(n+1) + sort_pairs_tmp(n) + 8;
+  if (do_symm)
+    { int64_t m = 2*n;
+      symm = 2*ent*(m+1) + m + sort_pairs_tmp(m) + 8;
+      if (kmer > 32)
+        symm += 2*4*m;
+    }
+  return trim > symm ? trim : symm;
+}
+
+/* scratch of hm_sort_keys for up to n keys: the other buffers of the radix sort + CUB's temporary storage */
+int64_t hm_sort_keys_bytes(int64_t n, int kmer)
+{ size_t need = 0;
+  if (n < 1) n = 1;
+  if (kmer <= 32)
+    cub::DeviceRadixSort::SortKeys(NULL,need,(const uint64_t *) NULL,(uint64_t *) NULL,n,0,64);
+  else
+    need = (size_t) sort_pairs_tmp(n);
+  return ((8*n+255) & ~255ll)*(kmer > 32 ? 2 : 1) + (int64_t) need + 256;
+}
+
+/* Sort n packed keys in place, in the caller's scratch (hm_sort_keys_bytes), enqueued on st: one radix sort
+ * for one-word keys; for two-word keys the least significant word first, then a stable sort on the most
+ * significant word (the order of hm_condition_arrays, the other word riding along as the value).       */
+int hm_sort_keys(uint64_t *keys, uint64_t *lo, int64_t n, int kmer, void *scratch, int64_t scratch_bytes,
+                 cudaStream_t st)
+{ if (n <= 1)
+    return HM_OK;
+  if (scratch_bytes < hm_sort_keys_bytes(n,kmer))
+    return hm_set_error(HM_EINVAL,"hm_sort_keys: %lld bytes of scratch for %lld keys",(long long) scratch_bytes,(long long) n);
+  uint8_t  *b   = (uint8_t *) scratch;
+  int64_t   arr = (8*n+255) & ~255ll;
+  uint64_t *k2  = (uint64_t *) b;
+  uint64_t *l2  = (uint64_t *) (b + arr);
+  void     *tmp = b + arr*(kmer > 32 ? 2 : 1);
+  size_t    tb  = (size_t) (scratch_bytes - arr*(kmer > 32 ? 2 : 1));
+  if (kmer <= 32)
+    { int bb = kmer < 32 ? 64-2*kmer : 0;
+      HM_CUDA(cub::DeviceRadixSort::SortKeys(tmp,tb,keys,k2,n,bb,64,st));
+      HM_CUDA(cudaMemcpyAsync(keys,k2,sizeof(uint64_t)*(size_t) n,cudaMemcpyDeviceToDevice,st));
+    }
+  else
+    { int bb = kmer < 64 ? 128-2*kmer : 0;
+      HM_CUDA(cub::DeviceRadixSort::SortPairs(tmp,tb,lo,l2,keys,k2,n,bb,64,st));     /* by the second word */
+      HM_CUDA(cub::DeviceRadixSort::SortPairs(tmp,tb,k2,keys,l2,lo,n,0,64,st));      /* stable, by the first */
+    }
+  return HM_OK;
+}

@@ -23,8 +23,36 @@ int hm_build_bucket_index_range(const uint64_t *d_keys, int64_t n, int bits, voi
 int hm_build_filter_range(const uint64_t *d_keys, int filter_bits, uint32_t *d_filter,
                           int64_t i0, int64_t i1, void *stream);
 
+/* streamed symmetric scan (hm_symm.cu; driven by hm_scan.cu, DESIGN.md §4c): resident candidate records and
+ * the S list (every key pass 1 puts into the Bloom filter), appended to by the chunks                        */
+typedef struct hm_stream_lists
+  { uint64_t *cand_key, *cand_lo, *cand_meta;
+    int64_t   cand_cap;
+    uint64_t *s_key, *s_lo;
+    int64_t   s_cap;
+    uint64_t *runs;                         /* heads of the current chunk's runs of three or more entries */
+    int64_t   runs_cap;
+  } hm_stream_lists;
+
+int hm_symm_stream_begin(void *d_work, const hm_symm_layout *L, void *stream);
+int hm_symm_stream_chunk(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                         int64_t n, const void *d_bucket, int bits, int kmer, int64_t hi,
+                         void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, void *stream);
+int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t *n_cand,
+                          uint64_t *status, uint64_t *n_s, void *stream);
+int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
+                           const void *d_s_bucket, int bits, int idx64, int kmer, int64_t range,
+                           void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                           unsigned long long *d_plot, void *stream);
+
 #include <cuda_runtime.h>
 int hm_cuda_fail(cudaError_t e, const char *what);
+/* sort n packed keys (two words for k > 32) in place, in scratch of hm_sort_keys_bytes (hm_condition.cu) */
+int64_t hm_sort_keys_bytes(int64_t n, int kmer);
+int     hm_sort_keys(uint64_t *keys, uint64_t *lo, int64_t n, int kmer, void *scratch, int64_t scratch_bytes,
+                     cudaStream_t st);
+/* device bytes hm_condition_arrays borrows besides the table it is given                              */
+int64_t hm_condition_bytes(int kmer, int64_t n, int do_trim, int do_symm);
 #define HM_CUDA(call)                                              \
   do { cudaError_t _e = (call);                                    \
        if (_e != cudaSuccess) return hm_cuda_fail(_e,#call);       \

@@ -15,6 +15,8 @@
  * native NVLink atomics); the
  * one-process-per-GPU variant (torch.distributed / NCCL) lives in smudgeplot_b200/dist.py and
  * uses layer A directly.
+ * A table whose in-core footprint exceeds the device budget is not loaded here: every run streams it
+ * through one GPU in run-aligned chunks (run_stream, DESIGN.md §4c).
  *******************************************************************************************/
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -67,6 +69,13 @@ struct hm_scan
     int      invalid;                     /* a failed conditioning left the replicas inconsistent            */
     hm_symm_shards ssh[HM_MAX_GPUS];
     uint64_t seed[2];
+    /* residency (DESIGN.md §4c) */
+    int64_t  budget;                      /* device bytes this scan may hold per GPU                          */
+    int64_t  incore_bytes;                /* what the in-core scan allocates per GPU                          */
+    int      streamed;                    /* nothing resident: every run streams the host table through GPU 0 */
+    const hm_host_table *host;            /* (streamed) the caller's table, valid until hm_scan_destroy        */
+    hm_stream_layout plan;
+    int64_t  held, peak, chunks;          /* (streamed) device bytes held now / at most; chunks of the last run */
   };
 
 static double now_ms(void)
@@ -281,46 +290,74 @@ static int is_pageable(const void *p)
   return (a.type == cudaMemoryTypeUnregistered);
 }
 
-/* Load ordinals [first, first+count) of the table onto device D (keys/cnt already allocated for
- * the full table).  Walks the parts, copies payload chunks H2D on st_copy into one of two device
- * staging buffers and unpacks them on st (copy of chunk c+1 overlaps the unpack of chunk c);
- * pageable sources additionally go through two pinned host buffers filled by host threads.      */
-static int load_range(hm_scan *s, DevTable *D, const hm_host_table *t, const int64_t *d_index,
-                      int64_t first, int64_t count)
+/* Host -> device staging of table records: two device staging buffers (the copy of chunk c+1 overlaps the
+ * unpack of chunk c) and, for pageable sources, two pinned host buffers filled by host threads.          */
+typedef struct
+  { uint8_t    *stage[2], *pin[2];
+    int         pin_cached[2], staged, used[2], b;
+    cudaEvent_t copied[2], unpacked[2];
+    int64_t     chunk;                /* records per H2D copy */
+    int64_t     bytes;                /* device bytes of the staging buffers */
+  } Stager;
+
+static int stager_open(hm_scan *s, DevTable *D, const hm_host_table *t, int64_t count, Stager *G)
+{ int kbyte = (t->kmer+3)>>2;
+  int pbyte = kbyte - t->ibyte + 2;
+  memset(G,0,sizeof(*G));
+  G->chunk = LOAD_CHUNK;
+  for (int p = 0; p < t->nparts && !G->staged; p++)
+    if (t->part_nels[p] > 0 &&
+        ((t->part_fd != NULL && t->part_fd[p] >= 0) || is_pageable(t->part_rec[p])))
+      G->staged = 1;
+  if (G->staged)
+    G->chunk = LOAD_CHUNK/2;
+  if (G->chunk > count) G->chunk = count;
+  for (int i = 0; i < 2; i++)
+    { HM_CUDA(dalloc(D->dev,D->st,(void **) &G->stage[i],(size_t) G->chunk*pbyte));
+      G->bytes += G->chunk*pbyte;
+      if (G->staged)
+        { if (s->ngpu == 1 && g_pin_cache[i] != NULL && (size_t) G->chunk*pbyte <= PIN_CACHE_BYTES)
+            { G->pin[i] = g_pin_cache[i]; g_pin_cache[i] = NULL; G->pin_cached[i] = 1; }   /* from hm_prewarm */
+          else
+            HM_CUDA(cudaHostAlloc(&G->pin[i],(size_t) G->chunk*pbyte,cudaHostAllocDefault));
+        }
+      HM_CUDA(cudaEventCreateWithFlags(&G->copied[i],cudaEventDisableTiming));
+      HM_CUDA(cudaEventCreateWithFlags(&G->unpacked[i],cudaEventDisableTiming));
+    }
+  HM_CUDA(cudaStreamSynchronize(D->st));         /* (pool) allocations are used on both streams */
+  return HM_OK;
+}
+
+static void stager_close(DevTable *D, Stager *G)
+{ for (int i = 0; i < 2; i++)
+    { if (G->stage[i] != NULL) dfree(D->dev,D->st,G->stage[i]);
+      if (G->copied[i] != NULL)   cudaEventDestroy(G->copied[i]);
+      if (G->unpacked[i] != NULL) cudaEventDestroy(G->unpacked[i]);
+      if (G->pin[i] != NULL)
+        { if (G->pin_cached[i]) g_pin_cache[i] = G->pin[i];        /* back into the cache for the next table */
+          else                  cudaFreeHost(G->pin[i]);
+        }
+    }
+  memset(G,0,sizeof(*G));
+}
+
+/* Load ordinals [first, first+count) of the table into keys/keys_lo/cnt (which receive ordinal `first`
+ * at index 0).  Walks the parts, copies payload chunks H2D on st_copy into the stager's device buffers
+ * and unpacks them on st.  extras: D's arrays hold the whole table -- build its bucket index chunk by chunk
+ * (one GPU) and add the symmetry fingerprint of what is loaded.                                        */
+static int load_into(hm_scan *s, DevTable *D, const hm_host_table *t, const int64_t *d_index,
+                     int64_t first, int64_t count, uint64_t *keys, uint64_t *keys_lo, uint16_t *cnt,
+                     int extras, Stager *G)
 { int      kbyte = (t->kmer+3)>>2;
   int      pbyte = kbyte - t->ibyte + 2;
-  uint8_t *stage[2] = { NULL, NULL };
-  uint8_t *pin[2]   = { NULL, NULL };
-  cudaEvent_t copied[2], unpacked[2];
-  int64_t  chunk = LOAD_CHUNK;
-  int      rc = HM_OK, b = 0, used[2] = {0,0};
-  int      staged = 0;
+  int64_t  chunk = G->chunk;
+  int      rc = HM_OK;
 
   if (count <= 0)
     return HM_OK;
-  for (int p = 0; p < t->nparts && !staged; p++)
-    if (t->part_nels[p] > 0 &&
-        ((t->part_fd != NULL && t->part_fd[p] >= 0) || is_pageable(t->part_rec[p])))
-      staged = 1;
-  if (staged)
-    chunk = LOAD_CHUNK/2;
-  if (chunk > count) chunk = count;
-  int pin_cached[2] = {0,0};
-  for (int i = 0; i < 2; i++)
-    { HM_CUDA(dalloc(D->dev,D->st,(void **) &stage[i],(size_t) chunk*pbyte));
-      if (staged)
-        { if (s->ngpu == 1 && g_pin_cache[i] != NULL && (size_t) chunk*pbyte <= PIN_CACHE_BYTES)
-            { pin[i] = g_pin_cache[i]; g_pin_cache[i] = NULL; pin_cached[i] = 1; }   /* from hm_prewarm */
-          else
-            HM_CUDA(cudaHostAlloc(&pin[i],(size_t) chunk*pbyte,cudaHostAllocDefault));
-        }
-      HM_CUDA(cudaEventCreateWithFlags(&copied[i],cudaEventDisableTiming));
-      HM_CUDA(cudaEventCreateWithFlags(&unpacked[i],cudaEventDisableTiming));
-    }
   /* one GPU: the whole table arrives here in order, so the bucket index is built chunk by chunk
    * right behind the unpack (hidden behind the next chunk's H2D); so is the symmetry fingerprint   */
-  const int inc = (s->ngpu == 1 && first == 0 && count == s->n);
-  HM_CUDA(cudaStreamSynchronize(D->st));         /* (pool) allocations are used on both streams */
+  const int inc = extras && (s->ngpu == 1 && first == 0 && count == s->n);
   int64_t pstart = 0;                               /* ordinal of the part's first record */
   for (int p = 0; p < t->nparts && rc == HM_OK; p++)
     { int64_t pn   = t->part_nels[p];
@@ -329,55 +366,64 @@ static int load_range(hm_scan *s, DevTable *D, const hm_host_table *t, const int
       for (int64_t o = from; o < to && rc == HM_OK; o += chunk)
         { int64_t        m   = to-o < chunk ? to-o : chunk;
           const uint8_t *src = t->part_rec[p] + (o-pstart)*pbyte;
-          if (staged)
-            { if (used[b])
-                cudaEventSynchronize(copied[b]);      /* pin[b] has left for the GPU */
+          int            b   = G->b;
+          if (G->staged)
+            { if (G->used[b])
+                cudaEventSynchronize(G->copied[b]);   /* pin[b] has left for the GPU */
               int ferr;
               if (t->part_fd != NULL && t->part_fd[p] >= 0)
-                ferr = parallel_fill(pin[b],NULL,t->part_fd[p],t->part_fd_off[p]+(o-pstart)*pbyte,(size_t) m*pbyte);
+                ferr = parallel_fill(G->pin[b],NULL,t->part_fd[p],t->part_fd_off[p]+(o-pstart)*pbyte,(size_t) m*pbyte);
               else
-                ferr = parallel_fill(pin[b],src,-1,0,(size_t) m*pbyte);
+                ferr = parallel_fill(G->pin[b],src,-1,0,(size_t) m*pbyte);
               if (ferr != 0)
                 { rc = hm_set_error(HM_EIO,"short read on part %d of the table (%s)",p+1,
                                     ferr > 0 ? strerror(ferr) : "file truncated");
                   break;
                 }
-              src = pin[b];
+              src = G->pin[b];
             }
-          if (used[b])
-            cudaStreamWaitEvent(D->st_copy,unpacked[b],0);
-          cudaError_t e = cudaMemcpyAsync(stage[b],src,(size_t) m*pbyte,cudaMemcpyHostToDevice,D->st_copy);
+          if (G->used[b])
+            cudaStreamWaitEvent(D->st_copy,G->unpacked[b],0);
+          cudaError_t e = cudaMemcpyAsync(G->stage[b],src,(size_t) m*pbyte,cudaMemcpyHostToDevice,D->st_copy);
           if (e != cudaSuccess) { rc = hm_cuda_fail(e,"cudaMemcpyAsync(H2D records)"); break; }
-          cudaEventRecord(copied[b],D->st_copy);
-          cudaStreamWaitEvent(D->st,copied[b],0);
-          rc = hm_k_unpack_records(stage[b],m,o,d_index,t->ibyte,t->kmer,D->keys+o,
-                                   D->keys_lo ? D->keys_lo+o : NULL,D->cnt+o,D->st);
+          cudaEventRecord(G->copied[b],D->st_copy);
+          cudaStreamWaitEvent(D->st,G->copied[b],0);
+          int64_t at = o-first;
+          rc = hm_k_unpack_records(G->stage[b],m,o,d_index,t->ibyte,t->kmer,keys+at,
+                                   keys_lo ? keys_lo+at : NULL,cnt+at,D->st);
           __sync_fetch_and_add(&s->launches,1);
-          cudaEventRecord(unpacked[b],D->st);
+          cudaEventRecord(G->unpacked[b],D->st);
           if (inc && rc == HM_OK)
             { rc = hm_build_bucket_index_range(D->keys,s->n,s->bits,D->bucket,s->idx64,o,o+m,D->st);
               __sync_fetch_and_add(&s->launches,1);
             }
-          if (rc == HM_OK && s->kmer >= HM_SYMM_MIN_KMER)       /* symmetry fingerprint of what this device loads */
+          if (extras && rc == HM_OK && s->kmer >= HM_SYMM_MIN_KMER)   /* symmetry fingerprint of what this device loads */
             { rc = hm_k_symm_fingerprint(D->keys,D->keys_lo,D->cnt,o,o+m,s->kmer,s->seed,D->fp_acc,D->st);
               __sync_fetch_and_add(&s->launches,1);
             }
-          used[b] = 1;
-          b ^= 1;
+          G->used[b] = 1;
+          G->b ^= 1;
         }
       pstart += pn;
     }
   cudaStreamSynchronize(D->st_copy);
   cudaError_t e = cudaStreamSynchronize(D->st);
-  for (int i = 0; i < 2; i++)
-    { dfree(D->dev,D->st,stage[i]); cudaEventDestroy(copied[i]); cudaEventDestroy(unpacked[i]);
-      if (pin[i] != NULL)
-        { if (pin_cached[i]) g_pin_cache[i] = pin[i];        /* back into the cache for the next table */
-          else               cudaFreeHost(pin[i]);
-        }
-    }
   if (rc == HM_OK && e != cudaSuccess)
     rc = hm_cuda_fail(e,"unpack");
+  return rc;
+}
+
+/* ordinals [first, first+count) into D's full-table arrays */
+static int load_range(hm_scan *s, DevTable *D, const hm_host_table *t, const int64_t *d_index,
+                      int64_t first, int64_t count)
+{ Stager G;
+  if (count <= 0)
+    return HM_OK;
+  int rc = stager_open(s,D,t,count,&G);
+  if (rc == HM_OK)
+    rc = load_into(s,D,t,d_index,first,count,D->keys+first,D->keys_lo ? D->keys_lo+first : NULL,
+                   D->cnt+first,1,&G);
+  stager_close(D,&G);
   return rc;
 }
 
@@ -422,6 +468,133 @@ static int fingerprint_verdict(hm_scan *s)
   return HM_OK;
 }
 
+/* ---- device budget ---------------------------------------------------------------------------------- */
+static int64_t g_budget = 0;
+
+extern "C" void hm_set_device_budget(int64_t bytes) { g_budget = bytes > 0 ? bytes : 0; }
+
+/* the budget per GPU: the one set, or the smallest free memory of the devices (counting what an idle
+ * stream-ordered pool keeps reserved for us) minus a reserve for the CUDA runtime and library code      */
+static int64_t device_budget(const int *dev, int n_gpus)
+{ if (g_budget > 0)
+    return g_budget;
+  int64_t best = -1;
+  for (int g = 0; g < n_gpus; g++)
+    { int    d = dev ? dev[g] : g;
+      size_t fr = 0, tot = 0;
+      if (cudaSetDevice(d) != cudaSuccess || cudaMemGetInfo(&fr,&tot) != cudaSuccess)
+        { cudaGetLastError(); continue; }
+      int64_t f = (int64_t) fr;
+      cudaMemPool_t pool;
+      unsigned long long res = 0, used = 0;
+      if (cudaDeviceGetDefaultMemPool(&pool,d) == cudaSuccess &&
+          cudaMemPoolGetAttribute(pool,cudaMemPoolAttrReservedMemCurrent,&res) == cudaSuccess &&
+          cudaMemPoolGetAttribute(pool,cudaMemPoolAttrUsedMemCurrent,&used) == cudaSuccess && res > used)
+        f += (int64_t) (res-used);
+      cudaGetLastError();
+      if (best < 0 || f < best) best = f;
+    }
+  if (best < 0)
+    return 0;
+  return best > HM_BUDGET_RESERVE ? best-HM_BUDGET_RESERVE : 0;
+}
+
+/* device bytes the in-core scan allocates per GPU: table arrays, bucket index, plot, fingerprint sums and the
+ * symmetric scan's work area (the direct passes' buffers come on top only for tables that need them)     */
+static int64_t incore_bytes(int64_t n, int kmer, int n_gpus, int bits, int idx64)
+{ int64_t b = 8*(n+1) + (kmer > 32 ? 8*(n+1) : 0) + 2*(n+8) + (int64_t) (idx64 ? 8 : 4)*((1ll << bits)+1) +
+              8*(int64_t) HM_PLOT_CELLS + 32;
+  hm_symm_layout L;
+  if (kmer >= HM_SYMM_MIN_KMER && hm_symm_plan(n,(n+n_gpus-1)/n_gpus < n ? (n+n_gpus-1)/n_gpus : n,kmer,n_gpus,&L) == HM_OK)
+    b += L.bytes;
+  return b;
+}
+
+/* ---- the streamed scan's plan --------------------------------------------------------------------- */
+#define STREAM_MIN_CHUNK 256
+
+/* work area of the streamed scan: header + the whole-table Bloom filter of hm_symm_plan (one segment) */
+static int stream_work_layout(int64_t n, int kmer, hm_symm_layout *L)
+{ int rc = hm_symm_plan(n,0,kmer,1,L);
+  if (rc != HM_OK) return rc;
+  L->bytes = (L->off_cand_key+255) & ~255ll;
+  L->cand_cap = 0; L->runs_cap = 0;
+  return HM_OK;
+}
+
+static int64_t stage_bytes(int64_t chunk, int kmer, int ibyte)
+{ int64_t c = chunk < LOAD_CHUNK ? chunk : LOAD_CHUNK;
+  return 2*c*(((kmer+3)>>2) - ibyte + 2);
+}
+
+/* two chunk buffers (keys, second words, counts), their bucket index, the run list, staging, and the
+ * scratch that sorts a chunk's S keys                                                                 */
+static int64_t chunk_bytes(int64_t c, int kmer, int ibyte)
+{ int KW = kmer > 32 ? 2 : 1;
+  return 2*(8*KW*(c+1) + 2*(c+8)) + 4*((1ll << hm_pick_bucket_bits(c))+1) + 8*(c/3+1024) + stage_bytes(c,kmer,ibyte) +
+         hm_sort_keys_bytes(c+1024,kmer);
+}
+
+/* list room one chunk of c entries may take: a candidate record per two entries, an S key per entry */
+static int64_t chunk_list_bytes(int64_t c, int kmer)
+{ int KW = kmer > 32 ? 2 : 1;
+  return (8*KW+8)*(c/2+1024) + 8*KW*(c+1024);
+}
+
+extern "C" int hm_stream_plan(int64_t n, int kmer, int ibyte, int64_t budget, hm_stream_layout *out)
+{ if (out == NULL || n < 0 || kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || budget < 0)
+    return hm_set_error(HM_EINVAL,"hm_stream_plan: bad arguments");
+  hm_symm_layout L;
+  int rc = stream_work_layout(n,kmer,&L);
+  if (rc != HM_OK) return rc;
+  memset(out,0,sizeof(*out));
+  out->budget = budget;
+  out->fixed_bytes = 8*(1ll << (8*ibyte)) + 8*(int64_t) HM_PLOT_CELLS + 32 + L.bytes;
+  /* the largest chunk whose buffers + list room take at most a quarter of what is left: the rest is for
+   * the candidate records and S keys of the chunks before it (a few B per entry of the whole table) and
+   * for growing those lists, which holds the old and the new array at once                             */
+  int64_t avail = budget - out->fixed_bytes, lo = 0, hi = n < (1ll << 31) ? n : (1ll << 31);
+  if (avail > 0)
+    while (lo < hi)
+      { int64_t mid = lo + (hi-lo+1)/2;
+        if (chunk_bytes(mid,kmer,ibyte) + chunk_list_bytes(mid,kmer) <= avail/4) lo = mid;
+        else                                                                   hi = mid-1;
+      }
+  int64_t need = n < STREAM_MIN_CHUNK ? n : STREAM_MIN_CHUNK;
+  if (avail <= 0 || lo < need || lo < 1)
+    return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes cannot hold one chunk of the streamed scan: "
+                        "%lld bytes are fixed (stub index, plot, Bloom filter of %lld entries) and a chunk of "
+                        "%lld entries needs %lld more",(long long) budget,(long long) out->fixed_bytes,(long long) n,
+                        (long long) need,(long long) (chunk_bytes(need,kmer,ibyte)+chunk_list_bytes(need,kmer)));
+  out->chunk = lo;
+  out->chunk_bytes = chunk_bytes(lo,kmer,ibyte);
+  out->chunk_list_bytes = chunk_list_bytes(lo,kmer);
+  out->list_bytes = budget - out->fixed_bytes - out->chunk_bytes;
+  return HM_OK;
+}
+
+extern "C" int hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks)
+{ if (device_bytes) *device_bytes = s->streamed ? s->peak : s->incore_bytes;
+  if (chunks)       *chunks = s->streamed ? s->chunks : 0;
+  return s->streamed;
+}
+
+/* streamed scans: device allocations counted against the budget */
+static cudaError_t salloc(hm_scan *s, DevTable *D, void **p, int64_t bytes)
+{ cudaError_t e = dalloc(D->dev,D->st,p,(size_t) bytes);
+  if (e == cudaSuccess)
+    { s->held += bytes;
+      if (s->held > s->peak) s->peak = s->held;
+    }
+  return e;
+}
+
+static void sfree(hm_scan *s, DevTable *D, void *p, int64_t bytes)
+{ if (p == NULL) return;
+  dfree(D->dev,D->st,p);
+  s->held -= bytes;
+}
+
 extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out)
 { double t0 = now_ms();
   if (t == NULL || out == NULL || n_gpus < 1 || n_gpus > HM_MAX_GPUS)
@@ -447,6 +620,46 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   int64_t n  = s->n;
   size_t  ib = s->idx64 ? 8 : 4;
   int     rc = HM_OK;
+
+  s->budget = device_budget(dev,n_gpus);
+  s->incore_bytes = incore_bytes(n,t->kmer,n_gpus,s->bits,s->idx64);
+  const char *force = getenv("HETMERS_STREAM");            /* =1: stream whatever the budget (tests, capping) */
+  if (s->incore_bytes > s->budget || (force != NULL && strcmp(force,"1") == 0))
+    { /* streamed: only the plot and the fingerprint sums are allocated now; the table stays on the host */
+      if (n_gpus > 1)
+        { free(s);
+          return hm_set_error(HM_EUNSUPPORTED,"the table of %lld entries needs %lld device bytes per GPU in core, more "
+                              "than the device budget of %lld; it can be streamed through one GPU, not several",
+                              (long long) n,(long long) incore_bytes(n,t->kmer,n_gpus,s->bits,s->idx64),(long long) s->budget);
+        }
+      if ((rc = hm_stream_plan(n,t->kmer,t->ibyte,s->budget,&s->plan)) != HM_OK)
+        { free(s); return rc; }
+      const char *cc = getenv("HETMERS_STREAM_CHUNK");         /* smaller chunks than the budget allows */
+      if (cc != NULL && atoll(cc) >= 1 && atoll(cc) < s->plan.chunk)
+        { s->plan.chunk = atoll(cc);
+          s->plan.chunk_bytes = chunk_bytes(s->plan.chunk,t->kmer,t->ibyte);
+          s->plan.chunk_list_bytes = chunk_list_bytes(s->plan.chunk,t->kmer);
+          s->plan.list_bytes = s->budget - s->plan.fixed_bytes - s->plan.chunk_bytes;
+        }
+      s->streamed = 1; s->host = t;
+      DevTable *D = s->d;
+      cudaError_t e;
+      D->dev = dev ? dev[0] : 0;
+      D->lo = 0; D->hi = n;
+#define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
+      TRY(cudaSetDevice(D->dev));
+      pool_setup(D->dev,1);
+      TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
+      TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
+      TRY(salloc(s,D,(void **) &D->plot,8*(int64_t) HM_PLOT_CELLS));
+      TRY(salloc(s,D,(void **) &D->fp_acc,4*sizeof(uint64_t)));
+#undef TRY
+      if (rc != HM_OK)
+        { hm_scan_destroy(s); return rc; }
+      s->ms_load = now_ms()-t0;
+      *out = s;
+      return HM_OK;
+    }
 
   if (n_gpus > 1 && (rc = hm_peer_enable(dev,n_gpus)) != HM_OK)
     { free(s); return rc; }
@@ -616,6 +829,16 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
     { if (nels_out) *nels_out = s->n;
       return HM_OK;
     }
+  if (s->streamed)
+    return hm_set_error(HM_EUNSUPPORTED,"conditioning on the GPU needs the table resident; this one does not fit in "
+                                        "device memory (budget %lld bytes)",(long long) s->budget);
+  { /* before anything is touched: the table arrays + what conditioning borrows must fit the budget */
+    int64_t need = 8*(s->n+1) + (s->kmer > 32 ? 8*(s->n+1) : 0) + 2*(s->n+8) + 8*(int64_t) HM_PLOT_CELLS +
+                   hm_condition_bytes(s->kmer,s->n,do_trim,do_symm);
+    if (need > s->budget)
+      return hm_set_error(HM_ENOMEM,"conditioning %lld entries on the GPU needs %lld device bytes, more than the "
+                          "budget of %lld",(long long) s->n,(long long) need,(long long) s->budget);
+  }
   /* everything derived from the old table goes first: work buffers of both paths, the index */
   s->ran = 0; s->have_direct = 0; s->have_symm = 0;
   for (int g = 0; g < G; g++)
@@ -713,8 +936,12 @@ static void revcomp128(uint64_t hi, uint64_t lo, int k, uint64_t *rhi, uint64_t 
 /* examine_table (PloidyPlot.c:1167-1230).  trim: smallest non-zero count among the middle <=1e8
  * entries >= ethresh.  symm: reverse complement of entry 1 (moving on past palindromes, where
  * the reference's loop would never terminate) is present.                                      */
+static int examine_streamed(hm_scan *s, int ethresh, int *trim, int *symm);
+
 extern "C" int hm_scan_examine(hm_scan *s, int ethresh, int *trim, int *symm)
-{ DevTable *D = s->d;
+{ if (s->streamed)
+    return examine_streamed(s,ethresh,trim,symm);
+  DevTable *D = s->d;
   int64_t   n = s->n, frst, last;
   int       h_min = 0x8000, *d_min = NULL;
   uint64_t *d_q = NULL;
@@ -996,6 +1223,379 @@ static int run_symm(hm_scan *s, int64_t *plot, hm_scan_stats *stats, uint64_t *s
   return HM_OK;
 }
 
+/* ---- the streamed symmetric scan (DESIGN.md §4c) ------------------------------------------------------ */
+
+/* largest i in [1,m) where a run (entries sharing their first k/2 bases) starts; 0 if all m share one */
+static int last_run_start(const uint64_t *d_keys, int64_t m, int kmer, int64_t *out)
+{ const int psh = 64-2*(kmer>>1);
+  uint64_t  buf[4096];
+  int64_t   end = m;
+  while (end > 1)
+    { int64_t from = end > 4096 ? end-4096 : 0;
+      HM_CUDA(cudaMemcpy(buf,d_keys+from,sizeof(uint64_t)*(size_t) (end-from),cudaMemcpyDeviceToHost));
+      for (int64_t i = end-1; i > from; i--)
+        if (((buf[i-from] ^ buf[i-1-from]) >> psh) != 0)
+          { *out = i; return HM_OK; }
+      end = from+1;
+    }
+  *out = 0;
+  return HM_OK;
+}
+
+/* everything one streamed run allocates */
+typedef struct
+  { int64_t   cap;                                     /* entries per chunk buffer */
+    uint64_t *keys[2], *klo[2];
+    uint16_t *cnt[2];
+    void     *bucket;
+    int       bits;
+    int64_t  *d_index;
+    void     *work;
+    hm_symm_layout L;
+    hm_stream_lists R;
+    Stager    G;
+    void     *s_bucket;
+    int64_t   s_bucket_bytes;
+    void     *sort_tmp;                                /* sorts the S keys of one chunk */
+    int64_t   sort_bytes;
+    cudaStream_t sc;                                   /* the chunks' kernels: overlap the next chunk's load */
+  } StreamRun;
+
+static int64_t stream_list_bytes(const hm_scan *s, const StreamRun *R)
+{ int KW = s->kmer > 32 ? 2 : 1;
+  return (8*KW+8)*R->R.cand_cap + 8*KW*R->R.s_cap;
+}
+
+static void stream_free_chunks(hm_scan *s, DevTable *D, StreamRun *R)
+{ int KW = s->kmer > 32 ? 2 : 1;
+  if (R->sc) cudaStreamSynchronize(R->sc);
+  for (int b = 0; b < 2; b++)
+    { sfree(s,D,R->keys[b],8*(R->cap+1)); R->keys[b] = NULL;
+      if (KW == 2) sfree(s,D,R->klo[b],8*(R->cap+1));
+      R->klo[b] = NULL;
+      sfree(s,D,R->cnt[b],2*(R->cap+8)); R->cnt[b] = NULL;
+    }
+  sfree(s,D,R->bucket,4*((1ll << R->bits)+1)); R->bucket = NULL;
+  sfree(s,D,R->R.runs,8*R->R.runs_cap);        R->R.runs = NULL;
+  sfree(s,D,R->sort_tmp,R->sort_bytes);        R->sort_tmp = NULL;
+  if (R->G.bytes > 0) s->held -= R->G.bytes;
+  stager_close(D,&R->G);
+}
+
+/* chunk buffers for `cap` entries (+ bucket index, run list, staging), within the budget */
+static int stream_alloc_chunks(hm_scan *s, DevTable *D, StreamRun *R, int64_t cap)
+{ int KW = s->kmer > 32 ? 2 : 1;
+  int64_t need = chunk_bytes(cap,s->kmer,s->ibyte);
+  if (s->held + need > s->budget)
+    return HM_ENOMEM;
+  cudaError_t e = cudaSuccess;
+  R->cap = cap;
+  R->bits = hm_pick_bucket_bits(cap);
+  for (int b = 0; b < 2 && e == cudaSuccess; b++)
+    { e = salloc(s,D,(void **) &R->keys[b],8*(cap+1));
+      if (e == cudaSuccess && KW == 2) e = salloc(s,D,(void **) &R->klo[b],8*(cap+1));
+      if (e == cudaSuccess) e = salloc(s,D,(void **) &R->cnt[b],2*(cap+8));
+    }
+  if (e == cudaSuccess) e = salloc(s,D,&R->bucket,4*((1ll << R->bits)+1));
+  R->R.runs_cap = cap/3+1024;
+  if (e == cudaSuccess) e = salloc(s,D,(void **) &R->R.runs,8*R->R.runs_cap);
+  R->sort_bytes = hm_sort_keys_bytes(cap+1024,s->kmer);
+  if (e == cudaSuccess) e = salloc(s,D,&R->sort_tmp,R->sort_bytes);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"streamed scan: chunk buffers");
+  int rc = stager_open(s,D,s->host,cap,&R->G);
+  s->held += R->G.bytes;
+  if (s->held > s->peak) s->peak = s->held;
+  return rc;
+}
+
+/* grow a group of resident arrays (same capacity, 8-byte elements) to hold `need` entries: doubling, but
+ * no further than the final size projected from the `used` entries the first `done` table entries gave */
+static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[], int narr, int64_t *cap,
+                       int64_t used, int64_t need, int64_t done, const char *what)
+{ if (need <= *cap)
+    return HM_OK;
+  int64_t nc = 2 * *cap;
+  if (done > 0)
+    { int64_t proj = need + (int64_t) ((double) used / (double) done * (double) (s->n - done) * 1.02);
+      if (nc > proj) nc = proj;
+    }
+  if (nc < need) nc = need;
+  int64_t room = (s->budget - s->held) / (8*narr);        /* the old arrays are held until the copy is done */
+  if (nc > room) nc = room;
+  if (nc < need)
+    return hm_set_error(HM_ENOMEM,"the streamed scan's %s list needs %lld entries (%lld bytes) but the device budget "
+                        "of %lld bytes has room for %lld more while %lld bytes are held; give the scan a larger "
+                        "budget (HETMERS_DEVICE_BUDGET)",what,(long long) need,(long long) (8*narr*need),
+                        (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) s->held);
+  for (int a = 0; a < narr; a++)
+    { uint64_t *p = NULL;
+      cudaError_t e = salloc(s,D,(void **) &p,8*nc);
+      if (e != cudaSuccess) return hm_cuda_fail(e,"streamed scan: resident lists");
+      if (used > 0 && *arr[a] != NULL)
+        HM_CUDA(cudaMemcpyAsync(p,*arr[a],8*(size_t) used,cudaMemcpyDeviceToDevice,st));
+      HM_CUDA(cudaStreamSynchronize(st));
+      sfree(s,D,*arr[a],8 * *cap);
+      *arr[a] = p;
+    }
+  *cap = nc;
+  return HM_OK;
+}
+
+static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, float *ms_kernels)
+{ const hm_host_table *t = s->host;
+  int      KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
+  int64_t  n = s->n, c0 = 0, chunks = 0;
+  int      b = 0;
+  uint64_t nc = 0, status = 0, ns = 0, ns0 = 0;     /* ns0: S keys before the chunk in flight */
+  cudaEvent_t e0, e1;
+  HM_CUDA(cudaEventCreate(&e0)); HM_CUDA(cudaEventCreate(&e1));
+  HM_CUDA(cudaEventRecord(e0,R->sc));
+  while (c0 < n && rc == HM_OK)
+    { int64_t m = n-c0 < R->cap ? n-c0 : R->cap;
+      /* the copy + unpack of this chunk overlaps the kernels of the previous one (on R->sc) */
+      rc = load_into(s,D,t,R->d_index,c0,m,R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],0,&R->G);
+      if (rc != HM_OK) break;
+      int64_t cut = m;
+      if (c0+m < n && (rc = last_run_start(R->keys[b],m,s->kmer,&cut)) != HM_OK)
+        break;
+      if (cut == 0)
+        { /* one run fills the whole chunk: larger buffers, and load it again */
+          int64_t cap = 2*R->cap;
+          stream_free_chunks(s,D,R);
+          rc = stream_alloc_chunks(s,D,R,cap);
+          if (rc == HM_ENOMEM)
+            rc = hm_set_error(HM_ENOMEM,"a run of more than %lld entries (k-mers sharing their first %d bases) does "
+                              "not fit in one chunk of the streamed scan under the device budget of %lld bytes",
+                              (long long) m,s->kmer>>1,(long long) s->budget);
+          b = 0;
+          continue;
+        }
+      if ((rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) != HM_OK)   /* previous chunk done */
+        break;
+      /* its S keys, sorted in place: chunks come in key order, so the list stays sorted as a whole */
+      if ((rc = hm_sort_keys(R->R.s_key+ns0,KW == 2 ? R->R.s_lo+ns0 : NULL,(int64_t) (ns-ns0),s->kmer,
+                             R->sort_tmp,R->sort_bytes,R->sc)) != HM_OK)
+        break;
+      ns0 = ns;
+      { uint64_t **ca[3] = { &R->R.cand_key, &R->R.cand_meta, &R->R.cand_lo };
+        uint64_t **sa[2] = { &R->R.s_key, &R->R.s_lo };
+        rc = stream_grow(s,D,R->sc,ca,KW == 2 ? 3 : 2,&R->R.cand_cap,(int64_t) nc,(int64_t) nc + cut/2 + 1024,c0,"candidate");
+        if (rc == HM_OK)
+          rc = stream_grow(s,D,R->sc,sa,KW,&R->R.s_cap,(int64_t) ns,(int64_t) ns + cut + 1024,c0,"S");
+        if (rc != HM_OK) break;
+      }
+      rc = hm_k_build_bucket_index(R->keys[b],m,R->bits,R->bucket,0,R->sc);
+      if (rc == HM_OK)
+        rc = hm_k_symm_fingerprint(R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],0,cut,s->kmer,s->seed,D->fp_acc,R->sc);
+      if (rc == HM_OK)
+        rc = hm_symm_stream_chunk(R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],m,R->bucket,R->bits,s->kmer,cut,
+                                  R->work,&R->L,&R->R,R->sc);
+      s->launches += 4;
+      c0 += cut;
+      chunks += 1;
+      b ^= 1;
+    }
+  if (rc == HM_OK && (rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) == HM_OK)
+    rc = hm_sort_keys(R->R.s_key+ns0,KW == 2 ? R->R.s_lo+ns0 : NULL,(int64_t) (ns-ns0),s->kmer,
+                      R->sort_tmp,R->sort_bytes,R->sc);
+  cudaEventRecord(e1,R->sc);
+  cudaError_t e = cudaStreamSynchronize(R->sc);
+  if (rc == HM_OK && e != cudaSuccess) rc = hm_cuda_fail(e,"streamed scan: pass 1");
+  cudaEventElapsedTime(ms_kernels,e0,e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  s->chunks = chunks;
+  return rc;
+}
+
+static int run_stream_body(hm_scan *s, DevTable *D, StreamRun *R, int64_t *plot, hm_scan_stats *stats)
+{ int     KW = s->kmer > 32 ? 2 : 1, rc;
+  int64_t ixlen = (int64_t) 1 << (8*s->ibyte);
+  double  t0 = now_ms();
+  float   ms1 = 0, ms2 = 0;
+  cudaError_t e;
+  HM_CUDA(cudaSetDevice(D->dev));
+  HM_CUDA(cudaStreamCreateWithFlags(&R->sc,cudaStreamNonBlocking));
+  if ((rc = stream_work_layout(s->n,s->kmer,&R->L)) != HM_OK) return rc;
+  if ((e = salloc(s,D,(void **) &R->d_index,8*ixlen)) != cudaSuccess ||
+      (e = salloc(s,D,&R->work,R->L.bytes)) != cudaSuccess)
+    return hm_cuda_fail(e,"streamed scan: work area");
+  HM_CUDA(cudaMemcpyAsync(R->d_index,s->host->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,R->sc));
+  HM_CUDA(cudaMemsetAsync(D->fp_acc,0,4*sizeof(uint64_t),R->sc));
+  HM_CUDA(cudaMemsetAsync(D->plot,0,8*(size_t) HM_PLOT_CELLS,R->sc));
+  if ((rc = hm_symm_stream_begin(R->work,&R->L,R->sc)) != HM_OK) return rc;
+  HM_CUDA(cudaStreamSynchronize(R->sc));
+  if ((rc = stream_alloc_chunks(s,D,R,s->plan.chunk)) != HM_OK)
+    return rc == HM_ENOMEM ? hm_set_error(HM_ENOMEM,"the streamed scan's chunk buffers do not fit the device budget") : rc;
+  double t_load0 = now_ms();
+  if ((rc = stream_pass(s,D,R,&ms1)) != HM_OK)
+    return rc;
+  double t_pass1 = now_ms();
+
+  uint64_t nc = 0, status = 0, ns = 0;
+  if ((rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) != HM_OK) return rc;
+  if (status != 0)
+    return hm_set_error(HM_ECUDA,"streamed scan: list overflow in pass 1 (status %llu)",(unsigned long long) status);
+  if ((rc = fingerprint_verdict(s)) != HM_OK) return rc;
+  if (!s->symmetric)
+    return hm_set_error(HM_EUNSUPPORTED,"the table of %lld entries does not fit in device memory (budget %lld bytes) and "
+                        "is not strand-symmetric; the direct passes need it resident",(long long) s->n,(long long) s->budget);
+  /* S (sorted chunk by chunk) gets a bucket index in the room the chunk buffers leave: as fine as
+   * hm_pick_bucket_bits asks, coarser if the budget says so (look-ups then bisect longer buckets)        */
+  stream_free_chunks(s,D,R);
+  sfree(s,D,R->d_index,8*ixlen); R->d_index = NULL;
+  int sbits = hm_pick_bucket_bits((int64_t) ns), sidx64 = ((int64_t) ns >= 0xFFFFFFF0ll);
+  while (sbits > 1 && s->held + (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits)+1) > s->budget)
+    sbits -= 1;
+  R->s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits)+1);
+  if ((e = salloc(s,D,&R->s_bucket,R->s_bucket_bytes)) != cudaSuccess)
+    return hm_cuda_fail(e,"streamed scan: S index");
+  if ((rc = hm_k_build_bucket_index(R->R.s_key,(int64_t) ns,sbits,R->s_bucket,sidx64,R->sc)) != HM_OK) return rc;
+
+  cudaEvent_t e2, e3;
+  HM_CUDA(cudaEventCreate(&e2)); HM_CUDA(cudaEventCreate(&e3));
+  cudaEventRecord(e2,R->sc);
+  rc = hm_symm_stream_resolve(R->R.s_key,KW == 2 ? R->R.s_lo : NULL,(int64_t) ns,R->s_bucket,sbits,sidx64,s->kmer,
+                              s->n,R->work,&R->L,&R->R,D->plot,R->sc);
+  cudaEventRecord(e3,R->sc);
+  s->launches += 3;
+  if (rc == HM_OK && (e = cudaMemcpyAsync(plot,D->plot,sizeof(int64_t)*HM_PLOT_CELLS,cudaMemcpyDeviceToHost,R->sc)) != cudaSuccess)
+    rc = hm_cuda_fail(e,"plot D2H");
+  if (rc == HM_OK)
+    rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc);
+  cudaEventElapsedTime(&ms2,e2,e3);
+  cudaEventDestroy(e2); cudaEventDestroy(e3);
+  if (rc == HM_OK && status != 0)
+    rc = hm_set_error(HM_ECUDA,"streamed scan: pass 2 status %llu",(unsigned long long) status);
+  if (rc != HM_OK)
+    return rc;
+  double t1 = now_ms();
+  s->last_path = HM_PATH_SYMM;
+  if (stats != NULL)
+    { stats->nels = s->n; stats->n_gpus = 1; stats->bucket_bits = R->bits;
+      stats->filter_bits = 0; stats->path = HM_PATH_SYMM;
+      stats->ms_h2d_unpack = s->ms_load + (t_pass1-t_load0);    /* the loads, with pass 1 running behind them */
+      stats->ms_pass1 = ms1; stats->ms_pass2 = ms2;
+      stats->ms_scan = t1-t0;
+      stats->ms_total = s->ms_load + (t1-t0);
+      stats->kernel_launches = s->launches;
+      stats->ms_alloc = s->ms_alloc; stats->ms_records = t_pass1-t_load0; stats->ms_index = t1-t_pass1;
+    }
+  return HM_OK;
+}
+
+static int run_stream(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
+{ DevTable *D = s->d;
+  StreamRun R;
+  if (s->kmer < HM_SYMM_MIN_KMER)
+    return hm_set_error(HM_EUNSUPPORTED,"the table does not fit in device memory and k = %d has no strand-symmetric "
+                        "scan; the direct passes need it resident",s->kmer);
+  memset(&R,0,sizeof(R));
+  int64_t held0 = s->held;
+  s->peak = held0;
+  int rc = run_stream_body(s,D,&R,plot,stats);
+  cudaSetDevice(D->dev);
+  if (R.sc) cudaStreamSynchronize(R.sc);
+  stream_free_chunks(s,D,&R);
+  sfree(s,D,R.d_index,8*((int64_t) 1 << (8*s->ibyte)));
+  sfree(s,D,R.work,R.L.bytes);
+  sfree(s,D,R.s_bucket,R.s_bucket_bytes);
+  { int KW = s->kmer > 32 ? 2 : 1;
+    sfree(s,D,R.R.cand_key,8*R.R.cand_cap); sfree(s,D,R.R.cand_meta,8*R.R.cand_cap);
+    if (KW == 2) sfree(s,D,R.R.cand_lo,8*R.R.cand_cap);
+    sfree(s,D,R.R.s_key,8*R.R.s_cap);
+    if (KW == 2) sfree(s,D,R.R.s_lo,8*R.R.s_cap);
+  }
+  if (D->st) cudaStreamSynchronize(D->st);
+  if (R.sc) cudaStreamDestroy(R.sc);
+  cudaCtxResetPersistingL2Cache();
+  cudaGetLastError();
+  s->held = held0;
+  return rc;
+}
+
+/* examine_table's decisions on a streamed scan: the trim minimum over the same middle entries, chunk by
+ * chunk; the symmetry probe fetches entry sidx, and searches the stub-index bucket that must hold its
+ * reverse complement                                                                                     */
+static int examine_streamed(hm_scan *s, int ethresh, int *trim, int *symm)
+{ DevTable *D = s->d;
+  const hm_host_table *t = s->host;
+  int      KW = s->kmer > 32 ? 2 : 1, two = (KW == 2), rc = HM_OK;
+  int64_t  n = s->n, frst, last, cap = s->plan.chunk, ixlen = (int64_t) 1 << (8*s->ibyte);
+  int      h_min = 0x8000, *d_min = NULL;
+  uint64_t *keys = NULL, *klo = NULL, *d_q = NULL;
+  uint16_t *cnt = NULL;
+  int64_t  *d_index = NULL, *d_pos = NULL;
+  void     *bucket = NULL;
+  int      bits = hm_pick_bucket_bits(cap);
+  Stager   G;
+  memset(&G,0,sizeof(G));
+  HM_CUDA(cudaSetDevice(D->dev));
+  cudaError_t e = cudaMalloc(&keys,8*(size_t) (cap+1));
+  if (e == cudaSuccess && two) e = cudaMalloc(&klo,8*(size_t) (cap+1));
+  if (e == cudaSuccess) e = cudaMalloc(&cnt,2*(size_t) (cap+8));
+  if (e == cudaSuccess) e = cudaMalloc(&bucket,4*(((size_t) 1 << bits)+1));
+  if (e == cudaSuccess) e = cudaMalloc(&d_index,8*(size_t) ixlen);
+  if (e == cudaSuccess) e = cudaMalloc(&d_min,sizeof(int));
+  if (e == cudaSuccess) e = cudaMalloc(&d_q,2*sizeof(uint64_t));
+  if (e == cudaSuccess) e = cudaMalloc(&d_pos,sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaMemcpy(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(d_min,&h_min,sizeof(int),cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) rc = hm_cuda_fail(e,"streamed examine: buffers");
+  if (rc == HM_OK) rc = stager_open(s,D,t,cap,&G);
+
+  if (n+3 < 100000000) { frst = 0; last = n; }
+  else { frst = n/2-50000000; last = n/2+50000000; }
+  for (int64_t o = frst; o < last && rc == HM_OK; o += cap)
+    { int64_t m = last-o < cap ? last-o : cap;
+      rc = load_into(s,D,t,d_index,o,m,keys,klo,cnt,0,&G);
+      if (rc == HM_OK) rc = hm_k_min_count(cnt,0,m,d_min,D->st);
+      s->launches += 1;
+    }
+  if (rc == HM_OK)
+    { e = cudaMemcpyAsync(&h_min,d_min,sizeof(int),cudaMemcpyDeviceToHost,D->st);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(D->st);
+      if (e != cudaSuccess) rc = hm_cuda_fail(e,"min_count");
+    }
+  if (rc == HM_OK)
+    *trim = (h_min >= ethresh);
+
+  *symm = 1;
+  const int psh = 64 - 8*s->ibyte;                    /* the stub index is over the first ibyte bytes */
+  for (int64_t sidx = 1; sidx < n && rc == HM_OK; sidx++)
+    { uint64_t x, xw = 0, q[2];
+      int64_t  pos = -1;
+      if ((rc = load_into(s,D,t,d_index,sidx,1,keys,klo,cnt,0,&G)) != HM_OK) break;
+      e = cudaMemcpy(&x,keys,sizeof(uint64_t),cudaMemcpyDeviceToHost);
+      if (e == cudaSuccess && two) e = cudaMemcpy(&xw,klo,sizeof(uint64_t),cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) { rc = hm_cuda_fail(e,"examine: key fetch"); break; }
+      if (two) revcomp128(x,xw,s->kmer,q,q+1);
+      else     { q[0] = revcomp64(x,s->kmer); q[1] = 0; }
+      uint64_t p  = q[0] >> psh;
+      int64_t  b0 = p > 0 ? t->index[p-1] : 0, b1 = t->index[p];
+      HM_CUDA(cudaMemcpy(d_q,q,2*sizeof(uint64_t),cudaMemcpyHostToDevice));
+      for (int64_t o = b0; o < b1 && rc == HM_OK && pos < 0; o += cap)
+        { int64_t m = b1-o < cap ? b1-o : cap;
+          rc = load_into(s,D,t,d_index,o,m,keys,klo,cnt,0,&G);
+          if (rc == HM_OK) rc = hm_k_build_bucket_index(keys,m,bits,bucket,0,D->st);
+          if (rc == HM_OK) rc = hm_k_find_keys(keys,klo,m,bucket,bits,0,d_q,two ? d_q+1 : NULL,1,d_pos,D->st);
+          s->launches += 2;
+          if (rc != HM_OK) break;
+          e = cudaMemcpyAsync(&pos,d_pos,sizeof(int64_t),cudaMemcpyDeviceToHost,D->st);
+          if (e == cudaSuccess) e = cudaStreamSynchronize(D->st);
+          if (e != cudaSuccess) { rc = hm_cuda_fail(e,"examine: lookup"); break; }
+          if (pos >= 0) pos += o;
+        }
+      if (rc != HM_OK) break;
+      if (pos < 0) { *symm = 0; break; }
+      if (pos != sidx) { *symm = 1; break; }
+    }
+  stager_close(D,&G);
+  cudaFree(keys); cudaFree(klo); cudaFree(cnt); cudaFree(bucket); cudaFree(d_index);
+  cudaFree(d_min); cudaFree(d_q); cudaFree(d_pos);
+  return rc;
+}
+
 extern "C" int hm_scan_is_symmetric(const hm_scan *s) { return s->symmetric; }
 
 extern "C" int hm_scan_run_path(hm_scan *s, int path, int64_t *plot, hm_scan_stats *stats)
@@ -1005,6 +1605,14 @@ extern "C" int hm_scan_run_path(hm_scan *s, int path, int64_t *plot, hm_scan_sta
     { const char *e = getenv("HETMERS_PATH");
       if (e != NULL && strcmp(e,"direct") == 0) path = HM_PATH_DIRECT;
       if (e != NULL && strcmp(e,"symm") == 0)   path = HM_PATH_SYMM;
+    }
+  if (s->streamed)
+    { if (path == HM_PATH_DIRECT)
+        return hm_set_error(HM_EUNSUPPORTED,"the direct passes need the table resident; this one does not fit in "
+                                            "device memory (budget %lld bytes) and is streamed",(long long) s->budget);
+      if (path != HM_PATH_AUTO && path != HM_PATH_SYMM)
+        return hm_set_error(HM_EINVAL,"hm_scan_run_path: unknown path %d",path);
+      return run_stream(s,plot,stats);
     }
   if (path == HM_PATH_DIRECT || (path == HM_PATH_AUTO && !s->symmetric))
     return run_direct(s,plot,stats);
@@ -1055,6 +1663,9 @@ static int rec_cmp(const void *a, const void *b)
  * recorded partners of a preceding hm_scan_run.  Two launches per GPU: count, then fill.        */
 extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out)
 { int G = s->ngpu, rc = HM_OK;
+  if (s->streamed)
+    return hm_set_error(HM_EUNSUPPORTED,"listing k-mer pairs needs the direct passes' arrays, and this table does not "
+                                        "fit in device memory (budget %lld bytes)",(long long) s->budget);
   if (s->invalid)
     return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
   if ((rc = need_direct_results(s)) != HM_OK)
@@ -1123,6 +1734,8 @@ extern "C" int hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpu
 
 extern "C" int hm_scan_download(hm_scan *s, uint64_t *keys, uint64_t *keys_lo, uint16_t *cnt, uint8_t *deg)
 { DevTable *D = s->d;
+  if (s->streamed)
+    return hm_set_error(HM_EUNSUPPORTED,"a streamed scan holds no table on the device to download");
   HM_CUDA(cudaSetDevice(D->dev));
   HM_CUDA(cudaStreamSynchronize(D->st));
   if (keys != NULL)

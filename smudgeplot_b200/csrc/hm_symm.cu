@@ -386,11 +386,35 @@ __device__ __forceinline__ void stage_candidates(const RsSmem<KW> &S, unsigned *
     }
 }
 
+/* streamed scan (SL = true): every key that goes into the Bloom filter is also appended to the S list, so that
+ * the list is exactly the set the filter over-approximates.  Header words 3..6 of the work area hold the list's
+ * count, capacity and arrays (the kernels' parameters stay those of the in-core scan); one atomic per warp.   */
+#define SY_HDR_S 3
+
 template <int KW>
+__device__ __forceinline__ void s_push(const SymmView &W, uint64_t x, uint64_t xl)
+{ unsigned long long *h = W.cand_n + SY_HDR_S;         /* count, capacity, key array, second-word array */
+  const unsigned m = __activemask();
+  const int      lane = threadIdx.x & 31, lead = __ffs(m)-1;
+  unsigned long long at = 0;
+  if (lane == lead)
+    at = atomicAdd(h,(unsigned long long) __popc(m));
+  at = __shfl_sync(m,at,lead) + (unsigned long long) __popc(m & ((1u << lane)-1));
+  if (at < h[1])
+    { ((uint64_t *) h[2])[at] = x;
+      if (KW == 2) ((uint64_t *) h[3])[at] = xl;
+    }
+  else
+    atomicOr(W.status,SY_STATUS_OVERFLOW);
+}
+
+template <int KW, bool SL>
 __device__ __forceinline__ void bloom_insert(const SymmView &W, int kmer, uint64_t x, uint64_t xl)
 { uint32_t *word, mask;
   bloom_slot<KW>(W,W.self,kmer,x,xl,word,mask);
   atomicOr(word,mask);
+  if (SL)
+    s_push<KW>(W,x,xl);
 }
 
 /* Pass 1b: the runs of three or more entries (1-2 % of the entries; collisions of a heterozygous pair
@@ -400,7 +424,7 @@ __device__ __forceinline__ void bloom_insert(const SymmView &W, int kmer, uint64
  *   3..8 entries: every pair once, the members' partner counts packed into nibbles
  *   longer:       the warp takes the run together, one member per lane and trip, with one bucket
  *                 look-up per candidate partner (neighbours_slow) -- dense / tiny-k tables live here   */
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(256)
 runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
             const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
@@ -451,7 +475,7 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
             { const int64_t g = h+i;
               if (g < lo || g >= hi) continue;
               if (((U >> (4*i)) & 15) != 0)
-                bloom_insert<KW>(W,kmer,__ldg(keys+g),KW == 2 ? __ldg(keys_lo+g) : 0);
+                bloom_insert<KW,SL>(W,kmer,__ldg(keys+g),KW == 2 ? __ldg(keys_lo+g) : 0);
               const int j = (int) ((PT >> (3*i)) & 7);
               if (((H >> (4*i)) & 15) == 1 && j > i && ((H >> (4*j)) & 15) == 1)
                 nrec += 1;
@@ -517,7 +541,7 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
                   int Hn, Un, ppos; int64_t part;
                   neighbours_slow<IdxT,KW>(keys,keys_lo,cnt,bucket,bshift,kmer,Pr,pup,x,xl,cx,Hn,Un,part,ppos);
                   if (Un > 0)
-                    bloom_insert<KW>(W,kmer,x,xl);
+                    bloom_insert<KW,SL>(W,kmer,x,xl);
                   if (Hn == 1 && part > g)
                     { const uint64_t y = __ldg(keys+part), yl = KW == 2 ? __ldg(keys_lo+part) : 0;
                       const int cy = __ldg(cnt+part);
@@ -569,7 +593,7 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
  * (The alternatives -- every entry scanning its run in place, per-entry classification with predicated
  * list writes, CTA-wide task lists with a barrier per phase, longer runs handled by single lanes of
  * every warp in place -- need more instructions, leave more lanes idle or wait at the barriers.)      */
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(RS_THREADS,RS_MINBLOCKS)
 runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
@@ -725,8 +749,8 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
             { emit = true;
               meta = pack_meta(cx,cy,pos,base_at<KW>(y,yl,pos));
               if (pos >= pup)                                              /* U(x) = U(y) = 1: both are in S */
-                { bloom_insert<KW>(W,kmer,x,xl);
-                  bloom_insert<KW>(W,kmer,y,yl);
+                { bloom_insert<KW,SL>(W,kmer,x,xl);
+                  bloom_insert<KW,SL>(W,kmer,y,yl);
                 }
             }
         }
@@ -786,7 +810,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
  * run are compared exactly once, the comparisons are spread evenly over the lanes, and the cost grows
  * with the run length instead of falling off a cliff as one thread per run does.  Runs of more than
  * RS_LONGRUN entries are listed for runs_kernel as before.                                            */
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(RS_THREADS,RS_MINBLOCKS)
 runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                      const uint16_t *__restrict__ cnt, int64_t n, int kmer, int64_t lo, int64_t hi,
@@ -950,7 +974,7 @@ runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
             { x = S.key[i];
               if (KW == 2) xl = S.klo[i];
               if (U > 0)
-                bloom_insert<KW>(W,kmer,x,xl);
+                bloom_insert<KW,SL>(W,kmer,x,xl);
               const int j = s_part[i];
               if (H == 1 && j > i && ((hu[j>>1] >> (16*(j&1))) & 0xffu) == 1)
                 { const uint64_t y = S.key[j], yl = KW == 2 ? S.klo[j] : 0;
@@ -1006,7 +1030,7 @@ runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
     }
 }
 
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL = false>
 static cudaError_t launch_runscan(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                   const void *bucket, int bits, int kmer, int64_t lo, int64_t hi,
                                   const SymmView &W, cudaStream_t st)
@@ -1028,35 +1052,35 @@ static cudaError_t launch_runscan(const uint64_t *keys, const uint64_t *keys_lo,
     { size_t smem = (size_t) RS_WIN*(8*KW+2) + (size_t) RS_STAGE*8*(KW+1) +
                     2*(size_t) (RS_WIN+RS_TILE/8+RS_WIN) + 4*(size_t) (RS_WIN/2+RS_WIN);   /* 52 KB (k <= 32) / 74 KB */
       if (smem > 48*1024 && (dev >= 64 || !(configured[dev] & 2)))
-        { e = cudaFuncSetAttribute(runscan_dense_kernel<IdxT,KW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
+        { e = cudaFuncSetAttribute(runscan_dense_kernel<IdxT,KW,SL>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
           if (e != cudaSuccess) return e;
           if (dev < 64) configured[dev] |= 2;
         }
-      runscan_dense_kernel<IdxT,KW><<<(unsigned) (tile1-tile0),RS_THREADS,smem,st>>>
+      runscan_dense_kernel<IdxT,KW,SL><<<(unsigned) (tile1-tile0),RS_THREADS,smem,st>>>
           (keys,keys_lo,cnt,n,kmer,lo,hi,tile0,tma,W);
     }
   else
     { size_t smem = (size_t) RS_WIN*(8*KW+2) + (size_t) RS_STAGE*8*(KW+1) +
                     2*(size_t) (RS_TILE/2+RS_TILE/2);                                /* 34 KB (k <= 32) / 55 KB */
       if (smem > 48*1024 && (dev >= 64 || !(configured[dev] & 1)))
-        { e = cudaFuncSetAttribute(runscan_kernel<IdxT,KW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
+        { e = cudaFuncSetAttribute(runscan_kernel<IdxT,KW,SL>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
           if (e != cudaSuccess) return e;
           if (dev < 64) configured[dev] |= 1;
         }
-      runscan_kernel<IdxT,KW><<<(unsigned) (tile1-tile0),RS_THREADS,smem,st>>>
+      runscan_kernel<IdxT,KW,SL><<<(unsigned) (tile1-tile0),RS_THREADS,smem,st>>>
           (keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,lo,hi,tile0,tma,W);
     }
   return cudaGetLastError();
 }
 
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL = false>
 static cudaError_t launch_runs(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                const void *bucket, int bits, int kmer, int64_t lo, int64_t hi,
                                const SymmView &W, cudaStream_t st)
 { /* (the Bloom filter is filled inside runscan_kernel: a kernel of its own would read the records once more) */
   int64_t want = ((hi-lo)/64+255)/256;                        /* ~1 run of three or more per 60 entries: a thread each */
   int     grid = (int) (want < 0x7fffffff ? (want > 0 ? want : 1) : 0x7fffffff);
-  runs_kernel<IdxT,KW><<<grid,256,0,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,lo,hi,W);
+  runs_kernel<IdxT,KW,SL><<<grid,256,0,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,lo,hi,W);
   return cudaGetLastError();
 }
 
@@ -1184,9 +1208,10 @@ __device__ __noinline__ bool has_upper_partner(const uint64_t *__restrict__ keys
   return (U > 0);
 }
 
-/* one candidate: are rc x / rc y in S?  Bloom bits first; EXACT = also settle the hits.
- * -> 0 isolated pair, 1 not isolated, 2 undecided (a Bloom hit, EXACT == false)                  */
-template <typename IdxT, int KW, bool EXACT>
+/* one candidate: are rc x / rc y in S?  Bloom bits first; EXACT = also settle the hits: SL = false looks
+ * for an upper partner in the table, SL = true (streamed scan: keys / bucket are the sorted S list and its
+ * index) looks the key up in S.  -> 0 isolated pair, 1 not isolated, 2 undecided (a Bloom hit, EXACT == false) */
+template <typename IdxT, int KW, bool EXACT, bool SL>
 __device__ __forceinline__ int judge_candidate(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                                                const uint16_t *__restrict__ cnt, int64_t n,
                                                const IdxT *__restrict__ bucket, int bshift, int kmer,
@@ -1207,6 +1232,9 @@ __device__ __forceinline__ int judge_candidate(const uint64_t *__restrict__ keys
     return 0;
   if (!EXACT)
     return 2;
+  if (SL)
+    return ((ha && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
+            (hb && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0)) ? 1 : 0;
   if (ha && has_upper_partner<IdxT,KW>(keys,keys_lo,cnt,n,bucket,bshift,kmer,rx,rxl,cx,W.status))
     return 1;
   if (hb && has_upper_partner<IdxT,KW>(keys,keys_lo,cnt,n,bucket,bshift,kmer,ry,ryl,cy,W.status))
@@ -1232,7 +1260,7 @@ __device__ __forceinline__ void count_pair(uint32_t *tile, unsigned long long *_
  * lane does that stalls all 32: they are parked in a per-warp queue and settled 32 at a time, every
  * lane busy.  RV_ILP candidates per thread and trip keep that many record / Bloom loads in flight
  * (the kernel is bound by the latency of record -> Bloom word, not by bytes or instructions).         */
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(RV_THREADS,RV_CTAS_PER_SM)
 resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
@@ -1302,7 +1330,7 @@ resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
           __syncwarp();
           const int64_t j = first-lane + (int64_t) (e & 31) + (int64_t) (e >> 5)*stride;
           const uint64_t xx = W.cand_key[j], xxl = KW == 2 ? W.cand_lo[j] : 0, mm = W.cand_meta[j];
-          if (judge_candidate<IdxT,KW,true>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm) == 0)
+          if (judge_candidate<IdxT,KW,true,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm) == 0)
             count_pair(tile,plot,mm,kmer);
         }
     }
@@ -1310,7 +1338,7 @@ resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
     { const uint32_t e = q[lane];
       const int64_t j = first-lane + (int64_t) (e & 31) + (int64_t) (e >> 5)*stride;
       const uint64_t xx = W.cand_key[j], xxl = KW == 2 ? W.cand_lo[j] : 0, mm = W.cand_meta[j];
-      if (judge_candidate<IdxT,KW,true>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm) == 0)
+      if (judge_candidate<IdxT,KW,true,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm) == 0)
         count_pair(tile,plot,mm,kmer);
     }
   __syncthreads();
@@ -1321,7 +1349,7 @@ resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
     }
 }
 
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool SL = false>
 static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                   const void *bucket, int bits, int kmer, const SymmView &W,
                                   unsigned long long *plot, int64_t range, cudaStream_t st)
@@ -1330,14 +1358,14 @@ static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo,
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (dev >= 64 || !configured[dev])
-    { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
+    { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW,SL>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
       if (e != cudaSuccess) return e;
       if (dev < 64) configured[dev] = 1;
     }
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = (range/8+RV_THREADS-1)/RV_THREADS;            /* ~1 candidate per 10 entries */
   int     grid = (int) (want < sms*RV_CTAS_PER_SM ? (want > 0 ? want : 1) : sms*RV_CTAS_PER_SM);
-  resolve_kernel<IdxT,KW><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
+  resolve_kernel<IdxT,KW,SL><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
   return cudaGetLastError();
 }
 
@@ -1398,5 +1426,90 @@ extern "C" int hm_symm_align_cut(const uint64_t *d_keys, int64_t n, int kmer, in
       cut += m;
     }
   *out = n;
+  return HM_OK;
+}
+
+/* ------------------------------------------------------------------ streamed scan -------- */
+/* The table passes through the GPU chunk by chunk (hm_scan.cu drives it, DESIGN.md §4c).  The work area of
+ * hm_symm_plan(n, 0, kmer, 1) supplies the header and the whole-table Bloom filter (only they are used); the
+ * run list of one chunk, the candidate records and the S list are arrays of the caller's, the last two
+ * resident and grown between chunks.                                                                      */
+static SymmView stream_view(void *d_work, const hm_symm_layout *L, const hm_stream_lists *R)
+{ SymmView W = make_view(d_work,L,NULL);
+  W.cand_key = R->cand_key; W.cand_lo = R->cand_lo; W.cand_meta = R->cand_meta;
+  W.cand_cap = (unsigned long long) R->cand_cap;
+  W.runs = R->runs; W.runs_cap = (unsigned long long) R->runs_cap;
+  return W;
+}
+
+int hm_symm_stream_begin(void *d_work, const hm_symm_layout *L, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = make_view(d_work,L,NULL);
+  HM_CUDA(cudaMemsetAsync(W.cand_n,0,256,st));
+  HM_CUDA(cudaMemsetAsync(W.bloom,0,sizeof(uint32_t)*(size_t) W.seg_words,st));
+  if (l2_persist())
+    bloom_window(st,W.bloom,sizeof(uint32_t)*(size_t) W.seg_words,1);
+  return HM_OK;
+}
+
+int hm_symm_stream_chunk(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                                    int64_t n, const void *d_bucket, int bits, int kmer, int64_t hi,
+                                    void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || hi < 0 || hi > n || bits < 1 || bits > 30 ||
+      (kmer > 32) != (d_keys_lo != NULL))
+    return hm_set_error(HM_EINVAL,"symm_stream_chunk: bad arguments (k=%d, %lld of %lld entries)",
+                        kmer,(long long) hi,(long long) n);
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = stream_view(d_work,L,R);
+  uint64_t h[4] = { (uint64_t) R->s_cap, (uint64_t) (uintptr_t) R->s_key, (uint64_t) (uintptr_t) R->s_lo, 0 };
+  HM_CUDA(cudaMemsetAsync(W.runs_n,0,sizeof(uint64_t),st));                 /* the run list is per chunk */
+  HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_S+1,h,3*sizeof(uint64_t),cudaMemcpyHostToDevice,st));
+  if (hi == 0)
+    return HM_OK;
+  cudaError_t e;
+  if (kmer <= 32)
+    { e = launch_runscan<uint32_t,1,true>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,0,hi,W,st);
+      if (e == cudaSuccess) e = launch_runs<uint32_t,1,true>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,0,hi,W,st);
+    }
+  else
+    { e = launch_runscan<uint32_t,2,true>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,0,hi,W,st);
+      if (e == cudaSuccess) e = launch_runs<uint32_t,2,true>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,0,hi,W,st);
+    }
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"runscan_kernel / runs_kernel (streamed)");
+  return HM_OK;
+}
+
+/* header words: candidates so far, status bits, S entries so far (synchronises) */
+int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t *n_cand,
+                                     uint64_t *status, uint64_t *n_s, void *stream)
+{ uint64_t h[SY_HDR_S+1];
+  HM_CUDA(cudaMemcpyAsync(h,(const uint8_t *) d_work + L->off_header,sizeof(h),cudaMemcpyDeviceToHost,
+                          (cudaStream_t) stream));
+  HM_CUDA(cudaStreamSynchronize((cudaStream_t) stream));
+  *n_cand = h[0]; *status = h[1]; *n_s = h[SY_HDR_S];
+  return HM_OK;
+}
+
+/* pass 2 of the streamed scan: the exact check of a Bloom hit is a look-up in the sorted S list */
+int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
+                                      const void *d_s_bucket, int bits, int idx64, int kmer, int64_t range,
+                                      void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                                      unsigned long long *d_plot, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_plot == NULL)
+    return hm_set_error(HM_EINVAL,"symm_stream_resolve: bad arguments");
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = stream_view(d_work,L,R);
+  cudaError_t e;
+  if (kmer <= 32)
+    e = idx64 ? launch_resolve<uint64_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
+              : launch_resolve<uint32_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
+  else
+    e = idx64 ? launch_resolve<uint64_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
+              : launch_resolve<uint32_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
+  if (l2_persist())
+    bloom_window(st,NULL,0,0);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"resolve_kernel (streamed)");
   return HM_OK;
 }

@@ -100,13 +100,18 @@ def _host_table(kt: KtabFiles):
 
 
 class Scan:
-    """Device-resident table + both passes (hm_scan_*)."""
+    """Device-resident table + both passes (hm_scan_*).  A table whose in-core scan does not fit the device
+    budget is streamed through the GPU on every run() instead (residency()); device_budget (bytes per GPU)
+    sets that budget for this and later scans of the process (0: free device memory minus a reserve)."""
 
-    def __init__(self, kt: KtabFiles, gpus: int = 1, devices=None):
+    def __init__(self, kt: KtabFiles, gpus: int = 1, devices=None, device_budget: int | None = None):
         L = _lib.lib()
         self._L = L
         self.kt = kt
-        ht, self._keep = _host_table(kt)
+        if device_budget is not None:
+            L.hm_set_device_budget(int(device_budget))
+        ht, self._keep = _host_table(kt)          # a streamed scan reads these buffers on every run
+        self._ht = ht
         devs = list(devices) if devices is not None else list(range(gpus))
         arr = (C.c_int * len(devs))(*devs)
         h = C.c_void_p()
@@ -128,6 +133,12 @@ class Scan:
         return n.value
 
     PATHS = {"auto": 0, "direct": 1, "symm": 2}
+
+    def residency(self):
+        """-> (streamed?, peak device bytes per GPU, chunks of the last run)"""
+        b, c = C.c_int64(), C.c_int64()
+        r = self._L.hm_scan_residency(self._h, C.byref(b), C.byref(c))
+        return bool(r), b.value, c.value
 
     def is_symmetric(self) -> bool:
         """whole-table verdict of the symmetry fingerprint (hm_scan_create / hm_scan_condition)"""

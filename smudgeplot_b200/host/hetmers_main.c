@@ -358,7 +358,8 @@ int main(int argc, char *argv[])
   start_cuda_early();            /* background: nothing below waits for it before hm_device_count() */
 
   { char *command, *tname;
-    int   symm, trim;
+    int   symm, trim, condition_rc = HM_OK;
+    int64_t conditioned_n = 0;
 
     tname   = malloc(strlen(SRC) + strlen(troot) + 10);
     command = malloc(strlen(SRC) + strlen(troot) + strlen(SORT_PATH) + 100);
@@ -375,6 +376,10 @@ int main(int argc, char *argv[])
     t_open = wall_ms();
     ngpu = pick_gpus(devs);        /* after the table is known to exist: same first error as the reference */
     hm_set_io_threads(NTHREADS);   /* -T = host threads staging the part files towards the GPU */
+    { const char *b = getenv("HETMERS_DEVICE_BUDGET");     /* device bytes the scan may hold per GPU */
+      if (b != NULL && *b != '\0')
+        hm_set_device_budget(strtoll(b,NULL,10));
+    }
     if (hm_table_view(T)->nels < 2)
       { fprintf(stderr,"%s: k-mer table %s has fewer than 2 entries\n",Prog_Name,SRC);
         exit (1);
@@ -406,14 +411,16 @@ int main(int argc, char *argv[])
       { free(command);                 //  nothing to do: the table is scanned as it is
         free(tname);
       }
-    else if (getenv("HETMERS_EXTERNAL_CONDITIONING") == NULL)
+    else if (getenv("HETMERS_EXTERNAL_CONDITIONING") == NULL && !hm_scan_residency(S,NULL,NULL) &&
+             (condition_rc = hm_scan_condition(S,ETHRESH,!trim,!symm,&conditioned_n)) != HM_ENOMEM)
       { //  Condition the table where it already is -- on the GPU -- instead of shelling out to
-        //  FastK's Logex / Symmex and re-reading their output (same progress lines with -v)
-        int64_t nn;
+        //  FastK's Logex / Symmex and re-reading their output (same progress lines with -v).  A table
+        //  that is streamed, or too large to condition within the device budget, takes the shell-outs below.
+        int64_t nn = conditioned_n;
+        if (condition_rc != HM_OK)
+          die_hm();
         if (!trim) announce_step(VERBOSE,'t',trim,ETHRESH);
         if (!symm) announce_step(VERBOSE,'s',trim,ETHRESH);
-        if (hm_scan_condition(S,ETHRESH,!trim,!symm,&nn) != HM_OK)
-          die_hm();
         if (nn < 2)
           { fprintf(stderr,"%s: fewer than 2 k-mers are left after conditioning\n",Prog_Name);
             exit (1);
@@ -483,15 +490,20 @@ int main(int argc, char *argv[])
   //   context by hand costs ~0.1 s of wall clock for nothing)
 
   if (getenv("HETMERS_STATS") != NULL)
-    fprintf(stderr,"{\"nels\": %lld, \"n_gpus\": %d, \"path\": \"%s\", \"bucket_bits\": %d, \"ms_load\": %.3f, "
+    { int64_t dev_bytes = 0, chunks = 0;
+      int     streamed = hm_scan_residency(S,&dev_bytes,&chunks);
+      fprintf(stderr,"{\"nels\": %lld, \"n_gpus\": %d, \"path\": \"%s\", \"bucket_bits\": %d, \"ms_load\": %.3f, "
                    "\"ms_pass1\": %.3f, \"ms_pass2\": %.3f, \"ms_scan\": %.3f, \"kernel_launches\": %lld, "
+                   "\"streamed\": %s, \"chunks\": %lld, \"device_bytes\": %lld, "
                    "\"wall_ms\": {\"open\": %.1f, \"cuda_init_load\": %.1f, \"examine\": %.1f, \"scan\": %.1f}, "
                    "\"load_ms\": {\"alloc\": %.1f, \"records\": %.1f, \"index\": %.1f}}\n",
             (long long) stats.nels,stats.n_gpus,stats.path == HM_PATH_SYMM ? "symmetric" : "direct",
             stats.bucket_bits,stats.ms_h2d_unpack,
             stats.ms_pass1,stats.ms_pass2,stats.ms_scan,(long long) stats.kernel_launches,
+            streamed ? "true" : "false",(long long) chunks,(long long) dev_bytes,
             t_open-t_start,t_load-t_open,t_exam-t_load,t_scan-t_exam,
             stats.ms_alloc,stats.ms_records,stats.ms_index);
+    }
 
   if (input != NULL)                                              /* PloidyPlot.c:1584-1592 */
     { char *command = malloc(strlen(input)+100);
