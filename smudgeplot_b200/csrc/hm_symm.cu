@@ -22,10 +22,11 @@
  *                             either way.
  *   runscan_kernel            ("pass 1") tiles of the sorted table are staged into shared memory by
  *                             TMA bulk copies; entries are classified by the adjacency of their
- *                             runs, runs of two are settled by one comparison (H, U, the partner).
+ *                             runs, runs of two are settled by one comparison (H, U, the partner),
+ *                             runs of three to RS_RUNCAP entries from the same shared-memory window.
  *                             Entries with U > 0 (the set S) are added to a Bloom filter; pairs
  *                             (x < y) with H(x) = H(y) = 1 become candidate records.
- *   runs_kernel               the runs of three or more entries that runscan_kernel only lists
+ *   runs_kernel               the runs runscan_kernel only lists (longer than its window can hold)
  *   runscan_dense_kernel      pass 1 for crowded tables (many run mates per entry): all pairs of
  *                             every run, counted with shared-memory atomics
  *   resolve_kernel            ("pass 2") a candidate is an isolated pair iff neither rc x nor rc y
@@ -54,6 +55,8 @@
 #define RS_HALO    64                          /* entries staged on either side of the tile      */
 #define RS_WIN     (RS_TILE+2*RS_HALO)
 #define RS_SCANCAP RS_HALO                     /* longest run half scanned linearly               */
+#define RS_RUNCAP  (RS_HALO+1)                 /* runscan_kernel settles runs of up to this many entries itself:
+                                                *   a run whose head lies in the tile is then inside the window  */
 #define RS_LONGRUN 32                          /* dense kernel: runs of more entries go to runs_kernel */
 #ifndef RS_MINBLOCKS
 #define RS_MINBLOCKS 5                         /* resident CTAs per SM the register budget must allow (48 regs, no
@@ -340,8 +343,8 @@ template <int KW> struct RsSmem
   { uint64_t *key, *klo;                /* window: RS_WIN slots (+1 spare)                        */
     uint16_t *cnt;
     uint64_t *ckey, *clo, *cmeta;       /* staged candidate records: RS_STAGE                     */
-    uint16_t *t1;                       /* per warp: heads of two-entry runs (RS_TILE/2 in all)    */
-    uint16_t *t2r;                      /* CTA: heads of longer runs                               */
+    uint16_t *t1;                       /* per warp: heads of runs of two, then of longer runs (RS_TILE/2 in all) */
+    uint16_t *t2r;                      /* CTA: heads of runs left to runs_kernel                  */
   };
 
 __device__ __forceinline__ uint64_t pack_meta(int cx, int cy, int pos, int yb)
@@ -417,13 +420,12 @@ __device__ __forceinline__ void bloom_insert(const SymmView &W, int kmer, uint64
     s_push<KW>(W,x,xl);
 }
 
-/* Pass 1b: the runs of three or more entries (1-2 % of the entries; collisions of a heterozygous pair
- * with an unrelated k-mer, repeats, low-complexity sequence) are irregular work: runscan_kernel only
- * lists their heads, this kernel takes one run per thread, straight from global memory (the keys of a
- * run are neighbours in the table).
- *   3..8 entries: every pair once, the members' partner counts packed into nibbles
- *   longer:       the warp takes the run together, one member per lane and trip, with one bucket
- *                 look-up per candidate partner (neighbours_slow) -- dense / tiny-k tables live here   */
+/* Pass 1b: the runs runscan_kernel only lists -- more than RS_RUNCAP entries (or runs that may reach
+ * past its window), and on crowded tables the runs runscan_dense_kernel leaves (more than RS_LONGRUN):
+ * repeats, low-complexity sequence, tiny k.  The listed count is only known on the device, so the grid
+ * is at most one wave and strides over the list.  Each warp takes its lanes' runs one after the other,
+ * straight from global memory (the keys of a run are neighbours in the table): one member per lane and
+ * trip, with one bucket look-up per candidate partner (neighbours_slow).                              */
 template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(256)
 runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
@@ -443,85 +445,17 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
       const bool    valid = (r < nr);
       int64_t  h = 0;
       uint64_t x0 = 0;
-      int      L = 1;
       if (valid)
         { h  = (int64_t) W.runs[r];
           x0 = __ldg(keys+h);
-          while (L <= 8 && h+L < n && ((__ldg(keys+h+L) ^ x0) & pmask) == 0)
-            L += 1;
         }
-      const bool islong = valid && (L > 8);
-      /* ---- short run: all pairs ---- */
-      uint32_t H = 0, U = 0, PT = 0;
-      uint64_t PP = 0;
-      int      nrec = 0;
-      if (valid && !islong)
-        { for (int i = 0; i+1 < L; i++)
-            { const uint64_t xi = __ldg(keys+h+i), xil = KW == 2 ? __ldg(keys_lo+h+i) : 0;
-              const int      ci = __ldg(cnt+h+i);
-              for (int j = i+1; j < L; j++)
-                { int pos;
-                  if (one_base_apart<KW>(xi,xil,__ldg(keys+h+j),KW == 2 ? __ldg(keys_lo+h+j) : 0,pos) &&
-                      ci + (int) __ldg(cnt+h+j) <= HM_SMAX)
-                    { H += (1u << (4*i)) + (1u << (4*j));
-                      if (pos >= pup) U += (1u << (4*i)) + (1u << (4*j));
-                      PT = (PT & ~((7u << (3*i)) | (7u << (3*j)))) | ((uint32_t) j << (3*i)) | ((uint32_t) i << (3*j));
-                      PP = (PP & ~(((uint64_t) 255 << (8*i)) | ((uint64_t) 255 << (8*j)))) |
-                           ((uint64_t) pos << (8*i)) | ((uint64_t) pos << (8*j));
-                    }
-                }
-            }
-          for (int i = 0; i < L; i++)
-            { const int64_t g = h+i;
-              if (g < lo || g >= hi) continue;
-              if (((U >> (4*i)) & 15) != 0)
-                bloom_insert<KW,SL>(W,kmer,__ldg(keys+g),KW == 2 ? __ldg(keys_lo+g) : 0);
-              const int j = (int) ((PT >> (3*i)) & 7);
-              if (((H >> (4*i)) & 15) == 1 && j > i && ((H >> (4*j)) & 15) == 1)
-                nrec += 1;
-            }
-        }
-      /* candidate records of the short runs: one global atomic per warp */
-      { int pre = nrec;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1)
-          { int v = __shfl_up_sync(FULL,pre,o);
-            if (lane >= o) pre += v;
-          }
-        const int tot = __shfl_sync(FULL,pre,31);
-        if (tot > 0)
-          { unsigned long long base = 0;
-            if (lane == 0)
-              base = atomicAdd(W.cand_n,(unsigned long long) tot);
-            base = __shfl_sync(FULL,base,0) + (unsigned long long) (pre-nrec);
-            if (nrec > 0)
-              for (int i = 0; i < L; i++)
-                { const int64_t g = h+i;
-                  if (g < lo || g >= hi) continue;
-                  const int j = (int) ((PT >> (3*i)) & 7);
-                  if (((H >> (4*i)) & 15) == 1 && j > i && ((H >> (4*j)) & 15) == 1)
-                    { const int      pos = (int) ((PP >> (8*i)) & 255);
-                      const uint64_t y = __ldg(keys+h+j), yl = KW == 2 ? __ldg(keys_lo+h+j) : 0;
-                      if (base < W.cand_cap)
-                        { W.cand_key[base] = __ldg(keys+g);
-                          if (KW == 2) W.cand_lo[base] = __ldg(keys_lo+g);
-                          W.cand_meta[base] = pack_meta(__ldg(cnt+g),__ldg(cnt+h+j),pos,base_at<KW>(y,yl,pos));
-                        }
-                      else
-                        atomicOr(W.status,SY_STATUS_OVERFLOW);
-                      base += 1;
-                    }
-                }
-          }
-      }
-      /* ---- long runs: the whole warp, one after the other ---- */
-      unsigned lb = __ballot_sync(FULL,islong);
+      unsigned lb = __ballot_sync(FULL,valid);
       while (lb != 0)
         { const int     src = __ffs(lb)-1;
           lb &= lb-1;
           const int64_t hh = __shfl_sync(FULL,h,src);
           const uint64_t xx = __shfl_sync(FULL,x0,src);
-          int64_t end = hh+9;                          /* entries hh .. hh+8 are known to be in the run */
+          int64_t end = hh+1;
           while (true)
             { const int64_t t = end+lane;
               const bool same = (t < n) && (((__ldg(keys+t) ^ xx) & pmask) == 0);
@@ -574,6 +508,42 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
     }
 }
 
+/* runscan_kernel, step 4: member a of the run of L entries at window slots h .. h+L-1.  Its partners in the
+ * run give H and U (Bloom insert when U > 0); a candidate record when H(x) = H(partner) = 1 and x is the
+ * lower member (the partner's H is counted here too, so no member waits for another's counts).  -> emit  */
+template <int KW, bool SL>
+__device__ __forceinline__ bool settle_member(const RsSmem<KW> &S, const SymmView &W, int kmer, int pup,
+                                              int h, int L, int a, uint64_t &x, uint64_t &xl, uint64_t &meta)
+{ x  = S.key[h+a];
+  xl = KW == 2 ? S.klo[h+a] : 0;
+  const int cx = S.cnt[h+a];
+  int Hx = 0, Ux = 0, part = 0, ppos = 0;
+  for (int b = 0; b < L; b++)
+    { int pos;
+      if (b != a && one_base_apart<KW>(x,xl,S.key[h+b],KW == 2 ? S.klo[h+b] : 0,pos) && cx + (int) S.cnt[h+b] <= HM_SMAX)
+        { Hx += 1;
+          if (pos >= pup) Ux += 1;
+          part = b; ppos = pos;
+        }
+    }
+  if (Ux > 0)
+    bloom_insert<KW,SL>(W,kmer,x,xl);
+  if (Hx != 1 || part < a)
+    return false;
+  const uint64_t y = S.key[h+part], yl = KW == 2 ? S.klo[h+part] : 0;
+  const int      cy = S.cnt[h+part];
+  int Hy = 0;
+  for (int b = 0; b < L; b++)
+    { int pos;
+      if (b != part && one_base_apart<KW>(y,yl,S.key[h+b],KW == 2 ? S.klo[h+b] : 0,pos) && cy + (int) S.cnt[h+b] <= HM_SMAX)
+        Hy += 1;
+    }
+  if (Hy != 1)
+    return false;
+  meta = pack_meta(cx,cy,ppos,base_at<KW>(y,yl,ppos));
+  return true;
+}
+
 /* Pass 1.  83 % of the entries of a genome-sized table are alone in their run (no other entry shares
  * their first k/2 bases) and 15 % sit in a run of exactly two -- almost always the two alleles of one
  * heterozygous site.  The kernel is limited by instruction issue and by the latency of its few serial
@@ -585,14 +555,20 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
  *   2. classification of 8 x 32 entries with bit operations, one WORD PER LANE:
  *      head of a two-entry run / head of a longer run / nothing
  *   3. two-entry runs: one comparison settles both members (per-warp task list, every lane busy)
- *   4. heads of longer runs are only LISTED (1-2 % of the entries, irregular work): runs_kernel
- *      takes them one per thread afterwards
+ *   4. longer runs (5 % of the entries, a few per warp) from the same per-warp list, still from shared
+ *      memory: a run whose head is in the tile and that has at most RS_RUNCAP = RS_HALO+1 entries lies
+ *      inside the window.  3..8 entries: a lane per member, the members of all the warp's runs one
+ *      after the other (a run per lane, every pair once, costs the warp its longest run's L^2/2
+ *      comparisons and a staging call per member: 2.07-2.11 against 1.98-2.01 ms per benchmark step);
+ *      9..RS_RUNCAP: the whole warp, one member per lane.  Only runs that may reach past the window
+ *      are listed for runs_kernel (none in the 2e8-entry benchmark table, whose 3.4e6 runs of three or
+ *      more took runs_kernel 0.40 ms on one H100 SXM at 400 W when it settled them all)
  *   5. candidate records and run heads are staged in shared memory; the LAST warp to finish moves
  *      them out with one global atomic per CTA and list (one per record, or per warp, on the one
  *      list counter serialises in L2)
  * (The alternatives -- every entry scanning its run in place, per-entry classification with predicated
- * list writes, CTA-wide task lists with a barrier per phase, longer runs handled by single lanes of
- * every warp in place -- need more instructions, leave more lanes idle or wait at the barriers.)      */
+ * list writes, CTA-wide task lists with a barrier per phase -- need more instructions, leave more lanes
+ * idle or wait at the barriers.)                                                                      */
 template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(RS_THREADS,RS_MINBLOCKS)
 runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
@@ -687,7 +663,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
   const int a0 = RS_HALO + (lo > T0 ? (int) (lo-T0 < RS_TILE ? lo-T0 : RS_TILE) : 0);   /* slots this CTA answers for */
   const int a1 = RS_HALO + (hi-T0 < RS_TILE ? (int) (hi-T0) : RS_TILE);
   uint16_t *my1  = S.t1  + warp*(RS_TILE/2/(RS_THREADS/32));
-  int n1;
+  int n1, n3;
   { const unsigned P = __shfl_up_sync(FULL,eqw,1), N = __shfl_down_sync(FULL,eqw,1);
     unsigned m2 = 0, m3 = 0;
     const int wd = wd0-1+lane;
@@ -702,9 +678,10 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         if (s0+32 > a1)   act &= (a1-s0 <= 0)  ? 0u : (0xffffffffu >> (s0+32-a1));
         const unsigned more = (em1 & E) | (E & ep1) | (em1 & em2);
         m2 = (E & ~em1 & ~ep1) & act;                                  /* head of a run of exactly two */
-        m3 = more & act & ~em1;                                        /* head of a longer run: listed for runs_kernel */
+        m3 = more & act & ~em1;                                        /* head of a longer run */
       }
-    /* per-warp task lists: inclusive scans of the counts over the lanes */
+    /* per-warp task lists: inclusive scans of the counts over the lanes.  Heads of longer runs follow the
+     * heads of runs of two in the same list: two heads are at least two slots apart, so both fit in 128 */
     const int c2 = __popc(m2), c3 = __popc(m3);
     int pre2 = c2, pre3 = c3;
 #pragma unroll
@@ -713,21 +690,16 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         if (lane >= o) { pre2 += v2; pre3 += v3; }
       }
     n1 = __shfl_sync(FULL,pre2,RS_EPT);
-    const int n3 = __shfl_sync(FULL,pre3,RS_EPT);
+    n3 = __shfl_sync(FULL,pre3,RS_EPT);
     int at = pre2-c2;
     while (m2 != 0)
       { my1[at++] = (uint16_t) (wd*32 + __ffs(m2)-1);
         m2 &= m2-1;
       }
-    if (n3 > 0)                                          /* (warp-uniform) heads of longer runs: CTA list */
-      { unsigned b3 = 0;
-        if (lane == 0)
-          b3 = atomicAdd(&s_nr,(unsigned) n3);
-        at = (int) __shfl_sync(FULL,b3,0) + pre3-c3;
-        while (m3 != 0)
-          { S.t2r[at++] = (uint16_t) (wd*32 + __ffs(m3)-1);
-            m3 &= m3-1;
-          }
+    at = n1 + pre3-c3;
+    while (m3 != 0)
+      { my1[at++] = (uint16_t) (wd*32 + __ffs(m3)-1);
+        m3 &= m3-1;
       }
   }
   __syncwarp();
@@ -755,6 +727,72 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
             }
         }
       stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
+    }
+
+  /* ---- 4. longer runs, from the window: a run whose head is in the tile and that has at most RS_RUNCAP
+   *         entries lies inside it.  Members at or after hi are not ours (slots >= b1) ---- */
+  const int b1 = hi-T0 < RS_TILE+RS_HALO ? RS_HALO + (int) (hi-T0) : RS_WIN;
+  for (int i0 = 0; i0 < n3; i0 += 32)
+    { const int i = i0+lane;
+      int h = 0, L = 0;                                  /* head slot, run length (counted up to 9) */
+      if (i < n3)
+        { h = my1[n1+i];
+          const uint64_t xh = S.key[h];
+          L = 3;
+          while (L <= 8 && ((S.key[h+L] ^ xh) & pmask) == 0)        /* h+8 < RS_WIN */
+            L += 1;
+        }
+      /* 3..8 entries: a lane per member, the members of all the lanes' runs one after the other */
+      const int Ls = L <= 8 ? L : 0;
+      int inc = Ls;                                      /* inclusive scan of the members over the lanes */
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1)
+        { const int v = __shfl_up_sync(FULL,inc,o);
+          if (lane >= o) inc += v;
+        }
+      const int M = __shfl_sync(FULL,inc,31);
+      for (int t0 = 0; t0 < M; t0 += 32)
+        { const int t = t0+lane;
+          int r = 0;                                     /* member t's run: the first lane whose inc > t */
+#pragma unroll
+          for (int s = 16; s > 0; s >>= 1)
+            if (__shfl_sync(FULL,inc,r+s-1) <= t) r += s;
+          const int hr = __shfl_sync(FULL,h,r), Lr = __shfl_sync(FULL,Ls,r);
+          const int a  = t - (__shfl_sync(FULL,inc,r) - Lr);
+          bool     emit = false;
+          uint64_t x = 0, xl = 0, meta = 0;
+          if (t < M && hr+a < b1)
+            emit = settle_member<KW,SL>(S,W,kmer,pup,hr,Lr,a,x,xl,meta);
+          stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
+        }
+      /* 9..RS_RUNCAP entries: the whole warp, one run after the other, a member per lane */
+      unsigned lb = __ballot_sync(FULL,L > 8);
+      while (lb != 0)
+        { const int src = __ffs(lb)-1;
+          lb &= lb-1;
+          const int      hh = __shfl_sync(FULL,h,src);
+          const uint64_t xh = S.key[hh];
+          int LL = 9;                                    /* slots hh .. hh+8 are known to be in the run */
+          while (LL <= RS_RUNCAP)
+            { const int      t = hh+LL+lane;
+              const unsigned sb = __ballot_sync(FULL,t < RS_WIN && ((S.key[t] ^ xh) & pmask) == 0);
+              if (sb != FULL) { LL += __ffs(~sb)-1; break; }
+              LL += 32;
+            }
+          if (LL > RS_RUNCAP || hh+LL >= RS_WIN)           /* (warp-uniform) may go on past the window: runs_kernel */
+            { if (lane == 0)
+                S.t2r[atomicAdd(&s_nr,1u)] = (uint16_t) hh;
+              continue;
+            }
+          for (int a0 = 0; a0 < LL; a0 += 32)
+            { const int a = a0+lane;
+              bool     emit = false;
+              uint64_t x = 0, xl = 0, meta = 0;
+              if (a < LL && hh+a < b1)
+                emit = settle_member<KW,SL>(S,W,kmer,pup,hh,LL,a,x,xl,meta);
+              stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
+            }
+        }
     }
 
   /* ---- 5. the last warp to get here moves the staged records out ---- */
@@ -1078,8 +1116,13 @@ static cudaError_t launch_runs(const uint64_t *keys, const uint64_t *keys_lo, co
                                const void *bucket, int bits, int kmer, int64_t lo, int64_t hi,
                                const SymmView &W, cudaStream_t st)
 { /* (the Bloom filter is filled inside runscan_kernel: a kernel of its own would read the records once more) */
-  int64_t want = ((hi-lo)/64+255)/256;                        /* ~1 run of three or more per 60 entries: a thread each */
-  int     grid = (int) (want < 0x7fffffff ? (want > 0 ? want : 1) : 0x7fffffff);
+  /* the count of listed runs is only known on the device, and on sparse tables it is ~0 (runscan_kernel settles
+   * runs of up to RS_RUNCAP entries itself): at most one wave of CTAs, striding over the list               */
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
+  int64_t want = ((hi-lo)/64+255)/256;                        /* a thread per run if every 60th entry headed one */
+  int     grid = (int) (want < sms*8 ? (want > 0 ? want : 1) : sms*8);
   runs_kernel<IdxT,KW,SL><<<grid,256,0,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,lo,hi,W);
   return cudaGetLastError();
 }
@@ -1147,16 +1190,53 @@ extern "C" int hm_k_symm_runs(const uint64_t *d_keys, const uint64_t *d_keys_lo,
 
 /* ------------------------------------------------------------------------ pass 2 -------- */
 
-#define RV_TS 192      /* shared-memory plot tile: sums < 192, mins < 96 (72 KB) */
-#define RV_TM 96
-#define RV_THREADS 512
-#define RV_CTAS_PER_SM 2
-#define RV_ILP 4
+#define RV_TS   192     /* shared-memory plot tile: sums < 192, mins < 96 */
+#define RV_TM   96
+#define RV_TROW 97      /* its row stride: odd, so that cells of one min in different rows are in different banks */
+#define RV_THREADS 1024
+#ifndef RV_ILP
+#define RV_ILP 2                   /* candidates per thread and trip (4 spills at 64 registers: slower) */
+#endif
+#define RV_QCAP  (32*(RV_ILP+1))   /* queued Bloom hits per warp: fewer than 32 left over + a trip's */
+#define RV_PROBE 4                 /* keys of a bucket the exact check loads at once */
+#define RV_HA    (1ull << 48)      /* a queued record's meta: the Bloom bits of rc x / rc y were set */
+#define RV_HB    (1ull << 49)
 
-/* does table entry q (count cq: the table is symmetric, so it is the count of the candidate member
- * whose reverse complement q is) have a partner at a position >= pup?  Exact.  The bucket index is at
- * most as fine as a run (bits <= 2*Pr), so q's bucket holds q's whole run: one pass over those few keys
- * finds q itself and its partners -- bucket offsets -> keys -> counts, three dependent accesses.        */
+/* q's bucket [l,r) holds q's whole run (the bucket prefix is no longer than the run prefix): is q there
+ * (found), and has it a partner at a position >= pup with a count sum <= HM_SMAX?  RV_PROBE keys and
+ * counts are loaded at once.                                                                          */
+template <int KW>
+__device__ __forceinline__ bool bucket_upper_partner(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+                                                     const uint16_t *__restrict__ cnt, int64_t l, int64_t r,
+                                                     int psh, int pup, uint64_t q, uint64_t ql, int cq, bool &found)
+{ bool hit = false;
+  found = false;
+  for (int64_t i0 = l; i0 < r; i0 += RV_PROBE)
+    { uint64_t z[RV_PROBE], zl[RV_PROBE];
+      int      c[RV_PROBE];
+#pragma unroll
+      for (int u = 0; u < RV_PROBE; u++)
+        { const bool in = (i0+u < r);
+          z[u]  = in ? __ldg(keys+i0+u) : ~q;                 /* ~q: another run */
+          zl[u] = (KW == 2 && in) ? __ldg(keys_lo+i0+u) : 0;
+          c[u]  = in ? (int) __ldg(cnt+i0+u) : 0;
+        }
+#pragma unroll
+      for (int u = 0; u < RV_PROBE; u++)
+        { int pos;
+          if (z[u] == q && (KW == 1 || zl[u] == ql))
+            found = true;
+          else if (((z[u] ^ q) >> psh) == 0 && one_base_apart<KW>(q,ql,z[u],zl[u],pos) && pos >= pup &&
+                   cq + c[u] <= HM_SMAX)
+            hit = true;
+        }
+    }
+  return hit;
+}
+
+/* The general case of the exact check (a bucket prefix longer than the run prefix -- tiny tables -- or a
+ * bucket of more than 48 keys): does table entry q (count cq: the table is symmetric, so it is the count
+ * of the candidate member whose reverse complement q is) have a partner at a position >= pup?  Exact.  */
 template <typename IdxT, int KW>
 __device__ __noinline__ bool has_upper_partner(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                                                const uint16_t *__restrict__ cnt, int64_t n,
@@ -1208,38 +1288,55 @@ __device__ __noinline__ bool has_upper_partner(const uint64_t *__restrict__ keys
   return (U > 0);
 }
 
-/* one candidate: are rc x / rc y in S?  Bloom bits first; EXACT = also settle the hits: SL = false looks
- * for an upper partner in the table, SL = true (streamed scan: keys / bucket are the sorted S list and its
- * index) looks the key up in S.  -> 0 isolated pair, 1 not isolated, 2 undecided (a Bloom hit, EXACT == false) */
-template <typename IdxT, int KW, bool EXACT, bool SL>
-__device__ __forceinline__ int judge_candidate(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
-                                               const uint16_t *__restrict__ cnt, int64_t n,
-                                               const IdxT *__restrict__ bucket, int bshift, int kmer,
-                                               const SymmView &W, uint64_t x, uint64_t xl, uint64_t meta)
-{ const int cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
-  const int p  = (int) ((meta >> 32) & 0xff), yb = (int) ((meta >> 40) & 3);
+/* one candidate whose Bloom bits were set for rc x (RV_HA in its meta) and/or rc y (RV_HB): is it isolated
+ * after all?  SL = false looks for an upper partner in the table, SL = true (streamed scan: keys / bucket are
+ * the sorted S list and its index) looks the key up in S.  Exact.  When the bucket prefix is no longer than
+ * the run prefix (every table of more than a few entries) both buckets' offsets are loaded at once and then
+ * RV_PROBE keys and counts of a bucket at once: two dependent accesses instead of one per key.             */
+template <typename IdxT, int KW, bool SL>
+__device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+                                                   const uint16_t *__restrict__ cnt, int64_t n,
+                                                   const IdxT *__restrict__ bucket, int bshift, int kmer,
+                                                   const SymmView &W, uint64_t x, uint64_t xl, uint64_t meta)
+{ const int  cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
+  const int  p  = (int) ((meta >> 32) & 0xff), yb = (int) ((meta >> 40) & 3);
+  const bool ha = (meta & RV_HA) != 0, hb = (meta & RV_HB) != 0;
   uint64_t rx, rxl, ry, ryl;
   revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
   ry = rx; ryl = rxl;
   set_base<KW>(ry,ryl,kmer-1-p,3-yb);                      /* rc y = rc x with the mirrored base swapped */
-  uint32_t *wa, *wb, ba, bb;
-  bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,rx) : 0,kmer,rx,rxl,wa,ba);
-  bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,ry) : 0,kmer,ry,ryl,wb,bb);
-  const uint32_t va = ld_keep(wa);
-  const uint32_t vb = (wb == wa) ? va : ld_keep(wb);       /* one shard owns both: the same word */
-  const bool ha = (va & ba) == ba, hb = (vb & bb) == bb;
-  if (!ha && !hb)
-    return 0;
-  if (!EXACT)
-    return 2;
   if (SL)
-    return ((ha && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
-            (hb && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0)) ? 1 : 0;
+    return !((ha && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
+             (hb && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0));
+  const int Pr = kmer >> 1, pup = kmer-Pr, psh = 64-2*Pr;
+  if (bshift >= psh)
+    { int64_t la = 0, ra = 0, lb = 0, rb = 0;
+      if (ha) { const uint64_t bk = rx >> bshift; la = (int64_t) bucket[bk]; ra = (int64_t) bucket[bk+1]; }
+      if (hb) { const uint64_t bk = ry >> bshift; lb = (int64_t) bucket[bk]; rb = (int64_t) bucket[bk+1]; }
+      if (ra-la <= 48 && rb-lb <= 48)
+        { bool found;
+          if (ha)
+            { const bool up = bucket_upper_partner<KW>(keys,keys_lo,cnt,la,ra,psh,pup,rx,rxl,cx,found);
+              if (!found)
+                atomicOr(W.status,SY_STATUS_ASYMMETRIC);
+              if (up)
+                return false;
+            }
+          if (hb)
+            { const bool up = bucket_upper_partner<KW>(keys,keys_lo,cnt,lb,rb,psh,pup,ry,ryl,cy,found);
+              if (!found)
+                atomicOr(W.status,SY_STATUS_ASYMMETRIC);
+              if (up)
+                return false;
+            }
+          return true;
+        }
+    }
   if (ha && has_upper_partner<IdxT,KW>(keys,keys_lo,cnt,n,bucket,bshift,kmer,rx,rxl,cx,W.status))
-    return 1;
+    return false;
   if (hb && has_upper_partner<IdxT,KW>(keys,keys_lo,cnt,n,bucket,bshift,kmer,ry,ryl,cy,W.status))
-    return 1;
-  return 0;
+    return false;
+  return true;
 }
 
 __device__ __forceinline__ void count_pair(uint32_t *tile, unsigned long long *__restrict__ plot,
@@ -1250,29 +1347,33 @@ __device__ __forceinline__ void count_pair(uint32_t *tile, unsigned long long *_
   const int s = cx+cy;
   const int m = cx < cy ? cx : cy;
   if (s < RV_TS && m < RV_TM)
-    atomicAdd(tile + s*RV_TM + m, wgt);
+    atomicAdd(tile + s*RV_TROW + m, wgt);
   else
     atomicAdd(plot + s*HM_PLOT_W + m, (unsigned long long) wgt);
 }
 
-/* Candidates whose Bloom look-up misses (~95 %) are counted at once.  The others need the exact
- * answer -- bucket offsets, keys, counts: three dependent random accesses -- and a warp in which one
- * lane does that stalls all 32: they are parked in a per-warp queue and settled 32 at a time, every
- * lane busy.  RV_ILP candidates per thread and trip keep that many record / Bloom loads in flight
- * (the kernel is bound by the latency of record -> Bloom word, not by bytes or instructions).         */
+/* Candidates whose Bloom look-up misses (~95 %) are counted at once.  The others need the exact answer
+ * and a warp in which one lane does that stalls all 32: they are parked in a per-warp queue in shared
+ * memory -- the whole record, with the two Bloom answers in its meta -- and settled 32 at a time, every
+ * lane busy, without reading the record or the filter again.  RV_ILP candidates per thread and trip keep
+ * that many record / Bloom loads in flight (the kernel is bound by latency: record -> Bloom word, and
+ * for the hits bucket offsets -> keys, not by bytes or instructions).  One CTA of 1024 threads per SM:
+ * one plot tile per SM, the rest of shared memory holds the queues.                                  */
 template <typename IdxT, int KW, bool SL>
-__global__ void __launch_bounds__(RV_THREADS,RV_CTAS_PER_SM)
+__global__ void __launch_bounds__(RV_THREADS,1)
 resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
                int kmer, const SymmView W, unsigned long long *__restrict__ plot)
-{ extern __shared__ uint32_t tile[];
-  __shared__ uint32_t s_q[RV_THREADS/32][32*(RV_ILP+1)];
+{ extern __shared__ __align__(16) uint64_t rv_smem[];
+  uint32_t *tile = (uint32_t *) rv_smem;                  /* RV_TS x RV_TROW counters */
   const unsigned FULL = 0xffffffffu;
   const int      lane = threadIdx.x & 31;
   const unsigned lt   = (1u << lane) - 1;
-  uint32_t *q  = s_q[threadIdx.x >> 5];
+  uint64_t *qk = rv_smem + RV_TS*RV_TROW/2 + (threadIdx.x >> 5)*RV_QCAP*(KW+1);   /* this warp's queue */
+  uint64_t *ql = qk + (KW == 2 ? RV_QCAP : 0);
+  uint64_t *qm = qk + KW*RV_QCAP;
   int       qn = 0;
-  for (int t = threadIdx.x; t < RV_TS*RV_TM; t += blockDim.x)
+  for (int t = threadIdx.x; t < RV_TS*RV_TROW; t += blockDim.x)
     tile[t] = 0;
   __syncthreads();
   unsigned long long ncl = *W.cand_n;
@@ -1310,42 +1411,43 @@ resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         { va[u] = 0; vb[u] = 0;
           if (ok[u])
             { va[u] = ld_keep(wa[u]);
-              vb[u] = (wb[u] == wa[u]) ? va[u] : ld_keep(wb[u]);
+              vb[u] = (wb[u] == wa[u]) ? va[u] : ld_keep(wb[u]);   /* one shard owns both: the same word */
             }
         }
 #pragma unroll
       for (int u = 0; u < RV_ILP; u++)
-        { const bool hit = ok[u] && ((va[u] & ba[u]) == ba[u] || (vb[u] & bb[u]) == bb[u]);
+        { const bool ha = (va[u] & ba[u]) == ba[u], hb = (vb[u] & bb[u]) == bb[u];
+          const bool hit = ok[u] && (ha || hb);
           if (ok[u] && !hit)
             count_pair(tile,plot,meta[u],kmer);
           const unsigned bal = __ballot_sync(FULL,hit);
           if (hit)
-            q[qn + __popc(bal & lt)] = ((it*RV_ILP+u) << 5) | (uint32_t) lane;
+            { const int at = qn + __popc(bal & lt);
+              qk[at] = x[u];
+              if (KW == 2) ql[at] = xl[u];
+              qm[at] = meta[u] | (ha ? RV_HA : 0) | (hb ? RV_HB : 0);
+            }
           qn += __popc(bal);
         }
       __syncwarp();
       while (qn >= 32)
         { qn -= 32;
-          const uint32_t e = q[qn+lane];
+          const uint64_t xx = qk[qn+lane], xxl = KW == 2 ? ql[qn+lane] : 0, mm = qm[qn+lane];
           __syncwarp();
-          const int64_t j = first-lane + (int64_t) (e & 31) + (int64_t) (e >> 5)*stride;
-          const uint64_t xx = W.cand_key[j], xxl = KW == 2 ? W.cand_lo[j] : 0, mm = W.cand_meta[j];
-          if (judge_candidate<IdxT,KW,true,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm) == 0)
+          if (isolated_after_all<IdxT,KW,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
             count_pair(tile,plot,mm,kmer);
         }
     }
   if (lane < qn)
-    { const uint32_t e = q[lane];
-      const int64_t j = first-lane + (int64_t) (e & 31) + (int64_t) (e >> 5)*stride;
-      const uint64_t xx = W.cand_key[j], xxl = KW == 2 ? W.cand_lo[j] : 0, mm = W.cand_meta[j];
-      if (judge_candidate<IdxT,KW,true,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm) == 0)
+    { const uint64_t xx = qk[lane], xxl = KW == 2 ? ql[lane] : 0, mm = qm[lane];
+      if (isolated_after_all<IdxT,KW,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
         count_pair(tile,plot,mm,kmer);
     }
   __syncthreads();
-  for (int t = threadIdx.x; t < RV_TS*RV_TM; t += blockDim.x)
+  for (int t = threadIdx.x; t < RV_TS*RV_TROW; t += blockDim.x)
     { uint32_t v = tile[t];
-      if (v != 0)
-        atomicAdd(plot + (t/RV_TM)*HM_PLOT_W + (t%RV_TM), (unsigned long long) v);
+      if (v != 0)                                          /* (column RV_TM is padding: always 0) */
+        atomicAdd(plot + (t/RV_TROW)*HM_PLOT_W + (t%RV_TROW), (unsigned long long) v);
     }
 }
 
@@ -1354,7 +1456,7 @@ static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo,
                                   const void *bucket, int bits, int kmer, const SymmView &W,
                                   unsigned long long *plot, int64_t range, cudaStream_t st)
 { static int configured[64] = {0};                            /* per instantiation */
-  size_t smem = (size_t) RV_TS*RV_TM*sizeof(uint32_t);
+  size_t smem = (size_t) RV_TS*RV_TROW*sizeof(uint32_t) + (size_t) (RV_THREADS/32)*RV_QCAP*8*(KW+1);   /* 121 KB / 145 KB */
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (dev >= 64 || !configured[dev])
@@ -1364,7 +1466,7 @@ static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo,
     }
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = (range/8+RV_THREADS-1)/RV_THREADS;            /* ~1 candidate per 10 entries */
-  int     grid = (int) (want < sms*RV_CTAS_PER_SM ? (want > 0 ? want : 1) : sms*RV_CTAS_PER_SM);
+  int     grid = (int) (want < sms ? (want > 0 ? want : 1) : sms);
   resolve_kernel<IdxT,KW,SL><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
   return cudaGetLastError();
 }

@@ -1,4 +1,9 @@
-"""time the strand-symmetric scan against the direct passes on the bench workload (one GPU)"""
+"""time the strand-symmetric scan against the direct passes on the bench workload (one GPU)
+
+The symmetric scan is timed kernel by kernel: `runscan_ms` (runscan_kernel, with the clearing of the
+work-area header and the Bloom filter), `runs_ms` (runs_kernel) and `resolve_ms` (resolve_kernel), each
+the mean over `reps` scans bracketed by CUDA events.  `runs_listed` is the number of runs runscan_kernel
+left to runs_kernel (header word 2 of the work area)."""
 import json
 import os
 import sys
@@ -38,26 +43,30 @@ def main():
             ev[0].record()
             if name == "direct":
                 t.pass1()
-            else:
-                t.runscan()
-            ev[1].record()
-            if name == "direct":
+                ev[1].record()
+                ev[2].record()
                 t.pass2()
             else:
+                t.runscan(mid_event=ev[1])
+                ev[2].record()
                 t.resolve()
-            ev[2].record()
+            ev[3].record()
             torch.cuda.synchronize()
             if r >= 3:
-                tms.append((ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])))
+                tms.append([ev[i].elapsed_time(ev[i + 1]) for i in range(3)])
         res[name] = t.plot.clone()
-        a = sum(x[0] for x in tms) / len(tms)
-        b = sum(x[1] for x in tms) / len(tms)
-        out[name] = {"k1_ms": a, "k2_ms": b, "kmers_per_s": t.n / ((a + b) * 1e-3)}
+        a, b, c = (sum(x[i] for x in tms) / len(tms) for i in range(3))
+        if name == "direct":
+            out[name] = {"k1_ms": a, "k2_ms": c, "kmers_per_s": t.n / ((a + c) * 1e-3)}
+        else:
+            out[name] = {"k1_ms": a + b, "k2_ms": c, "runscan_ms": a, "runs_ms": b, "resolve_ms": c,
+                         "kmers_per_s": t.n / ((a + b + c) * 1e-3)}
     if direct:
         out["plots_equal"] = bool(torch.equal(res["direct"], res["symm"]))
     out["plot_sum"] = int(res["symm"].sum())
     nc, st = t.symm_status()
-    out["candidates"], out["status"] = nc, st
+    hdr = t.symm_work[t.symm_layout.off_header:t.symm_layout.off_header + 24].view(torch.int64)
+    out["candidates"], out["runs_listed"], out["status"] = nc, int(hdr[2]), st
     print(json.dumps(out))
 
 
