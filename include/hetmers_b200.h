@@ -305,9 +305,15 @@ int  hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int6
  * pass) and reads the host table again on every run: the hm_host_table given to hm_scan_create (its
  * buffers or descriptors) must stay valid until hm_scan_destroy.  Streamed scans refuse what needs the
  * whole table resident (HM_EUNSUPPORTED): hm_scan_condition, hm_scan_extract, hm_scan_download and
- * hm_scan_run_path(HM_PATH_DIRECT); hm_scan_examine streams.  Several GPUs are not streamed over.
- * HETMERS_STREAM=1 streams one-GPU scans whatever their size (the budget then only sizes the chunks);
- * HETMERS_STREAM_CHUNK=<entries> caps the chunk length below what the budget allows.                */
+ * hm_scan_run_path(HM_PATH_DIRECT); hm_scan_examine streams (on dev[0]).
+ * Several GPUs (n_gpus = G > 1): shard r streams [c_r, c_r+1) through dev[r], c_r = the first run start at
+ * or after n*r/G (hm_symm_align_cut's rule; shards may be empty).  Every shard holds the whole-table Bloom
+ * filter (its own segment filled by its pass 1, the others all-gathered), its own candidates and S list;
+ * pass 2 checks a Bloom hit in the S list of the key's owner through peer memory.  A device id may repeat
+ * in dev[] for a streamed scan: those shards share the device and the default budget (an in-core scan
+ * refuses repeated ids).  The budget applies to each shard.
+ * HETMERS_STREAM=1 streams scans whatever their size (the budget then only sizes the chunks);
+ * HETMERS_STREAM_CHUNK=<entries> caps each shard's chunk length below what the budget allows.          */
 
 /* device bytes a scan may hold per GPU; 0 (default) = what cudaMemGetInfo reports free at
  * hm_scan_create (plus the idle part of the memory pool) minus HM_BUDGET_RESERVE.  The executable passes
@@ -328,8 +334,13 @@ typedef struct hm_stream_layout            /* what hm_stream_plan chooses for a 
  * fixed + chunk + list bytes <= budget, chunk is monotone in the budget; HM_ENOMEM if the budget cannot
  * hold one chunk                                                                                     */
 int  hm_stream_plan(int64_t n, int kmer, int ibyte, int64_t budget, hm_stream_layout *out);
+/* the plan of each of n_shards shards (budget per shard): fixed_bytes holds the whole-table Bloom filter of
+ * n_shards segments, chunk and list room are for a share of ceil(n / n_shards) entries (chunks no longer
+ * than the share).  n_shards = 1 is hm_stream_plan.                                                    */
+int  hm_stream_plan_shards(int64_t n, int kmer, int ibyte, int64_t budget, int n_shards, hm_stream_layout *out);
 /* 1 if the scan is streamed, else 0.  *device_bytes: the most device memory the scan held per GPU (in
- * core: what it allocates); *chunks: chunks of the last run (0 in core).  Either pointer may be NULL.  */
+ * core: what it allocates; streamed: the largest peak of a shard); *chunks: chunks of the last run, summed
+ * over the shards (0 in core).  Either pointer may be NULL.                                           */
 int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks);
 
 /* one call: create + run + destroy (what bench.py's e2e leg times) */

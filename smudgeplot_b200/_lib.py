@@ -24,7 +24,7 @@ ABI_SYMBOLS = [
     "hm_scan_create", "hm_prewarm", "hm_set_io_threads", "hm_scan_destroy", "hm_scan_examine", "hm_scan_condition", "hm_scan_run", "hm_hetmers_host",
     "hm_scan_run_path", "hm_scan_is_symmetric", "hm_symm_plan", "hm_symm_seeds", "hm_k_symm_fingerprint", "hm_k_symm_runscan", "hm_k_symm_runs", "hm_k_symm_resolve",
     "hm_symm_status", "hm_symm_align_cut",
-    "hm_scan_download", "hm_set_device_budget", "hm_stream_plan", "hm_scan_residency", "hm_table_open", "hm_table_close", "hm_table_view", "hm_write_smu",
+    "hm_scan_download", "hm_set_device_budget", "hm_stream_plan", "hm_stream_plan_shards", "hm_scan_residency", "hm_table_open", "hm_table_close", "hm_table_view", "hm_write_smu",
 ]
 
 
@@ -153,6 +153,7 @@ def lib():
     L.hm_set_device_budget.argtypes = [i64]
     L.hm_set_device_budget.restype = None
     L.hm_stream_plan.argtypes = [i64, i32, i32, i64, C.POINTER(StreamLayout)]
+    L.hm_stream_plan_shards.argtypes = [i64, i32, i32, i64, i32, C.POINTER(StreamLayout)]
     L.hm_scan_residency.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     L.hm_table_open.argtypes = [C.c_char_p, C.POINTER(vp)]
     L.hm_table_close.argtypes = [vp]

@@ -34,15 +34,30 @@ typedef struct hm_stream_lists
     int64_t   runs_cap;
   } hm_stream_lists;
 
+/* several shards: the sorted S list of one shard and its bucket index, as the other shards' pass 2 reads it (peer
+ * memory when the shard is on another GPU).  The shards' views form a device array of the reading shard.     */
+typedef struct hm_stream_sview
+  { const uint64_t *s_key, *s_lo;
+    const void     *s_bucket;                /* uint32 or uint64 offsets: the same width for every shard */
+    int64_t         n_s;
+    int32_t         bits, pad;
+  } hm_stream_sview;
+
+/* shards: NULL (or n_seg == 1) for one shard; else this shard's descriptor -- n_seg = the shards up to the last
+ * non-empty one, self, first_key -- over a work area of hm_symm_plan(n, 0, kmer, G) (G >= n_seg segments)   */
 int hm_symm_stream_begin(void *d_work, const hm_symm_layout *L, void *stream);
 int hm_symm_stream_chunk(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
                          int64_t n, const void *d_bucket, int bits, int kmer, int64_t hi,
-                         void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, void *stream);
+                         void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                         const hm_symm_shards *shards, void *stream);
 int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t *n_cand,
                           uint64_t *status, uint64_t *n_s, void *stream);
+/* one shard: the exact checks look up this shard's S list (d_s_key ...); several: the owner's, through
+ * d_views[owner] (device array of shards->n_seg views)                                                 */
 int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
                            const void *d_s_bucket, int bits, int idx64, int kmer, int64_t range,
                            void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                           const hm_symm_shards *shards, const hm_stream_sview *d_views,
                            unsigned long long *d_plot, void *stream);
 
 #include <cuda_runtime.h>

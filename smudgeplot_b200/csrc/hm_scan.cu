@@ -16,7 +16,8 @@
  * one-process-per-GPU variant (torch.distributed / NCCL) lives in smudgeplot_b200/dist.py and
  * uses layer A directly.
  * A table whose in-core footprint exceeds the device budget is not loaded here: every run streams it
- * through one GPU in run-aligned chunks (run_stream, DESIGN.md §4c).
+ * in run-aligned chunks (run_stream, DESIGN.md §4c), through one GPU or, sharded, each GPU its own
+ * run-aligned share of the table.
  *******************************************************************************************/
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -52,6 +53,7 @@ typedef struct
     hm_symm_layout      symm_layout;
     int64_t             slo, shi;     /* its run-aligned range */
     uint64_t           *fp_acc;       /* device uint64[4]: symmetry fingerprint sums of the entries loaded here */
+    int64_t             held, peak, chunks;   /* (streamed) this shard's device bytes now / at most; chunks of the last run */
   } DevTable;
 
 struct hm_scan
@@ -70,12 +72,13 @@ struct hm_scan
     hm_symm_shards ssh[HM_MAX_GPUS];
     uint64_t seed[2];
     /* residency (DESIGN.md §4c) */
-    int64_t  budget;                      /* device bytes this scan may hold per GPU                          */
+    int64_t  budget;                      /* device bytes this scan may hold per GPU (streamed: per shard)    */
     int64_t  incore_bytes;                /* what the in-core scan allocates per GPU                          */
-    int      streamed;                    /* nothing resident: every run streams the host table through GPU 0 */
+    int      streamed;                    /* nothing resident: every run streams the host table, each shard   */
+                                          /*   its run-aligned range [d[r].lo, d[r].hi) through d[r].dev      */
     const hm_host_table *host;            /* (streamed) the caller's table, valid until hm_scan_destroy        */
-    hm_stream_layout plan;
-    int64_t  held, peak, chunks;          /* (streamed) device bytes held now / at most; chunks of the last run */
+    hm_stream_layout plan;                /* (streamed) per shard                                              */
+    volatile int stop;                    /* (streamed) a shard failed: the others leave their chunk loops     */
   };
 
 static double now_ms(void)
@@ -474,13 +477,16 @@ static int64_t g_budget = 0;
 extern "C" void hm_set_device_budget(int64_t bytes) { g_budget = bytes > 0 ? bytes : 0; }
 
 /* the budget per GPU: the one set, or the smallest free memory of the devices (counting what an idle
- * stream-ordered pool keeps reserved for us) minus a reserve for the CUDA runtime and library code      */
+ * stream-ordered pool keeps reserved for us) minus a reserve for the CUDA runtime and library code; a device
+ * listed m times (shards of a streamed scan sharing it) gives each of them 1/m of that                  */
 static int64_t device_budget(const int *dev, int n_gpus)
 { if (g_budget > 0)
     return g_budget;
   int64_t best = -1;
   for (int g = 0; g < n_gpus; g++)
-    { int    d = dev ? dev[g] : g;
+    { int    d = dev ? dev[g] : g, m = 0;
+      for (int h = 0; h < n_gpus; h++)
+        m += ((dev ? dev[h] : h) == d);
       size_t fr = 0, tot = 0;
       if (cudaSetDevice(d) != cudaSuccess || cudaMemGetInfo(&fr,&tot) != cudaSuccess)
         { cudaGetLastError(); continue; }
@@ -492,11 +498,10 @@ static int64_t device_budget(const int *dev, int n_gpus)
           cudaMemPoolGetAttribute(pool,cudaMemPoolAttrUsedMemCurrent,&used) == cudaSuccess && res > used)
         f += (int64_t) (res-used);
       cudaGetLastError();
+      f = f > HM_BUDGET_RESERVE ? (f-HM_BUDGET_RESERVE)/m : 0;
       if (best < 0 || f < best) best = f;
     }
-  if (best < 0)
-    return 0;
-  return best > HM_BUDGET_RESERVE ? best-HM_BUDGET_RESERVE : 0;
+  return best < 0 ? 0 : best;
 }
 
 /* device bytes the in-core scan allocates per GPU: table arrays, bucket index, plot, fingerprint sums and the
@@ -513,9 +518,9 @@ static int64_t incore_bytes(int64_t n, int kmer, int n_gpus, int bits, int idx64
 /* ---- the streamed scan's plan --------------------------------------------------------------------- */
 #define STREAM_MIN_CHUNK 256
 
-/* work area of the streamed scan: header + the whole-table Bloom filter of hm_symm_plan (one segment) */
-static int stream_work_layout(int64_t n, int kmer, hm_symm_layout *L)
-{ int rc = hm_symm_plan(n,0,kmer,1,L);
+/* work area of the streamed scan: header + the whole-table Bloom filter of hm_symm_plan (a segment per shard) */
+static int stream_work_layout(int64_t n, int kmer, int n_seg, hm_symm_layout *L)
+{ int rc = hm_symm_plan(n,0,kmer,n_seg,L);
   if (rc != HM_OK) return rc;
   L->bytes = (L->off_cand_key+255) & ~255ll;
   L->cand_cap = 0; L->runs_cap = 0;
@@ -541,26 +546,30 @@ static int64_t chunk_list_bytes(int64_t c, int kmer)
   return (8*KW+8)*(c/2+1024) + 8*KW*(c+1024);
 }
 
-extern "C" int hm_stream_plan(int64_t n, int kmer, int ibyte, int64_t budget, hm_stream_layout *out)
-{ if (out == NULL || n < 0 || kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || budget < 0)
-    return hm_set_error(HM_EINVAL,"hm_stream_plan: bad arguments");
+/* several shards: the room for each one's lists and chunks is planned from its share of n/G entries (chunks no
+ * longer than the share); every shard holds the whole-table Bloom filter of G segments                  */
+extern "C" int hm_stream_plan_shards(int64_t n, int kmer, int ibyte, int64_t budget, int n_shards, hm_stream_layout *out)
+{ if (out == NULL || n < 0 || kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || budget < 0 ||
+      n_shards < 1 || n_shards > HM_MAX_GPUS)
+    return hm_set_error(HM_EINVAL,"hm_stream_plan_shards: bad arguments");
   hm_symm_layout L;
-  int rc = stream_work_layout(n,kmer,&L);
+  int rc = stream_work_layout(n,kmer,n_shards,&L);
   if (rc != HM_OK) return rc;
   memset(out,0,sizeof(*out));
   out->budget = budget;
   out->fixed_bytes = 8*(1ll << (8*ibyte)) + 8*(int64_t) HM_PLOT_CELLS + 32 + L.bytes;
   /* the largest chunk whose buffers + list room take at most a quarter of what is left: the rest is for
-   * the candidate records and S keys of the chunks before it (a few B per entry of the whole table) and
+   * the candidate records and S keys of the chunks before it (a few B per entry of the share) and
    * for growing those lists, which holds the old and the new array at once                             */
-  int64_t avail = budget - out->fixed_bytes, lo = 0, hi = n < (1ll << 31) ? n : (1ll << 31);
+  int64_t share = (n+n_shards-1)/n_shards;
+  int64_t avail = budget - out->fixed_bytes, lo = 0, hi = share < (1ll << 31) ? share : (1ll << 31);
   if (avail > 0)
     while (lo < hi)
       { int64_t mid = lo + (hi-lo+1)/2;
         if (chunk_bytes(mid,kmer,ibyte) + chunk_list_bytes(mid,kmer) <= avail/4) lo = mid;
         else                                                                   hi = mid-1;
       }
-  int64_t need = n < STREAM_MIN_CHUNK ? n : STREAM_MIN_CHUNK;
+  int64_t need = share < STREAM_MIN_CHUNK ? share : STREAM_MIN_CHUNK;
   if (avail <= 0 || lo < need || lo < 1)
     return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes cannot hold one chunk of the streamed scan: "
                         "%lld bytes are fixed (stub index, plot, Bloom filter of %lld entries) and a chunk of "
@@ -573,26 +582,103 @@ extern "C" int hm_stream_plan(int64_t n, int kmer, int ibyte, int64_t budget, hm
   return HM_OK;
 }
 
+extern "C" int hm_stream_plan(int64_t n, int kmer, int ibyte, int64_t budget, hm_stream_layout *out)
+{ if (out == NULL || n < 0 || kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || budget < 0)
+    return hm_set_error(HM_EINVAL,"hm_stream_plan: bad arguments");
+  return hm_stream_plan_shards(n,kmer,ibyte,budget,1,out);
+}
+
+/* streamed: the largest peak of a shard, the chunks of all shards */
 extern "C" int hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks)
-{ if (device_bytes) *device_bytes = s->streamed ? s->peak : s->incore_bytes;
-  if (chunks)       *chunks = s->streamed ? s->chunks : 0;
+{ int64_t peak = 0, nch = 0;
+  for (int g = 0; g < s->ngpu; g++)
+    { if (s->d[g].peak > peak) peak = s->d[g].peak;
+      nch += s->d[g].chunks;
+    }
+  if (device_bytes) *device_bytes = s->streamed ? peak : s->incore_bytes;
+  if (chunks)       *chunks = s->streamed ? nch : 0;
   return s->streamed;
 }
 
-/* streamed scans: device allocations counted against the budget */
+/* streamed scans: device allocations counted against the shard's budget */
 static cudaError_t salloc(hm_scan *s, DevTable *D, void **p, int64_t bytes)
 { cudaError_t e = dalloc(D->dev,D->st,p,(size_t) bytes);
+  (void) s;
   if (e == cudaSuccess)
-    { s->held += bytes;
-      if (s->held > s->peak) s->peak = s->held;
+    { D->held += bytes;
+      if (D->held > D->peak) D->peak = D->held;
     }
   return e;
 }
 
 static void sfree(hm_scan *s, DevTable *D, void *p, int64_t bytes)
-{ if (p == NULL) return;
+{ (void) s;
+  if (p == NULL) return;
   dfree(D->dev,D->st,p);
-  s->held -= bytes;
+  D->held -= bytes;
+}
+
+/* Shard cuts of a streamed scan over G = s->ngpu shards, from the host table: c_r is the first run start (a run =
+ * the entries sharing their first k/2 bases) at or after n*r/G -- hm_symm_align_cut's rule -- found by loading
+ * a few records at a time around each nominal cut on the first shard's device.  Sets every shard's range,
+ * descriptor (first_key[r] = word 0 of entry c_r) and how many shards own keys: those up to the last non-empty
+ * one (a run longer than a share can leave shards empty, in the middle or at the end).                   */
+static int stream_cuts(hm_scan *s, const hm_host_table *t)
+{ DevTable *D = s->d;
+  int      G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
+  int64_t  n = s->n, cut[HM_MAX_GPUS+1], ixlen = (int64_t) 1 << (8*s->ibyte);
+  uint64_t first[HM_MAX_GPUS];
+  const int64_t W = 4096;
+  const int psh = 64-2*(s->kmer>>1);
+  uint64_t *keys = NULL, *klo = NULL, buf[4096];
+  uint16_t *cnt = NULL;
+  int64_t  *d_index = NULL;
+  Stager    SG;
+  memset(&SG,0,sizeof(SG));
+  HM_CUDA(cudaSetDevice(D->dev));
+  cudaError_t e = cudaMalloc(&keys,8*(size_t) (W+1));
+  if (e == cudaSuccess && KW == 2) e = cudaMalloc(&klo,8*(size_t) (W+1));
+  if (e == cudaSuccess) e = cudaMalloc(&cnt,2*(size_t) (W+8));
+  if (e == cudaSuccess) e = cudaMalloc(&d_index,8*(size_t) ixlen);
+  if (e == cudaSuccess) e = cudaMemcpy(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) rc = hm_cuda_fail(e,"streamed scan: shard cuts");
+  if (rc == HM_OK) rc = stager_open(s,D,t,W,&SG);
+  cut[0] = 0; cut[G] = n; first[0] = 0;
+  for (int r = 1; r < G && rc == HM_OK; r++)
+    { int64_t  c = n*r/G;
+      uint64_t prev;
+      if (c <= cut[r-1])                                   /* the run before reaches past this share's start */
+        { cut[r] = cut[r-1]; first[r] = first[r-1]; continue; }
+      if ((rc = load_into(s,D,t,d_index,c-1,1,keys,klo,cnt,0,&SG)) != HM_OK) break;
+      if ((e = cudaMemcpy(&prev,keys,8,cudaMemcpyDeviceToHost)) != cudaSuccess) { rc = hm_cuda_fail(e,"cut key"); break; }
+      cut[r] = n; first[r] = ~0ull;
+      for (int64_t o = c; o < n && rc == HM_OK; o += W)
+        { int64_t m = n-o < W ? n-o : W, i;
+          if ((rc = load_into(s,D,t,d_index,o,m,keys,klo,cnt,0,&SG)) != HM_OK) break;
+          if ((e = cudaMemcpy(buf,keys,8*(size_t) m,cudaMemcpyDeviceToHost)) != cudaSuccess)
+            { rc = hm_cuda_fail(e,"cut keys"); break; }
+          for (i = 0; i < m && ((buf[i] ^ prev) >> psh) == 0; i++)
+            ;
+          if (i < m)
+            { cut[r] = o+i; first[r] = buf[i]; break; }
+        }
+    }
+  stager_close(D,&SG);
+  cudaFree(keys); cudaFree(klo); cudaFree(cnt); cudaFree(d_index);
+  if (rc != HM_OK)
+    return rc;
+  int live = 1;                                            /* shards up to the last non-empty one */
+  for (int r = 1; r < G; r++)
+    if (cut[r] < n) live = r+1;
+  for (int g = 0; g < G; g++)
+    { hm_symm_shards *sh = s->ssh+g;
+      memset(sh,0,sizeof(*sh));
+      sh->n_seg = live; sh->self = g;
+      for (int r = 0; r <= G; r++) sh->off[r] = cut[r];
+      for (int r = 0; r < G; r++)  sh->first_key[r] = first[r];
+      s->d[g].lo = cut[g]; s->d[g].hi = cut[g+1];
+    }
+  return HM_OK;
 }
 
 extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out)
@@ -625,14 +711,9 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   s->incore_bytes = incore_bytes(n,t->kmer,n_gpus,s->bits,s->idx64);
   const char *force = getenv("HETMERS_STREAM");            /* =1: stream whatever the budget (tests, capping) */
   if (s->incore_bytes > s->budget || (force != NULL && strcmp(force,"1") == 0))
-    { /* streamed: only the plot and the fingerprint sums are allocated now; the table stays on the host */
-      if (n_gpus > 1)
-        { free(s);
-          return hm_set_error(HM_EUNSUPPORTED,"the table of %lld entries needs %lld device bytes per GPU in core, more "
-                              "than the device budget of %lld; it can be streamed through one GPU, not several",
-                              (long long) n,(long long) incore_bytes(n,t->kmer,n_gpus,s->bits,s->idx64),(long long) s->budget);
-        }
-      if ((rc = hm_stream_plan(n,t->kmer,t->ibyte,s->budget,&s->plan)) != HM_OK)
+    { /* streamed: only the plot and the fingerprint sums are allocated now; the table stays on the host.
+       * Several GPUs: shard r streams its run-aligned share [c_r, c_r+1) through dev[r] (DESIGN.md §4c) */
+      if ((rc = hm_stream_plan_shards(n,t->kmer,t->ibyte,s->budget,n_gpus,&s->plan)) != HM_OK)
         { free(s); return rc; }
       const char *cc = getenv("HETMERS_STREAM_CHUNK");         /* smaller chunks than the budget allows */
       if (cc != NULL && atoll(cc) >= 1 && atoll(cc) < s->plan.chunk)
@@ -642,18 +723,24 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
           s->plan.list_bytes = s->budget - s->plan.fixed_bytes - s->plan.chunk_bytes;
         }
       s->streamed = 1; s->host = t;
-      DevTable *D = s->d;
-      cudaError_t e;
-      D->dev = dev ? dev[0] : 0;
-      D->lo = 0; D->hi = n;
+      if (n_gpus > 1 && (rc = hm_peer_enable(dev,n_gpus)) != HM_OK)   /* pass 2 reads the owners' S lists */
+        { free(s); return rc; }
+      for (int g = 0; g < n_gpus && rc == HM_OK; g++)
+        { DevTable *D = s->d+g;
+          cudaError_t e;
+          D->dev = dev ? dev[g] : g;
+          D->lo = 0; D->hi = n;
 #define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
-      TRY(cudaSetDevice(D->dev));
-      pool_setup(D->dev,1);
-      TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
-      TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
-      TRY(salloc(s,D,(void **) &D->plot,8*(int64_t) HM_PLOT_CELLS));
-      TRY(salloc(s,D,(void **) &D->fp_acc,4*sizeof(uint64_t)));
+          TRY(cudaSetDevice(D->dev));
+          pool_setup(D->dev,n_gpus == 1);                      /* several: the peers map the S lists */
+          TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
+          TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
+          TRY(salloc(s,D,(void **) &D->plot,8*(int64_t) HM_PLOT_CELLS));
+          TRY(salloc(s,D,(void **) &D->fp_acc,4*sizeof(uint64_t)));
 #undef TRY
+        }
+      if (rc == HM_OK && n_gpus > 1 && t->kmer >= HM_SYMM_MIN_KMER)   /* (smaller k: refused by the run) */
+        rc = stream_cuts(s,t);
       if (rc != HM_OK)
         { hm_scan_destroy(s); return rc; }
       s->ms_load = now_ms()-t0;
@@ -661,6 +748,13 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
       return HM_OK;
     }
 
+  for (int g = 0; g < n_gpus; g++)
+    for (int h = 0; h < g; h++)
+      if ((dev ? dev[g] : g) == (dev ? dev[h] : h))
+        { free(s);
+          return hm_set_error(HM_EINVAL,"GPU %d is listed twice: only a streamed scan can run several shards on one "
+                              "device",dev ? dev[g] : g);
+        }
   if (n_gpus > 1 && (rc = hm_peer_enable(dev,n_gpus)) != HM_OK)
     { free(s); return rc; }
 
@@ -1259,6 +1353,7 @@ typedef struct
     void     *sort_tmp;                                /* sorts the S keys of one chunk */
     int64_t   sort_bytes;
     cudaStream_t sc;                                   /* the chunks' kernels: overlap the next chunk's load */
+    hm_stream_sview *views;                            /* several shards: every shard's S view, on this device */
   } StreamRun;
 
 static int64_t stream_list_bytes(const hm_scan *s, const StreamRun *R)
@@ -1278,7 +1373,7 @@ static void stream_free_chunks(hm_scan *s, DevTable *D, StreamRun *R)
   sfree(s,D,R->bucket,4*((1ll << R->bits)+1)); R->bucket = NULL;
   sfree(s,D,R->R.runs,8*R->R.runs_cap);        R->R.runs = NULL;
   sfree(s,D,R->sort_tmp,R->sort_bytes);        R->sort_tmp = NULL;
-  if (R->G.bytes > 0) s->held -= R->G.bytes;
+  if (R->G.bytes > 0) D->held -= R->G.bytes;
   stager_close(D,&R->G);
 }
 
@@ -1286,7 +1381,7 @@ static void stream_free_chunks(hm_scan *s, DevTable *D, StreamRun *R)
 static int stream_alloc_chunks(hm_scan *s, DevTable *D, StreamRun *R, int64_t cap)
 { int KW = s->kmer > 32 ? 2 : 1;
   int64_t need = chunk_bytes(cap,s->kmer,s->ibyte);
-  if (s->held + need > s->budget)
+  if (D->held + need > s->budget)
     return HM_ENOMEM;
   cudaError_t e = cudaSuccess;
   R->cap = cap;
@@ -1304,30 +1399,32 @@ static int stream_alloc_chunks(hm_scan *s, DevTable *D, StreamRun *R, int64_t ca
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"streamed scan: chunk buffers");
   int rc = stager_open(s,D,s->host,cap,&R->G);
-  s->held += R->G.bytes;
-  if (s->held > s->peak) s->peak = s->held;
+  D->held += R->G.bytes;
+  if (D->held > D->peak) D->peak = D->held;
   return rc;
 }
 
 /* grow a group of resident arrays (same capacity, 8-byte elements) to hold `need` entries: doubling, but
- * no further than the final size projected from the `used` entries the first `done` table entries gave */
+ * no further than the final size projected from the `used` entries the first `done` of the shard's `total`
+ * entries gave                                                                                           */
 static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[], int narr, int64_t *cap,
-                       int64_t used, int64_t need, int64_t done, const char *what)
+                       int64_t used, int64_t need, int64_t done, int64_t total, const char *what)
 { if (need <= *cap)
     return HM_OK;
   int64_t nc = 2 * *cap;
   if (done > 0)
-    { int64_t proj = need + (int64_t) ((double) used / (double) done * (double) (s->n - done) * 1.02);
+    { int64_t proj = need + (int64_t) ((double) used / (double) done * (double) (total - done) * 1.02);
       if (nc > proj) nc = proj;
     }
   if (nc < need) nc = need;
-  int64_t room = (s->budget - s->held) / (8*narr);        /* the old arrays are held until the copy is done */
+  int64_t room = (s->budget - D->held) / (8*narr);        /* the old arrays are held until the copy is done */
   if (nc > room) nc = room;
   if (nc < need)
     return hm_set_error(HM_ENOMEM,"the streamed scan's %s list needs %lld entries (%lld bytes) but the device budget "
                         "of %lld bytes has room for %lld more while %lld bytes are held; give the scan a larger "
-                        "budget (HETMERS_DEVICE_BUDGET)",what,(long long) need,(long long) (8*narr*need),
-                        (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) s->held);
+                        "budget (HETMERS_DEVICE_BUDGET)%s",what,(long long) need,(long long) (8*narr*need),
+                        (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) D->held,
+                        s->ngpu > 1 ? "" : " or more GPUs (HETMERS_GPUS)");
   for (int a = 0; a < narr; a++)
     { uint64_t *p = NULL;
       cudaError_t e = salloc(s,D,(void **) &p,8*nc);
@@ -1342,22 +1439,23 @@ static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[
   return HM_OK;
 }
 
-static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, float *ms_kernels)
+/* pass 1 of one shard: its range [D->lo, D->hi) chunk by chunk (leaves early, with HM_OK, once s->stop is set) */
+static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shards *sh, float *ms_kernels)
 { const hm_host_table *t = s->host;
   int      KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
-  int64_t  n = s->n, c0 = 0, chunks = 0;
+  int64_t  lo = D->lo, hi = D->hi, c0 = lo, chunks = 0;
   int      b = 0;
   uint64_t nc = 0, status = 0, ns = 0, ns0 = 0;     /* ns0: S keys before the chunk in flight */
   cudaEvent_t e0, e1;
   HM_CUDA(cudaEventCreate(&e0)); HM_CUDA(cudaEventCreate(&e1));
   HM_CUDA(cudaEventRecord(e0,R->sc));
-  while (c0 < n && rc == HM_OK)
-    { int64_t m = n-c0 < R->cap ? n-c0 : R->cap;
+  while (c0 < hi && rc == HM_OK && !s->stop)
+    { int64_t m = hi-c0 < R->cap ? hi-c0 : R->cap;
       /* the copy + unpack of this chunk overlaps the kernels of the previous one (on R->sc) */
       rc = load_into(s,D,t,R->d_index,c0,m,R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],0,&R->G);
       if (rc != HM_OK) break;
       int64_t cut = m;
-      if (c0+m < n && (rc = last_run_start(R->keys[b],m,s->kmer,&cut)) != HM_OK)
+      if (c0+m < hi && (rc = last_run_start(R->keys[b],m,s->kmer,&cut)) != HM_OK)
         break;
       if (cut == 0)
         { /* one run fills the whole chunk: larger buffers, and load it again */
@@ -1380,9 +1478,10 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, float *ms_kernels)
       ns0 = ns;
       { uint64_t **ca[3] = { &R->R.cand_key, &R->R.cand_meta, &R->R.cand_lo };
         uint64_t **sa[2] = { &R->R.s_key, &R->R.s_lo };
-        rc = stream_grow(s,D,R->sc,ca,KW == 2 ? 3 : 2,&R->R.cand_cap,(int64_t) nc,(int64_t) nc + cut/2 + 1024,c0,"candidate");
+        rc = stream_grow(s,D,R->sc,ca,KW == 2 ? 3 : 2,&R->R.cand_cap,(int64_t) nc,(int64_t) nc + cut/2 + 1024,
+                         c0-lo,hi-lo,"candidate");
         if (rc == HM_OK)
-          rc = stream_grow(s,D,R->sc,sa,KW,&R->R.s_cap,(int64_t) ns,(int64_t) ns + cut + 1024,c0,"S");
+          rc = stream_grow(s,D,R->sc,sa,KW,&R->R.s_cap,(int64_t) ns,(int64_t) ns + cut + 1024,c0-lo,hi-lo,"S");
         if (rc != HM_OK) break;
       }
       rc = hm_k_build_bucket_index(R->keys[b],m,R->bits,R->bucket,0,R->sc);
@@ -1390,8 +1489,8 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, float *ms_kernels)
         rc = hm_k_symm_fingerprint(R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],0,cut,s->kmer,s->seed,D->fp_acc,R->sc);
       if (rc == HM_OK)
         rc = hm_symm_stream_chunk(R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],m,R->bucket,R->bits,s->kmer,cut,
-                                  R->work,&R->L,&R->R,R->sc);
-      s->launches += 4;
+                                  R->work,&R->L,&R->R,sh,R->sc);
+      __sync_fetch_and_add(&s->launches,4);
       c0 += cut;
       chunks += 1;
       b ^= 1;
@@ -1404,19 +1503,32 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, float *ms_kernels)
   if (rc == HM_OK && e != cudaSuccess) rc = hm_cuda_fail(e,"streamed scan: pass 1");
   cudaEventElapsedTime(ms_kernels,e0,e1);
   cudaEventDestroy(e0); cudaEventDestroy(e1);
-  s->chunks = chunks;
+  D->chunks = chunks;
   return rc;
 }
 
-static int run_stream_body(hm_scan *s, DevTable *D, StreamRun *R, int64_t *plot, hm_scan_stats *stats)
-{ int     KW = s->kmer > 32 ? 2 : 1, rc;
+/* one shard's pass 1 on its own device: stub index, work area (the whole-table Bloom filter), chunk buffers,
+ * the chunk loop; then the chunk buffers and the stub index go again, to make room for the S index       */
+typedef struct
+  { hm_scan   *s;
+    int        g, rc;
+    StreamRun *R;
+    float      ms1;                                    /* pass-1 kernels (CUDA events)     */
+    double     ms_loop;                                /* the chunk loop, wall clock       */
+    char       msg[512];
+  } ShardJob;
+
+static int shard_pass1(ShardJob *J)
+{ hm_scan   *s = J->s;
+  DevTable  *D = s->d+J->g;
+  StreamRun *R = J->R;
+  const hm_symm_shards *sh = s->ngpu > 1 ? s->ssh+J->g : NULL;
   int64_t ixlen = (int64_t) 1 << (8*s->ibyte);
-  double  t0 = now_ms();
-  float   ms1 = 0, ms2 = 0;
+  int     rc;
   cudaError_t e;
   HM_CUDA(cudaSetDevice(D->dev));
   HM_CUDA(cudaStreamCreateWithFlags(&R->sc,cudaStreamNonBlocking));
-  if ((rc = stream_work_layout(s->n,s->kmer,&R->L)) != HM_OK) return rc;
+  if ((rc = stream_work_layout(s->n,s->kmer,s->ngpu,&R->L)) != HM_OK) return rc;
   if ((e = salloc(s,D,(void **) &R->d_index,8*ixlen)) != cudaSuccess ||
       (e = salloc(s,D,&R->work,R->L.bytes)) != cudaSuccess)
     return hm_cuda_fail(e,"streamed scan: work area");
@@ -1427,90 +1539,218 @@ static int run_stream_body(hm_scan *s, DevTable *D, StreamRun *R, int64_t *plot,
   HM_CUDA(cudaStreamSynchronize(R->sc));
   if ((rc = stream_alloc_chunks(s,D,R,s->plan.chunk)) != HM_OK)
     return rc == HM_ENOMEM ? hm_set_error(HM_ENOMEM,"the streamed scan's chunk buffers do not fit the device budget") : rc;
-  double t_load0 = now_ms();
-  if ((rc = stream_pass(s,D,R,&ms1)) != HM_OK)
+  double t0 = now_ms();
+  if ((rc = stream_pass(s,D,R,sh,&J->ms1)) != HM_OK)
     return rc;
-  double t_pass1 = now_ms();
-
+  J->ms_loop = now_ms()-t0;
   uint64_t nc = 0, status = 0, ns = 0;
   if ((rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) != HM_OK) return rc;
   if (status != 0)
     return hm_set_error(HM_ECUDA,"streamed scan: list overflow in pass 1 (status %llu)",(unsigned long long) status);
+  return HM_OK;
+}
+
+static void *shard_worker(void *arg)
+{ ShardJob *J = (ShardJob *) arg;
+  J->rc = shard_pass1(J);
+  if (J->rc != HM_OK)
+    { J->s->stop = 1;                                   /* the other shards leave their chunk loops */
+      strncpy(J->msg,hm_last_error(),sizeof(J->msg)-1); J->msg[sizeof(J->msg)-1] = 0;
+    }
+  return NULL;
+}
+
+/* Pass 1 of every shard at once (a host thread each, the calling thread takes the last); the verdict over all
+ * shards' fingerprints; the Bloom segments all-gathered; each shard's S list indexed; pass 2 of every shard,
+ * whose exact checks look keys up in the S list of their owner (peer memory); the plots summed on the host. */
+static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_stats *stats)
+{ int       G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
+  double    t0 = now_ms();
+  float     ms1 = 0, ms2 = 0;
+  double    ms_loop = 0;
+  ShardJob  job[HM_MAX_GPUS];
+  pthread_t th[HM_MAX_GPUS];
+  int       created[HM_MAX_GPUS];
+  cudaError_t e;
+  s->stop = 0;
+  for (int g = 0; g < G; g++)
+    { memset(job+g,0,sizeof(job[g]));
+      job[g].s = s; job[g].g = g; job[g].R = RR+g;
+      created[g] = 0;
+      if (g == G-1 || pthread_create(th+g,NULL,shard_worker,job+g) != 0)
+        shard_worker(job+g);
+      else
+        created[g] = 1;
+    }
+  for (int g = 0; g < G; g++)
+    { if (created[g]) pthread_join(th[g],NULL);
+      if (job[g].rc != HM_OK && rc == HM_OK)
+        rc = G == 1 ? hm_set_error(job[g].rc,"%s",job[g].msg)
+                    : hm_set_error(job[g].rc,"shard %d of %d (GPU %d, entries %lld..%lld): %s",g,G,s->d[g].dev,
+                                   (long long) s->d[g].lo,(long long) s->d[g].hi,job[g].msg);
+      if (job[g].ms1 > ms1)         ms1 = job[g].ms1;
+      if (job[g].ms_loop > ms_loop) ms_loop = job[g].ms_loop;
+    }
+  if (rc != HM_OK)
+    return rc;
+  double t_pass1 = now_ms();
   if ((rc = fingerprint_verdict(s)) != HM_OK) return rc;
   if (!s->symmetric)
     return hm_set_error(HM_EUNSUPPORTED,"the table of %lld entries does not fit in device memory (budget %lld bytes) and "
                         "is not strand-symmetric; the direct passes need it resident",(long long) s->n,(long long) s->budget);
+
+  uint64_t ns[HM_MAX_GPUS];
+  int      sbits[HM_MAX_GPUS], sidx64 = 0;
+  for (int g = 0; g < G; g++)
+    { uint64_t nc = 0, status = 0;
+      HM_CUDA(cudaSetDevice(s->d[g].dev));
+      if ((rc = hm_symm_stream_counts(RR[g].work,&RR[g].L,&nc,&status,&ns[g],RR[g].sc)) != HM_OK) return rc;
+      if ((int64_t) ns[g] >= 0xFFFFFFF0ll) sidx64 = 1;    /* one offset width for every shard's index */
+    }
+  if (G > 1)                                    /* every shard pulls the other shards' Bloom segments */
+    for (int g = 0; g < G; g++)
+      { DevTable *D = s->d+g;
+        size_t    segb = sizeof(uint32_t)*(size_t) RR[g].L.seg_words;
+        HM_CUDA(cudaSetDevice(D->dev));
+        for (int h = 0; h < G; h++)
+          if (h != g && s->d[h].hi > s->d[h].lo)
+            HM_CUDA(cudaMemcpyPeerAsync((uint8_t *) RR[g].work + RR[g].L.off_bloom + segb*h,D->dev,
+                                        (uint8_t *) RR[h].work + RR[h].L.off_bloom + segb*h,s->d[h].dev,segb,RR[g].sc));
+      }
   /* S (sorted chunk by chunk) gets a bucket index in the room the chunk buffers leave: as fine as
    * hm_pick_bucket_bits asks, coarser if the budget says so (look-ups then bisect longer buckets)        */
-  stream_free_chunks(s,D,R);
-  sfree(s,D,R->d_index,8*ixlen); R->d_index = NULL;
-  int sbits = hm_pick_bucket_bits((int64_t) ns), sidx64 = ((int64_t) ns >= 0xFFFFFFF0ll);
-  while (sbits > 1 && s->held + (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits)+1) > s->budget)
-    sbits -= 1;
-  R->s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits)+1);
-  if ((e = salloc(s,D,&R->s_bucket,R->s_bucket_bytes)) != cudaSuccess)
-    return hm_cuda_fail(e,"streamed scan: S index");
-  if ((rc = hm_k_build_bucket_index(R->R.s_key,(int64_t) ns,sbits,R->s_bucket,sidx64,R->sc)) != HM_OK) return rc;
+  for (int g = 0; g < G; g++)
+    { DevTable  *D = s->d+g;
+      StreamRun *R = RR+g;
+      HM_CUDA(cudaSetDevice(D->dev));
+      stream_free_chunks(s,D,R);
+      sfree(s,D,R->d_index,8*((int64_t) 1 << (8*s->ibyte))); R->d_index = NULL;
+      sbits[g] = hm_pick_bucket_bits((int64_t) ns[g]);
+      while (sbits[g] > 1 && D->held + (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1) > s->budget)
+        sbits[g] -= 1;
+      R->s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1);
+      if ((e = salloc(s,D,&R->s_bucket,R->s_bucket_bytes)) != cudaSuccess)
+        return hm_cuda_fail(e,"streamed scan: S index");
+      if (G > 1)
+        HM_CUDA(cudaMemsetAsync(R->s_bucket,0,(size_t) R->s_bucket_bytes,R->sc));   /* (an empty S list: all 0) */
+      if ((G == 1 || ns[g] > 0) &&
+          (rc = hm_k_build_bucket_index(R->R.s_key,(int64_t) ns[g],sbits[g],R->s_bucket,sidx64,R->sc)) != HM_OK)
+        return rc;
+    }
+  if (G > 1)                                    /* each shard's pass 2 reads every shard's S view */
+    { hm_stream_sview V[HM_MAX_GPUS];
+      memset(V,0,sizeof(V));
+      for (int h = 0; h < G; h++)
+        { V[h].s_key = RR[h].R.s_key; V[h].s_lo = KW == 2 ? RR[h].R.s_lo : NULL;
+          V[h].s_bucket = RR[h].s_bucket; V[h].n_s = (int64_t) ns[h]; V[h].bits = sbits[h];
+        }
+      for (int g = 0; g < G; g++)
+        { DevTable *D = s->d+g;
+          HM_CUDA(cudaSetDevice(D->dev));
+          if ((e = salloc(s,D,(void **) &RR[g].views,sizeof(V))) != cudaSuccess)
+            return hm_cuda_fail(e,"streamed scan: S views");
+          HM_CUDA(cudaMemcpyAsync(RR[g].views,V,sizeof(V),cudaMemcpyHostToDevice,RR[g].sc));
+        }
+      for (int g = 0; g < G; g++)               /* every S index and Bloom segment is in place */
+        { HM_CUDA(cudaSetDevice(s->d[g].dev)); HM_CUDA(cudaStreamSynchronize(RR[g].sc)); }
+    }
 
-  cudaEvent_t e2, e3;
-  HM_CUDA(cudaEventCreate(&e2)); HM_CUDA(cudaEventCreate(&e3));
-  cudaEventRecord(e2,R->sc);
-  rc = hm_symm_stream_resolve(R->R.s_key,KW == 2 ? R->R.s_lo : NULL,(int64_t) ns,R->s_bucket,sbits,sidx64,s->kmer,
-                              s->n,R->work,&R->L,&R->R,D->plot,R->sc);
-  cudaEventRecord(e3,R->sc);
-  s->launches += 3;
-  if (rc == HM_OK && (e = cudaMemcpyAsync(plot,D->plot,sizeof(int64_t)*HM_PLOT_CELLS,cudaMemcpyDeviceToHost,R->sc)) != cudaSuccess)
-    rc = hm_cuda_fail(e,"plot D2H");
-  if (rc == HM_OK)
-    rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc);
-  cudaEventElapsedTime(&ms2,e2,e3);
-  cudaEventDestroy(e2); cudaEventDestroy(e3);
-  if (rc == HM_OK && status != 0)
-    rc = hm_set_error(HM_ECUDA,"streamed scan: pass 2 status %llu",(unsigned long long) status);
+  cudaEvent_t ev[HM_MAX_GPUS][2];
+  memset(ev,0,sizeof(ev));
+  for (int g = 0; g < G; g++)
+    { DevTable  *D = s->d+g;
+      StreamRun *R = RR+g;
+      HM_CUDA(cudaSetDevice(D->dev));
+      HM_CUDA(cudaEventCreate(&ev[g][0])); HM_CUDA(cudaEventCreate(&ev[g][1]));
+      cudaEventRecord(ev[g][0],R->sc);
+      rc = hm_symm_stream_resolve(R->R.s_key,KW == 2 ? R->R.s_lo : NULL,(int64_t) ns[g],R->s_bucket,sbits[g],sidx64,
+                                  s->kmer,G == 1 ? s->n : D->hi-D->lo,R->work,&R->L,&R->R,G > 1 ? s->ssh+g : NULL,
+                                  R->views,D->plot,R->sc);
+      cudaEventRecord(ev[g][1],R->sc);
+      __sync_fetch_and_add(&s->launches,3);
+      if (rc != HM_OK) break;
+    }
+  int64_t *tmp = NULL;
+  if (rc == HM_OK && G > 1)
+    { tmp = (int64_t *) malloc(sizeof(int64_t)*HM_PLOT_CELLS);
+      if (tmp == NULL) rc = hm_set_error(HM_ENOMEM,"out of host memory");
+      else             memset(plot,0,sizeof(int64_t)*HM_PLOT_CELLS);
+    }
+  for (int g = 0; g < G; g++)
+    { DevTable  *D = s->d+g;
+      StreamRun *R = RR+g;
+      uint64_t   nc = 0, status = 0, nsx = 0;
+      float      b = 0;
+      cudaSetDevice(D->dev);
+      if (rc == HM_OK && (e = cudaMemcpyAsync(G == 1 ? plot : tmp,D->plot,sizeof(int64_t)*HM_PLOT_CELLS,
+                                              cudaMemcpyDeviceToHost,R->sc)) != cudaSuccess)
+        rc = hm_cuda_fail(e,"plot D2H");
+      if (rc == HM_OK)
+        rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&nsx,R->sc);      /* (synchronises) */
+      if (rc == HM_OK && status != 0)
+        rc = hm_set_error(HM_ECUDA,"streamed scan: pass 2 status %llu%s",(unsigned long long) status,G > 1 ? " on a shard" : "");
+      if (rc == HM_OK && G > 1)
+        for (int64_t i = 0; i < HM_PLOT_CELLS; i++)
+          plot[i] += tmp[i];
+      cudaStreamSynchronize(R->sc);
+      if (ev[g][1] != NULL && cudaEventElapsedTime(&b,ev[g][0],ev[g][1]) == cudaSuccess && b > ms2)
+        ms2 = b;
+      cudaGetLastError();
+      if (ev[g][0] != NULL) cudaEventDestroy(ev[g][0]);
+      if (ev[g][1] != NULL) cudaEventDestroy(ev[g][1]);
+    }
+  free(tmp);
   if (rc != HM_OK)
     return rc;
   double t1 = now_ms();
   s->last_path = HM_PATH_SYMM;
   if (stats != NULL)
-    { stats->nels = s->n; stats->n_gpus = 1; stats->bucket_bits = R->bits;
+    { stats->nels = s->n; stats->n_gpus = G; stats->bucket_bits = RR[0].bits;
       stats->filter_bits = 0; stats->path = HM_PATH_SYMM;
-      stats->ms_h2d_unpack = s->ms_load + (t_pass1-t_load0);    /* the loads, with pass 1 running behind them */
-      stats->ms_pass1 = ms1; stats->ms_pass2 = ms2;
+      stats->ms_h2d_unpack = s->ms_load + ms_loop;              /* the loads, with pass 1 running behind them */
+      stats->ms_pass1 = ms1; stats->ms_pass2 = ms2;             /* (the slowest shard's) */
       stats->ms_scan = t1-t0;
       stats->ms_total = s->ms_load + (t1-t0);
       stats->kernel_launches = s->launches;
-      stats->ms_alloc = s->ms_alloc; stats->ms_records = t_pass1-t_load0; stats->ms_index = t1-t_pass1;
+      stats->ms_alloc = s->ms_alloc; stats->ms_records = ms_loop; stats->ms_index = t1-t_pass1;
     }
   return HM_OK;
 }
 
 static int run_stream(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
-{ DevTable *D = s->d;
-  StreamRun R;
+{ int       G = s->ngpu;
+  StreamRun R[HM_MAX_GPUS];
+  int64_t   held0[HM_MAX_GPUS];
   if (s->kmer < HM_SYMM_MIN_KMER)
     return hm_set_error(HM_EUNSUPPORTED,"the table does not fit in device memory and k = %d has no strand-symmetric "
                         "scan; the direct passes need it resident",s->kmer);
-  memset(&R,0,sizeof(R));
-  int64_t held0 = s->held;
-  s->peak = held0;
-  int rc = run_stream_body(s,D,&R,plot,stats);
-  cudaSetDevice(D->dev);
-  if (R.sc) cudaStreamSynchronize(R.sc);
-  stream_free_chunks(s,D,&R);
-  sfree(s,D,R.d_index,8*((int64_t) 1 << (8*s->ibyte)));
-  sfree(s,D,R.work,R.L.bytes);
-  sfree(s,D,R.s_bucket,R.s_bucket_bytes);
-  { int KW = s->kmer > 32 ? 2 : 1;
-    sfree(s,D,R.R.cand_key,8*R.R.cand_cap); sfree(s,D,R.R.cand_meta,8*R.R.cand_cap);
-    if (KW == 2) sfree(s,D,R.R.cand_lo,8*R.R.cand_cap);
-    sfree(s,D,R.R.s_key,8*R.R.s_cap);
-    if (KW == 2) sfree(s,D,R.R.s_lo,8*R.R.s_cap);
-  }
-  if (D->st) cudaStreamSynchronize(D->st);
-  if (R.sc) cudaStreamDestroy(R.sc);
-  cudaCtxResetPersistingL2Cache();
-  cudaGetLastError();
-  s->held = held0;
+  memset(R,0,sizeof(R));
+  for (int g = 0; g < G; g++)
+    { held0[g] = s->d[g].held;
+      s->d[g].peak = held0[g];
+      s->d[g].chunks = 0;
+    }
+  int rc = run_stream_body(s,R,plot,stats);
+  for (int g = 0; g < G; g++)                  /* every shard's thread has been joined: free it all */
+    { DevTable *D = s->d+g;
+      int KW = s->kmer > 32 ? 2 : 1;
+      cudaSetDevice(D->dev);
+      if (R[g].sc) cudaStreamSynchronize(R[g].sc);
+      stream_free_chunks(s,D,R+g);
+      sfree(s,D,R[g].d_index,8*((int64_t) 1 << (8*s->ibyte)));
+      sfree(s,D,R[g].work,R[g].L.bytes);
+      sfree(s,D,R[g].s_bucket,R[g].s_bucket_bytes);
+      sfree(s,D,R[g].views,sizeof(hm_stream_sview)*HM_MAX_GPUS);
+      sfree(s,D,R[g].R.cand_key,8*R[g].R.cand_cap); sfree(s,D,R[g].R.cand_meta,8*R[g].R.cand_cap);
+      if (KW == 2) sfree(s,D,R[g].R.cand_lo,8*R[g].R.cand_cap);
+      sfree(s,D,R[g].R.s_key,8*R[g].R.s_cap);
+      if (KW == 2) sfree(s,D,R[g].R.s_lo,8*R[g].R.s_cap);
+      if (D->st) cudaStreamSynchronize(D->st);
+      if (R[g].sc) cudaStreamDestroy(R[g].sc);
+      cudaCtxResetPersistingL2Cache();
+      cudaGetLastError();
+      D->held = held0[g];
+    }
   return rc;
 }
 

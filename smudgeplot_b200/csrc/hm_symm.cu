@@ -1305,6 +1305,20 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
   revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
   ry = rx; ryl = rxl;
   set_base<KW>(ry,ryl,kmer-1-p,3-yb);                      /* rc y = rc x with the mirrored base swapped */
+  if (SL && W.n_seg > 1)                                   /* several shards: the S list of the key's owner */
+    { const hm_stream_sview *V = (const hm_stream_sview *) W.cand_n[SY_HDR_S+4];
+      if (ha)
+        { const hm_stream_sview &a = V[owner_of(W,rx)];
+          if (bucket_find<IdxT,KW>(a.s_key,a.s_lo,(const IdxT *) a.s_bucket,64-a.bits,rx,rxl) >= 0)
+            return false;
+        }
+      if (hb)
+        { const hm_stream_sview &b = V[owner_of(W,ry)];
+          if (bucket_find<IdxT,KW>(b.s_key,b.s_lo,(const IdxT *) b.s_bucket,64-b.bits,ry,ryl) >= 0)
+            return false;
+        }
+      return true;
+    }
   if (SL)
     return !((ha && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
              (hb && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0));
@@ -1535,9 +1549,18 @@ extern "C" int hm_symm_align_cut(const uint64_t *d_keys, int64_t n, int kmer, in
 /* The table passes through the GPU chunk by chunk (hm_scan.cu drives it, DESIGN.md §4c).  The work area of
  * hm_symm_plan(n, 0, kmer, 1) supplies the header and the whole-table Bloom filter (only they are used); the
  * run list of one chunk, the candidate records and the S list are arrays of the caller's, the last two
- * resident and grown between chunks.                                                                      */
-static SymmView stream_view(void *d_work, const hm_symm_layout *L, const hm_stream_lists *R)
+ * resident and grown between chunks.  Several shards: hm_symm_plan(n, 0, kmer, G) -- shard r fills segment r,
+ * the caller all-gathers the segments before pass 2; n_seg of the view is the shards' descriptor's (the
+ * shards up to the last non-empty one), so that no key is owned by an empty shard at the end.           */
+static SymmView stream_view(void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, const hm_symm_shards *sh)
 { SymmView W = make_view(d_work,L,NULL);
+  W.n_seg = 1;
+  if (sh != NULL && sh->n_seg > 1)
+    { W.n_seg = sh->n_seg; W.self = sh->self;
+      for (int r = 0; r < sh->n_seg; r++) W.first_key[r] = sh->first_key[r];
+    }
+  else if (sh != NULL)
+    W.self = sh->self;
   W.cand_key = R->cand_key; W.cand_lo = R->cand_lo; W.cand_meta = R->cand_meta;
   W.cand_cap = (unsigned long long) R->cand_cap;
   W.runs = R->runs; W.runs_cap = (unsigned long long) R->runs_cap;
@@ -1547,22 +1570,25 @@ static SymmView stream_view(void *d_work, const hm_symm_layout *L, const hm_stre
 int hm_symm_stream_begin(void *d_work, const hm_symm_layout *L, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   SymmView W = make_view(d_work,L,NULL);
+  size_t bloom_bytes = sizeof(uint32_t)*(size_t) W.seg_words*(size_t) L->n_seg;   /* every segment */
   HM_CUDA(cudaMemsetAsync(W.cand_n,0,256,st));
-  HM_CUDA(cudaMemsetAsync(W.bloom,0,sizeof(uint32_t)*(size_t) W.seg_words,st));
+  HM_CUDA(cudaMemsetAsync(W.bloom,0,bloom_bytes,st));
   if (l2_persist())
-    bloom_window(st,W.bloom,sizeof(uint32_t)*(size_t) W.seg_words,1);
+    bloom_window(st,W.bloom,bloom_bytes,1);
   return HM_OK;
 }
 
 int hm_symm_stream_chunk(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
                                     int64_t n, const void *d_bucket, int bits, int kmer, int64_t hi,
-                                    void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, void *stream)
+                                    void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                                    const hm_symm_shards *shards, void *stream)
 { if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || hi < 0 || hi > n || bits < 1 || bits > 30 ||
-      (kmer > 32) != (d_keys_lo != NULL))
+      (kmer > 32) != (d_keys_lo != NULL) || (shards != NULL && (shards->self < 0 || shards->self >= L->n_seg ||
+                                                                shards->n_seg > L->n_seg)))
     return hm_set_error(HM_EINVAL,"symm_stream_chunk: bad arguments (k=%d, %lld of %lld entries)",
                         kmer,(long long) hi,(long long) n);
   cudaStream_t st = (cudaStream_t) stream;
-  SymmView W = stream_view(d_work,L,R);
+  SymmView W = stream_view(d_work,L,R,shards);
   uint64_t h[4] = { (uint64_t) R->s_cap, (uint64_t) (uintptr_t) R->s_key, (uint64_t) (uintptr_t) R->s_lo, 0 };
   HM_CUDA(cudaMemsetAsync(W.runs_n,0,sizeof(uint64_t),st));                 /* the run list is per chunk */
   HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_S+1,h,3*sizeof(uint64_t),cudaMemcpyHostToDevice,st));
@@ -1593,15 +1619,22 @@ int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t 
   return HM_OK;
 }
 
-/* pass 2 of the streamed scan: the exact check of a Bloom hit is a look-up in the sorted S list */
+/* pass 2 of the streamed scan: the exact check of a Bloom hit is a look-up in the sorted S list (several shards:
+ * the S list of the key's owner, reached through d_views, whose address goes into header word SY_HDR_S+4)    */
 int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
                                       const void *d_s_bucket, int bits, int idx64, int kmer, int64_t range,
                                       void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                                      const hm_symm_shards *shards, const hm_stream_sview *d_views,
                                       unsigned long long *d_plot, void *stream)
-{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_plot == NULL)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_plot == NULL ||
+      (shards != NULL && shards->n_seg > 1 && d_views == NULL))
     return hm_set_error(HM_EINVAL,"symm_stream_resolve: bad arguments");
   cudaStream_t st = (cudaStream_t) stream;
-  SymmView W = stream_view(d_work,L,R);
+  SymmView W = stream_view(d_work,L,R,shards);
+  if (W.n_seg > 1)
+    { uint64_t v = (uint64_t) (uintptr_t) d_views;
+      HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_S+4,&v,sizeof(v),cudaMemcpyHostToDevice,st));
+    }
   cudaError_t e;
   if (kmer <= 32)
     e = idx64 ? launch_resolve<uint64_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)

@@ -4,7 +4,10 @@ configs[1]): ms per hm_hetmers_host call from the same pinned host table, chunks
 over PCIe, with the card name and power limit.  Prints one JSON line; exits 3 unless the streamed plot equals
 the in-core plot.  Writes nothing to the tree.
 
-    python tools/time_stream.py --budget-gb 1.6 [--nels 2e8] [--steps 5] [--warmup 2]
+    python tools/time_stream.py --budget-gb 1.6 [--nels 2e8] [--steps 5] [--warmup 2] [--gpus N]
+
+--gpus N streams over devices 0..N-1, a run-aligned share of the table each (the budget is per GPU); the
+in-core scan it is compared with runs on the same devices.
 """
 import argparse
 import ctypes as C
@@ -61,6 +64,7 @@ def main():
     ap.add_argument("--nels", type=float, default=2e8)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--gpus", type=int, default=1, help="stream over devices 0..N-1")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -74,7 +78,10 @@ def main():
     del keys, cnt
     torch.cuda.empty_cache()
     L = _lib.lib()
-    devs = (C.c_int * 1)(0)
+    ng = a.gpus
+    if not 1 <= ng <= torch.cuda.device_count():
+        raise SystemExit(f"time_stream.py: --gpus {ng} asks for more GPUs than the {torch.cuda.device_count()} visible")
+    devs = (C.c_int * ng)(*range(ng))
     budget = int(a.budget_gb * 1e9)
 
     def timed(stream):
@@ -85,13 +92,13 @@ def main():
         st = _lib.ScanStats()
         try:
             for _ in range(max(a.warmup, 1)):
-                _lib.check(L.hm_hetmers_host(C.byref(ht), devs, 1, plot.data_ptr(), C.byref(st)))
+                _lib.check(L.hm_hetmers_host(C.byref(ht), devs, ng, plot.data_ptr(), C.byref(st)))
             t0 = time.perf_counter()
             for _ in range(a.steps):
-                _lib.check(L.hm_hetmers_host(C.byref(ht), devs, 1, plot.data_ptr(), C.byref(st)))
+                _lib.check(L.hm_hetmers_host(C.byref(ht), devs, ng, plot.data_ptr(), C.byref(st)))
             dt = (time.perf_counter() - t0) / a.steps
             h = C.c_void_p()                         # one more scan, kept open to read its residency
-            _lib.check(L.hm_scan_create(C.byref(ht), devs, 1, C.byref(h)))
+            _lib.check(L.hm_scan_create(C.byref(ht), devs, ng, C.byref(h)))
             try:
                 p2 = torch.empty(_lib.PLOT_CELLS, dtype=torch.int64)
                 _lib.check(L.hm_scan_run(h, p2.data_ptr(), None))
@@ -110,7 +117,7 @@ def main():
     rec_bytes = int(h_rec.numel())
     line = {"metric": "ms per hm_hetmers_host call, streamed vs in core", "unit": "ms",
             "workload": workload_name(1), "nels": n, "steps": a.steps, "warmup": max(a.warmup, 1),
-            "gpu": torch.cuda.get_device_name(0), "power_limit": power_limit(), "budget_bytes": budget,
+            "gpu": torch.cuda.get_device_name(0), "gpus": ng, "power_limit": power_limit(), "budget_bytes": budget,
             "in_core": {"ms_per_call": ms_in, "device_bytes": res_in[1],
                         "records_gbs": rec_bytes / (ms_in * 1e-3) / 1e9,
                         "last_call_ms": {"load": st_in.ms_h2d_unpack, "pass1": st_in.ms_pass1, "pass2": st_in.ms_pass2}},
