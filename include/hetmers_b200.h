@@ -199,6 +199,17 @@ int  hm_k_symm_resolve(const uint64_t *d_keys, const uint64_t *d_keys_lo, const 
                        const void *d_bucket, int bits, int idx64, int kmer,
                        void *d_work, const hm_symm_layout *layout, const hm_symm_shards *shards,
                        unsigned long long *d_plot, void *stream);
+/* extract_kmer_pairs on the same work area, after hm_k_symm_runscan + hm_k_symm_runs (one GPU, or each GPU of an
+ * in-core scan with the Bloom segments all-gathered): the isolated pairs among candidates [c0, c1) whose pixel
+ * (sum, min) has a non-zero label in d_pixmap are appended to d_out as hm_k_pass2_extract lists them -- each
+ * candidate once, and its mirror image (rc y, rc x) too unless the pair differs at the middle base of an odd k
+ * (DESIGN.md §4a).  At most 2 (c1-c0) records; *d_count (zeroed by the caller) counts all of them, also those
+ * beyond `cap`.  The candidate count is in the work-area header (hm_symm_status).                          */
+int  hm_k_symm_extract(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
+                       const void *d_bucket, int bits, int idx64, int kmer,
+                       void *d_work, const hm_symm_layout *layout, const hm_symm_shards *shards,
+                       const uint16_t *d_pixmap, int64_t c0, int64_t c1, hm_pair_rec *d_out, int64_t cap,
+                       unsigned long long *d_count, void *stream);
 int  hm_symm_status(const void *d_work, const hm_symm_layout *layout, uint64_t *n_cand, uint64_t *status,
                     void *stream);
 int  hm_symm_align_cut(const uint64_t *d_keys, int64_t n, int kmer, int64_t cut, int64_t *out);
@@ -293,8 +304,17 @@ int  hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_symm, int64_
 int  hm_scan_run(hm_scan *s, int64_t *plot, hm_scan_stats *stats);
 int  hm_scan_run_path(hm_scan *s, int path, int64_t *plot, hm_scan_stats *stats);
 int  hm_scan_is_symmetric(const hm_scan *s);
-/* the pair list of extract_kmer_pairs (runs the direct passes first if the last run did not) for a pixel->smudge map (host
- * uint16[HM_PLOT_CELLS]); *out is malloc'ed (caller frees), sorted by (smudge, k-mer).          */
+/* the pair list of extract_kmer_pairs for a pixel->smudge map (host uint16[HM_PLOT_CELLS]); *out is malloc'ed
+ * (caller frees), sorted by (smudge, k-mer).  The route follows hm_scan_run's rule: on a table the fingerprint
+ * found strand-symmetric (k >= HM_SYMM_MIN_KMER) the pairs are listed from the candidates of the last symmetric
+ * run (hm_k_symm_extract, one launch per GPU and slice) -- a symmetric run is done first when the last run left
+ * none with a clean status, and one that fails its checks falls back to the direct route; other tables take the
+ * direct passes' results (the direct passes run first if the last run did not leave them).  HETMERS_PATH=
+ * direct|symm forces a route as it does for a run (symm on a table that is not symmetric is an error).  Either
+ * route gives the same list.  The symmetric route's record buffer on each GPU is what the device budget leaves
+ * beyond the scan's arrays (HM_ENOMEM, before any launch, if that is less than HM_EXTRACT_MIN_BYTES); the
+ * candidates pass through it in slices.  A streamed scan refuses (HM_EUNSUPPORTED).                          */
+#define HM_EXTRACT_MIN_BYTES (2ll*HM_PLOT_CELLS + (1ll << 16))   /* device pixmap + 64 KiB of records */
 int  hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out);
 /* ---- device budget and the streamed symmetric scan (DESIGN.md §4c) --------------------------------
  * hm_scan_create computes the bytes the in-core scan would allocate per GPU (table arrays, bucket index,

@@ -23,6 +23,7 @@ ABI_SYMBOLS = [
     "hm_dev_alloc", "hm_dev_free", "hm_ipc_export", "hm_ipc_open", "hm_ipc_close", "hm_p2p_native_atomics",
     "hm_scan_create", "hm_prewarm", "hm_set_io_threads", "hm_scan_destroy", "hm_scan_examine", "hm_scan_condition", "hm_scan_run", "hm_hetmers_host",
     "hm_scan_run_path", "hm_scan_is_symmetric", "hm_symm_plan", "hm_symm_seeds", "hm_k_symm_fingerprint", "hm_k_symm_runscan", "hm_k_symm_runs", "hm_k_symm_resolve",
+    "hm_k_symm_extract",
     "hm_symm_status", "hm_symm_align_cut",
     "hm_scan_download", "hm_set_device_budget", "hm_stream_plan", "hm_stream_plan_shards", "hm_scan_residency", "hm_table_open", "hm_table_close", "hm_table_view", "hm_write_smu",
 ]
@@ -68,6 +69,7 @@ class StreamLayout(C.Structure):
 
 
 BUDGET_RESERVE = 1 << 30
+EXTRACT_MIN_BYTES = 2 * PLOT_CELLS + (1 << 16)   # HM_EXTRACT_MIN_BYTES: device room hm_scan_extract's symmetric route needs
 
 
 class PairRec(C.Structure):
@@ -137,6 +139,8 @@ def lib():
                                  C.POINTER(SymmShards), vp]
     L.hm_k_symm_resolve.argtypes = [vp, vp, vp, i64, vp, i32, i32, i32, vp, C.POINTER(SymmLayout),
                                     C.POINTER(SymmShards), vp, vp]
+    L.hm_k_symm_extract.argtypes = [vp, vp, vp, i64, vp, i32, i32, i32, vp, C.POINTER(SymmLayout),
+                                    C.POINTER(SymmShards), vp, i64, i64, vp, i64, vp, vp]
     L.hm_symm_status.argtypes = [vp, C.POINTER(SymmLayout), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), vp]
     L.hm_symm_align_cut.argtypes = [vp, i64, i32, i64, C.POINTER(i64)]
     L.hm_scan_create.argtypes = [C.POINTER(HostTable), C.POINTER(i32), i32, C.POINTER(vp)]

@@ -67,6 +67,8 @@ struct hm_scan
     int      symmetric;                   /* fingerprint verdict: every rc(x) present with count(x)        */
     int      have_direct;                 /* deg / up / filter allocated and the filter built               */
     int      have_symm;                   /* symmetric-scan work areas allocated, cuts aligned              */
+    int      symm_ready;                  /* they hold the candidates of a symmetric run with a clean status  */
+                                          /*   (what hm_scan_extract lists the pairs from)                    */
     int      last_path;                   /* HM_PATH_DIRECT / HM_PATH_SYMM of the last run                  */
     int      invalid;                     /* a failed conditioning left the replicas inconsistent            */
     hm_symm_shards ssh[HM_MAX_GPUS];
@@ -906,7 +908,7 @@ static int ensure_symm(hm_scan *s)
       if (D->symm_work != NULL) { dfree(D->dev,D->st,D->symm_work); D->symm_work = NULL; }
       HM_CUDA(dalloc(D->dev,D->st,&D->symm_work,(size_t) D->symm_layout.bytes));
     }
-  s->have_symm = 1;
+  s->have_symm = 1; s->symm_ready = 0;
   return HM_OK;
 }
 
@@ -934,7 +936,7 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
                           "budget of %lld",(long long) s->n,(long long) need,(long long) s->budget);
   }
   /* everything derived from the old table goes first: work buffers of both paths, the index */
-  s->ran = 0; s->have_direct = 0; s->have_symm = 0;
+  s->ran = 0; s->have_direct = 0; s->have_symm = 0; s->symm_ready = 0;
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
@@ -1223,6 +1225,7 @@ static int run_symm(hm_scan *s, int64_t *plot, hm_scan_stats *stats, uint64_t *s
   float       ms1 = 0, ms2 = 0, msall = 0;
   if ((rc = ensure_symm(s)) != HM_OK)
     return rc;
+  s->symm_ready = 0;
   double      t0 = now_ms();
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
@@ -1304,6 +1307,7 @@ static int run_symm(hm_scan *s, int64_t *plot, hm_scan_stats *stats, uint64_t *s
         cudaEventDestroy(ev[g][k]);
     }
   s->last_path = HM_PATH_SYMM;
+  s->symm_ready = (*status == 0);
   if (stats != NULL)
     { stats->nels = n; stats->n_gpus = G; stats->bucket_bits = s->bits;
       stats->filter_bits = 0; stats->path = HM_PATH_SYMM;
@@ -1899,15 +1903,49 @@ static int rec_cmp(const void *a, const void *b)
   return ((int) x->alt - (int) y->alt);
 }
 
-/* extract_kmer_pairs' output as a list (PloidyList.c:425-450): needs the incidence array and the
- * recorded partners of a preceding hm_scan_run.  Two launches per GPU: count, then fill.        */
-extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out)
+/* the order hm_scan_extract returns: qsort with rec_cmp.  Its time depends on the order the records arrive in, so
+ * for long lists a stable counting pass by (smudge, first 8 bases) puts every record into its final bucket first
+ * and qsort only has to order the buckets' insides.  configs[1] (2.6e7 records, the host of an H100 machine): a
+ * whole call took 6.9-7.3 s on the direct route and 7.7-8.8 s on the symmetric one (half of its records, the
+ * mirror images, come in no key order) with qsort alone, 4.7-4.8 s on either with the pass.  The result does not
+ * depend on the pass (without host memory for its copy the records go to qsort as they are).                  */
+static void sort_records(hm_pair_rec *r, int64_t n)
+{ if (n >= (1 << 16))
+    { uint32_t top = 0;
+      for (int64_t i = 0; i < n; i++)
+        if (r[i].smudge > top) top = r[i].smudge;
+      int32_t *rank = top <= 0xffff ? (int32_t *) calloc((size_t) top+1,sizeof(int32_t)) : NULL;
+      if (rank != NULL)
+        { int32_t nl = 0;
+          int     b  = 16;
+          for (int64_t i = 0; i < n; i++)
+            rank[r[i].smudge] = 1;
+          for (uint32_t l = 0; l <= top; l++)                /* used labels in ascending order -> 0, 1, ... */
+            rank[l] = rank[l] ? nl++ : -1;
+          while (b > 4 && ((int64_t) nl << b) > (1ll << 22))
+            b -= 1;
+          int64_t     nb  = (int64_t) nl << b;
+          int64_t    *at  = (int64_t *) calloc((size_t) nb+1,sizeof(int64_t));
+          hm_pair_rec *o  = (hm_pair_rec *) malloc(sizeof(hm_pair_rec)*(size_t) n);
+          if (at != NULL && o != NULL)
+            { for (int64_t i = 0; i < n; i++)
+                at[1 + ((int64_t) rank[r[i].smudge] << b) + (int64_t) (r[i].key_hi >> (64-b))] += 1;
+              for (int64_t k = 0; k < nb; k++)
+                at[k+1] += at[k];
+              for (int64_t i = 0; i < n; i++)
+                o[at[((int64_t) rank[r[i].smudge] << b) + (int64_t) (r[i].key_hi >> (64-b))]++] = r[i];
+              memcpy(r,o,sizeof(hm_pair_rec)*(size_t) n);
+            }
+          free(at); free(o); free(rank);
+        }
+    }
+  qsort(r,(size_t) n,sizeof(hm_pair_rec),rec_cmp);
+}
+
+/* the direct route of hm_scan_extract: the incidence array and recorded partners of the direct passes (run first if
+ * the last run did not leave them).  Two launches per GPU: count, then fill.                                    */
+static int extract_direct(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out)
 { int G = s->ngpu, rc = HM_OK;
-  if (s->streamed)
-    return hm_set_error(HM_EUNSUPPORTED,"listing k-mer pairs needs the direct passes' arrays, and this table does not "
-                                        "fit in device memory (budget %lld bytes)",(long long) s->budget);
-  if (s->invalid)
-    return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
   if ((rc = need_direct_results(s)) != HM_OK)
     return rc;
   int64_t      total = 0, cnts[HM_MAX_GPUS];
@@ -1956,7 +1994,172 @@ extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec *
     }
   if (rc != HM_OK)
     { free(host); return rc; }
-  qsort(host,(size_t) total,sizeof(hm_pair_rec),rec_cmp);      /* deterministic order */
+  *out = host; *n_out = total;
+  return HM_OK;
+}
+
+/* the symmetric route: the candidates the last symmetric run left in each GPU's work area, listed by
+ * hm_k_symm_extract against that GPU's replica (DESIGN.md §4a).  The record buffer of a GPU is what the device
+ * budget leaves beyond the scan's own arrays (at most two records per candidate); the candidates go through it
+ * in slices of half its records, and the host list grows slice by slice.  *status: the OR of the work areas'
+ * status words afterwards (non-zero: the list must not be used).                                            */
+static int extract_symm(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out, uint64_t *status)
+{ int     G = s->ngpu, rc = HM_OK;
+  int64_t held = incore_bytes(s->n,s->kmer,G,s->bits,s->idx64);    /* (conditioning may have grown the table) */
+  int64_t nc[HM_MAX_GPUS], c0[HM_MAX_GPUS], slice[HM_MAX_GPUS];
+  if (held < s->incore_bytes) held = s->incore_bytes;
+  for (int g = 0; g < G; g++)
+    { DevTable *D = s->d+g;
+      int64_t   direct = 0, room;
+      uint64_t  n_cand = 0;
+      if (D->deg != NULL)    direct += (s->n+4) & ~3ll;                /* the direct passes' buffers, if held */
+      if (D->up != NULL)     direct += (int64_t) (s->idx64 ? 8 : 4)*(D->hi-D->lo+1);
+      if (D->filter != NULL) direct += 4*hm_filter_words(s->fpos);
+      if (D->p2scratch != NULL) direct += D->p2scratch_bytes;
+      room = s->budget - held - direct;
+      if (room < HM_EXTRACT_MIN_BYTES)
+        return hm_set_error(HM_ENOMEM,"listing k-mer pairs needs at least %lld device bytes beside the scan's %lld on "
+                            "GPU %d, but the device budget of %lld bytes leaves %lld",(long long) HM_EXTRACT_MIN_BYTES,
+                            (long long) (held+direct),D->dev,(long long) s->budget,(long long) (room > 0 ? room : 0));
+      HM_CUDA(cudaSetDevice(D->dev));
+      if ((rc = hm_symm_status(D->symm_work,&D->symm_layout,&n_cand,NULL,D->st)) != HM_OK)
+        return rc;
+      nc[g] = (int64_t) n_cand < D->symm_layout.cand_cap ? (int64_t) n_cand : D->symm_layout.cand_cap;
+      int64_t recs = (room - 2*(int64_t) HM_PLOT_CELLS - 256) / (int64_t) sizeof(hm_pair_rec);
+      if (recs > 2*nc[g]) recs = 2*nc[g];
+      slice[g] = recs/2 > 0 ? recs/2 : 1;
+      c0[g] = 0;
+    }
+  hm_pair_rec *d_out[HM_MAX_GPUS], *host = NULL;
+  uint16_t    *d_pix[HM_MAX_GPUS];
+  unsigned long long *d_cnt[HM_MAX_GPUS];
+  int64_t      total = 0, hcap = 0;
+  memset(d_out,0,sizeof(d_out)); memset(d_pix,0,sizeof(d_pix)); memset(d_cnt,0,sizeof(d_cnt));
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    { DevTable *D = s->d+g;
+      cudaError_t e;
+#define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
+      TRY(cudaSetDevice(D->dev));
+      TRY(dalloc(D->dev,D->st,(void **) &d_pix[g],sizeof(uint16_t)*HM_PLOT_CELLS));
+      TRY(dalloc(D->dev,D->st,(void **) &d_cnt[g],256));
+      TRY(dalloc(D->dev,D->st,(void **) &d_out[g],sizeof(hm_pair_rec)*(size_t) (2*slice[g])));
+      TRY(cudaMemcpyAsync(d_pix[g],pixmap,sizeof(uint16_t)*HM_PLOT_CELLS,cudaMemcpyHostToDevice,D->st));
+#undef TRY
+    }
+  for (int more = 1; more && rc == HM_OK; )
+    { int64_t c1[HM_MAX_GPUS];
+      more = 0;
+      for (int g = 0; g < G && rc == HM_OK; g++)             /* a slice on every GPU that has candidates left */
+        { DevTable *D = s->d+g;
+          c1[g] = c0[g] + slice[g] < nc[g] ? c0[g] + slice[g] : nc[g];
+          if (c0[g] >= nc[g])
+            continue;
+          cudaError_t e;
+          if ((e = cudaSetDevice(D->dev)) != cudaSuccess ||
+              (e = cudaMemsetAsync(d_cnt[g],0,sizeof(unsigned long long),D->st)) != cudaSuccess)
+            { rc = hm_cuda_fail(e,"extract slice"); break; }
+          rc = hm_k_symm_extract(D->keys,D->keys_lo,D->cnt,s->n,D->bucket,s->bits,s->idx64,s->kmer,D->symm_work,
+                                 &D->symm_layout,G > 1 ? &s->ssh[g] : NULL,d_pix[g],c0[g],c1[g],d_out[g],
+                                 2*slice[g],d_cnt[g],D->st);
+          s->launches += 1;
+          more = 1;
+        }
+      for (int g = 0; g < G && rc == HM_OK; g++)
+        { DevTable *D = s->d+g;
+          unsigned long long c = 0;
+          if (c0[g] >= nc[g])
+            continue;
+          cudaError_t e;
+          if ((e = cudaSetDevice(D->dev)) != cudaSuccess ||
+              (e = cudaMemcpyAsync(&c,d_cnt[g],sizeof(c),cudaMemcpyDeviceToHost,D->st)) != cudaSuccess ||
+              (e = cudaStreamSynchronize(D->st)) != cudaSuccess)
+            { rc = hm_cuda_fail(e,"extract_kernel"); break; }
+          if ((int64_t) c > 2*slice[g])
+            { rc = hm_set_error(HM_ECUDA,"extract_kernel listed %llu records for %lld candidates",c,
+                                (long long) (c1[g]-c0[g]));
+              break;
+            }
+          if (total + (int64_t) c > hcap)
+            { int64_t      nh = 2*hcap > total + (int64_t) c ? 2*hcap : total + (int64_t) c;
+              hm_pair_rec *h2 = (hm_pair_rec *) realloc(host,sizeof(hm_pair_rec)*(size_t) nh);
+              if (h2 == NULL)
+                { rc = hm_set_error(HM_ENOMEM,"out of host memory for %lld pair records",(long long) nh); break; }
+              host = h2; hcap = nh;
+            }
+          if (c > 0 && (e = cudaMemcpy(host+total,d_out[g],sizeof(hm_pair_rec)*(size_t) c,cudaMemcpyDeviceToHost))
+                       != cudaSuccess)
+            { rc = hm_cuda_fail(e,"cudaMemcpy(pair records)"); break; }
+          total += (int64_t) c;
+          c0[g] = c1[g];
+        }
+    }
+  *status = 0;
+  for (int g = 0; g < G; g++)
+    { DevTable *D = s->d+g;
+      uint64_t  st = 0;
+      cudaSetDevice(D->dev);
+      if (rc == HM_OK)
+        { rc = hm_symm_status(D->symm_work,&D->symm_layout,NULL,&st,D->st);
+          *status |= st;
+        }
+      dfree(D->dev,D->st,d_out[g]); dfree(D->dev,D->st,d_pix[g]); dfree(D->dev,D->st,d_cnt[g]);
+    }
+  if (rc == HM_OK && host == NULL && (host = (hm_pair_rec *) malloc(sizeof(hm_pair_rec))) == NULL)
+    rc = hm_set_error(HM_ENOMEM,"out of host memory");
+  if (rc != HM_OK)
+    { free(host); return rc; }
+  *out = host; *n_out = total;
+  return HM_OK;
+}
+
+/* extract_kmer_pairs' output as a list (PloidyList.c:425-450).  The route follows hm_scan_run_path(HM_PATH_AUTO)'s
+ * rule and HETMERS_PATH: the symmetric one lists the candidates of the last symmetric run (running one first if
+ * the work areas do not hold a clean one), the direct one the direct passes' results; a symmetric run that fails
+ * its own checks falls back to the direct route, as a run does.                                                */
+extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out)
+{ int rc = HM_OK, path = HM_PATH_AUTO;
+  if (s->streamed)
+    return hm_set_error(HM_EUNSUPPORTED,"listing k-mer pairs needs the direct passes' arrays, and this table does not "
+                                        "fit in device memory (budget %lld bytes)",(long long) s->budget);
+  if (s->invalid)
+    return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
+  const char *e = getenv("HETMERS_PATH");
+  if (e != NULL && strcmp(e,"direct") == 0) path = HM_PATH_DIRECT;
+  if (e != NULL && strcmp(e,"symm") == 0)   path = HM_PATH_SYMM;
+  if (path == HM_PATH_SYMM && (s->kmer < HM_SYMM_MIN_KMER || !s->symmetric))
+    return hm_set_error(HM_EINVAL,"the table is not strand-symmetric (or k < %d): the symmetric scan "
+                                  "would not give the reference's answer",HM_SYMM_MIN_KMER);
+  int symm = (path == HM_PATH_SYMM || (path == HM_PATH_AUTO && s->symmetric && s->kmer >= HM_SYMM_MIN_KMER));
+  hm_pair_rec *host = NULL;
+  int64_t      total = 0;
+  if (symm)
+    { uint64_t status = 0;
+      if (!s->symm_ready)
+        { int64_t *tmp = (int64_t *) malloc(sizeof(int64_t)*HM_PLOT_CELLS);
+          if (tmp == NULL)
+            return hm_set_error(HM_ENOMEM,"out of host memory");
+          rc = run_symm(s,tmp,NULL,&status);
+          free(tmp);
+          if (rc != HM_OK)
+            return rc;
+        }
+      if (status == 0)
+        { if ((rc = extract_symm(s,pixmap,&host,&total,&status)) != HM_OK)
+            return rc;
+          if (status != 0)
+            { free(host); host = NULL; total = 0; }
+        }
+      if (status != 0)                /* the fingerprint was fooled: the direct passes are always right */
+        { if (path == HM_PATH_SYMM)
+            return hm_set_error(HM_EINVAL,"symmetric scan failed its own checks (status %llu)",
+                                (unsigned long long) status);
+          s->symmetric = 0; s->symm_ready = 0;
+          symm = 0;
+        }
+    }
+  if (!symm && (rc = extract_direct(s,pixmap,&host,&total)) != HM_OK)
+    return rc;
+  sort_records(host,total);                                       /* deterministic order */
   *out = host; *n_out = total;
   return HM_OK;
 }

@@ -1511,6 +1511,216 @@ extern "C" int hm_k_symm_resolve(const uint64_t *d_keys, const uint64_t *d_keys_
   return HM_OK;
 }
 
+/* ------------------------------------------------------------------ pair listing -------- */
+
+/* extract_kmer_pairs' records of isolated candidates (warp-wide call; lab = the candidate's pixel label, 0 for
+ * lanes that list nothing).  A candidate (x < y, differing at p, bases bx < by, counts cx, cy) stands for the
+ * pair itself and, unless 2p = k-1, its mirror image (u, v) = (rc y, rc x) at p' = k-1-p with cu = cy, cv = cx
+ * -- a pair of its own that the direct passes find from u.  Each is listed as pass2_extract_kernel lists it: the
+ * member with the higher count (the lower one on a tie), the other member's base at the varying position.
+ * One atomic per warp on the counter, which counts every record, also those beyond cap.                    */
+template <int KW>
+__device__ __forceinline__ void list_pairs(uint64_t x, uint64_t xl, uint64_t meta, unsigned lab, int kmer,
+                                           hm_pair_rec *__restrict__ out, unsigned long long cap,
+                                           unsigned long long *__restrict__ count, int lane, unsigned lt)
+{ const int      cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
+  const int      p  = (int) ((meta >> 32) & 0xff), by = (int) ((meta >> 40) & 3);
+  const int      nr = lab == 0 ? 0 : (2*p == kmer-1 ? 1 : 2);
+  const unsigned b1 = __ballot_sync(0xffffffffu,nr >= 1), b2 = __ballot_sync(0xffffffffu,nr == 2);
+  if (b1 == 0)
+    return;
+  unsigned long long at = 0;
+  if (lane == 0)
+    at = atomicAdd(count,(unsigned long long) (__popc(b1)+__popc(b2)));
+  at = __shfl_sync(0xffffffffu,at,0) + (unsigned long long) (__popc(b1 & lt)+__popc(b2 & lt));
+  if (nr == 0)
+    return;
+  const int bx = base_at<KW>(x,xl,p);
+  hm_pair_rec r;
+  r.smudge = lab; r.pad = 0;
+  r.pos = (uint8_t) p;
+  if (cx < cy)                                             /* y, alt bx */
+    { uint64_t y = x, yl = xl;
+      set_base<KW>(y,yl,p,by);
+      r.key_hi = y; r.key_lo = yl; r.alt = (uint8_t) bx;
+    }
+  else                                                     /* x, alt by */
+    { r.key_hi = x; r.key_lo = xl; r.alt = (uint8_t) by; }
+  if (at < cap)
+    out[at] = r;
+  if (nr == 2)
+    { const int q = kmer-1-p;
+      uint64_t  rx, rxl;
+      revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
+      r.pos = (uint8_t) q;
+      if (cy < cx)                                         /* v = rc x, alt = u's base 3-by */
+        { r.key_hi = rx; r.key_lo = rxl; r.alt = (uint8_t) (3-by); }
+      else                                                 /* u = rc y, alt = v's base 3-bx */
+        { set_base<KW>(rx,rxl,q,3-by);
+          r.key_hi = rx; r.key_lo = rxl; r.alt = (uint8_t) (3-bx);
+        }
+      if (at+1 < cap)
+        out[at+1] = r;
+    }
+}
+
+#define EX_THREADS 512              /* k <= 32: 2 CTAs per SM (64 registers); k > 32 spilled at 64 registers: 1 CTA */
+#define EX_ILP     RV_ILP
+#define EX_QCAP    (32*(EX_ILP+1))
+
+/* extract_kmer_pairs on the symmetric scan's work area: resolve_kernel (SL = false) over the candidates
+ * [c0, c1) of the last run, with the same Bloom-first structure and per-warp queue of hits settled by
+ * isolated_after_all, but an isolated candidate whose pixel carries a label is listed (list_pairs) instead
+ * of counted.  No plot tile: shared memory holds only the queues.                                        */
+template <typename IdxT, int KW>
+__global__ void __launch_bounds__(EX_THREADS,KW == 1 ? 2 : 1)
+extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+               const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
+               int kmer, const SymmView W, const uint16_t *__restrict__ pixmap, int64_t c0, int64_t c1,
+               hm_pair_rec *__restrict__ out, unsigned long long cap, unsigned long long *__restrict__ count)
+{ extern __shared__ __align__(16) uint64_t rv_smem[];
+  const unsigned FULL = 0xffffffffu;
+  const int      lane = threadIdx.x & 31;
+  const unsigned lt   = (1u << lane) - 1;
+  uint64_t *qk = rv_smem + (threadIdx.x >> 5)*EX_QCAP*(KW+1);      /* this warp's queue */
+  uint64_t *ql = qk + (KW == 2 ? EX_QCAP : 0);
+  uint64_t *qm = qk + KW*EX_QCAP;
+  int       qn = 0;
+  unsigned long long ncl = *W.cand_n;
+  if (ncl > W.cand_cap) ncl = W.cand_cap;
+  const int64_t nc     = (int64_t) ncl < c1 ? (int64_t) ncl : c1;
+  const int64_t stride = (int64_t) gridDim.x * blockDim.x;
+  const int64_t first  = c0 + (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t it = 0; first-lane + (int64_t) it*EX_ILP*stride < nc; it++)
+    { uint64_t x[EX_ILP], xl[EX_ILP], meta[EX_ILP];
+      uint32_t *wa[EX_ILP], *wb[EX_ILP], ba[EX_ILP], bb[EX_ILP], va[EX_ILP], vb[EX_ILP];
+      bool     ok[EX_ILP];
+#pragma unroll
+      for (int u = 0; u < EX_ILP; u++)
+        { const int64_t i = first + ((int64_t) it*EX_ILP+u)*stride;
+          ok[u] = (i < nc);
+          x[u] = 0; xl[u] = 0; meta[u] = 0;
+          if (ok[u])
+            { x[u] = ld_stream(W.cand_key+i);
+              if (KW == 2) xl[u] = ld_stream(W.cand_lo+i);
+              meta[u] = ld_stream(W.cand_meta+i);
+            }
+        }
+#pragma unroll
+      for (int u = 0; u < EX_ILP; u++)
+        { const int p  = (int) ((meta[u] >> 32) & 0xff), yb = (int) ((meta[u] >> 40) & 3);
+          uint64_t rx, rxl, ry, ryl;
+          revcomp_kmer<KW>(x[u],xl[u],kmer,rx,rxl);
+          ry = rx; ryl = rxl;
+          set_base<KW>(ry,ryl,kmer-1-p,3-yb);
+          bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,rx) : 0,kmer,rx,rxl,wa[u],ba[u]);
+          bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,ry) : 0,kmer,ry,ryl,wb[u],bb[u]);
+        }
+#pragma unroll
+      for (int u = 0; u < EX_ILP; u++)
+        { va[u] = 0; vb[u] = 0;
+          if (ok[u])
+            { va[u] = ld_keep(wa[u]);
+              vb[u] = (wb[u] == wa[u]) ? va[u] : ld_keep(wb[u]);
+            }
+        }
+#pragma unroll
+      for (int u = 0; u < EX_ILP; u++)
+        { const bool ha = (va[u] & ba[u]) == ba[u], hb = (vb[u] & bb[u]) == bb[u];
+          const bool hit = ok[u] && (ha || hb);
+          unsigned   lab = 0;
+          if (ok[u] && !hit)
+            { const int cx = (int) (meta[u] & 0xffff), cy = (int) ((meta[u] >> 16) & 0xffff);
+              lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
+            }
+          list_pairs<KW>(x[u],xl[u],meta[u],lab,kmer,out,cap,count,lane,lt);
+          const unsigned bal = __ballot_sync(FULL,hit);
+          if (hit)
+            { const int at = qn + __popc(bal & lt);
+              qk[at] = x[u];
+              if (KW == 2) ql[at] = xl[u];
+              qm[at] = meta[u] | (ha ? RV_HA : 0) | (hb ? RV_HB : 0);
+            }
+          qn += __popc(bal);
+        }
+      __syncwarp();
+      while (qn >= 32)                 /* (the key is read from the queue again to list it: fewer live registers) */
+        { qn -= 32;
+          const uint64_t mm = qm[qn+lane];
+          unsigned lab = 0;
+          if (isolated_after_all<IdxT,KW,false>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,qk[qn+lane],
+                                                KW == 2 ? ql[qn+lane] : 0,mm))
+            { const int cx = (int) (mm & 0xffff), cy = (int) ((mm >> 16) & 0xffff);
+              lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
+            }
+          list_pairs<KW>(qk[qn+lane],KW == 2 ? ql[qn+lane] : 0,mm,lab,kmer,out,cap,count,lane,lt);
+          __syncwarp();
+        }
+    }
+  uint64_t xx = 0, xxl = 0, mm = 0;
+  unsigned lab = 0;
+  if (lane < qn)
+    { xx = qk[lane]; xxl = KW == 2 ? ql[lane] : 0; mm = qm[lane];
+      if (isolated_after_all<IdxT,KW,false>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
+        { const int cx = (int) (mm & 0xffff), cy = (int) ((mm >> 16) & 0xffff);
+          lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
+        }
+    }
+  list_pairs<KW>(xx,xxl,mm,lab,kmer,out,cap,count,lane,lt);
+}
+
+template <typename IdxT, int KW>
+static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
+                                  const void *bucket, int bits, int kmer, const SymmView &W,
+                                  const uint16_t *pixmap, int64_t c0, int64_t c1, hm_pair_rec *out,
+                                  int64_t cap, unsigned long long *count, cudaStream_t st)
+{ static int per_sm[64] = {0};                                /* per instantiation */
+  size_t smem = (size_t) (EX_THREADS/32)*EX_QCAP*8*(KW+1);       /* 24 KB / 36 KB */
+  int dev = 0, sms = 132, occ = 1;
+  cudaGetDevice(&dev);
+  if (dev >= 64 || per_sm[dev] == 0)                           /* one wave of resident CTAs */
+    { cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ,extract_kernel<IdxT,KW>,EX_THREADS,smem);
+      if (e != cudaSuccess) return e;
+      if (occ < 1) occ = 1;
+      if (dev < 64) per_sm[dev] = occ;
+    }
+  else
+    occ = per_sm[dev];
+  cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
+  int64_t want = (c1-c0+EX_THREADS*EX_ILP-1)/(EX_THREADS*EX_ILP);
+  int     grid = (int) (want < sms*occ ? (want > 0 ? want : 1) : sms*occ);
+  extract_kernel<IdxT,KW><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,
+                                                       pixmap,c0,c1,out,(unsigned long long) cap,count);
+  return cudaGetLastError();
+}
+
+extern "C" int hm_k_symm_extract(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
+                                 const void *d_bucket, int bits, int idx64, int kmer,
+                                 void *d_work, const hm_symm_layout *layout, const hm_symm_shards *shards,
+                                 const uint16_t *d_pixmap, int64_t c0, int64_t c1, hm_pair_rec *d_out, int64_t cap,
+                                 unsigned long long *d_count, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || d_work == NULL || layout == NULL || d_pixmap == NULL ||
+      d_count == NULL || c0 < 0 || c1 < c0 || cap < 0 || (cap > 0 && d_out == NULL))
+    return hm_set_error(HM_EINVAL,"symm_extract: bad arguments");
+  if ((kmer > 32) != (d_keys_lo != NULL))
+    return hm_set_error(HM_EINVAL,"symm_extract: second key word array %s for k=%d",
+                        d_keys_lo ? "given" : "missing",kmer);
+  if (c1 == c0)
+    return HM_OK;
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = make_view(d_work,layout,shards);
+  cudaError_t e;
+  if (kmer <= 32)
+    e = idx64 ? launch_extract<uint64_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
+              : launch_extract<uint32_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
+  else
+    e = idx64 ? launch_extract<uint64_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
+              : launch_extract<uint32_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"extract_kernel");
+  return HM_OK;
+}
+
 /* candidate count + status word of the last runscan/resolve on this work area (synchronises) */
 extern "C" int hm_symm_status(const void *d_work, const hm_symm_layout *layout, uint64_t *n_cand,
                               uint64_t *status, void *stream)

@@ -201,6 +201,21 @@ class DeviceTable:
                                                 _ptr(self.plot), _stream()))
         self.launches += 1
 
+    def extract(self, pixmap: torch.Tensor, out: torch.Tensor, count: torch.Tensor, c0: int = 0, c1: int | None = None):
+        """extract_kmer_pairs from the symmetric scan's work area (after runscan()): the isolated pairs among
+        candidates [c0, c1) whose pixel has a label in pixmap (int16[1001*501], device) are appended to `out`
+        (uint8[cap * 24] device tensor of hm_pair_rec) and counted in count (int64[1], zeroed by the caller;
+        it counts every record, also those beyond cap).  At most two records per candidate."""
+        import ctypes as C
+        c1 = self.symm_layout.cand_cap if c1 is None else c1
+        cap = out.numel() // C.sizeof(_lib.PairRec)
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.hm_k_symm_extract(_ptr(self.keys), _ptr(self.keys_lo), _ptr(self.cnt), self.n,
+                                                _ptr(self.bucket), self.bits, self.idx64, self.kmer,
+                                                _ptr(self.symm_work), C.byref(self.symm_layout), self._symm_shards(),
+                                                _ptr(pixmap), int(c0), int(c1), _ptr(out), cap, _ptr(count), _stream()))
+        self.launches += 1
+
     def symm_status(self):
         """(candidate pairs, status bits) of the last symmetric scan; synchronises"""
         import ctypes as C

@@ -153,8 +153,10 @@ class Scan:
         return plot.reshape(_lib.SMAX + 1, _lib.PLOT_W), st.as_dict()
 
     def extract(self, pixmap: np.ndarray):
-        """pair list of extract_kmer_pairs (after run()): pixmap uint16[1001,501], label 0 = none;
-        -> structured array (key_hi, key_lo, smudge, pos, alt) sorted by (smudge, k-mer)"""
+        """pair list of extract_kmer_pairs: pixmap uint16[1001,501], label 0 = none;
+        -> structured array (key_hi, key_lo, smudge, pos, alt) sorted by (smudge, k-mer).  Takes the route
+        run() takes: on a symmetric table the pairs are listed from the last symmetric run's candidates (a run is
+        done first if there is none), else from the direct passes; HETMERS_PATH=direct|symm forces one."""
         pm = np.ascontiguousarray(pixmap, dtype=np.uint16).reshape(-1)
         assert pm.size == _lib.PLOT_CELLS
         out = C.POINTER(_lib.PairRec)()
