@@ -137,11 +137,13 @@ struct Scratch
     void free_now(void *q) { if (q != NULL) { release(q); cudaFree(q); } }
   };
 
-/* Replace (*pk, *pl, *pc, *pn) by the conditioned table (new cudaMalloc'ed arrays with one spare
- * element).  *pl is NULL for k <= 32.  The caller's arrays are freed and replaced only when the whole
- * call has succeeded; on any failure they are untouched and every temporary is released.        */
+/* Replace (*pk, *pl, *pc, *pn) by the conditioned table: new cudaMalloc'ed arrays of *pcap entries
+ * each (at least one spare: they are sized before the duplicates or the trimmed entries go).  *pl is
+ * NULL for k <= 32.  The pointers are replaced only when the whole call has succeeded and produced a
+ * new table; the caller's arrays are never freed here, and on any failure every temporary is
+ * released.                                                                                      */
 int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
-                        uint64_t **pk, uint64_t **pl, uint16_t **pc, int64_t *pn, cudaStream_t st)
+                        uint64_t **pk, uint64_t **pl, uint16_t **pc, int64_t *pn, int64_t *pcap, cudaStream_t st)
 { int64_t   n = *pn;
   const int two = (*pl != NULL);
   Scratch   S;
@@ -154,6 +156,7 @@ int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
   uint64_t *ck = *pk, *cl = *pl;
   uint16_t *cc = *pc;
   int       own = 0;
+  int64_t   cap = 0;                           /* entries each array of ours holds */
 
   if (do_symm && two && 2*n >= 0xFFFFFFF0ll)   /* before anything is allocated or touched */
     return hm_set_error(HM_EUNSUPPORTED,"symmetrising %lld entries of k=%d needs 64-bit sort indices",
@@ -175,7 +178,7 @@ int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
       CK(cudaMemcpyAsync(&nsel,d_nsel,sizeof(int64_t),cudaMemcpyDeviceToHost,st));
       CK(cudaStreamSynchronize(st));
       S.free_now(flag); flag = NULL;
-      ck = k2; cc = c2; cl = l2; n = nsel; own = 1;
+      ck = k2; cc = c2; cl = l2; cap = n+1; n = nsel; own = 1;
     }
 
   if (do_symm && n > 0)
@@ -226,17 +229,16 @@ int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
       RC(select_flagged(c1,flag,c0,m,d_nsel,&tmp,&tmp_bytes,st));
       CK(cudaMemcpyAsync(&nsel,d_nsel,sizeof(int64_t),cudaMemcpyDeviceToHost,st));
       CK(cudaStreamSynchronize(st));
-      ck = h0; cc = c0; cl = l0; n = nsel; own = 1;
+      ck = h0; cc = c0; cl = l0; cap = m+1; n = nsel; own = 1;
     }
 
   CK(cudaStreamSynchronize(st));
 #undef CK
 #undef RC
   if (tmp) cudaFree(tmp);
-  if (own)                                           /* success: swap the new table in */
+  if (own)                                           /* success: hand the new table over */
     { S.release(ck); S.release(cc); if (cl) S.release(cl);
-      cudaFree(*pk); cudaFree(*pc); if (*pl) cudaFree(*pl);
-      *pk = ck; *pc = cc; *pl = cl;
+      *pk = ck; *pc = cc; *pl = cl; *pcap = cap;
     }
   *pn = n;
   return HM_OK;

@@ -53,7 +53,11 @@ typedef struct
     hm_symm_layout      symm_layout;
     int64_t             slo, shi;     /* its run-aligned range */
     uint64_t           *fp_acc;       /* device uint64[4]: symmetry fingerprint sums of the entries loaded here */
-    int64_t             held, peak, chunks;   /* (streamed) this shard's device bytes now / at most; chunks of the last run */
+    cudaEvent_t         ev[4];        /* a run's pass 1 from ev[0] to ev[1], pass 2 from ev[2] to ev[3] */
+    int                 pool;         /* allocations come from the device's stream-ordered pool */
+    struct DevBlock    *blocks;       /* every device allocation held (dev_alloc) */
+    int64_t             held, peak, chunks;   /* device bytes now / at most (streamed: since the last run began);
+                                                 (streamed) chunks of the last run */
   } DevTable;
 
 struct hm_scan
@@ -96,67 +100,157 @@ int hm_peer_sum_deg(uint8_t **deg, const int64_t *lo, const int64_t *hi, const i
 int hm_peer_sum_plot(unsigned long long **plot, const int *dev, cudaStream_t *st, int n);
 /* GPU trim / symmetrise (hm_condition.cu) */
 int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
-                        uint64_t **pk, uint64_t **pl, uint16_t **pc, int64_t *pn, cudaStream_t st);
+                        uint64_t **pk, uint64_t **pl, uint16_t **pc, int64_t *pn, int64_t *pcap, cudaStream_t st);
 
-/* Device allocations of a one-GPU scan come from the device's stream-ordered memory pool with a
- * release threshold of "never": a second hm_scan_create in the same process (bench e2e leg, a
- * service handling many tables) reuses the memory instead of paying cudaMalloc / cudaFree of
- * several GB every call.  Multi-GPU scans keep cudaMalloc:
- * their arrays are mapped by the peers.  HETMERS_NO_POOL=1 disables the pool.                  */
-#define POOL_MAX 32
-typedef struct { void *p[POOL_MAX]; int n, enabled; } PoolReg;
-static PoolReg g_pool[64];
+/* rc = the first failure of a sequence of CUDA calls (needs cudaError_t e and int rc in scope) */
+#define TRY(call) do { if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call); } while (0)
 
-static void pool_setup(int dev, int enable)
+/* Every device allocation of a DevTable goes through dev_alloc / dev_free, which keep its size in D->held and
+ * D->peak.  Allocations of a one-GPU scan come from the device's stream-ordered memory pool with a release
+ * threshold of "never": a second hm_scan_create in the same process (bench e2e leg, a service handling many
+ * tables) reuses the memory instead of paying cudaMalloc / cudaFree of several GB every call.  Multi-GPU scans
+ * keep cudaMalloc: their arrays are mapped by the peers.  HETMERS_NO_POOL=1 disables the pool.               */
+typedef struct DevBlock { void *p; int64_t bytes; int pooled; struct DevBlock *next; } DevBlock;
+
+/* whether D's allocations may come from the pool */
+static int pool_setup(int dev, int enable)
 { static int configured[64] = {0};
-  if (dev < 0 || dev >= 64) return;
-  g_pool[dev].enabled = enable && getenv("HETMERS_NO_POOL") == NULL;
-  if (g_pool[dev].enabled && !configured[dev])
+  if (!enable || dev < 0 || dev >= 64 || getenv("HETMERS_NO_POOL") != NULL)
+    return 0;
+  if (configured[dev] == 0)
     { cudaMemPool_t pool;
       unsigned long long never = ~0ull;
+      configured[dev] = 1;
       if (cudaDeviceGetDefaultMemPool(&pool,dev) != cudaSuccess ||
           cudaMemPoolSetAttribute(pool,cudaMemPoolAttrReleaseThreshold,&never) != cudaSuccess)
-        { cudaGetLastError(); g_pool[dev].enabled = 0; }
-      configured[dev] = 1;
+        { cudaGetLastError(); configured[dev] = -1; }
     }
+  return configured[dev] == 1;
 }
 
-static cudaError_t dalloc(int dev, cudaStream_t st, void **p, size_t bytes)
-{ PoolReg *R = (dev >= 0 && dev < 64) ? g_pool+dev : NULL;
-  if (R != NULL && R->enabled && R->n < POOL_MAX)
-    { cudaError_t e = cudaMallocAsync(p,bytes,st);
-      if (e == cudaSuccess)
-        { R->p[R->n++] = *p; return e; }
-      cudaGetLastError();
-    }
-  return cudaMalloc(p,bytes);
+static void dev_release(DevTable *D, void *p, int pooled)
+{ if (pooled) cudaFreeAsync(p,D->st);
+  else        cudaFree(p);
 }
 
-static void dfree(int dev, cudaStream_t st, void *p)
-{ PoolReg *R = (dev >= 0 && dev < 64) ? g_pool+dev : NULL;
-  if (p == NULL) return;
-  if (R != NULL)
-    for (int k = 0; k < R->n; k++)
-      if (R->p[k] == p)
-        { R->p[k] = R->p[--R->n];
-          cudaFreeAsync(p,st);
-          return;
-        }
-  cudaFree(p);
+/* counts device memory p of `bytes` as D's; if it cannot (out of host memory), frees p and fails */
+static cudaError_t dev_track(DevTable *D, void *p, int64_t bytes, int pooled)
+{ DevBlock *b = (DevBlock *) malloc(sizeof(DevBlock));
+  if (b == NULL)
+    { dev_release(D,p,pooled);
+      return cudaErrorMemoryAllocation;
+    }
+  b->p = p; b->bytes = bytes; b->pooled = pooled; b->next = D->blocks;
+  D->blocks = b;
+  D->held += bytes;
+  if (D->held > D->peak) D->peak = D->held;
+  return cudaSuccess;
+}
+
+/* *pp = `bytes` of device memory on D's device (current), stream-ordered on D->st when pooled */
+static cudaError_t dev_alloc(DevTable *D, void *pp, int64_t bytes)
+{ void      **p = (void **) pp;
+  cudaError_t e = cudaErrorMemoryAllocation;
+  int         pooled = 0;
+  if (D->pool)
+    { if ((e = cudaMallocAsync(p,(size_t) bytes,D->st)) == cudaSuccess) pooled = 1;
+      else                                                               cudaGetLastError();
+    }
+  if (!pooled && (e = cudaMalloc(p,(size_t) bytes)) != cudaSuccess)
+    return e;
+  if ((e = dev_track(D,*p,bytes,pooled)) != cudaSuccess)
+    *p = NULL;
+  return e;
+}
+
+static void dev_unlink(DevTable *D, DevBlock **at)
+{ DevBlock *b = *at;
+  *at = b->next;
+  dev_release(D,b->p,b->pooled);
+  D->held -= b->bytes;
+  free(b);
+}
+
+/* frees what dev_alloc (or dev_track) gave; NULL is ignored */
+static void dev_free(DevTable *D, void *p)
+{ for (DevBlock **at = &D->blocks; p != NULL && *at != NULL; at = &(*at)->next)
+    if ((*at)->p == p)
+      { dev_unlink(D,at);
+        return;
+      }
 }
 
 static void free_dev(DevTable *D)
 { cudaSetDevice(D->dev);
-  dfree(D->dev,D->st,D->keys);  dfree(D->dev,D->st,D->keys_lo); dfree(D->dev,D->st,D->cnt);
-  dfree(D->dev,D->st,D->deg);   dfree(D->dev,D->st,D->bucket);  dfree(D->dev,D->st,D->filter);
-  dfree(D->dev,D->st,D->up);    dfree(D->dev,D->st,D->plot);
-  dfree(D->dev,D->st,D->fp_acc);
-  if (D->p2scratch) cudaFree(D->p2scratch);
-  dfree(D->dev,D->st,D->symm_work);
+  while (D->blocks != NULL)
+    dev_unlink(D,&D->blocks);
   if (D->st) cudaStreamSynchronize(D->st);
   if (D->st)      cudaStreamDestroy(D->st);
   if (D->st_copy) cudaStreamDestroy(D->st_copy);
+  for (int k = 0; k < 4; k++)
+    if (D->ev[k]) cudaEventDestroy(D->ev[k]);
   memset(D,0,sizeof(*D));
+}
+
+/* set each GPU's device and synchronise its stream; the first error */
+static int sync_all(hm_scan *s, const char *what)
+{ int rc = HM_OK;
+  for (int g = 0; g < s->ngpu; g++)
+    { cudaError_t e = cudaSetDevice(s->d[g].dev);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(s->d[g].st);
+      if (e != cudaSuccess && rc == HM_OK) rc = hm_cuda_fail(e,what);
+    }
+  return rc;
+}
+
+/* the slowest GPU's time from its event a to its event b */
+static float slowest_ms(hm_scan *s, int a, int b)
+{ float worst = 0;
+  for (int g = 0; g < s->ngpu; g++)
+    { float ms = 0;
+      cudaSetDevice(s->d[g].dev);
+      if (cudaEventElapsedTime(&ms,s->d[g].ev[a],s->d[g].ev[b]) == cudaSuccess && ms > worst) worst = ms;
+    }
+  cudaGetLastError();
+  return worst;
+}
+
+/* fn(s, g, arg) for every GPU g at once, a host thread each (the calling thread takes the last).  A failure sets
+ * s->stop, which the shards of a streamed run watch; the first failing GPU's error wins, naming its shard when
+ * there are several                                                                                            */
+typedef int (*GpuFn)(hm_scan *s, int g, void *arg);
+typedef struct { hm_scan *s; int g; GpuFn fn; void *arg; int rc; char msg[512]; } GpuJob;
+
+static void *gpu_worker(void *p)
+{ GpuJob *J = (GpuJob *) p;
+  J->rc = J->fn(J->s,J->g,J->arg);
+  if (J->rc != HM_OK)
+    { J->s->stop = 1;
+      strncpy(J->msg,hm_last_error(),sizeof(J->msg)-1); J->msg[sizeof(J->msg)-1] = 0;
+    }
+  return NULL;
+}
+
+static int on_every_gpu(hm_scan *s, GpuFn fn, void *arg)
+{ int       G = s->ngpu, rc = HM_OK;
+  GpuJob    job[HM_MAX_GPUS];
+  pthread_t th[HM_MAX_GPUS];
+  int       created[HM_MAX_GPUS];
+  for (int g = 0; g < G; g++)
+    { memset(job+g,0,sizeof(job[g]));
+      job[g].s = s; job[g].g = g; job[g].fn = fn; job[g].arg = arg;
+      created[g] = (g < G-1 && pthread_create(th+g,NULL,gpu_worker,job+g) == 0);
+      if (!created[g])
+        gpu_worker(job+g);
+    }
+  for (int g = 0; g < G; g++)
+    { if (created[g]) pthread_join(th[g],NULL);
+      if (job[g].rc != HM_OK && rc == HM_OK)
+        rc = G == 1 ? hm_set_error(job[g].rc,"%s",job[g].msg)
+                    : hm_set_error(job[g].rc,"shard %d of %d (GPU %d, entries %lld..%lld): %s",g,G,s->d[g].dev,
+                                   (long long) s->d[g].lo,(long long) s->d[g].hi,job[g].msg);
+    }
+  return rc;
 }
 
 extern "C" void hm_scan_destroy(hm_scan *s)
@@ -302,7 +396,6 @@ typedef struct
     int         pin_cached[2], staged, used[2], b;
     cudaEvent_t copied[2], unpacked[2];
     int64_t     chunk;                /* records per H2D copy */
-    int64_t     bytes;                /* device bytes of the staging buffers */
   } Stager;
 
 static int stager_open(hm_scan *s, DevTable *D, const hm_host_table *t, int64_t count, Stager *G)
@@ -318,8 +411,7 @@ static int stager_open(hm_scan *s, DevTable *D, const hm_host_table *t, int64_t 
     G->chunk = LOAD_CHUNK/2;
   if (G->chunk > count) G->chunk = count;
   for (int i = 0; i < 2; i++)
-    { HM_CUDA(dalloc(D->dev,D->st,(void **) &G->stage[i],(size_t) G->chunk*pbyte));
-      G->bytes += G->chunk*pbyte;
+    { HM_CUDA(dev_alloc(D,&G->stage[i],G->chunk*pbyte));
       if (G->staged)
         { if (s->ngpu == 1 && g_pin_cache[i] != NULL && (size_t) G->chunk*pbyte <= PIN_CACHE_BYTES)
             { G->pin[i] = g_pin_cache[i]; g_pin_cache[i] = NULL; G->pin_cached[i] = 1; }   /* from hm_prewarm */
@@ -335,7 +427,7 @@ static int stager_open(hm_scan *s, DevTable *D, const hm_host_table *t, int64_t 
 
 static void stager_close(DevTable *D, Stager *G)
 { for (int i = 0; i < 2; i++)
-    { if (G->stage[i] != NULL) dfree(D->dev,D->st,G->stage[i]);
+    { dev_free(D,G->stage[i]);
       if (G->copied[i] != NULL)   cudaEventDestroy(G->copied[i]);
       if (G->unpacked[i] != NULL) cudaEventDestroy(G->unpacked[i]);
       if (G->pin[i] != NULL)
@@ -432,29 +524,20 @@ static int load_range(hm_scan *s, DevTable *D, const hm_host_table *t, const int
   return rc;
 }
 
-/* one host thread per device: stub index upload + this device's shard of the records */
-typedef struct { hm_scan *s; int g; const hm_host_table *t; int rc; char msg[512]; } LoadJob;
-
-static void *load_worker(void *arg)
-{ LoadJob  *J = (LoadJob *) arg;
-  hm_scan  *s = J->s;
-  DevTable *D = s->d+J->g;
+/* on_every_gpu: stub index upload + this device's shard of the records of table t */
+static int load_shard(hm_scan *s, int g, void *t)
+{ const hm_host_table *T = (const hm_host_table *) t;
+  DevTable *D = s->d+g;
   int64_t  *d_index = NULL;
-  int64_t   ixlen = (int64_t) 1 << (8*J->t->ibyte);
-  J->rc = HM_OK;
+  int64_t   ixlen = (int64_t) 1 << (8*T->ibyte);
   cudaError_t e = cudaSetDevice(D->dev);
-  if (e == cudaSuccess) e = dalloc(D->dev,D->st,(void **) &d_index,sizeof(int64_t)*ixlen);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_index,J->t->index,sizeof(int64_t)*ixlen,cudaMemcpyHostToDevice,D->st);
+  if (e == cudaSuccess) e = dev_alloc(D,&d_index,sizeof(int64_t)*ixlen);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_index,T->index,sizeof(int64_t)*ixlen,cudaMemcpyHostToDevice,D->st);
   if (e == cudaSuccess) e = cudaMemsetAsync(D->fp_acc,0,4*sizeof(uint64_t),D->st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(D->st);     /* pool memory is about to be used on the copy stream too */
-  if (e != cudaSuccess)
-    J->rc = hm_cuda_fail(e,"stub index upload");
-  else
-    J->rc = load_range(s,D,J->t,d_index,D->lo,D->hi-D->lo);
-  if (d_index != NULL) dfree(D->dev,D->st,d_index);
-  if (J->rc != HM_OK)
-    { strncpy(J->msg,hm_last_error(),sizeof(J->msg)-1); J->msg[sizeof(J->msg)-1] = 0; }
-  return NULL;
+  int rc = e != cudaSuccess ? hm_cuda_fail(e,"stub index upload") : load_range(s,D,T,d_index,D->lo,D->hi-D->lo);
+  dev_free(D,d_index);
+  return rc;
 }
 
 /* sum of the per-device fingerprint accumulators -> s->symmetric */
@@ -602,62 +685,70 @@ extern "C" int hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_
   return s->streamed;
 }
 
-/* streamed scans: device allocations counted against the shard's budget */
-static cudaError_t salloc(hm_scan *s, DevTable *D, void **p, int64_t bytes)
-{ cudaError_t e = dalloc(D->dev,D->st,p,(size_t) bytes);
-  (void) s;
-  if (e == cudaSuccess)
-    { D->held += bytes;
-      if (D->held > D->peak) D->peak = D->held;
-    }
-  return e;
+/* A window of `cap` entries onto the host table of a streamed scan, on the first GPU: keys, second words, counts,
+ * the stub index and a Stager.  Between runs: it leaves the peak the last run reported as it was.           */
+typedef struct { uint64_t *keys, *klo; uint16_t *cnt; int64_t *d_index; Stager G; int64_t peak; } Window;
+
+static void window_close(hm_scan *s, Window *W)
+{ DevTable *D = s->d;
+  stager_close(D,&W->G);
+  dev_free(D,W->keys); dev_free(D,W->klo); dev_free(D,W->cnt); dev_free(D,W->d_index);
+  D->peak = W->peak;
 }
 
-static void sfree(hm_scan *s, DevTable *D, void *p, int64_t bytes)
-{ (void) s;
-  if (p == NULL) return;
-  dfree(D->dev,D->st,p);
-  D->held -= bytes;
+static int window_open(hm_scan *s, int64_t cap, Window *W)
+{ DevTable *D = s->d;
+  int64_t   ixlen = (int64_t) 1 << (8*s->ibyte);
+  int       rc = HM_OK;
+  cudaError_t e;
+  memset(W,0,sizeof(*W));
+  W->peak = D->peak;
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&W->keys,8*(cap+1)));
+  if (s->kmer > 32) TRY(dev_alloc(D,&W->klo,8*(cap+1)));
+  TRY(dev_alloc(D,&W->cnt,2*(cap+8)));
+  TRY(dev_alloc(D,&W->d_index,8*ixlen));
+  TRY(cudaMemcpyAsync(W->d_index,s->host->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,D->st));
+  if (rc == HM_OK)
+    rc = stager_open(s,D,s->host,cap,&W->G);
+  if (rc != HM_OK)
+    window_close(s,W);
+  return rc;
 }
+
+/* ordinals [first, first+count) into the window */
+static int window_load(hm_scan *s, Window *W, int64_t first, int64_t count)
+{ return load_into(s,s->d,s->host,W->d_index,first,count,W->keys,W->klo,W->cnt,0,&W->G); }
 
 /* Shard cuts of a streamed scan over G = s->ngpu shards, from the host table: c_r is the first run start (a run =
  * the entries sharing their first k/2 bases) at or after n*r/G -- hm_symm_align_cut's rule -- found by loading
  * a few records at a time around each nominal cut on the first shard's device.  Sets every shard's range,
  * descriptor (first_key[r] = word 0 of entry c_r) and how many shards own keys: those up to the last non-empty
  * one (a run longer than a share can leave shards empty, in the middle or at the end).                   */
-static int stream_cuts(hm_scan *s, const hm_host_table *t)
-{ DevTable *D = s->d;
-  int      G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
-  int64_t  n = s->n, cut[HM_MAX_GPUS+1], ixlen = (int64_t) 1 << (8*s->ibyte);
+static int stream_cuts(hm_scan *s)
+{ int      G = s->ngpu, rc;
+  int64_t  n = s->n, cut[HM_MAX_GPUS+1];
   uint64_t first[HM_MAX_GPUS];
   const int64_t W = 4096;
   const int psh = 64-2*(s->kmer>>1);
-  uint64_t *keys = NULL, *klo = NULL, buf[4096];
-  uint16_t *cnt = NULL;
-  int64_t  *d_index = NULL;
-  Stager    SG;
-  memset(&SG,0,sizeof(SG));
-  HM_CUDA(cudaSetDevice(D->dev));
-  cudaError_t e = cudaMalloc(&keys,8*(size_t) (W+1));
-  if (e == cudaSuccess && KW == 2) e = cudaMalloc(&klo,8*(size_t) (W+1));
-  if (e == cudaSuccess) e = cudaMalloc(&cnt,2*(size_t) (W+8));
-  if (e == cudaSuccess) e = cudaMalloc(&d_index,8*(size_t) ixlen);
-  if (e == cudaSuccess) e = cudaMemcpy(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) rc = hm_cuda_fail(e,"streamed scan: shard cuts");
-  if (rc == HM_OK) rc = stager_open(s,D,t,W,&SG);
+  uint64_t buf[4096];
+  Window   win;
+  cudaError_t e;
+  if ((rc = window_open(s,W,&win)) != HM_OK)
+    return rc;
   cut[0] = 0; cut[G] = n; first[0] = 0;
   for (int r = 1; r < G && rc == HM_OK; r++)
     { int64_t  c = n*r/G;
       uint64_t prev;
       if (c <= cut[r-1])                                   /* the run before reaches past this share's start */
         { cut[r] = cut[r-1]; first[r] = first[r-1]; continue; }
-      if ((rc = load_into(s,D,t,d_index,c-1,1,keys,klo,cnt,0,&SG)) != HM_OK) break;
-      if ((e = cudaMemcpy(&prev,keys,8,cudaMemcpyDeviceToHost)) != cudaSuccess) { rc = hm_cuda_fail(e,"cut key"); break; }
+      if ((rc = window_load(s,&win,c-1,1)) != HM_OK) break;
+      if ((e = cudaMemcpy(&prev,win.keys,8,cudaMemcpyDeviceToHost)) != cudaSuccess) { rc = hm_cuda_fail(e,"cut key"); break; }
       cut[r] = n; first[r] = ~0ull;
       for (int64_t o = c; o < n && rc == HM_OK; o += W)
         { int64_t m = n-o < W ? n-o : W, i;
-          if ((rc = load_into(s,D,t,d_index,o,m,keys,klo,cnt,0,&SG)) != HM_OK) break;
-          if ((e = cudaMemcpy(buf,keys,8*(size_t) m,cudaMemcpyDeviceToHost)) != cudaSuccess)
+          if ((rc = window_load(s,&win,o,m)) != HM_OK) break;
+          if ((e = cudaMemcpy(buf,win.keys,8*(size_t) m,cudaMemcpyDeviceToHost)) != cudaSuccess)
             { rc = hm_cuda_fail(e,"cut keys"); break; }
           for (i = 0; i < m && ((buf[i] ^ prev) >> psh) == 0; i++)
             ;
@@ -665,8 +756,7 @@ static int stream_cuts(hm_scan *s, const hm_host_table *t)
             { cut[r] = o+i; first[r] = buf[i]; break; }
         }
     }
-  stager_close(D,&SG);
-  cudaFree(keys); cudaFree(klo); cudaFree(cnt); cudaFree(d_index);
+  window_close(s,&win);
   if (rc != HM_OK)
     return rc;
   int live = 1;                                            /* shards up to the last non-empty one */
@@ -725,24 +815,46 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
           s->plan.list_bytes = s->budget - s->plan.fixed_bytes - s->plan.chunk_bytes;
         }
       s->streamed = 1; s->host = t;
-      if (n_gpus > 1 && (rc = hm_peer_enable(dev,n_gpus)) != HM_OK)   /* pass 2 reads the owners' S lists */
-        { free(s); return rc; }
-      for (int g = 0; g < n_gpus && rc == HM_OK; g++)
-        { DevTable *D = s->d+g;
-          cudaError_t e;
-          D->dev = dev ? dev[g] : g;
-          D->lo = 0; D->hi = n;
-#define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
-          TRY(cudaSetDevice(D->dev));
-          pool_setup(D->dev,n_gpus == 1);                      /* several: the peers map the S lists */
-          TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
-          TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
-          TRY(salloc(s,D,(void **) &D->plot,8*(int64_t) HM_PLOT_CELLS));
-          TRY(salloc(s,D,(void **) &D->fp_acc,4*sizeof(uint64_t)));
-#undef TRY
+    }
+  else
+    for (int g = 0; g < n_gpus; g++)
+      for (int h = 0; h < g; h++)
+        if ((dev ? dev[g] : g) == (dev ? dev[h] : h))
+          { free(s);
+            return hm_set_error(HM_EINVAL,"GPU %d is listed twice: only a streamed scan can run several shards on one "
+                                "device",dev ? dev[g] : g);
+          }
+  /* several GPUs: the peers map the table arrays (in core) or read the owners' S lists (streamed) */
+  if (n_gpus > 1 && (rc = hm_peer_enable(dev,n_gpus)) != HM_OK)
+    { free(s); return rc; }
+
+  /* in core: table arrays + bucket index; the work buffers of either scan path are allocated by the path
+   * that runs (ensure_direct / ensure_symm)                                                              */
+  for (int g = 0; g < n_gpus && rc == HM_OK; g++)
+    { DevTable *D = s->d+g;
+      cudaError_t e;
+      D->dev = dev ? dev[g] : g;
+      D->lo  = s->streamed ? 0 : n*g/n_gpus;
+      D->hi  = s->streamed ? n : n*(g+1)/n_gpus;
+      TRY(cudaSetDevice(D->dev));
+      D->pool = pool_setup(D->dev,n_gpus == 1);
+      TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
+      TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
+      for (int k = 0; k < 4; k++)
+        TRY(cudaEventCreate(&D->ev[k]));
+      if (!s->streamed)
+        { TRY(dev_alloc(D,&D->keys,sizeof(uint64_t)*(n+1)));
+          if (t->kmer > 32)
+            TRY(dev_alloc(D,&D->keys_lo,sizeof(uint64_t)*(n+1)));
+          TRY(dev_alloc(D,&D->cnt,sizeof(uint16_t)*(n+8)));
+          TRY(dev_alloc(D,&D->bucket,(int64_t) ib*((1ll << s->bits)+1)));
         }
-      if (rc == HM_OK && n_gpus > 1 && t->kmer >= HM_SYMM_MIN_KMER)   /* (smaller k: refused by the run) */
-        rc = stream_cuts(s,t);
+      TRY(dev_alloc(D,&D->plot,sizeof(unsigned long long)*HM_PLOT_CELLS));
+      TRY(dev_alloc(D,&D->fp_acc,4*sizeof(uint64_t)));
+    }
+  if (s->streamed)
+    { if (rc == HM_OK && n_gpus > 1 && t->kmer >= HM_SYMM_MIN_KMER)   /* (smaller k: refused by the run) */
+        rc = stream_cuts(s);
       if (rc != HM_OK)
         { hm_scan_destroy(s); return rc; }
       s->ms_load = now_ms()-t0;
@@ -750,60 +862,11 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
       return HM_OK;
     }
 
-  for (int g = 0; g < n_gpus; g++)
-    for (int h = 0; h < g; h++)
-      if ((dev ? dev[g] : g) == (dev ? dev[h] : h))
-        { free(s);
-          return hm_set_error(HM_EINVAL,"GPU %d is listed twice: only a streamed scan can run several shards on one "
-                              "device",dev ? dev[g] : g);
-        }
-  if (n_gpus > 1 && (rc = hm_peer_enable(dev,n_gpus)) != HM_OK)
-    { free(s); return rc; }
-
-  /* table arrays + bucket index; the work buffers of either scan path are allocated by the path
-   * that runs (ensure_direct / ensure_symm)                                                     */
-  for (int g = 0; g < n_gpus && rc == HM_OK; g++)
-    { DevTable *D = s->d+g;
-      D->dev = dev ? dev[g] : g;
-      D->lo  = n*g/n_gpus;
-      D->hi  = n*(g+1)/n_gpus;
-      cudaError_t e;
-#define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
-      TRY(cudaSetDevice(D->dev));
-      pool_setup(D->dev,n_gpus == 1);
-      TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
-      TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
-      TRY(dalloc(D->dev,D->st,(void **) &D->keys,sizeof(uint64_t)*(size_t) (n+1)));
-      if (t->kmer > 32)
-        TRY(dalloc(D->dev,D->st,(void **) &D->keys_lo,sizeof(uint64_t)*(size_t) (n+1)));
-      TRY(dalloc(D->dev,D->st,(void **) &D->cnt,sizeof(uint16_t)*(size_t) (n+8)));
-      TRY(dalloc(D->dev,D->st,(void **) &D->bucket,ib*(((size_t) 1<<s->bits)+1)));
-      TRY(dalloc(D->dev,D->st,(void **) &D->plot,sizeof(unsigned long long)*HM_PLOT_CELLS));
-      TRY(dalloc(D->dev,D->st,(void **) &D->fp_acc,4*sizeof(uint64_t)));
-#undef TRY
-    }
-
   double t_alloc = now_ms();
   /* each device unpacks its own shard from the host -- all devices at once, one host thread each --
    * then the shards are exchanged over peer copies so that every device ends with the full table */
   if (rc == HM_OK)
-    { LoadJob   job[HM_MAX_GPUS];
-      pthread_t th[HM_MAX_GPUS];
-      int       created[HM_MAX_GPUS];
-      for (int g = 0; g < n_gpus; g++)
-        { job[g].s = s; job[g].g = g; job[g].t = t; job[g].rc = HM_OK; job[g].msg[0] = 0;
-          created[g] = 0;
-          if (g == n_gpus-1 || pthread_create(th+g,NULL,load_worker,job+g) != 0)
-            load_worker(job+g);                              /* the calling thread takes the last device */
-          else
-            created[g] = 1;
-        }
-      for (int g = 0; g < n_gpus; g++)
-        { if (created[g]) pthread_join(th[g],NULL);
-          if (job[g].rc != HM_OK && rc == HM_OK)
-            rc = hm_set_error(job[g].rc,"%s",job[g].msg);
-        }
-    }
+    rc = on_every_gpu(s,load_shard,(void *) t);
   double t_rec = now_ms();
   if (n_gpus > 1 && rc == HM_OK)
     { for (int g = 0; g < n_gpus && rc == HM_OK; g++)        /* all-gather by peer copies */
@@ -823,8 +886,8 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
                                         sizeof(uint16_t)*(size_t) m,D->st);
               if (e != cudaSuccess) rc = hm_cuda_fail(e,"cudaMemcpyPeerAsync(table shard)");
             }
-      for (int g = 0; g < n_gpus; g++)
-        { cudaSetDevice(s->d[g].dev); cudaStreamSynchronize(s->d[g].st); }
+      int rc2 = sync_all(s,"table shards");
+      if (rc == HM_OK) rc = rc2;
     }
   for (int g = 0; g < n_gpus && rc == HM_OK && n_gpus > 1; g++)     /* (one GPU: done chunk-wise) */
     { DevTable *D = s->d+g;
@@ -832,11 +895,8 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
       rc = hm_k_build_bucket_index(D->keys,n,s->bits,D->bucket,s->idx64,D->st);
       s->launches += 1;
     }
-  for (int g = 0; g < n_gpus; g++)
-    { cudaSetDevice(s->d[g].dev);
-      cudaError_t e = cudaStreamSynchronize(s->d[g].st);
-      if (rc == HM_OK && e != cudaSuccess) rc = hm_cuda_fail(e,"table load");
-    }
+  int rc2 = sync_all(s,"table load");
+  if (rc == HM_OK) rc = rc2;
   if (rc == HM_OK)
     rc = fingerprint_verdict(s);
   if (rc != HM_OK)
@@ -857,21 +917,16 @@ static int ensure_direct(hm_scan *s)
   for (int g = 0; g < s->ngpu && rc == HM_OK; g++)
     { DevTable *D = s->d+g;
       cudaError_t e;
-#define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
       TRY(cudaSetDevice(D->dev));
-      if (D->deg == NULL)    TRY(dalloc(D->dev,D->st,(void **) &D->deg,(size_t) ((n+4)&~3ll)));
-      if (D->up == NULL)     TRY(dalloc(D->dev,D->st,(void **) &D->up,ib*(size_t) (D->hi-D->lo+1)));
-      if (D->filter == NULL) TRY(dalloc(D->dev,D->st,(void **) &D->filter,sizeof(uint32_t)*(size_t) hm_filter_words(s->fpos)));
-#undef TRY
+      if (D->deg == NULL)    TRY(dev_alloc(D,&D->deg,(n+4)&~3ll));
+      if (D->up == NULL)     TRY(dev_alloc(D,&D->up,(int64_t) ib*(D->hi-D->lo+1)));
+      if (D->filter == NULL) TRY(dev_alloc(D,&D->filter,sizeof(uint32_t)*hm_filter_words(s->fpos)));
       if (rc == HM_OK)
         rc = hm_k_build_filter(D->keys,n,s->fpos,D->filter,D->st);
       s->launches += 1;
     }
-  for (int g = 0; g < s->ngpu; g++)
-    { cudaSetDevice(s->d[g].dev);
-      cudaError_t e = cudaStreamSynchronize(s->d[g].st);
-      if (rc == HM_OK && e != cudaSuccess) rc = hm_cuda_fail(e,"prefix filter");
-    }
+  int rc2 = sync_all(s,"prefix filter");
+  if (rc == HM_OK) rc = rc2;
   if (rc == HM_OK)
     s->have_direct = 1;
   return rc;
@@ -905,8 +960,9 @@ static int ensure_symm(hm_scan *s)
       D->slo = cut[g]; D->shi = cut[g+1];
       int rc = hm_symm_plan(n,D->shi-D->slo,s->kmer,G,&D->symm_layout);
       if (rc != HM_OK) return rc;
-      if (D->symm_work != NULL) { dfree(D->dev,D->st,D->symm_work); D->symm_work = NULL; }
-      HM_CUDA(dalloc(D->dev,D->st,&D->symm_work,(size_t) D->symm_layout.bytes));
+      dev_free(D,D->symm_work);
+      D->symm_work = NULL;
+      HM_CUDA(dev_alloc(D,&D->symm_work,D->symm_layout.bytes));
     }
   s->have_symm = 1; s->symm_ready = 0;
   return HM_OK;
@@ -937,30 +993,41 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
   }
   /* everything derived from the old table goes first: work buffers of both paths, the index */
   s->ran = 0; s->have_direct = 0; s->have_symm = 0; s->symm_ready = 0;
+  if ((rc = sync_all(s,"conditioning")) != HM_OK)
+    return rc;
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
-      HM_CUDA(cudaSetDevice(D->dev));
-      HM_CUDA(cudaStreamSynchronize(D->st));
-      dfree(D->dev,D->st,D->deg);    D->deg = NULL;
-      dfree(D->dev,D->st,D->up);     D->up = NULL;
-      dfree(D->dev,D->st,D->bucket); D->bucket = NULL;
-      dfree(D->dev,D->st,D->filter); D->filter = NULL;
-      if (D->symm_work != NULL) { dfree(D->dev,D->st,D->symm_work); D->symm_work = NULL; }
-      /* the table arrays are about to be replaced by plain cudaMalloc'ed ones: hand pooled ones back
-       * (conditioning frees them with cudaFree, which is legal for pool memory)                    */
-      PoolReg *R = g_pool + (D->dev < 64 ? D->dev : 0);
-      void *arr[3] = { D->keys, D->keys_lo, D->cnt };
-      for (int a = 0; a < 3; a++)
-        for (int k = 0; k < R->n; k++)
-          if (arr[a] != NULL && R->p[k] == arr[a])
-            R->p[k] = R->p[--R->n];
+      cudaSetDevice(D->dev);
+      dev_free(D,D->deg);    D->deg = NULL;
+      dev_free(D,D->up);     D->up = NULL;
+      dev_free(D,D->bucket); D->bucket = NULL;
+      dev_free(D,D->filter); D->filter = NULL;
+      dev_free(D,D->symm_work); D->symm_work = NULL;
     }
   for (int g = 0; g < G && rc == HM_OK; g++)
     { DevTable *D = s->d+g;
-      int64_t   n = s->n;
-      HM_CUDA(cudaSetDevice(D->dev));
-      rc = hm_condition_arrays(s->kmer,ethresh,do_trim,do_symm,&D->keys,&D->keys_lo,&D->cnt,&n,D->st);
+      int64_t   n = s->n, cap = 0;
+      uint64_t *keys = D->keys, *keys_lo = D->keys_lo;
+      uint16_t *cnt = D->cnt;
+      cudaError_t e;
+      TRY(cudaSetDevice(D->dev));
+      if (rc == HM_OK)
+        rc = hm_condition_arrays(s->kmer,ethresh,do_trim,do_symm,&D->keys,&D->keys_lo,&D->cnt,&n,&cap,D->st);
       s->launches += 6;
+      if (rc == HM_OK && D->keys != keys)          /* the new table (cap entries per array) replaces the old one */
+        { cudaError_t ek = dev_track(D,D->keys,8*cap,0);
+          cudaError_t el = D->keys_lo != NULL ? dev_track(D,D->keys_lo,8*cap,0) : cudaSuccess;
+          cudaError_t ec = dev_track(D,D->cnt,2*cap,0);
+          void *drop[3] = { keys, keys_lo, cnt };
+          if (ek != cudaSuccess || el != cudaSuccess || ec != cudaSuccess)
+            { /* (dev_track has freed what it could not count): the old table stays */
+              drop[0] = D->keys; drop[1] = D->keys_lo; drop[2] = D->cnt;
+              D->keys = keys; D->keys_lo = keys_lo; D->cnt = cnt;
+              rc = hm_set_error(HM_ENOMEM,"out of host memory");
+            }
+          for (int a = 0; a < 3; a++)
+            dev_free(D,drop[a]);
+        }
       if (rc == HM_OK && n_new >= 0 && n != n_new)
         rc = hm_set_error(HM_ECUDA,"conditioning gave %lld entries on GPU %d but %lld on GPU 0",
                           (long long) n,D->dev,(long long) n_new);
@@ -976,35 +1043,31 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
     }
   /* index (also after a failure on GPU 0: the old table is intact and stays usable) */
   size_t ib = s->idx64 ? 8 : 4;
-  int    rc2 = HM_OK;
-  for (int g = 0; g < G && rc2 == HM_OK && !s->invalid; g++)
+  int    rc_cond = rc;
+  rc = HM_OK;
+  for (int g = 0; g < G && rc == HM_OK && !s->invalid; g++)
     { DevTable *D = s->d+g;
       int64_t   n = s->n;
       cudaError_t e;
       D->lo = n*g/G;
       D->hi = n*(g+1)/G;
-#define TRY(call) if (rc2 == HM_OK && (e = (call)) != cudaSuccess) rc2 = hm_cuda_fail(e,#call)
       TRY(cudaSetDevice(D->dev));
-      TRY(dalloc(D->dev,D->st,(void **) &D->bucket,ib*(((size_t) 1<<s->bits)+1)));
+      TRY(dev_alloc(D,&D->bucket,(int64_t) ib*((1ll << s->bits)+1)));
       TRY(cudaMemsetAsync(D->fp_acc,0,4*sizeof(uint64_t),D->st));
-#undef TRY
-      if (rc2 == HM_OK)
-        rc2 = hm_k_build_bucket_index(D->keys,n,s->bits,D->bucket,s->idx64,D->st);
-      if (rc2 == HM_OK && s->kmer >= HM_SYMM_MIN_KMER)
-        rc2 = hm_k_symm_fingerprint(D->keys,D->keys_lo,D->cnt,D->lo,D->hi,s->kmer,s->seed,D->fp_acc,D->st);
+      if (rc == HM_OK)
+        rc = hm_k_build_bucket_index(D->keys,n,s->bits,D->bucket,s->idx64,D->st);
+      if (rc == HM_OK && s->kmer >= HM_SYMM_MIN_KMER)
+        rc = hm_k_symm_fingerprint(D->keys,D->keys_lo,D->cnt,D->lo,D->hi,s->kmer,s->seed,D->fp_acc,D->st);
       s->launches += 2;
     }
-  for (int g = 0; g < G; g++)
-    { cudaSetDevice(s->d[g].dev);
-      cudaError_t e = cudaStreamSynchronize(s->d[g].st);
-      if (rc2 == HM_OK && e != cudaSuccess) rc2 = hm_cuda_fail(e,"re-index after conditioning");
-    }
-  if (rc2 == HM_OK && !s->invalid)
-    rc2 = fingerprint_verdict(s);
-  if (rc2 != HM_OK)
+  int rc_sync = sync_all(s,"re-index after conditioning");
+  if (rc == HM_OK) rc = rc_sync;
+  if (rc == HM_OK && !s->invalid)
+    rc = fingerprint_verdict(s);
+  if (rc != HM_OK)
     s->invalid = 1;
   if (nels_out) *nels_out = s->n;
-  return rc != HM_OK ? rc : rc2;
+  return rc_cond != HM_OK ? rc_cond : rc;
 }
 
 /* reverse complement of a left-aligned packed k-mer (k <= 32) */
@@ -1039,35 +1102,36 @@ extern "C" int hm_scan_examine(hm_scan *s, int ethresh, int *trim, int *symm)
     return examine_streamed(s,ethresh,trim,symm);
   DevTable *D = s->d;
   int64_t   n = s->n, frst, last;
-  int       h_min = 0x8000, *d_min = NULL;
+  int       h_min = 0x8000, *d_min = NULL, rc = HM_OK;
   uint64_t *d_q = NULL;
   int64_t  *d_pos = NULL;
   int       two = (D->keys_lo != NULL);
+  cudaError_t e;
 
-  HM_CUDA(cudaSetDevice(D->dev));
   if (n+3 < 100000000) { frst = 0; last = n; }
   else { frst = n/2-50000000; last = n/2+50000000; }
-  HM_CUDA(cudaMalloc(&d_min,sizeof(int)));
-  HM_CUDA(cudaMemcpyAsync(d_min,&h_min,sizeof(int),cudaMemcpyHostToDevice,D->st));
-  int rc = hm_k_min_count(D->cnt,frst,last,d_min,D->st);
-  s->launches += 1;
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&d_min,sizeof(int)));
+  TRY(dev_alloc(D,&d_q,2*sizeof(uint64_t)));
+  TRY(dev_alloc(D,&d_pos,sizeof(int64_t)));
+  TRY(cudaMemcpyAsync(d_min,&h_min,sizeof(int),cudaMemcpyHostToDevice,D->st));
   if (rc == HM_OK)
-    { cudaError_t e = cudaMemcpyAsync(&h_min,d_min,sizeof(int),cudaMemcpyDeviceToHost,D->st);
+    { rc = hm_k_min_count(D->cnt,frst,last,d_min,D->st);
+      s->launches += 1;
+    }
+  if (rc == HM_OK)
+    { e = cudaMemcpyAsync(&h_min,d_min,sizeof(int),cudaMemcpyDeviceToHost,D->st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(D->st);
       if (e != cudaSuccess) rc = hm_cuda_fail(e,"min_count");
     }
-  cudaFree(d_min);
-  if (rc != HM_OK)
-    return rc;
-  *trim = (h_min >= ethresh);
-
-  *symm = 1;
-  HM_CUDA(cudaMalloc(&d_q,2*sizeof(uint64_t)));
-  HM_CUDA(cudaMalloc(&d_pos,sizeof(int64_t)));
-  for (int64_t sidx = 1; sidx < n; sidx++)
+  if (rc == HM_OK)
+    { *trim = (h_min >= ethresh);
+      *symm = 1;
+    }
+  for (int64_t sidx = 1; sidx < n && rc == HM_OK; sidx++)
     { uint64_t x, xw = 0, q[2];
       int64_t  pos;
-      cudaError_t e = cudaMemcpyAsync(&x,D->keys+sidx,sizeof(uint64_t),cudaMemcpyDeviceToHost,D->st);
+      e = cudaMemcpyAsync(&x,D->keys+sidx,sizeof(uint64_t),cudaMemcpyDeviceToHost,D->st);
       if (e == cudaSuccess && two)
         e = cudaMemcpyAsync(&xw,D->keys_lo+sidx,sizeof(uint64_t),cudaMemcpyDeviceToHost,D->st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(D->st);
@@ -1084,19 +1148,63 @@ extern "C" int hm_scan_examine(hm_scan *s, int ethresh, int *trim, int *symm)
       if (pos < 0) { *symm = 0; break; }
       if (pos != sidx) { *symm = 1; break; }
     }
-  cudaFree(d_q); cudaFree(d_pos);
+  dev_free(D,d_min); dev_free(D,d_q); dev_free(D,d_pos);
   return rc;
+}
+
+/* several GPUs: their plots summed into GPU 0's; then GPU 0's plot to the host (queued on its stream) */
+static int plot_to_host(hm_scan *s, int64_t *plot)
+{ int G = s->ngpu;
+  if (G > 1)
+    { unsigned long long *pl[HM_MAX_GPUS]; int dev[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
+      for (int g = 0; g < G; g++)
+        { pl[g] = s->d[g].plot; dev[g] = s->d[g].dev; st[g] = s->d[g].st; }
+      int rc = hm_peer_sum_plot(pl,dev,st,G);
+      if (rc != HM_OK) return rc;
+      s->launches += 1;
+    }
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  HM_CUDA(cudaMemcpyAsync(plot,s->d[0].plot,sizeof(int64_t)*HM_PLOT_CELLS,cudaMemcpyDeviceToHost,s->d[0].st));
+  return HM_OK;
+}
+
+/* every GPU g pulls the Bloom segments the other GPUs filled (segment h: GPU h) into its work area work[g], on
+ * st[g]; skip_empty: not from shards without entries.  One layout L serves every GPU: hm_symm_plan places the
+ * segments (off_bloom, seg_words) by n and the segment count alone, not by a GPU's range.                   */
+static int gather_bloom(hm_scan *s, void *const *work, const hm_symm_layout *L, const cudaStream_t *st, int skip_empty)
+{ size_t segb = sizeof(uint32_t)*(size_t) L->seg_words;
+  for (int g = 0; g < s->ngpu; g++)
+    { HM_CUDA(cudaSetDevice(s->d[g].dev));
+      for (int h = 0; h < s->ngpu; h++)
+        if (h != g && !(skip_empty && s->d[h].hi <= s->d[h].lo))
+          HM_CUDA(cudaMemcpyPeerAsync((uint8_t *) work[g] + L->off_bloom + segb*h,s->d[g].dev,
+                                      (uint8_t *) work[h] + L->off_bloom + segb*h,s->d[h].dev,segb,st[g]));
+    }
+  return HM_OK;
+}
+
+/* a run's stats: what differs by path comes as arguments; ms_run is the run's wall clock */
+static void fill_stats(const hm_scan *s, hm_scan_stats *st, int path, int bucket_bits, int filter_bits, double ms_h2d,
+                       float ms1, float ms2, double ms_scan, double ms_run, double ms_records, double ms_index)
+{ if (st == NULL)
+    return;
+  st->nels = s->n; st->n_gpus = s->ngpu; st->bucket_bits = bucket_bits;
+  st->filter_bits = filter_bits; st->path = path;
+  st->ms_h2d_unpack = ms_h2d;
+  st->ms_pass1 = ms1; st->ms_pass2 = ms2;
+  st->ms_scan = ms_scan;
+  st->ms_total = s->ms_load + ms_run;
+  st->kernel_launches = s->launches;
+  st->ms_alloc = s->ms_alloc; st->ms_records = ms_records; st->ms_index = ms_index;
 }
 
 /* the direct passes of hm_kernels.cu: any table */
 static int run_direct(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
 { int         G = s->ngpu, rc = HM_OK;
-  int64_t     n = s->n, launches0 = s->launches;
+  int64_t     n = s->n;
   if ((rc = ensure_direct(s)) != HM_OK)
     return rc;
   double      t0 = now_ms();
-  cudaEvent_t ev[HM_MAX_GPUS][4];
-  float       ms1 = 0, ms2 = 0, msall = 0;
 
   /* several GPUs: foreign incidence bytes are reached through the owner's array (remote atomics
    * in pass 1, remote loads in pass 2) when every pair of GPUs has native NVLink atomics; otherwise
@@ -1120,8 +1228,9 @@ static int run_direct(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
         int64_t need = hm_pass2_scratch_bytes(D->hi-D->lo,s->idx64);
         if (D->p2scratch == NULL || D->p2scratch_bytes < need)
           { HM_CUDA(cudaSetDevice(D->dev));
-            if (D->p2scratch) cudaFree(D->p2scratch);
-            HM_CUDA(cudaMalloc(&D->p2scratch,(size_t) need));
+            dev_free(D,D->p2scratch);
+            D->p2scratch = NULL;
+            HM_CUDA(dev_alloc(D,&D->p2scratch,need));
             D->p2scratch_bytes = need;
           }
         sh[g].scratch = D->p2scratch; sh[g].scratch_bytes = D->p2scratch_bytes;
@@ -1130,15 +1239,12 @@ static int run_direct(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
-      for (int k = 0; k < 4; k++)
-        HM_CUDA(cudaEventCreate(&ev[g][k]));
-      HM_CUDA(cudaEventRecord(ev[g][0],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[0],D->st));
       HM_CUDA(cudaMemsetAsync(D->deg,0,(size_t) ((n+4)&~3ll),D->st));
       HM_CUDA(cudaMemsetAsync(D->plot,0,sizeof(unsigned long long)*HM_PLOT_CELLS,D->st));
     }
-  if (peer_mode)                                /* nobody adds to a peer before it has been zeroed */
-    for (int g = 0; g < G; g++)
-      { HM_CUDA(cudaSetDevice(s->d[g].dev)); HM_CUDA(cudaStreamSynchronize(s->d[g].st)); }
+  if (peer_mode && (rc = sync_all(s,"zero the incidence arrays")) != HM_OK)   /* nobody adds to a peer before it has been zeroed */
+    return rc;
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
@@ -1146,7 +1252,7 @@ static int run_direct(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
                              D->lo,D->hi,D->deg,D->up,peer_mode ? &sh[g] : NULL,D->st);
       if (rc != HM_OK) return rc;
       s->launches += (D->hi > D->lo);
-      HM_CUDA(cudaEventRecord(ev[g][1],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[1],D->st));
     }
   if (G > 1 && !peer_mode)
     { uint8_t *deg[HM_MAX_GPUS]; int64_t lo[HM_MAX_GPUS], hi[HM_MAX_GPUS];
@@ -1159,59 +1265,24 @@ static int run_direct(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
       if (rc != HM_OK) return rc;
       s->launches += G;
     }
-  if (peer_mode)                                /* every pass 1 (and its remote atomics) has landed */
-    for (int g = 0; g < G; g++)
-      { HM_CUDA(cudaSetDevice(s->d[g].dev)); HM_CUDA(cudaStreamSynchronize(s->d[g].st)); }
+  if (peer_mode && (rc = sync_all(s,"pass 1")) != HM_OK)   /* every pass 1 (and its remote atomics) has landed */
+    return rc;
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
-      HM_CUDA(cudaEventRecord(ev[g][2],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[2],D->st));
       rc = hm_k_pass2_plot(D->cnt,D->deg,D->up,s->idx64,D->lo,D->hi,D->plot,
                            peer_mode ? &sh[g] : NULL,D->st);
       if (rc != HM_OK) return rc;
       s->launches += (D->hi > D->lo);
-      HM_CUDA(cudaEventRecord(ev[g][3],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[3],D->st));
     }
-  if (G > 1)
-    { unsigned long long *pl[HM_MAX_GPUS]; int dev[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
-      for (int g = 0; g < G; g++)
-        { pl[g] = s->d[g].plot; dev[g] = s->d[g].dev; st[g] = s->d[g].st; }
-      rc = hm_peer_sum_plot(pl,dev,st,G);
-      if (rc != HM_OK) return rc;
-      s->launches += 1;
-    }
-  HM_CUDA(cudaSetDevice(s->d[0].dev));
-  HM_CUDA(cudaMemcpyAsync(plot,s->d[0].plot,sizeof(int64_t)*HM_PLOT_CELLS,
-                          cudaMemcpyDeviceToHost,s->d[0].st));
-  for (int g = 0; g < G; g++)
-    { HM_CUDA(cudaSetDevice(s->d[g].dev));
-      HM_CUDA(cudaStreamSynchronize(s->d[g].st));
-    }
+  if ((rc = plot_to_host(s,plot)) != HM_OK || (rc = sync_all(s,"direct passes")) != HM_OK)
+    return rc;
   double t1 = now_ms();
-  for (int g = 0; g < G; g++)
-    { float a = 0, b = 0, c = 0;
-      cudaSetDevice(s->d[g].dev);
-      cudaEventElapsedTime(&a,ev[g][0],ev[g][1]);
-      cudaEventElapsedTime(&b,ev[g][2],ev[g][3]);
-      cudaEventElapsedTime(&c,ev[g][0],ev[g][3]);
-      if (a > ms1) ms1 = a;
-      if (b > ms2) ms2 = b;
-      if (c > msall) msall = c;
-      for (int k = 0; k < 4; k++)
-        cudaEventDestroy(ev[g][k]);
-    }
   s->ran = 1; s->peer_mode = peer_mode; s->last_path = HM_PATH_DIRECT;
-  if (stats != NULL)
-    { stats->nels = n; stats->n_gpus = G; stats->bucket_bits = s->bits;
-      stats->filter_bits = s->fpos; stats->path = HM_PATH_DIRECT;
-      stats->ms_h2d_unpack = s->ms_load;
-      stats->ms_pass1 = ms1; stats->ms_pass2 = ms2;
-      stats->ms_scan = G > 1 ? (t1-t0) : msall;
-      stats->ms_total = s->ms_load + (t1-t0);
-      stats->kernel_launches = s->launches;
-      stats->ms_alloc = s->ms_alloc; stats->ms_records = s->ms_records; stats->ms_index = s->ms_index;
-    }
-  (void) launches0;
+  fill_stats(s,stats,HM_PATH_DIRECT,s->bits,s->fpos,s->ms_load,slowest_ms(s,0,1),slowest_ms(s,2,3),
+             G > 1 ? t1-t0 : slowest_ms(s,0,3),t1-t0,s->ms_records,s->ms_index);
   return HM_OK;
 }
 
@@ -1221,8 +1292,6 @@ static int run_direct(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
 static int run_symm(hm_scan *s, int64_t *plot, hm_scan_stats *stats, uint64_t *status)
 { int         G = s->ngpu, rc = HM_OK;
   int64_t     n = s->n;
-  cudaEvent_t ev[HM_MAX_GPUS][4];
-  float       ms1 = 0, ms2 = 0, msall = 0;
   if ((rc = ensure_symm(s)) != HM_OK)
     return rc;
   s->symm_ready = 0;
@@ -1230,9 +1299,7 @@ static int run_symm(hm_scan *s, int64_t *plot, hm_scan_stats *stats, uint64_t *s
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
-      for (int k = 0; k < 4; k++)
-        HM_CUDA(cudaEventCreate(&ev[g][k]));
-      HM_CUDA(cudaEventRecord(ev[g][0],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[0],D->st));
       HM_CUDA(cudaMemsetAsync(D->plot,0,sizeof(unsigned long long)*HM_PLOT_CELLS,D->st));
       rc = hm_k_symm_runscan(D->keys,D->keys_lo,D->cnt,n,D->bucket,s->bits,s->idx64,s->kmer,D->slo,D->shi,
                              D->symm_work,&D->symm_layout,G > 1 ? &s->ssh[g] : NULL,D->st);
@@ -1241,83 +1308,45 @@ static int run_symm(hm_scan *s, int64_t *plot, hm_scan_stats *stats, uint64_t *s
                             D->symm_work,&D->symm_layout,G > 1 ? &s->ssh[g] : NULL,D->st);
       if (rc != HM_OK) return rc;
       s->launches += 2*(D->shi > D->slo);
-      HM_CUDA(cudaEventRecord(ev[g][1],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[1],D->st));
     }
   if (G > 1)                                    /* every device pulls the other devices' Bloom segments */
-    { for (int g = 0; g < G; g++)
-        { HM_CUDA(cudaSetDevice(s->d[g].dev)); HM_CUDA(cudaStreamSynchronize(s->d[g].st)); }
+    { void *work[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
       for (int g = 0; g < G; g++)
-        { DevTable *D = s->d+g;
-          size_t    segb = sizeof(uint32_t)*(size_t) D->symm_layout.seg_words;
-          HM_CUDA(cudaSetDevice(D->dev));
-          for (int h = 0; h < G; h++)
-            if (h != g)
-              { DevTable *S = s->d+h;
-                HM_CUDA(cudaMemcpyPeerAsync((uint8_t *) D->symm_work + D->symm_layout.off_bloom + segb*h,D->dev,
-                                            (uint8_t *) S->symm_work + S->symm_layout.off_bloom + segb*h,S->dev,
-                                            segb,D->st));
-              }
-        }
+        { work[g] = s->d[g].symm_work; st[g] = s->d[g].st; }
+      if ((rc = sync_all(s,"symmetric pass 1")) != HM_OK ||
+          (rc = gather_bloom(s,work,&s->d[0].symm_layout,st,0)) != HM_OK)
+        return rc;
     }
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
-      HM_CUDA(cudaEventRecord(ev[g][2],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[2],D->st));
       rc = hm_k_symm_resolve(D->keys,D->keys_lo,D->cnt,n,D->bucket,s->bits,s->idx64,s->kmer,
                              D->symm_work,&D->symm_layout,G > 1 ? &s->ssh[g] : NULL,D->plot,D->st);
       if (rc != HM_OK) return rc;
       s->launches += 1;
-      HM_CUDA(cudaEventRecord(ev[g][3],D->st));
+      HM_CUDA(cudaEventRecord(D->ev[3],D->st));
     }
-  if (G > 1)
-    { unsigned long long *pl[HM_MAX_GPUS]; int dev[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
-      for (int g = 0; g < G; g++)
-        { pl[g] = s->d[g].plot; dev[g] = s->d[g].dev; st[g] = s->d[g].st; }
-      rc = hm_peer_sum_plot(pl,dev,st,G);
-      if (rc != HM_OK) return rc;
-      s->launches += 1;
-    }
+  if ((rc = plot_to_host(s,plot)) != HM_OK)
+    return rc;
   uint64_t hdr[HM_MAX_GPUS][2];
-  HM_CUDA(cudaSetDevice(s->d[0].dev));
-  HM_CUDA(cudaMemcpyAsync(plot,s->d[0].plot,sizeof(int64_t)*HM_PLOT_CELLS,
-                          cudaMemcpyDeviceToHost,s->d[0].st));
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       HM_CUDA(cudaSetDevice(D->dev));
       HM_CUDA(cudaMemcpyAsync(hdr[g],(uint8_t *) D->symm_work + D->symm_layout.off_header,2*sizeof(uint64_t),
                               cudaMemcpyDeviceToHost,D->st));
     }
-  for (int g = 0; g < G; g++)
-    { HM_CUDA(cudaSetDevice(s->d[g].dev));
-      HM_CUDA(cudaStreamSynchronize(s->d[g].st));
-    }
+  if ((rc = sync_all(s,"symmetric scan")) != HM_OK)
+    return rc;
   double t1 = now_ms();
   *status = 0;
   for (int g = 0; g < G; g++)
-    { float a = 0, b = 0, c = 0;
-      *status |= hdr[g][1];
-      cudaSetDevice(s->d[g].dev);
-      cudaEventElapsedTime(&a,ev[g][0],ev[g][1]);
-      cudaEventElapsedTime(&b,ev[g][2],ev[g][3]);
-      cudaEventElapsedTime(&c,ev[g][0],ev[g][3]);
-      if (a > ms1) ms1 = a;
-      if (b > ms2) ms2 = b;
-      if (c > msall) msall = c;
-      for (int k = 0; k < 4; k++)
-        cudaEventDestroy(ev[g][k]);
-    }
+    *status |= hdr[g][1];
   s->last_path = HM_PATH_SYMM;
   s->symm_ready = (*status == 0);
-  if (stats != NULL)
-    { stats->nels = n; stats->n_gpus = G; stats->bucket_bits = s->bits;
-      stats->filter_bits = 0; stats->path = HM_PATH_SYMM;
-      stats->ms_h2d_unpack = s->ms_load;
-      stats->ms_pass1 = ms1; stats->ms_pass2 = ms2;
-      stats->ms_scan = G > 1 ? (t1-t0) : msall;
-      stats->ms_total = s->ms_load + (t1-t0);
-      stats->kernel_launches = s->launches;
-      stats->ms_alloc = s->ms_alloc; stats->ms_records = s->ms_records; stats->ms_index = s->ms_index;
-    }
+  fill_stats(s,stats,HM_PATH_SYMM,s->bits,0,s->ms_load,slowest_ms(s,0,1),slowest_ms(s,2,3),
+             G > 1 ? t1-t0 : slowest_ms(s,0,3),t1-t0,s->ms_records,s->ms_index);
   return HM_OK;
 }
 
@@ -1353,31 +1382,22 @@ typedef struct
     hm_stream_lists R;
     Stager    G;
     void     *s_bucket;
-    int64_t   s_bucket_bytes;
     void     *sort_tmp;                                /* sorts the S keys of one chunk */
     int64_t   sort_bytes;
     cudaStream_t sc;                                   /* the chunks' kernels: overlap the next chunk's load */
     hm_stream_sview *views;                            /* several shards: every shard's S view, on this device */
+    double    ms_loop;                                 /* the chunk loop, wall clock */
   } StreamRun;
 
-static int64_t stream_list_bytes(const hm_scan *s, const StreamRun *R)
-{ int KW = s->kmer > 32 ? 2 : 1;
-  return (8*KW+8)*R->R.cand_cap + 8*KW*R->R.s_cap;
-}
-
-static void stream_free_chunks(hm_scan *s, DevTable *D, StreamRun *R)
-{ int KW = s->kmer > 32 ? 2 : 1;
-  if (R->sc) cudaStreamSynchronize(R->sc);
+static void stream_free_chunks(DevTable *D, StreamRun *R)
+{ if (R->sc) cudaStreamSynchronize(R->sc);
   for (int b = 0; b < 2; b++)
-    { sfree(s,D,R->keys[b],8*(R->cap+1)); R->keys[b] = NULL;
-      if (KW == 2) sfree(s,D,R->klo[b],8*(R->cap+1));
-      R->klo[b] = NULL;
-      sfree(s,D,R->cnt[b],2*(R->cap+8)); R->cnt[b] = NULL;
+    { dev_free(D,R->keys[b]); dev_free(D,R->klo[b]); dev_free(D,R->cnt[b]);
+      R->keys[b] = NULL; R->klo[b] = NULL; R->cnt[b] = NULL;
     }
-  sfree(s,D,R->bucket,4*((1ll << R->bits)+1)); R->bucket = NULL;
-  sfree(s,D,R->R.runs,8*R->R.runs_cap);        R->R.runs = NULL;
-  sfree(s,D,R->sort_tmp,R->sort_bytes);        R->sort_tmp = NULL;
-  if (R->G.bytes > 0) D->held -= R->G.bytes;
+  dev_free(D,R->bucket);   R->bucket = NULL;
+  dev_free(D,R->R.runs);   R->R.runs = NULL;
+  dev_free(D,R->sort_tmp); R->sort_tmp = NULL;
   stager_close(D,&R->G);
 }
 
@@ -1391,21 +1411,18 @@ static int stream_alloc_chunks(hm_scan *s, DevTable *D, StreamRun *R, int64_t ca
   R->cap = cap;
   R->bits = hm_pick_bucket_bits(cap);
   for (int b = 0; b < 2 && e == cudaSuccess; b++)
-    { e = salloc(s,D,(void **) &R->keys[b],8*(cap+1));
-      if (e == cudaSuccess && KW == 2) e = salloc(s,D,(void **) &R->klo[b],8*(cap+1));
-      if (e == cudaSuccess) e = salloc(s,D,(void **) &R->cnt[b],2*(cap+8));
+    { e = dev_alloc(D,&R->keys[b],8*(cap+1));
+      if (e == cudaSuccess && KW == 2) e = dev_alloc(D,&R->klo[b],8*(cap+1));
+      if (e == cudaSuccess) e = dev_alloc(D,&R->cnt[b],2*(cap+8));
     }
-  if (e == cudaSuccess) e = salloc(s,D,&R->bucket,4*((1ll << R->bits)+1));
+  if (e == cudaSuccess) e = dev_alloc(D,&R->bucket,4*((1ll << R->bits)+1));
   R->R.runs_cap = cap/3+1024;
-  if (e == cudaSuccess) e = salloc(s,D,(void **) &R->R.runs,8*R->R.runs_cap);
+  if (e == cudaSuccess) e = dev_alloc(D,&R->R.runs,8*R->R.runs_cap);
   R->sort_bytes = hm_sort_keys_bytes(cap+1024,s->kmer);
-  if (e == cudaSuccess) e = salloc(s,D,&R->sort_tmp,R->sort_bytes);
+  if (e == cudaSuccess) e = dev_alloc(D,&R->sort_tmp,R->sort_bytes);
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"streamed scan: chunk buffers");
-  int rc = stager_open(s,D,s->host,cap,&R->G);
-  D->held += R->G.bytes;
-  if (D->held > D->peak) D->peak = D->held;
-  return rc;
+  return stager_open(s,D,s->host,cap,&R->G);
 }
 
 /* grow a group of resident arrays (same capacity, 8-byte elements) to hold `need` entries: doubling, but
@@ -1431,12 +1448,12 @@ static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[
                         s->ngpu > 1 ? "" : " or more GPUs (HETMERS_GPUS)");
   for (int a = 0; a < narr; a++)
     { uint64_t *p = NULL;
-      cudaError_t e = salloc(s,D,(void **) &p,8*nc);
+      cudaError_t e = dev_alloc(D,&p,8*nc);
       if (e != cudaSuccess) return hm_cuda_fail(e,"streamed scan: resident lists");
       if (used > 0 && *arr[a] != NULL)
         HM_CUDA(cudaMemcpyAsync(p,*arr[a],8*(size_t) used,cudaMemcpyDeviceToDevice,st));
       HM_CUDA(cudaStreamSynchronize(st));
-      sfree(s,D,*arr[a],8 * *cap);
+      dev_free(D,*arr[a]);
       *arr[a] = p;
     }
   *cap = nc;
@@ -1444,15 +1461,13 @@ static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[
 }
 
 /* pass 1 of one shard: its range [D->lo, D->hi) chunk by chunk (leaves early, with HM_OK, once s->stop is set) */
-static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shards *sh, float *ms_kernels)
+static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shards *sh)
 { const hm_host_table *t = s->host;
   int      KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
   int64_t  lo = D->lo, hi = D->hi, c0 = lo, chunks = 0;
   int      b = 0;
   uint64_t nc = 0, status = 0, ns = 0, ns0 = 0;     /* ns0: S keys before the chunk in flight */
-  cudaEvent_t e0, e1;
-  HM_CUDA(cudaEventCreate(&e0)); HM_CUDA(cudaEventCreate(&e1));
-  HM_CUDA(cudaEventRecord(e0,R->sc));
+  HM_CUDA(cudaEventRecord(D->ev[0],R->sc));
   while (c0 < hi && rc == HM_OK && !s->stop)
     { int64_t m = hi-c0 < R->cap ? hi-c0 : R->cap;
       /* the copy + unpack of this chunk overlaps the kernels of the previous one (on R->sc) */
@@ -1464,7 +1479,7 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shar
       if (cut == 0)
         { /* one run fills the whole chunk: larger buffers, and load it again */
           int64_t cap = 2*R->cap;
-          stream_free_chunks(s,D,R);
+          stream_free_chunks(D,R);
           rc = stream_alloc_chunks(s,D,R,cap);
           if (rc == HM_ENOMEM)
             rc = hm_set_error(HM_ENOMEM,"a run of more than %lld entries (k-mers sharing their first %d bases) does "
@@ -1502,39 +1517,27 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shar
   if (rc == HM_OK && (rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) == HM_OK)
     rc = hm_sort_keys(R->R.s_key+ns0,KW == 2 ? R->R.s_lo+ns0 : NULL,(int64_t) (ns-ns0),s->kmer,
                       R->sort_tmp,R->sort_bytes,R->sc);
-  cudaEventRecord(e1,R->sc);
+  cudaEventRecord(D->ev[1],R->sc);
   cudaError_t e = cudaStreamSynchronize(R->sc);
   if (rc == HM_OK && e != cudaSuccess) rc = hm_cuda_fail(e,"streamed scan: pass 1");
-  cudaEventElapsedTime(ms_kernels,e0,e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
   D->chunks = chunks;
   return rc;
 }
 
-/* one shard's pass 1 on its own device: stub index, work area (the whole-table Bloom filter), chunk buffers,
- * the chunk loop; then the chunk buffers and the stub index go again, to make room for the S index       */
-typedef struct
-  { hm_scan   *s;
-    int        g, rc;
-    StreamRun *R;
-    float      ms1;                                    /* pass-1 kernels (CUDA events)     */
-    double     ms_loop;                                /* the chunk loop, wall clock       */
-    char       msg[512];
-  } ShardJob;
-
-static int shard_pass1(ShardJob *J)
-{ hm_scan   *s = J->s;
-  DevTable  *D = s->d+J->g;
-  StreamRun *R = J->R;
-  const hm_symm_shards *sh = s->ngpu > 1 ? s->ssh+J->g : NULL;
+/* on_every_gpu: shard g's pass 1 on its own device (arg: the runs of every shard): stub index, work area (the
+ * whole-table Bloom filter), chunk buffers, the chunk loop                                                  */
+static int shard_pass1(hm_scan *s, int g, void *arg)
+{ DevTable  *D = s->d+g;
+  StreamRun *R = (StreamRun *) arg + g;
+  const hm_symm_shards *sh = s->ngpu > 1 ? s->ssh+g : NULL;
   int64_t ixlen = (int64_t) 1 << (8*s->ibyte);
   int     rc;
   cudaError_t e;
   HM_CUDA(cudaSetDevice(D->dev));
   HM_CUDA(cudaStreamCreateWithFlags(&R->sc,cudaStreamNonBlocking));
   if ((rc = stream_work_layout(s->n,s->kmer,s->ngpu,&R->L)) != HM_OK) return rc;
-  if ((e = salloc(s,D,(void **) &R->d_index,8*ixlen)) != cudaSuccess ||
-      (e = salloc(s,D,&R->work,R->L.bytes)) != cudaSuccess)
+  if ((e = dev_alloc(D,&R->d_index,8*ixlen)) != cudaSuccess ||
+      (e = dev_alloc(D,&R->work,R->L.bytes)) != cudaSuccess)
     return hm_cuda_fail(e,"streamed scan: work area");
   HM_CUDA(cudaMemcpyAsync(R->d_index,s->host->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,R->sc));
   HM_CUDA(cudaMemsetAsync(D->fp_acc,0,4*sizeof(uint64_t),R->sc));
@@ -1544,9 +1547,9 @@ static int shard_pass1(ShardJob *J)
   if ((rc = stream_alloc_chunks(s,D,R,s->plan.chunk)) != HM_OK)
     return rc == HM_ENOMEM ? hm_set_error(HM_ENOMEM,"the streamed scan's chunk buffers do not fit the device budget") : rc;
   double t0 = now_ms();
-  if ((rc = stream_pass(s,D,R,sh,&J->ms1)) != HM_OK)
+  if ((rc = stream_pass(s,D,R,sh)) != HM_OK)
     return rc;
-  J->ms_loop = now_ms()-t0;
+  R->ms_loop = now_ms()-t0;
   uint64_t nc = 0, status = 0, ns = 0;
   if ((rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) != HM_OK) return rc;
   if (status != 0)
@@ -1554,49 +1557,20 @@ static int shard_pass1(ShardJob *J)
   return HM_OK;
 }
 
-static void *shard_worker(void *arg)
-{ ShardJob *J = (ShardJob *) arg;
-  J->rc = shard_pass1(J);
-  if (J->rc != HM_OK)
-    { J->s->stop = 1;                                   /* the other shards leave their chunk loops */
-      strncpy(J->msg,hm_last_error(),sizeof(J->msg)-1); J->msg[sizeof(J->msg)-1] = 0;
-    }
-  return NULL;
-}
-
-/* Pass 1 of every shard at once (a host thread each, the calling thread takes the last); the verdict over all
- * shards' fingerprints; the Bloom segments all-gathered; each shard's S list indexed; pass 2 of every shard,
- * whose exact checks look keys up in the S list of their owner (peer memory); the plots summed on the host. */
+/* Pass 1 of every shard at once; the verdict over all shards' fingerprints; the Bloom segments all-gathered; the
+ * chunk buffers and stub index freed, to make room for each shard's S index; pass 2 of every shard, whose exact
+ * checks look keys up in the S list of their owner (peer memory); the plots summed on the host.              */
 static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_stats *stats)
 { int       G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
   double    t0 = now_ms();
-  float     ms1 = 0, ms2 = 0;
   double    ms_loop = 0;
-  ShardJob  job[HM_MAX_GPUS];
-  pthread_t th[HM_MAX_GPUS];
-  int       created[HM_MAX_GPUS];
   cudaError_t e;
   s->stop = 0;
-  for (int g = 0; g < G; g++)
-    { memset(job+g,0,sizeof(job[g]));
-      job[g].s = s; job[g].g = g; job[g].R = RR+g;
-      created[g] = 0;
-      if (g == G-1 || pthread_create(th+g,NULL,shard_worker,job+g) != 0)
-        shard_worker(job+g);
-      else
-        created[g] = 1;
-    }
-  for (int g = 0; g < G; g++)
-    { if (created[g]) pthread_join(th[g],NULL);
-      if (job[g].rc != HM_OK && rc == HM_OK)
-        rc = G == 1 ? hm_set_error(job[g].rc,"%s",job[g].msg)
-                    : hm_set_error(job[g].rc,"shard %d of %d (GPU %d, entries %lld..%lld): %s",g,G,s->d[g].dev,
-                                   (long long) s->d[g].lo,(long long) s->d[g].hi,job[g].msg);
-      if (job[g].ms1 > ms1)         ms1 = job[g].ms1;
-      if (job[g].ms_loop > ms_loop) ms_loop = job[g].ms_loop;
-    }
-  if (rc != HM_OK)
+  if ((rc = on_every_gpu(s,shard_pass1,RR)) != HM_OK)
     return rc;
+  for (int g = 0; g < G; g++)
+    if (RR[g].ms_loop > ms_loop) ms_loop = RR[g].ms_loop;
+  float  ms1 = slowest_ms(s,0,1);
   double t_pass1 = now_ms();
   if ((rc = fingerprint_verdict(s)) != HM_OK) return rc;
   if (!s->symmetric)
@@ -1612,31 +1586,28 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
       if ((int64_t) ns[g] >= 0xFFFFFFF0ll) sidx64 = 1;    /* one offset width for every shard's index */
     }
   if (G > 1)                                    /* every shard pulls the other shards' Bloom segments */
-    for (int g = 0; g < G; g++)
-      { DevTable *D = s->d+g;
-        size_t    segb = sizeof(uint32_t)*(size_t) RR[g].L.seg_words;
-        HM_CUDA(cudaSetDevice(D->dev));
-        for (int h = 0; h < G; h++)
-          if (h != g && s->d[h].hi > s->d[h].lo)
-            HM_CUDA(cudaMemcpyPeerAsync((uint8_t *) RR[g].work + RR[g].L.off_bloom + segb*h,D->dev,
-                                        (uint8_t *) RR[h].work + RR[h].L.off_bloom + segb*h,s->d[h].dev,segb,RR[g].sc));
-      }
+    { void *work[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
+      for (int g = 0; g < G; g++)
+        { work[g] = RR[g].work; st[g] = RR[g].sc; }
+      if ((rc = gather_bloom(s,work,&RR[0].L,st,1)) != HM_OK)
+        return rc;
+    }
   /* S (sorted chunk by chunk) gets a bucket index in the room the chunk buffers leave: as fine as
    * hm_pick_bucket_bits asks, coarser if the budget says so (look-ups then bisect longer buckets)        */
   for (int g = 0; g < G; g++)
     { DevTable  *D = s->d+g;
       StreamRun *R = RR+g;
       HM_CUDA(cudaSetDevice(D->dev));
-      stream_free_chunks(s,D,R);
-      sfree(s,D,R->d_index,8*((int64_t) 1 << (8*s->ibyte))); R->d_index = NULL;
+      stream_free_chunks(D,R);
+      dev_free(D,R->d_index); R->d_index = NULL;
       sbits[g] = hm_pick_bucket_bits((int64_t) ns[g]);
       while (sbits[g] > 1 && D->held + (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1) > s->budget)
         sbits[g] -= 1;
-      R->s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1);
-      if ((e = salloc(s,D,&R->s_bucket,R->s_bucket_bytes)) != cudaSuccess)
+      int64_t s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1);
+      if ((e = dev_alloc(D,&R->s_bucket,s_bucket_bytes)) != cudaSuccess)
         return hm_cuda_fail(e,"streamed scan: S index");
       if (G > 1)
-        HM_CUDA(cudaMemsetAsync(R->s_bucket,0,(size_t) R->s_bucket_bytes,R->sc));   /* (an empty S list: all 0) */
+        HM_CUDA(cudaMemsetAsync(R->s_bucket,0,(size_t) s_bucket_bytes,R->sc));   /* (an empty S list: all 0) */
       if ((G == 1 || ns[g] > 0) &&
           (rc = hm_k_build_bucket_index(R->R.s_key,(int64_t) ns[g],sbits[g],R->s_bucket,sidx64,R->sc)) != HM_OK)
         return rc;
@@ -1651,7 +1622,7 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
       for (int g = 0; g < G; g++)
         { DevTable *D = s->d+g;
           HM_CUDA(cudaSetDevice(D->dev));
-          if ((e = salloc(s,D,(void **) &RR[g].views,sizeof(V))) != cudaSuccess)
+          if ((e = dev_alloc(D,&RR[g].views,sizeof(V))) != cudaSuccess)
             return hm_cuda_fail(e,"streamed scan: S views");
           HM_CUDA(cudaMemcpyAsync(RR[g].views,V,sizeof(V),cudaMemcpyHostToDevice,RR[g].sc));
         }
@@ -1659,35 +1630,31 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
         { HM_CUDA(cudaSetDevice(s->d[g].dev)); HM_CUDA(cudaStreamSynchronize(RR[g].sc)); }
     }
 
-  cudaEvent_t ev[HM_MAX_GPUS][2];
-  memset(ev,0,sizeof(ev));
   for (int g = 0; g < G; g++)
     { DevTable  *D = s->d+g;
       StreamRun *R = RR+g;
       HM_CUDA(cudaSetDevice(D->dev));
-      HM_CUDA(cudaEventCreate(&ev[g][0])); HM_CUDA(cudaEventCreate(&ev[g][1]));
-      cudaEventRecord(ev[g][0],R->sc);
+      cudaEventRecord(D->ev[2],R->sc);
       rc = hm_symm_stream_resolve(R->R.s_key,KW == 2 ? R->R.s_lo : NULL,(int64_t) ns[g],R->s_bucket,sbits[g],sidx64,
                                   s->kmer,G == 1 ? s->n : D->hi-D->lo,R->work,&R->L,&R->R,G > 1 ? s->ssh+g : NULL,
                                   R->views,D->plot,R->sc);
-      cudaEventRecord(ev[g][1],R->sc);
+      cudaEventRecord(D->ev[3],R->sc);
       __sync_fetch_and_add(&s->launches,3);
-      if (rc != HM_OK) break;
+      if (rc != HM_OK) return rc;
     }
   int64_t *tmp = NULL;
-  if (rc == HM_OK && G > 1)
-    { tmp = (int64_t *) malloc(sizeof(int64_t)*HM_PLOT_CELLS);
-      if (tmp == NULL) rc = hm_set_error(HM_ENOMEM,"out of host memory");
-      else             memset(plot,0,sizeof(int64_t)*HM_PLOT_CELLS);
+  if (G > 1)
+    { if ((tmp = (int64_t *) malloc(sizeof(int64_t)*HM_PLOT_CELLS)) == NULL)
+        return hm_set_error(HM_ENOMEM,"out of host memory");
+      memset(plot,0,sizeof(int64_t)*HM_PLOT_CELLS);
     }
-  for (int g = 0; g < G; g++)
+  for (int g = 0; g < G && rc == HM_OK; g++)
     { DevTable  *D = s->d+g;
       StreamRun *R = RR+g;
       uint64_t   nc = 0, status = 0, nsx = 0;
-      float      b = 0;
       cudaSetDevice(D->dev);
-      if (rc == HM_OK && (e = cudaMemcpyAsync(G == 1 ? plot : tmp,D->plot,sizeof(int64_t)*HM_PLOT_CELLS,
-                                              cudaMemcpyDeviceToHost,R->sc)) != cudaSuccess)
+      if ((e = cudaMemcpyAsync(G == 1 ? plot : tmp,D->plot,sizeof(int64_t)*HM_PLOT_CELLS,
+                               cudaMemcpyDeviceToHost,R->sc)) != cudaSuccess)
         rc = hm_cuda_fail(e,"plot D2H");
       if (rc == HM_OK)
         rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&nsx,R->sc);      /* (synchronises) */
@@ -1696,64 +1663,41 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
       if (rc == HM_OK && G > 1)
         for (int64_t i = 0; i < HM_PLOT_CELLS; i++)
           plot[i] += tmp[i];
-      cudaStreamSynchronize(R->sc);
-      if (ev[g][1] != NULL && cudaEventElapsedTime(&b,ev[g][0],ev[g][1]) == cudaSuccess && b > ms2)
-        ms2 = b;
-      cudaGetLastError();
-      if (ev[g][0] != NULL) cudaEventDestroy(ev[g][0]);
-      if (ev[g][1] != NULL) cudaEventDestroy(ev[g][1]);
     }
   free(tmp);
   if (rc != HM_OK)
     return rc;
   double t1 = now_ms();
   s->last_path = HM_PATH_SYMM;
-  if (stats != NULL)
-    { stats->nels = s->n; stats->n_gpus = G; stats->bucket_bits = RR[0].bits;
-      stats->filter_bits = 0; stats->path = HM_PATH_SYMM;
-      stats->ms_h2d_unpack = s->ms_load + ms_loop;              /* the loads, with pass 1 running behind them */
-      stats->ms_pass1 = ms1; stats->ms_pass2 = ms2;             /* (the slowest shard's) */
-      stats->ms_scan = t1-t0;
-      stats->ms_total = s->ms_load + (t1-t0);
-      stats->kernel_launches = s->launches;
-      stats->ms_alloc = s->ms_alloc; stats->ms_records = ms_loop; stats->ms_index = t1-t_pass1;
-    }
+  fill_stats(s,stats,HM_PATH_SYMM,RR[0].bits,0,s->ms_load+ms_loop,              /* the loads, with pass 1 behind them */
+             ms1,slowest_ms(s,2,3),t1-t0,t1-t0,ms_loop,t1-t_pass1);              /* (the slowest shard's passes)       */
   return HM_OK;
 }
 
 static int run_stream(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
 { int       G = s->ngpu;
   StreamRun R[HM_MAX_GPUS];
-  int64_t   held0[HM_MAX_GPUS];
   if (s->kmer < HM_SYMM_MIN_KMER)
     return hm_set_error(HM_EUNSUPPORTED,"the table does not fit in device memory and k = %d has no strand-symmetric "
                         "scan; the direct passes need it resident",s->kmer);
   memset(R,0,sizeof(R));
   for (int g = 0; g < G; g++)
-    { held0[g] = s->d[g].held;
-      s->d[g].peak = held0[g];
+    { s->d[g].peak = s->d[g].held;
       s->d[g].chunks = 0;
     }
   int rc = run_stream_body(s,R,plot,stats);
   for (int g = 0; g < G; g++)                  /* every shard's thread has been joined: free it all */
     { DevTable *D = s->d+g;
-      int KW = s->kmer > 32 ? 2 : 1;
       cudaSetDevice(D->dev);
-      if (R[g].sc) cudaStreamSynchronize(R[g].sc);
-      stream_free_chunks(s,D,R+g);
-      sfree(s,D,R[g].d_index,8*((int64_t) 1 << (8*s->ibyte)));
-      sfree(s,D,R[g].work,R[g].L.bytes);
-      sfree(s,D,R[g].s_bucket,R[g].s_bucket_bytes);
-      sfree(s,D,R[g].views,sizeof(hm_stream_sview)*HM_MAX_GPUS);
-      sfree(s,D,R[g].R.cand_key,8*R[g].R.cand_cap); sfree(s,D,R[g].R.cand_meta,8*R[g].R.cand_cap);
-      if (KW == 2) sfree(s,D,R[g].R.cand_lo,8*R[g].R.cand_cap);
-      sfree(s,D,R[g].R.s_key,8*R[g].R.s_cap);
-      if (KW == 2) sfree(s,D,R[g].R.s_lo,8*R[g].R.s_cap);
+      stream_free_chunks(D,R+g);
+      dev_free(D,R[g].d_index);  dev_free(D,R[g].work);
+      dev_free(D,R[g].s_bucket); dev_free(D,R[g].views);
+      dev_free(D,R[g].R.cand_key); dev_free(D,R[g].R.cand_meta); dev_free(D,R[g].R.cand_lo);
+      dev_free(D,R[g].R.s_key);    dev_free(D,R[g].R.s_lo);
       if (D->st) cudaStreamSynchronize(D->st);
       if (R[g].sc) cudaStreamDestroy(R[g].sc);
       cudaCtxResetPersistingL2Cache();
       cudaGetLastError();
-      D->held = held0[g];
     }
   return rc;
 }
@@ -1764,36 +1708,29 @@ static int run_stream(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
 static int examine_streamed(hm_scan *s, int ethresh, int *trim, int *symm)
 { DevTable *D = s->d;
   const hm_host_table *t = s->host;
-  int      KW = s->kmer > 32 ? 2 : 1, two = (KW == 2), rc = HM_OK;
-  int64_t  n = s->n, frst, last, cap = s->plan.chunk, ixlen = (int64_t) 1 << (8*s->ibyte);
+  int      two = (s->kmer > 32), rc = HM_OK;
+  int64_t  n = s->n, frst, last, cap = s->plan.chunk;
   int      h_min = 0x8000, *d_min = NULL;
-  uint64_t *keys = NULL, *klo = NULL, *d_q = NULL;
-  uint16_t *cnt = NULL;
-  int64_t  *d_index = NULL, *d_pos = NULL;
+  uint64_t *d_q = NULL;
+  int64_t  *d_pos = NULL;
   void     *bucket = NULL;
   int      bits = hm_pick_bucket_bits(cap);
-  Stager   G;
-  memset(&G,0,sizeof(G));
-  HM_CUDA(cudaSetDevice(D->dev));
-  cudaError_t e = cudaMalloc(&keys,8*(size_t) (cap+1));
-  if (e == cudaSuccess && two) e = cudaMalloc(&klo,8*(size_t) (cap+1));
-  if (e == cudaSuccess) e = cudaMalloc(&cnt,2*(size_t) (cap+8));
-  if (e == cudaSuccess) e = cudaMalloc(&bucket,4*(((size_t) 1 << bits)+1));
-  if (e == cudaSuccess) e = cudaMalloc(&d_index,8*(size_t) ixlen);
-  if (e == cudaSuccess) e = cudaMalloc(&d_min,sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&d_q,2*sizeof(uint64_t));
-  if (e == cudaSuccess) e = cudaMalloc(&d_pos,sizeof(int64_t));
-  if (e == cudaSuccess) e = cudaMemcpy(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(d_min,&h_min,sizeof(int),cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) rc = hm_cuda_fail(e,"streamed examine: buffers");
-  if (rc == HM_OK) rc = stager_open(s,D,t,cap,&G);
+  Window   W;
+  cudaError_t e;
+  if ((rc = window_open(s,cap,&W)) != HM_OK)
+    return rc;
+  TRY(dev_alloc(D,&bucket,4*((1ll << bits)+1)));
+  TRY(dev_alloc(D,&d_min,sizeof(int)));
+  TRY(dev_alloc(D,&d_q,2*sizeof(uint64_t)));
+  TRY(dev_alloc(D,&d_pos,sizeof(int64_t)));
+  TRY(cudaMemcpyAsync(d_min,&h_min,sizeof(int),cudaMemcpyHostToDevice,D->st));
 
   if (n+3 < 100000000) { frst = 0; last = n; }
   else { frst = n/2-50000000; last = n/2+50000000; }
   for (int64_t o = frst; o < last && rc == HM_OK; o += cap)
     { int64_t m = last-o < cap ? last-o : cap;
-      rc = load_into(s,D,t,d_index,o,m,keys,klo,cnt,0,&G);
-      if (rc == HM_OK) rc = hm_k_min_count(cnt,0,m,d_min,D->st);
+      rc = window_load(s,&W,o,m);
+      if (rc == HM_OK) rc = hm_k_min_count(W.cnt,0,m,d_min,D->st);
       s->launches += 1;
     }
   if (rc == HM_OK)
@@ -1802,27 +1739,28 @@ static int examine_streamed(hm_scan *s, int ethresh, int *trim, int *symm)
       if (e != cudaSuccess) rc = hm_cuda_fail(e,"min_count");
     }
   if (rc == HM_OK)
-    *trim = (h_min >= ethresh);
-
-  *symm = 1;
+    { *trim = (h_min >= ethresh);
+      *symm = 1;
+    }
   const int psh = 64 - 8*s->ibyte;                    /* the stub index is over the first ibyte bytes */
   for (int64_t sidx = 1; sidx < n && rc == HM_OK; sidx++)
     { uint64_t x, xw = 0, q[2];
       int64_t  pos = -1;
-      if ((rc = load_into(s,D,t,d_index,sidx,1,keys,klo,cnt,0,&G)) != HM_OK) break;
-      e = cudaMemcpy(&x,keys,sizeof(uint64_t),cudaMemcpyDeviceToHost);
-      if (e == cudaSuccess && two) e = cudaMemcpy(&xw,klo,sizeof(uint64_t),cudaMemcpyDeviceToHost);
+      if ((rc = window_load(s,&W,sidx,1)) != HM_OK) break;
+      e = cudaMemcpy(&x,W.keys,sizeof(uint64_t),cudaMemcpyDeviceToHost);
+      if (e == cudaSuccess && two) e = cudaMemcpy(&xw,W.klo,sizeof(uint64_t),cudaMemcpyDeviceToHost);
       if (e != cudaSuccess) { rc = hm_cuda_fail(e,"examine: key fetch"); break; }
       if (two) revcomp128(x,xw,s->kmer,q,q+1);
       else     { q[0] = revcomp64(x,s->kmer); q[1] = 0; }
       uint64_t p  = q[0] >> psh;
       int64_t  b0 = p > 0 ? t->index[p-1] : 0, b1 = t->index[p];
-      HM_CUDA(cudaMemcpy(d_q,q,2*sizeof(uint64_t),cudaMemcpyHostToDevice));
+      if ((e = cudaMemcpy(d_q,q,2*sizeof(uint64_t),cudaMemcpyHostToDevice)) != cudaSuccess)
+        { rc = hm_cuda_fail(e,"examine: key upload"); break; }
       for (int64_t o = b0; o < b1 && rc == HM_OK && pos < 0; o += cap)
         { int64_t m = b1-o < cap ? b1-o : cap;
-          rc = load_into(s,D,t,d_index,o,m,keys,klo,cnt,0,&G);
-          if (rc == HM_OK) rc = hm_k_build_bucket_index(keys,m,bits,bucket,0,D->st);
-          if (rc == HM_OK) rc = hm_k_find_keys(keys,klo,m,bucket,bits,0,d_q,two ? d_q+1 : NULL,1,d_pos,D->st);
+          rc = window_load(s,&W,o,m);
+          if (rc == HM_OK) rc = hm_k_build_bucket_index(W.keys,m,bits,bucket,0,D->st);
+          if (rc == HM_OK) rc = hm_k_find_keys(W.keys,W.klo,m,bucket,bits,0,d_q,two ? d_q+1 : NULL,1,d_pos,D->st);
           s->launches += 2;
           if (rc != HM_OK) break;
           e = cudaMemcpyAsync(&pos,d_pos,sizeof(int64_t),cudaMemcpyDeviceToHost,D->st);
@@ -1834,48 +1772,56 @@ static int examine_streamed(hm_scan *s, int ethresh, int *trim, int *symm)
       if (pos < 0) { *symm = 0; break; }
       if (pos != sidx) { *symm = 1; break; }
     }
-  stager_close(D,&G);
-  cudaFree(keys); cudaFree(klo); cudaFree(cnt); cudaFree(bucket); cudaFree(d_index);
-  cudaFree(d_min); cudaFree(d_q); cudaFree(d_pos);
+  dev_free(D,bucket); dev_free(D,d_min); dev_free(D,d_q); dev_free(D,d_pos);
+  window_close(s,&W);
   return rc;
 }
 
 extern "C" int hm_scan_is_symmetric(const hm_scan *s) { return s->symmetric; }
 
-extern "C" int hm_scan_run_path(hm_scan *s, int path, int64_t *plot, hm_scan_stats *stats)
-{ if (s->invalid)
-    return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
-  if (path == HM_PATH_AUTO)
+/* The scan a run or an extraction takes: HETMERS_PATH (direct / symm) stands in for HM_PATH_AUTO, which takes the
+ * symmetric scan on a strand-symmetric table and the direct passes on any other.  *symm: the route; *forced: the
+ * symmetric scan was asked for, so it may not fall back to the direct passes.                                  */
+static int choose_route(const hm_scan *s, int path, int *symm, int *forced)
+{ if (path == HM_PATH_AUTO)
     { const char *e = getenv("HETMERS_PATH");
       if (e != NULL && strcmp(e,"direct") == 0) path = HM_PATH_DIRECT;
       if (e != NULL && strcmp(e,"symm") == 0)   path = HM_PATH_SYMM;
     }
-  if (s->streamed)
-    { if (path == HM_PATH_DIRECT)
-        return hm_set_error(HM_EUNSUPPORTED,"the direct passes need the table resident; this one does not fit in "
-                                            "device memory (budget %lld bytes) and is streamed",(long long) s->budget);
-      if (path != HM_PATH_AUTO && path != HM_PATH_SYMM)
-        return hm_set_error(HM_EINVAL,"hm_scan_run_path: unknown path %d",path);
-      return run_stream(s,plot,stats);
-    }
-  if (path == HM_PATH_DIRECT || (path == HM_PATH_AUTO && !s->symmetric))
-    return run_direct(s,plot,stats);
-  if (path != HM_PATH_AUTO && path != HM_PATH_SYMM)
+  if (s->streamed && path == HM_PATH_DIRECT)
+    return hm_set_error(HM_EUNSUPPORTED,"the direct passes need the table resident; this one does not fit in "
+                                        "device memory (budget %lld bytes) and is streamed",(long long) s->budget);
+  if (path != HM_PATH_AUTO && path != HM_PATH_DIRECT && path != HM_PATH_SYMM)
     return hm_set_error(HM_EINVAL,"hm_scan_run_path: unknown path %d",path);
-  if (s->kmer < HM_SYMM_MIN_KMER || (path == HM_PATH_SYMM && !s->symmetric))
+  *forced = (path == HM_PATH_SYMM);
+  *symm = s->streamed || path == HM_PATH_SYMM || (path == HM_PATH_AUTO && s->symmetric);
+  if (!s->streamed && *symm && (s->kmer < HM_SYMM_MIN_KMER || !s->symmetric))
     return hm_set_error(HM_EINVAL,"the table is not strand-symmetric (or k < %d): the symmetric scan "
                                   "would not give the reference's answer",HM_SYMM_MIN_KMER);
-  uint64_t status = 0;
-  int rc = run_symm(s,plot,stats,&status);
-  if (rc != HM_OK)
-    return rc;
-  if (status == 0)
-    return HM_OK;
-  /* the fingerprint was fooled (2^-128) or a cut missed a run boundary: the direct passes are
-   * always right                                                                                */
-  if (path == HM_PATH_SYMM)
+  return HM_OK;
+}
+
+/* a symmetric run or listing whose status word is not 0: the fingerprint was fooled (2^-128) or a cut missed a run
+ * boundary.  The direct passes are always right: HM_OK to fall back to them, unless the symmetric scan was forced */
+static int symm_failed(hm_scan *s, int forced, uint64_t status)
+{ if (forced)
     return hm_set_error(HM_EINVAL,"symmetric scan failed its own checks (status %llu)",(unsigned long long) status);
-  s->symmetric = 0;
+  s->symmetric = 0; s->symm_ready = 0;
+  return HM_OK;
+}
+
+extern "C" int hm_scan_run_path(hm_scan *s, int path, int64_t *plot, hm_scan_stats *stats)
+{ int symm = 0, forced = 0, rc;
+  uint64_t status = 0;
+  if (s->invalid)
+    return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
+  if ((rc = choose_route(s,path,&symm,&forced)) != HM_OK)
+    return rc;
+  if (s->streamed)
+    return run_stream(s,plot,stats);
+  if (symm && ((rc = run_symm(s,plot,stats,&status)) != HM_OK || status == 0 ||
+               (rc = symm_failed(s,forced,status)) != HM_OK))
+    return rc;
   return run_direct(s,plot,stats);
 }
 
@@ -1952,45 +1898,46 @@ static int extract_direct(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out,
   hm_pair_rec *d_out[HM_MAX_GPUS];
   uint16_t    *d_pix[HM_MAX_GPUS];
   unsigned long long *d_cnt[HM_MAX_GPUS];
+  cudaError_t  e;
   memset(d_out,0,sizeof(d_out)); memset(d_pix,0,sizeof(d_pix)); memset(d_cnt,0,sizeof(d_cnt));
   for (int pass = 0; pass < 2 && rc == HM_OK; pass++)
     { for (int g = 0; g < G && rc == HM_OK; g++)
         { DevTable *D = s->d+g;
-          HM_CUDA(cudaSetDevice(D->dev));
+          TRY(cudaSetDevice(D->dev));
           if (pass == 0)
-            { HM_CUDA(cudaMalloc(&d_pix[g],sizeof(uint16_t)*HM_PLOT_CELLS));
-              HM_CUDA(cudaMalloc(&d_cnt[g],sizeof(unsigned long long)));
-              HM_CUDA(cudaMemcpyAsync(d_pix[g],pixmap,sizeof(uint16_t)*HM_PLOT_CELLS,cudaMemcpyHostToDevice,D->st));
+            { TRY(dev_alloc(D,&d_pix[g],sizeof(uint16_t)*HM_PLOT_CELLS));
+              TRY(dev_alloc(D,&d_cnt[g],sizeof(unsigned long long)));
+              TRY(cudaMemcpyAsync(d_pix[g],pixmap,sizeof(uint16_t)*HM_PLOT_CELLS,cudaMemcpyHostToDevice,D->st));
             }
           else if (cnts[g] > 0)
-            HM_CUDA(cudaMalloc(&d_out[g],sizeof(hm_pair_rec)*(size_t) cnts[g]));
-          HM_CUDA(cudaMemsetAsync(d_cnt[g],0,sizeof(unsigned long long),D->st));
-          rc = hm_k_pass2_extract(D->keys,D->keys_lo,D->cnt,D->deg,D->up,s->idx64,D->lo,D->hi,d_pix[g],
-                                  d_out[g],pass == 0 ? 0 : cnts[g],d_cnt[g],s->peer_mode ? &s->sh[g] : NULL,D->st);
-          s->launches += (D->hi > D->lo);
+            TRY(dev_alloc(D,&d_out[g],sizeof(hm_pair_rec)*cnts[g]));
+          TRY(cudaMemsetAsync(d_cnt[g],0,sizeof(unsigned long long),D->st));
+          if (rc == HM_OK)
+            { rc = hm_k_pass2_extract(D->keys,D->keys_lo,D->cnt,D->deg,D->up,s->idx64,D->lo,D->hi,d_pix[g],
+                                      d_out[g],pass == 0 ? 0 : cnts[g],d_cnt[g],s->peer_mode ? &s->sh[g] : NULL,D->st);
+              s->launches += (D->hi > D->lo);
+            }
         }
       for (int g = 0; g < G && rc == HM_OK; g++)
         { unsigned long long c = 0;
-          HM_CUDA(cudaSetDevice(s->d[g].dev));
-          HM_CUDA(cudaMemcpyAsync(&c,d_cnt[g],sizeof(c),cudaMemcpyDeviceToHost,s->d[g].st));
-          HM_CUDA(cudaStreamSynchronize(s->d[g].st));
+          TRY(cudaSetDevice(s->d[g].dev));
+          TRY(cudaMemcpyAsync(&c,d_cnt[g],sizeof(c),cudaMemcpyDeviceToHost,s->d[g].st));
+          TRY(cudaStreamSynchronize(s->d[g].st));
           if (pass == 0) { cnts[g] = (int64_t) c; total += cnts[g]; }
         }
     }
-  hm_pair_rec *host = (hm_pair_rec *) malloc(sizeof(hm_pair_rec)*(size_t) (total > 0 ? total : 1));
+  hm_pair_rec *host = rc == HM_OK ? (hm_pair_rec *) malloc(sizeof(hm_pair_rec)*(size_t) (total > 0 ? total : 1)) : NULL;
   if (host == NULL && rc == HM_OK)
     rc = hm_set_error(HM_ENOMEM,"out of host memory for %lld pair records",(long long) total);
   int64_t at = 0;
   for (int g = 0; g < G; g++)
-    { cudaSetDevice(s->d[g].dev);
+    { DevTable *D = s->d+g;
+      cudaSetDevice(D->dev);
       if (rc == HM_OK && cnts[g] > 0)
-        { cudaError_t e = cudaMemcpy(host+at,d_out[g],sizeof(hm_pair_rec)*(size_t) cnts[g],cudaMemcpyDeviceToHost);
-          if (e != cudaSuccess) rc = hm_cuda_fail(e,"cudaMemcpy(pair records)");
+        { TRY(cudaMemcpy(host+at,d_out[g],sizeof(hm_pair_rec)*(size_t) cnts[g],cudaMemcpyDeviceToHost));
           at += cnts[g];
         }
-      if (d_out[g]) cudaFree(d_out[g]);
-      if (d_pix[g]) cudaFree(d_pix[g]);
-      if (d_cnt[g]) cudaFree(d_cnt[g]);
+      dev_free(D,d_out[g]); dev_free(D,d_pix[g]); dev_free(D,d_cnt[g]);
     }
   if (rc != HM_OK)
     { free(host); return rc; }
@@ -2005,22 +1952,15 @@ static int extract_direct(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out,
  * status words afterwards (non-zero: the list must not be used).                                            */
 static int extract_symm(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out, uint64_t *status)
 { int     G = s->ngpu, rc = HM_OK;
-  int64_t held = incore_bytes(s->n,s->kmer,G,s->bits,s->idx64);    /* (conditioning may have grown the table) */
   int64_t nc[HM_MAX_GPUS], c0[HM_MAX_GPUS], slice[HM_MAX_GPUS];
-  if (held < s->incore_bytes) held = s->incore_bytes;
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
-      int64_t   direct = 0, room;
+      int64_t   room = s->budget - D->held;
       uint64_t  n_cand = 0;
-      if (D->deg != NULL)    direct += (s->n+4) & ~3ll;                /* the direct passes' buffers, if held */
-      if (D->up != NULL)     direct += (int64_t) (s->idx64 ? 8 : 4)*(D->hi-D->lo+1);
-      if (D->filter != NULL) direct += 4*hm_filter_words(s->fpos);
-      if (D->p2scratch != NULL) direct += D->p2scratch_bytes;
-      room = s->budget - held - direct;
       if (room < HM_EXTRACT_MIN_BYTES)
         return hm_set_error(HM_ENOMEM,"listing k-mer pairs needs at least %lld device bytes beside the scan's %lld on "
                             "GPU %d, but the device budget of %lld bytes leaves %lld",(long long) HM_EXTRACT_MIN_BYTES,
-                            (long long) (held+direct),D->dev,(long long) s->budget,(long long) (room > 0 ? room : 0));
+                            (long long) D->held,D->dev,(long long) s->budget,(long long) (room > 0 ? room : 0));
       HM_CUDA(cudaSetDevice(D->dev));
       if ((rc = hm_symm_status(D->symm_work,&D->symm_layout,&n_cand,NULL,D->st)) != HM_OK)
         return rc;
@@ -2038,13 +1978,11 @@ static int extract_symm(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, i
   for (int g = 0; g < G && rc == HM_OK; g++)
     { DevTable *D = s->d+g;
       cudaError_t e;
-#define TRY(call) if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call)
       TRY(cudaSetDevice(D->dev));
-      TRY(dalloc(D->dev,D->st,(void **) &d_pix[g],sizeof(uint16_t)*HM_PLOT_CELLS));
-      TRY(dalloc(D->dev,D->st,(void **) &d_cnt[g],256));
-      TRY(dalloc(D->dev,D->st,(void **) &d_out[g],sizeof(hm_pair_rec)*(size_t) (2*slice[g])));
+      TRY(dev_alloc(D,&d_pix[g],sizeof(uint16_t)*HM_PLOT_CELLS));
+      TRY(dev_alloc(D,&d_cnt[g],256));
+      TRY(dev_alloc(D,&d_out[g],sizeof(hm_pair_rec)*(2*slice[g])));
       TRY(cudaMemcpyAsync(d_pix[g],pixmap,sizeof(uint16_t)*HM_PLOT_CELLS,cudaMemcpyHostToDevice,D->st));
-#undef TRY
     }
   for (int more = 1; more && rc == HM_OK; )
     { int64_t c1[HM_MAX_GPUS];
@@ -2102,7 +2040,7 @@ static int extract_symm(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, i
         { rc = hm_symm_status(D->symm_work,&D->symm_layout,NULL,&st,D->st);
           *status |= st;
         }
-      dfree(D->dev,D->st,d_out[g]); dfree(D->dev,D->st,d_pix[g]); dfree(D->dev,D->st,d_cnt[g]);
+      dev_free(D,d_out[g]); dev_free(D,d_pix[g]); dev_free(D,d_cnt[g]);
     }
   if (rc == HM_OK && host == NULL && (host = (hm_pair_rec *) malloc(sizeof(hm_pair_rec))) == NULL)
     rc = hm_set_error(HM_ENOMEM,"out of host memory");
@@ -2117,19 +2055,14 @@ static int extract_symm(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, i
  * the work areas do not hold a clean one), the direct one the direct passes' results; a symmetric run that fails
  * its own checks falls back to the direct route, as a run does.                                                */
 extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out)
-{ int rc = HM_OK, path = HM_PATH_AUTO;
+{ int rc, symm = 0, forced = 0;
   if (s->streamed)
     return hm_set_error(HM_EUNSUPPORTED,"listing k-mer pairs needs the direct passes' arrays, and this table does not "
                                         "fit in device memory (budget %lld bytes)",(long long) s->budget);
   if (s->invalid)
     return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
-  const char *e = getenv("HETMERS_PATH");
-  if (e != NULL && strcmp(e,"direct") == 0) path = HM_PATH_DIRECT;
-  if (e != NULL && strcmp(e,"symm") == 0)   path = HM_PATH_SYMM;
-  if (path == HM_PATH_SYMM && (s->kmer < HM_SYMM_MIN_KMER || !s->symmetric))
-    return hm_set_error(HM_EINVAL,"the table is not strand-symmetric (or k < %d): the symmetric scan "
-                                  "would not give the reference's answer",HM_SYMM_MIN_KMER);
-  int symm = (path == HM_PATH_SYMM || (path == HM_PATH_AUTO && s->symmetric && s->kmer >= HM_SYMM_MIN_KMER));
+  if ((rc = choose_route(s,HM_PATH_AUTO,&symm,&forced)) != HM_OK)
+    return rc;
   hm_pair_rec *host = NULL;
   int64_t      total = 0;
   if (symm)
@@ -2149,11 +2082,9 @@ extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec *
           if (status != 0)
             { free(host); host = NULL; total = 0; }
         }
-      if (status != 0)                /* the fingerprint was fooled: the direct passes are always right */
-        { if (path == HM_PATH_SYMM)
-            return hm_set_error(HM_EINVAL,"symmetric scan failed its own checks (status %llu)",
-                                (unsigned long long) status);
-          s->symmetric = 0; s->symm_ready = 0;
+      if (status != 0)
+        { if ((rc = symm_failed(s,forced,status)) != HM_OK)
+            return rc;
           symm = 0;
         }
     }
