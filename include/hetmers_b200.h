@@ -363,6 +363,40 @@ int  hm_stream_plan_shards(int64_t n, int kmer, int ibyte, int64_t budget, int n
  * over the shards (0 in core).  Either pointer may be NULL.                                           */
 int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks);
 
+/* ---- one rank of a one-process-per-GPU job streaming a strand-symmetric table (DESIGN.md §4c, *Ranks*) ----
+ * Rank `rank` of `world` streams its run-aligned share [c_rank, c_rank+1) (the cuts of the in-process shards)
+ * through `device` under the device budget; no rank holds the table, and no call reads another rank's memory.
+ * The caller runs the collectives between the calls (smudgeplot_b200/dist.py), in this order:
+ *   create (seed: the same fingerprint seeds on every rank) -> cuts (the same on every rank)
+ *   pass1 -> fingerprint sums summed over the ranks -> prepare(verdict) (an asymmetric table: HM_EUNSUPPORTED)
+ *   -> the Bloom segments all-gathered in place (bloom) -> slices(the smallest max_slice of all ranks, capped
+ *   by the largest candidate count) -> for every round up to the largest `rounds` of all ranks:
+ *   route (counts[q] = queries for rank q) -> the key words all-to-all'ed from send into recv (KW = 1 word per
+ *   query, 2 for k > 32) -> answer(keys received) -> the answers all-to-all'ed back from ans_recv into ans_sent
+ *   -> settle; then result -> the partial plots summed over the ranks.
+ * Device pointers are returned; they stay valid until the next pass1 or destroy.                          */
+typedef struct hm_rank_scan hm_rank_scan;
+int  hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
+                         hm_rank_scan **out);
+void hm_rank_scan_destroy(hm_rank_scan *r);
+/* cuts: int64[world+1]; first_keys (optional): uint64[world], word 0 of the first entry of each share */
+int  hm_rank_scan_cuts(const hm_rank_scan *r, int64_t *cuts, uint64_t *first_keys);
+/* fp: host uint64[4], the fingerprint sums of the entries this rank scanned */
+int  hm_rank_scan_pass1(hm_rank_scan *r, uint64_t *fp);
+/* world Bloom segments of seg_bytes each; segment q is rank q's */
+int  hm_rank_scan_bloom(const hm_rank_scan *r, void **d_segments, int64_t *seg_bytes);
+/* max_slice: the most candidates per round the budget leaves room for (HM_ENOMEM below 256) */
+int  hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_cand, int64_t *max_slice);
+int  hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send, void **d_recv,
+                         void **d_ans_recv, void **d_ans_sent);
+int  hm_rank_scan_route(hm_rank_scan *r, int64_t round, int64_t *counts);
+int  hm_rank_scan_answer(hm_rank_scan *r, int64_t n_received);
+int  hm_rank_scan_settle(hm_rank_scan *r);
+/* d_plot: device int64[HM_PLOT_CELLS], this rank's partial plot; status: non-zero = do not use the plot */
+int  hm_rank_scan_result(hm_rank_scan *r, void **d_plot, uint64_t *status);
+/* the most device bytes held since the last pass1 began, that pass's chunks, and the budget */
+int  hm_rank_scan_residency(const hm_rank_scan *r, int64_t *device_bytes, int64_t *chunks, int64_t *budget);
+
 /* one call: create + run + destroy (what bench.py's e2e leg times) */
 int  hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,
                      int64_t *plot, hm_scan_stats *stats);

@@ -60,6 +60,32 @@ int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int6
                            const hm_symm_shards *shards, const hm_stream_sview *d_views,
                            unsigned long long *d_plot, void *stream);
 
+/* routed pass 2 of one rank of a one-process-per-GPU job (hm_rank_scan_*): over candidate slices [c0, c1) of at
+ * most pend_cap candidates, resolve parks every candidate with a Bloom hit on a key another rank owns (pend, one
+ * meta each) and lists those keys as queries (q_key / q_lo / q_tag = owner << 32 | pending slot, 2 per candidate
+ * at most); route_group sorts them by owner into send (KW words per query) and send_slot; counts: device
+ * uint64[2 * HM_MAX_SHARDS] scratch                                                                         */
+typedef struct hm_route_bufs
+  { uint64_t *pend;
+    int64_t   pend_cap;
+    uint64_t *q_key, *q_lo, *q_tag;
+    int64_t   q_cap;
+    uint64_t *send;
+    uint32_t *send_slot;
+    unsigned long long *counts;
+  } hm_route_bufs;
+
+int hm_symm_route_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
+                          const void *d_s_bucket, int bits, int idx64, int kmer, int64_t c0, int64_t c1,
+                          void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                          const hm_symm_shards *shards, const hm_route_bufs *B, unsigned long long *d_plot, void *stream);
+int hm_symm_route_group(int kmer, int world, void *d_work, const hm_symm_layout *L, const hm_route_bufs *B,
+                        int64_t *counts, int64_t *n_sent, int64_t *n_pend, uint64_t *status, void *stream);
+int hm_symm_route_answer(const uint64_t *d_s_key, const uint64_t *d_s_lo, const void *d_s_bucket, int bits,
+                         int idx64, int kmer, const uint64_t *d_recv, int64_t n, uint8_t *d_ans, void *stream);
+int hm_symm_route_settle(int kmer, const hm_route_bufs *B, const uint8_t *d_ans, int64_t n_sent, int64_t n_pend,
+                         unsigned long long *d_plot, void *stream);
+
 #include <cuda_runtime.h>
 int hm_cuda_fail(cudaError_t e, const char *what);
 /* sort n packed keys (two words for k > 32) in place, in scratch of hm_sort_keys_bytes (hm_condition.cu) */

@@ -14,7 +14,8 @@
  * fused into the two kernels; summed by a peer-memory kernel of hm_peer.cu if there are no
  * native NVLink atomics); the
  * one-process-per-GPU variant (torch.distributed / NCCL) lives in smudgeplot_b200/dist.py and
- * uses layer A directly.
+ * uses layer A directly; its streamed counterpart drives one rank's share through the hm_rank_scan_* calls
+ * at the end of this file.
  * A table whose in-core footprint exceeds the device budget is not loaded here: every run streams it
  * in run-aligned chunks (run_stream, DESIGN.md §4c), through one GPU or, sharded, each GPU its own
  * run-aligned share of the table.
@@ -85,6 +86,8 @@ struct hm_scan
     const hm_host_table *host;            /* (streamed) the caller's table, valid until hm_scan_destroy        */
     hm_stream_layout plan;                /* (streamed) per shard                                              */
     volatile int stop;                    /* (streamed) a shard failed: the others leave their chunk loops     */
+    int      nshard, rank;                /* (streamed) shards of the table, and the one d[0] streams: n_gpus and 0  */
+                                          /*   in one process, (world, rank) for one rank of a job (hm_rank_scan)  */
   };
 
 static double now_ms(void)
@@ -720,13 +723,14 @@ static int window_open(hm_scan *s, int64_t cap, Window *W)
 static int window_load(hm_scan *s, Window *W, int64_t first, int64_t count)
 { return load_into(s,s->d,s->host,W->d_index,first,count,W->keys,W->klo,W->cnt,0,&W->G); }
 
-/* Shard cuts of a streamed scan over G = s->ngpu shards, from the host table: c_r is the first run start (a run =
+/* Shard cuts of a streamed scan over G = s->nshard shards, from the host table: c_r is the first run start (a run =
  * the entries sharing their first k/2 bases) at or after n*r/G -- hm_symm_align_cut's rule -- found by loading
- * a few records at a time around each nominal cut on the first shard's device.  Sets every shard's range,
- * descriptor (first_key[r] = word 0 of entry c_r) and how many shards own keys: those up to the last non-empty
- * one (a run longer than a share can leave shards empty, in the middle or at the end).                   */
+ * a few records at a time around each nominal cut on the first device.  Sets the range and descriptor
+ * (first_key[r] = word 0 of entry c_r) of the shards this process streams (shard s->rank + g on d[g]) and how
+ * many shards own keys: those up to the last non-empty one (a run longer than a share can leave shards empty,
+ * in the middle or at the end).                                                                          */
 static int stream_cuts(hm_scan *s)
-{ int      G = s->ngpu, rc;
+{ int      G = s->nshard, rc;
   int64_t  n = s->n, cut[HM_MAX_GPUS+1];
   uint64_t first[HM_MAX_GPUS];
   const int64_t W = 4096;
@@ -762,15 +766,45 @@ static int stream_cuts(hm_scan *s)
   int live = 1;                                            /* shards up to the last non-empty one */
   for (int r = 1; r < G; r++)
     if (cut[r] < n) live = r+1;
-  for (int g = 0; g < G; g++)
+  for (int g = 0; g < s->ngpu; g++)
     { hm_symm_shards *sh = s->ssh+g;
       memset(sh,0,sizeof(*sh));
-      sh->n_seg = live; sh->self = g;
+      sh->n_seg = live; sh->self = s->rank+g;
       for (int r = 0; r <= G; r++) sh->off[r] = cut[r];
       for (int r = 0; r < G; r++)  sh->first_key[r] = first[r];
-      s->d[g].lo = cut[g]; s->d[g].hi = cut[g+1];
+      s->d[g].lo = cut[s->rank+g]; s->d[g].hi = cut[s->rank+g+1];
     }
   return HM_OK;
+}
+
+/* streamed: the plan of each of s->nshard shards under s->budget (HETMERS_STREAM_CHUNK: smaller chunks) */
+static int stream_setup(hm_scan *s, const hm_host_table *t)
+{ int rc = hm_stream_plan_shards(s->n,t->kmer,t->ibyte,s->budget,s->nshard,&s->plan);
+  if (rc != HM_OK)
+    return rc;
+  const char *cc = getenv("HETMERS_STREAM_CHUNK");         /* smaller chunks than the budget allows */
+  if (cc != NULL && atoll(cc) >= 1 && atoll(cc) < s->plan.chunk)
+    { s->plan.chunk = atoll(cc);
+      s->plan.chunk_bytes = chunk_bytes(s->plan.chunk,t->kmer,t->ibyte);
+      s->plan.chunk_list_bytes = chunk_list_bytes(s->plan.chunk,t->kmer);
+      s->plan.list_bytes = s->budget - s->plan.fixed_bytes - s->plan.chunk_bytes;
+    }
+  s->streamed = 1; s->host = t;
+  return HM_OK;
+}
+
+/* a device's streams and timing events; its allocations come from the pool if `pool` */
+static int open_device(DevTable *D, int dev, int pool)
+{ int rc = HM_OK;
+  cudaError_t e;
+  D->dev = dev;
+  TRY(cudaSetDevice(D->dev));
+  D->pool = pool_setup(D->dev,pool);
+  TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
+  TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
+  for (int k = 0; k < 4; k++)
+    TRY(cudaEventCreate(&D->ev[k]));
+  return rc;
 }
 
 extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out)
@@ -790,7 +824,7 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   hm_scan *s = (hm_scan *) calloc(1,sizeof(hm_scan));
   if (s == NULL)
     return hm_set_error(HM_ENOMEM,"out of host memory");
-  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = t->nels; s->ngpu = n_gpus;
+  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = t->nels; s->ngpu = n_gpus; s->nshard = n_gpus;
   s->bits  = hm_pick_bucket_bits(s->n);
   s->fpos  = hm_pick_filter_bits(s->n);
   s->idx64 = (s->n >= 0xFFFFFFF0ll);
@@ -805,16 +839,8 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   if (s->incore_bytes > s->budget || (force != NULL && strcmp(force,"1") == 0))
     { /* streamed: only the plot and the fingerprint sums are allocated now; the table stays on the host.
        * Several GPUs: shard r streams its run-aligned share [c_r, c_r+1) through dev[r] (DESIGN.md §4c) */
-      if ((rc = hm_stream_plan_shards(n,t->kmer,t->ibyte,s->budget,n_gpus,&s->plan)) != HM_OK)
+      if ((rc = stream_setup(s,t)) != HM_OK)
         { free(s); return rc; }
-      const char *cc = getenv("HETMERS_STREAM_CHUNK");         /* smaller chunks than the budget allows */
-      if (cc != NULL && atoll(cc) >= 1 && atoll(cc) < s->plan.chunk)
-        { s->plan.chunk = atoll(cc);
-          s->plan.chunk_bytes = chunk_bytes(s->plan.chunk,t->kmer,t->ibyte);
-          s->plan.chunk_list_bytes = chunk_list_bytes(s->plan.chunk,t->kmer);
-          s->plan.list_bytes = s->budget - s->plan.fixed_bytes - s->plan.chunk_bytes;
-        }
-      s->streamed = 1; s->host = t;
     }
   else
     for (int g = 0; g < n_gpus; g++)
@@ -833,15 +859,9 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   for (int g = 0; g < n_gpus && rc == HM_OK; g++)
     { DevTable *D = s->d+g;
       cudaError_t e;
-      D->dev = dev ? dev[g] : g;
       D->lo  = s->streamed ? 0 : n*g/n_gpus;
       D->hi  = s->streamed ? n : n*(g+1)/n_gpus;
-      TRY(cudaSetDevice(D->dev));
-      D->pool = pool_setup(D->dev,n_gpus == 1);
-      TRY(cudaStreamCreateWithFlags(&D->st,cudaStreamNonBlocking));
-      TRY(cudaStreamCreateWithFlags(&D->st_copy,cudaStreamNonBlocking));
-      for (int k = 0; k < 4; k++)
-        TRY(cudaEventCreate(&D->ev[k]));
+      rc = open_device(D,dev ? dev[g] : g,n_gpus == 1);
       if (!s->streamed)
         { TRY(dev_alloc(D,&D->keys,sizeof(uint64_t)*(n+1)));
           if (t->kmer > 32)
@@ -1445,7 +1465,7 @@ static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[
                         "of %lld bytes has room for %lld more while %lld bytes are held; give the scan a larger "
                         "budget (HETMERS_DEVICE_BUDGET)%s",what,(long long) need,(long long) (8*narr*need),
                         (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) D->held,
-                        s->ngpu > 1 ? "" : " or more GPUs (HETMERS_GPUS)");
+                        s->nshard > 1 ? "" : " or more GPUs (HETMERS_GPUS)");
   for (int a = 0; a < narr; a++)
     { uint64_t *p = NULL;
       cudaError_t e = dev_alloc(D,&p,8*nc);
@@ -1529,13 +1549,13 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shar
 static int shard_pass1(hm_scan *s, int g, void *arg)
 { DevTable  *D = s->d+g;
   StreamRun *R = (StreamRun *) arg + g;
-  const hm_symm_shards *sh = s->ngpu > 1 ? s->ssh+g : NULL;
+  const hm_symm_shards *sh = s->nshard > 1 ? s->ssh+g : NULL;
   int64_t ixlen = (int64_t) 1 << (8*s->ibyte);
   int     rc;
   cudaError_t e;
   HM_CUDA(cudaSetDevice(D->dev));
   HM_CUDA(cudaStreamCreateWithFlags(&R->sc,cudaStreamNonBlocking));
-  if ((rc = stream_work_layout(s->n,s->kmer,s->ngpu,&R->L)) != HM_OK) return rc;
+  if ((rc = stream_work_layout(s->n,s->kmer,s->nshard,&R->L)) != HM_OK) return rc;
   if ((e = dev_alloc(D,&R->d_index,8*ixlen)) != cudaSuccess ||
       (e = dev_alloc(D,&R->work,R->L.bytes)) != cudaSuccess)
     return hm_cuda_fail(e,"streamed scan: work area");
@@ -1557,6 +1577,50 @@ static int shard_pass1(hm_scan *s, int g, void *arg)
   return HM_OK;
 }
 
+static int refuse_asymmetric(const hm_scan *s)
+{ return hm_set_error(HM_EUNSUPPORTED,"the table of %lld entries does not fit in device memory (budget %lld bytes) and "
+                      "is not strand-symmetric; the direct passes need it resident",(long long) s->n,(long long) s->budget);
+}
+
+/* after pass 1: the chunk buffers and stub index of shard g freed, and its S list (sorted chunk by chunk) given a
+ * bucket index in the room they leave: as fine as hm_pick_bucket_bits asks, coarser if the budget says so
+ * (look-ups then bisect longer buckets).  zero: clear the index first (an empty S list: all offsets 0).      */
+static int stream_s_index(hm_scan *s, int g, StreamRun *R, uint64_t ns, int sidx64, int zero, int *sbits)
+{ DevTable *D = s->d+g;
+  cudaError_t e;
+  HM_CUDA(cudaSetDevice(D->dev));
+  stream_free_chunks(D,R);
+  dev_free(D,R->d_index); R->d_index = NULL;
+  int bits = hm_pick_bucket_bits((int64_t) ns);
+  while (bits > 1 && D->held + (int64_t) (sidx64 ? 8 : 4)*((1ll << bits)+1) > s->budget)
+    bits -= 1;
+  int64_t s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << bits)+1);
+  if ((e = dev_alloc(D,&R->s_bucket,s_bucket_bytes)) != cudaSuccess)
+    return hm_cuda_fail(e,"streamed scan: S index");
+  if (zero)
+    HM_CUDA(cudaMemsetAsync(R->s_bucket,0,(size_t) s_bucket_bytes,R->sc));
+  *sbits = bits;
+  if (!zero || ns > 0)
+    return hm_k_build_bucket_index(R->R.s_key,(int64_t) ns,bits,R->s_bucket,sidx64,R->sc);
+  return HM_OK;
+}
+
+/* everything a streamed run allocated on shard g (its thread has been joined) */
+static void stream_release(hm_scan *s, int g, StreamRun *R)
+{ DevTable *D = s->d+g;
+  cudaSetDevice(D->dev);
+  stream_free_chunks(D,R);
+  dev_free(D,R->d_index);  dev_free(D,R->work);
+  dev_free(D,R->s_bucket); dev_free(D,R->views);
+  dev_free(D,R->R.cand_key); dev_free(D,R->R.cand_meta); dev_free(D,R->R.cand_lo);
+  dev_free(D,R->R.s_key);    dev_free(D,R->R.s_lo);
+  if (D->st) cudaStreamSynchronize(D->st);
+  if (R->sc) cudaStreamDestroy(R->sc);
+  cudaCtxResetPersistingL2Cache();
+  cudaGetLastError();
+  memset(R,0,sizeof(*R));
+}
+
 /* Pass 1 of every shard at once; the verdict over all shards' fingerprints; the Bloom segments all-gathered; the
  * chunk buffers and stub index freed, to make room for each shard's S index; pass 2 of every shard, whose exact
  * checks look keys up in the S list of their owner (peer memory); the plots summed on the host.              */
@@ -1574,8 +1638,7 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
   double t_pass1 = now_ms();
   if ((rc = fingerprint_verdict(s)) != HM_OK) return rc;
   if (!s->symmetric)
-    return hm_set_error(HM_EUNSUPPORTED,"the table of %lld entries does not fit in device memory (budget %lld bytes) and "
-                        "is not strand-symmetric; the direct passes need it resident",(long long) s->n,(long long) s->budget);
+    return refuse_asymmetric(s);
 
   uint64_t ns[HM_MAX_GPUS];
   int      sbits[HM_MAX_GPUS], sidx64 = 0;
@@ -1592,26 +1655,9 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
       if ((rc = gather_bloom(s,work,&RR[0].L,st,1)) != HM_OK)
         return rc;
     }
-  /* S (sorted chunk by chunk) gets a bucket index in the room the chunk buffers leave: as fine as
-   * hm_pick_bucket_bits asks, coarser if the budget says so (look-ups then bisect longer buckets)        */
   for (int g = 0; g < G; g++)
-    { DevTable  *D = s->d+g;
-      StreamRun *R = RR+g;
-      HM_CUDA(cudaSetDevice(D->dev));
-      stream_free_chunks(D,R);
-      dev_free(D,R->d_index); R->d_index = NULL;
-      sbits[g] = hm_pick_bucket_bits((int64_t) ns[g]);
-      while (sbits[g] > 1 && D->held + (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1) > s->budget)
-        sbits[g] -= 1;
-      int64_t s_bucket_bytes = (int64_t) (sidx64 ? 8 : 4)*((1ll << sbits[g])+1);
-      if ((e = dev_alloc(D,&R->s_bucket,s_bucket_bytes)) != cudaSuccess)
-        return hm_cuda_fail(e,"streamed scan: S index");
-      if (G > 1)
-        HM_CUDA(cudaMemsetAsync(R->s_bucket,0,(size_t) s_bucket_bytes,R->sc));   /* (an empty S list: all 0) */
-      if ((G == 1 || ns[g] > 0) &&
-          (rc = hm_k_build_bucket_index(R->R.s_key,(int64_t) ns[g],sbits[g],R->s_bucket,sidx64,R->sc)) != HM_OK)
-        return rc;
-    }
+    if ((rc = stream_s_index(s,g,RR+g,ns[g],sidx64,G > 1,&sbits[g])) != HM_OK)
+      return rc;
   if (G > 1)                                    /* each shard's pass 2 reads every shard's S view */
     { hm_stream_sview V[HM_MAX_GPUS];
       memset(V,0,sizeof(V));
@@ -1687,18 +1733,7 @@ static int run_stream(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
     }
   int rc = run_stream_body(s,R,plot,stats);
   for (int g = 0; g < G; g++)                  /* every shard's thread has been joined: free it all */
-    { DevTable *D = s->d+g;
-      cudaSetDevice(D->dev);
-      stream_free_chunks(D,R+g);
-      dev_free(D,R[g].d_index);  dev_free(D,R[g].work);
-      dev_free(D,R[g].s_bucket); dev_free(D,R[g].views);
-      dev_free(D,R[g].R.cand_key); dev_free(D,R[g].R.cand_meta); dev_free(D,R[g].R.cand_lo);
-      dev_free(D,R[g].R.s_key);    dev_free(D,R[g].R.s_lo);
-      if (D->st) cudaStreamSynchronize(D->st);
-      if (R[g].sc) cudaStreamDestroy(R[g].sc);
-      cudaCtxResetPersistingL2Cache();
-      cudaGetLastError();
-    }
+    stream_release(s,g,R+g);
   return rc;
 }
 
@@ -2130,5 +2165,284 @@ extern "C" int hm_scan_download(hm_scan *s, uint64_t *keys, uint64_t *keys_lo, u
         if (O->hi > O->lo)
           HM_CUDA(cudaMemcpy(deg+O->lo,O->deg+O->lo,(size_t) (O->hi-O->lo),cudaMemcpyDeviceToHost));
       }
+  return HM_OK;
+}
+
+/* ---- one rank of a one-process-per-GPU job (DESIGN.md §4c, *Ranks*) ---------------------------------------
+ * The rank streams its run-aligned share [c_rank, c_rank+1) through one device with the chunk loop of the
+ * in-process shards (shard_pass1), and settles pass 2 without reading another rank's memory: the caller runs
+ * the collectives between the calls (smudgeplot_b200/dist.py).                                              */
+#define ROUTE_MIN_SLICE 256
+
+struct hm_rank_scan
+  { hm_scan      *s;                         /* one device (d[0]), s->nshard = world, s->rank = rank          */
+    StreamRun     R;
+    int           stage;                     /* 0 created, 1 pass 1 done, 2 pass 2 prepared, 3 buffers sized  */
+    uint64_t      ns;                        /* S keys of this rank                                          */
+    int           sbits, sidx64;
+    int64_t       ncand, slice, rounds;
+    hm_route_bufs B;
+    uint64_t     *recv;                      /* keys that arrive: (world-1) * 2 * slice queries at most       */
+    uint8_t      *ans_recv, *ans_sent;       /* answers to them / to this rank's queries                     */
+    int64_t       n_sent, n_pend;            /* of the last round                                            */
+    uint64_t      status;                    /* OR of the status words seen since pass 1                     */
+  };
+
+static void rank_free_route(hm_rank_scan *r)
+{ DevTable *D = r->s->d;
+  cudaSetDevice(D->dev);
+  dev_free(D,r->B.pend); dev_free(D,r->B.q_key); dev_free(D,r->B.q_lo); dev_free(D,r->B.q_tag);
+  dev_free(D,r->B.send); dev_free(D,r->B.send_slot); dev_free(D,r->B.counts);
+  dev_free(D,r->recv); dev_free(D,r->ans_recv); dev_free(D,r->ans_sent);
+  memset(&r->B,0,sizeof(r->B));
+  r->recv = NULL; r->ans_recv = NULL; r->ans_sent = NULL;
+}
+
+/* device bytes of the route buffers for slices of `slice` candidates */
+static int64_t route_bytes(int64_t slice, int kmer, int world)
+{ int64_t KW = kmer > 32 ? 2 : 1, q = 2*slice, o = world-1;
+  return 8*slice + q*(8*KW+8+(KW == 2 ? 8 : 0)) + q*(8*KW+4) + o*q*8*KW + o*q + q + 16*HM_MAX_SHARDS + 10*256;
+}
+
+extern "C" void hm_rank_scan_destroy(hm_rank_scan *r)
+{ if (r == NULL)
+    return;
+  if (r->s != NULL)
+    { rank_free_route(r);
+      stream_release(r->s,0,&r->R);
+      hm_scan_destroy(r->s);
+    }
+  free(r);
+}
+
+extern "C" int hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
+                                   hm_rank_scan **out)
+{ if (t == NULL || out == NULL || seed == NULL || world < 1 || world > HM_MAX_GPUS || rank < 0 || rank >= world ||
+      device < 0)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_create: bad arguments");
+  if (t->kmer < HM_SYMM_MIN_KMER || t->kmer > HM_MAX_KMER)
+    return hm_set_error(HM_EUNSUPPORTED,"the table does not fit in device memory and k = %d has no strand-symmetric "
+                        "scan; the direct passes need it resident",t->kmer);
+  if (t->ibyte < 1 || t->ibyte > 3 || t->ibyte > ((t->kmer+3)>>2))
+    return hm_set_error(HM_EFORMAT,"table has ibyte=%d with k=%d",t->ibyte,t->kmer);
+  prewarm_join();
+  if (hm_device_count() <= device)
+    return hm_set_error(HM_ECUDA,"CUDA device %d is not visible (this build has no CPU fallback)",device);
+  hm_rank_scan *r = (hm_rank_scan *) calloc(1,sizeof(hm_rank_scan));
+  hm_scan      *s = (hm_scan *) calloc(1,sizeof(hm_scan));
+  if (r == NULL || s == NULL)
+    { free(r); free(s); return hm_set_error(HM_ENOMEM,"out of host memory"); }
+  r->s = s;
+  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = t->nels; s->ngpu = 1; s->nshard = world; s->rank = rank;
+  s->bits = hm_pick_bucket_bits(s->n); s->fpos = hm_pick_filter_bits(s->n); s->idx64 = (s->n >= 0xFFFFFFF0ll);
+  s->seed[0] = seed[0]; s->seed[1] = seed[1];               /* the same on every rank: the sums are added */
+  s->budget = device_budget(&device,1);
+  s->incore_bytes = incore_bytes(s->n,t->kmer,1,s->bits,s->idx64);
+  int rc = stream_setup(s,t);
+  DevTable *D = s->d;
+  cudaError_t e;
+  if (rc == HM_OK) rc = open_device(D,device,1);
+  TRY(dev_alloc(D,&D->plot,sizeof(unsigned long long)*HM_PLOT_CELLS));
+  TRY(dev_alloc(D,&D->fp_acc,4*sizeof(uint64_t)));
+  D->lo = 0; D->hi = s->n;
+  if (rc == HM_OK && world > 1)
+    rc = stream_cuts(s);
+  if (rc != HM_OK)
+    { r->s = NULL; free(r);
+      hm_scan_destroy(s);
+      return rc;
+    }
+  *out = r;
+  return HM_OK;
+}
+
+/* cuts: int64[world+1], c_0 = 0 ... c_world = n; first_keys (optional): uint64[world], word 0 of entry c_r */
+extern "C" int hm_rank_scan_cuts(const hm_rank_scan *r, int64_t *cuts, uint64_t *first_keys)
+{ if (r == NULL || cuts == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_cuts: bad arguments");
+  const hm_scan *s = r->s;
+  for (int q = 0; q <= s->nshard; q++)
+    cuts[q] = s->nshard > 1 ? s->ssh[0].off[q] : (q == 0 ? 0 : s->n);
+  if (first_keys != NULL)
+    for (int q = 0; q < s->nshard; q++)
+      first_keys[q] = s->nshard > 1 ? s->ssh[0].first_key[q] : 0;
+  return HM_OK;
+}
+
+/* pass 1 over the rank's share; fp: host uint64[4], the fingerprint sums of the entries it scanned */
+extern "C" int hm_rank_scan_pass1(hm_rank_scan *r, uint64_t *fp)
+{ if (r == NULL || fp == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_pass1: bad arguments");
+  hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  rank_free_route(r);
+  stream_release(s,0,&r->R);
+  r->stage = 0; r->status = 0;
+  D->peak = D->held; D->chunks = 0; s->stop = 0;
+  int rc = shard_pass1(s,0,&r->R);
+  if (rc != HM_OK)
+    return rc;
+  uint64_t nc = 0, status = 0;
+  if ((rc = hm_symm_stream_counts(r->R.work,&r->R.L,&nc,&status,&r->ns,r->R.sc)) != HM_OK)
+    return rc;
+  HM_CUDA(cudaMemcpy(fp,D->fp_acc,4*sizeof(uint64_t),cudaMemcpyDeviceToHost));
+  r->ncand = (int64_t) nc;
+  r->stage = 1;
+  return HM_OK;
+}
+
+/* Bloom segments of the work area: segment q (seg_bytes each, world of them) is filled by rank q's pass 1 */
+extern "C" int hm_rank_scan_bloom(const hm_rank_scan *r, void **d_segments, int64_t *seg_bytes)
+{ if (r == NULL || r->stage < 1 || d_segments == NULL || seg_bytes == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_bloom: no pass 1 has run");
+  *d_segments = (uint8_t *) r->R.work + r->R.L.off_bloom;
+  *seg_bytes = 4*r->R.L.seg_words;
+  return HM_OK;
+}
+
+/* symmetric = the job-wide fingerprint verdict.  Frees the chunk buffers, indexes the S list and reports the
+ * rank's candidates and the largest slice its budget leaves room for (HM_ENOMEM below ROUTE_MIN_SLICE).     */
+extern "C" int hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_cand, int64_t *max_slice)
+{ if (r == NULL || r->stage != 1 || n_cand == NULL || max_slice == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_prepare: pass 1 first");
+  hm_scan *s = r->s;
+  s->symmetric = symmetric != 0;
+  if (!symmetric)
+    return refuse_asymmetric(s);
+  int rc;
+  r->sidx64 = ((int64_t) r->ns >= 0xFFFFFFF0ll);
+  if ((rc = stream_s_index(s,0,&r->R,r->ns,r->sidx64,1,&r->sbits)) != HM_OK)
+    return rc;
+  HM_CUDA(cudaStreamSynchronize(r->R.sc));
+  int64_t room = s->budget - s->d[0].held, lo = 0, hi = (int64_t) 1 << 31;
+  while (lo < hi)
+    { int64_t mid = lo + (hi-lo+1)/2;
+      if (route_bytes(mid,s->kmer,s->nshard) <= room) lo = mid;
+      else                                            hi = mid-1;
+    }
+  if (lo < ROUTE_MIN_SLICE)
+    return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes leaves %lld bytes beside the resident lists of this rank "
+                        "(%lld held), and pass 2's exchange buffers for a slice of %d candidates need %lld",
+                        (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) s->d[0].held,ROUTE_MIN_SLICE,
+                        (long long) route_bytes(ROUTE_MIN_SLICE,s->kmer,s->nshard));
+  *n_cand = r->ncand;
+  *max_slice = lo;
+  r->stage = 2;
+  return HM_OK;
+}
+
+/* slice: the same on every rank (at most every rank's max_slice).  Allocates the route buffers; *rounds = the
+ * slices this rank's candidates take.  The device buffers the caller's collectives read and write:
+ * send (uint64, KW words per query, grouped by owner), recv (the same for what arrives), ans_recv (a byte per
+ * key that arrived) and ans_sent (a byte per query sent, in send order).                                    */
+extern "C" int hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send, void **d_recv,
+                                   void **d_ans_recv, void **d_ans_sent)
+{ if (r == NULL || r->stage != 2 || slice < 1 || rounds == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_slices: bad arguments");
+  hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  int64_t   KW = s->kmer > 32 ? 2 : 1, q = 2*slice, o = s->nshard-1;
+  int       rc = HM_OK;
+  cudaError_t e;
+  if (D->held + route_bytes(slice,s->kmer,s->nshard) > s->budget)
+    return hm_set_error(HM_ENOMEM,"pass 2's exchange buffers for slices of %lld candidates need %lld bytes and the device "
+                        "budget of %lld bytes has room for %lld",(long long) slice,
+                        (long long) route_bytes(slice,s->kmer,s->nshard),(long long) s->budget,(long long) (s->budget-D->held));
+  rank_free_route(r);
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&r->B.pend,8*slice));
+  TRY(dev_alloc(D,&r->B.q_key,8*q));
+  if (KW == 2) TRY(dev_alloc(D,&r->B.q_lo,8*q));
+  TRY(dev_alloc(D,&r->B.q_tag,8*q));
+  TRY(dev_alloc(D,&r->B.send,8*KW*q));
+  TRY(dev_alloc(D,&r->B.send_slot,4*q));
+  TRY(dev_alloc(D,&r->B.counts,16*HM_MAX_SHARDS));
+  TRY(dev_alloc(D,&r->recv,8*KW*(o*q > 0 ? o*q : 1)));
+  TRY(dev_alloc(D,&r->ans_recv,o*q > 0 ? o*q : 1));
+  TRY(dev_alloc(D,&r->ans_sent,q));
+  if (rc != HM_OK)
+    { rank_free_route(r); return rc; }
+  r->B.pend_cap = slice; r->B.q_cap = q;
+  r->slice = slice;
+  r->rounds = (r->ncand + slice-1)/slice;
+  *rounds = r->rounds;
+  if (d_send)     *d_send = r->B.send;
+  if (d_recv)     *d_recv = r->recv;
+  if (d_ans_recv) *d_ans_recv = r->ans_recv;
+  if (d_ans_sent) *d_ans_sent = r->ans_sent;
+  r->stage = 3;
+  return HM_OK;
+}
+
+/* round `round`: resolve the slice [round*slice, ...) of this rank's candidates (none once they are done) and
+ * group its queries by owner; counts: int64[world], the queries for each rank, in the order of send       */
+extern "C" int hm_rank_scan_route(hm_rank_scan *r, int64_t round, int64_t *counts)
+{ if (r == NULL || r->stage != 3 || counts == NULL || round < 0)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_route: bad arguments");
+  hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  int64_t   c0 = round*r->slice < r->ncand ? round*r->slice : r->ncand;
+  int64_t   c1 = c0 + r->slice < r->ncand ? c0 + r->slice : r->ncand;
+  int       KW = s->kmer > 32 ? 2 : 1, rc;
+  uint64_t  status = 0;
+  HM_CUDA(cudaSetDevice(D->dev));
+  if (round == 0)
+    HM_CUDA(cudaEventRecord(D->ev[2],r->R.sc));
+  if ((rc = hm_symm_route_resolve(r->R.R.s_key,KW == 2 ? r->R.R.s_lo : NULL,(int64_t) r->ns,r->R.s_bucket,r->sbits,
+                                  r->sidx64,s->kmer,c0,c1,r->R.work,&r->R.L,&r->R.R,s->nshard > 1 ? s->ssh : NULL,&r->B,
+                                  D->plot,r->R.sc)) != HM_OK)
+    return rc;
+  __sync_fetch_and_add(&s->launches,(int64_t) (c1 > c0));
+  if ((rc = hm_symm_route_group(s->kmer,s->nshard,r->R.work,&r->R.L,&r->B,counts,&r->n_sent,&r->n_pend,&status,
+                                r->R.sc)) != HM_OK)
+    return rc;
+  r->status |= status;
+  return HM_OK;
+}
+
+/* the n keys that arrived in recv: one byte each into ans_recv (synchronises) */
+extern "C" int hm_rank_scan_answer(hm_rank_scan *r, int64_t n)
+{ hm_scan *s = r ? r->s : NULL;
+  if (r == NULL || r->stage != 3 || n < 0 || n > (s->nshard-1)*2*r->slice)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_answer: bad arguments");
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  return hm_symm_route_answer(r->R.R.s_key,s->kmer > 32 ? r->R.R.s_lo : NULL,r->R.s_bucket,r->sbits,r->sidx64,s->kmer,
+                              r->recv,n,r->ans_recv,r->R.sc);
+}
+
+/* ans_sent holds the answers to the round's queries: count the parked candidates none of whose keys was found */
+extern "C" int hm_rank_scan_settle(hm_rank_scan *r)
+{ if (r == NULL || r->stage != 3)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_settle: bad arguments");
+  hm_scan *s = r->s;
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  int rc = hm_symm_route_settle(s->kmer,&r->B,r->ans_sent,r->n_sent,r->n_pend,s->d[0].plot,r->R.sc);
+  __sync_fetch_and_add(&s->launches,2);
+  return rc;
+}
+
+/* after the last round: this rank's partial plot (device int64[HM_PLOT_CELLS]) and the OR of its status words */
+extern "C" int hm_rank_scan_result(hm_rank_scan *r, void **d_plot, uint64_t *status)
+{ if (r == NULL || r->stage != 3 || d_plot == NULL || status == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_result: bad arguments");
+  hm_scan *s = r->s;
+  uint64_t nc = 0, st = 0, ns = 0;
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  HM_CUDA(cudaEventRecord(s->d[0].ev[3],r->R.sc));
+  int rc = hm_symm_stream_counts(r->R.work,&r->R.L,&nc,&st,&ns,r->R.sc);     /* (synchronises) */
+  if (rc != HM_OK)
+    return rc;
+  *d_plot = s->d[0].plot;
+  *status = r->status | st;
+  return HM_OK;
+}
+
+/* the most device memory the rank held since its last pass 1 began, and that pass's chunks; *budget: the budget */
+extern "C" int hm_rank_scan_residency(const hm_rank_scan *r, int64_t *device_bytes, int64_t *chunks, int64_t *budget)
+{ if (r == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_residency: bad arguments");
+  if (device_bytes) *device_bytes = r->s->d[0].peak;
+  if (chunks)       *chunks = r->s->d[0].chunks;
+  if (budget)       *budget = r->s->budget;
   return HM_OK;
 }

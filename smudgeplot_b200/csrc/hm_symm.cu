@@ -1288,12 +1288,41 @@ __device__ __noinline__ bool has_upper_partner(const uint64_t *__restrict__ keys
   return (U > 0);
 }
 
+/* Routed pass 2 (one rank of a one-process-per-GPU job, DESIGN.md §4c): header words SY_HDR_R.. hold the pending
+ * count, the query count, the pending list (one meta per candidate), the query keys, their second words, their
+ * tags (owner << 32 | pending slot) and the two capacities.  A candidate with a Bloom hit on a key owned by
+ * another rank is parked there; every such key becomes a query to its owner.                                  */
+#define SY_HDR_R 8
+
+template <int KW>
+__device__ __noinline__ void route_push(const SymmView &W, uint64_t meta, bool fa, int oa, uint64_t rx, uint64_t rxl,
+                                        bool fb, int ob, uint64_t ry, uint64_t ryl)
+{ unsigned long long *h = W.cand_n + SY_HDR_R;
+  const unsigned long long nq = (fa ? 1ull : 0ull) + (fb ? 1ull : 0ull);
+  const unsigned long long slot = atomicAdd(h,1ull), q = atomicAdd(h+1,nq);
+  if (slot >= h[6] || q+nq > h[7])
+    { atomicOr(W.status,SY_STATUS_OVERFLOW); return; }
+  ((uint64_t *) h[2])[slot] = meta & ~(RV_HA | RV_HB);
+  uint64_t *qk = (uint64_t *) h[3], *ql = (uint64_t *) h[4], *qt = (uint64_t *) h[5];
+  unsigned long long at = q;
+  if (fa)
+    { qk[at] = rx; if (KW == 2) ql[at] = rxl;
+      qt[at] = ((uint64_t) oa << 32) | slot; at++;
+    }
+  if (fb)
+    { qk[at] = ry; if (KW == 2) ql[at] = ryl;
+      qt[at] = ((uint64_t) ob << 32) | slot;
+    }
+}
+
 /* one candidate whose Bloom bits were set for rc x (RV_HA in its meta) and/or rc y (RV_HB): is it isolated
  * after all?  SL = false looks for an upper partner in the table, SL = true (streamed scan: keys / bucket are
  * the sorted S list and its index) looks the key up in S.  Exact.  When the bucket prefix is no longer than
  * the run prefix (every table of more than a few entries) both buckets' offsets are loaded at once and then
- * RV_PROBE keys and counts of a bucket at once: two dependent accesses instead of one per key.             */
-template <typename IdxT, int KW, bool SL>
+ * RV_PROBE keys and counts of a bucket at once: two dependent accesses instead of one per key.
+ * RT = true (with SL): keys this rank owns are looked up in its S list; a candidate that is not settled by them
+ * and has a hit on a key owned elsewhere is parked (route_push) and counted later, so it is not isolated here. */
+template <typename IdxT, int KW, bool SL, bool RT = false>
 __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                                                    const uint16_t *__restrict__ cnt, int64_t n,
                                                    const IdxT *__restrict__ bucket, int bshift, int kmer,
@@ -1305,6 +1334,17 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
   revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
   ry = rx; ryl = rxl;
   set_base<KW>(ry,ryl,kmer-1-p,3-yb);                      /* rc y = rc x with the mirrored base swapped */
+  if (SL && RT)
+    { const int  oa = (ha && W.n_seg > 1) ? owner_of(W,rx) : W.self, ob = (hb && W.n_seg > 1) ? owner_of(W,ry) : W.self;
+      if ((ha && oa == W.self && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
+          (hb && ob == W.self && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0))
+        return false;
+      const bool fa = ha && oa != W.self, fb = hb && ob != W.self;
+      if (!fa && !fb)
+        return true;
+      route_push<KW>(W,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
+      return false;
+    }
   if (SL && W.n_seg > 1)                                   /* several shards: the S list of the key's owner */
     { const hm_stream_sview *V = (const hm_stream_sview *) W.cand_n[SY_HDR_S+4];
       if (ha)
@@ -1372,8 +1412,9 @@ __device__ __forceinline__ void count_pair(uint32_t *tile, unsigned long long *_
  * lane busy, without reading the record or the filter again.  RV_ILP candidates per thread and trip keep
  * that many record / Bloom loads in flight (the kernel is bound by latency: record -> Bloom word, and
  * for the hits bucket offsets -> keys, not by bytes or instructions).  One CTA of 1024 threads per SM:
- * one plot tile per SM, the rest of shared memory holds the queues.                                  */
-template <typename IdxT, int KW, bool SL>
+ * one plot tile per SM, the rest of shared memory holds the queues.
+ * RT = true: routed pass 2 of one rank (isolated_after_all); the rest of the kernel is the same.      */
+template <typename IdxT, int KW, bool SL, bool RT = false>
 __global__ void __launch_bounds__(RV_THREADS,1)
 resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
@@ -1448,13 +1489,13 @@ resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         { qn -= 32;
           const uint64_t xx = qk[qn+lane], xxl = KW == 2 ? ql[qn+lane] : 0, mm = qm[qn+lane];
           __syncwarp();
-          if (isolated_after_all<IdxT,KW,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
+          if (isolated_after_all<IdxT,KW,SL,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
             count_pair(tile,plot,mm,kmer);
         }
     }
   if (lane < qn)
     { const uint64_t xx = qk[lane], xxl = KW == 2 ? ql[lane] : 0, mm = qm[lane];
-      if (isolated_after_all<IdxT,KW,SL>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
+      if (isolated_after_all<IdxT,KW,SL,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
         count_pair(tile,plot,mm,kmer);
     }
   __syncthreads();
@@ -1465,7 +1506,7 @@ resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
     }
 }
 
-template <typename IdxT, int KW, bool SL = false>
+template <typename IdxT, int KW, bool SL = false, bool RT = false>
 static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                   const void *bucket, int bits, int kmer, const SymmView &W,
                                   unsigned long long *plot, int64_t range, cudaStream_t st)
@@ -1474,14 +1515,14 @@ static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo,
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (dev >= 64 || !configured[dev])
-    { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW,SL>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
+    { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW,SL,RT>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
       if (e != cudaSuccess) return e;
       if (dev < 64) configured[dev] = 1;
     }
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = (range/8+RV_THREADS-1)/RV_THREADS;            /* ~1 candidate per 10 entries */
   int     grid = (int) (want < sms ? (want > 0 ? want : 1) : sms);
-  resolve_kernel<IdxT,KW,SL><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
+  resolve_kernel<IdxT,KW,SL,RT><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
   return cudaGetLastError();
 }
 
@@ -1856,5 +1897,175 @@ int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int6
     bloom_window(st,NULL,0,0);
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"resolve_kernel (streamed)");
+  return HM_OK;
+}
+
+/* ------------------------------------------------------------------ routed pass 2 --------- */
+/* One rank of a one-process-per-GPU job streams its own share (hm_scan.cu hm_rank_scan_*, DESIGN.md §4c): nobody
+ * can read another rank's S list, so pass 2 goes in rounds over slices [c0, c1) of the rank's candidates.
+ * resolve_kernel<..., SL = true, RT = true> settles what the rank's own S list decides and parks the rest
+ * (route_push); route_count / route_scatter group the queries by owner (a one-digit radix sort: not a hot path);
+ * the caller sends the key words to their owners, route_answer_kernel answers the keys that arrive, the
+ * answers come back in the order they were sent, and route_mark / route_settle count every parked candidate
+ * none of whose queried keys was found.                                                                    */
+static SymmView route_view(void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, const hm_symm_shards *sh,
+                           int64_t c0, int64_t c1)
+{ SymmView W = stream_view(d_work,L,R,sh);
+  W.cand_key += c0; W.cand_meta += c0;
+  if (W.cand_lo != NULL) W.cand_lo += c0;
+  W.cand_cap = (unsigned long long) (c1-c0);             /* the header's count (all candidates) is >= c1 */
+  return W;
+}
+
+int hm_symm_route_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
+                          const void *d_s_bucket, int bits, int idx64, int kmer, int64_t c0, int64_t c1,
+                          void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                          const hm_symm_shards *shards, const hm_route_bufs *B, unsigned long long *d_plot, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_plot == NULL ||
+      B == NULL || c0 < 0 || c1 < c0 || c1 > R->cand_cap || c1-c0 > B->pend_cap || 2*(c1-c0) > B->q_cap)
+    return hm_set_error(HM_EINVAL,"symm_route_resolve: bad arguments");
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = route_view(d_work,L,R,shards,c0,c1);
+  uint64_t h[8] = { 0, 0, (uint64_t) (uintptr_t) B->pend, (uint64_t) (uintptr_t) B->q_key, (uint64_t) (uintptr_t) B->q_lo,
+                    (uint64_t) (uintptr_t) B->q_tag, (uint64_t) B->pend_cap, (uint64_t) B->q_cap };
+  HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_R,h,sizeof(h),cudaMemcpyHostToDevice,st));
+  HM_CUDA(cudaStreamSynchronize(st));                    /* (h is on the stack) */
+  if (c1 == c0)
+    return HM_OK;
+  cudaError_t e;
+  int64_t range = 8*(c1-c0);
+  if (kmer <= 32)
+    e = idx64 ? launch_resolve<uint64_t,1,true,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
+              : launch_resolve<uint32_t,1,true,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
+  else
+    e = idx64 ? launch_resolve<uint64_t,2,true,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
+              : launch_resolve<uint32_t,2,true,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
+  if (l2_persist())
+    bloom_window(st,NULL,0,0);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"resolve_kernel (routed)");
+  return HM_OK;
+}
+
+__global__ void route_count_kernel(const uint64_t *__restrict__ tag, int64_t nq, unsigned long long *__restrict__ counts)
+{ for (int64_t j = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; j < nq; j += (int64_t) gridDim.x*blockDim.x)
+    atomicAdd(counts + (tag[j] >> 32),1ull);
+}
+
+template <int KW>
+__global__ void route_scatter_kernel(const uint64_t *__restrict__ qk, const uint64_t *__restrict__ ql,
+                                     const uint64_t *__restrict__ tag, int64_t nq, unsigned long long *__restrict__ cursor,
+                                     uint64_t *__restrict__ send, uint32_t *__restrict__ send_slot)
+{ for (int64_t j = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; j < nq; j += (int64_t) gridDim.x*blockDim.x)
+    { const uint64_t t = tag[j];
+      const unsigned long long at = atomicAdd(cursor + (t >> 32),1ull);
+      send[KW*at] = qk[j];
+      if (KW == 2) send[KW*at+1] = ql[j];
+      send_slot[at] = (uint32_t) t;
+    }
+}
+
+static int route_grid(int64_t n)
+{ int64_t g = (n+255)/256;
+  return (int) (g < 1 ? 1 : (g > 4096 ? 4096 : g));
+}
+
+/* the last round's queries grouped by owner into B->send (KW words each) and B->send_slot; counts[r] = queries
+ * for rank r (r < world), *n_pend = parked candidates, *status = the header's status word (synchronises)     */
+int hm_symm_route_group(int kmer, int world, void *d_work, const hm_symm_layout *L, const hm_route_bufs *B,
+                        int64_t *counts, int64_t *n_sent, int64_t *n_pend, uint64_t *status, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  uint64_t h[SY_HDR_R+2];
+  HM_CUDA(cudaMemcpyAsync(h,(const uint8_t *) d_work + L->off_header,sizeof(h),cudaMemcpyDeviceToHost,st));
+  HM_CUDA(cudaMemsetAsync(B->counts,0,2*HM_MAX_SHARDS*sizeof(unsigned long long),st));
+  HM_CUDA(cudaStreamSynchronize(st));
+  int64_t nq = (int64_t) h[SY_HDR_R+1];
+  *status = h[1];
+  *n_pend = (int64_t) h[SY_HDR_R] < B->pend_cap ? (int64_t) h[SY_HDR_R] : B->pend_cap;
+  if (nq > B->q_cap) nq = B->q_cap;                       /* (an overflow is in the status word) */
+  *n_sent = nq;
+  for (int r = 0; r < world; r++) counts[r] = 0;
+  if (nq == 0)
+    return HM_OK;
+  route_count_kernel<<<route_grid(nq),256,0,st>>>(B->q_tag,nq,B->counts);
+  unsigned long long c[HM_MAX_SHARDS], cur[HM_MAX_SHARDS], acc = 0;
+  HM_CUDA(cudaMemcpyAsync(c,B->counts,sizeof(c),cudaMemcpyDeviceToHost,st));
+  HM_CUDA(cudaStreamSynchronize(st));
+  for (int r = 0; r < HM_MAX_SHARDS; r++)
+    { cur[r] = acc; acc += c[r];
+      if (r < world) counts[r] = (int64_t) c[r];
+    }
+  HM_CUDA(cudaMemcpyAsync(B->counts+HM_MAX_SHARDS,cur,sizeof(cur),cudaMemcpyHostToDevice,st));
+  if (kmer > 32)
+    route_scatter_kernel<2><<<route_grid(nq),256,0,st>>>(B->q_key,B->q_lo,B->q_tag,nq,B->counts+HM_MAX_SHARDS,B->send,B->send_slot);
+  else
+    route_scatter_kernel<1><<<route_grid(nq),256,0,st>>>(B->q_key,B->q_lo,B->q_tag,nq,B->counts+HM_MAX_SHARDS,B->send,B->send_slot);
+  HM_CUDA(cudaGetLastError());
+  HM_CUDA(cudaStreamSynchronize(st));
+  return HM_OK;
+}
+
+/* one thread per key that arrived (KW words each): is it in this rank's S list?  One byte back per key */
+template <typename IdxT, int KW>
+__global__ void route_answer_kernel(const uint64_t *__restrict__ s_key, const uint64_t *__restrict__ s_lo,
+                                    const IdxT *__restrict__ s_bucket, int bshift, const uint64_t *__restrict__ recv,
+                                    int64_t n, uint8_t *__restrict__ ans)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    { const uint64_t q = recv[KW*i], ql = KW == 2 ? recv[KW*i+1] : 0;
+      ans[i] = bucket_find<IdxT,KW>(s_key,s_lo,s_bucket,bshift,q,ql) >= 0 ? 1 : 0;
+    }
+}
+
+int hm_symm_route_answer(const uint64_t *d_s_key, const uint64_t *d_s_lo, const void *d_s_bucket, int bits,
+                         int idx64, int kmer, const uint64_t *d_recv, int64_t n, uint8_t *d_ans, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (n > 0)
+    { const int g = route_grid(n), sh = 64-bits;
+      if (kmer <= 32)
+        { if (idx64) route_answer_kernel<uint64_t,1><<<g,256,0,st>>>(d_s_key,NULL,(const uint64_t *) d_s_bucket,sh,d_recv,n,d_ans);
+          else       route_answer_kernel<uint32_t,1><<<g,256,0,st>>>(d_s_key,NULL,(const uint32_t *) d_s_bucket,sh,d_recv,n,d_ans);
+        }
+      else
+        { if (idx64) route_answer_kernel<uint64_t,2><<<g,256,0,st>>>(d_s_key,d_s_lo,(const uint64_t *) d_s_bucket,sh,d_recv,n,d_ans);
+          else       route_answer_kernel<uint32_t,2><<<g,256,0,st>>>(d_s_key,d_s_lo,(const uint32_t *) d_s_bucket,sh,d_recv,n,d_ans);
+        }
+      HM_CUDA(cudaGetLastError());
+    }
+  HM_CUDA(cudaStreamSynchronize(st));
+  return HM_OK;
+}
+
+#define ROUTE_FOUND (1ull << 63)                           /* a parked candidate's meta: some queried key is in S */
+
+__global__ void route_mark_kernel(const uint8_t *__restrict__ ans, const uint32_t *__restrict__ send_slot, int64_t n,
+                                  unsigned long long *__restrict__ pend)
+{ for (int64_t j = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; j < n; j += (int64_t) gridDim.x*blockDim.x)
+    if (ans[j])
+      atomicOr(pend + send_slot[j],ROUTE_FOUND);
+}
+
+/* count_pair's weight rule, straight into the plot (few candidates) */
+__global__ void route_settle_kernel(const uint64_t *__restrict__ pend, int64_t n, int kmer,
+                                    unsigned long long *__restrict__ plot)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    { const uint64_t meta = pend[i];
+      if (meta & ROUTE_FOUND)
+        continue;
+      const int cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff), p = (int) ((meta >> 32) & 0xff);
+      const int s = cx+cy, m = cx < cy ? cx : cy;
+      atomicAdd(plot + s*HM_PLOT_W + m,(unsigned long long) ((2*p == kmer-1) ? 1 : 2));
+    }
+}
+
+/* d_ans: the answers to the round's n_sent queries, in the order they were sent (synchronises) */
+int hm_symm_route_settle(int kmer, const hm_route_bufs *B, const uint8_t *d_ans, int64_t n_sent, int64_t n_pend,
+                         unsigned long long *d_plot, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (n_sent > 0)
+    route_mark_kernel<<<route_grid(n_sent),256,0,st>>>(d_ans,B->send_slot,n_sent,(unsigned long long *) B->pend);
+  if (n_pend > 0)
+    route_settle_kernel<<<route_grid(n_pend),256,0,st>>>(B->pend,n_pend,kmer,d_plot);
+  HM_CUDA(cudaGetLastError());
+  HM_CUDA(cudaStreamSynchronize(st));
   return HM_OK;
 }

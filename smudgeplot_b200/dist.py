@@ -591,3 +591,223 @@ class ShardedScan:
                        ("fingerprint -> runscan -> all-gather(Bloom) -> resolve" if self.path == "symm" else
                         "filter -> pass1 -> deg exchange -> pass2") + " -> all-reduce(plot) -> D2H",
                 "plot_matches_resident_scan": same, "exchange": self.exchange}
+
+
+# ---- streaming a strand-symmetric table, each rank its own share (DESIGN.md §4c, *Ranks*) ------------------
+
+def file_run_aligned_cuts(kt, world: int, window: int = 4096):
+    """run_aligned_cuts of a FastK table (fastk.KtabFiles) from its files alone, the rule hm_rank_scan_create
+    applies: c_r = the first run start at or after n*r/world, found by reading `window` records at a time after
+    each nominal cut.  -> [0, c_1, ..., n]"""
+    import numpy as np
+    n, k = kt.nels, kt.kmer
+    sh = np.uint64(64 - 2 * (k >> 1))
+    part_end = np.cumsum(np.asarray(kt.part_nels, dtype=np.int64))
+
+    def words(a, b):                       # word 0 of the keys of ordinals [a, b)
+        out = np.zeros(b - a, dtype=np.uint64)
+        pre = np.searchsorted(kt.index, np.arange(a, b, dtype=np.int64), side="right").astype(np.uint64)
+        out |= pre << np.uint64(64 - 8 * kt.ibyte)
+        for i in range(a, b):
+            p = int(np.searchsorted(part_end, i, side="right"))
+            j = i - (int(part_end[p - 1]) if p > 0 else 0)
+            rec = kt.records[p][j * kt.pbyte:(j + 1) * kt.pbyte]
+            for t in range(min(kt.hbyte, 8 - kt.ibyte)):
+                out[i - a] |= np.uint64(int(rec[t])) << np.uint64(56 - 8 * (kt.ibyte + t))
+        return out
+
+    cuts = [0]
+    for r in range(1, world):
+        c = (n * r) // world
+        if c <= cuts[-1]:
+            cuts.append(cuts[-1])
+            continue
+        prev = words(c - 1, c)[0] >> sh
+        at = n
+        while c < n:
+            w = words(c, min(n, c + window))
+            d = np.nonzero((w >> sh) != prev)[0]
+            if d.size:
+                at = c + int(d[0])
+                break
+            c += w.size
+        cuts.append(at)
+    return cuts + [n]
+
+
+def _nccl(group) -> bool:
+    return dist.get_backend(group) == "nccl"
+
+
+def _in_place(fn, t: torch.Tensor, group):
+    """run collective fn(tensor) on t in place (NCCL), or through a host copy when the backend (gloo) has no
+    collective for device tensors"""
+    if t.is_cuda and not _nccl(group):
+        h = t.cpu()
+        fn(h)
+        t.copy_(h)
+    else:
+        fn(t)
+    return t
+
+
+def _all_to_all(out: torch.Tensor, inp: torch.Tensor, out_splits, in_splits, group):
+    """all_to_all_single with per-rank splits; device tensors go through host copies on gloo"""
+    if out.is_cuda and not _nccl(group):
+        h = torch.empty(out.shape, dtype=out.dtype)
+        dist.all_to_all_single(h, inp.cpu(), out_splits, in_splits, group=group)
+        out.copy_(h)
+    else:
+        dist.all_to_all_single(out, inp, out_splits, in_splits, group=group)
+    return out
+
+
+class StreamedShardedScan:
+    """The streamed counterpart of ShardedScan: rank r of the group streams its run-aligned share of the FastK
+    table at the path `table` (or the `_lib.HostTable` `table`, whose buffers must outlive the scan) through
+    `device` under the device budget (`budget` bytes, else free memory minus a reserve);
+    no rank holds the table.  Pass 2 settles a Bloom hit on a key another rank owns by asking that rank: the keys
+    go to their owners with all_to_all_single, one byte per key comes back (hm_rank_scan_*, DESIGN.md §4c).
+    scan() -> the plot (int64[SMAX+1, FMAX+1] on every rank), equal to the in-core scan's."""
+
+    def __init__(self, table, group=None, device=None, budget: int | None = None):
+        import ctypes as C
+        from . import _lib, fastk
+        from .hetmers import _host_table
+        self.group = group
+        self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
+        dev = torch.device(device if device is not None else "cuda")
+        self.device = dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
+        self._coll_dev = self.device if _nccl(group) else torch.device("cpu")
+        self.L = L = _lib.lib()
+        if isinstance(table, _lib.HostTable):
+            self._ht, self._keep = table, None
+        else:
+            self._ht, self._keep = _host_table(fastk.read_ktab(table, mmap=True))   # read again by every scan
+        self.kmer = self._ht.kmer
+        seeds = common_seeds(self._coll_dev, group)
+        sd = (C.c_uint64 * 2)(*seeds)
+        if budget is not None:
+            L.hm_set_device_budget(int(budget))
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _lib.check(L.hm_rank_scan_create(C.byref(self._ht), self.device.index, self.rank, self.world, sd, C.byref(h)))
+        self._h = h
+        cuts = (C.c_int64 * (self.world + 1))()
+        _lib.check(L.hm_rank_scan_cuts(h, cuts, None))
+        self.cuts = [int(c) for c in cuts]
+        mine = torch.tensor(self.cuts, dtype=torch.int64, device=self._coll_dev)
+        every = [torch.empty_like(mine) for _ in range(self.world)]
+        dist.all_gather(every, mine, group=group)
+        if any(not torch.equal(e, mine) for e in every):
+            self.close()
+            raise RuntimeError(f"rank {self.rank}: the ranks computed different shard cuts from the table files "
+                               f"({[e.tolist() for e in every]})")
+        self.status = 0
+        self.stats = {}
+
+    def _view(self, ptr: int, nbytes: int) -> torch.Tensor:
+        return _cuda_view(ptr, max(nbytes, 1), self.device)[:nbytes]
+
+    def scan(self, timings: dict | None = None) -> torch.Tensor:
+        import ctypes as C
+        from . import _lib
+        L, h, g, W = self.L, self._h, self.group, self.world
+        kw = 2 if self.kmer > 32 else 1
+        tm = {} if timings is None else timings
+        sync = lambda: torch.cuda.synchronize(self.device)     # noqa: E731  (the library works on its own streams)
+
+        def lap(name, t0):
+            tm[name] = tm.get(name, 0.0) + (time.perf_counter() - t0) * 1e3
+            return time.perf_counter()
+
+        with torch.cuda.device(self.device):
+            t = time.perf_counter()
+            fp = (C.c_uint64 * 4)()
+            _lib.check(L.hm_rank_scan_pass1(h, fp))
+            t = lap("pass1", t)
+            acc = torch.tensor([v - (1 << 64) if v >= (1 << 63) else v for v in fp], dtype=torch.int64,
+                               device=self._coll_dev)
+            symmetric = fingerprint_verdict(acc, g)
+            nc, ms = C.c_int64(), C.c_int64()
+            _lib.check(L.hm_rank_scan_prepare(h, int(symmetric), C.byref(nc), C.byref(ms)))
+            t = lap("verdict_and_s_index", t)
+            seg, segb = C.c_void_p(), C.c_int64()
+            _lib.check(L.hm_rank_scan_bloom(h, C.byref(seg), C.byref(segb)))
+            if W > 1:
+                view = self._view(seg.value, W * segb.value).view(W, segb.value)
+                _in_place(lambda x: exchange_segments(x, self.rank, g), view, g)
+                sync()
+            t = lap("bloom_allgather", t)
+            lim = torch.tensor([ms.value, -nc.value], dtype=torch.int64, device=self._coll_dev)
+            dist.all_reduce(lim, op=dist.ReduceOp.MIN, group=g)
+            slice_ = max(1, min(int(lim[0]), -int(lim[1])))        # the smallest room, no more than the most candidates
+            rounds = C.c_int64()
+            ptr = [C.c_void_p() for _ in range(4)]
+            _lib.check(L.hm_rank_scan_slices(h, slice_, C.byref(rounds), *[C.byref(p) for p in ptr]))
+            rt = torch.tensor([rounds.value], dtype=torch.int64, device=self._coll_dev)
+            dist.all_reduce(rt, op=dist.ReduceOp.MAX, group=g)
+            n_rounds = int(rt.item())
+            q = 2 * slice_
+            send = self._view(ptr[0].value, 8 * kw * q).view(torch.int64)
+            recv = self._view(ptr[1].value, 8 * kw * q * (W - 1)).view(torch.int64)
+            ans_recv = self._view(ptr[2].value, q * (W - 1))
+            ans_sent = self._view(ptr[3].value, q)
+            t = lap("slices", t)
+            counts = (C.c_int64 * W)()
+            sent_to = [0] * W
+            for rd in range(n_rounds):
+                _lib.check(L.hm_rank_scan_route(h, rd, counts))
+                t = lap("resolve", t)
+                if W > 1:
+                    out_c = [int(c) for c in counts]
+                    sc = torch.tensor(out_c, dtype=torch.int64, device=self._coll_dev)
+                    rc = torch.empty_like(sc)
+                    dist.all_to_all_single(rc, sc, group=g)
+                    in_c = [int(c) for c in rc.tolist()]
+                    ns, nr = sum(out_c), sum(in_c)
+                    for r_, c in enumerate(out_c):
+                        sent_to[r_] += c
+                    _all_to_all(recv[:kw * nr], send[:kw * ns], [kw * c for c in in_c], [kw * c for c in out_c], g)
+                    sync()
+                    t = lap("exchange_queries", t)
+                    _lib.check(L.hm_rank_scan_answer(h, nr))
+                    t = lap("answer", t)
+                    _all_to_all(ans_sent[:ns], ans_recv[:nr], out_c, in_c, g)
+                    sync()
+                    t = lap("exchange_answers", t)
+                _lib.check(L.hm_rank_scan_settle(h))
+                t = lap("settle", t)
+            dp, st = C.c_void_p(), C.c_uint64()
+            _lib.check(L.hm_rank_scan_result(h, C.byref(dp), C.byref(st)))
+            plot = self._view(dp.value, 8 * _lib.PLOT_CELLS).view(torch.int64)
+            if W > 1:
+                _in_place(lambda x: allreduce_plot(x, g), plot, g)
+                sync()
+            out = plot.clone().view(_lib.SMAX + 1, _lib.PLOT_W)
+            lap("plot_allreduce", t)
+        self.status = int(st.value)
+        self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms.value, "candidates": nc.value,
+                      "queries_sent_to": sent_to}
+        return out
+
+    def residency(self):
+        """-> (peak device bytes since the last scan began, its chunks, the budget)"""
+        import ctypes as C
+        b, c, bud = C.c_int64(), C.c_int64(), C.c_int64()
+        from . import _lib
+        _lib.check(self.L.hm_rank_scan_residency(self._h, C.byref(b), C.byref(c), C.byref(bud)))
+        return b.value, c.value, bud.value
+
+    def symm_ok(self) -> bool:
+        """status words of the last scan on every rank: all clean?"""
+        bad = torch.tensor([int(self.status != 0)], dtype=torch.int32, device=self._coll_dev)
+        if self.world > 1:
+            dist.all_reduce(bad, op=dist.ReduceOp.MAX, group=self.group)
+        return int(bad.item()) == 0
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            with torch.cuda.device(self.device):
+                self.L.hm_rank_scan_destroy(self._h)
+        self._h = None
