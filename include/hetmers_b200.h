@@ -374,7 +374,14 @@ int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks)
  *   route (counts[q] = queries for rank q) -> the key words all-to-all'ed from send into recv (KW = 1 word per
  *   query, 2 for k > 32) -> answer(keys received) -> the answers all-to-all'ed back from ans_recv into ans_sent
  *   -> settle; then result -> the partial plots summed over the ranks.
- * Device pointers are returned; they stay valid until the next pass1 or destroy.                          */
+ * extract_kmer_pairs' list goes the same way from a prepared pass 1 (after prepare and the Bloom all-gather, or
+ * after a finished scan or listing whose status words were clean on every rank; else pass1 ... bloom first):
+ *   extract_prepare(pixmap) -> extract_slices(the smallest max_slice of all ranks, capped by the largest
+ *   candidate count) -> for every round up to the largest `rounds` of all ranks: extract_route -> the key words
+ *   all-to-all'ed as above -> answer -> the answers all-to-all'ed back -> extract_settle; then extract_result ->
+ *   the ranks' records gathered on one rank and sorted there with hm_sort_pair_records.
+ * Device pointers are returned; they stay valid until the next pass1, slices / extract_slices, extract_result
+ * or destroy.                                                                                              */
 typedef struct hm_rank_scan hm_rank_scan;
 int  hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
                          hm_rank_scan **out);
@@ -396,6 +403,18 @@ int  hm_rank_scan_settle(hm_rank_scan *r);
 int  hm_rank_scan_result(hm_rank_scan *r, void **d_plot, uint64_t *status);
 /* the most device bytes held since the last pass1 began, that pass's chunks, and the budget */
 int  hm_rank_scan_residency(const hm_rank_scan *r, int64_t *device_bytes, int64_t *chunks, int64_t *budget);
+/* pixmap: host uint16[HM_PLOT_CELLS], pixel -> smudge label (0 = none).  max_slice: the most candidates per
+ * round the budget leaves room for beside the pixmap (HM_ENOMEM below 256, before any launch)             */
+int  hm_rank_scan_extract_prepare(hm_rank_scan *r, const uint16_t *pixmap, int64_t *n_cand, int64_t *max_slice);
+int  hm_rank_scan_extract_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send, void **d_recv,
+                                 void **d_ans_recv, void **d_ans_sent);
+int  hm_rank_scan_extract_route(hm_rank_scan *r, int64_t round, int64_t *counts);
+int  hm_rank_scan_extract_settle(hm_rank_scan *r);
+/* this rank's records (*records malloc'ed, caller frees), sorted as hm_scan_extract sorts; status: non-zero = do
+ * not use them.  Pass 1 stays resident for another extract_prepare.                                         */
+int  hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status);
+/* sort n records in place into hm_scan_extract's order: (smudge, key, position, alternative base) */
+int  hm_sort_pair_records(hm_pair_rec *records, int64_t n);
 
 /* one call: create + run + destroy (what bench.py's e2e leg times) */
 int  hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,

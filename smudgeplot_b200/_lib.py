@@ -29,6 +29,8 @@ ABI_SYMBOLS = [
     "hm_rank_scan_create", "hm_rank_scan_destroy", "hm_rank_scan_cuts", "hm_rank_scan_pass1", "hm_rank_scan_bloom",
     "hm_rank_scan_prepare", "hm_rank_scan_slices", "hm_rank_scan_route", "hm_rank_scan_answer", "hm_rank_scan_settle",
     "hm_rank_scan_result", "hm_rank_scan_residency",
+    "hm_rank_scan_extract_prepare", "hm_rank_scan_extract_slices", "hm_rank_scan_extract_route",
+    "hm_rank_scan_extract_settle", "hm_rank_scan_extract_result", "hm_sort_pair_records",
 ]
 
 
@@ -176,6 +178,12 @@ def lib():
     L.hm_rank_scan_settle.argtypes = [vp]
     L.hm_rank_scan_result.argtypes = [vp, C.POINTER(vp), u64p]
     L.hm_rank_scan_residency.argtypes = [vp, i64p, i64p, i64p]
+    L.hm_rank_scan_extract_prepare.argtypes = [vp, vp, i64p, i64p]
+    L.hm_rank_scan_extract_slices.argtypes = L.hm_rank_scan_slices.argtypes
+    L.hm_rank_scan_extract_route.argtypes = [vp, i64, i64p]
+    L.hm_rank_scan_extract_settle.argtypes = [vp]
+    L.hm_rank_scan_extract_result.argtypes = [vp, C.POINTER(C.POINTER(PairRec)), i64p, u64p]
+    L.hm_sort_pair_records.argtypes = [vp, i64]
     L.hm_table_open.argtypes = [C.c_char_p, C.POINTER(vp)]
     L.hm_table_close.argtypes = [vp]
     L.hm_table_close.restype = None

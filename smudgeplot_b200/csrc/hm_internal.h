@@ -73,6 +73,7 @@ typedef struct hm_route_bufs
     uint64_t *send;
     uint32_t *send_slot;
     unsigned long long *counts;
+    uint64_t *pend_key, *pend_lo;            /* the routed listing only: the parked candidates' key words      */
   } hm_route_bufs;
 
 int hm_symm_route_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
@@ -85,6 +86,17 @@ int hm_symm_route_answer(const uint64_t *d_s_key, const uint64_t *d_s_lo, const 
                          int idx64, int kmer, const uint64_t *d_recv, int64_t n, uint8_t *d_ans, void *stream);
 int hm_symm_route_settle(int kmer, const hm_route_bufs *B, const uint8_t *d_ans, int64_t n_sent, int64_t n_pend,
                          unsigned long long *d_plot, void *stream);
+/* the routed listing of extract_kmer_pairs (hm_rank_scan_extract_*): route_extract lists the slice's settled
+ * candidates into d_out (cap >= 2 per candidate; *d_count counts every record) and parks the rest with their
+ * keys (pend_key / pend_lo); route_group as above; route_list lists the parked ones none of whose keys was found */
+int hm_symm_route_extract(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
+                          const void *d_s_bucket, int bits, int idx64, int kmer, int64_t c0, int64_t c1,
+                          void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                          const hm_symm_shards *shards, const hm_route_bufs *B, const uint16_t *d_pixmap,
+                          hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count, void *stream);
+int hm_symm_route_list(int kmer, const hm_route_bufs *B, const uint8_t *d_ans, int64_t n_sent, int64_t n_pend,
+                       const uint16_t *d_pixmap, hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count,
+                       void *stream);
 
 #include <cuda_runtime.h>
 int hm_cuda_fail(cudaError_t e, const char *what);

@@ -2177,7 +2177,8 @@ extern "C" int hm_scan_download(hm_scan *s, uint64_t *keys, uint64_t *keys_lo, u
 struct hm_rank_scan
   { hm_scan      *s;                         /* one device (d[0]), s->nshard = world, s->rank = rank          */
     StreamRun     R;
-    int           stage;                     /* 0 created, 1 pass 1 done, 2 pass 2 prepared, 3 buffers sized  */
+    int           stage;                     /* 0 created, 1 pass 1 done, 2 pass 2 prepared, 3 buffers sized,
+                                              * 4 listing prepared, 5 listing buffers sized                    */
     uint64_t      ns;                        /* S keys of this rank                                          */
     int           sbits, sidx64;
     int64_t       ncand, slice, rounds;
@@ -2186,6 +2187,11 @@ struct hm_rank_scan
     uint8_t      *ans_recv, *ans_sent;       /* answers to them / to this rank's queries                     */
     int64_t       n_sent, n_pend;            /* of the last round                                            */
     uint64_t      status;                    /* OR of the status words seen since pass 1                     */
+    uint16_t     *pix;                       /* the listing: device pixmap, record counter, a round's records */
+    unsigned long long *rec_n;
+    hm_pair_rec  *rec;
+    hm_pair_rec  *host;                      /* the records of the rounds so far                              */
+    int64_t       host_n, host_cap;
   };
 
 static void rank_free_route(hm_rank_scan *r)
@@ -2193,9 +2199,18 @@ static void rank_free_route(hm_rank_scan *r)
   cudaSetDevice(D->dev);
   dev_free(D,r->B.pend); dev_free(D,r->B.q_key); dev_free(D,r->B.q_lo); dev_free(D,r->B.q_tag);
   dev_free(D,r->B.send); dev_free(D,r->B.send_slot); dev_free(D,r->B.counts);
+  dev_free(D,r->B.pend_key); dev_free(D,r->B.pend_lo); dev_free(D,r->rec);
   dev_free(D,r->recv); dev_free(D,r->ans_recv); dev_free(D,r->ans_sent);
   memset(&r->B,0,sizeof(r->B));
-  r->recv = NULL; r->ans_recv = NULL; r->ans_sent = NULL;
+  r->recv = NULL; r->ans_recv = NULL; r->ans_sent = NULL; r->rec = NULL;
+}
+
+static void rank_free_listing(hm_rank_scan *r)
+{ DevTable *D = r->s->d;
+  cudaSetDevice(D->dev);
+  dev_free(D,r->pix); dev_free(D,r->rec_n);
+  free(r->host);
+  r->pix = NULL; r->rec_n = NULL; r->host = NULL; r->host_n = r->host_cap = 0;
 }
 
 /* device bytes of the route buffers for slices of `slice` candidates */
@@ -2204,11 +2219,19 @@ static int64_t route_bytes(int64_t slice, int kmer, int world)
   return 8*slice + q*(8*KW+8+(KW == 2 ? 8 : 0)) + q*(8*KW+4) + o*q*8*KW + o*q + q + 16*HM_MAX_SHARDS + 10*256;
 }
 
+/* the routed listing's: the route buffers, the parked keys and two records per candidate of the slice */
+static int64_t listing_bytes(int64_t slice, int kmer, int world)
+{ int64_t KW = kmer > 32 ? 2 : 1;
+  return route_bytes(slice,kmer,world) + 8*KW*slice + 2*slice*(int64_t) sizeof(hm_pair_rec) + 3*256;
+}
+#define LISTING_FIXED_BYTES (2ll*HM_PLOT_CELLS + 256)    /* the device pixmap and the record counter */
+
 extern "C" void hm_rank_scan_destroy(hm_rank_scan *r)
 { if (r == NULL)
     return;
   if (r->s != NULL)
     { rank_free_route(r);
+      rank_free_listing(r);
       stream_release(r->s,0,&r->R);
       hm_scan_destroy(r->s);
     }
@@ -2276,6 +2299,7 @@ extern "C" int hm_rank_scan_pass1(hm_rank_scan *r, uint64_t *fp)
   hm_scan  *s = r->s;
   DevTable *D = s->d;
   rank_free_route(r);
+  rank_free_listing(r);
   stream_release(s,0,&r->R);
   r->stage = 0; r->status = 0;
   D->peak = D->held; D->chunks = 0; s->stop = 0;
@@ -2300,6 +2324,17 @@ extern "C" int hm_rank_scan_bloom(const hm_rank_scan *r, void **d_segments, int6
   return HM_OK;
 }
 
+/* the most candidates per slice whose buffers (bytes(slice, kmer, world)) fit in room */
+static int64_t largest_slice(int64_t room, int kmer, int world, int64_t (*bytes)(int64_t, int, int))
+{ int64_t lo = 0, hi = (int64_t) 1 << 31;
+  while (lo < hi)
+    { int64_t mid = lo + (hi-lo+1)/2;
+      if (bytes(mid,kmer,world) <= room) lo = mid;
+      else                               hi = mid-1;
+    }
+  return lo;
+}
+
 /* symmetric = the job-wide fingerprint verdict.  Frees the chunk buffers, indexes the S list and reports the
  * rank's candidates and the largest slice its budget leaves room for (HM_ENOMEM below ROUTE_MIN_SLICE).     */
 extern "C" int hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_cand, int64_t *max_slice)
@@ -2314,12 +2349,7 @@ extern "C" int hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_c
   if ((rc = stream_s_index(s,0,&r->R,r->ns,r->sidx64,1,&r->sbits)) != HM_OK)
     return rc;
   HM_CUDA(cudaStreamSynchronize(r->R.sc));
-  int64_t room = s->budget - s->d[0].held, lo = 0, hi = (int64_t) 1 << 31;
-  while (lo < hi)
-    { int64_t mid = lo + (hi-lo+1)/2;
-      if (route_bytes(mid,s->kmer,s->nshard) <= room) lo = mid;
-      else                                            hi = mid-1;
-    }
+  int64_t room = s->budget - s->d[0].held, lo = largest_slice(room,s->kmer,s->nshard,route_bytes);
   if (lo < ROUTE_MIN_SLICE)
     return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes leaves %lld bytes beside the resident lists of this rank "
                         "(%lld held), and pass 2's exchange buffers for a slice of %d candidates need %lld",
@@ -2335,19 +2365,19 @@ extern "C" int hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_c
  * slices this rank's candidates take.  The device buffers the caller's collectives read and write:
  * send (uint64, KW words per query, grouped by owner), recv (the same for what arrives), ans_recv (a byte per
  * key that arrived) and ans_sent (a byte per query sent, in send order).                                    */
-extern "C" int hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send, void **d_recv,
-                                   void **d_ans_recv, void **d_ans_sent)
-{ if (r == NULL || r->stage != 2 || slice < 1 || rounds == NULL)
-    return hm_set_error(HM_EINVAL,"hm_rank_scan_slices: bad arguments");
-  hm_scan  *s = r->s;
+/* the route buffers of slices of `slice` candidates (listing: with the parked keys and the records) */
+static int rank_alloc_route(hm_rank_scan *r, int64_t slice, int listing, int64_t *rounds, void **d_send, void **d_recv,
+                            void **d_ans_recv, void **d_ans_sent)
+{ hm_scan  *s = r->s;
   DevTable *D = s->d;
   int64_t   KW = s->kmer > 32 ? 2 : 1, q = 2*slice, o = s->nshard-1;
+  int64_t   need = listing ? listing_bytes(slice,s->kmer,s->nshard) : route_bytes(slice,s->kmer,s->nshard);
   int       rc = HM_OK;
   cudaError_t e;
-  if (D->held + route_bytes(slice,s->kmer,s->nshard) > s->budget)
-    return hm_set_error(HM_ENOMEM,"pass 2's exchange buffers for slices of %lld candidates need %lld bytes and the device "
-                        "budget of %lld bytes has room for %lld",(long long) slice,
-                        (long long) route_bytes(slice,s->kmer,s->nshard),(long long) s->budget,(long long) (s->budget-D->held));
+  if (D->held + need > s->budget)
+    return hm_set_error(HM_ENOMEM,"%s for slices of %lld candidates need %lld bytes and the device budget of %lld bytes "
+                        "has room for %lld",listing ? "the pair listing's buffers" : "pass 2's exchange buffers",
+                        (long long) slice,(long long) need,(long long) s->budget,(long long) (s->budget-D->held));
   rank_free_route(r);
   TRY(cudaSetDevice(D->dev));
   TRY(dev_alloc(D,&r->B.pend,8*slice));
@@ -2360,6 +2390,11 @@ extern "C" int hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *roun
   TRY(dev_alloc(D,&r->recv,8*KW*(o*q > 0 ? o*q : 1)));
   TRY(dev_alloc(D,&r->ans_recv,o*q > 0 ? o*q : 1));
   TRY(dev_alloc(D,&r->ans_sent,q));
+  if (listing)
+    { TRY(dev_alloc(D,&r->B.pend_key,8*slice));
+      if (KW == 2) TRY(dev_alloc(D,&r->B.pend_lo,8*slice));
+      TRY(dev_alloc(D,&r->rec,2*slice*(int64_t) sizeof(hm_pair_rec)));
+    }
   if (rc != HM_OK)
     { rank_free_route(r); return rc; }
   r->B.pend_cap = slice; r->B.q_cap = q;
@@ -2370,8 +2405,23 @@ extern "C" int hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *roun
   if (d_recv)     *d_recv = r->recv;
   if (d_ans_recv) *d_ans_recv = r->ans_recv;
   if (d_ans_sent) *d_ans_sent = r->ans_sent;
-  r->stage = 3;
   return HM_OK;
+}
+
+extern "C" int hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send, void **d_recv,
+                                   void **d_ans_recv, void **d_ans_sent)
+{ if (r == NULL || r->stage != 2 || slice < 1 || rounds == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_slices: bad arguments");
+  int rc = rank_alloc_route(r,slice,0,rounds,d_send,d_recv,d_ans_recv,d_ans_sent);
+  if (rc == HM_OK)
+    r->stage = 3;
+  return rc;
+}
+
+/* the candidates [c0, c1) of round `round` (an empty slice once they are done) */
+static void rank_round(const hm_rank_scan *r, int64_t round, int64_t *c0, int64_t *c1)
+{ *c0 = round*r->slice < r->ncand ? round*r->slice : r->ncand;
+  *c1 = *c0 + r->slice < r->ncand ? *c0 + r->slice : r->ncand;
 }
 
 /* round `round`: resolve the slice [round*slice, ...) of this rank's candidates (none once they are done) and
@@ -2381,10 +2431,10 @@ extern "C" int hm_rank_scan_route(hm_rank_scan *r, int64_t round, int64_t *count
     return hm_set_error(HM_EINVAL,"hm_rank_scan_route: bad arguments");
   hm_scan  *s = r->s;
   DevTable *D = s->d;
-  int64_t   c0 = round*r->slice < r->ncand ? round*r->slice : r->ncand;
-  int64_t   c1 = c0 + r->slice < r->ncand ? c0 + r->slice : r->ncand;
+  int64_t   c0, c1;
   int       KW = s->kmer > 32 ? 2 : 1, rc;
   uint64_t  status = 0;
+  rank_round(r,round,&c0,&c1);
   HM_CUDA(cudaSetDevice(D->dev));
   if (round == 0)
     HM_CUDA(cudaEventRecord(D->ev[2],r->R.sc));
@@ -2403,7 +2453,7 @@ extern "C" int hm_rank_scan_route(hm_rank_scan *r, int64_t round, int64_t *count
 /* the n keys that arrived in recv: one byte each into ans_recv (synchronises) */
 extern "C" int hm_rank_scan_answer(hm_rank_scan *r, int64_t n)
 { hm_scan *s = r ? r->s : NULL;
-  if (r == NULL || r->stage != 3 || n < 0 || n > (s->nshard-1)*2*r->slice)
+  if (r == NULL || (r->stage != 3 && r->stage != 5) || n < 0 || n > (s->nshard-1)*2*r->slice)
     return hm_set_error(HM_EINVAL,"hm_rank_scan_answer: bad arguments");
   HM_CUDA(cudaSetDevice(s->d[0].dev));
   return hm_symm_route_answer(r->R.R.s_key,s->kmer > 32 ? r->R.R.s_lo : NULL,r->R.s_bucket,r->sbits,r->sidx64,s->kmer,
@@ -2444,5 +2494,133 @@ extern "C" int hm_rank_scan_residency(const hm_rank_scan *r, int64_t *device_byt
   if (device_bytes) *device_bytes = r->s->d[0].peak;
   if (chunks)       *chunks = r->s->d[0].chunks;
   if (budget)       *budget = r->s->budget;
+  return HM_OK;
+}
+
+/* ---- the rank's pair listing (extract_kmer_pairs, DESIGN.md §4c, *Ranks*): the rounds of routed pass 2 over the
+ * candidates pass 1 left resident, each listing its isolated candidates instead of counting them               */
+
+/* stage >= 2: the candidates, the S index and the gathered Bloom filter of a pass 1 are resident.  Frees the
+ * route buffers, uploads the pixmap and reports the largest slice the budget leaves room for (HM_ENOMEM below
+ * ROUTE_MIN_SLICE, before any launch)                                                                        */
+extern "C" int hm_rank_scan_extract_prepare(hm_rank_scan *r, const uint16_t *pixmap, int64_t *n_cand, int64_t *max_slice)
+{ if (r == NULL || r->stage < 2 || pixmap == NULL || n_cand == NULL || max_slice == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_prepare: needs a prepared pass 1");
+  hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  int       rc = HM_OK;
+  cudaError_t e;
+  rank_free_route(r);
+  rank_free_listing(r);
+  int64_t room = s->budget - D->held - LISTING_FIXED_BYTES, lo = largest_slice(room,s->kmer,s->nshard,listing_bytes);
+  if (lo < ROUTE_MIN_SLICE)
+    return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes leaves %lld bytes beside the resident lists of this rank "
+                        "(%lld held) and the pixmap (%lld), and listing k-mer pairs in slices of %d candidates needs %lld",
+                        (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) D->held,
+                        (long long) LISTING_FIXED_BYTES,ROUTE_MIN_SLICE,
+                        (long long) listing_bytes(ROUTE_MIN_SLICE,s->kmer,s->nshard));
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&r->pix,sizeof(uint16_t)*HM_PLOT_CELLS));
+  TRY(dev_alloc(D,&r->rec_n,256));
+  TRY(cudaMemcpy(r->pix,pixmap,sizeof(uint16_t)*HM_PLOT_CELLS,cudaMemcpyHostToDevice));
+  if (rc != HM_OK)
+    { rank_free_listing(r); return rc; }
+  *n_cand = r->ncand;
+  *max_slice = lo;
+  r->stage = 4;
+  return HM_OK;
+}
+
+/* hm_rank_scan_slices for the listing (stage 4): also the parked keys and a round's records */
+extern "C" int hm_rank_scan_extract_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send,
+                                           void **d_recv, void **d_ans_recv, void **d_ans_sent)
+{ if (r == NULL || r->stage != 4 || slice < 1 || rounds == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_slices: bad arguments");
+  int rc = rank_alloc_route(r,slice,1,rounds,d_send,d_recv,d_ans_recv,d_ans_sent);
+  if (rc == HM_OK)
+    r->stage = 5;
+  return rc;
+}
+
+/* hm_rank_scan_route for the listing: extract_kernel<..., RT = true> over the round's slice, its queries grouped
+ * by owner */
+extern "C" int hm_rank_scan_extract_route(hm_rank_scan *r, int64_t round, int64_t *counts)
+{ if (r == NULL || r->stage != 5 || counts == NULL || round < 0)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_route: bad arguments");
+  hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  int64_t   c0, c1;
+  int       KW = s->kmer > 32 ? 2 : 1, rc;
+  uint64_t  status = 0;
+  rank_round(r,round,&c0,&c1);
+  HM_CUDA(cudaSetDevice(D->dev));
+  if ((rc = hm_symm_route_extract(r->R.R.s_key,KW == 2 ? r->R.R.s_lo : NULL,(int64_t) r->ns,r->R.s_bucket,r->sbits,
+                                  r->sidx64,s->kmer,c0,c1,r->R.work,&r->R.L,&r->R.R,s->nshard > 1 ? s->ssh : NULL,&r->B,
+                                  r->pix,r->rec,2*r->slice,r->rec_n,r->R.sc)) != HM_OK)
+    return rc;
+  __sync_fetch_and_add(&s->launches,(int64_t) (c1 > c0));
+  if ((rc = hm_symm_route_group(s->kmer,s->nshard,r->R.work,&r->R.L,&r->B,counts,&r->n_sent,&r->n_pend,&status,
+                                r->R.sc)) != HM_OK)
+    return rc;
+  r->status |= status;
+  return HM_OK;
+}
+
+/* ans_sent holds the answers to the round's queries: list the parked candidates none of whose keys was found,
+ * then append the round's records to the host list (synchronises)                                           */
+extern "C" int hm_rank_scan_extract_settle(hm_rank_scan *r)
+{ if (r == NULL || r->stage != 5)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_settle: bad arguments");
+  hm_scan *s = r->s;
+  unsigned long long c = 0;
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  int rc = hm_symm_route_list(s->kmer,&r->B,r->ans_sent,r->n_sent,r->n_pend,r->pix,r->rec,2*r->slice,r->rec_n,r->R.sc);
+  __sync_fetch_and_add(&s->launches,2);
+  if (rc != HM_OK)
+    return rc;
+  HM_CUDA(cudaMemcpy(&c,r->rec_n,sizeof(c),cudaMemcpyDeviceToHost));
+  if ((int64_t) c > 2*r->slice)
+    return hm_set_error(HM_ECUDA,"the routed listing gave %llu records for a slice of %lld candidates",c,
+                        (long long) r->slice);
+  if (r->host_n + (int64_t) c > r->host_cap)
+    { int64_t      nh = 2*r->host_cap > r->host_n + (int64_t) c ? 2*r->host_cap : r->host_n + (int64_t) c;
+      hm_pair_rec *h2 = (hm_pair_rec *) realloc(r->host,sizeof(hm_pair_rec)*(size_t) nh);
+      if (h2 == NULL)
+        return hm_set_error(HM_ENOMEM,"out of host memory for %lld pair records",(long long) nh);
+      r->host = h2; r->host_cap = nh;
+    }
+  if (c > 0)
+    HM_CUDA(cudaMemcpy(r->host+r->host_n,r->rec,sizeof(hm_pair_rec)*(size_t) c,cudaMemcpyDeviceToHost));
+  r->host_n += (int64_t) c;
+  return HM_OK;
+}
+
+/* after the last round: this rank's records (*records malloc'ed, the caller frees; sorted as hm_scan_extract sorts)
+ * and the OR of its status words (non-zero: do not use them).  The listing's buffers are freed.             */
+extern "C" int hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status)
+{ if (r == NULL || r->stage != 5 || records == NULL || n == NULL || status == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_result: bad arguments");
+  hm_scan *s = r->s;
+  uint64_t nc = 0, st = 0, ns = 0;
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  int rc = hm_symm_stream_counts(r->R.work,&r->R.L,&nc,&st,&ns,r->R.sc);     /* (synchronises) */
+  if (rc != HM_OK)
+    return rc;
+  if (r->host == NULL && (r->host = (hm_pair_rec *) malloc(sizeof(hm_pair_rec))) == NULL)
+    return hm_set_error(HM_ENOMEM,"out of host memory");
+  sort_records(r->host,r->host_n);
+  *records = r->host; *n = r->host_n;
+  *status = r->status | st;
+  r->host = NULL;
+  rank_free_route(r);
+  rank_free_listing(r);
+  r->stage = 2;                                  /* (pass 1 stays resident: another listing may follow) */
+  return HM_OK;
+}
+
+extern "C" int hm_sort_pair_records(hm_pair_rec *records, int64_t n)
+{ if (n < 0 || (n > 0 && records == NULL))
+    return hm_set_error(HM_EINVAL,"hm_sort_pair_records: bad arguments");
+  sort_records(records,n);
   return HM_OK;
 }

@@ -1315,14 +1315,40 @@ __device__ __noinline__ void route_push(const SymmView &W, uint64_t meta, bool f
     }
 }
 
+/* route_push of the routed listing (extract_kernel<..., RT = true>): listing a parked candidate needs its key, so
+ * its key words go to header words SY_HDR_R+8 / +9 (the parked keys and their second words) as well        */
+template <int KW>
+__device__ __noinline__ void route_push_key(const SymmView &W, uint64_t x, uint64_t xl, uint64_t meta, bool fa, int oa,
+                                            uint64_t rx, uint64_t rxl, bool fb, int ob, uint64_t ry, uint64_t ryl)
+{ unsigned long long *h = W.cand_n + SY_HDR_R;
+  const unsigned long long nq = (fa ? 1ull : 0ull) + (fb ? 1ull : 0ull);
+  const unsigned long long slot = atomicAdd(h,1ull), q = atomicAdd(h+1,nq);
+  if (slot >= h[6] || q+nq > h[7])
+    { atomicOr(W.status,SY_STATUS_OVERFLOW); return; }
+  ((uint64_t *) h[2])[slot] = meta & ~(RV_HA | RV_HB);
+  ((uint64_t *) h[8])[slot] = x;
+  if (KW == 2) ((uint64_t *) h[9])[slot] = xl;
+  uint64_t *qk = (uint64_t *) h[3], *ql = (uint64_t *) h[4], *qt = (uint64_t *) h[5];
+  unsigned long long at = q;
+  if (fa)
+    { qk[at] = rx; if (KW == 2) ql[at] = rxl;
+      qt[at] = ((uint64_t) oa << 32) | slot; at++;
+    }
+  if (fb)
+    { qk[at] = ry; if (KW == 2) ql[at] = ryl;
+      qt[at] = ((uint64_t) ob << 32) | slot;
+    }
+}
+
 /* one candidate whose Bloom bits were set for rc x (RV_HA in its meta) and/or rc y (RV_HB): is it isolated
  * after all?  SL = false looks for an upper partner in the table, SL = true (streamed scan: keys / bucket are
  * the sorted S list and its index) looks the key up in S.  Exact.  When the bucket prefix is no longer than
  * the run prefix (every table of more than a few entries) both buckets' offsets are loaded at once and then
  * RV_PROBE keys and counts of a bucket at once: two dependent accesses instead of one per key.
  * RT = true (with SL): keys this rank owns are looked up in its S list; a candidate that is not settled by them
- * and has a hit on a key owned elsewhere is parked (route_push) and counted later, so it is not isolated here. */
-template <typename IdxT, int KW, bool SL, bool RT = false>
+ * and has a hit on a key owned elsewhere is parked (route_push) and counted later, so it is not isolated here.
+ * KEY = true (with RT): it is parked with its key words (route_push_key), to be listed later.                   */
+template <typename IdxT, int KW, bool SL, bool RT = false, bool KEY = false>
 __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                                                    const uint16_t *__restrict__ cnt, int64_t n,
                                                    const IdxT *__restrict__ bucket, int bshift, int kmer,
@@ -1342,7 +1368,8 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
       const bool fa = ha && oa != W.self, fb = hb && ob != W.self;
       if (!fa && !fb)
         return true;
-      route_push<KW>(W,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
+      if (KEY) route_push_key<KW>(W,x,xl,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
+      else     route_push<KW>(W,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
       return false;
     }
   if (SL && W.n_seg > 1)                                   /* several shards: the S list of the key's owner */
@@ -1605,16 +1632,21 @@ __device__ __forceinline__ void list_pairs(uint64_t x, uint64_t xl, uint64_t met
     }
 }
 
-#define EX_THREADS 512              /* k <= 32: 2 CTAs per SM (64 registers); k > 32 spilled at 64 registers: 1 CTA */
+#define EX_THREADS 512              /* k <= 32: 2 CTAs per SM (64 registers); k > 32 spilled at 64 registers: 1 CTA,
+                                     * and so did the routed listing (RT) at k <= 32: 1 CTA                        */
 #define EX_ILP     RV_ILP
 #define EX_QCAP    (32*(EX_ILP+1))
 
 /* extract_kmer_pairs on the symmetric scan's work area: resolve_kernel (SL = false) over the candidates
  * [c0, c1) of the last run, with the same Bloom-first structure and per-warp queue of hits settled by
  * isolated_after_all, but an isolated candidate whose pixel carries a label is listed (list_pairs) instead
- * of counted.  No plot tile: shared memory holds only the queues.                                        */
-template <typename IdxT, int KW>
-__global__ void __launch_bounds__(EX_THREADS,KW == 1 ? 2 : 1)
+ * of counted.  No plot tile: shared memory holds only the queues.
+ * RT = true: the routed listing of one rank (DESIGN.md §4c, *Ranks*) over a slice [c0, c1) of its candidates;
+ * keys / bucket are its sorted S list and S index.  A hit on a key the rank owns is settled in that list; a
+ * candidate left with a hit on a key owned elsewhere is parked with its key words (route_push_key) and listed
+ * by route_list_kernel once the owners have answered.                                                    */
+template <typename IdxT, int KW, bool RT = false>
+__global__ void __launch_bounds__(EX_THREADS,KW == 1 && !RT ? 2 : 1)
 extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
                int kmer, const SymmView W, const uint16_t *__restrict__ pixmap, int64_t c0, int64_t c1,
@@ -1689,8 +1721,8 @@ extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         { qn -= 32;
           const uint64_t mm = qm[qn+lane];
           unsigned lab = 0;
-          if (isolated_after_all<IdxT,KW,false>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,qk[qn+lane],
-                                                KW == 2 ? ql[qn+lane] : 0,mm))
+          if (isolated_after_all<IdxT,KW,RT,RT,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,qk[qn+lane],
+                                                   KW == 2 ? ql[qn+lane] : 0,mm))
             { const int cx = (int) (mm & 0xffff), cy = (int) ((mm >> 16) & 0xffff);
               lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
             }
@@ -1702,7 +1734,7 @@ extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
   unsigned lab = 0;
   if (lane < qn)
     { xx = qk[lane]; xxl = KW == 2 ? ql[lane] : 0; mm = qm[lane];
-      if (isolated_after_all<IdxT,KW,false>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
+      if (isolated_after_all<IdxT,KW,RT,RT,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
         { const int cx = (int) (mm & 0xffff), cy = (int) ((mm >> 16) & 0xffff);
           lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
         }
@@ -1710,7 +1742,7 @@ extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
   list_pairs<KW>(xx,xxl,mm,lab,kmer,out,cap,count,lane,lt);
 }
 
-template <typename IdxT, int KW>
+template <typename IdxT, int KW, bool RT = false>
 static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                   const void *bucket, int bits, int kmer, const SymmView &W,
                                   const uint16_t *pixmap, int64_t c0, int64_t c1, hm_pair_rec *out,
@@ -1720,7 +1752,7 @@ static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo,
   int dev = 0, sms = 132, occ = 1;
   cudaGetDevice(&dev);
   if (dev >= 64 || per_sm[dev] == 0)                           /* one wave of resident CTAs */
-    { cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ,extract_kernel<IdxT,KW>,EX_THREADS,smem);
+    { cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ,extract_kernel<IdxT,KW,RT>,EX_THREADS,smem);
       if (e != cudaSuccess) return e;
       if (occ < 1) occ = 1;
       if (dev < 64) per_sm[dev] = occ;
@@ -1730,8 +1762,8 @@ static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo,
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = (c1-c0+EX_THREADS*EX_ILP-1)/(EX_THREADS*EX_ILP);
   int     grid = (int) (want < sms*occ ? (want > 0 ? want : 1) : sms*occ);
-  extract_kernel<IdxT,KW><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,
-                                                       pixmap,c0,c1,out,(unsigned long long) cap,count);
+  extract_kernel<IdxT,KW,RT><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,
+                                                          pixmap,c0,c1,out,(unsigned long long) cap,count);
   return cudaGetLastError();
 }
 
@@ -2065,6 +2097,90 @@ int hm_symm_route_settle(int kmer, const hm_route_bufs *B, const uint8_t *d_ans,
     route_mark_kernel<<<route_grid(n_sent),256,0,st>>>(d_ans,B->send_slot,n_sent,(unsigned long long *) B->pend);
   if (n_pend > 0)
     route_settle_kernel<<<route_grid(n_pend),256,0,st>>>(B->pend,n_pend,kmer,d_plot);
+  HM_CUDA(cudaGetLastError());
+  HM_CUDA(cudaStreamSynchronize(st));
+  return HM_OK;
+}
+
+/* ------------------------------------------------------------------ routed pair listing ---- */
+/* extract_kmer_pairs on one rank (hm_rank_scan_extract_*, DESIGN.md §4c): the rounds of routed pass 2, with
+ * extract_kernel<..., RT = true> in place of resolve_kernel and route_list_kernel in place of route_settle_kernel.
+ * A round's records (at most two per candidate of its slice) go to out through one counter, which counts every
+ * record, also those beyond cap.                                                                          */
+int hm_symm_route_extract(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
+                          const void *d_s_bucket, int bits, int idx64, int kmer, int64_t c0, int64_t c1,
+                          void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                          const hm_symm_shards *shards, const hm_route_bufs *B, const uint16_t *d_pixmap,
+                          hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_pixmap == NULL ||
+      d_count == NULL || B == NULL || B->pend_key == NULL || (kmer > 32 && B->pend_lo == NULL) || c0 < 0 || c1 < c0 ||
+      c1 > R->cand_cap || c1-c0 > B->pend_cap || 2*(c1-c0) > B->q_cap || cap < 2*(c1-c0) || d_out == NULL)
+    return hm_set_error(HM_EINVAL,"symm_route_extract: bad arguments");
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = stream_view(d_work,L,R,shards);
+  uint64_t h[10] = { 0, 0, (uint64_t) (uintptr_t) B->pend, (uint64_t) (uintptr_t) B->q_key, (uint64_t) (uintptr_t) B->q_lo,
+                     (uint64_t) (uintptr_t) B->q_tag, (uint64_t) B->pend_cap, (uint64_t) B->q_cap,
+                     (uint64_t) (uintptr_t) B->pend_key, (uint64_t) (uintptr_t) B->pend_lo };
+  HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_R,h,sizeof(h),cudaMemcpyHostToDevice,st));
+  HM_CUDA(cudaMemsetAsync(d_count,0,sizeof(unsigned long long),st));
+  HM_CUDA(cudaStreamSynchronize(st));                    /* (h is on the stack) */
+  if (c1 == c0)
+    return HM_OK;
+  cudaError_t e;
+  if (kmer <= 32)
+    e = idx64 ? launch_extract<uint64_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
+              : launch_extract<uint32_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
+  else
+    e = idx64 ? launch_extract<uint64_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
+              : launch_extract<uint32_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"extract_kernel (routed)");
+  return HM_OK;
+}
+
+/* every parked candidate none of whose queried keys was found (no ROUTE_FOUND) is isolated: listed if its pixel
+ * has a label.  list_pairs is warp-wide, so every lane of a warp stays in the loop (one atomic per warp).      */
+template <int KW>
+__global__ void route_list_kernel(const uint64_t *__restrict__ pend, const uint64_t *__restrict__ pkey,
+                                  const uint64_t *__restrict__ plo, int64_t n, int kmer,
+                                  const uint16_t *__restrict__ pixmap, hm_pair_rec *__restrict__ out,
+                                  unsigned long long cap, unsigned long long *__restrict__ count)
+{ const int      lane = threadIdx.x & 31;
+  const unsigned lt   = (1u << lane) - 1;
+  const int64_t  stride = (int64_t) gridDim.x*blockDim.x;
+  for (int64_t w = (int64_t) blockIdx.x*blockDim.x + (threadIdx.x & ~31); w < n; w += stride)
+    { const int64_t i = w + lane;
+      uint64_t meta = 0, x = 0, xl = 0;
+      unsigned lab = 0;
+      if (i < n)
+        { meta = pend[i];
+          if (!(meta & ROUTE_FOUND))
+            { const int cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
+              x = pkey[i];
+              if (KW == 2) xl = plo[i];
+              lab = pixmap[(cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy)];
+            }
+        }
+      list_pairs<KW>(x,xl,meta,lab,kmer,out,cap,count,lane,lt);
+    }
+}
+
+/* d_ans: the answers to the round's n_sent queries, in send order; lists the round's parked candidates that are
+ * isolated after all into d_out (synchronises)                                                            */
+int hm_symm_route_list(int kmer, const hm_route_bufs *B, const uint8_t *d_ans, int64_t n_sent, int64_t n_pend,
+                       const uint16_t *d_pixmap, hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count,
+                       void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (n_sent > 0)
+    route_mark_kernel<<<route_grid(n_sent),256,0,st>>>(d_ans,B->send_slot,n_sent,(unsigned long long *) B->pend);
+  if (n_pend > 0)
+    { if (kmer > 32)
+        route_list_kernel<2><<<route_grid(n_pend),256,0,st>>>(B->pend,B->pend_key,B->pend_lo,n_pend,kmer,d_pixmap,
+                                                              d_out,(unsigned long long) cap,d_count);
+      else
+        route_list_kernel<1><<<route_grid(n_pend),256,0,st>>>(B->pend,B->pend_key,NULL,n_pend,kmer,d_pixmap,
+                                                              d_out,(unsigned long long) cap,d_count);
+    }
   HM_CUDA(cudaGetLastError());
   HM_CUDA(cudaStreamSynchronize(st));
   return HM_OK;

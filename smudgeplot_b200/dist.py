@@ -662,13 +662,66 @@ def _all_to_all(out: torch.Tensor, inp: torch.Tensor, out_splits, in_splits, gro
     return out
 
 
+def _libc_free(p):
+    import ctypes as C
+    libc = C.CDLL(None)
+    libc.free.argtypes = [C.c_void_p]
+    libc.free(p)
+
+
+def sort_pair_records(recs):
+    """sort a structured array of pair records (hetmers.PAIR_DTYPE) in place into the order hm_scan_extract
+    returns (hm_sort_pair_records)"""
+    from . import _lib
+    if len(recs) > 1:
+        _lib.lib().hm_sort_pair_records(recs.ctypes.data, len(recs))
+    return recs
+
+
+def gather_pairs(records, dst: int = 0, group=None):
+    """the ranks' pair records (structured numpy arrays of hetmers.PAIR_DTYPE, any length, on the host) -> on rank
+    `dst` of the group all of them in hm_scan_extract's order (sort_pair_records); None on the other ranks.  Each
+    rank's bytes go to dst point-to-point, staged through a device tensor on NCCL."""
+    import numpy as np
+    from .hetmers import PAIR_DTYPE
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    recs = np.ascontiguousarray(records, dtype=PAIR_DTYPE)
+    dev = torch.device("cuda", torch.cuda.current_device()) if _nccl(group) else torch.device("cpu")
+    n = torch.tensor([len(recs)], dtype=torch.int64, device=dev)
+    every = [torch.empty_like(n) for _ in range(world)]
+    dist.all_gather(every, n, group=group)
+    sizes = [int(e.item()) for e in every]
+    peer = (lambda r: dist.get_global_rank(group, r)) if group is not None else (lambda r: r)   # noqa: E731
+    item = PAIR_DTYPE.itemsize
+    if rank != dst:
+        if sizes[rank] > 0:
+            buf = torch.from_numpy(recs.view(np.uint8)).to(dev)
+            for w in dist.batch_isend_irecv([dist.P2POp(dist.isend, buf, peer(dst), group)]):
+                w.wait()
+        return None
+    bufs, ops = [], []
+    for r in range(world):
+        if r == dst or sizes[r] == 0:
+            bufs.append(None)
+            continue
+        bufs.append(torch.empty(sizes[r] * item, dtype=torch.uint8, device=dev))
+        ops.append(dist.P2POp(dist.irecv, bufs[-1], peer(r), group))
+    if ops:
+        for w in dist.batch_isend_irecv(ops):
+            w.wait()
+    parts = [recs if r == dst else bufs[r].cpu().numpy().view(PAIR_DTYPE) for r in range(world) if sizes[r] > 0]
+    out = np.concatenate(parts) if parts else np.empty(0, dtype=PAIR_DTYPE)
+    return sort_pair_records(np.ascontiguousarray(out))
+
+
 class StreamedShardedScan:
     """The streamed counterpart of ShardedScan: rank r of the group streams its run-aligned share of the FastK
     table at the path `table` (or the `_lib.HostTable` `table`, whose buffers must outlive the scan) through
     `device` under the device budget (`budget` bytes, else free memory minus a reserve);
     no rank holds the table.  Pass 2 settles a Bloom hit on a key another rank owns by asking that rank: the keys
     go to their owners with all_to_all_single, one byte per key comes back (hm_rank_scan_*, DESIGN.md §4c).
-    scan() -> the plot (int64[SMAX+1, FMAX+1] on every rank), equal to the in-core scan's."""
+    scan() -> the plot (int64[SMAX+1, FMAX+1] on every rank), equal to the in-core scan's; extract(pixmap, dst) ->
+    extract_kmer_pairs' records on rank dst, equal to the in-core list."""
 
     def __init__(self, table, group=None, device=None, budget: int | None = None):
         import ctypes as C
@@ -705,91 +758,168 @@ class StreamedShardedScan:
                                f"({[e.tolist() for e in every]})")
         self.status = 0
         self.stats = {}
+        self._pass1_done = False                                # candidates, S list and Bloom filter resident
 
     def _view(self, ptr: int, nbytes: int) -> torch.Tensor:
         return _cuda_view(ptr, max(nbytes, 1), self.device)[:nbytes]
+
+    def _lap(self, tm):
+        def lap(name, t0):
+            tm[name] = tm.get(name, 0.0) + (time.perf_counter() - t0) * 1e3
+            return time.perf_counter()
+        return lap
+
+    def _sync(self):
+        torch.cuda.synchronize(self.device)                    # (the library works on its own streams)
+
+    def _pass1(self, lap):
+        """pass 1 over this rank's share, the job-wide fingerprint verdict (HM_EUNSUPPORTED on every rank for an
+        asymmetric table), the S index and the Bloom segments all-gathered in place -> (candidates, max_slice)"""
+        import ctypes as C
+        from . import _lib
+        L, h, g, W = self.L, self._h, self.group, self.world
+        self._pass1_done = False
+        t = time.perf_counter()
+        fp = (C.c_uint64 * 4)()
+        _lib.check(L.hm_rank_scan_pass1(h, fp))
+        t = lap("pass1", t)
+        acc = torch.tensor([v - (1 << 64) if v >= (1 << 63) else v for v in fp], dtype=torch.int64,
+                           device=self._coll_dev)
+        symmetric = fingerprint_verdict(acc, g)
+        nc, ms = C.c_int64(), C.c_int64()
+        _lib.check(L.hm_rank_scan_prepare(h, int(symmetric), C.byref(nc), C.byref(ms)))
+        t = lap("verdict_and_s_index", t)
+        seg, segb = C.c_void_p(), C.c_int64()
+        _lib.check(L.hm_rank_scan_bloom(h, C.byref(seg), C.byref(segb)))
+        if W > 1:
+            view = self._view(seg.value, W * segb.value).view(W, segb.value)
+            _in_place(lambda x: exchange_segments(x, self.rank, g), view, g)
+            self._sync()
+        lap("bloom_allgather", t)
+        self._pass1_done = True
+        return nc.value, ms.value
+
+    def _rounds(self, n_cand, max_slice, slices_fn, route_fn, settle_fn, lap):
+        """the slice every rank can hold, its buffers (slices_fn), then every round up to the most any rank needs:
+        route_fn(round, counts) -> the query keys all-to-all'ed to their owners -> answer -> the answer bytes
+        all-to-all'ed back -> settle_fn().  -> (rounds, slice, queries sent to each rank)"""
+        import ctypes as C
+        from . import _lib
+        L, h, g, W = self.L, self._h, self.group, self.world
+        kw = 2 if self.kmer > 32 else 1
+        t = time.perf_counter()
+        lim = torch.tensor([max_slice, -n_cand], dtype=torch.int64, device=self._coll_dev)
+        dist.all_reduce(lim, op=dist.ReduceOp.MIN, group=g)
+        slice_ = max(1, min(int(lim[0]), -int(lim[1])))        # the smallest room, no more than the most candidates
+        rounds = C.c_int64()
+        ptr = [C.c_void_p() for _ in range(4)]
+        _lib.check(slices_fn(h, slice_, C.byref(rounds), *[C.byref(p) for p in ptr]))
+        rt = torch.tensor([rounds.value], dtype=torch.int64, device=self._coll_dev)
+        dist.all_reduce(rt, op=dist.ReduceOp.MAX, group=g)
+        n_rounds = int(rt.item())
+        q = 2 * slice_
+        send = self._view(ptr[0].value, 8 * kw * q).view(torch.int64)
+        recv = self._view(ptr[1].value, 8 * kw * q * (W - 1)).view(torch.int64)
+        ans_recv = self._view(ptr[2].value, q * (W - 1))
+        ans_sent = self._view(ptr[3].value, q)
+        t = lap("slices", t)
+        counts = (C.c_int64 * W)()
+        sent_to = [0] * W
+        for rd in range(n_rounds):
+            _lib.check(route_fn(h, rd, counts))
+            t = lap("resolve", t)
+            if W > 1:
+                out_c = [int(c) for c in counts]
+                sc = torch.tensor(out_c, dtype=torch.int64, device=self._coll_dev)
+                rc = torch.empty_like(sc)
+                dist.all_to_all_single(rc, sc, group=g)
+                in_c = [int(c) for c in rc.tolist()]
+                ns, nr = sum(out_c), sum(in_c)
+                for r_, c in enumerate(out_c):
+                    sent_to[r_] += c
+                _all_to_all(recv[:kw * nr], send[:kw * ns], [kw * c for c in in_c], [kw * c for c in out_c], g)
+                self._sync()
+                t = lap("exchange_queries", t)
+                _lib.check(L.hm_rank_scan_answer(h, nr))
+                t = lap("answer", t)
+                _all_to_all(ans_sent[:ns], ans_recv[:nr], out_c, in_c, g)
+                self._sync()
+                t = lap("exchange_answers", t)
+            _lib.check(settle_fn(h))
+            t = lap("settle", t)
+        return n_rounds, slice_, sent_to
 
     def scan(self, timings: dict | None = None) -> torch.Tensor:
         import ctypes as C
         from . import _lib
         L, h, g, W = self.L, self._h, self.group, self.world
-        kw = 2 if self.kmer > 32 else 1
-        tm = {} if timings is None else timings
-        sync = lambda: torch.cuda.synchronize(self.device)     # noqa: E731  (the library works on its own streams)
-
-        def lap(name, t0):
-            tm[name] = tm.get(name, 0.0) + (time.perf_counter() - t0) * 1e3
-            return time.perf_counter()
-
+        lap = self._lap({} if timings is None else timings)
         with torch.cuda.device(self.device):
+            nc, ms = self._pass1(lap)
+            n_rounds, slice_, sent_to = self._rounds(nc, ms, L.hm_rank_scan_slices, L.hm_rank_scan_route,
+                                                     L.hm_rank_scan_settle, lap)
             t = time.perf_counter()
-            fp = (C.c_uint64 * 4)()
-            _lib.check(L.hm_rank_scan_pass1(h, fp))
-            t = lap("pass1", t)
-            acc = torch.tensor([v - (1 << 64) if v >= (1 << 63) else v for v in fp], dtype=torch.int64,
-                               device=self._coll_dev)
-            symmetric = fingerprint_verdict(acc, g)
-            nc, ms = C.c_int64(), C.c_int64()
-            _lib.check(L.hm_rank_scan_prepare(h, int(symmetric), C.byref(nc), C.byref(ms)))
-            t = lap("verdict_and_s_index", t)
-            seg, segb = C.c_void_p(), C.c_int64()
-            _lib.check(L.hm_rank_scan_bloom(h, C.byref(seg), C.byref(segb)))
-            if W > 1:
-                view = self._view(seg.value, W * segb.value).view(W, segb.value)
-                _in_place(lambda x: exchange_segments(x, self.rank, g), view, g)
-                sync()
-            t = lap("bloom_allgather", t)
-            lim = torch.tensor([ms.value, -nc.value], dtype=torch.int64, device=self._coll_dev)
-            dist.all_reduce(lim, op=dist.ReduceOp.MIN, group=g)
-            slice_ = max(1, min(int(lim[0]), -int(lim[1])))        # the smallest room, no more than the most candidates
-            rounds = C.c_int64()
-            ptr = [C.c_void_p() for _ in range(4)]
-            _lib.check(L.hm_rank_scan_slices(h, slice_, C.byref(rounds), *[C.byref(p) for p in ptr]))
-            rt = torch.tensor([rounds.value], dtype=torch.int64, device=self._coll_dev)
-            dist.all_reduce(rt, op=dist.ReduceOp.MAX, group=g)
-            n_rounds = int(rt.item())
-            q = 2 * slice_
-            send = self._view(ptr[0].value, 8 * kw * q).view(torch.int64)
-            recv = self._view(ptr[1].value, 8 * kw * q * (W - 1)).view(torch.int64)
-            ans_recv = self._view(ptr[2].value, q * (W - 1))
-            ans_sent = self._view(ptr[3].value, q)
-            t = lap("slices", t)
-            counts = (C.c_int64 * W)()
-            sent_to = [0] * W
-            for rd in range(n_rounds):
-                _lib.check(L.hm_rank_scan_route(h, rd, counts))
-                t = lap("resolve", t)
-                if W > 1:
-                    out_c = [int(c) for c in counts]
-                    sc = torch.tensor(out_c, dtype=torch.int64, device=self._coll_dev)
-                    rc = torch.empty_like(sc)
-                    dist.all_to_all_single(rc, sc, group=g)
-                    in_c = [int(c) for c in rc.tolist()]
-                    ns, nr = sum(out_c), sum(in_c)
-                    for r_, c in enumerate(out_c):
-                        sent_to[r_] += c
-                    _all_to_all(recv[:kw * nr], send[:kw * ns], [kw * c for c in in_c], [kw * c for c in out_c], g)
-                    sync()
-                    t = lap("exchange_queries", t)
-                    _lib.check(L.hm_rank_scan_answer(h, nr))
-                    t = lap("answer", t)
-                    _all_to_all(ans_sent[:ns], ans_recv[:nr], out_c, in_c, g)
-                    sync()
-                    t = lap("exchange_answers", t)
-                _lib.check(L.hm_rank_scan_settle(h))
-                t = lap("settle", t)
             dp, st = C.c_void_p(), C.c_uint64()
             _lib.check(L.hm_rank_scan_result(h, C.byref(dp), C.byref(st)))
             plot = self._view(dp.value, 8 * _lib.PLOT_CELLS).view(torch.int64)
             if W > 1:
                 _in_place(lambda x: allreduce_plot(x, g), plot, g)
-                sync()
+                self._sync()
             out = plot.clone().view(_lib.SMAX + 1, _lib.PLOT_W)
             lap("plot_allreduce", t)
         self.status = int(st.value)
-        self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms.value, "candidates": nc.value,
+        self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms, "candidates": nc,
                       "queries_sent_to": sent_to}
         return out
+
+    def extract(self, pixmap, dst: int = 0, timings: dict | None = None):
+        """extract_kmer_pairs' pair list for a pixel -> smudge map (uint16[SMAX+1, FMAX+1], label 0 = none): on rank
+        `dst` the structured array hetmers.Scan.extract returns for the table, the same records in the same order;
+        None on the other ranks.  Reuses the candidates of the last scan() (or extract()) when every rank left a
+        clean pass 1, else runs pass 1 first.  A Bloom hit on a key another rank owns is settled by that rank, as
+        in scan(); the records each rank lists are gathered on dst (gather_pairs).  stats["pass1_reused"] tells
+        which happened."""
+        import ctypes as C
+        import numpy as np
+        from . import _lib
+        from .hetmers import PAIR_DTYPE
+        L, h, g = self.L, self._h, self.group
+        pm = np.ascontiguousarray(pixmap, dtype=np.uint16).reshape(-1)
+        if pm.size != _lib.PLOT_CELLS:
+            raise ValueError(f"pixmap has {pm.size} cells, not {_lib.PLOT_CELLS}")
+        lap = self._lap({} if timings is None else timings)
+        with torch.cuda.device(self.device):
+            reuse = self._pass1_done and self.status == 0
+            if self.world > 1:                                  # (every rank must take the same branch)
+                bad = torch.tensor([int(not reuse)], dtype=torch.int32, device=self._coll_dev)
+                dist.all_reduce(bad, op=dist.ReduceOp.MAX, group=g)
+                reuse = int(bad.item()) == 0
+            if not reuse:
+                self.status = 0
+                self._pass1(lap)
+            t = time.perf_counter()
+            nc, ms = C.c_int64(), C.c_int64()
+            _lib.check(L.hm_rank_scan_extract_prepare(h, pm.ctypes.data, C.byref(nc), C.byref(ms)))
+            lap("extract_prepare", t)
+            n_rounds, slice_, sent_to = self._rounds(nc.value, ms.value, L.hm_rank_scan_extract_slices,
+                                                     L.hm_rank_scan_extract_route, L.hm_rank_scan_extract_settle, lap)
+            t = time.perf_counter()
+            out, n, st = C.POINTER(_lib.PairRec)(), C.c_int64(), C.c_uint64()
+            _lib.check(L.hm_rank_scan_extract_result(h, C.byref(out), C.byref(n), C.byref(st)))
+            recs = np.empty(n.value, dtype=PAIR_DTYPE)
+            if n.value:
+                C.memmove(recs.ctypes.data, out, n.value * PAIR_DTYPE.itemsize)
+            _libc_free(out)
+            t = lap("rank_sort", t)
+        self.status = int(st.value)
+        self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms.value, "candidates": nc.value,
+                      "queries_sent_to": sent_to, "pass1_reused": reuse, "records": int(n.value)}
+        if not self.symm_ok():
+            raise RuntimeError(f"rank {self.rank}: the routed pair listing ended with a non-zero status word on some "
+                               f"rank (here {self.status:#x}); its records must not be used")
+        res = gather_pairs(recs, dst, g)
+        lap("gather_and_sort", t)
+        return res
 
     def residency(self):
         """-> (peak device bytes since the last scan began, its chunks, the budget)"""

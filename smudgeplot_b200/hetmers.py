@@ -87,6 +87,11 @@ def run_extract(infile, sma, o="kmerpairs", t=4, verbose=False, tmp=".", gpus=No
 
 # ------------------------------------------------------------------ in-process (C ABI layer B) --
 
+# one record of extract_kmer_pairs' list (hm_pair_rec), as Scan.extract and dist.StreamedShardedScan.extract return it
+PAIR_DTYPE = np.dtype([("key_hi", "<u8"), ("key_lo", "<u8"), ("smudge", "<u4"), ("pos", "u1"), ("alt", "u1"),
+                       ("pad", "<u2")])
+
+
 def _host_table(kt: KtabFiles):
     """hm_host_table view over a KtabFiles (keeps the numpy buffers alive via the returned refs)."""
     index = np.ascontiguousarray(kt.index, dtype=np.int64)
@@ -162,8 +167,7 @@ class Scan:
         out = C.POINTER(_lib.PairRec)()
         n = C.c_int64()
         _lib.check(self._L.hm_scan_extract(self._h, pm.ctypes.data, C.byref(out), C.byref(n)))
-        dt = np.dtype([("key_hi", "<u8"), ("key_lo", "<u8"), ("smudge", "<u4"), ("pos", "u1"), ("alt", "u1"),
-                       ("pad", "<u2")])
+        dt = PAIR_DTYPE
         arr = np.empty(n.value, dtype=dt)
         if n.value:
             C.memmove(arr.ctypes.data, out, n.value * dt.itemsize)
