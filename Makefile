@@ -1,6 +1,7 @@
 # Build everything in-tree (artefacts are git-ignored):
 #   smudgeplot_b200/lib/libhetmers_b200.so   CUDA kernels (sm_90a, H100) + C ABI (include/hetmers_b200.h)
 #   smudgeplot_b200/bin/hetmers              the drop-in executable (plain C host)
+#   smudgeplot_b200/bin/condition_kmer_table trim + symmetrise a table of any size into new table files
 #   oracle/...                               the CPU checker (test infrastructure, see oracle/Makefile)
 NVCC   ?= nvcc
 CC     ?= gcc
@@ -12,10 +13,10 @@ LIBDIR := smudgeplot_b200/lib
 BINDIR := smudgeplot_b200/bin
 OBJDIR := build
 LIB    := $(LIBDIR)/libhetmers_b200.so
-BIN    := $(BINDIR)/hetmers $(BINDIR)/extract_kmer_pairs
+BIN    := $(BINDIR)/hetmers $(BINDIR)/extract_kmer_pairs $(BINDIR)/condition_kmer_table
 
 CU_SRC := smudgeplot_b200/csrc/hm_kernels.cu smudgeplot_b200/csrc/hm_scan.cu smudgeplot_b200/csrc/hm_peer.cu \
-          smudgeplot_b200/csrc/hm_condition.cu smudgeplot_b200/csrc/hm_symm.cu
+          smudgeplot_b200/csrc/hm_condition.cu smudgeplot_b200/csrc/hm_symm.cu smudgeplot_b200/csrc/hm_condition_files.cu
 CU_OBJ := $(patsubst smudgeplot_b200/csrc/%.cu,$(OBJDIR)/%.o,$(CU_SRC))
 C_OBJ  := $(OBJDIR)/fastk_table.o
 HDRS   := include/hetmers_b200.h smudgeplot_b200/csrc/hm_internal.h smudgeplot_b200/csrc/hm_device.cuh
@@ -46,6 +47,11 @@ $(BINDIR)/hetmers: smudgeplot_b200/host/hetmers_main.c $(LIB) $(HDRS)
 $(BINDIR)/extract_kmer_pairs: smudgeplot_b200/host/hetmers_main.c $(LIB) $(HDRS)
 	@mkdir -p $(BINDIR)
 	$(CC) $(CFLAGS) -DEXTRACT_PAIRS -o $@ $< -L$(LIBDIR) -lhetmers_b200 -Wl,-rpath,'$$ORIGIN/../lib'
+
+# conditioning of tables of any size into new table files (hm_scan_condition_files)
+$(BINDIR)/condition_kmer_table: smudgeplot_b200/host/condition_main.c $(LIB) $(HDRS)
+	@mkdir -p $(BINDIR)
+	$(CC) $(CFLAGS) -o $@ $< -L$(LIBDIR) -lhetmers_b200 -Wl,-rpath,'$$ORIGIN/../lib'
 
 oracle:
 	$(MAKE) -C oracle

@@ -416,6 +416,58 @@ int  hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t
 /* sort n records in place into hm_scan_extract's order: (smudge, key, position, alternative base) */
 int  hm_sort_pair_records(hm_pair_rec *records, int64_t n);
 
+/* ---- conditioning to table files, for tables of any size (csrc/hm_condition_files.cu, DESIGN.md §4d) ----
+ * hm_scan_condition_files writes what hm_scan_condition + hm_scan_download would give -- the source's entries
+ * with count >= ethresh (do_trim), plus every kept k-mer's reverse complement with the same count (do_symm),
+ * sorted, the original winning where both are present -- as the FastK table `dst` (same kmer, ibyte and parts
+ * as the source, parts cut on stub-index buckets).  It reads the table the scan was created from (that
+ * hm_host_table must still be valid), in or out of core alike, on dev[0], and leaves the scan as it was.  The
+ * source passes through the GPU once to histogram the output by key prefix (HM_COND_HIST_BITS bits of the
+ * first word), then once per key range of hm_condition_plan: each pass gathers the range's kept originals and
+ * reverse complements, sorts the latter, merges, packs FastK records and hands them to a host thread that
+ * writes them while the next range is gathered.  The call's own device bytes stay within what the scan's
+ * resident arrays leave of the budget set with hm_set_device_budget, or without one within what is free at the
+ * call minus HM_BUDGET_RESERVE.  Refused before any file is
+ * written: a scan conditioned in place (HM_EINVAL), a dst one of whose files is one of the source's part files
+ * (HM_EINVAL; seen through the part descriptors hm_table_open keeps open -- smudgeplot_b200.hetmers.Scan checks
+ * by name for the tables it reads), a budget below one range's smallest working set (HM_ENOMEM).                                                                */
+#define HM_COND_HIST_BITS 20                /* output histogram: 2^min(20, 2k) key prefixes         */
+#define HM_COND_MAX_RANGE (1ll << 31)       /* entries one range may hold                           */
+
+typedef struct hm_condition_stats
+  { int64_t nels_in, nels_out;
+    int32_t ranges, passes;                 /* key ranges; passes over the source (ranges + 1)      */
+    int64_t peak_bytes;                     /* most device bytes the call held                       */
+    int64_t bytes_read, bytes_written;      /* source bytes sent H2D; table bytes written            */
+    double  ms_hist, ms_ranges, ms_write, ms_total;   /* histogram pass; range passes (gather to pack); */
+                                            /*   host time writing (overlaps the next range); call  */
+    int64_t budget_bytes;                   /* the budget the call planned with: the one set less what */
+  } hm_condition_stats;                     /*   the scan holds, or free memory less the reserve      */
+
+typedef struct hm_condition_layout         /* what hm_condition_plan chooses                            */
+  { int64_t budget;
+    int64_t chunk;                          /* source entries per loaded chunk                           */
+    int64_t fixed_bytes;                    /* stub index, bucket counts, histogram, chunk + staging     */
+    int64_t range_room;                     /* bytes a range's working set may take: 3/4 of the budget   */
+                                            /*   minus the fixed part besides the chunk                  */
+    int64_t range_cap;                      /* entries of the largest range                              */
+    int64_t range_bytes;                    /* hm_condition_range_bytes(range_cap, ...)                  */
+    int32_t n_ranges, hist_bits;
+  } hm_condition_layout;
+
+/* device bytes of a range of t output entries at most (kept originals + reverse complements): the region
+ * both are gathered into and their FastK records; when symmetrising also the sort buffers (+ a uint32
+ * permutation pair for k > 32), the sort scratch, the merged table and the merge's tile counts           */
+int64_t hm_condition_range_bytes(int64_t t, int do_symm, int kmer, int ibyte);
+/* Cut the 2^hist_bits key prefixes into ranges: cuts[0] = 0 < cuts[1] < ... < cuts[n_ranges] = 2^hist_bits
+ * (cuts: room for 2^hist_bits + 1), greedily in key order, no range holding more than the entries whose
+ * hm_condition_range_bytes fits range_room.  hist: kept originals + (do_symm) their reverse complements
+ * per prefix.  HM_ENOMEM (with the sizes) if the fixed part or one prefix alone does not fit.             */
+int hm_condition_plan(int64_t n, int kmer, int ibyte, int64_t budget, int do_symm, const int64_t *hist,
+                      int hist_bits, int64_t *cuts, hm_condition_layout *out);
+int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
+                            hm_condition_stats *st);
+
 /* one call: create + run + destroy (what bench.py's e2e leg times) */
 int  hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,
                      int64_t *plot, hm_scan_stats *stats);
@@ -431,6 +483,22 @@ typedef struct hm_table hm_table;          /* parsed stub + mapped part payloads
 int  hm_table_open(const char *name, hm_table **out);
 void hm_table_close(hm_table *t);
 const hm_host_table *hm_table_view(const hm_table *t);
+
+/* Incremental table writer: stub int32 kmer, nparts, minval, ibyte + int64 index[1 << 8*ibyte]; parts
+ * ".<root>.ktab.<p>" with int32 kmer, int64 n (set on close).  Records (kbyte-ibyte suffix bytes, then a
+ * little-endian uint16 count) come in table order; hm_table_write_buckets announces the buckets the next
+ * records fill (counts[i] records for bucket b0+i; b0 at or after the last bucket announced, which it
+ * continues).  Parts end where fastk.write_ktab(cut_on_buckets=True) ends them for a table of nels_hint
+ * entries (byte-identical files when nels_hint is the exact count).  Files are written under temporary
+ * names and renamed into place by hm_table_write_close (the stub last); a failure, or
+ * hm_table_write_abort, leaves nothing under the final names.  close and abort free the writer.          */
+typedef struct hm_table_writer hm_table_writer;
+int  hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int nparts, int64_t nels_hint,
+                         hm_table_writer **out);
+int  hm_table_write_buckets(hm_table_writer *w, int64_t b0, int64_t nb, const int64_t *counts);
+int  hm_table_write_append(hm_table_writer *w, const uint8_t *rec, int64_t n);
+int  hm_table_write_close(hm_table_writer *w);
+void hm_table_write_abort(hm_table_writer *w);
 
 /* .smu writer: "min\t(sum-min)\tcount\n", sum-major, min < FMAX (PloidyPlot.c:1603-1617) */
 int  hm_write_smu(const char *path, const int64_t *plot);

@@ -31,6 +31,9 @@ ABI_SYMBOLS = [
     "hm_rank_scan_result", "hm_rank_scan_residency",
     "hm_rank_scan_extract_prepare", "hm_rank_scan_extract_slices", "hm_rank_scan_extract_route",
     "hm_rank_scan_extract_settle", "hm_rank_scan_extract_result", "hm_sort_pair_records",
+    "hm_condition_range_bytes", "hm_condition_plan", "hm_scan_condition_files",
+    "hm_table_write_open", "hm_table_write_buckets", "hm_table_write_append", "hm_table_write_close",
+    "hm_table_write_abort",
 ]
 
 
@@ -71,6 +74,26 @@ class StreamLayout(C.Structure):
     """hm_stream_layout: what the streamed scan plans for a table under a device budget"""
     _fields_ = [("budget", C.c_int64), ("chunk", C.c_int64), ("fixed_bytes", C.c_int64), ("chunk_bytes", C.c_int64),
                 ("list_bytes", C.c_int64), ("chunk_list_bytes", C.c_int64)]
+
+
+COND_HIST_BITS = 20
+
+
+class ConditionStats(C.Structure):
+    """hm_condition_stats: what hm_scan_condition_files did"""
+    _fields_ = [("nels_in", C.c_int64), ("nels_out", C.c_int64), ("ranges", C.c_int32), ("passes", C.c_int32),
+                ("peak_bytes", C.c_int64), ("bytes_read", C.c_int64), ("bytes_written", C.c_int64),
+                ("ms_hist", C.c_double), ("ms_ranges", C.c_double), ("ms_write", C.c_double), ("ms_total", C.c_double),
+                ("budget_bytes", C.c_int64)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class ConditionLayout(C.Structure):
+    """hm_condition_layout: what hm_condition_plan chooses for a table under a device budget"""
+    _fields_ = [("budget", C.c_int64), ("chunk", C.c_int64), ("fixed_bytes", C.c_int64), ("range_room", C.c_int64),
+                ("range_cap", C.c_int64), ("range_bytes", C.c_int64), ("n_ranges", C.c_int32), ("hist_bits", C.c_int32)]
 
 
 BUDGET_RESERVE = 1 << 30
@@ -190,6 +213,16 @@ def lib():
     L.hm_table_view.argtypes = [vp]
     L.hm_table_view.restype = C.POINTER(HostTable)
     L.hm_write_smu.argtypes = [C.c_char_p, vp]
+    L.hm_condition_range_bytes.argtypes = [i64, i32, i32, i32]
+    L.hm_condition_range_bytes.restype = i64
+    L.hm_condition_plan.argtypes = [i64, i32, i32, i64, i32, vp, i32, vp, C.POINTER(ConditionLayout)]
+    L.hm_scan_condition_files.argtypes = [vp, i32, i32, i32, C.c_char_p, C.POINTER(ConditionStats)]
+    L.hm_table_write_open.argtypes = [C.c_char_p, i32, i32, i32, i32, i64, C.POINTER(vp)]
+    L.hm_table_write_buckets.argtypes = [vp, i64, i64, vp]
+    L.hm_table_write_append.argtypes = [vp, vp, i64]
+    L.hm_table_write_close.argtypes = [vp]
+    L.hm_table_write_abort.argtypes = [vp]
+    L.hm_table_write_abort.restype = None
     _lib = L
     return L
 

@@ -106,6 +106,31 @@ int     hm_sort_keys(uint64_t *keys, uint64_t *lo, int64_t n, int kmer, void *sc
                      cudaStream_t st);
 /* device bytes hm_condition_arrays borrows besides the table it is given                              */
 int64_t hm_condition_bytes(int kmer, int64_t n, int do_trim, int do_symm);
+/* conditioning to files (hm_condition_files.cu, driven by hm_scan_condition_files): the device buffers of one
+ * range of at most `cap` output entries.  key / lo / cnt: the region the kept originals fill from the front
+ * and the reverse complements from the back; alt_*, idx: sort buffers; m_*: the merged range; rec: its
+ * records; bcount: stub-bucket counts; ctr: [0] originals, [1] reverse complements, [3] overflow, [4..5]
+ * merge scratch                                                                                             */
+typedef struct hm_cond_bufs
+  { int       kmer, ibyte, hb, ethresh, do_symm;
+    int64_t   cap;
+    uint64_t *key, *lo, *alt_key, *alt_lo, *m_key, *m_lo;
+    uint16_t *cnt, *alt_cnt, *m_cnt;
+    uint32_t *idx[2];
+    uint8_t  *rec;
+    unsigned long long *mtiles, *ctr, *bcount;
+    void     *sort_tmp;
+    int64_t   sort_bytes;
+  } hm_cond_bufs;
+
+int hm_cond_hist(const uint64_t *keys, const uint64_t *klo, const uint16_t *cnt, int64_t m, int kmer, int ethresh,
+                 int do_symm, int hb, unsigned long long *hist, cudaStream_t st);
+int hm_cond_gather(const uint64_t *keys, const uint64_t *klo, const uint16_t *cnt, int64_t m, const hm_cond_bufs *B,
+                   uint64_t p0, uint64_t p1, unsigned long long *tiles, cudaStream_t st);
+int hm_cond_finish(const hm_cond_bufs *B, uint64_t b0, int64_t nb, int64_t *n_out, cudaStream_t st);
+int64_t hm_cond_chunk(int64_t n, int kmer, int ibyte, int64_t budget);
+int64_t hm_cond_tiles_bytes(int64_t n);
+int64_t hm_cond_sort_room(int64_t c);
 #define HM_CUDA(call)                                              \
   do { cudaError_t _e = (call);                                    \
        if (_e != cudaSuccess) return hm_cuda_fail(_e,#call);       \

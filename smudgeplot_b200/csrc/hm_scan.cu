@@ -29,6 +29,7 @@
 #include <pthread.h>
 #include <unistd.h>
 #include <errno.h>
+#include <sys/stat.h>
 
 #include "hetmers_b200.h"
 #include "hm_internal.h"
@@ -76,6 +77,8 @@ struct hm_scan
                                           /*   (what hm_scan_extract lists the pairs from)                    */
     int      last_path;                   /* HM_PATH_DIRECT / HM_PATH_SYMM of the last run                  */
     int      invalid;                     /* a failed conditioning left the replicas inconsistent            */
+    int      conditioned;                 /* hm_scan_condition changed the table: its files no longer describe it */
+    const hm_host_table *src;             /* the table hm_scan_create was given (hm_scan_condition_files reads it) */
     hm_symm_shards ssh[HM_MAX_GPUS];
     uint64_t seed[2];
     /* residency (DESIGN.md §4c) */
@@ -824,7 +827,7 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   hm_scan *s = (hm_scan *) calloc(1,sizeof(hm_scan));
   if (s == NULL)
     return hm_set_error(HM_ENOMEM,"out of host memory");
-  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = t->nels; s->ngpu = n_gpus; s->nshard = n_gpus;
+  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = t->nels; s->ngpu = n_gpus; s->nshard = n_gpus; s->src = t;
   s->bits  = hm_pick_bucket_bits(s->n);
   s->fpos  = hm_pick_filter_bits(s->n);
   s->idx64 = (s->n >= 0xFFFFFFF0ll);
@@ -1012,6 +1015,7 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
                           "budget of %lld",(long long) s->n,(long long) need,(long long) s->budget);
   }
   /* everything derived from the old table goes first: work buffers of both paths, the index */
+  s->conditioned = 1;
   s->ran = 0; s->have_direct = 0; s->have_symm = 0; s->symm_ready = 0;
   if ((rc = sync_all(s,"conditioning")) != HM_OK)
     return rc;
@@ -1088,6 +1092,244 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
     s->invalid = 1;
   if (nels_out) *nels_out = s->n;
   return rc_cond != HM_OK ? rc_cond : rc;
+}
+
+/* ---- conditioning into table files (DESIGN.md §4d; kernels and plan in hm_condition_files.cu) ----------- */
+
+/* 1 if the table `dst` would be written over holds one of the source's part files */
+static int names_source(const hm_host_table *t, const char *dst)
+{ hm_table *d = NULL;
+  int       same = 0;
+  if (t->part_fd == NULL || hm_table_open(dst,&d) != HM_OK)
+    return 0;
+  const hm_host_table *v = hm_table_view(d);
+  for (int p = 0; p < v->nparts && !same; p++)
+    for (int q = 0; q < t->nparts && !same; q++)
+      { struct stat a, b;
+        if (v->part_fd[p] >= 0 && t->part_fd[q] >= 0 && fstat(v->part_fd[p],&a) == 0 && fstat(t->part_fd[q],&b) == 0)
+          same = (a.st_dev == b.st_dev && a.st_ino == b.st_ino);
+      }
+  hm_table_close(d);
+  return same;
+}
+
+/* one range's records, from the device to the table files on a host thread: pinned pieces, the copy of the next
+ * piece overlapping the write of this one                                                                  */
+typedef struct
+  { int             dev, pbyte, rc;
+    hm_table_writer *w;
+    const uint8_t  *d_rec;
+    int64_t         n, b0, nb, *counts, pin_bytes;
+    uint8_t        *pin[2];
+    cudaStream_t    st;
+    double          ms;
+    char            msg[512];
+  } WriteJob;
+
+static void *write_worker(void *p)
+{ WriteJob *J = (WriteJob *) p;
+  double    t0 = now_ms();
+  int64_t   per = J->pin_bytes/J->pbyte;
+  cudaError_t e = cudaSetDevice(J->dev);
+  J->rc = e != cudaSuccess ? hm_cuda_fail(e,"writer thread") : hm_table_write_buckets(J->w,J->b0,J->nb,J->counts);
+  if (J->rc == HM_OK && J->n > 0)
+    { e = cudaMemcpyAsync(J->pin[0],J->d_rec,(size_t) ((J->n < per ? J->n : per)*J->pbyte),cudaMemcpyDeviceToHost,J->st);
+      for (int64_t o = 0, i = 0; o < J->n && J->rc == HM_OK; o += per, i++)
+        { int64_t m = J->n-o < per ? J->n-o : per;
+          if (e == cudaSuccess) e = cudaStreamSynchronize(J->st);
+          if (e == cudaSuccess && o+per < J->n)
+            { int64_t m2 = J->n-o-per < per ? J->n-o-per : per;
+              e = cudaMemcpyAsync(J->pin[(i+1)&1],J->d_rec+(o+per)*J->pbyte,(size_t) (m2*J->pbyte),cudaMemcpyDeviceToHost,J->st);
+            }
+          if (e != cudaSuccess) { J->rc = hm_cuda_fail(e,"records to the host"); break; }
+          J->rc = hm_table_write_append(J->w,J->pin[i&1],m);
+        }
+      cudaStreamSynchronize(J->st);
+    }
+  if (J->rc != HM_OK)
+    { strncpy(J->msg,hm_last_error(),sizeof(J->msg)-1); J->msg[sizeof(J->msg)-1] = 0; }
+  J->ms += now_ms()-t0;
+  return NULL;
+}
+
+extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
+                                       hm_condition_stats *st)
+{ double t0 = now_ms();
+  if (s == NULL || dst == NULL)
+    return hm_set_error(HM_EINVAL,"hm_scan_condition_files: NULL argument");
+  if (s->conditioned || s->invalid)
+    return hm_set_error(HM_EINVAL,"this scan's table was conditioned in place: the files it was created from no longer "
+                        "describe it");
+  if (!do_trim && !do_symm)
+    return hm_set_error(HM_EINVAL,"hm_scan_condition_files: neither trimming nor symmetrising was asked for");
+  const hm_host_table *t = s->src;
+  if (names_source(t,dst))
+    return hm_set_error(HM_EINVAL,"%s names the source table: conditioning writes a new table",dst);
+
+  DevTable *D = s->d;
+  const int kmer = s->kmer, ibyte = t->ibyte, KW = kmer > 32 ? 2 : 1;
+  const int pbyte = ((kmer+3)>>2) - ibyte + 2;
+  const int hb = 2*kmer < HM_COND_HIST_BITS ? 2*kmer : HM_COND_HIST_BITS;
+  const int64_t n = t->nels, np = (int64_t) 1 << hb, ixlen = (int64_t) 1 << (8*ibyte);
+  const int ethr = do_trim ? ethresh : 0;
+  int       rc = HM_OK;
+  cudaError_t e;
+  HM_CUDA(cudaSetDevice(D->dev));
+  /* what the call may hold: an explicit budget covers the scan too (as hm_scan_condition counts its table), so
+   * the scan's resident arrays come off it; the default one is free memory, which already excludes them       */
+  const int64_t budget = g_budget > 0 ? g_budget - D->held : device_budget(&D->dev,1);
+
+  hm_condition_stats S;
+  memset(&S,0,sizeof(S));
+  S.nels_in = n;
+  S.budget_bytes = budget;
+  hm_condition_layout lay;
+  int64_t *hist = (int64_t *) calloc((size_t) np,sizeof(int64_t));
+  int64_t *cuts = (int64_t *) malloc(sizeof(int64_t)*(size_t) (np+1));
+  int64_t *hcnt = (int64_t *) malloc(sizeof(int64_t)*(size_t) ixlen);
+  if (hist == NULL || cuts == NULL || hcnt == NULL)
+    { free(hist); free(cuts); free(hcnt); return hm_set_error(HM_ENOMEM,"out of host memory"); }
+  /* the fixed part and a chunk must fit before the source is read (an empty histogram asks nothing more) */
+  if ((rc = hm_condition_plan(n,kmer,ibyte,budget,do_symm,hist,hb,cuts,&lay)) != HM_OK)
+    { free(hist); free(cuts); free(hcnt); return rc; }
+  const int64_t chunk = lay.chunk;
+
+  const int64_t held0 = D->held, peak0 = D->peak;
+  D->peak = D->held;
+  hm_cond_bufs B;
+  memset(&B,0,sizeof(B));
+  B.kmer = kmer; B.ibyte = ibyte; B.hb = hb; B.ethresh = ethr; B.do_symm = do_symm;
+  int64_t *d_index = NULL;
+  uint64_t *ck = NULL, *cl = NULL;
+  uint16_t *cc = NULL;
+  unsigned long long *d_hist = NULL, *tiles = NULL;
+  Stager    G;
+  memset(&G,0,sizeof(G));
+  hm_table_writer *w = NULL;
+  WriteJob  J;
+  memset(&J,0,sizeof(J));
+  pthread_t th;
+  int       writing = 0;
+  TRY(dev_alloc(D,&d_index,8*ixlen));
+  TRY(dev_alloc(D,&B.bcount,8*ixlen));
+  TRY(dev_alloc(D,&d_hist,8*np));
+  TRY(dev_alloc(D,&B.ctr,256));
+  TRY(dev_alloc(D,&ck,8*(chunk+1)));
+  if (KW == 2) TRY(dev_alloc(D,&cl,8*(chunk+1)));
+  TRY(dev_alloc(D,&cc,2*(chunk+8)));
+  TRY(dev_alloc(D,&tiles,hm_cond_tiles_bytes(chunk)));
+  TRY(cudaMemcpyAsync(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,D->st));
+  TRY(cudaMemsetAsync(d_hist,0,8*(size_t) np,D->st));
+  if (rc == HM_OK)
+    rc = stager_open(s,D,t,chunk,&G);
+
+  /* pass 0: the output histogram */
+  for (int64_t o = 0; o < n && rc == HM_OK; o += chunk)
+    { int64_t m = n-o < chunk ? n-o : chunk;
+      rc = load_into(s,D,t,d_index,o,m,ck,cl,cc,0,&G);
+      if (rc == HM_OK) rc = hm_cond_hist(ck,cl,cc,m,kmer,ethr,do_symm,hb,d_hist,D->st);
+    }
+  TRY(cudaMemcpyAsync(hist,d_hist,8*(size_t) np,cudaMemcpyDeviceToHost,D->st));
+  TRY(cudaStreamSynchronize(D->st));
+  S.ms_hist = now_ms()-t0;
+  if (rc == HM_OK)
+    rc = hm_condition_plan(n,kmer,ibyte,budget,do_symm,hist,hb,cuts,&lay);
+  int64_t hint = 0;
+  for (int64_t p = 0; p < np; p++) hint += hist[p];
+
+  /* the range buffers, sized for the largest range */
+  const int64_t T = lay.range_cap > 0 ? lay.range_cap : 1;
+  B.cap = T;
+  TRY(dev_alloc(D,&B.key,8*T));
+  if (KW == 2) TRY(dev_alloc(D,&B.lo,8*T));
+  TRY(dev_alloc(D,&B.cnt,2*T));
+  TRY(dev_alloc(D,&B.rec,pbyte*T));
+  if (do_symm)
+    { TRY(dev_alloc(D,&B.alt_key,8*T));
+      TRY(dev_alloc(D,&B.alt_cnt,2*T));
+      TRY(dev_alloc(D,&B.m_key,8*T));
+      TRY(dev_alloc(D,&B.m_cnt,2*T));
+      if (KW == 2)
+        { TRY(dev_alloc(D,&B.alt_lo,8*T));
+          TRY(dev_alloc(D,&B.m_lo,8*T));
+          TRY(dev_alloc(D,&B.idx[0],4*T));
+          TRY(dev_alloc(D,&B.idx[1],4*T));
+        }
+      TRY(dev_alloc(D,&B.mtiles,2*hm_cond_tiles_bytes(T)));
+      B.sort_bytes = hm_cond_sort_room(T);
+      TRY(dev_alloc(D,&B.sort_tmp,B.sort_bytes));
+    }
+  if (rc == HM_OK)
+    rc = hm_table_write_open(dst,kmer,ibyte,do_trim && ethresh > t->minval ? ethresh : t->minval,
+                             t->nparts > 0 ? t->nparts : 1,hint,&w);
+  if (rc == HM_OK)
+    { J.dev = D->dev; J.pbyte = pbyte; J.w = w; J.d_rec = B.rec;
+      J.pin_bytes = (int64_t) pbyte*((64ll << 20)/pbyte);
+      TRY(cudaStreamCreateWithFlags(&J.st,cudaStreamNonBlocking));
+      TRY(cudaHostAlloc(&J.pin[0],(size_t) J.pin_bytes,cudaHostAllocDefault));
+      TRY(cudaHostAlloc(&J.pin[1],(size_t) J.pin_bytes,cudaHostAllocDefault));
+    }
+
+  /* passes 1..R: a key range each */
+  double t_ranges = now_ms();
+  for (int r = 0; r < lay.n_ranges && rc == HM_OK; r++)
+    { const uint64_t p0 = (uint64_t) cuts[r], p1 = (uint64_t) cuts[r+1];
+      TRY(cudaMemsetAsync(B.ctr,0,256,D->st));
+      for (int64_t o = 0; o < n && rc == HM_OK; o += chunk)
+        { int64_t m = n-o < chunk ? n-o : chunk;
+          rc = load_into(s,D,t,d_index,o,m,ck,cl,cc,0,&G);
+          if (rc == HM_OK) rc = hm_cond_gather(ck,cl,cc,m,&B,p0,p1,tiles,D->st);
+        }
+      /* the stub buckets the range's keys fall in */
+      const uint64_t b0 = 8*ibyte >= hb ? p0 << (8*ibyte-hb) : p0 >> (hb-8*ibyte);
+      const uint64_t b1 = 8*ibyte >= hb ? p1 << (8*ibyte-hb) : ((p1-1) >> (hb-8*ibyte)) + 1;
+      if (writing)                                             /* the last range's records have left B.rec */
+        { pthread_join(th,NULL); writing = 0;
+          if (J.rc != HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
+        }
+      int64_t n_r = 0;
+      if (rc == HM_OK) rc = hm_cond_finish(&B,b0,(int64_t) (b1-b0),&n_r,D->st);
+      TRY(cudaMemcpy(hcnt,B.bcount,8*(size_t) (b1-b0),cudaMemcpyDeviceToHost));
+      if (rc == HM_OK)
+        { J.n = n_r; J.b0 = (int64_t) b0; J.nb = (int64_t) (b1-b0); J.counts = hcnt;
+          S.nels_out += n_r;
+          if (pthread_create(&th,NULL,write_worker,&J) == 0) writing = 1;
+          else                                                write_worker(&J);
+          if (!writing && J.rc != HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
+        }
+      S.ranges++;
+    }
+  if (writing)
+    { pthread_join(th,NULL);
+      if (J.rc != HM_OK && rc == HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
+    }
+  S.ms_ranges = now_ms()-t_ranges;
+  if (w != NULL)
+    { int rw = rc == HM_OK ? hm_table_write_close(w) : (hm_table_write_abort(w), HM_OK);
+      if (rc == HM_OK) rc = rw;
+    }
+
+  /* everything the call allocated goes; the scan's own residency report is left as it was */
+  stager_close(D,&G);
+  cudaStreamSynchronize(D->st);
+  void *mine[] = { d_index, B.bcount, d_hist, B.ctr, ck, cl, cc, tiles, B.key, B.lo, B.cnt, B.rec, B.alt_key, B.alt_cnt,
+                   B.m_key, B.m_cnt, B.alt_lo, B.m_lo, B.idx[0], B.idx[1], B.mtiles, B.sort_tmp };
+  for (size_t k = 0; k < sizeof(mine)/sizeof(mine[0]); k++)
+    dev_free(D,mine[k]);
+  cudaStreamSynchronize(D->st);
+  if (J.st) cudaStreamDestroy(J.st);
+  if (J.pin[0]) cudaFreeHost(J.pin[0]);
+  if (J.pin[1]) cudaFreeHost(J.pin[1]);
+  S.peak_bytes = D->peak-held0;
+  D->peak = peak0 > D->held ? peak0 : D->held;
+  free(hist); free(cuts); free(hcnt);
+  S.passes = S.ranges+1;
+  S.bytes_read = (int64_t) S.passes*n*pbyte;
+  S.bytes_written = 16 + 8*ixlen + 12ll*(t->nparts > 0 ? t->nparts : 1) + S.nels_out*pbyte;
+  S.ms_write = J.ms;
+  S.ms_total = now_ms()-t0;
+  if (st != NULL) *st = S;
+  return rc;
 }
 
 /* reverse complement of a left-aligned packed k-mer (k <= 32) */

@@ -56,6 +56,7 @@ class KtabFiles:
     index: np.ndarray                      # int64[1 << 8*ibyte]
     part_nels: list = field(default_factory=list)
     records: list = field(default_factory=list)   # per part: uint8[n*pbyte] (payload, header stripped)
+    name: str | None = None                # the table's files (read_ktab / write_ktab), None if built in memory
 
     @property
     def kbyte(self) -> int:
@@ -94,7 +95,7 @@ def read_ktab(name: str, mmap: bool = False) -> KtabFiles:
         index = np.fromfile(f, dtype="<i8", count=ixlen)
         if index.size != ixlen:
             raise ValueError(f"{sp}: truncated prefix index")
-    kt = KtabFiles(kmer, nparts, minval, ibyte, index)
+    kt = KtabFiles(kmer, nparts, minval, ibyte, index, name=name)
     for p in range(1, nparts + 1):
         pp = part_path(name, p)
         if not os.path.exists(pp):
@@ -185,7 +186,7 @@ def write_ktab(name: str, kmer: int, keys: np.ndarray, cnt: np.ndarray, ibyte: i
     with open(stub_path(name), "wb") as f:
         f.write(struct.pack("<4i", kmer, nparts, minval, ibyte))
         index.tofile(f)
-    kt = KtabFiles(kmer, nparts, minval, ibyte, index)
+    kt = KtabFiles(kmer, nparts, minval, ibyte, index, name=name)
     for p in range(1, nparts + 1):
         lo, hi = cuts[p - 1], cuts[p]
         with open(part_path(name, p), "wb") as f:
@@ -194,6 +195,16 @@ def write_ktab(name: str, kmer: int, keys: np.ndarray, cnt: np.ndarray, ibyte: i
         kt.part_nels.append(hi - lo)
         kt.records.append(rec[lo:hi].reshape(-1))
     return kt
+
+
+def same_table_files(a: str, a_parts: int, b: str) -> bool:
+    """whether writing table `b` would write over a file of table `a` (a_parts parts): its stub or one of its
+    parts is one of a's files (any spelling of the name, links included)"""
+    mine = [stub_path(a)] + [part_path(a, p) for p in range(1, a_parts + 1)]
+    mine = [os.stat(f) for f in mine if os.path.exists(f)]
+    ids = {(st.st_dev, st.st_ino) for st in mine}
+    theirs = [stub_path(b)] + [part_path(b, p) for p in range(1, max(a_parts, 1) + 1)]
+    return any((os.stat(f).st_dev, os.stat(f).st_ino) in ids for f in theirs if os.path.exists(f))
 
 
 def remove_ktab(name: str) -> None:

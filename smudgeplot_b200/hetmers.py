@@ -137,6 +137,23 @@ class Scan:
         self.nels = n.value
         return n.value
 
+    def condition_files(self, dst: str, ethresh: int, trim: bool, symm: bool, device_budget: int | None = None):
+        """write the trimmed (count >= ethresh) and / or symmetrised table as the FastK table `dst`, one key range
+        at a time on the first GPU, for a table of any size (hm_scan_condition_files); the scan itself is left as
+        it was.  A `dst` whose files are the source's (kt.name) is refused (HM_EINVAL) before anything is written.
+        device_budget sets the process-wide device budget (bytes per GPU, as Scan's does) for this and later calls;
+        an explicit budget counts what the scan already holds on the device.
+        -> stats dict (entries in / out, ranges, passes, peak device bytes, bytes read / written, times)"""
+        from .fastk import same_table_files
+        if self.kt.name is not None and same_table_files(self.kt.name, self.kt.nparts, str(dst)):
+            raise _lib.HetmersError(-1, f"{dst} names the source table: conditioning writes a new table")
+        if device_budget is not None:
+            self._L.hm_set_device_budget(int(device_budget))
+        st = _lib.ConditionStats()
+        _lib.check(self._L.hm_scan_condition_files(self._h, int(ethresh), int(trim), int(symm), str(dst).encode(),
+                                                   C.byref(st)))
+        return st.as_dict()
+
     PATHS = {"auto": 0, "direct": 1, "symm": 2}
 
     def residency(self):
@@ -216,6 +233,20 @@ def scan_table(kt: KtabFiles, gpus: int = 1):
     _lib.check(L.hm_hetmers_host(C.byref(ht), devs, gpus, plot.ctypes.data, C.byref(st)))
     del keep
     return plot.reshape(_lib.SMAX + 1, _lib.PLOT_W), st.as_dict()
+
+
+def condition_table(src, dst, L: int, device_budget: int | None = None):
+    """`condition_kmer_table` in process: examine `src` as hetmers does (-e L) and write it trimmed and / or
+    symmetrised as needed to `dst`, streaming it through the GPU if it is larger.  device_budget sets the
+    process-wide device budget, as Scan's does.  -> stats dict, or None when the table needs neither step
+    (nothing is written).  A `dst` naming `src` is refused (HM_EINVAL) before anything is written."""
+    if device_budget is not None:
+        _lib.lib().hm_set_device_budget(int(device_budget))
+    with Scan(read_ktab(str(src), mmap=True)) as sc:
+        trim, symm = sc.examine(int(L))
+        if trim and symm:
+            return None
+        return sc.condition_files(dst, int(L), not trim, not symm)
 
 
 def smu_text(plot: np.ndarray) -> str:

@@ -189,6 +189,271 @@ fail:
   return rc;
 }
 
+/* ---- incremental writer ------------------------------------------------------------------------
+ * Records arrive in table order, announced bucket by bucket (hm_table_write_buckets) before they are
+ * appended.  Part q (q = 1..nparts-1) ends where fastk.write_ktab(cut_on_buckets=True) ends it for a
+ * table of nels_hint entries: at the start of the bucket holding ordinal nels_hint*q/nparts (the last
+ * bucket's start when there are fewer entries).  That bucket may have begun before the ordinal is
+ * reached, so a cut moves the bucket's records written so far from the old part to the new one --
+ * at most one bucket's worth per part.  Everything is written under temporary names and renamed into
+ * place by hm_table_write_close; any failure removes the temporaries.                             */
+struct hm_table_writer
+  { int      kmer, ibyte, minval, nparts, pbyte, part;   /* part: the one being written (0-based)  */
+    int64_t  hint, ixlen;
+    int64_t *count;                    /* records per bucket, as announced                         */
+    int64_t  declared, written, last;  /* records announced / appended; last bucket announced      */
+    int64_t  cur, cur_start, cur_left; /* bucket being appended, its first ordinal, records to come */
+    int64_t *part_first;               /* [nparts] first ordinal of each part                      */
+    int     *fd;                       /* [nparts] temporary part files                            */
+    char    *dir, *root, *tmp_tag;
+    int      failed;
+  };
+
+static char *writer_path(const hm_table_writer *w, int part, int tmp)   /* part 0 = the stub */
+{ size_t len = strlen(w->dir)+strlen(w->root)+strlen(w->tmp_tag)+48;
+  char  *p = malloc(len);
+  if (p == NULL)
+    return NULL;
+  if (part == 0) snprintf(p,len,"%s/%s.ktab%s",w->dir,w->root,tmp ? w->tmp_tag : "");
+  else           snprintf(p,len,"%s/.%s.ktab.%d%s",w->dir,w->root,part,tmp ? w->tmp_tag : "");
+  return p;
+}
+
+static int pwrite_all(int fd, const void *buf, size_t len, off_t off)
+{ const char *b = (const char *) buf;
+  while (len > 0)
+    { ssize_t r = pwrite(fd,b,len,off);
+      if (r <= 0) return -1;
+      b += r; len -= (size_t) r; off += r;
+    }
+  return 0;
+}
+
+static void writer_free(hm_table_writer *w, int unlink_tmp)
+{ if (w == NULL)
+    return;
+  for (int p = 0; p < w->nparts && w->fd != NULL; p++)
+    { if (w->fd[p] >= 0) close(w->fd[p]);
+      if (unlink_tmp)
+        { char *q = writer_path(w,p+1,1);
+          if (q != NULL) { unlink(q); free(q); }
+        }
+    }
+  if (unlink_tmp && w->dir != NULL)
+    { char *q = writer_path(w,0,1);
+      if (q != NULL) { unlink(q); free(q); }
+    }
+  free(w->count); free(w->part_first); free(w->fd); free(w->dir); free(w->root); free(w->tmp_tag);
+  free(w);
+}
+
+void hm_table_write_abort(hm_table_writer *w) { writer_free(w,1); }
+
+int hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int nparts, int64_t nels_hint,
+                        hm_table_writer **out)
+{ hm_table_writer *w;
+  if (name == NULL || out == NULL || kmer < 1 || ibyte < 1 || ibyte > 3 || ibyte > ((kmer+3)>>2) ||
+      nparts < 1 || nels_hint < 0)
+    return hm_set_error(HM_EINVAL,"hm_table_write_open: bad arguments");
+  *out = NULL;
+  w = calloc(1,sizeof(*w));
+  if (w == NULL)
+    return hm_set_error(HM_ENOMEM,"Out of memory (table writer)");
+  w->kmer = kmer; w->ibyte = ibyte; w->minval = minval; w->nparts = nparts; w->hint = nels_hint;
+  w->pbyte = ((kmer+3)>>2) - ibyte + 2;
+  w->ixlen = (int64_t) 1 << (8*ibyte);
+  w->cur = -1;
+  w->count      = calloc((size_t) w->ixlen,sizeof(int64_t));
+  w->part_first = calloc((size_t) nparts,sizeof(int64_t));
+  w->fd         = malloc(sizeof(int)*(size_t) nparts);
+  w->dir        = malloc(strlen(name)+8);
+  w->root       = malloc(strlen(name)+8);
+  w->tmp_tag    = malloc(64);
+  if (w->count == NULL || w->part_first == NULL || w->fd == NULL || w->dir == NULL || w->root == NULL ||
+      w->tmp_tag == NULL)
+    { writer_free(w,0); return hm_set_error(HM_ENOMEM,"Out of memory (table writer)"); }
+  for (int p = 0; p < nparts; p++) w->fd[p] = -1;
+  split_name(name,w->dir,w->root);
+  snprintf(w->tmp_tag,64,".tmp%ld",(long) getpid());
+  for (int p = 0; p < nparts; p++)
+    { char   *q = writer_path(w,p+1,1);
+      char    head[PART_HEADER];
+      int32_t k32 = kmer;
+      int64_t zero = 0;
+      if (q == NULL)
+        { writer_free(w,1); return hm_set_error(HM_ENOMEM,"Out of memory (table writer)"); }
+      w->fd[p] = open(q,O_RDWR|O_CREAT|O_TRUNC,0644);
+      memcpy(head,&k32,4); memcpy(head+4,&zero,8);
+      if (w->fd[p] < 0 || pwrite_all(w->fd[p],head,PART_HEADER,0) != 0)
+        { int rc = hm_set_error(HM_EIO,"Cannot create %s: %s",q,strerror(errno));
+          free(q); writer_free(w,1);
+          return rc;
+        }
+      free(q);
+    }
+  *out = w;
+  return HM_OK;
+}
+
+int hm_table_write_buckets(hm_table_writer *w, int64_t b0, int64_t nb, const int64_t *counts)
+{ if (w == NULL || w->failed)
+    return hm_set_error(HM_EINVAL,"hm_table_write_buckets: no usable writer");
+  for (int64_t i = 0; i < nb; i++)
+    { int64_t b = b0+i;
+      if (counts[i] == 0)
+        continue;
+      if (b < 0 || b >= w->ixlen || counts[i] < 0 || b < w->last)
+        { w->failed = 1;
+          return hm_set_error(HM_EINVAL,"hm_table_write_buckets: bucket %lld announced out of order",(long long) b);
+        }
+      w->count[b] += counts[i];
+      w->declared += counts[i];
+      w->last = b;
+      if (b == w->cur)                                      /* more of the bucket being appended */
+        w->cur_left += counts[i];
+    }
+  return HM_OK;
+}
+
+/* part w->part+1 begins at ordinal `at` (<= written): the records [at, written) move into it */
+static int writer_cut(hm_table_writer *w, int64_t at)
+{ int     p = w->part, q = p+1;
+  int64_t moved = w->written-at;
+  off_t   src = PART_HEADER + (off_t) (at-w->part_first[p])*w->pbyte;
+  char    buf[1 << 16];
+  int64_t left = moved*w->pbyte;
+  off_t   o = 0;
+  while (left > 0)
+    { size_t  m = left < (int64_t) sizeof(buf) ? (size_t) left : sizeof(buf);
+      ssize_t r = pread(w->fd[p],buf,m,src+o);
+      if (r != (ssize_t) m || pwrite_all(w->fd[q],buf,m,PART_HEADER+o) != 0)
+        return hm_set_error(HM_EIO,"writing table part %d: %s",q+1,strerror(errno));
+      o += (off_t) m; left -= (int64_t) m;
+    }
+  if (ftruncate(w->fd[p],src) != 0)
+    return hm_set_error(HM_EIO,"writing table part %d: %s",p+1,strerror(errno));
+  w->part = q;
+  w->part_first[q] = at;
+  return HM_OK;
+}
+
+/* the ordinal part q+1 is cut at (write_ktab's c = n*q/nparts), for q = w->part+1 */
+static int64_t writer_target(const hm_table_writer *w, int q)
+{ return (int64_t) ((__int128) w->hint*q/w->nparts); }
+
+/* records [from, w->written) of the current part, held at rec, go to its file in one write */
+static int writer_flush(hm_table_writer *w, const uint8_t *rec, int64_t from)
+{ if (w->written > from &&
+      pwrite_all(w->fd[w->part],rec,(size_t) (w->written-from)*w->pbyte,
+                 PART_HEADER + (off_t) (from-w->part_first[w->part])*w->pbyte) != 0)
+    return hm_set_error(HM_EIO,"writing table part %d: %s",w->part+1,strerror(errno));
+  return HM_OK;
+}
+
+int hm_table_write_append(hm_table_writer *w, const uint8_t *rec, int64_t n)
+{ if (w == NULL || w->failed)
+    return hm_set_error(HM_EINVAL,"hm_table_write_append: no usable writer");
+  if (w->written+n > w->declared)
+    { w->failed = 1;
+      return hm_set_error(HM_EINVAL,"hm_table_write_append: %lld records beyond the announced buckets",
+                          (long long) (w->written+n-w->declared));
+    }
+  int64_t from = w->written;                                /* not yet in a file: [from, written) at rec */
+  while (n > 0)
+    { if (w->cur_left == 0)                                 /* the next non-empty bucket starts here */
+        { do w->cur++; while (w->count[w->cur] == 0);
+          w->cur_start = w->written;
+          w->cur_left  = w->count[w->cur];
+        }
+      int64_t m = n < w->cur_left ? n : w->cur_left;
+      /* cuts whose ordinal falls in [written, written+m) lie in this bucket: they begin at its start */
+      while (w->part+1 < w->nparts && w->hint > 0 && writer_target(w,w->part+1) < w->written+m)
+        { if (writer_flush(w,rec,from) != HM_OK || writer_cut(w,w->cur_start) != HM_OK)
+            { w->failed = 1; return HM_EIO; }
+          rec += (w->written-from)*w->pbyte;
+          from = w->written;
+        }
+      n -= m; w->written += m; w->cur_left -= m;
+    }
+  if (writer_flush(w,rec,from) != HM_OK)
+    { w->failed = 1; return HM_EIO; }
+  return HM_OK;
+}
+
+int hm_table_write_close(hm_table_writer *w)
+{ int rc = HM_OK;
+  if (w == NULL)
+    return hm_set_error(HM_EINVAL,"hm_table_write_close: no writer");
+  if (w->failed || w->written != w->declared)
+    { rc = w->failed ? hm_set_error(HM_EINVAL,"hm_table_write_close: an earlier call failed")
+                     : hm_set_error(HM_EINVAL,"hm_table_write_close: %lld announced records were not appended",
+                                    (long long) (w->declared-w->written));
+      writer_free(w,1);
+      return rc;
+    }
+  /* cuts not reached (fewer entries than the hint): at the last bucket's start, as write_ktab cuts */
+  while (rc == HM_OK && w->part+1 < w->nparts)
+    rc = writer_cut(w,w->hint > 0 && w->written > 0 ? w->cur_start : w->written);
+  for (int p = 0; p < w->nparts && rc == HM_OK; p++)
+    { int64_t end = p+1 < w->nparts ? w->part_first[p+1] : w->written;
+      int64_t cnt = end-w->part_first[p];
+      if (pwrite_all(w->fd[p],&cnt,8,4) != 0)
+        rc = hm_set_error(HM_EIO,"writing table part %d: %s",p+1,strerror(errno));
+    }
+  char *stub = writer_path(w,0,1);
+  if (rc == HM_OK)
+    { int     f = stub ? open(stub,O_WRONLY|O_CREAT|O_TRUNC,0644) : -1;
+      int32_t hdr[4] = { w->kmer, w->nparts, w->minval, w->ibyte };
+      int64_t acc = 0;
+      for (int64_t b = 0; b < w->ixlen; b++)                /* counts -> bucket END offsets */
+        { acc += w->count[b]; w->count[b] = acc; }
+      if (f < 0 || pwrite_all(f,hdr,sizeof(hdr),0) != 0 ||
+          pwrite_all(f,w->count,sizeof(int64_t)*(size_t) w->ixlen,sizeof(hdr)) != 0)
+        rc = hm_set_error(HM_EIO,"Cannot write %s: %s",stub ? stub : "table stub",strerror(errno));
+      if (f >= 0 && close(f) != 0 && rc == HM_OK)
+        rc = hm_set_error(HM_EIO,"Cannot write %s: %s",stub,strerror(errno));
+    }
+  for (int p = 0; p < w->nparts; p++)
+    { if (w->fd[p] >= 0 && close(w->fd[p]) != 0 && rc == HM_OK)
+        rc = hm_set_error(HM_EIO,"writing table part %d: %s",p+1,strerror(errno));
+      w->fd[p] = -1;
+    }
+  /* into place: the parts, then (last) the stub that names them; parts an older table of this name
+   * had beyond nparts go                                                                           */
+  int old_parts = 0;
+  { char *final = writer_path(w,0,0);
+    int   f = final ? open(final,O_RDONLY) : -1;
+    int32_t hdr[4];
+    if (f >= 0 && read(f,hdr,sizeof(hdr)) == (ssize_t) sizeof(hdr) && hdr[1] > 0)
+      old_parts = hdr[1];
+    if (f >= 0) close(f);
+    free(final);
+  }
+  int renamed = 0;
+  for (int p = 0; p <= w->nparts && rc == HM_OK; p++)
+    { int   part = p < w->nparts ? p+1 : 0;
+      char *a = writer_path(w,part,1), *b = writer_path(w,part,0);
+      if (a == NULL || b == NULL || rename(a,b) != 0)
+        rc = hm_set_error(HM_EIO,"Cannot rename %s into place: %s",a ? a : "table part",strerror(errno));
+      else
+        renamed = p+1;
+      free(a); free(b);
+    }
+  if (rc != HM_OK)                                          /* nothing half-written under the final names */
+    for (int p = 0; p < renamed && p < w->nparts; p++)
+      { char *b = writer_path(w,p+1,0);
+        if (b != NULL) { unlink(b); free(b); }
+      }
+  else
+    for (int p = w->nparts+1; p <= old_parts; p++)
+      { char *b = writer_path(w,p,0);
+        if (b != NULL) { unlink(b); free(b); }
+      }
+  free(stub);
+  writer_free(w,1);
+  return rc;
+}
+
 /* "min \t sum-min \t count" for sum ascending, then min ascending, min < FMAX only
  * (PloidyPlot.c:1612-1615; the i < FMAX bound silently drops bin 500, kept for parity)        */
 int hm_write_smu(const char *path, const int64_t *plot)
