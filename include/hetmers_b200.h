@@ -204,7 +204,8 @@ int  hm_k_symm_resolve(const uint64_t *d_keys, const uint64_t *d_keys_lo, const 
  * (sum, min) has a non-zero label in d_pixmap are appended to d_out as hm_k_pass2_extract lists them -- each
  * candidate once, and its mirror image (rc y, rc x) too unless the pair differs at the middle base of an odd k
  * (DESIGN.md §4a).  At most 2 (c1-c0) records; *d_count (zeroed by the caller) counts all of them, also those
- * beyond `cap`.  The candidate count is in the work-area header (hm_symm_status).                          */
+ * beyond `cap`.  The candidate count is in the work-area header (hm_symm_status); c1 must not exceed it, except
+ * that c0 = 0 with a larger c1 lists every candidate.                                                      */
 int  hm_k_symm_extract(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
                        const void *d_bucket, int bits, int idx64, int kmer,
                        void *d_work, const hm_symm_layout *layout, const hm_symm_shards *shards,

@@ -2222,6 +2222,22 @@ static int extract_direct(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out,
   return HM_OK;
 }
 
+/* appends c device records to the host list *host of *n records (capacity *cap, grown by doubling) */
+static int append_records(hm_pair_rec **host, int64_t *n, int64_t *cap, const hm_pair_rec *d_rec, int64_t c)
+{ if (*n + c > *cap)
+    { int64_t      nh = 2 * *cap > *n + c ? 2 * *cap : *n + c;
+      hm_pair_rec *h2 = (hm_pair_rec *) realloc(*host,sizeof(hm_pair_rec)*(size_t) nh);
+      if (h2 == NULL)
+        return hm_set_error(HM_ENOMEM,"out of host memory for %lld pair records",(long long) nh);
+      *host = h2; *cap = nh;
+    }
+  cudaError_t e;
+  if (c > 0 && (e = cudaMemcpy(*host + *n,d_rec,sizeof(hm_pair_rec)*(size_t) c,cudaMemcpyDeviceToHost)) != cudaSuccess)
+    return hm_cuda_fail(e,"cudaMemcpy(pair records)");
+  *n += c;
+  return HM_OK;
+}
+
 /* the symmetric route: the candidates the last symmetric run left in each GPU's work area, listed by
  * hm_k_symm_extract against that GPU's replica (DESIGN.md §4a).  The record buffer of a GPU is what the device
  * budget leaves beyond the scan's own arrays (at most two records per candidate); the candidates go through it
@@ -2294,17 +2310,8 @@ static int extract_symm(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, i
                                 (long long) (c1[g]-c0[g]));
               break;
             }
-          if (total + (int64_t) c > hcap)
-            { int64_t      nh = 2*hcap > total + (int64_t) c ? 2*hcap : total + (int64_t) c;
-              hm_pair_rec *h2 = (hm_pair_rec *) realloc(host,sizeof(hm_pair_rec)*(size_t) nh);
-              if (h2 == NULL)
-                { rc = hm_set_error(HM_ENOMEM,"out of host memory for %lld pair records",(long long) nh); break; }
-              host = h2; hcap = nh;
-            }
-          if (c > 0 && (e = cudaMemcpy(host+total,d_out[g],sizeof(hm_pair_rec)*(size_t) c,cudaMemcpyDeviceToHost))
-                       != cudaSuccess)
-            { rc = hm_cuda_fail(e,"cudaMemcpy(pair records)"); break; }
-          total += (int64_t) c;
+          if ((rc = append_records(&host,&total,&hcap,d_out[g],(int64_t) c)) != HM_OK)
+            break;
           c0[g] = c1[g];
         }
     }
@@ -2784,7 +2791,7 @@ extern "C" int hm_rank_scan_extract_slices(hm_rank_scan *r, int64_t slice, int64
   return rc;
 }
 
-/* hm_rank_scan_route for the listing: extract_kernel<..., RT = true> over the round's slice, its queries grouped
+/* hm_rank_scan_route for the listing: extract_kernel<..., LK_ROUTED> over the round's slice, its queries grouped
  * by owner */
 extern "C" int hm_rank_scan_extract_route(hm_rank_scan *r, int64_t round, int64_t *counts)
 { if (r == NULL || r->stage != 5 || counts == NULL || round < 0)
@@ -2824,17 +2831,7 @@ extern "C" int hm_rank_scan_extract_settle(hm_rank_scan *r)
   if ((int64_t) c > 2*r->slice)
     return hm_set_error(HM_ECUDA,"the routed listing gave %llu records for a slice of %lld candidates",c,
                         (long long) r->slice);
-  if (r->host_n + (int64_t) c > r->host_cap)
-    { int64_t      nh = 2*r->host_cap > r->host_n + (int64_t) c ? 2*r->host_cap : r->host_n + (int64_t) c;
-      hm_pair_rec *h2 = (hm_pair_rec *) realloc(r->host,sizeof(hm_pair_rec)*(size_t) nh);
-      if (h2 == NULL)
-        return hm_set_error(HM_ENOMEM,"out of host memory for %lld pair records",(long long) nh);
-      r->host = h2; r->host_cap = nh;
-    }
-  if (c > 0)
-    HM_CUDA(cudaMemcpy(r->host+r->host_n,r->rec,sizeof(hm_pair_rec)*(size_t) c,cudaMemcpyDeviceToHost));
-  r->host_n += (int64_t) c;
-  return HM_OK;
+  return append_records(&r->host,&r->host_n,&r->host_cap,r->rec,(int64_t) c);
 }
 
 /* after the last round: this rank's records (*records malloc'ed, the caller frees; sorted as hm_scan_extract sorts)

@@ -71,9 +71,18 @@
 #define SY_STATUS_ASYMMETRIC 1ull              /* a reverse complement was not in the table      */
 #define SY_STATUS_OVERFLOW   2ull              /* candidate list full                             */
 
-/* device view of the work area (hm_symm_layout) */
+/* The work area's header holds only counters, which the kernels advance atomically.  Words 0..2 are read by
+ * hm_symm_status and tools/time_symm.py as well; hm_k_symm_runscan and hm_symm_stream_begin zero the header. */
+#define SY_HDR_CAND   0                        /* candidate records                                */
+#define SY_HDR_STATUS 1                        /* SY_STATUS_* bits                                 */
+#define SY_HDR_RUNS   2                        /* runs listed for runs_kernel                      */
+#define SY_HDR_S      3                        /* streamed scan: S list entries                    */
+#define SY_HDR_PEND   4                        /* routed pass 2: parked candidates, then ...       */
+#define SY_HDR_QUERY  5                        /*   ... their queries (both reset per round)       */
+
+/* device view of the work area (hm_symm_layout) and of the arrays the streamed and routed scans add to it */
 struct SymmView
-  { unsigned long long *cand_n;
+  { unsigned long long *cand_n;                 /* header word SY_HDR_CAND: the header's first word */
     unsigned long long *status;
     uint32_t *bloom;                            /* n_seg segments of seg_words words               */
     uint32_t  seg_words;
@@ -84,6 +93,12 @@ struct SymmView
     unsigned long long *runs_n;                 /* heads of runs of three or more entries (table indices) */
     uint64_t *runs;
     unsigned long long runs_cap;
+    uint64_t *s_key, *s_lo;                     /* streamed pass 1: the S list (count: header word SY_HDR_S) */
+    unsigned long long s_cap;
+    const hm_stream_sview *sviews;              /* streamed pass 2, several shards: every shard's S list */
+    uint64_t *pend, *pend_key, *pend_lo;        /* routed pass 2: parked candidates (meta; key words for listing) */
+    uint64_t *q_key, *q_lo, *q_tag;             /*   and their queries (tag = owner << 32 | pending slot) */
+    unsigned long long pend_cap, q_cap;
   };
 
 /* Bloom slot of key (hi,lo).  The WORD is chosen by the key's last k/2 bases, the two BITS inside it by
@@ -316,8 +331,8 @@ static SymmView make_view(void *d_work, const hm_symm_layout *L, const hm_symm_s
 { SymmView W;
   uint8_t *b = (uint8_t *) d_work;
   memset(&W,0,sizeof(W));
-  W.cand_n    = (unsigned long long *) (b + L->off_header);
-  W.status    = W.cand_n + 1;
+  W.cand_n    = (unsigned long long *) (b + L->off_header) + SY_HDR_CAND;
+  W.status    = W.cand_n + SY_HDR_STATUS;
   W.bloom     = (uint32_t *) (b + L->off_bloom);
   W.seg_words = (uint32_t) L->seg_words;
   W.n_seg     = L->n_seg;
@@ -330,7 +345,7 @@ static SymmView make_view(void *d_work, const hm_symm_layout *L, const hm_symm_s
   W.cand_lo   = (uint64_t *) (b + L->off_cand_lo);
   W.cand_meta = (uint64_t *) (b + L->off_cand_meta);
   W.cand_cap  = (unsigned long long) L->cand_cap;
-  W.runs_n    = W.cand_n + 2;
+  W.runs_n    = W.cand_n + SY_HDR_RUNS;
   W.runs      = (uint64_t *) (b + L->off_runs);
   W.runs_cap  = (unsigned long long) L->runs_cap;
   return W;
@@ -389,23 +404,19 @@ __device__ __forceinline__ void stage_candidates(const RsSmem<KW> &S, unsigned *
     }
 }
 
-/* streamed scan (SL = true): every key that goes into the Bloom filter is also appended to the S list, so that
- * the list is exactly the set the filter over-approximates.  Header words 3..6 of the work area hold the list's
- * count, capacity and arrays (the kernels' parameters stay those of the in-core scan); one atomic per warp.   */
-#define SY_HDR_S 3
-
+/* streamed scan (SL = true): every key that goes into the Bloom filter is also appended to the S list of the
+ * view, so that the list is exactly the set the filter over-approximates; one atomic per warp.              */
 template <int KW>
 __device__ __forceinline__ void s_push(const SymmView &W, uint64_t x, uint64_t xl)
-{ unsigned long long *h = W.cand_n + SY_HDR_S;         /* count, capacity, key array, second-word array */
-  const unsigned m = __activemask();
+{ const unsigned m = __activemask();
   const int      lane = threadIdx.x & 31, lead = __ffs(m)-1;
   unsigned long long at = 0;
   if (lane == lead)
-    at = atomicAdd(h,(unsigned long long) __popc(m));
+    at = atomicAdd(W.cand_n + SY_HDR_S,(unsigned long long) __popc(m));
   at = __shfl_sync(m,at,lead) + (unsigned long long) __popc(m & ((1u << lane)-1));
-  if (at < h[1])
-    { ((uint64_t *) h[2])[at] = x;
-      if (KW == 2) ((uint64_t *) h[3])[at] = xl;
+  if (at < W.s_cap)
+    { W.s_key[at] = x;
+      if (KW == 2) W.s_lo[at] = xl;
     }
   else
     atomicOr(W.status,SY_STATUS_OVERFLOW);
@@ -1068,6 +1079,16 @@ runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
     }
 }
 
+/* f(Inst<IdxT,KW>()) for the instantiation that serves (kmer, idx64): KW key words, IdxT bucket offsets */
+template <typename I, int K> struct Inst { typedef I IdxT; static constexpr int KW = K; };
+
+template <class F>
+static cudaError_t dispatch(int kmer, int idx64, F f)
+{ if (kmer <= 32)
+    return idx64 ? f(Inst<uint64_t,1>()) : f(Inst<uint32_t,1>());
+  return idx64 ? f(Inst<uint64_t,2>()) : f(Inst<uint32_t,2>());
+}
+
 template <typename IdxT, int KW, bool SL = false>
 static cudaError_t launch_runscan(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                   const void *bucket, int bits, int kmer, int64_t lo, int64_t hi,
@@ -1151,13 +1172,9 @@ extern "C" int hm_k_symm_runscan(const uint64_t *d_keys, const uint64_t *d_keys_
     bloom_window(st,W.bloom,sizeof(uint32_t)*(size_t) W.seg_words*(size_t) W.n_seg,1);
   if (hi == lo)
     return HM_OK;
-  cudaError_t e;
-  if (kmer <= 32)
-    e = idx64 ? launch_runscan<uint64_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st)
-              : launch_runscan<uint32_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st);
-  else
-    e = idx64 ? launch_runscan<uint64_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st)
-              : launch_runscan<uint32_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_runscan<typename decltype(I)::IdxT,decltype(I)::KW>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,
+                                                                       lo,hi,W,st); });
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"runscan_kernel");
   return HM_OK;
@@ -1176,13 +1193,9 @@ extern "C" int hm_k_symm_runs(const uint64_t *d_keys, const uint64_t *d_keys_lo,
     return HM_OK;
   cudaStream_t st = (cudaStream_t) stream;
   SymmView W = make_view(d_work,layout,shards);
-  cudaError_t e;
-  if (kmer <= 32)
-    e = idx64 ? launch_runs<uint64_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st)
-              : launch_runs<uint32_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st);
-  else
-    e = idx64 ? launch_runs<uint64_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st)
-              : launch_runs<uint32_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,lo,hi,W,st);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_runs<typename decltype(I)::IdxT,decltype(I)::KW>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,
+                                                                    lo,hi,W,st); });
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"runs_kernel");
   return HM_OK;
@@ -1288,67 +1301,49 @@ __device__ __noinline__ bool has_upper_partner(const uint64_t *__restrict__ keys
   return (U > 0);
 }
 
-/* Routed pass 2 (one rank of a one-process-per-GPU job, DESIGN.md §4c): header words SY_HDR_R.. hold the pending
- * count, the query count, the pending list (one meta per candidate), the query keys, their second words, their
- * tags (owner << 32 | pending slot) and the two capacities.  A candidate with a Bloom hit on a key owned by
- * another rank is parked there; every such key becomes a query to its owner.                                  */
-#define SY_HDR_R 8
+/* where pass 2 checks a Bloom hit exactly (isolated_after_all) */
+enum Lookup
+  { LK_TABLE,        /* in core: is there an upper partner of the key in its run of the table                     */
+    LK_SLIST,        /* streamed: is the key in the sorted S list (several shards: the owner's, through W.sviews) */
+    LK_ROUTED        /* one rank of a one-process-per-GPU job: keys it owns in its own S list; a candidate left
+                      *   with a hit on a key owned elsewhere is parked (route_push) and settled once the owners
+                      *   have answered                                                                         */
+  };
 
-template <int KW>
-__device__ __noinline__ void route_push(const SymmView &W, uint64_t meta, bool fa, int oa, uint64_t rx, uint64_t rxl,
-                                        bool fb, int ob, uint64_t ry, uint64_t ryl)
-{ unsigned long long *h = W.cand_n + SY_HDR_R;
-  const unsigned long long nq = (fa ? 1ull : 0ull) + (fb ? 1ull : 0ull);
-  const unsigned long long slot = atomicAdd(h,1ull), q = atomicAdd(h+1,nq);
-  if (slot >= h[6] || q+nq > h[7])
+/* Routed pass 2 (DESIGN.md §4c, *Ranks*): a parked candidate goes to the view's pending list -- its meta, and its
+ * key words as well when the sink lists pairs (KEY) -- and each of its keys owned by another rank becomes a query
+ * to the owner, tagged owner << 32 | pending slot.  Two atomics per parked candidate: not a hot path.          */
+template <int KW, bool KEY>
+__device__ __forceinline__ void route_push(const SymmView &W, uint64_t x, uint64_t xl, uint64_t meta,
+                                           bool fa, int oa, uint64_t rx, uint64_t rxl,
+                                           bool fb, int ob, uint64_t ry, uint64_t ryl)
+{ const unsigned long long nq = (fa ? 1ull : 0ull) + (fb ? 1ull : 0ull);
+  const unsigned long long slot = atomicAdd(W.cand_n+SY_HDR_PEND,1ull), q = atomicAdd(W.cand_n+SY_HDR_QUERY,nq);
+  if (slot >= W.pend_cap || q+nq > W.q_cap)
     { atomicOr(W.status,SY_STATUS_OVERFLOW); return; }
-  ((uint64_t *) h[2])[slot] = meta & ~(RV_HA | RV_HB);
-  uint64_t *qk = (uint64_t *) h[3], *ql = (uint64_t *) h[4], *qt = (uint64_t *) h[5];
+  W.pend[slot] = meta & ~(RV_HA | RV_HB);
+  if (KEY)
+    { W.pend_key[slot] = x;
+      if (KW == 2) W.pend_lo[slot] = xl;
+    }
   unsigned long long at = q;
   if (fa)
-    { qk[at] = rx; if (KW == 2) ql[at] = rxl;
-      qt[at] = ((uint64_t) oa << 32) | slot; at++;
+    { W.q_key[at] = rx; if (KW == 2) W.q_lo[at] = rxl;
+      W.q_tag[at] = ((uint64_t) oa << 32) | slot; at++;
     }
   if (fb)
-    { qk[at] = ry; if (KW == 2) ql[at] = ryl;
-      qt[at] = ((uint64_t) ob << 32) | slot;
-    }
-}
-
-/* route_push of the routed listing (extract_kernel<..., RT = true>): listing a parked candidate needs its key, so
- * its key words go to header words SY_HDR_R+8 / +9 (the parked keys and their second words) as well        */
-template <int KW>
-__device__ __noinline__ void route_push_key(const SymmView &W, uint64_t x, uint64_t xl, uint64_t meta, bool fa, int oa,
-                                            uint64_t rx, uint64_t rxl, bool fb, int ob, uint64_t ry, uint64_t ryl)
-{ unsigned long long *h = W.cand_n + SY_HDR_R;
-  const unsigned long long nq = (fa ? 1ull : 0ull) + (fb ? 1ull : 0ull);
-  const unsigned long long slot = atomicAdd(h,1ull), q = atomicAdd(h+1,nq);
-  if (slot >= h[6] || q+nq > h[7])
-    { atomicOr(W.status,SY_STATUS_OVERFLOW); return; }
-  ((uint64_t *) h[2])[slot] = meta & ~(RV_HA | RV_HB);
-  ((uint64_t *) h[8])[slot] = x;
-  if (KW == 2) ((uint64_t *) h[9])[slot] = xl;
-  uint64_t *qk = (uint64_t *) h[3], *ql = (uint64_t *) h[4], *qt = (uint64_t *) h[5];
-  unsigned long long at = q;
-  if (fa)
-    { qk[at] = rx; if (KW == 2) ql[at] = rxl;
-      qt[at] = ((uint64_t) oa << 32) | slot; at++;
-    }
-  if (fb)
-    { qk[at] = ry; if (KW == 2) ql[at] = ryl;
-      qt[at] = ((uint64_t) ob << 32) | slot;
+    { W.q_key[at] = ry; if (KW == 2) W.q_lo[at] = ryl;
+      W.q_tag[at] = ((uint64_t) ob << 32) | slot;
     }
 }
 
 /* one candidate whose Bloom bits were set for rc x (RV_HA in its meta) and/or rc y (RV_HB): is it isolated
- * after all?  SL = false looks for an upper partner in the table, SL = true (streamed scan: keys / bucket are
- * the sorted S list and its index) looks the key up in S.  Exact.  When the bucket prefix is no longer than
+ * after all?  Exact.  LK_TABLE looks for an upper partner in the table: when the bucket prefix is no longer than
  * the run prefix (every table of more than a few entries) both buckets' offsets are loaded at once and then
- * RV_PROBE keys and counts of a bucket at once: two dependent accesses instead of one per key.
- * RT = true (with SL): keys this rank owns are looked up in its S list; a candidate that is not settled by them
- * and has a hit on a key owned elsewhere is parked (route_push) and counted later, so it is not isolated here.
- * KEY = true (with RT): it is parked with its key words (route_push_key), to be listed later.                   */
-template <typename IdxT, int KW, bool SL, bool RT = false, bool KEY = false>
+ * RV_PROBE keys and counts of a bucket at once, two dependent accesses instead of one per key.  LK_SLIST and
+ * LK_ROUTED look the key up in an S list (keys / bucket: the sorted list and its index); a candidate LK_ROUTED
+ * parks is not isolated here, and it is parked with its key words when the sink lists pairs.                 */
+template <typename IdxT, int KW, Lookup LK, class Sink>
 __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                                                    const uint16_t *__restrict__ cnt, int64_t n,
                                                    const IdxT *__restrict__ bucket, int bshift, int kmer,
@@ -1360,7 +1355,7 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
   revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
   ry = rx; ryl = rxl;
   set_base<KW>(ry,ryl,kmer-1-p,3-yb);                      /* rc y = rc x with the mirrored base swapped */
-  if (SL && RT)
+  if (LK == LK_ROUTED)
     { const int  oa = (ha && W.n_seg > 1) ? owner_of(W,rx) : W.self, ob = (hb && W.n_seg > 1) ? owner_of(W,ry) : W.self;
       if ((ha && oa == W.self && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
           (hb && ob == W.self && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0))
@@ -1368,25 +1363,23 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
       const bool fa = ha && oa != W.self, fb = hb && ob != W.self;
       if (!fa && !fb)
         return true;
-      if (KEY) route_push_key<KW>(W,x,xl,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
-      else     route_push<KW>(W,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
+      route_push<KW,Sink::NEEDS_KEY>(W,x,xl,meta,fa,oa,rx,rxl,fb,ob,ry,ryl);
       return false;
     }
-  if (SL && W.n_seg > 1)                                   /* several shards: the S list of the key's owner */
-    { const hm_stream_sview *V = (const hm_stream_sview *) W.cand_n[SY_HDR_S+4];
-      if (ha)
-        { const hm_stream_sview &a = V[owner_of(W,rx)];
+  if (LK == LK_SLIST && W.n_seg > 1)                       /* several shards: the S list of the key's owner */
+    { if (ha)
+        { const hm_stream_sview &a = W.sviews[owner_of(W,rx)];
           if (bucket_find<IdxT,KW>(a.s_key,a.s_lo,(const IdxT *) a.s_bucket,64-a.bits,rx,rxl) >= 0)
             return false;
         }
       if (hb)
-        { const hm_stream_sview &b = V[owner_of(W,ry)];
+        { const hm_stream_sview &b = W.sviews[owner_of(W,ry)];
           if (bucket_find<IdxT,KW>(b.s_key,b.s_lo,(const IdxT *) b.s_bucket,64-b.bits,ry,ryl) >= 0)
             return false;
         }
       return true;
     }
-  if (SL)
+  if (LK == LK_SLIST)
     return !((ha && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
              (hb && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,ry,ryl) >= 0));
   const int Pr = kmer >> 1, pup = kmer-Pr, psh = 64-2*Pr;
@@ -1432,154 +1425,6 @@ __device__ __forceinline__ void count_pair(uint32_t *tile, unsigned long long *_
   else
     atomicAdd(plot + s*HM_PLOT_W + m, (unsigned long long) wgt);
 }
-
-/* Candidates whose Bloom look-up misses (~95 %) are counted at once.  The others need the exact answer
- * and a warp in which one lane does that stalls all 32: they are parked in a per-warp queue in shared
- * memory -- the whole record, with the two Bloom answers in its meta -- and settled 32 at a time, every
- * lane busy, without reading the record or the filter again.  RV_ILP candidates per thread and trip keep
- * that many record / Bloom loads in flight (the kernel is bound by latency: record -> Bloom word, and
- * for the hits bucket offsets -> keys, not by bytes or instructions).  One CTA of 1024 threads per SM:
- * one plot tile per SM, the rest of shared memory holds the queues.
- * RT = true: routed pass 2 of one rank (isolated_after_all); the rest of the kernel is the same.      */
-template <typename IdxT, int KW, bool SL, bool RT = false>
-__global__ void __launch_bounds__(RV_THREADS,1)
-resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
-               const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
-               int kmer, const SymmView W, unsigned long long *__restrict__ plot)
-{ extern __shared__ __align__(16) uint64_t rv_smem[];
-  uint32_t *tile = (uint32_t *) rv_smem;                  /* RV_TS x RV_TROW counters */
-  const unsigned FULL = 0xffffffffu;
-  const int      lane = threadIdx.x & 31;
-  const unsigned lt   = (1u << lane) - 1;
-  uint64_t *qk = rv_smem + RV_TS*RV_TROW/2 + (threadIdx.x >> 5)*RV_QCAP*(KW+1);   /* this warp's queue */
-  uint64_t *ql = qk + (KW == 2 ? RV_QCAP : 0);
-  uint64_t *qm = qk + KW*RV_QCAP;
-  int       qn = 0;
-  for (int t = threadIdx.x; t < RV_TS*RV_TROW; t += blockDim.x)
-    tile[t] = 0;
-  __syncthreads();
-  unsigned long long ncl = *W.cand_n;
-  if (ncl > W.cand_cap) ncl = W.cand_cap;
-  const int64_t nc     = (int64_t) ncl;
-  const int64_t stride = (int64_t) gridDim.x * blockDim.x;
-  const int64_t first  = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-  for (uint32_t it = 0; first-lane + (int64_t) it*RV_ILP*stride < nc; it++)
-    { uint64_t x[RV_ILP], xl[RV_ILP], meta[RV_ILP];
-      uint32_t *wa[RV_ILP], *wb[RV_ILP], ba[RV_ILP], bb[RV_ILP], va[RV_ILP], vb[RV_ILP];
-      bool     ok[RV_ILP];
-#pragma unroll
-      for (int u = 0; u < RV_ILP; u++)
-        { const int64_t i = first + ((int64_t) it*RV_ILP+u)*stride;
-          ok[u] = (i < nc);
-          x[u] = 0; xl[u] = 0; meta[u] = 0;
-          if (ok[u])
-            { x[u] = ld_stream(W.cand_key+i);
-              if (KW == 2) xl[u] = ld_stream(W.cand_lo+i);
-              meta[u] = ld_stream(W.cand_meta+i);
-            }
-        }
-#pragma unroll
-      for (int u = 0; u < RV_ILP; u++)
-        { const int p  = (int) ((meta[u] >> 32) & 0xff), yb = (int) ((meta[u] >> 40) & 3);
-          uint64_t rx, rxl, ry, ryl;
-          revcomp_kmer<KW>(x[u],xl[u],kmer,rx,rxl);
-          ry = rx; ryl = rxl;
-          set_base<KW>(ry,ryl,kmer-1-p,3-yb);
-          bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,rx) : 0,kmer,rx,rxl,wa[u],ba[u]);
-          bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,ry) : 0,kmer,ry,ryl,wb[u],bb[u]);
-        }
-#pragma unroll
-      for (int u = 0; u < RV_ILP; u++)
-        { va[u] = 0; vb[u] = 0;
-          if (ok[u])
-            { va[u] = ld_keep(wa[u]);
-              vb[u] = (wb[u] == wa[u]) ? va[u] : ld_keep(wb[u]);   /* one shard owns both: the same word */
-            }
-        }
-#pragma unroll
-      for (int u = 0; u < RV_ILP; u++)
-        { const bool ha = (va[u] & ba[u]) == ba[u], hb = (vb[u] & bb[u]) == bb[u];
-          const bool hit = ok[u] && (ha || hb);
-          if (ok[u] && !hit)
-            count_pair(tile,plot,meta[u],kmer);
-          const unsigned bal = __ballot_sync(FULL,hit);
-          if (hit)
-            { const int at = qn + __popc(bal & lt);
-              qk[at] = x[u];
-              if (KW == 2) ql[at] = xl[u];
-              qm[at] = meta[u] | (ha ? RV_HA : 0) | (hb ? RV_HB : 0);
-            }
-          qn += __popc(bal);
-        }
-      __syncwarp();
-      while (qn >= 32)
-        { qn -= 32;
-          const uint64_t xx = qk[qn+lane], xxl = KW == 2 ? ql[qn+lane] : 0, mm = qm[qn+lane];
-          __syncwarp();
-          if (isolated_after_all<IdxT,KW,SL,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
-            count_pair(tile,plot,mm,kmer);
-        }
-    }
-  if (lane < qn)
-    { const uint64_t xx = qk[lane], xxl = KW == 2 ? ql[lane] : 0, mm = qm[lane];
-      if (isolated_after_all<IdxT,KW,SL,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
-        count_pair(tile,plot,mm,kmer);
-    }
-  __syncthreads();
-  for (int t = threadIdx.x; t < RV_TS*RV_TROW; t += blockDim.x)
-    { uint32_t v = tile[t];
-      if (v != 0)                                          /* (column RV_TM is padding: always 0) */
-        atomicAdd(plot + (t/RV_TROW)*HM_PLOT_W + (t%RV_TROW), (unsigned long long) v);
-    }
-}
-
-template <typename IdxT, int KW, bool SL = false, bool RT = false>
-static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
-                                  const void *bucket, int bits, int kmer, const SymmView &W,
-                                  unsigned long long *plot, int64_t range, cudaStream_t st)
-{ static int configured[64] = {0};                            /* per instantiation */
-  size_t smem = (size_t) RV_TS*RV_TROW*sizeof(uint32_t) + (size_t) (RV_THREADS/32)*RV_QCAP*8*(KW+1);   /* 121 KB / 145 KB */
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  if (dev >= 64 || !configured[dev])
-    { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW,SL,RT>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
-      if (e != cudaSuccess) return e;
-      if (dev < 64) configured[dev] = 1;
-    }
-  cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
-  int64_t want = (range/8+RV_THREADS-1)/RV_THREADS;            /* ~1 candidate per 10 entries */
-  int     grid = (int) (want < sms ? (want > 0 ? want : 1) : sms);
-  resolve_kernel<IdxT,KW,SL,RT><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
-  return cudaGetLastError();
-}
-
-extern "C" int hm_k_symm_resolve(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
-                                 const void *d_bucket, int bits, int idx64, int kmer,
-                                 void *d_work, const hm_symm_layout *layout, const hm_symm_shards *shards,
-                                 unsigned long long *d_plot, void *stream)
-{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || d_work == NULL || layout == NULL || d_plot == NULL)
-    return hm_set_error(HM_EINVAL,"symm_resolve: bad arguments");
-  if ((kmer > 32) != (d_keys_lo != NULL))
-    return hm_set_error(HM_EINVAL,"symm_resolve: second key word array %s for k=%d",
-                        d_keys_lo ? "given" : "missing",kmer);
-  cudaStream_t st = (cudaStream_t) stream;
-  SymmView W = make_view(d_work,layout,shards);
-  int64_t range = layout->range;
-  cudaError_t e;
-  if (kmer <= 32)
-    e = idx64 ? launch_resolve<uint64_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,W,d_plot,range,st)
-              : launch_resolve<uint32_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,W,d_plot,range,st);
-  else
-    e = idx64 ? launch_resolve<uint64_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,d_plot,range,st)
-              : launch_resolve<uint32_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,d_plot,range,st);
-  if (l2_persist())
-    bloom_window(st,NULL,0,0);
-  if (e != cudaSuccess)
-    return hm_cuda_fail(e,"resolve_kernel");
-  return HM_OK;
-}
-
-/* ------------------------------------------------------------------ pair listing -------- */
 
 /* extract_kmer_pairs' records of isolated candidates (warp-wide call; lab = the candidate's pixel label, 0 for
  * lanes that list nothing).  A candidate (x < y, differing at p, bases bx < by, counts cx, cy) stands for the
@@ -1632,45 +1477,89 @@ __device__ __forceinline__ void list_pairs(uint64_t x, uint64_t xl, uint64_t met
     }
 }
 
-#define EX_THREADS 512              /* k <= 32: 2 CTAs per SM (64 registers); k > 32 spilled at 64 registers: 1 CTA,
-                                     * and so did the routed listing (RT) at k <= 32: 1 CTA                        */
-#define EX_ILP     RV_ILP
-#define EX_QCAP    (32*(EX_ILP+1))
+extern __shared__ __align__(16) uint64_t rv_smem[];     /* pass 2's dynamic shared memory (resolve / extract_kernel) */
 
-/* extract_kmer_pairs on the symmetric scan's work area: resolve_kernel (SL = false) over the candidates
- * [c0, c1) of the last run, with the same Bloom-first structure and per-warp queue of hits settled by
- * isolated_after_all, but an isolated candidate whose pixel carries a label is listed (list_pairs) instead
- * of counted.  No plot tile: shared memory holds only the queues.
- * RT = true: the routed listing of one rank (DESIGN.md §4c, *Ranks*) over a slice [c0, c1) of its candidates;
- * keys / bucket are its sorted S list and S index.  A hit on a key the rank owns is settled in that list; a
- * candidate left with a hit on a key owned elsewhere is parked with its key words (route_push_key) and listed
- * by route_list_kernel once the owners have answered.                                                    */
-template <typename IdxT, int KW, bool RT = false>
-__global__ void __launch_bounds__(EX_THREADS,KW == 1 && !RT ? 2 : 1)
-extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
-               const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
-               int kmer, const SymmView W, const uint16_t *__restrict__ pixmap, int64_t c0, int64_t c1,
-               hm_pair_rec *__restrict__ out, unsigned long long cap, unsigned long long *__restrict__ count)
-{ extern __shared__ __align__(16) uint64_t rv_smem[];
-  const unsigned FULL = 0xffffffffu;
+/* What pass 2 does with a candidate once it is known whether it is isolated.  take() is called by every lane of
+ * a warp at once, with iso = false where a lane has nothing to give; begin() and end() by every thread of the
+ * CTA before and after its sweep.  NEEDS_KEY: take() uses the candidate's key words, so the routed pass parks
+ * them with the candidate.  QUEUES: where the warps' queues start in rv_smem.                                */
+struct CountSink                                 /* the plot: resolve_kernel */
+  { uint32_t *tile;                              /* the CTA's shared-memory plot tile: RV_TS x RV_TROW counters */
+    unsigned long long *plot;
+    int kmer;
+    static constexpr bool NEEDS_KEY = false;
+    static constexpr int  QUEUES = RV_TS*RV_TROW/2;     /* after the tile */
+    __device__ __forceinline__ void begin() const
+    { for (int t = threadIdx.x; t < RV_TS*RV_TROW; t += blockDim.x)
+        tile[t] = 0;
+      __syncthreads();
+    }
+    __device__ __forceinline__ void take(bool iso, uint64_t, uint64_t, uint64_t meta) const
+    { if (iso)
+        count_pair(tile,plot,meta,kmer);
+    }
+    __device__ __forceinline__ void end() const
+    { __syncthreads();
+      for (int t = threadIdx.x; t < RV_TS*RV_TROW; t += blockDim.x)
+        { uint32_t v = tile[t];
+          if (v != 0)                                    /* (column RV_TM is padding: always 0) */
+            atomicAdd(plot + (t/RV_TROW)*HM_PLOT_W + (t%RV_TROW), (unsigned long long) v);
+        }
+    }
+  };
+
+template <int KW>
+struct ListSink                                  /* extract_kmer_pairs' records: extract_kernel */
+  { const uint16_t *pixmap;
+    hm_pair_rec *out;
+    unsigned long long cap, *count;
+    int kmer;
+    static constexpr bool NEEDS_KEY = true;
+    static constexpr int  QUEUES = 0;
+    __device__ __forceinline__ void begin() const {}
+    __device__ __forceinline__ void end() const {}
+    __device__ __forceinline__ void take(bool iso, uint64_t x, uint64_t xl, uint64_t meta) const
+    { const int lane = threadIdx.x & 31;
+      unsigned  lab = 0;
+      if (iso)
+        { const int cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
+          lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
+        }
+      list_pairs<KW>(x,xl,meta,lab,kmer,out,cap,count,lane,(1u << lane) - 1);
+    }
+  };
+
+/* Pass 2 over the view's candidates.  Candidates whose Bloom look-up misses (~95 %) go to the sink at once.
+ * The others need the exact answer, and a warp in which one lane does that stalls all 32: they are parked in
+ * the warp's queue in shared memory (RV_QCAP records of KW+1 words) -- the whole record, with the two Bloom
+ * answers in its meta -- and settled 32 at a time, every lane busy, without reading the record or the filter
+ * again.  RV_ILP candidates per thread and trip keep that many record / Bloom loads in flight (the sweep is
+ * bound by latency: record -> Bloom word, and for the hits bucket offsets -> keys, not by bytes or
+ * instructions).                                                                                            */
+template <typename IdxT, int KW, Lookup LK, class Sink>
+__device__ __forceinline__ void sweep(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+                                      const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket,
+                                      int bshift, int kmer, const SymmView &W, const Sink &sink)
+{ const unsigned FULL = 0xffffffffu;
   const int      lane = threadIdx.x & 31;
   const unsigned lt   = (1u << lane) - 1;
-  uint64_t *qk = rv_smem + (threadIdx.x >> 5)*EX_QCAP*(KW+1);      /* this warp's queue */
-  uint64_t *ql = qk + (KW == 2 ? EX_QCAP : 0);
-  uint64_t *qm = qk + KW*EX_QCAP;
+  uint64_t *qk = rv_smem + Sink::QUEUES + (threadIdx.x >> 5)*RV_QCAP*(KW+1);   /* this warp's queue */
+  uint64_t *ql = qk + (KW == 2 ? RV_QCAP : 0);
+  uint64_t *qm = qk + KW*RV_QCAP;
   int       qn = 0;
+  sink.begin();
   unsigned long long ncl = *W.cand_n;
   if (ncl > W.cand_cap) ncl = W.cand_cap;
-  const int64_t nc     = (int64_t) ncl < c1 ? (int64_t) ncl : c1;
+  const int64_t nc     = (int64_t) ncl;
   const int64_t stride = (int64_t) gridDim.x * blockDim.x;
-  const int64_t first  = c0 + (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-  for (uint32_t it = 0; first-lane + (int64_t) it*EX_ILP*stride < nc; it++)
-    { uint64_t x[EX_ILP], xl[EX_ILP], meta[EX_ILP];
-      uint32_t *wa[EX_ILP], *wb[EX_ILP], ba[EX_ILP], bb[EX_ILP], va[EX_ILP], vb[EX_ILP];
-      bool     ok[EX_ILP];
+  const int64_t first  = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t it = 0; first-lane + (int64_t) it*RV_ILP*stride < nc; it++)
+    { uint64_t x[RV_ILP], xl[RV_ILP], meta[RV_ILP];
+      uint32_t *wa[RV_ILP], *wb[RV_ILP], ba[RV_ILP], bb[RV_ILP], va[RV_ILP], vb[RV_ILP];
+      bool     ok[RV_ILP];
 #pragma unroll
-      for (int u = 0; u < EX_ILP; u++)
-        { const int64_t i = first + ((int64_t) it*EX_ILP+u)*stride;
+      for (int u = 0; u < RV_ILP; u++)
+        { const int64_t i = first + ((int64_t) it*RV_ILP+u)*stride;
           ok[u] = (i < nc);
           x[u] = 0; xl[u] = 0; meta[u] = 0;
           if (ok[u])
@@ -1680,7 +1569,7 @@ extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
             }
         }
 #pragma unroll
-      for (int u = 0; u < EX_ILP; u++)
+      for (int u = 0; u < RV_ILP; u++)
         { const int p  = (int) ((meta[u] >> 32) & 0xff), yb = (int) ((meta[u] >> 40) & 3);
           uint64_t rx, rxl, ry, ryl;
           revcomp_kmer<KW>(x[u],xl[u],kmer,rx,rxl);
@@ -1690,23 +1579,18 @@ extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
           bloom_slot<KW>(W,W.n_seg > 1 ? owner_of(W,ry) : 0,kmer,ry,ryl,wb[u],bb[u]);
         }
 #pragma unroll
-      for (int u = 0; u < EX_ILP; u++)
+      for (int u = 0; u < RV_ILP; u++)
         { va[u] = 0; vb[u] = 0;
           if (ok[u])
             { va[u] = ld_keep(wa[u]);
-              vb[u] = (wb[u] == wa[u]) ? va[u] : ld_keep(wb[u]);
+              vb[u] = (wb[u] == wa[u]) ? va[u] : ld_keep(wb[u]);   /* one shard owns both: the same word */
             }
         }
 #pragma unroll
-      for (int u = 0; u < EX_ILP; u++)
+      for (int u = 0; u < RV_ILP; u++)
         { const bool ha = (va[u] & ba[u]) == ba[u], hb = (vb[u] & bb[u]) == bb[u];
           const bool hit = ok[u] && (ha || hb);
-          unsigned   lab = 0;
-          if (ok[u] && !hit)
-            { const int cx = (int) (meta[u] & 0xffff), cy = (int) ((meta[u] >> 16) & 0xffff);
-              lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
-            }
-          list_pairs<KW>(x[u],xl[u],meta[u],lab,kmer,out,cap,count,lane,lt);
+          sink.take(ok[u] && !hit,x[u],xl[u],meta[u]);
           const unsigned bal = __ballot_sync(FULL,hit);
           if (hit)
             { const int at = qn + __popc(bal & lt);
@@ -1717,42 +1601,113 @@ extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
           qn += __popc(bal);
         }
       __syncwarp();
-      while (qn >= 32)                 /* (the key is read from the queue again to list it: fewer live registers) */
+      while (qn >= 32)
         { qn -= 32;
+          uint64_t       xx = qk[qn+lane], xxl = KW == 2 ? ql[qn+lane] : 0;
           const uint64_t mm = qm[qn+lane];
-          unsigned lab = 0;
-          if (isolated_after_all<IdxT,KW,RT,RT,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,qk[qn+lane],
-                                                   KW == 2 ? ql[qn+lane] : 0,mm))
-            { const int cx = (int) (mm & 0xffff), cy = (int) ((mm >> 16) & 0xffff);
-              lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
-            }
-          list_pairs<KW>(qk[qn+lane],KW == 2 ? ql[qn+lane] : 0,mm,lab,kmer,out,cap,count,lane,lt);
-          __syncwarp();
+          if (!Sink::NEEDS_KEY)                    /* the next trip refills the slots once every lane has read them */
+            __syncwarp();
+          const bool iso = isolated_after_all<IdxT,KW,LK,Sink>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm);
+          if (Sink::NEEDS_KEY)                     /* the key words again: not live across the exact check */
+            { xx = qk[qn+lane]; xxl = KW == 2 ? ql[qn+lane] : 0; }
+          sink.take(iso,xx,xxl,mm);
+          if (Sink::NEEDS_KEY)
+            __syncwarp();
         }
     }
   uint64_t xx = 0, xxl = 0, mm = 0;
-  unsigned lab = 0;
+  bool     iso = false;
   if (lane < qn)
     { xx = qk[lane]; xxl = KW == 2 ? ql[lane] : 0; mm = qm[lane];
-      if (isolated_after_all<IdxT,KW,RT,RT,RT>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm))
-        { const int cx = (int) (mm & 0xffff), cy = (int) ((mm >> 16) & 0xffff);
-          lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
-        }
+      iso = isolated_after_all<IdxT,KW,LK,Sink>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,xx,xxl,mm);
     }
-  list_pairs<KW>(xx,xxl,mm,lab,kmer,out,cap,count,lane,lt);
+  sink.take(iso,xx,xxl,mm);
+  sink.end();
 }
 
-template <typename IdxT, int KW, bool RT = false>
+/* Pass 2 of the plot: sweep with the count sink.  One CTA of 1024 threads per SM: one plot tile per SM, the rest of
+ * shared memory holds the queues.                                                                             */
+template <typename IdxT, int KW, Lookup LK>
+__global__ void __launch_bounds__(RV_THREADS,1)
+resolve_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+               const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
+               int kmer, const SymmView W, unsigned long long *__restrict__ plot)
+{ const CountSink sink = { (uint32_t *) rv_smem, plot, kmer };
+  sweep<IdxT,KW,LK>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,sink);
+}
+
+template <typename IdxT, int KW, Lookup LK = LK_TABLE>
+static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
+                                  const void *bucket, int bits, int kmer, const SymmView &W,
+                                  unsigned long long *plot, int64_t range, cudaStream_t st)
+{ static int configured[64] = {0};                            /* per instantiation */
+  size_t smem = (size_t) RV_TS*RV_TROW*sizeof(uint32_t) + (size_t) (RV_THREADS/32)*RV_QCAP*8*(KW+1);   /* 121 KB / 145 KB */
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  if (dev >= 64 || !configured[dev])
+    { cudaError_t e = cudaFuncSetAttribute(resolve_kernel<IdxT,KW,LK>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem);
+      if (e != cudaSuccess) return e;
+      if (dev < 64) configured[dev] = 1;
+    }
+  cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
+  int64_t want = (range/8+RV_THREADS-1)/RV_THREADS;            /* ~1 candidate per 10 entries */
+  int     grid = (int) (want < sms ? (want > 0 ? want : 1) : sms);
+  resolve_kernel<IdxT,KW,LK><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
+  return cudaGetLastError();
+}
+
+extern "C" int hm_k_symm_resolve(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
+                                 const void *d_bucket, int bits, int idx64, int kmer,
+                                 void *d_work, const hm_symm_layout *layout, const hm_symm_shards *shards,
+                                 unsigned long long *d_plot, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || d_work == NULL || layout == NULL || d_plot == NULL)
+    return hm_set_error(HM_EINVAL,"symm_resolve: bad arguments");
+  if ((kmer > 32) != (d_keys_lo != NULL))
+    return hm_set_error(HM_EINVAL,"symm_resolve: second key word array %s for k=%d",
+                        d_keys_lo ? "given" : "missing",kmer);
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = make_view(d_work,layout,shards);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_resolve<typename decltype(I)::IdxT,decltype(I)::KW>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,
+                                                                       d_plot,layout->range,st); });
+  if (l2_persist())
+    bloom_window(st,NULL,0,0);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"resolve_kernel");
+  return HM_OK;
+}
+
+/* ------------------------------------------------------------------ pair listing -------- */
+
+#define EX_THREADS 512              /* k <= 32: 2 CTAs per SM (64 registers); k > 32 spilled at 64 registers: 1 CTA,
+                                     * and so did the routed listing at k <= 32: 1 CTA                              */
+
+/* extract_kmer_pairs on the symmetric scan's work area: sweep with the list sink over the view's candidates (a
+ * slice of them: slice_view), so an isolated candidate whose pixel carries a label is listed instead of counted.
+ * No plot tile: shared memory holds only the queues.
+ * LK_ROUTED: the routed listing of one rank (DESIGN.md §4c, *Ranks*), with its sorted S list and S index as keys /
+ * bucket; route_list_kernel lists the candidates it parks once the owners have answered.                     */
+template <typename IdxT, int KW, Lookup LK>
+__global__ void __launch_bounds__(EX_THREADS,KW == 1 && LK == LK_TABLE ? 2 : 1)
+extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+               const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
+               int kmer, const SymmView W, const uint16_t *__restrict__ pixmap,
+               hm_pair_rec *__restrict__ out, unsigned long long cap, unsigned long long *__restrict__ count)
+{ const ListSink<KW> sink = { pixmap, out, cap, count, kmer };
+  sweep<IdxT,KW,LK>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,sink);
+}
+
+template <typename IdxT, int KW, Lookup LK = LK_TABLE>
 static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
                                   const void *bucket, int bits, int kmer, const SymmView &W,
-                                  const uint16_t *pixmap, int64_t c0, int64_t c1, hm_pair_rec *out,
-                                  int64_t cap, unsigned long long *count, cudaStream_t st)
+                                  const uint16_t *pixmap, hm_pair_rec *out, int64_t cap, unsigned long long *count,
+                                  cudaStream_t st)
 { static int per_sm[64] = {0};                                /* per instantiation */
-  size_t smem = (size_t) (EX_THREADS/32)*EX_QCAP*8*(KW+1);       /* 24 KB / 36 KB */
+  size_t smem = (size_t) (EX_THREADS/32)*RV_QCAP*8*(KW+1);       /* 24 KB / 36 KB */
   int dev = 0, sms = 132, occ = 1;
   cudaGetDevice(&dev);
   if (dev >= 64 || per_sm[dev] == 0)                           /* one wave of resident CTAs */
-    { cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ,extract_kernel<IdxT,KW,RT>,EX_THREADS,smem);
+    { cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ,extract_kernel<IdxT,KW,LK>,EX_THREADS,smem);
       if (e != cudaSuccess) return e;
       if (occ < 1) occ = 1;
       if (dev < 64) per_sm[dev] = occ;
@@ -1760,11 +1715,20 @@ static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo,
   else
     occ = per_sm[dev];
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
-  int64_t want = (c1-c0+EX_THREADS*EX_ILP-1)/(EX_THREADS*EX_ILP);
+  int64_t want = ((int64_t) W.cand_cap+EX_THREADS*RV_ILP-1)/(EX_THREADS*RV_ILP);
   int     grid = (int) (want < sms*occ ? (want > 0 ? want : 1) : sms*occ);
-  extract_kernel<IdxT,KW,RT><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,
-                                                          pixmap,c0,c1,out,(unsigned long long) cap,count);
+  extract_kernel<IdxT,KW,LK><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,
+                                                          pixmap,out,(unsigned long long) cap,count);
   return cudaGetLastError();
+}
+
+/* the candidates [c0, c1) of a view as its whole list: pass 2 reads min(header count, cand_cap) records from
+ * cand_key, so the header's count (of all candidates) must reach c1 unless c0 = 0                          */
+static SymmView slice_view(SymmView W, int64_t c0, int64_t c1)
+{ W.cand_key += c0; W.cand_meta += c0;
+  if (W.cand_lo != NULL) W.cand_lo += c0;
+  W.cand_cap = (unsigned long long) (c1-c0);
+  return W;
 }
 
 extern "C" int hm_k_symm_extract(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
@@ -1778,17 +1742,15 @@ extern "C" int hm_k_symm_extract(const uint64_t *d_keys, const uint64_t *d_keys_
   if ((kmer > 32) != (d_keys_lo != NULL))
     return hm_set_error(HM_EINVAL,"symm_extract: second key word array %s for k=%d",
                         d_keys_lo ? "given" : "missing",kmer);
-  if (c1 == c0)
+  if (c1 > layout->cand_cap)
+    c1 = layout->cand_cap;
+  if (c1 <= c0)
     return HM_OK;
   cudaStream_t st = (cudaStream_t) stream;
-  SymmView W = make_view(d_work,layout,shards);
-  cudaError_t e;
-  if (kmer <= 32)
-    e = idx64 ? launch_extract<uint64_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
-              : launch_extract<uint32_t,1>(d_keys,NULL,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
-  else
-    e = idx64 ? launch_extract<uint64_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
-              : launch_extract<uint32_t,2>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
+  SymmView W = slice_view(make_view(d_work,layout,shards),c0,c1);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_extract<typename decltype(I)::IdxT,decltype(I)::KW>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,
+                                                                       d_pixmap,d_out,cap,d_count,st); });
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"extract_kernel");
   return HM_OK;
@@ -1801,8 +1763,8 @@ extern "C" int hm_symm_status(const void *d_work, const hm_symm_layout *layout, 
   HM_CUDA(cudaMemcpyAsync(h,(const uint8_t *) d_work + layout->off_header,sizeof(h),cudaMemcpyDeviceToHost,
                           (cudaStream_t) stream));
   HM_CUDA(cudaStreamSynchronize((cudaStream_t) stream));
-  if (n_cand != NULL) *n_cand = h[0];
-  if (status != NULL) *status = h[1];
+  if (n_cand != NULL) *n_cand = h[SY_HDR_CAND];
+  if (status != NULL) *status = h[SY_HDR_STATUS];
   return HM_OK;
 }
 
@@ -1847,6 +1809,7 @@ static SymmView stream_view(void *d_work, const hm_symm_layout *L, const hm_stre
   W.cand_key = R->cand_key; W.cand_lo = R->cand_lo; W.cand_meta = R->cand_meta;
   W.cand_cap = (unsigned long long) R->cand_cap;
   W.runs = R->runs; W.runs_cap = (unsigned long long) R->runs_cap;
+  W.s_key = R->s_key; W.s_lo = R->s_lo; W.s_cap = (unsigned long long) R->s_cap;
   return W;
 }
 
@@ -1872,9 +1835,7 @@ int hm_symm_stream_chunk(const uint64_t *d_keys, const uint64_t *d_keys_lo, cons
                         kmer,(long long) hi,(long long) n);
   cudaStream_t st = (cudaStream_t) stream;
   SymmView W = stream_view(d_work,L,R,shards);
-  uint64_t h[4] = { (uint64_t) R->s_cap, (uint64_t) (uintptr_t) R->s_key, (uint64_t) (uintptr_t) R->s_lo, 0 };
   HM_CUDA(cudaMemsetAsync(W.runs_n,0,sizeof(uint64_t),st));                 /* the run list is per chunk */
-  HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_S+1,h,3*sizeof(uint64_t),cudaMemcpyHostToDevice,st));
   if (hi == 0)
     return HM_OK;
   cudaError_t e;
@@ -1898,12 +1859,12 @@ int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t 
   HM_CUDA(cudaMemcpyAsync(h,(const uint8_t *) d_work + L->off_header,sizeof(h),cudaMemcpyDeviceToHost,
                           (cudaStream_t) stream));
   HM_CUDA(cudaStreamSynchronize((cudaStream_t) stream));
-  *n_cand = h[0]; *status = h[1]; *n_s = h[SY_HDR_S];
+  *n_cand = h[SY_HDR_CAND]; *status = h[SY_HDR_STATUS]; *n_s = h[SY_HDR_S];
   return HM_OK;
 }
 
 /* pass 2 of the streamed scan: the exact check of a Bloom hit is a look-up in the sorted S list (several shards:
- * the S list of the key's owner, reached through d_views, whose address goes into header word SY_HDR_S+4)    */
+ * the S list of the key's owner, reached through the view's d_views)                                          */
 int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
                                       const void *d_s_bucket, int bits, int idx64, int kmer, int64_t range,
                                       void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
@@ -1914,17 +1875,10 @@ int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int6
     return hm_set_error(HM_EINVAL,"symm_stream_resolve: bad arguments");
   cudaStream_t st = (cudaStream_t) stream;
   SymmView W = stream_view(d_work,L,R,shards);
-  if (W.n_seg > 1)
-    { uint64_t v = (uint64_t) (uintptr_t) d_views;
-      HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_S+4,&v,sizeof(v),cudaMemcpyHostToDevice,st));
-    }
-  cudaError_t e;
-  if (kmer <= 32)
-    e = idx64 ? launch_resolve<uint64_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
-              : launch_resolve<uint32_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
-  else
-    e = idx64 ? launch_resolve<uint64_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
-              : launch_resolve<uint32_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
+  W.sviews = d_views;
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_resolve<typename decltype(I)::IdxT,decltype(I)::KW,LK_SLIST>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,
+                                                                                kmer,W,d_plot,range,st); });
   if (l2_persist())
     bloom_window(st,NULL,0,0);
   if (e != cudaSuccess)
@@ -1935,43 +1889,41 @@ int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int6
 /* ------------------------------------------------------------------ routed pass 2 --------- */
 /* One rank of a one-process-per-GPU job streams its own share (hm_scan.cu hm_rank_scan_*, DESIGN.md §4c): nobody
  * can read another rank's S list, so pass 2 goes in rounds over slices [c0, c1) of the rank's candidates.
- * resolve_kernel<..., SL = true, RT = true> settles what the rank's own S list decides and parks the rest
- * (route_push); route_count / route_scatter group the queries by owner (a one-digit radix sort: not a hot path);
- * the caller sends the key words to their owners, route_answer_kernel answers the keys that arrive, the
- * answers come back in the order they were sent, and route_mark / route_settle count every parked candidate
- * none of whose queried keys was found.                                                                    */
+ * resolve_kernel<..., LK_ROUTED> settles what the rank's own S list decides and parks the rest (route_push);
+ * route_count / route_scatter group the queries by owner (a one-digit radix sort: not a hot path); the caller
+ * sends the key words to their owners, route_answer_kernel answers the keys that arrive, the answers come back
+ * in the order they were sent, and route_mark / route_settle count every parked candidate none of whose
+ * queried keys was found.                                                                                     */
 static SymmView route_view(void *d_work, const hm_symm_layout *L, const hm_stream_lists *R, const hm_symm_shards *sh,
-                           int64_t c0, int64_t c1)
-{ SymmView W = stream_view(d_work,L,R,sh);
-  W.cand_key += c0; W.cand_meta += c0;
-  if (W.cand_lo != NULL) W.cand_lo += c0;
-  W.cand_cap = (unsigned long long) (c1-c0);             /* the header's count (all candidates) is >= c1 */
+                           const hm_route_bufs *B, int64_t c0, int64_t c1)
+{ SymmView W = slice_view(stream_view(d_work,L,R,sh),c0,c1);    /* (the header counts all candidates: >= c1) */
+  W.pend = B->pend; W.pend_key = B->pend_key; W.pend_lo = B->pend_lo;
+  W.q_key = B->q_key; W.q_lo = B->q_lo; W.q_tag = B->q_tag;
+  W.pend_cap = (unsigned long long) B->pend_cap; W.q_cap = (unsigned long long) B->q_cap;
   return W;
+}
+
+/* the arguments hm_symm_route_resolve and hm_symm_route_extract share: a slice the buffers can take */
+static bool route_args_ok(int kmer, const uint64_t *d_s_lo, const hm_stream_lists *R, const hm_route_bufs *B,
+                          int64_t c0, int64_t c1)
+{ return kmer >= HM_SYMM_MIN_KMER && kmer <= HM_MAX_KMER && (kmer > 32) == (d_s_lo != NULL) && B != NULL &&
+         c0 >= 0 && c1 >= c0 && c1 <= R->cand_cap && c1-c0 <= B->pend_cap && 2*(c1-c0) <= B->q_cap;
 }
 
 int hm_symm_route_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
                           const void *d_s_bucket, int bits, int idx64, int kmer, int64_t c0, int64_t c1,
                           void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
                           const hm_symm_shards *shards, const hm_route_bufs *B, unsigned long long *d_plot, void *stream)
-{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_plot == NULL ||
-      B == NULL || c0 < 0 || c1 < c0 || c1 > R->cand_cap || c1-c0 > B->pend_cap || 2*(c1-c0) > B->q_cap)
+{ if (d_plot == NULL || !route_args_ok(kmer,d_s_lo,R,B,c0,c1))
     return hm_set_error(HM_EINVAL,"symm_route_resolve: bad arguments");
   cudaStream_t st = (cudaStream_t) stream;
-  SymmView W = route_view(d_work,L,R,shards,c0,c1);
-  uint64_t h[8] = { 0, 0, (uint64_t) (uintptr_t) B->pend, (uint64_t) (uintptr_t) B->q_key, (uint64_t) (uintptr_t) B->q_lo,
-                    (uint64_t) (uintptr_t) B->q_tag, (uint64_t) B->pend_cap, (uint64_t) B->q_cap };
-  HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_R,h,sizeof(h),cudaMemcpyHostToDevice,st));
-  HM_CUDA(cudaStreamSynchronize(st));                    /* (h is on the stack) */
+  SymmView W = route_view(d_work,L,R,shards,B,c0,c1);
+  HM_CUDA(cudaMemsetAsync(W.cand_n+SY_HDR_PEND,0,2*sizeof(uint64_t),st));   /* the round's pending and query counts */
   if (c1 == c0)
     return HM_OK;
-  cudaError_t e;
-  int64_t range = 8*(c1-c0);
-  if (kmer <= 32)
-    e = idx64 ? launch_resolve<uint64_t,1,true,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
-              : launch_resolve<uint32_t,1,true,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
-  else
-    e = idx64 ? launch_resolve<uint64_t,2,true,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st)
-              : launch_resolve<uint32_t,2,true,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_plot,range,st);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_resolve<typename decltype(I)::IdxT,decltype(I)::KW,LK_ROUTED>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,
+                                                                                 kmer,W,d_plot,8*(c1-c0),st); });
   if (l2_persist())
     bloom_window(st,NULL,0,0);
   if (e != cudaSuccess)
@@ -2007,13 +1959,13 @@ static int route_grid(int64_t n)
 int hm_symm_route_group(int kmer, int world, void *d_work, const hm_symm_layout *L, const hm_route_bufs *B,
                         int64_t *counts, int64_t *n_sent, int64_t *n_pend, uint64_t *status, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
-  uint64_t h[SY_HDR_R+2];
+  uint64_t h[SY_HDR_QUERY+1];
   HM_CUDA(cudaMemcpyAsync(h,(const uint8_t *) d_work + L->off_header,sizeof(h),cudaMemcpyDeviceToHost,st));
   HM_CUDA(cudaMemsetAsync(B->counts,0,2*HM_MAX_SHARDS*sizeof(unsigned long long),st));
   HM_CUDA(cudaStreamSynchronize(st));
-  int64_t nq = (int64_t) h[SY_HDR_R+1];
-  *status = h[1];
-  *n_pend = (int64_t) h[SY_HDR_R] < B->pend_cap ? (int64_t) h[SY_HDR_R] : B->pend_cap;
+  int64_t nq = (int64_t) h[SY_HDR_QUERY];
+  *status = h[SY_HDR_STATUS];
+  *n_pend = (int64_t) h[SY_HDR_PEND] < B->pend_cap ? (int64_t) h[SY_HDR_PEND] : B->pend_cap;
   if (nq > B->q_cap) nq = B->q_cap;                       /* (an overflow is in the status word) */
   *n_sent = nq;
   for (int r = 0; r < world; r++) counts[r] = 0;
@@ -2053,15 +2005,10 @@ int hm_symm_route_answer(const uint64_t *d_s_key, const uint64_t *d_s_lo, const 
 { cudaStream_t st = (cudaStream_t) stream;
   if (n > 0)
     { const int g = route_grid(n), sh = 64-bits;
-      if (kmer <= 32)
-        { if (idx64) route_answer_kernel<uint64_t,1><<<g,256,0,st>>>(d_s_key,NULL,(const uint64_t *) d_s_bucket,sh,d_recv,n,d_ans);
-          else       route_answer_kernel<uint32_t,1><<<g,256,0,st>>>(d_s_key,NULL,(const uint32_t *) d_s_bucket,sh,d_recv,n,d_ans);
-        }
-      else
-        { if (idx64) route_answer_kernel<uint64_t,2><<<g,256,0,st>>>(d_s_key,d_s_lo,(const uint64_t *) d_s_bucket,sh,d_recv,n,d_ans);
-          else       route_answer_kernel<uint32_t,2><<<g,256,0,st>>>(d_s_key,d_s_lo,(const uint32_t *) d_s_bucket,sh,d_recv,n,d_ans);
-        }
-      HM_CUDA(cudaGetLastError());
+      HM_CUDA(dispatch(kmer,idx64,[&](auto I)
+        { typedef typename decltype(I)::IdxT IdxT;
+          route_answer_kernel<IdxT,decltype(I)::KW><<<g,256,0,st>>>(d_s_key,d_s_lo,(const IdxT *) d_s_bucket,sh,d_recv,n,d_ans);
+          return cudaGetLastError(); }));
     }
   HM_CUDA(cudaStreamSynchronize(st));
   return HM_OK;
@@ -2104,7 +2051,7 @@ int hm_symm_route_settle(int kmer, const hm_route_bufs *B, const uint8_t *d_ans,
 
 /* ------------------------------------------------------------------ routed pair listing ---- */
 /* extract_kmer_pairs on one rank (hm_rank_scan_extract_*, DESIGN.md §4c): the rounds of routed pass 2, with
- * extract_kernel<..., RT = true> in place of resolve_kernel and route_list_kernel in place of route_settle_kernel.
+ * extract_kernel<..., LK_ROUTED> in place of resolve_kernel and route_list_kernel in place of route_settle_kernel.
  * A round's records (at most two per candidate of its slice) go to out through one counter, which counts every
  * record, also those beyond cap.                                                                          */
 int hm_symm_route_extract(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
@@ -2112,27 +2059,18 @@ int hm_symm_route_extract(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64
                           void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
                           const hm_symm_shards *shards, const hm_route_bufs *B, const uint16_t *d_pixmap,
                           hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count, void *stream)
-{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || (kmer > 32) != (d_s_lo != NULL) || d_pixmap == NULL ||
-      d_count == NULL || B == NULL || B->pend_key == NULL || (kmer > 32 && B->pend_lo == NULL) || c0 < 0 || c1 < c0 ||
-      c1 > R->cand_cap || c1-c0 > B->pend_cap || 2*(c1-c0) > B->q_cap || cap < 2*(c1-c0) || d_out == NULL)
+{ if (d_pixmap == NULL || d_count == NULL || d_out == NULL || !route_args_ok(kmer,d_s_lo,R,B,c0,c1) ||
+      B->pend_key == NULL || (kmer > 32 && B->pend_lo == NULL) || cap < 2*(c1-c0))
     return hm_set_error(HM_EINVAL,"symm_route_extract: bad arguments");
   cudaStream_t st = (cudaStream_t) stream;
-  SymmView W = stream_view(d_work,L,R,shards);
-  uint64_t h[10] = { 0, 0, (uint64_t) (uintptr_t) B->pend, (uint64_t) (uintptr_t) B->q_key, (uint64_t) (uintptr_t) B->q_lo,
-                     (uint64_t) (uintptr_t) B->q_tag, (uint64_t) B->pend_cap, (uint64_t) B->q_cap,
-                     (uint64_t) (uintptr_t) B->pend_key, (uint64_t) (uintptr_t) B->pend_lo };
-  HM_CUDA(cudaMemcpyAsync(W.cand_n+SY_HDR_R,h,sizeof(h),cudaMemcpyHostToDevice,st));
+  SymmView W = route_view(d_work,L,R,shards,B,c0,c1);
+  HM_CUDA(cudaMemsetAsync(W.cand_n+SY_HDR_PEND,0,2*sizeof(uint64_t),st));   /* the round's pending and query counts */
   HM_CUDA(cudaMemsetAsync(d_count,0,sizeof(unsigned long long),st));
-  HM_CUDA(cudaStreamSynchronize(st));                    /* (h is on the stack) */
   if (c1 == c0)
     return HM_OK;
-  cudaError_t e;
-  if (kmer <= 32)
-    e = idx64 ? launch_extract<uint64_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
-              : launch_extract<uint32_t,1,true>(d_s_key,NULL,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
-  else
-    e = idx64 ? launch_extract<uint64_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st)
-              : launch_extract<uint32_t,2,true>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,kmer,W,d_pixmap,c0,c1,d_out,cap,d_count,st);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { return launch_extract<typename decltype(I)::IdxT,decltype(I)::KW,LK_ROUTED>(d_s_key,d_s_lo,NULL,n_s,d_s_bucket,bits,
+                                                                                 kmer,W,d_pixmap,d_out,cap,d_count,st); });
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"extract_kernel (routed)");
   return HM_OK;
