@@ -519,35 +519,80 @@ runs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys
     }
 }
 
-/* runscan_kernel, step 4: member a of the run of L entries at window slots h .. h+L-1.  Its partners in the
- * run give H and U (Bloom insert when U > 0); a candidate record when H(x) = H(partner) = 1 and x is the
- * lower member (the partner's H is counted here too, so no member waits for another's counts).  -> emit  */
-template <int KW, bool SL>
-__device__ __forceinline__ bool settle_member(const RsSmem<KW> &S, const SymmView &W, int kmer, int pup,
-                                              int h, int L, int a, uint64_t &x, uint64_t &xl, uint64_t &meta)
-{ x  = S.key[h+a];
-  xl = KW == 2 ? S.klo[h+a] : 0;
-  const int cx = S.cnt[h+a];
-  int Hx = 0, Ux = 0, part = 0, ppos = 0;
-  for (int b = 0; b < L; b++)
-    { int pos;
-      if (b != a && one_base_apart<KW>(x,xl,S.key[h+b],KW == 2 ? S.klo[h+b] : 0,pos) && cx + (int) S.cnt[h+b] <= HM_SMAX)
-        { Hx += 1;
-          if (pos >= pup) Ux += 1;
-          part = b; ppos = pos;
+/* runscan_kernel's pair test inside a run.  The members of a run share their first Pr = k/2 bases, so two
+ * of them differ only in the last k-Pr: 2(k-Pr) <= 32 bits for k <= 32, <= 64 bits for k <= 64.  run_sfx
+ * puts those bases left aligned into one word of RunSfx<KW>::T (of x ^ y: the xor of the two suffixes), and
+ * one_base_in_run tests that word and gives the same pos as one_base_apart on the whole keys.          */
+template <int KW> struct RunSfx    { typedef uint64_t T; };
+template <>       struct RunSfx<1> { typedef uint32_t T; };
+
+template <int KW>
+__device__ __forceinline__ typename RunSfx<KW>::T run_sfx(uint64_t hi, uint64_t lo, int Pr)
+{ if constexpr (KW == 1)
+    return (uint32_t) ((hi << 2*Pr) >> 32);                       /* Pr <= 16 */
+  else
+    return (hi << (2*Pr-32) << 32) | (lo >> (64-2*Pr));            /* 16 <= Pr <= 32 */
+}
+
+template <typename T>
+__device__ __forceinline__ bool one_base_in_run(T d, int Pr, int &pos)
+{ const T u = (d | (d >> 1)) & (T) HM_M5;
+  if constexpr (sizeof(T) == 4) pos = Pr + (__clz((int) d) >> 1);
+  else                          pos = Pr + (__clzll((long long) d) >> 1);
+  return (u & (u-1)) == 0;
+}
+
+/* runscan_kernel, step 4 (warp-wide): the lane's member a of the run of L entries at window slots h .. h+L-1,
+ * if it has one (in); own = the member is this CTA's to settle.  Its partners in the run give H and U (Bloom
+ * insert when U > 0); a candidate record when H(x) = H(partner) = 1 and x is the lower member.  The partner
+ * is member `part` of the same run, which lane + part - a holds and has counted in this same pass unless
+ * that lane lies past the warp's 32 (only runs straddling two passes): then its H is counted here.
+ * LMAX > 0: L <= LMAX, and the run mates are read in one unrolled sweep (slots h .. h+LMAX-1 lie in the
+ * window), so their loads overlap instead of forming a chain.                                         -> emit */
+template <int KW, bool SL, int LMAX>
+__device__ __forceinline__ bool settle_members(const RsSmem<KW> &S, const SymmView &W, int kmer, int Pr, int pup,
+                                               int h, int L, int a, bool in, bool own, int lane,
+                                               uint64_t &x, uint64_t &xl, uint64_t &meta)
+{ int Hx = 0, Ux = 0, part = 0, ppos = 0, cx = 0;
+  if (in)
+    { x  = S.key[h+a];
+      xl = KW == 2 ? S.klo[h+a] : 0;
+      cx = S.cnt[h+a];
+      auto mate = [&](int b)
+        { int pos;
+          if (b < L && b != a && one_base_in_run(run_sfx<KW>(x ^ S.key[h+b],KW == 2 ? xl ^ S.klo[h+b] : 0,Pr),Pr,pos) &&
+              cx + (int) S.cnt[h+b] <= HM_SMAX)
+            { Hx += 1;
+              if (pos >= pup) Ux += 1;
+              part = b; ppos = pos;
+            }
+        };
+      if constexpr (LMAX > 0)
+        {
+#pragma unroll
+          for (int b = 0; b < LMAX; b++)
+            mate(b);
         }
+      else
+        for (int b = 0; b < L; b++)
+          mate(b);
+      if (own && Ux > 0)
+        bloom_insert<KW,SL>(W,kmer,x,xl);
     }
-  if (Ux > 0)
-    bloom_insert<KW,SL>(W,kmer,x,xl);
-  if (Hx != 1 || part < a)
+  const int pl = lane + part - a;                                  /* the partner's lane */
+  int       Hy = __shfl_sync(0xffffffffu,Hx,pl & 31);
+  if (!in || !own || Hx != 1 || part < a)
     return false;
   const uint64_t y = S.key[h+part], yl = KW == 2 ? S.klo[h+part] : 0;
   const int      cy = S.cnt[h+part];
-  int Hy = 0;
-  for (int b = 0; b < L; b++)
-    { int pos;
-      if (b != part && one_base_apart<KW>(y,yl,S.key[h+b],KW == 2 ? S.klo[h+b] : 0,pos) && cy + (int) S.cnt[h+b] <= HM_SMAX)
-        Hy += 1;
+  if (pl > 31)                                                     /* (part > a, so pl > lane >= 0) */
+    { Hy = 0;
+      for (int b = 0; b < L; b++)
+        { int pos;
+          if (b != part && one_base_in_run(run_sfx<KW>(y ^ S.key[h+b],KW == 2 ? yl ^ S.klo[h+b] : 0,Pr),Pr,pos) &&
+              cy + (int) S.cnt[h+b] <= HM_SMAX)
+            Hy += 1;
+        }
     }
   if (Hy != 1)
     return false;
@@ -568,18 +613,68 @@ __device__ __forceinline__ bool settle_member(const RsSmem<KW> &S, const SymmVie
  *   3. two-entry runs: one comparison settles both members (per-warp task list, every lane busy)
  *   4. longer runs (5 % of the entries, a few per warp) from the same per-warp list, still from shared
  *      memory: a run whose head is in the tile and that has at most RS_RUNCAP = RS_HALO+1 entries lies
- *      inside the window.  3..8 entries: a lane per member, the members of all the warp's runs one
- *      after the other (a run per lane, every pair once, costs the warp its longest run's L^2/2
- *      comparisons and a staging call per member: 2.07-2.11 against 1.98-2.01 ms per benchmark step);
- *      9..RS_RUNCAP: the whole warp, one member per lane.  Only runs that may reach past the window
- *      are listed for runs_kernel (none in the 2e8-entry benchmark table, whose 3.4e6 runs of three or
- *      more took runs_kernel 0.40 ms on one H100 SXM at 400 W when it settled them all)
+ *      inside the window.  Its length is the count of ones from the head on in the adjacency bits of
+ *      step 1 (two shuffles, a funnel shift, __ffs; 33 or more: the rest from the keys).  3..8 entries:
+ *      a lane per member, the members of all the warp's runs one after the other (a run per lane, every
+ *      pair once, costs the warp its longest run's L^2/2 comparisons and a staging call per member:
+ *      2.07-2.11 against 1.98-2.01 ms per benchmark step); 9..RS_RUNCAP: the whole warp, one member
+ *      per lane.  A member counts its own partners only; the single partner's count is read from the
+ *      partner's lane.  Only runs that may reach past the window are listed for runs_kernel (none in
+ *      the 2e8-entry benchmark table, whose 3.4e6 runs of three or more took runs_kernel 0.40 ms on one
+ *      H100 SXM at 400 W when it settled them all)
+ *   Pair tests in steps 3 and 4 look at the bases after the run prefix only, one 32-bit word for k <= 32
+ *   and one 64-bit word for k <= 64 (run_sfx, one_base_in_run).
  *   5. candidate records and run heads are staged in shared memory; the LAST warp to finish moves
  *      them out with one global atomic per CTA and list (one per record, or per warp, on the one
  *      list counter serialises in L2)
  * (The alternatives -- every entry scanning its run in place, per-entry classification with predicated
  * list writes, CTA-wide task lists with a barrier per phase -- need more instructions, leave more lanes
  * idle or wait at the barriers.)                                                                      */
+#ifdef RS_PROBE
+/* Probe build only (make EXTRA=-DRS_PROBE=1, tools/time_runscan_phases.py): the clock64() cycles every warp
+ * spends in each phase (0 staging / TMA wait, 1..5 as numbered in the kernel), summed over all warps with one
+ * atomic per warp and phase -- into one of RS_PROBE_SLOTS rows by CTA, as a few hundred thousand atomics on
+ * six addresses would serialise in L2 and time themselves -- and a mode: 0 the full kernel, 1 stage the
+ * window and return (load-only bound), 2 every CTA stages tile blockIdx.x % 64, which stays in L2, and does
+ * the full work (compute-only bound).                                                                   */
+#define RS_PHASES 6
+#define RS_PROBE_SLOTS 1024
+__device__ unsigned long long rs_probe_cycles[RS_PROBE_SLOTS*RS_PHASES];
+__device__ int rs_probe_mode;
+#define RS_PROBE_TILE(b)  (rs_probe_mode == 2 ? (b) % 64 : (b))
+#define RS_PROBE_START    long long rs_t = clock64(); unsigned long long rs_acc[RS_PHASES] = {0, 0, 0, 0, 0, 0};
+#define RS_PROBE_MARK(ph) { const long long t_ = clock64(); rs_acc[ph] += (unsigned long long) (t_ - rs_t); rs_t = t_; }
+#define RS_PROBE_FLUSH()  { if (lane == 0) _Pragma("unroll") for (int p_ = 0; p_ < RS_PHASES; p_++) \
+                              atomicAdd(rs_probe_cycles + (blockIdx.x % RS_PROBE_SLOTS)*RS_PHASES + p_,rs_acc[p_]); }
+#define RS_PROBE_LOADONLY() if (rs_probe_mode == 1) { RS_PROBE_FLUSH(); return; }
+
+/* cycles != NULL: the sums since the last call into cycles[RS_PHASES]; then clear them and set the mode */
+extern "C" int hm_probe_runscan(int mode, unsigned long long *cycles)
+{ static unsigned long long rows[RS_PROBE_SLOTS*RS_PHASES];
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess && cycles != NULL)
+    { e = cudaMemcpyFromSymbol(rows,rs_probe_cycles,sizeof(rows));
+      for (int p = 0; p < RS_PHASES; p++)
+        { cycles[p] = 0;
+          for (int r = 0; r < RS_PROBE_SLOTS; r++)
+            cycles[p] += rows[r*RS_PHASES+p];
+        }
+    }
+  memset(rows,0,sizeof(rows));
+  if (e == cudaSuccess)
+    e = cudaMemcpyToSymbol(rs_probe_cycles,rows,sizeof(rows));
+  if (e == cudaSuccess)
+    e = cudaMemcpyToSymbol(rs_probe_mode,&mode,sizeof(mode));
+  return e == cudaSuccess ? HM_OK : hm_cuda_fail(e,"hm_probe_runscan");
+}
+#else
+#define RS_PROBE_TILE(b)  (b)
+#define RS_PROBE_START
+#define RS_PROBE_MARK(ph)
+#define RS_PROBE_FLUSH()
+#define RS_PROBE_LOADONLY()
+#endif
+
 template <typename IdxT, int KW, bool SL>
 __global__ void __launch_bounds__(RS_THREADS,RS_MINBLOCKS)
 runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
@@ -606,8 +701,9 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
   const int      lane = threadIdx.x & 31;
   const int      warp = threadIdx.x >> 5;
   const unsigned lt   = (1u << lane) - 1;
+  RS_PROBE_START
 
-  const int64_t T0 = (tile0 + blockIdx.x) * RS_TILE;
+  const int64_t T0 = (tile0 + RS_PROBE_TILE(blockIdx.x)) * RS_TILE;
   const int64_t ws = T0 - RS_HALO;
   const int64_t e0 = ws > 0 ? ws : 0;
   const int64_t e1 = T0+RS_TILE+RS_HALO < n ? T0+RS_TILE+RS_HALO : n;
@@ -650,6 +746,8 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
     }
   else
     mbar_wait(&s_bar,0);
+  RS_PROBE_MARK(0)
+  RS_PROBE_LOADONLY()
 
   /* ---- 1. adjacency bits of this warp's words wd0-1 .. wd0+RS_EPT, word t in lane t ---- */
   const int wd0 = RS_HALO/32 + warp*RS_EPT;            /* first word (32 slots) of this warp's part of the tile */
@@ -669,6 +767,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
       const unsigned bal = __ballot_sync(FULL,eq);
       if (lane == t) eqw = bal;
     }
+  RS_PROBE_MARK(1)
 
   /* ---- 2. classify: lane t in 1..RS_EPT takes word wd0-1+t ---- */
   const int a0 = RS_HALO + (lo > T0 ? (int) (lo-T0 < RS_TILE ? lo-T0 : RS_TILE) : 0);   /* slots this CTA answers for */
@@ -714,6 +813,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
       }
   }
   __syncwarp();
+  RS_PROBE_MARK(2)
 
   /* ---- 3. runs of two: one comparison settles both members ---- */
   for (int i0 = 0; i0 < n1; i0 += 32)
@@ -728,7 +828,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
           if (KW == 2) { xl = S.klo[w]; yl = S.klo[w+1]; }
           const int cx = S.cnt[w], cy = S.cnt[w+1];
           int pos;
-          if (one_base_apart<KW>(x,xl,y,yl,pos) && cx+cy <= HM_SMAX)      /* H(x) = H(y) = 1 */
+          if (one_base_in_run(run_sfx<KW>(x ^ y,xl ^ yl,Pr),Pr,pos) && cx+cy <= HM_SMAX)   /* H(x) = H(y) = 1 */
             { emit = true;
               meta = pack_meta(cx,cy,pos,base_at<KW>(y,yl,pos));
               if (pos >= pup)                                              /* U(x) = U(y) = 1: both are in S */
@@ -739,20 +839,23 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         }
       stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
     }
+  RS_PROBE_MARK(3)
 
   /* ---- 4. longer runs, from the window: a run whose head is in the tile and that has at most RS_RUNCAP
    *         entries lies inside it.  Members at or after hi are not ours (slots >= b1) ---- */
   const int b1 = hi-T0 < RS_TILE+RS_HALO ? RS_HALO + (int) (hi-T0) : RS_WIN;
   for (int i0 = 0; i0 < n3; i0 += 32)
     { const int i = i0+lane;
-      int h = 0, L = 0;                                  /* head slot, run length (counted up to 9) */
-      if (i < n3)
-        { h = my1[n1+i];
-          const uint64_t xh = S.key[h];
-          L = 3;
-          while (L <= 8 && ((S.key[h+L] ^ xh) & pmask) == 0)        /* h+8 < RS_WIN */
-            L += 1;
-        }
+      const int h = i < n3 ? my1[n1+i] : 0;              /* head slot */
+      int       L = 0;                                   /* run length; 33: 33 or more */
+      { /* the run's extent from the adjacency bits: eq[h], eq[h+1], ... are ones up to its last member.  h lies
+         * in word wd0-1+t, t in 1..RS_EPT; lanes t and t+1 hold that word and the next: 32 bits in view */
+        const int      t  = (h >> 5) - (wd0-1);
+        const unsigned w0 = __shfl_sync(FULL,eqw,t & 31), w1 = __shfl_sync(FULL,eqw,(t+1) & 31);
+        const unsigned up = __funnelshift_r(w0,w1,h & 31);                          /* eq[h .. h+31] */
+        if (i < n3)
+          L = (~up != 0) ? __ffs((int) ~up) : 33;
+      }
       /* 3..8 entries: a lane per member, the members of all the lanes' runs one after the other */
       const int Ls = L <= 8 ? L : 0;
       int inc = Ls;                                      /* inclusive scan of the members over the lanes */
@@ -772,8 +875,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
           const int a  = t - (__shfl_sync(FULL,inc,r) - Lr);
           bool     emit = false;
           uint64_t x = 0, xl = 0, meta = 0;
-          if (t < M && hr+a < b1)
-            emit = settle_member<KW,SL>(S,W,kmer,pup,hr,Lr,a,x,xl,meta);
+          emit = settle_members<KW,SL,8>(S,W,kmer,Pr,pup,hr,Lr,a,t < M,hr+a < b1,lane,x,xl,meta);
           stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
         }
       /* 9..RS_RUNCAP entries: the whole warp, one run after the other, a member per lane */
@@ -781,14 +883,16 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
       while (lb != 0)
         { const int src = __ffs(lb)-1;
           lb &= lb-1;
-          const int      hh = __shfl_sync(FULL,h,src);
-          const uint64_t xh = S.key[hh];
-          int LL = 9;                                    /* slots hh .. hh+8 are known to be in the run */
-          while (LL <= RS_RUNCAP)
-            { const int      t = hh+LL+lane;
-              const unsigned sb = __ballot_sync(FULL,t < RS_WIN && ((S.key[t] ^ xh) & pmask) == 0);
-              if (sb != FULL) { LL += __ffs(~sb)-1; break; }
-              LL += 32;
+          const int hh = __shfl_sync(FULL,h,src);
+          int       LL = __shfl_sync(FULL,L,src);
+          if (LL > 32)                                   /* (warp-uniform) slots hh .. hh+32 are in the run; the */
+            { const uint64_t xh = S.key[hh];             /*   rest of it from the keys, 32 slots at a time       */
+              while (LL <= RS_RUNCAP)
+                { const int      t = hh+LL+lane;
+                  const unsigned sb = __ballot_sync(FULL,t < RS_WIN && ((S.key[t] ^ xh) & pmask) == 0);
+                  if (sb != FULL) { LL += __ffs(~sb)-1; break; }
+                  LL += 32;
+                }
             }
           if (LL > RS_RUNCAP || hh+LL >= RS_WIN)           /* (warp-uniform) may go on past the window: runs_kernel */
             { if (lane == 0)
@@ -799,12 +903,12 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
             { const int a = a0+lane;
               bool     emit = false;
               uint64_t x = 0, xl = 0, meta = 0;
-              if (a < LL && hh+a < b1)
-                emit = settle_member<KW,SL>(S,W,kmer,pup,hh,LL,a,x,xl,meta);
+              emit = settle_members<KW,SL,0>(S,W,kmer,Pr,pup,hh,LL,a,a < LL,hh+a < b1,lane,x,xl,meta);
               stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
             }
         }
     }
+  RS_PROBE_MARK(4)
 
   /* ---- 5. the last warp to get here moves the staged records out ---- */
   __syncwarp();
@@ -815,7 +919,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
     }
   last = __shfl_sync(FULL,last,0);
   if (!last)
-    return;
+    { RS_PROBE_MARK(5) RS_PROBE_FLUSH() return; }
   __threadfence_block();
   const unsigned nr = s_nr;
   if (nr > 0)
@@ -831,7 +935,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
     }
   const unsigned nc = s_nc < RS_STAGE ? s_nc : RS_STAGE;
   if (nc == 0)
-    return;
+    { RS_PROBE_MARK(5) RS_PROBE_FLUSH() return; }
   unsigned long long base = 0;
   if (lane == 0)
     base = atomicAdd(W.cand_n,(unsigned long long) nc);
@@ -846,6 +950,8 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
       else
         atomicOr(W.status,SY_STATUS_OVERFLOW);
     }
+  RS_PROBE_MARK(5)
+  RS_PROBE_FLUSH()
 }
 
 /* Pass 1, crowded tables.  A run is the set of entries sharing their first k/2 bases, so an entry has
