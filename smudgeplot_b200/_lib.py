@@ -152,6 +152,7 @@ def lib():
     L.hm_filter_words.restype = i64
     L.hm_pick_filter_bits.argtypes = [i64]
     L.hm_k_pass2_plot.argtypes = [vp, vp, vp, i32, i64, i64, vp, C.POINTER(Shards), vp]
+    L.hm_k_pass2_extract.argtypes = [vp, vp, vp, vp, vp, i32, i64, i64, vp, vp, i64, vp, C.POINTER(Shards), vp]
     L.hm_k_min_count.argtypes = [vp, i64, i64, vp, vp]
     L.hm_k_find_keys.argtypes = [vp, vp, i64, vp, i32, i32, vp, vp, i64, vp, vp]
     L.hm_pick_bucket_bits.argtypes = [i64]

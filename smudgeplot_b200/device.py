@@ -273,6 +273,25 @@ class DeviceTable:
                                               self.lo, self.hi, _ptr(self.plot), self._shards(), _stream()))
         self.launches += 1
 
+    def pass2_extract(self, pixmap: torch.Tensor, out: torch.Tensor | None, count: torch.Tensor,
+                      lo: int | None = None, hi: int | None = None):
+        """extract_kmer_pairs from the direct passes' results (hm_k_pass2_extract, after pass 1 and the exchange of
+        the incidence bytes): the isolated pairs of entries [lo, hi) (default: the scan range [self.lo, self.hi))
+        whose pixel has a label in pixmap (int16[1001*501], device) are appended to `out` (uint8[cap * 24] device
+        tensor of hm_pair_rec; None = count only) and counted in count (int64[1], zeroed by the caller; it counts
+        every record, also those beyond cap).  At most one record per entry."""
+        import ctypes as C
+        lo = self.lo if lo is None else lo
+        hi = self.hi if hi is None else hi
+        assert self.lo <= lo <= hi <= self.hi, (lo, hi, self.lo, self.hi)
+        cap = out.numel() // C.sizeof(_lib.PairRec) if out is not None else 0
+        up = _ptr(self.up) + (lo - self.lo) * self.up.element_size()     # up[] is indexed from self.lo
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.hm_k_pass2_extract(_ptr(self.keys), _ptr(self.keys_lo), _ptr(self.cnt), self._deg(), up,
+                                                 self.idx64, lo, hi, _ptr(pixmap), _ptr(out), cap, _ptr(count),
+                                                 self._shards(), _stream()))
+        self.launches += 1
+
     def scan(self, path: str = "auto"):
         """one GPU; -> plot int64[1001,501] (device tensor).  path: "auto" = the symmetric scan when the
         fingerprint says the table is strand-symmetric, else the direct passes; "direct" / "symm" force one"""

@@ -299,7 +299,7 @@ class PeerDeg:
         else:
             ok = 0
         flag = torch.tensor([ok], dtype=torch.int32, device=device)
-        dist.all_reduce(flag, op=dist.ReduceOp.MIN, group=group)
+        _in_place(lambda x: dist.all_reduce(x, op=dist.ReduceOp.MIN, group=group), flag, group)
         if int(flag.item()) == 0:
             with torch.cuda.device(device):
                 for r, pp in enumerate(peers):
@@ -336,7 +336,9 @@ class PeerDeg:
 
 
 class ShardedScan:
-    """device-resident replica + this rank's work range; `scan()` = T_scan of SURVEY.md §8d"""
+    """device-resident replica + this rank's work range; `scan()` = T_scan of SURVEY.md §8d, `extract()` =
+    extract_kmer_pairs' list of the same job.  The collectives run on NCCL with a GPU per rank, or on gloo
+    through host copies (several ranks may then share one GPU)."""
 
     def __init__(self, kmer, keys_full, cnt_full, lo, hi, group=None, keys_lo_full=None, path="auto"):
         import os
@@ -344,16 +346,21 @@ class ShardedScan:
         self.group = group
         self.world = dist.get_world_size(group)
         self.rank = dist.get_rank(group)
+        self._coll_dev = keys_full.device if _nccl(group) else torch.device("cpu")
+        self._backend = "NCCL" if _nccl(group) else "gloo, through host memory"
         self.table = DeviceTable(kmer, keys_full, cnt_full, keys_lo=keys_lo_full).build_index(direct=False)
         self.load_lo, self.load_hi = lo, hi       # the shard this rank LOADED (equal prefix ranges)
         self.kmer = kmer
         self.n_total = keys_full.numel()
         self.bits = self.table.bits
         self.peer = None
+        self.stats = {}
+        self._scanned = False                     # the last scan_on() was a scan() of self.table
         # is the whole table strand-symmetric?  every rank fingerprints the shard it loaded
         path = os.environ.get("HETMERS_PATH", path)
-        self.seeds = common_seeds(keys_full.device, group)
-        self.symmetric = kmer >= 2 and fingerprint_verdict(self.table.fingerprint(lo, hi, self.seeds), group)
+        self.seeds = common_seeds(self._coll_dev, group)
+        self.symmetric = kmer >= 2 and fingerprint_verdict(
+            self.table.fingerprint(lo, hi, self.seeds).to(self._coll_dev), group)
         self.table.symmetric = self.symmetric
         self.path = "symm" if (self.symmetric and path != "direct") else "direct"
         if self.path == "symm":
@@ -362,7 +369,8 @@ class ShardedScan:
             lo, hi = self.offsets[self.rank], self.offsets[self.rank + 1]
             self.table.alloc_symm(lo, hi, self.table.make_symm_shards(self.offsets, self.rank) if self.world > 1 else None)
             self.lo, self.hi = lo, hi
-            self.exchange = "all-gather of Bloom segments (NCCL) between run scan and resolve" if self.world > 1 else "none"
+            self.exchange = f"all-gather of Bloom segments ({self._backend}) between run scan and resolve" \
+                if self.world > 1 else "none"
         else:
             self._init_direct(keys_full)
         self._barrier_t = torch.zeros(1, dtype=torch.int32, device=keys_full.device)
@@ -383,7 +391,7 @@ class ShardedScan:
         self.lo, self.hi = lo, hi
         self.peer = PeerDeg.create(self.n_total, keys_full.device, self.group) if self.world > 1 else None
         self.exchange = "peer-memory (remote atomics/loads over NVLink, CUDA IPC)" if self.peer else \
-                        ("all-reduce(uint8[n]) via NCCL" if self.world > 1 else "none")
+                        (f"all-reduce(uint8[n]) via {self._backend}" if self.world > 1 else "none")
 
     @classmethod
     def from_synthetic(cls, k, G, ploidy, het, cov, L, seed, device, group=None):
@@ -403,6 +411,53 @@ class ShardedScan:
         del keys, cnt16
         return cls(k, kf, cf, lo, hi, group)
 
+    @classmethod
+    def from_ktab(cls, name, group=None, device=None, path="auto"):
+        """the FastK table `name` (stub + part files): rank r reads the records of ordinals [n*r/W, n*(r+1)/W)
+        (a range may span part files), unpacks them on its GPU with the table's own ibyte, and the shares are
+        all-gathered into the replica every rank holds (gather_table; on gloo the shares meet in host memory)"""
+        import numpy as np
+        from . import fastk
+        from .device import DeviceTable
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        dev = torch.device(device if device is not None else "cuda")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        kt = fastk.read_ktab(str(name), mmap=True)
+        k, n, pb = kt.kmer, kt.nels, kt.pbyte
+        lo, hi = (n * rank) // world, (n * (rank + 1)) // world
+        rec = np.empty((hi - lo) * pb, dtype=np.uint8)
+        at = start = 0
+        for p, pn in enumerate(kt.part_nels):                  # the share's records, part by part
+            a, b = max(lo, start), min(hi, start + pn)
+            if a < b:
+                rec[at:at + (b - a) * pb] = kt.records[p][(a - start) * pb:(b - start) * pb]
+                at += (b - a) * pb
+            start += pn
+        with torch.cuda.device(dev):
+            room = n + world                                   # room for gather_table's even chunks
+            kb = torch.empty(room, dtype=torch.int64, device=dev)
+            cb = torch.empty(room, dtype=torch.int16, device=dev)
+            lb = torch.empty(room, dtype=torch.int64, device=dev) if k > 32 else None
+            if hi > lo:
+                d_rec = torch.from_numpy(rec).to(dev)
+                d_idx = torch.from_numpy(np.ascontiguousarray(kt.index, dtype=np.int64)).to(dev)
+                DeviceTable.from_records(k, kt.ibyte, d_rec, d_idx, first=lo, out=(kb, cb), out_lo=lb)
+                del d_rec, d_idx
+            del rec, kt
+            share = (kb[lo:hi], cb[lo:hi], lb[lo:hi] if lb is not None else None)
+            if _nccl(group):
+                got = gather_table(share[0], share[1], group, out=(kb, cb), local_lo=share[2], out_lo=lb)
+            else:
+                got = gather_table(share[0].cpu(), share[1].cpu(), group,
+                                   local_lo=share[2].cpu() if lb is not None else None)
+                kb[:n].copy_(got[0])
+                cb[:n].copy_(got[1])
+                if lb is not None:
+                    lb[:n].copy_(got[4])
+            assert (got[2], got[3]) == (lo, hi)
+            return cls(k, kb[:n], cb[:n], lo, hi, group, keys_lo_full=lb[:n] if lb is not None else None, path=path)
+
     def close(self):
         if self.peer is not None:
             torch.cuda.synchronize()
@@ -411,7 +466,9 @@ class ShardedScan:
             self.peer = None
 
     def scan(self, events=None):
-        return self.scan_on(self.table, events)
+        plot = self.scan_on(self.table, events)
+        self._scanned = True
+        return plot
 
     def scan_on(self, t, events=None):
         """one T_scan on table replica `t` (self.table for the resident scans, a freshly loaded
@@ -422,6 +479,8 @@ class ShardedScan:
         pass 2 of scan s-1 (it could not have passed that scan's plot all-reduce otherwise), and
         nobody writes it before the plot all-reduce of scan s, which the clearing rank joins only
         after its memset (stream order)."""
+        g = self.group
+        self._scanned = False
         if self.path == "symm":
             return self._scan_symm(t, events)
         if self.peer is None:
@@ -433,10 +492,10 @@ class ShardedScan:
             if events is not None:
                 events[1].record()
             if self.world > 1:
-                allreduce_deg(t.deg, self.group)
+                _in_place(lambda x: allreduce_deg(x, g), t.deg, g)
             t.pass2()
             if self.world > 1:
-                allreduce_plot(t.plot, self.group)
+                _in_place(lambda x: allreduce_plot(x, g), t.plot, g)
             return t.plot
         par = self._step & 1
         self._step += 1
@@ -456,7 +515,7 @@ class ShardedScan:
         if events is not None:
             events[1].record()
         if ph: ph[1].record()
-        dist.all_reduce(self._barrier_t, group=self.group)            # all pass 1 kernels have landed
+        _in_place(lambda x: dist.all_reduce(x, group=g), self._barrier_t, g)   # all pass 1 kernels have landed
         if ph: ph[2].record()
         main = torch.cuda.current_stream()
         self._side.wait_stream(main)
@@ -466,13 +525,14 @@ class ShardedScan:
         if ph: ph[3].record()
         main.wait_stream(self._side)
         if ph: ph[4].record()
-        allreduce_plot(t.plot, self.group)                            # ... and before anybody can use it
+        _in_place(lambda x: allreduce_plot(x, g), t.plot, g)          # ... and before anybody can use it
         if ph: ph[5].record()
         return t.plot
 
     def _scan_symm(self, t, events=None):
         """strand-symmetric scan, sharded: run scan of the own (run-aligned) range -> all-gather of the
         Bloom segments -> resolve of the own candidates -> plot all-reduce.  No peer memory needed."""
+        g = self.group
         ph = self._phase_events() if self.profile_phases else None
         t.plot.zero_()
         if events is not None:
@@ -481,12 +541,12 @@ class ShardedScan:
         t.runscan(mid_event=events[1] if events is not None else None)   # [0],[1]: the dominant kernel alone
         if ph: ph[1].record()
         if self.world > 1:
-            exchange_segments(t.bloom_view(), self.rank, self.group)
+            _in_place(lambda x: exchange_segments(x, self.rank, g), t.bloom_view(), g)
         if ph: ph[2].record()
         t.resolve()
         if ph: ph[3].record(); ph[4].record()
         if self.world > 1:
-            allreduce_plot(t.plot, self.group)
+            _in_place(lambda x: allreduce_plot(x, g), t.plot, g)
         if ph: ph[5].record()
         return t.plot
 
@@ -497,8 +557,100 @@ class ShardedScan:
             _, st = self.table.symm_status()
             bad[0] = int(st != 0)
         if self.world > 1:
-            dist.all_reduce(bad, op=dist.ReduceOp.MAX, group=self.group)
+            _in_place(lambda x: dist.all_reduce(x, op=dist.ReduceOp.MAX, group=self.group), bad, self.group)
         return int(bad.item()) == 0
+
+    def extract(self, pixmap, dst: int = 0, timings: dict | None = None, budget: int | None = None):
+        """extract_kmer_pairs' pair list for a pixel -> smudge map (uint16[SMAX+1, FMAX+1], label 0 = none): on rank
+        `dst` the structured array hetmers.Scan.extract returns for the table, the same records in the same order;
+        None on the other ranks.  Lists from the last scan() of the resident replica, or runs one first (its plot is
+        dropped); stats["scan_reused"] says which.  Each rank lists its own range against its own replica:
+          symm    the candidates of its run-aligned range (DeviceTable.extract); a dirty status word on any rank
+                  raises on every rank;
+          direct  its range of the direct passes' results (DeviceTable.pass2_extract), a count launch and then the
+                  fill, reading the incidence bytes of the last scan (the peers' through PeerDeg, or the
+                  all-reduced array in dense mode); a barrier at the end keeps the next scan_on from clearing an
+                  incidence buffer a peer still reads.
+        The records go through one device buffer of what `budget` (device bytes for the listing; default: free
+        device memory minus _lib.BUDGET_RESERVE) leaves beside the pixmap and the counter: symm candidates in slices
+        of half its records (at most two records each), direct entries in slices of its records (at most one each)
+        when the count exceeds it.  Too little room for one slice is HM_ENOMEM on every rank, before any launch.
+        The ranks' records are gathered on dst and sorted there (gather_pairs).
+        timings (ms): scan, listing, d2h, gather_and_sort; stats: route, scan_reused, slices, records, ..."""
+        import numpy as np
+        from . import _lib
+        from .hetmers import PAIR_DTYPE
+        g, t, dev = self.group, self.table, self.table.device
+        pm = np.ascontiguousarray(pixmap, dtype=np.uint16).reshape(-1)
+        if pm.size != _lib.PLOT_CELLS:
+            raise ValueError(f"pixmap has {pm.size} cells, not {_lib.PLOT_CELLS}")
+        lap = _lapper({} if timings is None else timings)
+        item = PAIR_DTYPE.itemsize
+        symm = self.path == "symm"
+        with torch.cuda.device(dev):
+            reused = self._scanned
+            t0 = time.perf_counter()
+            if not reused:                                      # (every rank has called the same methods)
+                self.scan()
+                torch.cuda.synchronize(dev)
+                t0 = lap("scan", t0)
+            if symm and not self.symm_ok():
+                raise RuntimeError(f"rank {self.rank}: the last symmetric scan left a non-zero status word on some "
+                                   f"rank; its candidates must not be listed")
+            fixed = 2 * _lib.PLOT_CELLS + 256                   # the device pixmap and the record counter
+            need = 2 if symm else 1                             # the records of one slice
+            if budget is None:
+                budget = torch.cuda.mem_get_info(dev)[0] - _lib.BUDGET_RESERVE
+            room = max((budget - fixed) // item, 0)
+            short = torch.tensor([int(room < need)], dtype=torch.int32, device=self._coll_dev)
+            if self.world > 1:
+                dist.all_reduce(short, op=dist.ReduceOp.MAX, group=g)
+            if int(short.item()):
+                raise _lib.HetmersError(-3, f"rank {self.rank}: listing k-mer pairs needs at least {fixed + need * item} "
+                                            f"device bytes on every rank ({2 * _lib.PLOT_CELLS} for the pixmap, 256 for "
+                                            f"the counter, {need} x {item} for one slice's records); the budget here is "
+                                            f"{budget} bytes")
+            d_pix = torch.from_numpy(pm.view(np.int16)).to(dev)
+            count = torch.zeros(1, dtype=torch.int64, device=dev)
+            if symm:
+                nc, _ = t.symm_status()
+                nc = min(nc, t.symm_layout.cand_cap)
+                cap = max(min(room, 2 * nc), need)
+                step = cap // 2
+                ranges = [(c, min(c + step, nc)) for c in range(0, nc, step)]
+            else:
+                t.pass2_extract(d_pix, None, count)             # count launch
+                total = int(count.item())
+                cap = max(min(room, total), need)
+                step = cap if total > cap else max(t.hi - t.lo, 1)
+                ranges = [(a, min(a + step, t.hi)) for a in range(t.lo, t.hi, step)] if total else []
+            out = torch.empty(cap * item, dtype=torch.uint8, device=dev)
+            t0 = lap("listing", t0)
+            parts = []
+            for a, b in ranges:
+                count.zero_()
+                if symm:
+                    t.extract(d_pix, out, count, a, b)
+                else:
+                    t.pass2_extract(d_pix, out, count, a, b)
+                c = int(count.item())
+                if c > cap:
+                    raise _lib.HetmersError(-2, f"rank {self.rank}: {c} records listed from [{a}, {b}), beyond the "
+                                                f"buffer of {cap}")
+                t0 = lap("listing", t0)
+                if c:
+                    parts.append(out[:c * item].cpu().numpy())
+                t0 = lap("d2h", t0)
+            del out, d_pix, count
+            recs = (np.concatenate(parts) if len(parts) > 1 else parts[0] if parts else
+                    np.empty(0, dtype=np.uint8)).view(PAIR_DTYPE)
+            if not symm and self.world > 1:                     # nobody clears what a peer still reads
+                _in_place(lambda x: dist.all_reduce(x, group=g), self._barrier_t, g)
+            self.stats = {"route": self.path, "scan_reused": reused, "slices": len(ranges), "records": len(recs),
+                          "buffer_records": cap, "budget": budget, "range": [t.lo, t.hi]}
+            res = gather_pairs(recs, dst, g)
+            lap("gather_and_sort", t0)
+        return res
 
     profile_phases = False
 
@@ -639,6 +791,14 @@ def _nccl(group) -> bool:
     return dist.get_backend(group) == "nccl"
 
 
+def _lapper(tm: dict):
+    """lap(name, t0): add the ms since t0 to tm[name] -> the time now"""
+    def lap(name, t0):
+        tm[name] = tm.get(name, 0.0) + (time.perf_counter() - t0) * 1e3
+        return time.perf_counter()
+    return lap
+
+
 def _in_place(fn, t: torch.Tensor, group):
     """run collective fn(tensor) on t in place (NCCL), or through a host copy when the backend (gloo) has no
     collective for device tensors"""
@@ -764,10 +924,7 @@ class StreamedShardedScan:
         return _cuda_view(ptr, max(nbytes, 1), self.device)[:nbytes]
 
     def _lap(self, tm):
-        def lap(name, t0):
-            tm[name] = tm.get(name, 0.0) + (time.perf_counter() - t0) * 1e3
-            return time.perf_counter()
-        return lap
+        return _lapper(tm)
 
     def _sync(self):
         torch.cuda.synchronize(self.device)                    # (the library works on its own streams)
