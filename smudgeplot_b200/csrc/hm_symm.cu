@@ -1321,9 +1321,53 @@ extern "C" int hm_k_symm_runs(const uint64_t *d_keys, const uint64_t *d_keys_lo,
 #define RV_HA    (1ull << 48)      /* a queued record's meta: the Bloom bits of rc x / rc y were set */
 #define RV_HB    (1ull << 49)
 
+#ifdef RESOLVE_PROBE
+/* Probe build only (make EXTRA=-DRESOLVE_PROBE=1, tools/time_resolve_phases.py).  A mode: 0 the full kernel, 1 the
+ * candidate records only (loaded and dropped: the bound the record stream sets), 2 records and Bloom look-ups with
+ * every hit taken as not isolated (no exact check), 3 the full kernel counting what it sees; and the counts of mode
+ * 3: candidates, Bloom hits on rc x only / rc y only / both, exact checks that take the general path
+ * (has_upper_partner), and the sizes of the buckets the exact checks scan (0 .. RVP_BINS-2 keys, then more).    */
+#define RVP_BINS 50
+#define RVP_CAND 0
+#define RVP_HA   1
+#define RVP_HB   2
+#define RVP_HAB  3
+#define RVP_GEN  4
+#define RVP_HIST 5
+#define RVP_NCTR (RVP_HIST+RVP_BINS)
+__device__ unsigned long long rvp_ctr[RVP_NCTR];
+__device__ int rvp_mode;
+#define RVP_MODE rvp_mode
+#define RVP_COUNT(i,v) { if (rvp_mode == 3) atomicAdd(rvp_ctr+(i),(unsigned long long) (v)); }
+#define RVP_BUCKET(sz) RVP_COUNT(RVP_HIST + ((sz) < RVP_BINS-1 ? (int) (sz) : RVP_BINS-1),1)
+
+/* ctr != NULL: the counts since the last call into ctr[RVP_NCTR]; then clear them and set the mode */
+extern "C" int hm_probe_resolve(int mode, unsigned long long *ctr)
+{ static unsigned long long rows[RVP_NCTR];
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess && ctr != NULL)
+    { e = cudaMemcpyFromSymbol(rows,rvp_ctr,sizeof(rows));
+      memcpy(ctr,rows,sizeof(rows));
+    }
+  memset(rows,0,sizeof(rows));
+  if (e == cudaSuccess)
+    e = cudaMemcpyToSymbol(rvp_ctr,rows,sizeof(rows));
+  if (e == cudaSuccess)
+    e = cudaMemcpyToSymbol(rvp_mode,&mode,sizeof(mode));
+  return e == cudaSuccess ? HM_OK : hm_cuda_fail(e,"hm_probe_resolve");
+}
+#else
+#define RVP_MODE 0
+#define RVP_COUNT(i,v)
+#define RVP_BUCKET(sz)
+#endif
+
 /* q's bucket [l,r) holds q's whole run (the bucket prefix is no longer than the run prefix): is q there
- * (found), and has it a partner at a position >= pup with a count sum <= HM_SMAX?  RV_PROBE keys and
- * counts are loaded at once.                                                                          */
+ * (found), and has it a partner at a position >= pup with a count sum <= HM_SMAX?  RV_PROBE keys (first
+ * words) are loaded at once.  The check reads sectors at random from the table, and it is bound by how many
+ * it reads, not by latency: so the second key word is read only for a key in q's run, and a count only for
+ * an actual partner of q (on the bench table that takes the counts' sector -- a quarter of what the check
+ * read -- out of nearly every check).                                                                  */
 template <int KW>
 __device__ __forceinline__ bool bucket_upper_partner(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
                                                      const uint16_t *__restrict__ cnt, int64_t l, int64_t r,
@@ -1331,22 +1375,19 @@ __device__ __forceinline__ bool bucket_upper_partner(const uint64_t *__restrict_
 { bool hit = false;
   found = false;
   for (int64_t i0 = l; i0 < r; i0 += RV_PROBE)
-    { uint64_t z[RV_PROBE], zl[RV_PROBE];
-      int      c[RV_PROBE];
+    { uint64_t z[RV_PROBE];
 #pragma unroll
       for (int u = 0; u < RV_PROBE; u++)
-        { const bool in = (i0+u < r);
-          z[u]  = in ? __ldg(keys+i0+u) : ~q;                 /* ~q: another run */
-          zl[u] = (KW == 2 && in) ? __ldg(keys_lo+i0+u) : 0;
-          c[u]  = in ? (int) __ldg(cnt+i0+u) : 0;
-        }
+        z[u] = (i0+u < r) ? __ldg(keys+i0+u) : ~q;             /* ~q: another run */
 #pragma unroll
       for (int u = 0; u < RV_PROBE; u++)
-        { int pos;
-          if (z[u] == q && (KW == 1 || zl[u] == ql))
+        { if (((z[u] ^ q) >> psh) != 0)                        /* another run: neither q nor a partner */
+            continue;
+          const uint64_t zl = KW == 2 ? __ldg(keys_lo+i0+u) : 0;
+          int pos;
+          if (z[u] == q && (KW == 1 || zl == ql))
             found = true;
-          else if (((z[u] ^ q) >> psh) == 0 && one_base_apart<KW>(q,ql,z[u],zl[u],pos) && pos >= pup &&
-                   cq + c[u] <= HM_SMAX)
+          else if (one_base_apart<KW>(q,ql,z[u],zl,pos) && pos >= pup && cq + (int) __ldg(cnt+i0+u) <= HM_SMAX)
             hit = true;
         }
     }
@@ -1493,6 +1534,8 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
     { int64_t la = 0, ra = 0, lb = 0, rb = 0;
       if (ha) { const uint64_t bk = rx >> bshift; la = (int64_t) bucket[bk]; ra = (int64_t) bucket[bk+1]; }
       if (hb) { const uint64_t bk = ry >> bshift; lb = (int64_t) bucket[bk]; rb = (int64_t) bucket[bk+1]; }
+      if (ha) RVP_BUCKET(ra-la);
+      if (hb) RVP_BUCKET(rb-lb);
       if (ra-la <= 48 && rb-lb <= 48)
         { bool found;
           if (ha)
@@ -1512,6 +1555,7 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
           return true;
         }
     }
+  RVP_COUNT(RVP_GEN,1)
   if (ha && has_upper_partner<IdxT,KW>(keys,keys_lo,cnt,n,bucket,bshift,kmer,rx,rxl,cx,W.status))
     return false;
   if (hb && has_upper_partner<IdxT,KW>(keys,keys_lo,cnt,n,bucket,bshift,kmer,ry,ryl,cy,W.status))
@@ -1674,6 +1718,14 @@ __device__ __forceinline__ void sweep(const uint64_t *__restrict__ keys, const u
               meta[u] = ld_stream(W.cand_meta+i);
             }
         }
+#ifdef RESOLVE_PROBE
+      if (RVP_MODE == 1)
+        { uint64_t d = 0;
+          for (int u = 0; u < RV_ILP; u++) d ^= x[u] ^ xl[u] ^ meta[u];
+          if (d == 0x5eedull) atomicOr(W.status,0ull);            /* keeps the loads */
+          continue;
+        }
+#endif
 #pragma unroll
       for (int u = 0; u < RV_ILP; u++)
         { const int p  = (int) ((meta[u] >> 32) & 0xff), yb = (int) ((meta[u] >> 40) & 3);
@@ -1695,8 +1747,10 @@ __device__ __forceinline__ void sweep(const uint64_t *__restrict__ keys, const u
 #pragma unroll
       for (int u = 0; u < RV_ILP; u++)
         { const bool ha = (va[u] & ba[u]) == ba[u], hb = (vb[u] & bb[u]) == bb[u];
-          const bool hit = ok[u] && (ha || hb);
+          bool hit = ok[u] && (ha || hb);
+          RVP_COUNT(RVP_CAND,ok[u]) RVP_COUNT(RVP_HA,hit && !hb) RVP_COUNT(RVP_HB,hit && !ha) RVP_COUNT(RVP_HAB,hit && ha && hb)
           sink.take(ok[u] && !hit,x[u],xl[u],meta[u]);
+          if (RVP_MODE == 2) hit = false;                        /* not isolated, not checked */
           const unsigned bal = __ballot_sync(FULL,hit);
           if (hit)
             { const int at = qn + __popc(bal & lt);
@@ -1731,6 +1785,15 @@ __device__ __forceinline__ void sweep(const uint64_t *__restrict__ keys, const u
   sink.end();
 }
 
+/* pass 2's grid: `want` CTAs, at most `most`; HETMERS_PASS2_CTAS=g caps it at g (each CTA then strides over more
+ * candidates: tests) */
+static int rv_grid(int64_t want, int64_t most)
+{ const char *e = getenv("HETMERS_PASS2_CTAS");
+  if (e != NULL && atoi(e) >= 1 && atoi(e) < most)
+    most = atoi(e);
+  return (int) (want < most ? (want > 0 ? want : 1) : most);
+}
+
 /* Pass 2 of the plot: sweep with the count sink.  One CTA of 1024 threads per SM: one plot tile per SM, the rest of
  * shared memory holds the queues.                                                                             */
 template <typename IdxT, int KW, Lookup LK>
@@ -1757,7 +1820,7 @@ static cudaError_t launch_resolve(const uint64_t *keys, const uint64_t *keys_lo,
     }
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = (range/8+RV_THREADS-1)/RV_THREADS;            /* ~1 candidate per 10 entries */
-  int     grid = (int) (want < sms ? (want > 0 ? want : 1) : sms);
+  int     grid = rv_grid(want,sms);
   resolve_kernel<IdxT,KW,LK><<<grid,RV_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,plot);
   return cudaGetLastError();
 }
@@ -1822,7 +1885,7 @@ static cudaError_t launch_extract(const uint64_t *keys, const uint64_t *keys_lo,
     occ = per_sm[dev];
   cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
   int64_t want = ((int64_t) W.cand_cap+EX_THREADS*RV_ILP-1)/(EX_THREADS*RV_ILP);
-  int     grid = (int) (want < sms*occ ? (want > 0 ? want : 1) : sms*occ);
+  int     grid = rv_grid(want,(int64_t) sms*occ);
   extract_kernel<IdxT,KW,LK><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,W,
                                                           pixmap,out,(unsigned long long) cap,count);
   return cudaGetLastError();
