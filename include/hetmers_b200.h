@@ -469,6 +469,48 @@ int hm_condition_plan(int64_t n, int kmer, int ibyte, int64_t budget, int do_sym
 int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
                             hm_condition_stats *st);
 
+/* ---- conditioning across the ranks of a one-process-per-GPU job (csrc/hm_shard_condition.cu, DESIGN.md §4e) ----
+ * Each rank holds a sorted share of the source (m entries; d_keys_lo only for k > 32) and the caller runs the
+ * collectives between the calls (smudgeplot_b200/dist.py, ShardedScan.from_ktab(L=...)):
+ *   cond_hist (one uint64 per key prefix, HM_COND_HIST_BITS bits of the first word or 2k if fewer; zeroed by the
+ *   caller) -> histograms summed over the ranks -> the prefixes cut into one contiguous range per rank -> d_dest
+ *   (int16 per prefix: the rank that owns it) -> route_count -> route_scatter -> the send buffer's two regions
+ *   all-to-all'ed -> settle (when symmetrising) -> the ranks' shares concatenated in rank order.
+ * ethresh: entries with count >= ethresh are kept (0 keeps all); do_symm: add every kept k-mer's reverse
+ * complement with its count.  The results are those of hm_scan_condition, the original winning over an equal
+ * reverse complement.                                                                                        */
+int hm_k_cond_hist(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m, int kmer,
+                   int ethresh, int do_symm, uint64_t *d_hist, void *stream);
+/* d_counts: uint64[2*world + 2], zeroed by the caller -> [d]: kept originals bound for rank d, [world+d]: reverse
+ * complements bound for rank d, [2*world]: all kept originals.  d_tiles: uint64[m/256 + 2] -> the kept
+ * originals' offsets per tile of 256 entries, read by route_scatter.                                          */
+int hm_k_shard_route_count(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m,
+                           int kmer, int ethresh, int do_symm, const int16_t *d_dest, int world, uint64_t *d_counts,
+                           uint64_t *d_tiles, void *stream);
+/* the send buffer (n_orig + n_rc entries): [0, n_orig) the kept originals in source order (rank d's are the
+ * slice after those of ranks below d), then from n_orig the reverse complements, rank d's segment starting at
+ * d_cursor[d] (uint64[world], preset by the caller, advanced here; any order inside a segment).  *d_flag
+ * (zeroed by the caller) becomes non-zero if an entry found no room.                                          */
+int hm_k_shard_route_scatter(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m,
+                             int kmer, int ethresh, int do_symm, const int16_t *d_dest, const uint64_t *d_tiles,
+                             uint64_t *d_send_key, uint64_t *d_send_lo, uint16_t *d_send_cnt, int64_t n_orig,
+                             int64_t n_rc, uint64_t *d_cursor, uint64_t *d_flag, void *stream);
+/* received region: [0, n_orig) sorted originals, [n_orig, n_orig + n_rc) reverse complements in any order
+ * (both are reordered here) -> d_out_* (room for n_orig + n_rc): the rank's conditioned share, *n_out entries
+ * (synchronises the stream).  Scratch: hm_k_shard_settle_bytes(kmer, n_orig + n_rc, n_rc) bytes.  k > 32:
+ * HM_EUNSUPPORTED from 2^32 - 16 reverse complements on (the sort carries a 32-bit permutation).           */
+int64_t hm_k_shard_settle_bytes(int kmer, int64_t t, int64_t c);
+int hm_k_shard_settle(int kmer, uint64_t *d_key, uint64_t *d_lo, uint16_t *d_cnt, int64_t n_orig, int64_t n_rc,
+                      void *d_scratch, int64_t scratch_bytes, uint64_t *d_out_key, uint64_t *d_out_lo,
+                      uint16_t *d_out_cnt, int64_t *n_out, void *stream);
+/* the most device bytes one rank's conditioning holds (its arrays rounded to 512 bytes, plus 1 MiB for small
+ * tensors): a share of `share` source entries unpacked (+ its records and the stub index of 2^(8 ibyte)
+ * entries), routed into `sent` entries, `received` entries of which rc_received are reverse complements,
+ * settled, and the replica of total_out entries gathered beside the rank's conditioned share; -1 on bad
+ * arguments                                                                                                */
+int64_t hm_shard_condition_bytes(int kmer, int ibyte, int world, int64_t share, int64_t sent, int64_t received,
+                                 int64_t rc_received, int64_t total_out, int do_symm);
+
 /* one call: create + run + destroy (what bench.py's e2e leg times) */
 int  hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,
                      int64_t *plot, hm_scan_stats *stats);

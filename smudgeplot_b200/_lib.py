@@ -34,6 +34,8 @@ ABI_SYMBOLS = [
     "hm_condition_range_bytes", "hm_condition_plan", "hm_scan_condition_files",
     "hm_table_write_open", "hm_table_write_buckets", "hm_table_write_append", "hm_table_write_close",
     "hm_table_write_abort",
+    "hm_k_cond_hist", "hm_k_shard_route_count", "hm_k_shard_route_scatter", "hm_k_shard_settle_bytes",
+    "hm_k_shard_settle", "hm_shard_condition_bytes",
 ]
 
 
@@ -224,6 +226,14 @@ def lib():
     L.hm_table_write_close.argtypes = [vp]
     L.hm_table_write_abort.argtypes = [vp]
     L.hm_table_write_abort.restype = None
+    L.hm_k_cond_hist.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp]
+    L.hm_k_shard_route_count.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, i32, vp, vp, vp]
+    L.hm_k_shard_route_scatter.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]
+    L.hm_k_shard_settle_bytes.argtypes = [i32, i64, i64]
+    L.hm_k_shard_settle_bytes.restype = i64
+    L.hm_k_shard_settle.argtypes = [i32, vp, vp, vp, i64, i64, vp, i64, vp, vp, vp, C.POINTER(i64), vp]
+    L.hm_shard_condition_bytes.argtypes = [i32, i32, i32, i64, i64, i64, i64, i64, i32]
+    L.hm_shard_condition_bytes.restype = i64
     _lib = L
     return L
 

@@ -444,6 +444,20 @@ static int merge_ranked(const hm_cond_bufs *B, int64_t o, const uint64_t *rk, co
   return HM_OK;
 }
 
+/* the steps above for the key-range conditioning of a one-process-per-GPU job (hm_shard_condition.cu) */
+int hm_cond_scan_tiles(unsigned long long *tiles, int64_t nt, unsigned long long *base, cudaStream_t st)
+{ cond_scan_kernel<<<1,1024,0,st>>>(tiles,nt,base);
+  LAUNCHED("cond_scan_kernel");
+  return HM_OK;
+}
+
+int hm_cond_sort_rc(const hm_cond_bufs *B, int64_t c, uint64_t **pk, uint64_t **pl, uint16_t **pc, cudaStream_t st)
+{ return sort_rc(B,c,pk,pl,pc,st); }
+
+int hm_cond_merge(const hm_cond_bufs *B, int64_t o, const uint64_t *rk, const uint64_t *rl, const uint16_t *rc_,
+                  int64_t c, cudaStream_t st)
+{ return B->kmer > 32 ? merge_ranked<2>(B,o,rk,rl,rc_,c,st) : merge_ranked<1>(B,o,rk,rl,rc_,c,st); }
+
 /* the range gathered in B -> FastK records in B->rec and the counts of stub buckets [b0, b0+nb) in B->bcount;
  * *n_out: its entries.  Synchronises st.                                                                  */
 int hm_cond_finish(const hm_cond_bufs *B, uint64_t b0, int64_t nb, int64_t *n_out, cudaStream_t st)

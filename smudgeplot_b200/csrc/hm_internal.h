@@ -131,7 +131,14 @@ int hm_cond_finish(const hm_cond_bufs *B, uint64_t b0, int64_t nb, int64_t *n_ou
 int64_t hm_cond_chunk(int64_t n, int kmer, int ibyte, int64_t budget);
 int64_t hm_cond_tiles_bytes(int64_t n);
 int64_t hm_cond_sort_room(int64_t c);
-#define HM_CUDA(call)                                              \
+/* the same steps over caller-placed buffers (hm_shard_condition.cu): tile counts -> exclusive offsets (+ *base;
+ * *base += total); the c reverse complements at the end of B's region sorted (*pk / *pl / *pc: where they are
+ * now); the o originals at its front merged with them into B->m_* (ctr[5]: reverse complements dropped)      */
+int hm_cond_scan_tiles(unsigned long long *tiles, int64_t nt, unsigned long long *base, cudaStream_t st);
+int hm_cond_sort_rc(const hm_cond_bufs *B, int64_t c, uint64_t **pk, uint64_t **pl, uint16_t **pc, cudaStream_t st);
+int hm_cond_merge(const hm_cond_bufs *B, int64_t o, const uint64_t *rk, const uint64_t *rl, const uint16_t *rc_,
+                  int64_t c, cudaStream_t st);
+#define HM_CUDA(call)                                             \
   do { cudaError_t _e = (call);                                    \
        if (_e != cudaSuccess) return hm_cuda_fail(_e,#call);       \
      } while (0)

@@ -149,7 +149,7 @@ class DeviceTable:
         for r, c in enumerate(cuts):
             sh.off[r] = c
         idx = torch.tensor([min(c, self.n - 1) for c in cuts[1:-1]], dtype=torch.int64, device=self.device)
-        first = self.keys[idx].tolist() if idx.numel() else []
+        first = self.keys[idx].tolist() if idx.numel() and self.n else [0] * idx.numel()   # (an empty table: no keys)
         for r, (c, v) in enumerate(zip(cuts[1:-1], first), start=1):
             sh.first_key[r] = (v & 0xFFFFFFFFFFFFFFFF) if c < self.n else 0xFFFFFFFFFFFFFFFF
         return sh

@@ -412,28 +412,27 @@ class ShardedScan:
         return cls(k, kf, cf, lo, hi, group)
 
     @classmethod
-    def from_ktab(cls, name, group=None, device=None, path="auto"):
+    def from_ktab(cls, name, group=None, device=None, path="auto", L=None, budget=None):
         """the FastK table `name` (stub + part files): rank r reads the records of ordinals [n*r/W, n*(r+1)/W)
         (a range may span part files), unpacks them on its GPU with the table's own ibyte, and the shares are
-        all-gathered into the replica every rank holds (gather_table; on gloo the shares meet in host memory)"""
+        all-gathered into the replica every rank holds (gather_table; on gloo the shares meet in host memory).
+        With L (hetmers' -e) the table is first trimmed and / or symmetrised as hm_scan_examine(L) decides on the
+        whole table, across the ranks (_from_ktab_conditioned, DESIGN.md §4e): the replica is what
+        hetmers.Scan(kt).condition(L, not trimmed, not symmetric) + download() give in one process.  budget: device
+        bytes per rank for that conditioning (default: free memory minus _lib.BUDGET_RESERVE)."""
         import numpy as np
         from . import fastk
         from .device import DeviceTable
+        if L is not None:
+            return cls._from_ktab_conditioned(name, group, device, path, int(L), budget)
         world, rank = dist.get_world_size(group), dist.get_rank(group)
         dev = torch.device(device if device is not None else "cuda")
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         kt = fastk.read_ktab(str(name), mmap=True)
-        k, n, pb = kt.kmer, kt.nels, kt.pbyte
+        k, n = kt.kmer, kt.nels
         lo, hi = (n * rank) // world, (n * (rank + 1)) // world
-        rec = np.empty((hi - lo) * pb, dtype=np.uint8)
-        at = start = 0
-        for p, pn in enumerate(kt.part_nels):                  # the share's records, part by part
-            a, b = max(lo, start), min(hi, start + pn)
-            if a < b:
-                rec[at:at + (b - a) * pb] = kt.records[p][(a - start) * pb:(b - start) * pb]
-                at += (b - a) * pb
-            start += pn
+        rec = _share_records(kt, lo, hi)
         with torch.cuda.device(dev):
             room = n + world                                   # room for gather_table's even chunks
             kb = torch.empty(room, dtype=torch.int64, device=dev)
@@ -457,6 +456,90 @@ class ShardedScan:
                     lb[:n].copy_(got[4])
             assert (got[2], got[3]) == (lo, hi)
             return cls(k, kb[:n], cb[:n], lo, hi, group, keys_lo_full=lb[:n] if lb is not None else None, path=path)
+
+    @classmethod
+    def _from_ktab_conditioned(cls, name, group, device, path, ethresh, budget):
+        """from_ktab(L=ethresh): rank r loads its share of the source, the ranks decide "trimmed?" / "symmetric?"
+        together (job_examine), and unless the table needs neither step every rank routes its kept entries (and
+        their reverse complements) to the rank that owns their key prefix, which settles what it receives into its
+        conditioned share (hm_k_shard_*); the shares are all-gathered into the replica.  The working set of every
+        rank is checked against its budget once the summed histogram gives the counts, before any entry moves:
+        HM_ENOMEM (or HM_EUNSUPPORTED, k > 32 and 2^32 - 16 reverse complements or more on one rank) on every
+        rank, with the sizes.  stats["condition"]: verdicts, steps, entries in / out, entries sent to / received
+        from each rank, peak device bytes of the call (torch's allocator; its peak statistics are reset), the
+        working set and budget, and ms per phase on this rank."""
+        import numpy as np
+        from . import _lib, fastk
+        from .device import DeviceTable, _ptr, _stream
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        dev = torch.device(device if device is not None else "cuda")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        coll = dev if _nccl(group) else torch.device("cpu")
+        Lb = _lib.lib()
+        ms = {}
+        lap = _lapper(ms)
+
+        def done(phase, t):                                    # the phase's kernels have finished
+            torch.cuda.synchronize(dev)
+            return lap(phase, t)
+
+        with torch.cuda.device(dev):
+            if budget is None:
+                budget = torch.cuda.mem_get_info(dev)[0] - _lib.BUDGET_RESERVE
+            torch.cuda.reset_peak_memory_stats(dev)
+            base = torch.cuda.memory_allocated(dev)
+            t = time.perf_counter()
+            kt = fastk.read_ktab(str(name), mmap=True)
+            k, n, ibyte = kt.kmer, kt.nels, kt.ibyte
+            two = k > 32
+            lo, hi = share_range(n, world, rank)
+            m = hi - lo
+            if m:
+                d_rec = torch.from_numpy(_share_records(kt, lo, hi)).to(dev)
+                d_idx = torch.from_numpy(np.ascontiguousarray(kt.index, dtype=np.int64)).to(dev)
+                src = DeviceTable.from_records(k, ibyte, d_rec, d_idx, first=lo)
+                sk, sc, sl = src.keys, src.cnt, src.keys_lo
+                del d_rec, d_idx, src
+            else:
+                sk = torch.empty(0, dtype=torch.int64, device=dev)
+                sc = torch.empty(0, dtype=torch.int16, device=dev)
+                sl = torch.empty(0, dtype=torch.int64, device=dev) if two else None
+            del kt
+            t = done("load", t)
+
+            def share_min(a, b):
+                out = torch.full((1,), 0x8000, dtype=torch.int32, device=dev)
+                _lib.check(Lb.hm_k_min_count(_ptr(sc), a, b, _ptr(out), _stream()))
+                return int(out.item())
+
+            trimmed, symmetric = job_examine(ethresh, k, n, sk, sl, share_min, group, coll)
+            do_trim, do_symm = not trimmed, not symmetric
+            t = lap("examine", t)
+            st = {"trimmed": trimmed, "symmetric": symmetric,
+                  "steps": (["trim"] if do_trim else []) + (["symmetrise"] if do_symm else []),
+                  "entries_in": n, "sent": [0] * world, "received": [0] * world, "budget": budget,
+                  "working_set_bytes": 0}
+            if do_trim or do_symm:
+                share = [sk, sc, sl]                           # handed over: a refusal frees it before it raises
+                del sk, sc, sl
+                sk, sc, sl = _condition_share(k, ibyte, m, share, ethresh if do_trim else 0, do_symm, budget, group,
+                                              coll, st, done, t)
+                t = time.perf_counter()
+            if _nccl(group):
+                got = gather_table(sk, sc, group, local_lo=sl)
+            else:
+                got = gather_table(sk.cpu(), sc.cpu(), group, local_lo=sl.cpu() if two else None)
+                got = [g.to(dev) if isinstance(g, torch.Tensor) else g for g in got]
+            del sk, sc, sl
+            done("gather", t)
+            st["peak_bytes"] = torch.cuda.max_memory_allocated(dev) - base
+        kf, cf, olo, ohi = got[:4]
+        st["entries_out"] = kf.numel()
+        st["ms"] = ms
+        out = cls(k, kf, cf, olo, ohi, group, keys_lo_full=got[4] if two else None, path=path)
+        out.stats["condition"] = st
+        return out
 
     def close(self):
         if self.peer is not None:
@@ -647,7 +730,8 @@ class ShardedScan:
             if not symm and self.world > 1:                     # nobody clears what a peer still reads
                 _in_place(lambda x: dist.all_reduce(x, group=g), self._barrier_t, g)
             self.stats = {"route": self.path, "scan_reused": reused, "slices": len(ranges), "records": len(recs),
-                          "buffer_records": cap, "budget": budget, "range": [t.lo, t.hi]}
+                          "buffer_records": cap, "budget": budget, "range": [t.lo, t.hi],
+                          **{key: v for key, v in self.stats.items() if key == "condition"}}
             res = gather_pairs(recs, dst, g)
             lap("gather_and_sort", t0)
         return res
@@ -785,6 +869,253 @@ def file_run_aligned_cuts(kt, world: int, window: int = 4096):
             c += w.size
         cuts.append(at)
     return cuts + [n]
+
+
+# ---- trimming and symmetrising across the ranks (ShardedScan.from_ktab(L=...), DESIGN.md §4e) ---------------------
+
+_U64 = (1 << 64) - 1
+
+
+def share_range(n: int, world: int, rank: int):
+    """the source ordinals rank `rank` of `world` loads: [n*rank/world, n*(rank+1)/world)"""
+    return (n * rank) // world, (n * (rank + 1)) // world
+
+
+def examine_window(n: int):
+    """the ordinals whose counts decide "trimmed?" in hm_scan_examine: all of them when n + 3 < 1e8, else the 1e8
+    around the middle -> (frst, last).  For n = 1e8 - 3 .. 1e8 - 1 that rule's window reaches 1 or 2 entries beyond
+    the table at either end; here it is clipped to the table."""
+    if n + 3 < 100_000_000:
+        return 0, n
+    return max(n // 2 - 50_000_000, 0), min(n // 2 + 50_000_000, n)
+
+
+def condition_cuts(hist, world: int):
+    """Cut the key prefixes into `world` contiguous ranges of near-equal output count, on prefix boundaries; hist:
+    output entries per prefix (the same summed histogram on every rank, so every rank computes the same cuts).
+    Cut r is the prefix boundary nearest to r/world of the total (the lower one on a tie), so a range is off its
+    share by at most one prefix's count; ranges may be empty (one prefix may hold most of the table).
+    -> [0, c_1, ..., c_{world-1}, len(hist)], rank d owning prefixes [c_d, c_{d+1})"""
+    import numpy as np
+    h = np.asarray(hist, dtype=np.int64)
+    np_ = h.size
+    before = np.zeros(np_ + 1, dtype=np.int64)                 # before[p]: entries under prefixes below p
+    np.cumsum(h, out=before[1:])
+    total = int(before[-1])
+    cuts = [0]
+    for r in range(1, world):
+        want = (total * r) // world
+        p = int(np.searchsorted(before, want, side="right")) - 1
+        if p < np_ and before[p + 1] - want < want - before[p]:
+            p += 1
+        cuts.append(max(p, cuts[-1]))
+    return cuts + [np_]
+
+
+def _signed(v: int) -> int:
+    return v - (1 << 64) if v >= (1 << 63) else v
+
+
+def _revcomp_words(x0: int, x1: int, k: int):
+    """reverse complement of a left-aligned packed k-mer (unsigned words; x1: bases 32.. for k > 32) -> (w0, w1)"""
+    bits = 128 if k > 32 else 64
+    v = ((x0 << 64) | x1 if k > 32 else x0) >> (bits - 2 * k)
+    r = 0
+    for _ in range(k):
+        r = (r << 2) | (3 - (v & 3))
+        v >>= 2
+    r <<= bits - 2 * k
+    return (r >> 64, r & _U64) if k > 32 else (r, 0)
+
+
+def _u64_bounds(keys: torch.Tensor, q: int, lo: int, hi: int):
+    """[a, b): the entries of keys[lo:hi] equal to the unsigned value q.  keys are sorted as unsigned numbers but
+    held as int64, which torch compares signed: the entries below 2^63 come first, then those at or above (negative
+    as int64), each part sorted in signed order too; q is searched in its part"""
+    a, b = lo, hi
+    while a < b:                                               # the first entry at or above 2^63
+        mid = (a + b) // 2
+        if int(keys[mid]) >= 0:
+            a = mid + 1
+        else:
+            b = mid
+    qs = _signed(q)
+    p0, p1 = (lo, a) if qs >= 0 else (a, hi)
+    if p0 >= p1:
+        return p0, p0
+    part, v = keys[p0:p1], torch.tensor([qs], dtype=torch.int64, device=keys.device)
+    return p0 + int(torch.searchsorted(part, v)), p0 + int(torch.searchsorted(part, v, right=True))
+
+
+def _share_find(keys: torch.Tensor, keys_lo, q0: int, q1: int) -> int:
+    """index of the k-mer (q0, q1) in a sorted share (keys_lo: second words, k > 32), or -1"""
+    a, b = _u64_bounds(keys, q0, 0, keys.numel())
+    if keys_lo is not None and a < b:
+        a, b = _u64_bounds(keys_lo, q1, a, b)
+    return a if a < b else -1
+
+
+def job_examine(ethresh: int, kmer: int, n: int, keys: torch.Tensor, keys_lo, min_count, group=None,
+                coll_dev=None):
+    """hm_scan_examine's decisions on a table of n entries whose ranks hold the shares of share_range: keys /
+    keys_lo (k > 32) this rank's sorted share; min_count(a, b) the smallest count >= 1 (read as int16) among its
+    entries [a, b), 0x8000 if none.  trim: the MIN over the ranks of min_count over their parts of examine_window(n)
+    is >= ethresh.  symm: from sidx = 1, the owner of entry sidx broadcasts the reverse complement of its key, every
+    rank looks it up in its share, and a MAX all-reduce gives its position or -1: -1 = not symmetric, another
+    position = symmetric, sidx itself (a palindrome) = go on with sidx + 1; n <= 1 counts as symmetric.
+    -> (trimmed?, symmetric?) on every rank"""
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    lo, hi = share_range(n, world, rank)
+    frst, last = examine_window(n)
+    a, b = max(lo, frst), min(hi, last)
+    low = torch.tensor([min_count(a - lo, b - lo) if a < b else 0x8000], dtype=torch.int64, device=coll_dev)
+    dist.all_reduce(low, op=dist.ReduceOp.MIN, group=group)
+    trimmed = int(low.item()) >= ethresh
+    symmetric = True
+    owner = lambda i: next(r for r in range(world) if share_range(n, world, r)[1] > i)   # noqa: E731
+    sidx = 1
+    while sidx < n:
+        src = owner(sidx)
+        q = torch.zeros(2, dtype=torch.int64, device=coll_dev)
+        if rank == src:
+            x1 = int(keys_lo[sidx - lo]) & _U64 if keys_lo is not None else 0
+            r0, r1 = _revcomp_words(int(keys[sidx - lo]) & _U64, x1, kmer)
+            q[0], q[1] = _signed(r0), _signed(r1)
+        dist.broadcast(q, src=dist.get_global_rank(group, src) if group is not None else src, group=group)
+        i = _share_find(keys, keys_lo, int(q[0]) & _U64, int(q[1]) & _U64)
+        pos = torch.tensor([lo + i if i >= 0 else -1], dtype=torch.int64, device=coll_dev)
+        dist.all_reduce(pos, op=dist.ReduceOp.MAX, group=group)
+        p = int(pos.item())
+        if p < 0:
+            symmetric = False
+            break
+        if p != sidx:
+            break
+        sidx += 1
+    return trimmed, symmetric
+
+
+def _condition_share(k, ibyte, m, share, ethr, do_symm, budget, group, coll, st, done, t):
+    """the conditioning steps of ShardedScan._from_ktab_conditioned on this rank's source share (share: [keys,
+    counts, second words or None] of m entries, emptied here so that the share is freed as soon as it has been
+    routed, or refused) -> this rank's conditioned share (keys, counts, second words or None)"""
+    import ctypes as C
+    import numpy as np
+    from . import _lib
+    from .device import _ptr, _stream
+    Lb = _lib.lib()
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    sk, sc, sl = share
+    share.clear()
+    dev, two = sk.device, k > 32
+    # histograms of this share: kept originals, and kept originals + reverse complements, per key prefix
+    hist = torch.zeros((2, 1 << min(_lib.COND_HIST_BITS, 2 * k)), dtype=torch.int64, device=dev)
+    for row, symm in ((0, 0), (1, do_symm)):
+        _lib.check(Lb.hm_k_cond_hist(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, symm, _ptr(hist[row]), _stream()))
+    sent = int(hist[1].sum())
+    _in_place(lambda x: dist.all_reduce(x, group=group), hist, group)
+    h = hist.cpu().numpy()
+    del hist
+    cuts = condition_cuts(h[1], world)
+    at_all = np.concatenate([[0], np.cumsum(h[1])])[cuts]
+    at_orig = np.concatenate([[0], np.cumsum(h[0])])[cuts]
+    recv = np.diff(at_all).tolist()
+    recv_rc = (np.diff(at_all) - np.diff(at_orig)).tolist()
+    total_orig, total = int(h[0].sum()), int(h[1].sum())
+    need = Lb.hm_shard_condition_bytes(k, ibyte, world, m, sent, recv[rank], recv_rc[rank], total, int(do_symm))
+    sizes = torch.zeros((world, 2), dtype=torch.int64, device=coll)
+    sizes[rank, 0], sizes[rank, 1] = need, budget
+    dist.all_reduce(sizes, group=group)
+    needs, budgets = sizes[:, 0].tolist(), sizes[:, 1].tolist()
+    st.update(working_set_bytes=need, prefix_cuts=cuts)
+    big = [d for d in range(world) if two and do_symm and recv_rc[d] >= 0xFFFFFFF0]
+    short = [d for d in range(world) if needs[d] > budgets[d]]
+    if big or short:
+        del sk, sc, sl
+        if big:
+            raise _lib.HetmersError(-6, f"rank {rank}: conditioning across {world} ranks would send ranks {big} "
+                                        f"{[recv_rc[d] for d in big]} reverse complements of k={k} to sort: 2^32 - 16 "
+                                        f"or more needs 64-bit sort indices")
+        raise _lib.HetmersError(-3, f"rank {rank}: conditioning across {world} ranks needs {needs} device bytes per "
+                                    f"rank, beyond the budgets {budgets} of ranks {short}")
+    t = done("hist_and_plan", t)
+
+    # route: every kept entry (and its reverse complement) to the rank owning its key prefix
+    dest = torch.from_numpy(np.repeat(np.arange(world, dtype=np.int16), np.diff(cuts))).to(dev)
+    counts = torch.zeros(2 * world + 2, dtype=torch.int64, device=dev)
+    tiles = torch.empty(m // 256 + 2, dtype=torch.int64, device=dev)
+    _lib.check(Lb.hm_k_shard_route_count(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, int(do_symm), _ptr(dest), world,
+                                         _ptr(counts), _ptr(tiles), _stream()))
+    c = counts.tolist()
+    so, sr = c[:world], c[world:2 * world]
+    n_o, n_r = sum(so), sum(sr)
+    assert n_o + n_r == sent and c[2 * world] == n_o, (so, sr, sent, c[2 * world])
+    send_k = torch.empty(max(n_o + n_r, 1), dtype=torch.int64, device=dev)
+    send_c = torch.empty(max(n_o + n_r, 1), dtype=torch.int16, device=dev)
+    send_l = torch.empty(max(n_o + n_r, 1), dtype=torch.int64, device=dev) if two else None
+    cursor = torch.tensor(np.concatenate([[0], np.cumsum(sr)[:-1]]).astype(np.int64), device=dev)
+    _lib.check(Lb.hm_k_shard_route_scatter(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, int(do_symm), _ptr(dest),
+                                           _ptr(tiles), _ptr(send_k), _ptr(send_l), _ptr(send_c), n_o, n_r,
+                                           _ptr(cursor), _ptr(counts[2 * world + 1:]), _stream()))
+    del sk, sc, sl, tiles, dest, cursor
+    flag = counts[2 * world + 1:].to(coll)
+    dist.all_reduce(flag, op=dist.ReduceOp.MAX, group=group)
+    if int(flag.item()):
+        raise _lib.HetmersError(-2, f"rank {rank}: routing the conditioned entries overran the send buffer on a rank")
+    t = done("route", t)
+
+    # exchange: the originals' region and the reverse complements' region, each all-to-all'ed
+    mine = torch.tensor([so, sr], dtype=torch.int64).t().contiguous().to(coll)
+    theirs = torch.empty_like(mine)
+    dist.all_to_all_single(theirs, mine, group=group)
+    ro, rr = theirs[:, 0].tolist(), theirs[:, 1].tolist()
+    r_o, r_c = sum(ro), sum(rr)
+    assert r_o + r_c == recv[rank] and r_c == recv_rc[rank], (ro, rr, recv[rank], recv_rc[rank])
+    room = max(r_o + r_c, 1)
+    rk = torch.empty(room, dtype=torch.int64, device=dev)
+    rc = torch.empty(room, dtype=torch.int16, device=dev)
+    rl = torch.empty(room, dtype=torch.int64, device=dev) if two else None
+    for (a, b, c0, c1, ins, outs, job_total) in ((0, r_o, 0, n_o, so, ro, total_orig),
+                                                 (r_o, r_o + r_c, n_o, n_o + n_r, sr, rr, total - total_orig)):
+        if job_total == 0:
+            continue
+        _all_to_all(rk[a:b], send_k[c0:c1], outs, ins, group)
+        if two:
+            _all_to_all(rl[a:b], send_l[c0:c1], outs, ins, group)
+        _all_to_all(rc[a:b].view(torch.uint8), send_c[c0:c1].view(torch.uint8), [2 * x for x in outs],
+                    [2 * x for x in ins], group)
+    del send_k, send_c, send_l
+    t = done("exchange", t)
+    st.update(sent=[a + b for a, b in zip(so, sr)], received=[a + b for a, b in zip(ro, rr)])
+    if not do_symm:                                            # the originals arrive sorted: nothing to settle
+        return rk[:r_o], rc[:r_o], rl[:r_o] if two else None
+
+    # settle: sort the received reverse complements, merge them with the originals
+    ok, oc = torch.empty(room, dtype=torch.int64, device=dev), torch.empty(room, dtype=torch.int16, device=dev)
+    ol = torch.empty(room, dtype=torch.int64, device=dev) if two else None
+    scratch = torch.empty(Lb.hm_k_shard_settle_bytes(k, r_o + r_c, r_c), dtype=torch.uint8, device=dev)
+    n_out = C.c_int64()
+    _lib.check(Lb.hm_k_shard_settle(k, _ptr(rk), _ptr(rl), _ptr(rc), r_o, r_c, _ptr(scratch), scratch.numel(),
+                                    _ptr(ok), _ptr(ol), _ptr(oc), C.byref(n_out), _stream()))
+    del rk, rc, rl, scratch
+    done("sort_and_merge", t)
+    e = n_out.value
+    return ok[:e], oc[:e], ol[:e] if two else None
+
+
+def _share_records(kt, lo: int, hi: int):
+    """the records of ordinals [lo, hi) of a FastK table (fastk.KtabFiles; the range may span part files)"""
+    import numpy as np
+    pb = kt.pbyte
+    rec = np.empty((hi - lo) * pb, dtype=np.uint8)
+    at = start = 0
+    for p, pn in enumerate(kt.part_nels):                  # the share's records, part by part
+        a, b = max(lo, start), min(hi, start + pn)
+        if a < b:
+            rec[at:at + (b - a) * pb] = kt.records[p][(a - start) * pb:(b - start) * pb]
+            at += (b - a) * pb
+        start += pn
+    return rec
 
 
 def _nccl(group) -> bool:
