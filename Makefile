@@ -16,7 +16,7 @@ LIB    := $(LIBDIR)/libhetmers_b200.so
 BIN    := $(BINDIR)/hetmers $(BINDIR)/extract_kmer_pairs $(BINDIR)/condition_kmer_table
 
 CU_SRC := smudgeplot_b200/csrc/hm_kernels.cu smudgeplot_b200/csrc/hm_scan.cu smudgeplot_b200/csrc/hm_peer.cu \
-          smudgeplot_b200/csrc/hm_condition.cu smudgeplot_b200/csrc/hm_symm.cu smudgeplot_b200/csrc/hm_condition_files.cu \
+          smudgeplot_b200/csrc/hm_condition.cu smudgeplot_b200/csrc/hm_symm.cu \
           smudgeplot_b200/csrc/hm_shard_condition.cu
 CU_OBJ := $(patsubst smudgeplot_b200/csrc/%.cu,$(OBJDIR)/%.o,$(CU_SRC))
 C_OBJ  := $(OBJDIR)/fastk_table.o

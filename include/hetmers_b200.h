@@ -291,8 +291,15 @@ void hm_scan_destroy(hm_scan *s);
 int  hm_scan_examine(hm_scan *s, int ethresh, int *trim, int *symm);
 /* Condition the device-resident table in place: trim = drop entries with count < ethresh (what
  * `Logex '...=A[<L>-]'` does), symm = add the reverse complement of every k-mer with the same
- * count (what `Symmex` does) -- PloidyPlot.c:1381-1426 shells out to those FastK tools; here the
- * table never leaves the GPU.  *nels_out = entries afterwards.                                  */
+ * count (what `Symmex` does; the original wins where both are present) -- PloidyPlot.c:1381-1426
+ * shells out to those FastK tools; here the table never leaves the GPU.  *nels_out = entries
+ * afterwards.  Each GPU conditions its replica a key range at a time (DESIGN.md §4d) into new
+ * arrays, which replace the old ones only when the whole call succeeds; the index is rebuilt and
+ * the fingerprint verdict taken again.  The table, the new arrays and one range's working set must
+ * fit the device budget: else HM_ENOMEM before anything is touched ("... needs N device bytes (M in
+ * one range) ...": N is the least budget under which the call succeeds).  A failure on GPU 0 leaves
+ * the old table usable; on a later GPU the scan is marked unusable.  A streamed scan refuses
+ * (HM_EUNSUPPORTED).                                                                             */
 int  hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_symm, int64_t *nels_out);
 /* both passes; plot: host int64[HM_PLOT_CELLS]; stats optional.  Tables that hm_scan_create found
  * strand-symmetric (fingerprint over the whole table) take the symmetric scan of csrc/hm_symm.cu,
@@ -417,7 +424,7 @@ int  hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t
 /* sort n records in place into hm_scan_extract's order: (smudge, key, position, alternative base) */
 int  hm_sort_pair_records(hm_pair_rec *records, int64_t n);
 
-/* ---- conditioning to table files, for tables of any size (csrc/hm_condition_files.cu, DESIGN.md §4d) ----
+/* ---- conditioning to table files, for tables of any size (csrc/hm_condition.cu, DESIGN.md §4d) ----
  * hm_scan_condition_files writes what hm_scan_condition + hm_scan_download would give -- the source's entries
  * with count >= ethresh (do_trim), plus every kept k-mer's reverse complement with the same count (do_symm),
  * sorted, the original winning where both are present -- as the FastK table `dst` (same kmer, ibyte and parts
@@ -425,7 +432,8 @@ int  hm_sort_pair_records(hm_pair_rec *records, int64_t n);
  * hm_host_table must still be valid), in or out of core alike, on dev[0], and leaves the scan as it was.  The
  * source passes through the GPU once to histogram the output by key prefix (HM_COND_HIST_BITS bits of the
  * first word), then once per key range of hm_condition_plan: each pass gathers the range's kept originals and
- * reverse complements, sorts the latter, merges, packs FastK records and hands them to a host thread that
+ * reverse complements, sorts the latter, merges (the steps hm_scan_condition takes in place), packs FastK
+ * records and hands them to a host thread that
  * writes them while the next range is gathered.  The call's own device bytes stay within what the scan's
  * resident arrays leave of the budget set with hm_set_device_budget, or without one within what is free at the
  * call minus HM_BUDGET_RESERVE.  Refused before any file is

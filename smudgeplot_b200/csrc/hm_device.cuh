@@ -66,6 +66,35 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned parity)
   while (!ok);
 }
 
+/* ---- one thread per entry, CT entries per CTA (the conditioning kernels) ---- */
+
+static constexpr int CT = 256;
+
+static inline unsigned grid(int64_t n) { return (unsigned) ((n+CT-1)/CT > 0 ? (n+CT-1)/CT : 1); }
+
+/* hist[key] += 1 for every lane with pred (lanes of a warp that share a key add once) */
+template <typename K>
+__device__ __forceinline__ void warp_count(unsigned long long *hist, bool pred, K key)
+{ const unsigned act = __ballot_sync(0xffffffffu,pred);
+  if (pred)
+    { const unsigned peers = __match_any_sync(act,key);
+      if ((threadIdx.x & 31) == (unsigned) (__ffs(peers)-1))
+        atomicAdd(hist+key,(unsigned long long) __popc(peers));
+    }
+}
+
+/* exclusive rank of this thread's pred among the CTA's (once per kernel: the shared counts are not reset) */
+__device__ __forceinline__ int cta_rank(bool pred)
+{ __shared__ int s_w[CT/32];
+  const int      lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned b = __ballot_sync(0xffffffffu,pred);
+  if (lane == 0) s_w[warp] = __popc(b);
+  __syncthreads();
+  int before = 0;
+  for (int w = 0; w < warp; w++) before += s_w[w];
+  return before + __popc(b & ((1u << lane)-1));
+}
+
 /* ---- packed k-mers: left aligned, base i in bits 63-2i..62-2i of word i/32 ---- */
 
 #define HM_M5 0x5555555555555555ull

@@ -104,13 +104,12 @@ int hm_cuda_fail(cudaError_t e, const char *what);
 int64_t hm_sort_keys_bytes(int64_t n, int kmer);
 int     hm_sort_keys(uint64_t *keys, uint64_t *lo, int64_t n, int kmer, void *scratch, int64_t scratch_bytes,
                      cudaStream_t st);
-/* device bytes hm_condition_arrays borrows besides the table it is given                              */
-int64_t hm_condition_bytes(int kmer, int64_t n, int do_trim, int do_symm);
-/* conditioning to files (hm_condition_files.cu, driven by hm_scan_condition_files): the device buffers of one
- * range of at most `cap` output entries.  key / lo / cnt: the region the kept originals fill from the front
- * and the reverse complements from the back; alt_*, idx: sort buffers; m_*: the merged range; rec: its
- * records; bcount: stub-bucket counts; ctr: [0] originals, [1] reverse complements, [3] overflow, [4..5]
- * merge scratch                                                                                             */
+/* conditioning, a key range at a time (hm_condition.cu; driven by hm_scan_condition and hm_scan_condition_files
+ * in hm_scan.cu and by hm_k_shard_settle): the device buffers of one range of at most `cap` output entries.
+ * key / lo / cnt: the region the kept originals fill from the front and the reverse complements from the back;
+ * alt_*, idx: sort buffers; m_*: where the settled range goes (NULL when only trimming: the region is the
+ * range); rec: its records; bcount: stub-bucket counts; ctr: [0] originals, [1] reverse complements, [3]
+ * overflow, [4..5] merge scratch                                                                             */
 typedef struct hm_cond_bufs
   { int       kmer, ibyte, hb, ethresh, do_symm;
     int64_t   cap;
@@ -123,21 +122,31 @@ typedef struct hm_cond_bufs
     int64_t   sort_bytes;
   } hm_cond_bufs;
 
+/* pass 0: hist[prefix] += kept originals (+ their reverse complements) of a chunk of m source entries */
 int hm_cond_hist(const uint64_t *keys, const uint64_t *klo, const uint16_t *cnt, int64_t m, int kmer, int ethresh,
                  int do_symm, int hb, unsigned long long *hist, cudaStream_t st);
+/* a chunk's share of the range [p0, p1) of key prefixes into B's region (tiles: hm_cond_tiles_bytes(m)) */
 int hm_cond_gather(const uint64_t *keys, const uint64_t *klo, const uint16_t *cnt, int64_t m, const hm_cond_bufs *B,
                    uint64_t p0, uint64_t p1, unsigned long long *tiles, cudaStream_t st);
-int hm_cond_finish(const hm_cond_bufs *B, uint64_t b0, int64_t nb, int64_t *n_out, cudaStream_t st);
+/* the range gathered in B settled: when symmetrising, its reverse complements sorted and merged with its
+ * originals into B->m_* (the originals copied there when it has no reverse complements); *n_out: its entries,
+ * in B->m_*, or in the region when B->m_key is NULL.  Synchronises st.                                    */
+int hm_cond_settle(const hm_cond_bufs *B, int64_t *n_out, cudaStream_t st);
+/* the settled range's n entries -> FastK records in B->rec and the counts of stub buckets [b0, b0+nb) in
+ * B->bcount.  Synchronises st.                                                                            */
+int hm_cond_pack(const hm_cond_bufs *B, int64_t n, uint64_t b0, int64_t nb, cudaStream_t st);
+/* tile counts -> exclusive offsets (+ *base; *base += total) */
+int hm_cond_scan_tiles(unsigned long long *tiles, int64_t nt, unsigned long long *base, cudaStream_t st);
 int64_t hm_cond_chunk(int64_t n, int kmer, int ibyte, int64_t budget);
 int64_t hm_cond_tiles_bytes(int64_t n);
 int64_t hm_cond_sort_room(int64_t c);
-/* the same steps over caller-placed buffers (hm_shard_condition.cu): tile counts -> exclusive offsets (+ *base;
- * *base += total); the c reverse complements at the end of B's region sorted (*pk / *pl / *pc: where they are
- * now); the o originals at its front merged with them into B->m_* (ctr[5]: reverse complements dropped)      */
-int hm_cond_scan_tiles(unsigned long long *tiles, int64_t nt, unsigned long long *base, cudaStream_t st);
-int hm_cond_sort_rc(const hm_cond_bufs *B, int64_t c, uint64_t **pk, uint64_t **pl, uint16_t **pc, cudaStream_t st);
-int hm_cond_merge(const hm_cond_bufs *B, int64_t o, const uint64_t *rk, const uint64_t *rl, const uint16_t *rc_,
-                  int64_t c, cudaStream_t st);
+/* the plan's two halves shared by the drivers: the most output entries one range may hold when a range of t
+ * needs bytes(t, do_symm, kmer, ibyte) <= room (bisection), and the greedy cuts of the 2^hb key prefixes into
+ * ranges of at most `limit` entries (cuts[0..R], R returned; *range_cap: the largest range; *big: the largest
+ * prefix -- 0 ranges when it alone exceeds the limit)                                                     */
+typedef int64_t (*hm_cond_bytes_fn)(int64_t t, int do_symm, int kmer, int ibyte);
+int64_t hm_cond_range_limit(int64_t room, hm_cond_bytes_fn bytes, int do_symm, int kmer, int ibyte);
+int     hm_cond_cut(const int64_t *hist, int hb, int64_t limit, int64_t *cuts, int64_t *range_cap, int64_t *big);
 #define HM_CUDA(call)                                             \
   do { cudaError_t _e = (call);                                    \
        if (_e != cudaSuccess) return hm_cuda_fail(_e,#call);       \

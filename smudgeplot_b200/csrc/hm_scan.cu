@@ -104,9 +104,6 @@ int hm_peer_enable(const int *dev, int n);
 int hm_peer_sum_deg(uint8_t **deg, const int64_t *lo, const int64_t *hi, const int *dev,
                     cudaStream_t *st, int n, int64_t nels);
 int hm_peer_sum_plot(unsigned long long **plot, const int *dev, cudaStream_t *st, int n);
-/* GPU trim / symmetrise (hm_condition.cu) */
-int hm_condition_arrays(int kmer, int ethresh, int do_trim, int do_symm,
-                        uint64_t **pk, uint64_t **pl, uint16_t **pc, int64_t *pn, int64_t *pcap, cudaStream_t st);
 
 /* rc = the first failure of a sequence of CUDA calls (needs cudaError_t e and int rc in scope) */
 #define TRY(call) do { if (rc == HM_OK && (e = (call)) != cudaSuccess) rc = hm_cuda_fail(e,#call); } while (0)
@@ -139,21 +136,7 @@ static void dev_release(DevTable *D, void *p, int pooled)
   else        cudaFree(p);
 }
 
-/* counts device memory p of `bytes` as D's; if it cannot (out of host memory), frees p and fails */
-static cudaError_t dev_track(DevTable *D, void *p, int64_t bytes, int pooled)
-{ DevBlock *b = (DevBlock *) malloc(sizeof(DevBlock));
-  if (b == NULL)
-    { dev_release(D,p,pooled);
-      return cudaErrorMemoryAllocation;
-    }
-  b->p = p; b->bytes = bytes; b->pooled = pooled; b->next = D->blocks;
-  D->blocks = b;
-  D->held += bytes;
-  if (D->held > D->peak) D->peak = D->held;
-  return cudaSuccess;
-}
-
-/* *pp = `bytes` of device memory on D's device (current), stream-ordered on D->st when pooled */
+/* *pp = `bytes` of device memory on D's device (current), stream-ordered on D->st when pooled, counted in D->held */
 static cudaError_t dev_alloc(DevTable *D, void *pp, int64_t bytes)
 { void      **p = (void **) pp;
   cudaError_t e = cudaErrorMemoryAllocation;
@@ -164,9 +147,17 @@ static cudaError_t dev_alloc(DevTable *D, void *pp, int64_t bytes)
     }
   if (!pooled && (e = cudaMalloc(p,(size_t) bytes)) != cudaSuccess)
     return e;
-  if ((e = dev_track(D,*p,bytes,pooled)) != cudaSuccess)
-    *p = NULL;
-  return e;
+  DevBlock *b = (DevBlock *) malloc(sizeof(DevBlock));
+  if (b == NULL)                                           /* out of host memory: it cannot be counted */
+    { dev_release(D,*p,pooled);
+      *p = NULL;
+      return cudaErrorMemoryAllocation;
+    }
+  b->p = *p; b->bytes = bytes; b->pooled = pooled; b->next = D->blocks;
+  D->blocks = b;
+  D->held += bytes;
+  if (D->held > D->peak) D->peak = D->held;
+  return cudaSuccess;
 }
 
 static void dev_unlink(DevTable *D, DevBlock **at)
@@ -177,13 +168,21 @@ static void dev_unlink(DevTable *D, DevBlock **at)
   free(b);
 }
 
-/* frees what dev_alloc (or dev_track) gave; NULL is ignored */
+/* frees what dev_alloc gave; NULL is ignored */
 static void dev_free(DevTable *D, void *p)
 { for (DevBlock **at = &D->blocks; p != NULL && *at != NULL; at = &(*at)->next)
     if ((*at)->p == p)
       { dev_unlink(D,at);
         return;
       }
+}
+
+/* the bytes of what dev_alloc gave as p; 0 for NULL */
+static int64_t dev_bytes(const DevTable *D, const void *p)
+{ for (const DevBlock *b = D->blocks; p != NULL && b != NULL; b = b->next)
+    if (b->p == p)
+      return b->bytes;
+  return 0;
 }
 
 static void free_dev(DevTable *D)
@@ -991,10 +990,161 @@ static int ensure_symm(hm_scan *s)
   return HM_OK;
 }
 
-/* Trim (count >= ethresh) and / or symmetrise (add reverse complements) the device-resident table
- * in place: what the reference gets from `Logex` and `Symmex` (PloidyPlot.c:1381-1426), without
- * leaving the GPU.  Every device conditions its own replica (deterministic, identical results);
- * the index structures and work buffers are rebuilt for the new size.                          */
+/* ---- conditioning (DESIGN.md §4d; kernels, settle step and plan in hm_condition.cu) --------------------------
+ * One range loop, two ends.  Pass 0 histograms the output by key prefix over the source; the plan cuts the
+ * prefixes into key ranges; each range is then gathered over the source's chunks and settled (sort + merge).
+ * Source: the host table through the loader, a chunk at a time (hm_scan_condition_files), or the resident
+ * table as one chunk (hm_scan_condition).  Sink: FastK records handed to a writer thread, or the new table's
+ * device arrays at the range's offset.                                                                     */
+
+static int cond_hist_bits(int kmer) { return 2*kmer < HM_COND_HIST_BITS ? 2*kmer : HM_COND_HIST_BITS; }
+
+typedef struct
+  { hm_scan             *s;
+    DevTable            *D;
+    const hm_host_table *t;                /* the host table, or NULL: the resident arrays below are the source */
+    const int64_t       *d_index;          /* (host table) its stub index on the device, and the loader        */
+    Stager              *G;
+    uint64_t            *keys, *klo;       /* the chunk buffers (host table) or the resident table            */
+    uint16_t            *cnt;
+    int64_t              n, chunk;         /* source entries; entries per chunk                               */
+  } CondSrc;
+
+/* ordinals [o, o+m) of the source: loaded into the chunk buffers, or where they lie in the resident arrays */
+static int cond_fetch(const CondSrc *S, int64_t o, int64_t m, const uint64_t **k, const uint64_t **l, const uint16_t **c)
+{ if (S->t == NULL)
+    { *k = S->keys+o; *l = S->klo ? S->klo+o : NULL; *c = S->cnt+o;
+      return HM_OK;
+    }
+  *k = S->keys; *l = S->klo; *c = S->cnt;
+  return load_into(S->s,S->D,S->t,S->d_index,o,m,S->keys,S->klo,S->cnt,0,S->G);
+}
+
+/* pass 0: kept originals (+ their reverse complements) per key prefix -> hist (host, 2^hb entries) */
+static int cond_histogram(const CondSrc *S, int ethr, int do_symm, int hb, unsigned long long *d_hist, int64_t *hist)
+{ cudaStream_t  st = S->D->st;
+  const int64_t np = (int64_t) 1 << hb;
+  int           rc = HM_OK;
+  HM_CUDA(cudaMemsetAsync(d_hist,0,8*(size_t) np,st));
+  for (int64_t o = 0; o < S->n && rc == HM_OK; o += S->chunk)
+    { const int64_t   m = S->n-o < S->chunk ? S->n-o : S->chunk;
+      const uint64_t *k, *l;
+      const uint16_t *c;
+      rc = cond_fetch(S,o,m,&k,&l,&c);
+      if (rc == HM_OK) rc = hm_cond_hist(k,l,c,m,S->s->kmer,ethr,do_symm,hb,d_hist,st);
+    }
+  if (rc != HM_OK)
+    return rc;
+  HM_CUDA(cudaMemcpyAsync(hist,d_hist,8*(size_t) np,cudaMemcpyDeviceToHost,st));
+  HM_CUDA(cudaStreamSynchronize(st));
+  return HM_OK;
+}
+
+/* the range [p0, p1) of key prefixes gathered over the source's chunks into B and settled; *n_r: its entries */
+static int cond_range(const CondSrc *S, const hm_cond_bufs *B, uint64_t p0, uint64_t p1, unsigned long long *tiles,
+                      int64_t *n_r)
+{ cudaStream_t st = S->D->st;
+  int          rc = HM_OK;
+  HM_CUDA(cudaMemsetAsync(B->ctr,0,256,st));
+  for (int64_t o = 0; o < S->n && rc == HM_OK; o += S->chunk)
+    { const int64_t   m = S->n-o < S->chunk ? S->n-o : S->chunk;
+      const uint64_t *k, *l;
+      const uint16_t *c;
+      rc = cond_fetch(S,o,m,&k,&l,&c);
+      if (rc == HM_OK) rc = hm_cond_gather(k,l,c,m,B,p0,p1,tiles,st);
+    }
+  return rc != HM_OK ? rc : hm_cond_settle(B,n_r,st);
+}
+
+/* ---- in place --------------------------------------------------------------------------------------------- */
+
+/* device bytes of the in-place conditioning of a range of t output entries: the region its originals and
+ * reverse complements are gathered into and, when symmetrising, the sort's other buffers (+ the uint32
+ * permutation pair at k > 32), CUB's scratch bound and the merge's tile counts.  The range settles straight
+ * into the new table's arrays: no records, no merged copy.                                                 */
+static int64_t in_place_range_bytes(int64_t t, int do_symm, int kmer, int ibyte)
+{ const int64_t E = kmer > 32 ? 18 : 10;
+  (void) ibyte;
+  if (t < 1) t = 1;
+  return E*t + (do_symm ? E*t + (kmer > 32 ? 8*t : 0) + hm_cond_sort_room(t) + 2*hm_cond_tiles_bytes(t) : 0);
+}
+
+typedef struct
+  { int      ethr, do_symm, hb, n_ranges;
+    int64_t *cuts;                         /* key-prefix bounds of the ranges                              */
+    int64_t  out_cap;                      /* entries of each new array: the histogram's total (an upper   */
+                                           /*   bound: duplicates go) or, trimming only, n; plus one       */
+    int64_t  range_cap;                    /* entries of the largest range                                 */
+  } InPlace;
+
+/* one GPU's replica conditioned into new arrays of P->out_cap entries, which replace D's only when every range
+ * has settled; every allocation goes through dev_alloc, and the temporaries are gone on return             */
+static int condition_replica(hm_scan *s, DevTable *D, const InPlace *P, int64_t *n_out)
+{ const int     two = s->kmer > 32;
+  const int64_t cap = P->out_cap, T = P->do_symm ? (P->range_cap > 0 ? P->range_cap : 1) : cap;
+  CondSrc S;
+  memset(&S,0,sizeof(S));
+  S.s = s; S.D = D; S.keys = D->keys; S.klo = D->keys_lo; S.cnt = D->cnt;
+  S.n = s->n; S.chunk = s->n > 0 ? s->n : 1;
+  hm_cond_bufs B;
+  memset(&B,0,sizeof(B));
+  B.kmer = s->kmer; B.ibyte = s->ibyte; B.hb = P->hb; B.ethresh = P->ethr; B.do_symm = P->do_symm; B.cap = T;
+  uint64_t *nk = NULL, *nl = NULL;
+  uint16_t *nc = NULL;
+  unsigned long long *tiles = NULL;
+  int       rc = HM_OK;
+  cudaError_t e;
+  TRY(dev_alloc(D,&nk,8*cap));
+  if (two) TRY(dev_alloc(D,&nl,8*cap));
+  TRY(dev_alloc(D,&nc,2*cap));
+  TRY(dev_alloc(D,&B.ctr,256));
+  TRY(dev_alloc(D,&tiles,hm_cond_tiles_bytes(S.n)));
+  if (!P->do_symm)                                         /* the kept originals are the new table */
+    { B.key = nk; B.lo = nl; B.cnt = nc; }
+  else
+    { TRY(dev_alloc(D,&B.key,8*T));
+      if (two) TRY(dev_alloc(D,&B.lo,8*T));
+      TRY(dev_alloc(D,&B.cnt,2*T));
+      TRY(dev_alloc(D,&B.alt_key,8*T));
+      TRY(dev_alloc(D,&B.alt_cnt,2*T));
+      if (two)
+        { TRY(dev_alloc(D,&B.alt_lo,8*T));
+          TRY(dev_alloc(D,&B.idx[0],4*T));
+          TRY(dev_alloc(D,&B.idx[1],4*T));
+        }
+      TRY(dev_alloc(D,&B.mtiles,2*hm_cond_tiles_bytes(T)));
+      B.sort_bytes = hm_cond_sort_room(T);
+      TRY(dev_alloc(D,&B.sort_tmp,B.sort_bytes));
+    }
+  int64_t out = 0;
+  for (int r = 0; r < P->n_ranges && rc == HM_OK; r++)
+    { int64_t n_r = 0;
+      if (P->do_symm)                                      /* the range's place in the new table */
+        { B.m_key = nk+out; B.m_lo = two ? nl+out : NULL; B.m_cnt = nc+out; }
+      rc = cond_range(&S,&B,(uint64_t) P->cuts[r],(uint64_t) P->cuts[r+1],tiles,&n_r);
+      s->launches += 3 + (P->do_symm ? 6 : 0);
+      out += n_r;
+    }
+  void *tmp[] = { B.ctr, tiles, B.alt_key, B.alt_cnt, B.alt_lo, B.idx[0], B.idx[1], B.mtiles, B.sort_tmp,
+                  P->do_symm ? B.key : NULL, P->do_symm ? B.lo : NULL, P->do_symm ? B.cnt : NULL };
+  for (size_t k = 0; k < sizeof(tmp)/sizeof(tmp[0]); k++)
+    dev_free(D,tmp[k]);
+  void *drop[3] = { nk, nl, nc };
+  if (rc == HM_OK)                                         /* the new table replaces the old one */
+    { drop[0] = D->keys; drop[1] = D->keys_lo; drop[2] = D->cnt;
+      D->keys = nk; D->keys_lo = nl; D->cnt = nc;
+    }
+  for (int a = 0; a < 3; a++)
+    dev_free(D,drop[a]);
+  *n_out = out;
+  return rc;
+}
+
+/* Trim (count >= ethresh) and / or symmetrise (add reverse complements) the device-resident table in place:
+ * what the reference gets from `Logex` and `Symmex` (PloidyPlot.c:1381-1426), without leaving the GPU.  The
+ * replicas are identical, so GPU 0 histograms the output and the plan is every GPU's; each GPU then conditions
+ * its own replica through the range passes, and the index structures and work buffers are rebuilt for the
+ * new size.  The plan is checked against the budget before anything is touched.                          */
 extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_symm, int64_t *nels_out)
 { int     G = s->ngpu, rc = HM_OK;
   int64_t n_new = -1;
@@ -1007,18 +1157,65 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
   if (s->streamed)
     return hm_set_error(HM_EUNSUPPORTED,"conditioning on the GPU needs the table resident; this one does not fit in "
                                         "device memory (budget %lld bytes)",(long long) s->budget);
-  { /* before anything is touched: the table arrays + what conditioning borrows must fit the budget */
-    int64_t need = 8*(s->n+1) + (s->kmer > 32 ? 8*(s->n+1) : 0) + 2*(s->n+8) + 8*(int64_t) HM_PLOT_CELLS +
-                   hm_condition_bytes(s->kmer,s->n,do_trim,do_symm);
-    if (need > s->budget)
-      return hm_set_error(HM_ENOMEM,"conditioning %lld entries on the GPU needs %lld device bytes, more than the "
-                          "budget of %lld",(long long) s->n,(long long) need,(long long) s->budget);
-  }
+  InPlace P;
+  memset(&P,0,sizeof(P));
+  P.ethr = do_trim ? ethresh : 0; P.do_symm = do_symm; P.hb = cond_hist_bits(s->kmer);
+  const int64_t np = (int64_t) 1 << P.hb;
+  int64_t whole[2] = { 0, np }, *hist = NULL, big = 0, total = s->n;
+  P.cuts = whole; P.n_ranges = 1; P.range_cap = s->n;
+  if (do_symm)                                             /* pass 0 on GPU 0: the output histogram */
+    { DevTable *D = s->d;
+      unsigned long long *d_hist = NULL;
+      cudaError_t e;
+      hist = (int64_t *) malloc(sizeof(int64_t)*(size_t) np);
+      P.cuts = (int64_t *) malloc(sizeof(int64_t)*(size_t) (np+1));
+      if (hist == NULL || P.cuts == NULL)
+        { free(hist); free(P.cuts); return hm_set_error(HM_ENOMEM,"out of host memory"); }
+      CondSrc S;
+      memset(&S,0,sizeof(S));
+      S.s = s; S.D = D; S.keys = D->keys; S.klo = D->keys_lo; S.cnt = D->cnt; S.n = s->n; S.chunk = s->n > 0 ? s->n : 1;
+      TRY(cudaSetDevice(D->dev));
+      TRY(dev_alloc(D,&d_hist,8*np));
+      if (rc == HM_OK) rc = cond_histogram(&S,P.ethr,1,P.hb,d_hist,hist);
+      dev_free(D,d_hist);
+      s->launches += 1;
+      total = 0;
+      for (int64_t p = 0; p < np; p++) total += hist[p];
+    }
+  P.out_cap = total + 1;
+  /* what each GPU holds meanwhile: its table and what stays of the scan (the index and work buffers go), the
+   * new arrays, the counters and the chunk's tile counts, and the working set of the largest range          */
+  int64_t held = 0;
+  for (int g = 0; g < G; g++)
+    { const DevTable *D = s->d+g;
+      int64_t h = D->held - dev_bytes(D,D->deg) - dev_bytes(D,D->up) - dev_bytes(D,D->bucket) -
+                  dev_bytes(D,D->filter) - dev_bytes(D,D->symm_work);
+      if (h > held) held = h;
+    }
+  const int64_t fixed = held + (s->kmer > 32 ? 18 : 10)*P.out_cap + 256 + hm_cond_tiles_bytes(s->n);
+  int64_t need = fixed, one = fixed;
+  if (rc == HM_OK && do_symm)
+    { const int64_t limit = hm_cond_range_limit(s->budget-fixed,in_place_range_bytes,1,s->kmer,s->ibyte);
+      P.n_ranges = hm_cond_cut(hist,P.hb,limit,P.cuts,&P.range_cap,&big);
+      need += in_place_range_bytes(big,1,s->kmer,s->ibyte);
+      one  += in_place_range_bytes(total,1,s->kmer,s->ibyte);
+    }
+  free(hist);
+  if (rc == HM_OK && (P.n_ranges < 1 || need > s->budget))
+    rc = hm_set_error(HM_ENOMEM,"conditioning %lld entries on the GPU needs %lld device bytes (%lld in one range), more "
+                      "than the budget of %lld",(long long) s->n,(long long) need,(long long) one,(long long) s->budget);
+  if (rc != HM_OK)
+    { if (P.cuts != whole) free(P.cuts);
+      return rc;
+    }
+
   /* everything derived from the old table goes first: work buffers of both paths, the index */
   s->conditioned = 1;
   s->ran = 0; s->have_direct = 0; s->have_symm = 0; s->symm_ready = 0;
   if ((rc = sync_all(s,"conditioning")) != HM_OK)
-    return rc;
+    { if (P.cuts != whole) free(P.cuts);
+      return rc;
+    }
   for (int g = 0; g < G; g++)
     { DevTable *D = s->d+g;
       cudaSetDevice(D->dev);
@@ -1030,28 +1227,11 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
     }
   for (int g = 0; g < G && rc == HM_OK; g++)
     { DevTable *D = s->d+g;
-      int64_t   n = s->n, cap = 0;
-      uint64_t *keys = D->keys, *keys_lo = D->keys_lo;
-      uint16_t *cnt = D->cnt;
+      int64_t   n = 0;
       cudaError_t e;
       TRY(cudaSetDevice(D->dev));
       if (rc == HM_OK)
-        rc = hm_condition_arrays(s->kmer,ethresh,do_trim,do_symm,&D->keys,&D->keys_lo,&D->cnt,&n,&cap,D->st);
-      s->launches += 6;
-      if (rc == HM_OK && D->keys != keys)          /* the new table (cap entries per array) replaces the old one */
-        { cudaError_t ek = dev_track(D,D->keys,8*cap,0);
-          cudaError_t el = D->keys_lo != NULL ? dev_track(D,D->keys_lo,8*cap,0) : cudaSuccess;
-          cudaError_t ec = dev_track(D,D->cnt,2*cap,0);
-          void *drop[3] = { keys, keys_lo, cnt };
-          if (ek != cudaSuccess || el != cudaSuccess || ec != cudaSuccess)
-            { /* (dev_track has freed what it could not count): the old table stays */
-              drop[0] = D->keys; drop[1] = D->keys_lo; drop[2] = D->cnt;
-              D->keys = keys; D->keys_lo = keys_lo; D->cnt = cnt;
-              rc = hm_set_error(HM_ENOMEM,"out of host memory");
-            }
-          for (int a = 0; a < 3; a++)
-            dev_free(D,drop[a]);
-        }
+        rc = condition_replica(s,D,&P,&n);
       if (rc == HM_OK && n_new >= 0 && n != n_new)
         rc = hm_set_error(HM_ECUDA,"conditioning gave %lld entries on GPU %d but %lld on GPU 0",
                           (long long) n,D->dev,(long long) n_new);
@@ -1059,6 +1239,7 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
         s->invalid = 1;                        /* the replicas no longer agree */
       n_new = n;
     }
+  if (P.cuts != whole) free(P.cuts);
   if (rc == HM_OK)
     { s->n     = n_new;
       s->bits  = hm_pick_bucket_bits(s->n);
@@ -1094,7 +1275,7 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
   return rc_cond != HM_OK ? rc_cond : rc;
 }
 
-/* ---- conditioning into table files (DESIGN.md §4d; kernels and plan in hm_condition_files.cu) ----------- */
+/* ---- into table files ------------------------------------------------------------------------------------ */
 
 /* 1 if the table `dst` would be written over holds one of the source's part files */
 static int names_source(const hm_host_table *t, const char *dst)
@@ -1169,7 +1350,7 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
   DevTable *D = s->d;
   const int kmer = s->kmer, ibyte = t->ibyte, KW = kmer > 32 ? 2 : 1;
   const int pbyte = ((kmer+3)>>2) - ibyte + 2;
-  const int hb = 2*kmer < HM_COND_HIST_BITS ? 2*kmer : HM_COND_HIST_BITS;
+  const int hb = cond_hist_bits(kmer);
   const int64_t n = t->nels, np = (int64_t) 1 << hb, ixlen = (int64_t) 1 << (8*ibyte);
   const int ethr = do_trim ? ethresh : 0;
   int       rc = HM_OK;
@@ -1219,18 +1400,13 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
   TRY(dev_alloc(D,&cc,2*(chunk+8)));
   TRY(dev_alloc(D,&tiles,hm_cond_tiles_bytes(chunk)));
   TRY(cudaMemcpyAsync(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,D->st));
-  TRY(cudaMemsetAsync(d_hist,0,8*(size_t) np,D->st));
   if (rc == HM_OK)
     rc = stager_open(s,D,t,chunk,&G);
+  CondSrc src = { s, D, t, d_index, &G, ck, cl, cc, n, chunk };
 
   /* pass 0: the output histogram */
-  for (int64_t o = 0; o < n && rc == HM_OK; o += chunk)
-    { int64_t m = n-o < chunk ? n-o : chunk;
-      rc = load_into(s,D,t,d_index,o,m,ck,cl,cc,0,&G);
-      if (rc == HM_OK) rc = hm_cond_hist(ck,cl,cc,m,kmer,ethr,do_symm,hb,d_hist,D->st);
-    }
-  TRY(cudaMemcpyAsync(hist,d_hist,8*(size_t) np,cudaMemcpyDeviceToHost,D->st));
-  TRY(cudaStreamSynchronize(D->st));
+  if (rc == HM_OK)
+    rc = cond_histogram(&src,ethr,do_symm,hb,d_hist,hist);
   S.ms_hist = now_ms()-t0;
   if (rc == HM_OK)
     rc = hm_condition_plan(n,kmer,ibyte,budget,do_symm,hist,hb,cuts,&lay);
@@ -1274,12 +1450,8 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
   double t_ranges = now_ms();
   for (int r = 0; r < lay.n_ranges && rc == HM_OK; r++)
     { const uint64_t p0 = (uint64_t) cuts[r], p1 = (uint64_t) cuts[r+1];
-      TRY(cudaMemsetAsync(B.ctr,0,256,D->st));
-      for (int64_t o = 0; o < n && rc == HM_OK; o += chunk)
-        { int64_t m = n-o < chunk ? n-o : chunk;
-          rc = load_into(s,D,t,d_index,o,m,ck,cl,cc,0,&G);
-          if (rc == HM_OK) rc = hm_cond_gather(ck,cl,cc,m,&B,p0,p1,tiles,D->st);
-        }
+      int64_t n_r = 0;
+      rc = cond_range(&src,&B,p0,p1,tiles,&n_r);
       /* the stub buckets the range's keys fall in */
       const uint64_t b0 = 8*ibyte >= hb ? p0 << (8*ibyte-hb) : p0 >> (hb-8*ibyte);
       const uint64_t b1 = 8*ibyte >= hb ? p1 << (8*ibyte-hb) : ((p1-1) >> (hb-8*ibyte)) + 1;
@@ -1287,8 +1459,7 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
         { pthread_join(th,NULL); writing = 0;
           if (J.rc != HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
         }
-      int64_t n_r = 0;
-      if (rc == HM_OK) rc = hm_cond_finish(&B,b0,(int64_t) (b1-b0),&n_r,D->st);
+      if (rc == HM_OK) rc = hm_cond_pack(&B,n_r,b0,(int64_t) (b1-b0),D->st);
       TRY(cudaMemcpy(hcnt,B.bcount,8*(size_t) (b1-b0),cudaMemcpyDeviceToHost));
       if (rc == HM_OK)
         { J.n = n_r; J.b0 = (int64_t) b0; J.nb = (int64_t) (b1-b0); J.counts = hcnt;

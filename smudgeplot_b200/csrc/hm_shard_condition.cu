@@ -10,7 +10,7 @@
  *                               offsets), then the reverse complements in per-destination segments (warp-aggregated
  *                               cursors; any order inside a segment)
  *   hm_k_shard_settle           the received reverse complements sorted and merged with the received originals
- *                               (already sorted): hm_condition_files.cu's sort_rc / merge_ranked
+ *                               (already sorted): hm_cond_settle, the step every conditioning driver settles with
  * The collectives between the calls are the caller's.
  *******************************************************************************************/
 #include <cuda_runtime.h>
@@ -21,30 +21,7 @@
 #include "hm_internal.h"
 #include "hm_device.cuh"
 
-#define CT 256                                   /* threads per CTA = entries per tile */
 #define FULL 0xffffffffu
-
-/* ctr[d] += lanes with pred whose destination is d (one atomic per destination and warp) */
-__device__ __forceinline__ void warp_add(unsigned long long *ctr, bool pred, int d)
-{ const unsigned act = __ballot_sync(FULL,pred);
-  if (pred)
-    { const unsigned peers = __match_any_sync(act,d);
-      if ((threadIdx.x & 31) == (unsigned) (__ffs(peers)-1))
-        atomicAdd(ctr+d,(unsigned long long) __popc(peers));
-    }
-}
-
-/* exclusive rank of this thread's pred among the CTA's */
-__device__ __forceinline__ int cta_rank(bool pred)
-{ __shared__ int s_w[CT/32];
-  const int      lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned b = __ballot_sync(FULL,pred);
-  if (lane == 0) s_w[warp] = __popc(b);
-  __syncthreads();
-  int before = 0;
-  for (int w = 0; w < warp; w++) before += s_w[w];
-  return before + __popc(b & ((1u << lane)-1));
-}
 
 /* counts[d]: kept originals bound for rank d; counts[world+d]: reverse complements; tiles[t]: kept originals of tile t */
 template <int KW>
@@ -58,11 +35,11 @@ route_count_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict
   if (kept) { x = keys[i]; if (KW == 2) xl = klo[i]; }
   const int n_in = __syncthreads_count(kept);
   if (threadIdx.x == 0) tiles[blockIdx.x] = (unsigned long long) n_in;
-  warp_add(counts,kept,kept ? dest[x >> (64-hb)] : 0);
+  warp_count(counts,kept,kept ? dest[x >> (64-hb)] : 0);
   if (do_symm)
     { uint64_t r, rl;
       revcomp_kmer<KW>(x,xl,kmer,r,rl);
-      warp_add(counts+world,kept,kept ? dest[r >> (64-hb)] : 0);
+      warp_count(counts+world,kept,kept ? dest[r >> (64-hb)] : 0);
     }
 }
 
@@ -107,8 +84,6 @@ route_scatter_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
         atomicOr(flag,1ull);
     }
 }
-
-static unsigned grid(int64_t n) { return (unsigned) ((n+CT-1)/CT > 0 ? (n+CT-1)/CT : 1); }
 
 static int64_t a256(int64_t b) { return (b+255) & ~255ll; }
 
@@ -189,22 +164,13 @@ extern "C" int hm_k_shard_settle(int kmer, uint64_t *d_key, uint64_t *d_lo, uint
     return hm_set_error(HM_EINVAL,"hm_k_shard_settle: %lld bytes of scratch, %lld needed",(long long) scratch_bytes,
                         (long long) hm_k_shard_settle_bytes(kmer,T,n_rc));
   cudaStream_t st = (cudaStream_t) stream;
-  if (n_rc == 0)                                           /* the received originals are the share */
-    { if (n_orig > 0)
-        { HM_CUDA(cudaMemcpyAsync(d_out_key,d_key,8*(size_t) n_orig,cudaMemcpyDeviceToDevice,st));
-          if (two) HM_CUDA(cudaMemcpyAsync(d_out_lo,d_lo,8*(size_t) n_orig,cudaMemcpyDeviceToDevice,st));
-          HM_CUDA(cudaMemcpyAsync(d_out_cnt,d_cnt,2*(size_t) n_orig,cudaMemcpyDeviceToDevice,st));
-        }
-      *n_out = n_orig;
-      return HM_OK;
-    }
   hm_cond_bufs B;
   memset(&B,0,sizeof(B));
   B.kmer = kmer; B.do_symm = 1; B.cap = T;
   B.key = d_key; B.lo = d_lo; B.cnt = d_cnt;
   B.m_key = d_out_key; B.m_lo = d_out_lo; B.m_cnt = d_out_cnt;
   uint8_t *p = (uint8_t *) d_scratch;
-  const int64_t c = n_rc;
+  const int64_t c = n_rc > 0 ? n_rc : 1;
   B.alt_key = (uint64_t *) p; p += a256(8*c);
   B.alt_cnt = (uint16_t *) p; p += a256(2*c);
   if (two)
@@ -216,16 +182,10 @@ extern "C" int hm_k_shard_settle(int kmer, uint64_t *d_key, uint64_t *d_lo, uint
   B.ctr = (unsigned long long *) p; p += 256;
   B.sort_tmp = p;
   B.sort_bytes = scratch_bytes - (int64_t) (p - (uint8_t *) d_scratch);
-  uint64_t *rk = NULL, *rl = NULL;
-  uint16_t *rc_ = NULL;
-  int rc = hm_cond_sort_rc(&B,c,&rk,&rl,&rc_,st);
-  if (rc == HM_OK) rc = hm_cond_merge(&B,n_orig,rk,rl,rc_,c,st);
-  if (rc != HM_OK) return rc;
-  unsigned long long dropped = 0;
-  HM_CUDA(cudaMemcpyAsync(&dropped,B.ctr+5,sizeof(dropped),cudaMemcpyDeviceToHost,st));
-  HM_CUDA(cudaStreamSynchronize(st));
-  *n_out = T - (int64_t) dropped;                          /* reverse complements equal to an original went */
-  return HM_OK;
+  /* the counters a gather would have left: originals at the region's front, reverse complements at its end */
+  const unsigned long long h[4] = { (unsigned long long) n_orig, (unsigned long long) n_rc, 0, 0 };
+  HM_CUDA(cudaMemcpyAsync(B.ctr,h,sizeof(h),cudaMemcpyHostToDevice,st));
+  return hm_cond_settle(&B,n_out,st);
 }
 
 /* device bytes one rank's conditioning holds at most (each array rounded to 512 bytes, as torch's allocator
