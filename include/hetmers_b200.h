@@ -519,6 +519,42 @@ int hm_k_shard_settle(int kmer, uint64_t *d_key, uint64_t *d_lo, uint16_t *d_cnt
 int64_t hm_shard_condition_bytes(int kmer, int ibyte, int world, int64_t share, int64_t sent, int64_t received,
                                  int64_t rc_received, int64_t total_out, int do_symm);
 
+/* ---- conditioning across the ranks into new table files (dist.condition_ktab, DESIGN.md §4f) ----
+ * The steps above in passes: in pass p, rank d owns the p-th sub-range (window) of its range of key prefixes, and
+ * d_dest maps the prefixes of this pass's windows to their ranks and every other prefix to -1.  The _window route
+ * calls take the arguments of the calls above; an entry (or reverse complement) whose prefix maps to -1 is neither
+ * counted nor written, and the tile counts cover the in-window kept originals only.                          */
+int hm_k_shard_route_count_window(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m,
+                                  int kmer, int ethresh, int do_symm, const int16_t *d_dest, int world,
+                                  uint64_t *d_counts, uint64_t *d_tiles, void *stream);
+int hm_k_shard_route_scatter_window(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                                    int64_t m, int kmer, int ethresh, int do_symm, const int16_t *d_dest,
+                                    const uint64_t *d_tiles, uint64_t *d_send_key, uint64_t *d_send_lo,
+                                    uint16_t *d_send_cnt, int64_t n_orig, int64_t n_rc, uint64_t *d_cursor,
+                                    uint64_t *d_flag, void *stream);
+/* n sorted entries -> FastK records at d_rec (suffix bytes ibyte..kbyte-1, then the little-endian count: stride
+ * kbyte - ibyte + 2) and d_bcount[b - b0] = the records in stub bucket b, for the nb buckets [b0, b0 + nb) that
+ * must hold every entry (zeroed here).  Synchronises the stream.                                              */
+int hm_k_cond_pack(int kmer, int ibyte, const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                   int64_t n, int64_t b0, int64_t nb, uint8_t *d_rec, uint64_t *d_bcount, void *stream);
+/* The memory model of one rank: resident for the whole call, its share of `share` source entries unpacked (E =
+ * 10 / 18 bytes per entry at k <= 32 / > 32) with its tile counts, the two histograms, the destination map, the
+ * route counters, the stub-bucket counts and 1 MiB of small tensors; beside it the larger of the load (the share's
+ * records and the stub index) and one pass -- route: `sent` entries; exchange: sent + `received`; settle (do_symm):
+ * received twice and hm_k_shard_settle_bytes(kmer, received, rc_received); pack: received + their records.  Arrays
+ * are rounded to 512 bytes, as torch's allocator rounds them.  -> the bytes of the pass (monotone in every count),
+ * -1 on bad arguments.                                                                                        */
+int64_t hm_rank_condition_bytes(int kmer, int ibyte, int world, int64_t share, int64_t sent, int64_t received,
+                                int64_t rc_received, int do_symm);
+/* Cut one rank's range of np key prefixes (hist: output entries per prefix, summed over the ranks) into
+ * sub-ranges, greedily in key order: cuts[0] = 0 < ... < cuts[*n_sub] = np (cuts: room for np + 1; no sub-range
+ * when np = 0), each of at
+ * most HM_COND_MAX_RANGE entries and of at most the t entries whose pass, counted as sending and receiving t,
+ * fits the budget beside the resident part.  HM_ENOMEM with the sizes when the load or one prefix alone does
+ * not fit.                                                                                                    */
+int hm_rank_condition_cut(int kmer, int ibyte, int world, int64_t share, int do_symm, int64_t budget,
+                          const int64_t *hist, int64_t np, int64_t *cuts, int64_t *n_sub);
+
 /* one call: create + run + destroy (what bench.py's e2e leg times) */
 int  hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,
                      int64_t *plot, hm_scan_stats *stats);

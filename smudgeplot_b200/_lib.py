@@ -36,6 +36,8 @@ ABI_SYMBOLS = [
     "hm_table_write_abort",
     "hm_k_cond_hist", "hm_k_shard_route_count", "hm_k_shard_route_scatter", "hm_k_shard_settle_bytes",
     "hm_k_shard_settle", "hm_shard_condition_bytes",
+    "hm_k_shard_route_count_window", "hm_k_shard_route_scatter_window", "hm_k_cond_pack", "hm_rank_condition_bytes",
+    "hm_rank_condition_cut",
 ]
 
 
@@ -234,6 +236,12 @@ def lib():
     L.hm_k_shard_settle.argtypes = [i32, vp, vp, vp, i64, i64, vp, i64, vp, vp, vp, C.POINTER(i64), vp]
     L.hm_shard_condition_bytes.argtypes = [i32, i32, i32, i64, i64, i64, i64, i64, i32]
     L.hm_shard_condition_bytes.restype = i64
+    L.hm_k_shard_route_count_window.argtypes = L.hm_k_shard_route_count.argtypes
+    L.hm_k_shard_route_scatter_window.argtypes = L.hm_k_shard_route_scatter.argtypes
+    L.hm_k_cond_pack.argtypes = [i32, i32, vp, vp, vp, i64, i64, i64, vp, vp, vp]
+    L.hm_rank_condition_bytes.argtypes = [i32, i32, i32, i64, i64, i64, i64, i32]
+    L.hm_rank_condition_bytes.restype = i64
+    L.hm_rank_condition_cut.argtypes = [i32, i32, i32, i64, i32, i64, vp, i64, vp, C.POINTER(i64)]
     _lib = L
     return L
 

@@ -294,7 +294,7 @@ extern "C" int hm_condition_plan(int64_t n, int kmer, int ibyte, int64_t budget,
   out->range_room  = budget - budget/4 - fixed;            /* the chunk takes at most the other quarter */
   const int64_t lo = hm_cond_range_limit(out->range_room,hm_condition_range_bytes,do_symm,kmer,ibyte);
   int64_t big = 0, cap = 0;
-  const int r = hm_cond_cut(hist,hist_bits,lo,cuts,&cap,&big);
+  const int r = hm_cond_cut(hist,(int64_t) 1 << hist_bits,lo,cuts,&cap,&big);
   if (cb > budget/4 || out->range_room <= 0 || r < 1 || (lo < 1 && n > 0))
     return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes cannot hold one range of the conditioning: %lld bytes "
                         "are fixed (stub index, bucket counts, histogram, a chunk of %lld entries) and the largest key "
@@ -317,9 +317,8 @@ int64_t hm_cond_range_limit(int64_t room, hm_cond_bytes_fn bytes, int do_symm, i
   return lo;
 }
 
-int hm_cond_cut(const int64_t *hist, int hb, int64_t limit, int64_t *cuts, int64_t *range_cap, int64_t *big)
-{ const int64_t np = (int64_t) 1 << hb;
-  int64_t t = 0, tmax = 0;
+int hm_cond_cut(const int64_t *hist, int64_t np, int64_t limit, int64_t *cuts, int64_t *range_cap, int64_t *big)
+{ int64_t t = 0, tmax = 0;
   int     r = 0;
   *big = 0;
   for (int64_t p = 0; p < np; p++)

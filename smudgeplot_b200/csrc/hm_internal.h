@@ -141,12 +141,12 @@ int64_t hm_cond_chunk(int64_t n, int kmer, int ibyte, int64_t budget);
 int64_t hm_cond_tiles_bytes(int64_t n);
 int64_t hm_cond_sort_room(int64_t c);
 /* the plan's two halves shared by the drivers: the most output entries one range may hold when a range of t
- * needs bytes(t, do_symm, kmer, ibyte) <= room (bisection), and the greedy cuts of the 2^hb key prefixes into
+ * needs bytes(t, do_symm, kmer, ibyte) <= room (bisection), and the greedy cuts of np key prefixes into
  * ranges of at most `limit` entries (cuts[0..R], R returned; *range_cap: the largest range; *big: the largest
  * prefix -- 0 ranges when it alone exceeds the limit)                                                     */
 typedef int64_t (*hm_cond_bytes_fn)(int64_t t, int do_symm, int kmer, int ibyte);
 int64_t hm_cond_range_limit(int64_t room, hm_cond_bytes_fn bytes, int do_symm, int kmer, int ibyte);
-int     hm_cond_cut(const int64_t *hist, int hb, int64_t limit, int64_t *cuts, int64_t *range_cap, int64_t *big);
+int     hm_cond_cut(const int64_t *hist, int64_t np, int64_t limit, int64_t *cuts, int64_t *range_cap, int64_t *big);
 #define HM_CUDA(call)                                             \
   do { cudaError_t _e = (call);                                    \
        if (_e != cudaSuccess) return hm_cuda_fail(_e,#call);       \

@@ -1196,7 +1196,7 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
   int64_t need = fixed, one = fixed;
   if (rc == HM_OK && do_symm)
     { const int64_t limit = hm_cond_range_limit(s->budget-fixed,in_place_range_bytes,1,s->kmer,s->ibyte);
-      P.n_ranges = hm_cond_cut(hist,P.hb,limit,P.cuts,&P.range_cap,&big);
+      P.n_ranges = hm_cond_cut(hist,np,limit,P.cuts,&P.range_cap,&big);
       need += in_place_range_bytes(big,1,s->kmer,s->ibyte);
       one  += in_place_range_bytes(total,1,s->kmer,s->ibyte);
     }

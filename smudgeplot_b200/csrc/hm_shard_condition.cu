@@ -11,6 +11,9 @@
  *                               cursors; any order inside a segment)
  *   hm_k_shard_settle           the received reverse complements sorted and merged with the received originals
  *                               (already sorted): hm_cond_settle, the step every conditioning driver settles with
+ * Into new table files (dist.condition_ktab, §4f) the same steps run in passes, each over one window of key prefixes
+ * per rank: the route kernels' WIN instantiations skip the entries outside the pass's windows, hm_k_cond_pack packs
+ * the settled entries into FastK records, and hm_rank_condition_cut / _bytes plan the passes.
  * The collectives between the calls are the caller's.
  *******************************************************************************************/
 #include <cuda_runtime.h>
@@ -23,8 +26,10 @@
 
 #define FULL 0xffffffffu
 
-/* counts[d]: kept originals bound for rank d; counts[world+d]: reverse complements; tiles[t]: kept originals of tile t */
-template <int KW>
+/* counts[d]: kept originals bound for rank d; counts[world+d]: reverse complements; tiles[t]: kept originals of tile t.
+ * WIN (one pass of a windowed conditioning): dest[prefix] < 0 marks a prefix outside this pass; an entry there
+ * is neither counted nor written, and the tile counts cover the in-window kept originals only                  */
+template <int KW, bool WIN>
 __global__ void __launch_bounds__(CT)
 route_count_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ klo, const uint16_t *__restrict__ cnt,
                    int64_t m, int kmer, int ethresh, int do_symm, int hb, const int16_t *__restrict__ dest, int world,
@@ -33,19 +38,28 @@ route_count_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict
   const bool    kept = i < m && cnt[i] >= ethresh;
   uint64_t x = 0, xl = 0;
   if (kept) { x = keys[i]; if (KW == 2) xl = klo[i]; }
-  const int n_in = __syncthreads_count(kept);
+  const int  d  = WIN && kept ? dest[x >> (64-hb)] : -1;
+  const bool in = WIN ? d >= 0 : kept;
+  const int n_in = __syncthreads_count(in);
   if (threadIdx.x == 0) tiles[blockIdx.x] = (unsigned long long) n_in;
-  warp_count(counts,kept,kept ? dest[x >> (64-hb)] : 0);
+  if (WIN) warp_count(counts,in,in ? d : 0);
+  else     warp_count(counts,kept,kept ? dest[x >> (64-hb)] : 0);
   if (do_symm)
     { uint64_t r, rl;
       revcomp_kmer<KW>(x,xl,kmer,r,rl);
-      warp_count(counts+world,kept,kept ? dest[r >> (64-hb)] : 0);
+      if (WIN)
+        { const int rd = kept ? dest[r >> (64-hb)] : -1;
+          warp_count(counts+world,rd >= 0,rd >= 0 ? rd : 0);
+        }
+      else
+        warp_count(counts+world,kept,kept ? dest[r >> (64-hb)] : 0);
     }
 }
 
 /* tiles: exclusive offsets of the kept originals (hm_cond_scan_tiles); cursor[d]: the next free slot of rank d's
- * reverse-complement segment, counted from s_* + n_orig; flag: set when a slot lies beyond the buffer         */
-template <int KW>
+ * reverse-complement segment, counted from s_* + n_orig; flag: set when a slot lies beyond the buffer.  WIN: as
+ * route_count_kernel                                                                                            */
+template <int KW, bool WIN>
 __global__ void __launch_bounds__(CT)
 route_scatter_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ klo, const uint16_t *__restrict__ cnt,
                      int64_t m, int kmer, int ethresh, int do_symm, int hb, const int16_t *__restrict__ dest,
@@ -57,8 +71,9 @@ route_scatter_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
   uint64_t x = 0, xl = 0;
   uint16_t c = 0;
   if (kept) { x = keys[i]; if (KW == 2) xl = klo[i]; c = cnt[i]; }
-  const int rank = cta_rank(kept);
-  if (kept)
+  const bool in = WIN ? kept && dest[x >> (64-hb)] >= 0 : kept;
+  const int rank = cta_rank(in);
+  if (in)
     { const int64_t g = (int64_t) tiles[blockIdx.x] + rank;   /* originals keep their order: the destination is */
       if (g < n_orig)                                         /* monotone in the key, so rank d's are one slice */
         { s_key[g] = x; if (KW == 2) s_lo[g] = xl; s_cnt[g] = c; }
@@ -69,9 +84,11 @@ route_scatter_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
     return;
   uint64_t r, rl;
   revcomp_kmer<KW>(x,xl,kmer,r,rl);
-  const unsigned act = __ballot_sync(FULL,kept);
-  if (kept)
-    { const int      d = dest[r >> (64-hb)];
+  const int  rd  = WIN && kept ? dest[r >> (64-hb)] : -1;
+  const bool rin = WIN ? rd >= 0 : kept;
+  const unsigned act = __ballot_sync(FULL,rin);
+  if (rin)
+    { const int      d = WIN ? rd : dest[r >> (64-hb)];
       const unsigned peers = __match_any_sync(act,d);
       const int      lane = threadIdx.x & 31, leader = __ffs(peers)-1;
       unsigned long long base = 0;
@@ -99,30 +116,31 @@ extern "C" int hm_k_cond_hist(const uint64_t *d_keys, const uint64_t *d_keys_lo,
                       (unsigned long long *) d_hist,(cudaStream_t) stream);
 }
 
-extern "C" int hm_k_shard_route_count(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m,
-                                      int kmer, int ethresh, int do_symm, const int16_t *d_dest, int world,
-                                      uint64_t *d_counts, uint64_t *d_tiles, void *stream)
+template <bool WIN>
+static int route_count(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m, int kmer,
+                       int ethresh, int do_symm, const int16_t *d_dest, int world, uint64_t *d_counts,
+                       uint64_t *d_tiles, void *stream, const char *name)
 { if (kmer < 1 || kmer > HM_MAX_KMER || m < 0 || world < 1 || (m > 0 && (kmer > 32) != (d_keys_lo != NULL)))
-    return hm_set_error(HM_EINVAL,"hm_k_shard_route_count: bad arguments");
+    return hm_set_error(HM_EINVAL,"%s: bad arguments",name);
   cudaStream_t st = (cudaStream_t) stream;
   unsigned long long *counts = (unsigned long long *) d_counts, *tiles = (unsigned long long *) d_tiles;
   const int hb = hist_bits_of(kmer);
   if (m > 0)
-    { if (kmer > 32) route_count_kernel<2><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,world,counts,tiles);
-      else           route_count_kernel<1><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,world,counts,tiles);
+    { if (kmer > 32) route_count_kernel<2,WIN><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,world,counts,tiles);
+      else           route_count_kernel<1,WIN><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,world,counts,tiles);
       LAUNCHED("route_count_kernel");
     }
   return hm_cond_scan_tiles(tiles,m > 0 ? grid(m) : 0,counts+2*world,st);
 }
 
-extern "C" int hm_k_shard_route_scatter(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
-                                        int64_t m, int kmer, int ethresh, int do_symm, const int16_t *d_dest,
-                                        const uint64_t *d_tiles, uint64_t *d_send_key, uint64_t *d_send_lo,
-                                        uint16_t *d_send_cnt, int64_t n_orig, int64_t n_rc, uint64_t *d_cursor,
-                                        uint64_t *d_flag, void *stream)
+template <bool WIN>
+static int route_scatter(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m, int kmer,
+                         int ethresh, int do_symm, const int16_t *d_dest, const uint64_t *d_tiles, uint64_t *d_send_key,
+                         uint64_t *d_send_lo, uint16_t *d_send_cnt, int64_t n_orig, int64_t n_rc, uint64_t *d_cursor,
+                         uint64_t *d_flag, void *stream, const char *name)
 { if (kmer < 1 || kmer > HM_MAX_KMER || m < 0 || n_orig < 0 || n_rc < 0 || (m > 0 && (kmer > 32) != (d_keys_lo != NULL)) ||
       (n_orig+n_rc > 0 && (kmer > 32) != (d_send_lo != NULL)))
-    return hm_set_error(HM_EINVAL,"hm_k_shard_route_scatter: bad arguments");
+    return hm_set_error(HM_EINVAL,"%s: bad arguments",name);
   if (m == 0)
     return HM_OK;
   cudaStream_t st = (cudaStream_t) stream;
@@ -130,13 +148,59 @@ extern "C" int hm_k_shard_route_scatter(const uint64_t *d_keys, const uint64_t *
   unsigned long long *cur = (unsigned long long *) d_cursor, *flag = (unsigned long long *) d_flag;
   const int hb = hist_bits_of(kmer);
   if (kmer > 32)
-    route_scatter_kernel<2><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,tiles,d_send_key,
-                                                 d_send_lo,d_send_cnt,n_orig,n_rc,cur,flag);
+    route_scatter_kernel<2,WIN><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,tiles,d_send_key,
+                                                     d_send_lo,d_send_cnt,n_orig,n_rc,cur,flag);
   else
-    route_scatter_kernel<1><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,tiles,d_send_key,
-                                                 d_send_lo,d_send_cnt,n_orig,n_rc,cur,flag);
+    route_scatter_kernel<1,WIN><<<grid(m),CT,0,st>>>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,hb,d_dest,tiles,d_send_key,
+                                                     d_send_lo,d_send_cnt,n_orig,n_rc,cur,flag);
   LAUNCHED("route_scatter_kernel");
   return HM_OK;
+}
+
+extern "C" int hm_k_shard_route_count(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t m,
+                                      int kmer, int ethresh, int do_symm, const int16_t *d_dest, int world,
+                                      uint64_t *d_counts, uint64_t *d_tiles, void *stream)
+{ return route_count<false>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,d_dest,world,d_counts,d_tiles,stream,
+                            "hm_k_shard_route_count");
+}
+
+extern "C" int hm_k_shard_route_scatter(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                                        int64_t m, int kmer, int ethresh, int do_symm, const int16_t *d_dest,
+                                        const uint64_t *d_tiles, uint64_t *d_send_key, uint64_t *d_send_lo,
+                                        uint16_t *d_send_cnt, int64_t n_orig, int64_t n_rc, uint64_t *d_cursor,
+                                        uint64_t *d_flag, void *stream)
+{ return route_scatter<false>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,d_dest,d_tiles,d_send_key,d_send_lo,d_send_cnt,
+                              n_orig,n_rc,d_cursor,d_flag,stream,"hm_k_shard_route_scatter");
+}
+
+extern "C" int hm_k_shard_route_count_window(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                                             int64_t m, int kmer, int ethresh, int do_symm, const int16_t *d_dest,
+                                             int world, uint64_t *d_counts, uint64_t *d_tiles, void *stream)
+{ return route_count<true>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,d_dest,world,d_counts,d_tiles,stream,
+                           "hm_k_shard_route_count_window");
+}
+
+extern "C" int hm_k_shard_route_scatter_window(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                                               int64_t m, int kmer, int ethresh, int do_symm, const int16_t *d_dest,
+                                               const uint64_t *d_tiles, uint64_t *d_send_key, uint64_t *d_send_lo,
+                                               uint16_t *d_send_cnt, int64_t n_orig, int64_t n_rc, uint64_t *d_cursor,
+                                               uint64_t *d_flag, void *stream)
+{ return route_scatter<true>(d_keys,d_keys_lo,d_cnt,m,kmer,ethresh,do_symm,d_dest,d_tiles,d_send_key,d_send_lo,d_send_cnt,
+                             n_orig,n_rc,d_cursor,d_flag,stream,"hm_k_shard_route_scatter_window");
+}
+
+extern "C" int hm_k_cond_pack(int kmer, int ibyte, const uint64_t *d_keys, const uint64_t *d_keys_lo,
+                              const uint16_t *d_cnt, int64_t n, int64_t b0, int64_t nb, uint8_t *d_rec,
+                              uint64_t *d_bcount, void *stream)
+{ if (kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || (kmer+3)/4 < ibyte || n < 0 || b0 < 0 || nb < 1 ||
+      b0+nb > (1ll << (8*ibyte)) || d_bcount == NULL || (n > 0 && (d_rec == NULL || (kmer > 32) != (d_keys_lo != NULL))))
+    return hm_set_error(HM_EINVAL,"hm_k_cond_pack: bad arguments");
+  hm_cond_bufs B;
+  memset(&B,0,sizeof(B));
+  B.kmer = kmer; B.ibyte = ibyte;
+  B.key = (uint64_t *) d_keys; B.lo = (uint64_t *) d_keys_lo; B.cnt = (uint16_t *) d_cnt;
+  B.rec = d_rec; B.bcount = (unsigned long long *) d_bcount;
+  return hm_cond_pack(&B,n,(uint64_t) b0,nb,(cudaStream_t) stream);
 }
 
 /* the settle's scratch for t received entries of which c are reverse complements: sort buffers (+ the permutation
@@ -213,4 +277,76 @@ extern "C" int64_t hm_shard_condition_bytes(int kmer, int ibyte, int world, int6
   if (settle > most) most = settle;
   if (gather > most) most = gather;
   return fixed + most;
+}
+
+/* ---- conditioning across the ranks into new table files (dist.condition_ktab, DESIGN.md §4f) ---------------
+ * Memory model of one rank (arrays rounded to 512 bytes as torch's allocator rounds them; 1 MiB for small
+ * tensors).  Resident for the whole call: the unpacked share (E = 10 / 18 bytes per entry at k <= 32 / > 32),
+ * its tile counts, the two histograms, the destination map (int16 per prefix), the route counters and the
+ * stub-bucket counts of one pass.  Beside it, at most one of: the load (the share's records and the stub index
+ * on the device), or one pass -- route: the send buffer; exchange: send + receive; settle (symmetrising): the
+ * received entries, the settled ones and the sort scratch; pack: the settled entries and their records.     */
+
+static int64_t ent1(int64_t t, int two) { return ent(t > 1 ? t : 1,two); }
+
+static int64_t rank_resident(int kmer, int ibyte, int world, int64_t share)
+{ const int64_t np = (int64_t) 1 << hist_bits_of(kmer);
+  return ent(share,kmer > 32) + a512(hm_cond_tiles_bytes(share)) + a512(16*np) + a512(2*np) + a512(8*(2*world+2)) +
+         a512(8*world) + a512(8ll << (8*ibyte)) + (1ll << 20);
+}
+
+static int64_t rank_load(int kmer, int ibyte, int64_t share)
+{ const int64_t pbyte = ((kmer+3)>>2) - ibyte + 2;
+  return a512(pbyte*share) + a512(8ll << (8*ibyte));
+}
+
+static int64_t rank_pass(int kmer, int ibyte, int64_t sent, int64_t received, int64_t rc_received, int do_symm)
+{ const int     two = kmer > 32;
+  const int64_t pbyte = ((kmer+3)>>2) - ibyte + 2;
+  const int64_t route = ent1(sent,two), xchg = ent1(sent,two) + ent1(received,two);
+  const int64_t settle = do_symm ? 2*ent1(received,two) + a512(hm_k_shard_settle_bytes(kmer,received,rc_received)) : 0;
+  const int64_t pack = ent1(received,two) + a512(pbyte*(received > 1 ? received : 1));
+  int64_t most = route;
+  if (xchg > most)   most = xchg;
+  if (settle > most) most = settle;
+  if (pack > most)   most = pack;
+  return most;
+}
+
+extern "C" int64_t hm_rank_condition_bytes(int kmer, int ibyte, int world, int64_t share, int64_t sent,
+                                           int64_t received, int64_t rc_received, int do_symm)
+{ if (kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || world < 1 || share < 0 || sent < 0 || received < 0 ||
+      rc_received < 0 || rc_received > received)
+    return -1;
+  const int64_t load = rank_load(kmer,ibyte,share), pass = rank_pass(kmer,ibyte,sent,received,rc_received,do_symm);
+  return rank_resident(kmer,ibyte,world,share) + (load > pass ? load : pass);
+}
+
+/* a sub-range of t output entries, sized as if the rank sent and received t entries, all reverse complements */
+static int64_t sub_range_bytes(int64_t t, int do_symm, int kmer, int ibyte)
+{ return rank_pass(kmer,ibyte,t,t,do_symm ? t : 0,do_symm); }
+
+extern "C" int hm_rank_condition_cut(int kmer, int ibyte, int world, int64_t share, int do_symm, int64_t budget,
+                                     const int64_t *hist, int64_t np, int64_t *cuts, int64_t *n_sub)
+{ if (kmer < 1 || kmer > HM_MAX_KMER || ibyte < 1 || ibyte > 3 || world < 1 || share < 0 || np < 0 ||
+      (np > 0 && hist == NULL) || cuts == NULL || n_sub == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_condition_cut: bad arguments");
+  *n_sub = 0;
+  const int64_t resident = rank_resident(kmer,ibyte,world,share), load = rank_load(kmer,ibyte,share);
+  const int64_t room = budget - resident;
+  const int64_t limit = room > 0 ? hm_cond_range_limit(room,sub_range_bytes,do_symm,kmer,ibyte) : 0;
+  int64_t cap = 0, big = 0;
+  int r = 0;
+  if (np > 0)
+    r = hm_cond_cut(hist,np,limit,cuts,&cap,&big);
+  else
+    cuts[0] = 0;                                           /* an empty range: no sub-range */
+  if ((np > 0 && r < 1) || load > room)
+    return hm_set_error(HM_ENOMEM,"conditioning into files on a rank with a budget of %lld device bytes: its share of "
+                        "%lld source entries holds %lld bytes resident and %lld more while it loads, and its largest "
+                        "key prefix of %lld output entries needs %lld more in one pass; use more ranks, or "
+                        "condition_kmer_table",(long long) budget,(long long) share,(long long) resident,
+                        (long long) load,(long long) big,(long long) sub_range_bytes(big,do_symm,kmer,ibyte));
+  *n_sub = r;
+  return HM_OK;
 }

@@ -15,6 +15,7 @@ The reference has no multi-process code at all; its only "collective" is that fi
 """
 from __future__ import annotations
 
+import os
 import time
 
 import torch
@@ -468,9 +469,8 @@ class ShardedScan:
         rank, with the sizes.  stats["condition"]: verdicts, steps, entries in / out, entries sent to / received
         from each rank, peak device bytes of the call (torch's allocator; its peak statistics are reset), the
         working set and budget, and ms per phase on this rank."""
-        import numpy as np
         from . import _lib, fastk
-        from .device import DeviceTable, _ptr, _stream
+        from .device import _ptr, _stream
         world, rank = dist.get_world_size(group), dist.get_rank(group)
         dev = torch.device(device if device is not None else "cuda")
         if dev.index is None:
@@ -495,16 +495,7 @@ class ShardedScan:
             two = k > 32
             lo, hi = share_range(n, world, rank)
             m = hi - lo
-            if m:
-                d_rec = torch.from_numpy(_share_records(kt, lo, hi)).to(dev)
-                d_idx = torch.from_numpy(np.ascontiguousarray(kt.index, dtype=np.int64)).to(dev)
-                src = DeviceTable.from_records(k, ibyte, d_rec, d_idx, first=lo)
-                sk, sc, sl = src.keys, src.cnt, src.keys_lo
-                del d_rec, d_idx, src
-            else:
-                sk = torch.empty(0, dtype=torch.int64, device=dev)
-                sc = torch.empty(0, dtype=torch.int16, device=dev)
-                sl = torch.empty(0, dtype=torch.int64, device=dev) if two else None
+            sk, sc, sl = _load_share(kt, lo, hi, dev)
             del kt
             t = done("load", t)
 
@@ -1039,24 +1030,54 @@ def _condition_share(k, ibyte, m, share, ethr, do_symm, budget, group, coll, st,
         raise _lib.HetmersError(-3, f"rank {rank}: conditioning across {world} ranks needs {needs} device bytes per "
                                     f"rank, beyond the budgets {budgets} of ranks {short}")
     t = done("hist_and_plan", t)
+    share = [sk, sc, sl]
+    del sk, sc, sl
+    dest = np.repeat(np.arange(world, dtype=np.int16), np.diff(cuts))
+    out, sent_to, got_from = _route_exchange_settle(k, m, share, ethr, do_symm, torch.from_numpy(dest).to(dev), False,
+                                                    (sent, recv[rank], recv_rc[rank], total_orig, total - total_orig),
+                                                    group, coll, done, t)
+    st.update(sent=sent_to, received=got_from)
+    return out
+
+
+def _route_exchange_settle(k, m, share, ethr, do_symm, dest, window, expect, group, coll, done, t):
+    """One pass of conditioning across the ranks: every kept entry of this rank's source share (share: [keys, counts,
+    second words or None] of m entries) and its reverse complement are routed to the rank owning its key prefix
+    (dest: int16 per prefix; with window, -1 marks a prefix outside this pass), the two regions are all-to-all'ed,
+    and the received entries are settled when symmetrising.  Without window the share list is emptied once routed,
+    so that its entries are freed before the exchange.  expect: (entries sent, received, reverse complements
+    received, and over all ranks kept originals and reverse complements routed) as the histograms count them.
+    done(phase, t): the phases "route", "exchange", "sort_and_merge".
+    -> ((keys, counts, second words or None) of the settled entries, entries sent to each rank, received from each)"""
+    import ctypes as C
+    import numpy as np
+    from . import _lib
+    from .device import _ptr, _stream
+    Lb = _lib.lib()
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    sk, sc, sl = share
+    if not window:
+        share.clear()
+    dev, two = sk.device, k > 32
+    route_count = Lb.hm_k_shard_route_count_window if window else Lb.hm_k_shard_route_count
+    route_scatter = Lb.hm_k_shard_route_scatter_window if window else Lb.hm_k_shard_route_scatter
 
     # route: every kept entry (and its reverse complement) to the rank owning its key prefix
-    dest = torch.from_numpy(np.repeat(np.arange(world, dtype=np.int16), np.diff(cuts))).to(dev)
     counts = torch.zeros(2 * world + 2, dtype=torch.int64, device=dev)
     tiles = torch.empty(m // 256 + 2, dtype=torch.int64, device=dev)
-    _lib.check(Lb.hm_k_shard_route_count(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, int(do_symm), _ptr(dest), world,
-                                         _ptr(counts), _ptr(tiles), _stream()))
+    _lib.check(route_count(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, int(do_symm), _ptr(dest), world, _ptr(counts),
+                           _ptr(tiles), _stream()))
     c = counts.tolist()
     so, sr = c[:world], c[world:2 * world]
     n_o, n_r = sum(so), sum(sr)
-    assert n_o + n_r == sent and c[2 * world] == n_o, (so, sr, sent, c[2 * world])
+    assert n_o + n_r == expect[0] and c[2 * world] == n_o, (so, sr, expect, c[2 * world])
     send_k = torch.empty(max(n_o + n_r, 1), dtype=torch.int64, device=dev)
     send_c = torch.empty(max(n_o + n_r, 1), dtype=torch.int16, device=dev)
     send_l = torch.empty(max(n_o + n_r, 1), dtype=torch.int64, device=dev) if two else None
     cursor = torch.tensor(np.concatenate([[0], np.cumsum(sr)[:-1]]).astype(np.int64), device=dev)
-    _lib.check(Lb.hm_k_shard_route_scatter(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, int(do_symm), _ptr(dest),
-                                           _ptr(tiles), _ptr(send_k), _ptr(send_l), _ptr(send_c), n_o, n_r,
-                                           _ptr(cursor), _ptr(counts[2 * world + 1:]), _stream()))
+    _lib.check(route_scatter(_ptr(sk), _ptr(sl), _ptr(sc), m, k, ethr, int(do_symm), _ptr(dest), _ptr(tiles),
+                             _ptr(send_k), _ptr(send_l), _ptr(send_c), n_o, n_r, _ptr(cursor),
+                             _ptr(counts[2 * world + 1:]), _stream()))
     del sk, sc, sl, tiles, dest, cursor
     flag = counts[2 * world + 1:].to(coll)
     dist.all_reduce(flag, op=dist.ReduceOp.MAX, group=group)
@@ -1070,13 +1091,13 @@ def _condition_share(k, ibyte, m, share, ethr, do_symm, budget, group, coll, st,
     dist.all_to_all_single(theirs, mine, group=group)
     ro, rr = theirs[:, 0].tolist(), theirs[:, 1].tolist()
     r_o, r_c = sum(ro), sum(rr)
-    assert r_o + r_c == recv[rank] and r_c == recv_rc[rank], (ro, rr, recv[rank], recv_rc[rank])
+    assert r_o + r_c == expect[1] and r_c == expect[2], (ro, rr, expect)
     room = max(r_o + r_c, 1)
     rk = torch.empty(room, dtype=torch.int64, device=dev)
     rc = torch.empty(room, dtype=torch.int16, device=dev)
     rl = torch.empty(room, dtype=torch.int64, device=dev) if two else None
-    for (a, b, c0, c1, ins, outs, job_total) in ((0, r_o, 0, n_o, so, ro, total_orig),
-                                                 (r_o, r_o + r_c, n_o, n_o + n_r, sr, rr, total - total_orig)):
+    for (a, b, c0, c1, ins, outs, job_total) in ((0, r_o, 0, n_o, so, ro, expect[3]),
+                                                 (r_o, r_o + r_c, n_o, n_o + n_r, sr, rr, expect[4])):
         if job_total == 0:
             continue
         _all_to_all(rk[a:b], send_k[c0:c1], outs, ins, group)
@@ -1086,9 +1107,9 @@ def _condition_share(k, ibyte, m, share, ethr, do_symm, budget, group, coll, st,
                     [2 * x for x in ins], group)
     del send_k, send_c, send_l
     t = done("exchange", t)
-    st.update(sent=[a + b for a, b in zip(so, sr)], received=[a + b for a, b in zip(ro, rr)])
+    sent_to, got_from = [a + b for a, b in zip(so, sr)], [a + b for a, b in zip(ro, rr)]
     if not do_symm:                                            # the originals arrive sorted: nothing to settle
-        return rk[:r_o], rc[:r_o], rl[:r_o] if two else None
+        return (rk[:r_o], rc[:r_o], rl[:r_o] if two else None), sent_to, got_from
 
     # settle: sort the received reverse complements, merge them with the originals
     ok, oc = torch.empty(room, dtype=torch.int64, device=dev), torch.empty(room, dtype=torch.int16, device=dev)
@@ -1100,7 +1121,372 @@ def _condition_share(k, ibyte, m, share, ethr, do_symm, budget, group, coll, st,
     del rk, rc, rl, scratch
     done("sort_and_merge", t)
     e = n_out.value
-    return ok[:e], oc[:e], ol[:e] if two else None
+    return (ok[:e], oc[:e], ol[:e] if two else None), sent_to, got_from
+
+
+# ---- trimming and symmetrising across the ranks into new table files (condition_ktab, DESIGN.md §4f) --------------
+
+def bucket_condition_cuts(hist, world: int, hb: int, ibyte: int):
+    """condition_cuts on stub-index bucket boundaries, so that every rank's part of the table starts on a bucket
+    (the reference bisects a table on disk by its buckets).  hist: output entries per hb-bit key prefix; a bucket
+    holds the first 8*ibyte bits.  Where buckets are coarser than prefixes (8*ibyte < hb) the cut is made over the
+    histogram summed per bucket and scaled back to prefixes.  -> [0, c_1, ..., c_{world-1}, 2^hb]"""
+    import numpy as np
+    sh = hb - 8 * ibyte
+    if sh <= 0:
+        return condition_cuts(hist, world)
+    h = np.asarray(hist, dtype=np.int64).reshape(-1, 1 << sh).sum(axis=1)
+    return [c << sh for c in condition_cuts(h, world)]
+
+
+def prefix_buckets(p0: int, p1: int, hb: int, ibyte: int):
+    """the stub buckets [b0, b1) that hold the keys of the hb-bit prefixes [p0, p1), p0 < p1"""
+    b = 8 * ibyte
+    if b >= hb:
+        return p0 << (b - hb), p1 << (b - hb)
+    return p0 >> (hb - b), ((p1 - 1) >> (hb - b)) + 1
+
+
+def rank_sub_cuts(kmer: int, ibyte: int, shares, do_symm, budgets, hist, cuts):
+    """every rank's range of key prefixes [cuts[d], cuts[d+1]) cut into the sub-ranges its budget allows beside its
+    resident share (hm_rank_condition_cut; shares[d]: rank d's source entries, budgets[d]: its device bytes, hist:
+    output entries per prefix summed over the ranks) -> per rank [cuts[d], ..., cuts[d+1]], the bounds of its
+    sub-ranges.  HM_ENOMEM naming the rank and the sizes when one prefix, or the load, does not fit."""
+    import ctypes as C
+    import numpy as np
+    from . import _lib
+    Lb = _lib.lib()
+    world = len(shares)
+    h = np.ascontiguousarray(hist, dtype=np.int64)
+    out = []
+    for d in range(world):
+        a, b = int(cuts[d]), int(cuts[d + 1])
+        seg = np.ascontiguousarray(h[a:b])
+        sub = np.zeros(b - a + 1, dtype=np.int64)
+        n_sub = C.c_int64()
+        rc = Lb.hm_rank_condition_cut(kmer, ibyte, world, int(shares[d]), int(do_symm), int(budgets[d]),
+                                      seg.ctypes.data, b - a, sub.ctypes.data, C.byref(n_sub))
+        if rc != 0:
+            raise _lib.HetmersError(rc, f"rank {d}: " + Lb.hm_last_error().decode(errors="replace"))
+        out.append((sub[:n_sub.value + 1] + a).tolist())
+    return out
+
+
+def rank_pass_counts(h_local, h_all, subs, rank: int):
+    """what the histograms say of each pass before any entry moves: pass p routes the p-th sub-range of every rank
+    that has one (subs: rank_sub_cuts).  h_local / h_all: [kept originals, kept originals + reverse complements] per
+    prefix of this rank's share / summed over the ranks.  -> per pass (entries this rank sends, entries it
+    receives, reverse complements among them, kept originals routed by all ranks, reverse complements routed)"""
+    import numpy as np
+
+    def cum(row):
+        return np.concatenate([[0], np.cumsum(np.asarray(row, dtype=np.int64))])
+    s_loc, a_orig, a_all = cum(h_local[1]), cum(h_all[0]), cum(h_all[1])
+    out = []
+    for p in range(max(len(s) - 1 for s in subs)):
+        win = [(s[p], s[p + 1]) for s in subs if p < len(s) - 1]
+        sent = sum(int(s_loc[b] - s_loc[a]) for a, b in win)
+        orig = sum(int(a_orig[b] - a_orig[a]) for a, b in win)
+        every = sum(int(a_all[b] - a_all[a]) for a, b in win)
+        if p < len(subs[rank]) - 1:
+            a, b = subs[rank][p], subs[rank][p + 1]
+            recv, rc = int(a_all[b] - a_all[a]), int((a_all[b] - a_all[a]) - (a_orig[b] - a_orig[a]))
+        else:
+            recv = rc = 0
+        out.append((sent, recv, rc, orig, every - orig))
+    return out
+
+
+def _reduce(vals, coll, group, op=dist.ReduceOp.SUM):
+    """all_reduce of a list of integers -> the reduced list"""
+    x = torch.tensor(vals, dtype=torch.int64, device=coll)
+    dist.all_reduce(x, op=op, group=group)
+    return x.tolist()
+
+
+def _write_atomic(path: str, data: bytes):
+    """write `data` as the file `path`: under a temporary name in its directory, then renamed into place"""
+    import tempfile
+    fd, tmp = tempfile.mkstemp(prefix="." + os.path.basename(path) + ".", suffix=".tmp", dir=os.path.dirname(path))
+    try:
+        with os.fdopen(fd, "wb") as f:
+            f.write(data)
+        os.rename(tmp, path)
+    except BaseException:
+        if os.path.exists(tmp):
+            os.unlink(tmp)
+        raise
+
+
+def condition_ktab(src, dst, L, group=None, device=None, budget=None):
+    """Trim and / or symmetrise the FastK table `src` into the new FastK table `dst` across the ranks of the group,
+    every rank calling this (DESIGN.md §4f).  hetmers' decisions are taken on the whole table as from_ktab(L=...)
+    takes them (job_examine): a table that needs neither step gives None on every rank and nothing is written.
+    Otherwise `dst` holds, entry for entry, what hetmers.condition_table(src, dst, L) writes: the kept entries
+    (count >= L when trimming) and, when symmetrising, their reverse complements with the same count, the original
+    winning over an equal reverse complement; the same kmer and ibyte; minval max(source minval, L) when trimmed.
+
+    Rank d owns one contiguous range of key prefixes, cut on stub-bucket boundaries, and writes its part
+    `.<root>.ktab.<p>`, p counting the ranks with a non-empty output up to d (a rank with none writes no part);
+    rank 0 writes the stub last.  Each rank loads its share of the source once and keeps it on the device while its
+    range is conditioned in passes, a sub-range per pass, sized to `budget` (device bytes per rank; default: free
+    memory minus _lib.BUDGET_RESERVE).  Refused on every rank before anything is written: a `dst` naming `src`
+    (HM_EINVAL), a rank whose share and one pass do not fit its budget (HM_ENOMEM, with the sizes).  A failure to
+    write on any rank raises on every rank and leaves no file under dst's names and no temporary file.  Returns on
+    every rank once the files are in place.  -> stats of this rank: verdicts, steps, entries in / out (the job's
+    and this rank's), passes, the prefix cuts and sub-ranges, entries sent / received per pass, part number and
+    part count, bytes written, peak device bytes (torch's allocator; its peak statistics are reset) against the
+    planned working set and the budget, and ms per phase (per pass: route, exchange, settle, pack)"""
+    import concurrent.futures as cf
+    import struct
+    import tempfile
+    import numpy as np
+    from . import _lib, fastk
+    from .device import _ptr, _stream
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    dev = torch.device(device if device is not None else "cuda")
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    coll = dev if _nccl(group) else torch.device("cpu")
+    Lb = _lib.lib()
+    ethresh = int(L)
+    src, dst = str(src), str(dst)
+    ms = {}
+    lap = _lapper(ms)
+
+    def done(phase, t):                                    # the phase's kernels have finished
+        torch.cuda.synchronize(dev)
+        return lap(phase, t)
+
+    with torch.cuda.device(dev):
+        if budget is None:
+            budget = torch.cuda.mem_get_info(dev)[0] - _lib.BUDGET_RESERVE
+        torch.cuda.reset_peak_memory_stats(dev)
+        base = torch.cuda.memory_allocated(dev)
+        t = time.perf_counter()
+        kt = fastk.read_ktab(src, mmap=True)
+        k, n, ibyte, src_parts = kt.kmer, kt.nels, kt.ibyte, kt.nparts
+        if max(_reduce([int(fastk.same_table_files(src, src_parts, dst))], coll, group, dist.ReduceOp.MAX)):
+            raise _lib.HetmersError(-1, f"rank {rank}: {dst} names the source table: conditioning writes a new table")
+        minval_src = kt.minval
+        lo, hi = share_range(n, world, rank)
+        m = hi - lo
+        share = list(_load_share(kt, lo, hi, dev))
+        del kt
+        t = done("load", t)
+
+        def share_min(a, b):
+            out = torch.full((1,), 0x8000, dtype=torch.int32, device=dev)
+            _lib.check(Lb.hm_k_min_count(_ptr(share[1]), a, b, _ptr(out), _stream()))
+            return int(out.item())
+
+        trimmed, symmetric = job_examine(ethresh, k, n, share[0], share[2], share_min, group, coll)
+        do_trim, do_symm = not trimmed, not symmetric
+        t = lap("examine", t)
+        if not (do_trim or do_symm):
+            share.clear()
+            return None
+        ethr = ethresh if do_trim else 0
+        hb = min(_lib.COND_HIST_BITS, 2 * k)
+
+        # histograms, the rank cuts on buckets, every rank's sub-ranges, and every pass's counts
+        hist = torch.zeros((2, 1 << hb), dtype=torch.int64, device=dev)
+        for row, symm in ((0, 0), (1, do_symm)):
+            _lib.check(Lb.hm_k_cond_hist(_ptr(share[0]), _ptr(share[2]), _ptr(share[1]), m, k, ethr, symm,
+                                         _ptr(hist[row]), _stream()))
+        h_loc = hist.cpu().numpy()
+        _in_place(lambda x: dist.all_reduce(x, group=group), hist, group)
+        h_all = hist.cpu().numpy()
+        del hist
+        cuts = bucket_condition_cuts(h_all[1], world, hb, ibyte)
+        budgets = _reduce([budget if d == rank else 0 for d in range(world)], coll, group)
+        shares = [b - a for a, b in (share_range(n, world, d) for d in range(world))]
+        try:
+            subs = rank_sub_cuts(k, ibyte, shares, do_symm, budgets, h_all[1], cuts)
+        except _lib.HetmersError:
+            share.clear()
+            raise
+        plan = rank_pass_counts(h_loc, h_all, subs, rank)
+        need = max(Lb.hm_rank_condition_bytes(k, ibyte, world, m, *c[:3], int(do_symm)) for c in plan)
+        needs = _reduce([need if d == rank else 0 for d in range(world)], coll, group)
+        short = [d for d in range(world) if needs[d] > budgets[d]]
+        if short:
+            share.clear()
+            raise _lib.HetmersError(-3, f"rank {rank}: conditioning {src} into files across {world} ranks needs "
+                                        f"{needs} device bytes per rank, beyond the budgets {budgets} of ranks {short}; "
+                                        f"use more ranks, or condition_kmer_table")
+        t = done("hist_and_plan", t)
+
+        # the passes: this rank's sub-range p conditioned, packed and appended to its temporary part
+        ddir, root = fastk.split_name(dst)
+        pbyte = ((k + 3) >> 2) - ibyte + 2
+        span = prefix_buckets(cuts[rank], cuts[rank + 1], hb, ibyte) if cuts[rank] < cuts[rank + 1] else (0, 0)
+        bcounts = np.zeros(span[1] - span[0], dtype=np.int64)
+        fd, tmp, err = -1, "", None
+        try:
+            fd, tmp = tempfile.mkstemp(prefix=f".{root}.ktab.", suffix=f".rank{rank}.tmp", dir=ddir)
+        except OSError as x:
+            err = f"{ddir}: {x}"
+        if max(_reduce([int(err is not None)], coll, group, dist.ReduceOp.MAX)):
+            share.clear()
+            if fd >= 0:
+                os.close(fd)
+                os.unlink(tmp)
+            raise _lib.HetmersError(-4, f"rank {rank}: cannot write {dst} on every rank" + (f": {err}" if err else ""))
+        busy = [0.0]
+
+        def append(buf):                                   # the writer thread (os.write releases the GIL)
+            t0 = time.perf_counter()
+            mv = memoryview(buf)
+            while len(mv):
+                mv = mv[os.write(fd, mv):]
+            busy[0] += (time.perf_counter() - t0) * 1e3
+
+        writer = cf.ThreadPoolExecutor(1)
+        pending, n_out, part, nparts, total = None, 0, None, 0, 0
+        st = {"trimmed": trimmed, "symmetric": symmetric,
+              "steps": (["trim"] if do_trim else []) + (["symmetrise"] if do_symm else []),
+              "entries_in": n, "passes": len(plan), "prefix_cuts": cuts, "sub_ranges": subs[rank],
+              "sent": [], "received": [], "budget": budget, "working_set_bytes": need}
+        ms["passes"] = []
+        try:
+            os.write(fd, struct.pack("<iq", k, 0))         # the count is set once every pass is written
+            for p, expect in enumerate(plan):
+                pm = {}
+                ms["passes"].append(pm)
+                plap = _lapper(pm)
+
+                def pdone(phase, t0):
+                    torch.cuda.synchronize(dev)
+                    return plap("settle" if phase == "sort_and_merge" else phase, t0)
+                dest = np.full(1 << hb, -1, dtype=np.int16)
+                for d in range(world):
+                    if p < len(subs[d]) - 1:
+                        dest[subs[d][p]:subs[d][p + 1]] = d
+                (ok, oc, ol), sent_to, got_from = _route_exchange_settle(
+                    k, m, share, ethr, do_symm, torch.from_numpy(dest).to(dev), True, expect, group, coll, pdone,
+                    time.perf_counter())
+                st["sent"].append(sum(sent_to))
+                st["received"].append(sum(got_from))
+                t = time.perf_counter()
+                e = ok.numel()
+                if e:
+                    b0, b1 = prefix_buckets(subs[rank][p], subs[rank][p + 1], hb, ibyte)
+                    rec = torch.empty(e * pbyte, dtype=torch.uint8, device=dev)
+                    bc = torch.empty(b1 - b0, dtype=torch.int64, device=dev)
+                    _lib.check(Lb.hm_k_cond_pack(k, ibyte, _ptr(ok), _ptr(ol), _ptr(oc), e, b0, b1 - b0, _ptr(rec),
+                                                 _ptr(bc), _stream()))
+                    bcounts[b0 - span[0]:b1 - span[0]] += bc.cpu().numpy()
+                    host = rec.cpu().numpy()
+                    del rec, bc
+                    if pending is not None and err is None:    # the last pass's records have been written
+                        try:
+                            pending.result()
+                        except OSError as x:
+                            err = f"{tmp}: {x}"
+                    if err is None:
+                        pending = writer.submit(append, host)
+                    n_out += e
+                del ok, oc, ol
+                pdone("pack", t)
+            share.clear()
+            t = time.perf_counter()
+            if pending is not None and err is None:
+                try:
+                    pending.result()
+                except OSError as x:
+                    err = f"{tmp}: {x}"
+            writer.shutdown(wait=True)
+            if err is None:
+                try:
+                    os.pwrite(fd, struct.pack("<q", n_out), 4)
+                except OSError as x:
+                    err = f"{tmp}: {x}"
+            os.close(fd)
+            fd = -1
+
+            # commit: every rank's part renamed into place once all succeeded, then the stub from rank 0
+            got = _reduce(sum(([n_out, int(err is not None)] if d == rank else [0, 0] for d in range(world)), []),
+                          coll, group)
+            outs, failed = got[0::2], [d for d in range(world) if got[2 * d + 1]]
+            if failed:
+                raise _lib.HetmersError(-4, f"rank {rank}: writing {dst} failed on ranks {failed}"
+                                            + (f": {err}" if err else ""))
+            total = sum(outs)
+            nparts = sum(1 for x in outs if x > 0)
+            old_parts = 0
+            if rank == 0 and os.path.exists(fastk.stub_path(dst)):
+                with open(fastk.stub_path(dst), "rb") as f:
+                    old_parts = max(struct.unpack("<4i", f.read(16))[1], 0)
+            bad = None
+            if n_out > 0:
+                part = sum(1 for x in outs[:rank + 1] if x > 0)
+                try:
+                    os.rename(tmp, fastk.part_path(dst, part))
+                except OSError as x:
+                    bad = f"{fastk.part_path(dst, part)}: {x}"
+            else:
+                os.unlink(tmp)
+            gathered = [None] * world if rank == 0 else None
+            dist.gather_object((span[0], bcounts, bad), gathered, dst=_global(group, 0), group=group)
+            written = 12 + n_out * pbyte if n_out > 0 else 0
+            if rank == 0:
+                bad = bad or next((g[2] for g in gathered if g[2]), None)
+                if bad is None:
+                    try:
+                        if total == 0:                     # what condition_table writes: the source's part count,
+                            nparts = max(src_parts, 1)     # every part empty
+                            for q in range(1, nparts + 1):
+                                _write_atomic(fastk.part_path(dst, q), struct.pack("<iq", k, 0))
+                            written += 12 * nparts
+                        index = np.zeros(1 << (8 * ibyte), dtype=np.int64)
+                        for s0, c, _ in gathered:
+                            index[s0:s0 + len(c)] += c
+                        minval = max(minval_src, ethresh) if do_trim else minval_src
+                        stub = struct.pack("<4i", k, nparts, minval, ibyte) + np.cumsum(index).astype("<i8").tobytes()
+                        _write_atomic(fastk.stub_path(dst), stub)
+                        written += len(stub)
+                    except OSError as x:
+                        bad = f"{fastk.stub_path(dst)}: {x}"
+            if max(_reduce([int(bad is not None)], coll, group, dist.ReduceOp.MAX)):
+                mine = [part] if part is not None else list(range(1, nparts + 1)) if rank == 0 and total == 0 else []
+                for q in mine:
+                    if os.path.exists(fastk.part_path(dst, q)):
+                        os.unlink(fastk.part_path(dst, q))
+                raise _lib.HetmersError(-4, f"rank {rank}: putting {dst} in place failed" + (f": {bad}" if bad else ""))
+            if rank == 0:
+                for q in range(nparts + 1, old_parts + 1):     # parts an older table of this name had beyond ours
+                    if os.path.exists(fastk.part_path(dst, q)):
+                        os.unlink(fastk.part_path(dst, q))
+            lap("commit", t)
+        finally:
+            share.clear()
+            writer.shutdown(wait=True)
+            if fd >= 0:
+                os.close(fd)
+            if os.path.exists(tmp):
+                os.unlink(tmp)
+        ms["writer_busy"] = busy[0]
+        st.update(entries_out=total, rank_entries_out=n_out, part=part, nparts=nparts, bytes_written=written,
+                  peak_bytes=torch.cuda.max_memory_allocated(dev) - base, ms=ms)
+    return st
+
+
+def _global(group, r: int) -> int:
+    return dist.get_global_rank(group, r) if group is not None else r
+
+
+def _load_share(kt, lo: int, hi: int, dev):
+    """ordinals [lo, hi) of a FastK table (fastk.KtabFiles) unpacked on dev -> (keys, counts, second words or None)"""
+    import numpy as np
+    from .device import DeviceTable
+    if hi > lo:
+        d_rec = torch.from_numpy(_share_records(kt, lo, hi)).to(dev)
+        d_idx = torch.from_numpy(np.ascontiguousarray(kt.index, dtype=np.int64)).to(dev)
+        src = DeviceTable.from_records(kt.kmer, kt.ibyte, d_rec, d_idx, first=lo)
+        return src.keys, src.cnt, src.keys_lo
+    return (torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int16, device=dev),
+            torch.empty(0, dtype=torch.int64, device=dev) if kt.kmer > 32 else None)
 
 
 def _share_records(kt, lo: int, hi: int):
