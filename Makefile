@@ -17,7 +17,7 @@ BIN    := $(BINDIR)/hetmers $(BINDIR)/extract_kmer_pairs $(BINDIR)/condition_kme
 
 CU_SRC := smudgeplot_b200/csrc/hm_kernels.cu smudgeplot_b200/csrc/hm_scan.cu smudgeplot_b200/csrc/hm_peer.cu \
           smudgeplot_b200/csrc/hm_condition.cu smudgeplot_b200/csrc/hm_symm.cu \
-          smudgeplot_b200/csrc/hm_shard_condition.cu
+          smudgeplot_b200/csrc/hm_shard_condition.cu smudgeplot_b200/csrc/hm_pairs.cu
 CU_OBJ := $(patsubst smudgeplot_b200/csrc/%.cu,$(OBJDIR)/%.o,$(CU_SRC))
 C_OBJ  := $(OBJDIR)/fastk_table.o
 HDRS   := include/hetmers_b200.h smudgeplot_b200/csrc/hm_internal.h smudgeplot_b200/csrc/hm_device.cuh

@@ -421,8 +421,42 @@ int  hm_rank_scan_extract_settle(hm_rank_scan *r);
 /* this rank's records (*records malloc'ed, caller frees), sorted as hm_scan_extract sorts; status: non-zero = do
  * not use them.  Pass 1 stays resident for another extract_prepare.                                         */
 int  hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status);
+/* the same records without the sort (the caller orders them, e.g. on the device: hm_k_pairs_sort) */
+int  hm_rank_scan_extract_records(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status);
 /* sort n records in place into hm_scan_extract's order: (smudge, key, position, alternative base) */
 int  hm_sort_pair_records(hm_pair_rec *records, int64_t n);
+
+/* ---- extract_kmer_pairs' pair files across the ranks of a one-process-per-GPU job (csrc/hm_pairs.cu, DESIGN.md
+ * §6b; dist.ShardedScan / StreamedShardedScan.write_pairs).  The caller runs the collectives between the calls:
+ *   pairs_hist over this rank's records (one uint64 per key prefix: the top min(HM_COND_HIST_BITS, 2k) bits of
+ *   key_hi; zeroed by the caller) -> histograms summed over the ranks -> the prefixes cut into windows, window j
+ *   going to pass j / world and rank j % world -> per pass, per staged chunk of records: d_dest (int16 per prefix:
+ *   the rank owning it in this pass, -1 outside the pass) -> route_count -> route_scatter -> all-to-all -> on the
+ *   owner: sort -> label_bounds -> format -> the text written at the offsets the line counts give.
+ * d_counts / d_cursor: uint64[world] (world <= 64); route_count adds the records bound for each rank, route_scatter
+ * places them from d_cursor[d] (preset to the start of rank d's segment, advanced here; any order inside a
+ * segment) and sets *d_flag (zeroed by the caller) when a slot lies at or beyond cap.                        */
+int hm_k_pairs_hist(const hm_pair_rec *d_rec, int64_t n, int kmer, uint64_t *d_hist, void *stream);
+int hm_k_pairs_route_count(const hm_pair_rec *d_rec, int64_t n, int kmer, const int16_t *d_dest, int world,
+                           uint64_t *d_counts, void *stream);
+int hm_k_pairs_route_scatter(const hm_pair_rec *d_rec, int64_t n, int kmer, const int16_t *d_dest, int world,
+                             uint64_t *d_cursor, hm_pair_rec *d_send, int64_t cap, uint64_t *d_flag, void *stream);
+/* n records into hm_sort_pair_records' order through the double buffer (d_rec, d_alt); *in_alt: the result is in
+ * d_alt.  Scratch: hm_pairs_sort_scratch_bytes(n) (a size query on the current device; 0 and the error set on
+ * failure), HM_ENOMEM if less is given.                                                                       */
+int64_t hm_pairs_sort_scratch_bytes(int64_t n);
+int hm_k_pairs_sort(hm_pair_rec *d_rec, hm_pair_rec *d_alt, int64_t n, void *d_scratch, int64_t scratch_bytes,
+                    int *in_alt, void *stream);
+/* sorted records -> d_bounds[2s], d_bounds[2s+1] = first and one-past-last record of smudge s, for s <= n_labels
+ * (uint64[2 (n_labels + 1)], zeroed by the caller)                                                            */
+int hm_k_pairs_label_bounds(const hm_pair_rec *d_sorted, int64_t n, int n_labels, uint64_t *d_bounds, void *stream);
+/* sorted records -> their print_het lines, k + 5 bytes each, at d_text (n (k + 5) bytes)                      */
+int hm_k_pairs_format(const hm_pair_rec *d_sorted, int64_t n, int kmer, char *d_text, void *stream);
+/* the most device bytes the file phase holds for a window of `records` records (arrays rounded to 512 bytes): the
+ * histogram and destination map, 2 MiB of small arrays, and the largest of route (the window's records, a staged
+ * chunk of records / 2 and its send buffer), sort (records twice, and 8 bytes per record + 1 MiB allowed for the
+ * sort's scratch) and format (the sorted records and their text); -1 on bad arguments                          */
+int64_t hm_pairs_bytes(int kmer, int64_t records);
 
 /* ---- conditioning to table files, for tables of any size (csrc/hm_condition.cu, DESIGN.md §4d) ----
  * hm_scan_condition_files writes what hm_scan_condition + hm_scan_download would give -- the source's entries

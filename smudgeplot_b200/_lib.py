@@ -38,6 +38,8 @@ ABI_SYMBOLS = [
     "hm_k_shard_settle", "hm_shard_condition_bytes",
     "hm_k_shard_route_count_window", "hm_k_shard_route_scatter_window", "hm_k_cond_pack", "hm_rank_condition_bytes",
     "hm_rank_condition_cut",
+    "hm_rank_scan_extract_records", "hm_k_pairs_hist", "hm_k_pairs_route_count", "hm_k_pairs_route_scatter",
+    "hm_pairs_sort_scratch_bytes", "hm_k_pairs_sort", "hm_k_pairs_label_bounds", "hm_k_pairs_format", "hm_pairs_bytes",
 ]
 
 
@@ -242,6 +244,17 @@ def lib():
     L.hm_rank_condition_bytes.argtypes = [i32, i32, i32, i64, i64, i64, i64, i32]
     L.hm_rank_condition_bytes.restype = i64
     L.hm_rank_condition_cut.argtypes = [i32, i32, i32, i64, i32, i64, vp, i64, vp, C.POINTER(i64)]
+    L.hm_rank_scan_extract_records.argtypes = L.hm_rank_scan_extract_result.argtypes
+    L.hm_k_pairs_hist.argtypes = [vp, i64, i32, vp, vp]
+    L.hm_k_pairs_route_count.argtypes = [vp, i64, i32, vp, i32, vp, vp]
+    L.hm_k_pairs_route_scatter.argtypes = [vp, i64, i32, vp, i32, vp, vp, i64, vp, vp]
+    L.hm_pairs_sort_scratch_bytes.argtypes = [i64]
+    L.hm_pairs_sort_scratch_bytes.restype = i64
+    L.hm_k_pairs_sort.argtypes = [vp, vp, i64, vp, i64, C.POINTER(i32), vp]
+    L.hm_k_pairs_label_bounds.argtypes = [vp, i64, i32, vp, vp]
+    L.hm_k_pairs_format.argtypes = [vp, i64, i32, vp, vp]
+    L.hm_pairs_bytes.argtypes = [i32, i64]
+    L.hm_pairs_bytes.restype = i64
     _lib = L
     return L
 

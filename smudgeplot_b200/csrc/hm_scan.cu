@@ -3007,9 +3007,23 @@ extern "C" int hm_rank_scan_extract_settle(hm_rank_scan *r)
 
 /* after the last round: this rank's records (*records malloc'ed, the caller frees; sorted as hm_scan_extract sorts)
  * and the OR of its status words (non-zero: do not use them).  The listing's buffers are freed.             */
+static int rank_extract_take(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status, int sorted);
+
 extern "C" int hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status)
 { if (r == NULL || r->stage != 5 || records == NULL || n == NULL || status == NULL)
     return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_result: bad arguments");
+  return rank_extract_take(r,records,n,status,1);
+}
+
+/* hm_rank_scan_extract_result's records in the order they were listed (write_pairs sorts them on the device) */
+extern "C" int hm_rank_scan_extract_records(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status)
+{ if (r == NULL || r->stage != 5 || records == NULL || n == NULL || status == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_extract_records: bad arguments");
+  return rank_extract_take(r,records,n,status,0);
+}
+
+static int rank_extract_take(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status, int sorted)
+{
   hm_scan *s = r->s;
   uint64_t nc = 0, st = 0, ns = 0;
   HM_CUDA(cudaSetDevice(s->d[0].dev));
@@ -3018,7 +3032,8 @@ extern "C" int hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **record
     return rc;
   if (r->host == NULL && (r->host = (hm_pair_rec *) malloc(sizeof(hm_pair_rec))) == NULL)
     return hm_set_error(HM_ENOMEM,"out of host memory");
-  sort_records(r->host,r->host_n);
+  if (sorted)
+    sort_records(r->host,r->host_n);
   *records = r->host; *n = r->host_n;
   *status = r->status | st;
   r->host = NULL;

@@ -651,6 +651,17 @@ class ShardedScan:
         when the count exceeds it.  Too little room for one slice is HM_ENOMEM on every rank, before any launch.
         The ranks' records are gathered on dst and sorted there (gather_pairs).
         timings (ms): scan, listing, d2h, gather_and_sort; stats: route, scan_reused, slices, records, ..."""
+        lap = _lapper({} if timings is None else timings)
+        with torch.cuda.device(self.table.device):
+            recs = self._list_pairs(pixmap, lap, budget)
+            t0 = time.perf_counter()
+            res = gather_pairs(recs, dst, self.group)
+            lap("gather_and_sort", t0)
+        return res
+
+    def _list_pairs(self, pixmap, lap, budget):
+        """the listing of extract(): this rank's records (host, in the order listed); self.stats as extract() sets it.
+        lap: the phases scan (when run), listing, d2h"""
         import numpy as np
         from . import _lib
         from .hetmers import PAIR_DTYPE
@@ -658,7 +669,6 @@ class ShardedScan:
         pm = np.ascontiguousarray(pixmap, dtype=np.uint16).reshape(-1)
         if pm.size != _lib.PLOT_CELLS:
             raise ValueError(f"pixmap has {pm.size} cells, not {_lib.PLOT_CELLS}")
-        lap = _lapper({} if timings is None else timings)
         item = PAIR_DTYPE.itemsize
         symm = self.path == "symm"
         with torch.cuda.device(dev):
@@ -723,9 +733,22 @@ class ShardedScan:
             self.stats = {"route": self.path, "scan_reused": reused, "slices": len(ranges), "records": len(recs),
                           "buffer_records": cap, "budget": budget, "range": [t.lo, t.hi],
                           **{key: v for key, v in self.stats.items() if key == "condition"}}
-            res = gather_pairs(recs, dst, g)
-            lap("gather_and_sort", t0)
-        return res
+        return recs
+
+    def write_pairs(self, sma, out, timings: dict | None = None, budget: int | None = None):
+        """extract_kmer_pairs' output files for the smudges of `sma` (hetmers.read_sma): `<out>.<a>A<b>B.txt` per label,
+        byte for byte what `extract_kmer_pairs -o<out> <table> <sma>` writes; every rank calls this.  The pairs are
+        listed as extract() lists them (the same scan reuse, routes, refusals and stats), then the file phase
+        (write_pair_files, DESIGN.md §6b) routes each record to the rank owning its key window, which sorts and formats
+        them on its GPU and writes its segment of every file.  budget: device bytes per rank for the listing and for
+        the file phase (default: free device memory minus _lib.BUDGET_RESERVE at each).  -> the file phase's stats,
+        on every rank; timings (ms): the listing's phases, then hist_and_plan, route, all_to_all, sort, format,
+        text_d2h, write"""
+        pix, labels = read_sma_on_ranks(sma, self.group, self._coll_dev)
+        lap = _lapper({} if timings is None else timings)
+        with torch.cuda.device(self.table.device):
+            recs = self._list_pairs(pix, lap, budget)
+            return write_pair_files(recs, self.kmer, labels, out, self.group, self.table.device, budget, lap)
 
     profile_phases = False
 
@@ -1591,6 +1614,293 @@ def gather_pairs(records, dst: int = 0, group=None):
     return sort_pair_records(np.ascontiguousarray(out))
 
 
+# ---- extract_kmer_pairs' files written by the ranks (write_pairs, DESIGN.md §6b) ---------------------------------
+
+def read_sma_on_ranks(sma, group, coll):
+    """hetmers.read_sma on every rank; a refusal on any rank raises ValueError on every rank -> (pixmap, labels)"""
+    from .hetmers import read_sma
+    err, res = None, None
+    try:
+        res = read_sma(sma)
+    except ValueError as e:
+        err = str(e)
+    if dist.get_world_size(group) > 1 and max(_reduce([int(err is not None)], coll, group, dist.ReduceOp.MAX)):
+        raise ValueError(err or f"rank {dist.get_rank(group)}: the smudge file {sma} was refused on another rank")
+    if err is not None:
+        raise ValueError(err)
+    return res
+
+
+def label_paths(out, labels):
+    """the output file of every label (a, b): <out>.<a>A<b>B.txt, as extract_kmer_pairs names them"""
+    return [f"{out}.{a}A{b}B.txt" for a, b in labels]
+
+
+def pairs_room(kmer: int, budget: int) -> int:
+    """the most records one window may hold under `budget` (hm_pairs_bytes); -1 if not even the fixed part fits"""
+    from . import _lib
+    f = _lib.lib().hm_pairs_bytes
+    if f(kmer, 0) > budget:
+        return -1
+    lo, hi = 0, max(budget // 24, 1)
+    while lo < hi:                                             # the largest r with f(r) <= budget
+        mid = (lo + hi + 1) // 2
+        if f(kmer, mid) <= budget:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
+
+
+def pair_windows(hist, world: int, room: int):
+    """The file phase's plan: the fewest passes P such that the key prefixes, cut into P*world windows of near-equal
+    record counts (condition_cuts), leave every window within `room` records; window j goes to pass j // world and
+    rank j % world.  hist: the records per key prefix, summed over the ranks.  -> (P, cuts [0, ..., len(hist)] of
+    P*world + 1 bounds).  A prefix alone above the room is HM_ENOMEM, with the sizes."""
+    import numpy as np
+    from . import _lib
+    h = np.asarray(hist, dtype=np.int64)
+    big = int(h.max()) if h.size else 0
+    if big > room:
+        p = int(np.argmax(h))
+        raise _lib.HetmersError(-3, f"writing the pair files: key prefix {p} holds {big} records, beyond the {room} "
+                                    f"records one window has room for under the smallest budget of the ranks")
+    before = np.concatenate([[0], np.cumsum(h)])
+    total = int(before[-1])
+    P = max(1, -(-total // (max(room, 1) * world)))
+    while True:                                                # ends: with a window per record every window fits
+        cuts = condition_cuts(h, P * world)
+        if int(np.max(np.diff(before[cuts]))) <= room:
+            return P, cuts
+        P += 1
+
+
+def window_segments(counts, rank: int, before, line: int):
+    """This rank's segments of one pass: counts[d][s] = lines of label s in the pass's window of rank d (all ranks;
+    s = 0 unused), before[s] = lines of label s in every earlier pass.  The window's text holds its labels' lines
+    in label order.  -> [(s, offset in the text, bytes, offset in the file of label s)] for its non-empty labels"""
+    import numpy as np
+    c = np.asarray(counts, dtype=np.int64)
+    own = c[rank]
+    at = np.concatenate([[0], np.cumsum(own)])
+    prior = np.asarray(before, dtype=np.int64) + c[:rank].sum(axis=0)
+    return [(s, int(at[s]) * line, int(own[s]) * line, int(prior[s]) * line) for s in range(1, len(own)) if own[s]]
+
+
+class PairFiles:
+    """The label files of one write_pairs call, shared by the ranks: rank 0 creates (truncates) every file, then
+    every rank opens them and pwrites its segments at their offsets.  A failure is kept until the next check(), a
+    collective: then every rank raises, and rank 0 removes the label files."""
+
+    def __init__(self, paths, group, coll):
+        self.paths, self.group, self.coll = list(paths), group, coll
+        self.rank = dist.get_rank(group)
+        self.fds, self.err = [], None
+        if self.rank == 0:
+            for p in self.paths:
+                try:
+                    os.close(os.open(p, os.O_WRONLY | os.O_CREAT | os.O_TRUNC, 0o666))
+                except OSError as x:
+                    self.err = f"{p}: {x}"
+                    break
+        self.check("creating the pair files")                 # (also the barrier after the creation)
+        for p in self.paths:
+            try:
+                self.fds.append(os.open(p, os.O_WRONLY))
+            except OSError as x:
+                self.err = f"{p}: {x}"
+                break
+        self.check("opening the pair files")
+
+    def write(self, s: int, data, offset: int):
+        """label s's (1-based) bytes at `offset` of its file"""
+        if self.err is not None:
+            return
+        mv = memoryview(data)
+        try:
+            while len(mv):
+                n = os.pwrite(self.fds[s - 1], mv, offset)
+                mv, offset = mv[n:], offset + n
+        except OSError as x:
+            self.err = f"{self.paths[s - 1]}: {x}"
+
+    def check(self, what: str):
+        """collective: a failure on any rank so far raises on every rank, rank 0 removing the label files"""
+        bad = _reduce([int(self.err is not None)], self.coll, self.group, dist.ReduceOp.MAX)[0] \
+            if dist.get_world_size(self.group) > 1 else int(self.err is not None)
+        if bad:
+            self.fail()
+            raise OSError(f"rank {self.rank}: {what} failed on some rank" + (f": {self.err}" if self.err else ""))
+
+    def close(self):
+        for fd in self.fds:
+            try:
+                os.close(fd)
+            except OSError as x:
+                self.err = self.err or f"close: {x}"
+        self.fds = []
+
+    def fail(self):
+        """close, and on rank 0 remove every label file (no partial output is left looking complete)"""
+        self.close()
+        if self.rank == 0:
+            for p in self.paths:
+                if os.path.exists(p):
+                    os.unlink(p)
+
+
+def write_pair_files(recs, kmer: int, labels, out, group, dev, budget=None, lap=None):
+    """The file phase of write_pairs: this rank's pair records (host, any order) -> every rank writes its part of
+    `<out>.<a>A<b>B.txt` for every label (a, b) (label s = labels[s - 1]), the files being what extract_kmer_pairs
+    writes.  Every rank calls this (DESIGN.md §6b):
+      histogram   records per key prefix (hm_k_pairs_hist over the staged records), summed over the ranks
+      plan        pair_windows under the smallest room of the ranks (pairs_room of each rank's budget; default: free
+                  device memory minus _lib.BUDGET_RESERVE); a prefix above it is HM_ENOMEM on every rank before any
+                  file is touched
+      per pass    the records staged through the device in chunks of half this rank's room, each chunk's records of
+                  the pass routed (hm_k_pairs_route_count / _scatter) and all-to-all'ed to their window's owner, which
+                  sorts them (hm_k_pairs_sort), counts lines per label, all-gathers the counts, formats the text
+                  (hm_k_pairs_format) and pwrites its segments (window_segments, PairFiles)
+    A failure to write on any rank raises on every rank, and rank 0 removes the label files.  -> stats: records (of
+    the job), passes, windows, room, chunk, lines per label name, peak device bytes of the phase (torch's allocator;
+    its peak statistics are reset), budget"""
+    import ctypes as C
+    import numpy as np
+    from . import _lib
+    from .device import _ptr, _stream
+    from .hetmers import PAIR_DTYPE
+    Lb = _lib.lib()
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    coll = dev if _nccl(group) else torch.device("cpu")
+    lap = lap or _lapper({})
+    recs = np.ascontiguousarray(recs, dtype=PAIR_DTYPE)
+    raw = recs.view(np.uint8)
+    item, line, nl = PAIR_DTYPE.itemsize, kmer + 5, len(labels)
+    hb = min(_lib.COND_HIST_BITS, 2 * kmer)
+
+    def done(phase, t0):                                       # the phase's kernels have finished
+        torch.cuda.synchronize(dev)
+        return lap(phase, t0)
+
+    with torch.cuda.device(dev):
+        if budget is None:
+            budget = torch.cuda.mem_get_info(dev)[0] - _lib.BUDGET_RESERVE
+        torch.cuda.reset_peak_memory_stats(dev)
+        base = torch.cuda.memory_allocated(dev)
+        t = time.perf_counter()
+        own_room = pairs_room(kmer, budget)
+        chunk = max(own_room // 2, 1)
+        n = len(recs)
+        hist = torch.zeros(1 << hb, dtype=torch.int64, device=dev)
+        if own_room >= 0:
+            for a in range(0, n, chunk):
+                d_in = torch.from_numpy(raw[a * item:min(a + chunk, n) * item]).to(dev)
+                _lib.check(Lb.hm_k_pairs_hist(_ptr(d_in), d_in.numel() // item, kmer, _ptr(hist), _stream()))
+                del d_in
+        _in_place(lambda x: dist.all_reduce(x, group=group), hist, group)
+        h = hist.cpu().numpy()
+        del hist
+        room, most = _reduce([own_room, -(-n // chunk)], coll, group, dist.ReduceOp.MIN)[0], \
+            _reduce([-(-n // chunk)], coll, group, dist.ReduceOp.MAX)[0]
+        if room < 0:
+            raise _lib.HetmersError(-3, f"rank {rank}: writing the pair files needs {Lb.hm_pairs_bytes(kmer, 0)} "
+                                        f"device bytes per rank before any record; the smallest budget of the ranks "
+                                        f"is below that (here {budget})")
+        P, cuts = pair_windows(h, world, room)
+        wsize = np.diff(np.concatenate([[0], np.cumsum(h)])[cuts])
+        t = done("hist_and_plan", t)
+
+        files = PairFiles(label_paths(out, labels), group, coll)
+        before = np.zeros(nl + 1, dtype=np.int64)
+        cursor_h = np.zeros(world, dtype=np.int64)
+        try:
+            for p in range(P):
+                dest = np.full(1 << hb, -1, dtype=np.int16)
+                for d in range(world):
+                    dest[cuts[p * world + d]:cuts[p * world + d + 1]] = d
+                d_dest = torch.from_numpy(dest).to(dev)
+                e = int(wsize[p * world + rank])
+                recv = torch.empty(max(e, 1) * item, dtype=torch.uint8, device=dev)
+                flag = torch.zeros(1, dtype=torch.int64, device=dev)
+                at = 0
+                for c in range(most):
+                    a, b = min(c * chunk, n), min((c + 1) * chunk, n)
+                    d_in = torch.from_numpy(raw[a * item:b * item]).to(dev)
+                    counts = torch.zeros(world, dtype=torch.int64, device=dev)
+                    _lib.check(Lb.hm_k_pairs_route_count(_ptr(d_in), b - a, kmer, _ptr(d_dest), world, _ptr(counts),
+                                                         _stream()))
+                    out_c = counts.tolist()
+                    cursor_h[1:] = np.cumsum(out_c)[:-1]
+                    counts.copy_(torch.from_numpy(cursor_h))
+                    ns = sum(out_c)
+                    send = torch.empty(max(ns, 1) * item, dtype=torch.uint8, device=dev)
+                    _lib.check(Lb.hm_k_pairs_route_scatter(_ptr(d_in), b - a, kmer, _ptr(d_dest), world, _ptr(counts),
+                                                           _ptr(send), ns, _ptr(flag), _stream()))
+                    del d_in
+                    t = done("route", t)
+                    sc = torch.tensor(out_c, dtype=torch.int64, device=coll)
+                    rc = torch.empty_like(sc)
+                    dist.all_to_all_single(rc, sc, group=group)
+                    in_c = rc.tolist()
+                    nr = sum(in_c)
+                    over = at + nr > e                             # (cannot happen: the histogram counted them)
+                    tgt = torch.empty(nr * item, dtype=torch.uint8, device=dev) if over else \
+                        recv[at * item:(at + nr) * item]
+                    _all_to_all(tgt, send[:ns * item], [x * item for x in in_c], [x * item for x in out_c], group)
+                    if over:
+                        flag.fill_(1)
+                    else:
+                        at += nr
+                    del tgt
+                    del send
+                    t = done("all_to_all", t)
+                if _reduce([int(at != e or flag.item() != 0)], coll, group, dist.ReduceOp.MAX)[0]:
+                    raise _lib.HetmersError(-2, f"rank {rank}: pass {p} routed {at} records into a window of {e}")
+                del d_dest, flag
+
+                alt = torch.empty_like(recv)
+                scratch = torch.empty(max(Lb.hm_pairs_sort_scratch_bytes(e), 1), dtype=torch.uint8, device=dev)
+                in_alt = C.c_int()
+                _lib.check(Lb.hm_k_pairs_sort(_ptr(recv), _ptr(alt), e, _ptr(scratch), scratch.numel(),
+                                              C.byref(in_alt), _stream()))
+                srt = alt if in_alt.value else recv
+                del scratch, alt, recv
+                bounds = torch.zeros(2 * (nl + 1), dtype=torch.int64, device=dev)
+                _lib.check(Lb.hm_k_pairs_label_bounds(_ptr(srt), e, nl, _ptr(bounds), _stream()))
+                own = (bounds[1::2] - bounds[0::2]).to(coll)
+                del bounds
+                t = done("sort", t)
+                every = torch.zeros((world, nl + 1), dtype=torch.int64, device=coll)
+                every[rank] = own
+                dist.all_reduce(every, group=group)
+                cnt = every.cpu().numpy()
+                short = cnt.sum(axis=1) != wsize[p * world:(p + 1) * world]
+                if short.any():                                    # (the same verdict on every rank)
+                    raise _lib.HetmersError(-2, f"rank {rank}: records of pass {p} on ranks "
+                                                f"{np.flatnonzero(short).tolist()} carry no label of the smudge file")
+                text = torch.empty(max(e * line, 1), dtype=torch.uint8, device=dev)
+                _lib.check(Lb.hm_k_pairs_format(_ptr(srt), e, kmer, _ptr(text), _stream()))
+                del srt
+                t = done("format", t)
+                host = text[:e * line].cpu().numpy()
+                del text
+                t = lap("text_d2h", t)
+                for s, a, nb, off in window_segments(cnt, rank, before, line):
+                    files.write(s, host[a:a + nb], off)
+                before += cnt.sum(axis=0)
+                del host
+                t = lap("write", t)
+            files.close()
+            files.check("writing the pair files")
+        except BaseException:
+            files.fail()
+            raise
+        lines = {f"{a}A{b}B": int(before[s + 1]) for s, (a, b) in enumerate(labels)}
+        return {"records": int(h.sum()), "passes": P, "windows": P * world, "room": room, "chunk": chunk,
+                "chunks": most,
+                "lines": lines, "budget": budget, "peak_bytes": torch.cuda.max_memory_allocated(dev) - base}
+
+
 class StreamedShardedScan:
     """The streamed counterpart of ShardedScan: rank r of the group streams its run-aligned share of the FastK
     table at the path `table` (or the `_lib.HostTable` `table`, whose buffers must outlive the scan) through
@@ -1753,6 +2063,29 @@ class StreamedShardedScan:
         clean pass 1, else runs pass 1 first.  A Bloom hit on a key another rank owns is settled by that rank, as
         in scan(); the records each rank lists are gathered on dst (gather_pairs).  stats["pass1_reused"] tells
         which happened."""
+        lap = self._lap({} if timings is None else timings)
+        recs = self._list_pairs(pixmap, lap, True)
+        t = time.perf_counter()
+        res = gather_pairs(recs, dst, self.group)
+        lap("gather_and_sort", t)
+        return res
+
+    def write_pairs(self, sma, out, timings: dict | None = None, budget: int | None = None):
+        """extract_kmer_pairs' output files for the smudges of `sma`, as ShardedScan.write_pairs writes them; every
+        rank calls this.  The pairs are listed as extract() lists them (the same pass-1 reuse and refusals), but each
+        rank's records are handed over unsorted (hm_rank_scan_extract_records) to the file phase (write_pair_files),
+        which sorts them on the GPUs.  budget: device bytes per rank for the file phase (default: free device memory
+        minus _lib.BUDGET_RESERVE, beside what the streamed scan holds).  -> the file phase's stats, on every rank;
+        timings (ms): the listing's phases, then hist_and_plan, route, all_to_all, sort, format, text_d2h, write"""
+        pix, labels = read_sma_on_ranks(sma, self.group, self._coll_dev)
+        lap = self._lap({} if timings is None else timings)
+        recs = self._list_pairs(pix, lap, False)
+        with torch.cuda.device(self.device):
+            return write_pair_files(recs, self.kmer, labels, out, self.group, self.device, budget, lap)
+
+    def _list_pairs(self, pixmap, lap, sort: bool):
+        """the routed listing of extract(): this rank's records (host; sorted as hm_scan_extract sorts them, or in the
+        order listed) and self.stats; raises on every rank when a status word is dirty on any"""
         import ctypes as C
         import numpy as np
         from . import _lib
@@ -1761,7 +2094,6 @@ class StreamedShardedScan:
         pm = np.ascontiguousarray(pixmap, dtype=np.uint16).reshape(-1)
         if pm.size != _lib.PLOT_CELLS:
             raise ValueError(f"pixmap has {pm.size} cells, not {_lib.PLOT_CELLS}")
-        lap = self._lap({} if timings is None else timings)
         with torch.cuda.device(self.device):
             reuse = self._pass1_done and self.status == 0
             if self.world > 1:                                  # (every rank must take the same branch)
@@ -1779,21 +2111,20 @@ class StreamedShardedScan:
                                                      L.hm_rank_scan_extract_route, L.hm_rank_scan_extract_settle, lap)
             t = time.perf_counter()
             out, n, st = C.POINTER(_lib.PairRec)(), C.c_int64(), C.c_uint64()
-            _lib.check(L.hm_rank_scan_extract_result(h, C.byref(out), C.byref(n), C.byref(st)))
+            take = L.hm_rank_scan_extract_result if sort else L.hm_rank_scan_extract_records
+            _lib.check(take(h, C.byref(out), C.byref(n), C.byref(st)))
             recs = np.empty(n.value, dtype=PAIR_DTYPE)
             if n.value:
                 C.memmove(recs.ctypes.data, out, n.value * PAIR_DTYPE.itemsize)
             _libc_free(out)
-            t = lap("rank_sort", t)
+            lap("rank_sort" if sort else "rank_records", t)
         self.status = int(st.value)
         self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms.value, "candidates": nc.value,
                       "queries_sent_to": sent_to, "pass1_reused": reuse, "records": int(n.value)}
         if not self.symm_ok():
             raise RuntimeError(f"rank {self.rank}: the routed pair listing ended with a non-zero status word on some "
                                f"rank (here {self.status:#x}); its records must not be used")
-        res = gather_pairs(recs, dst, g)
-        lap("gather_and_sort", t)
-        return res
+        return recs
 
     def residency(self):
         """-> (peak device bytes since the last scan began, its chunks, the budget)"""

@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 import shlex
 import subprocess
 import sys
@@ -83,6 +84,62 @@ def run_extract(infile, sma, o="kmerpairs", t=4, verbose=False, tmp=".", gpus=No
     if gpus is not None:
         env["HETMERS_GPUS"] = str(gpus)
     subprocess.run(cmd, check=True, env=env)
+
+
+_WS = "[ \t\n\v\f\r]*"
+_INT = _WS + "([+-]?[0-9]+)"
+_SMA_LINE = re.compile(_INT + _INT + _WS + "[+-]?[0-9]+" + _INT + "A" + _INT)   # sscanf " %d %d %*d %dA%dB"
+
+
+def _fgets_lines(data: bytes, size: int = 1000):
+    """the pieces fgets(line, size, f) returns one by one: up to and including a newline, at most size - 1 bytes"""
+    at = 0
+    while at < len(data):
+        nl = data.find(b"\n", at, at + size - 1)
+        end = nl + 1 if nl >= 0 else min(at + size - 1, len(data))
+        yield data[at:end]
+        at = end
+
+
+def read_sma(path):
+    """<path>[.sma] as extract_kmer_pairs reads it (read_sma / smudge_label in host/hetmers_main.c): the suffix is
+    optional and matched in any case, the header line is skipped, each further line is "covB covA freq <a>A<b>B"
+    (sscanf's " %d %d %*d %dA%dB": leading blanks and trailing text are accepted).  Labels are numbered 1, 2, ... in
+    order of first appearance; a later line for the same pixel wins.  -> (pixmap uint16[SMAX+1, FMAX+1]: pixel
+    (covA+covB, covB) -> label, 0 = none; [(a, b), ...] of labels 1, 2, ...).  The executable's refusals raise
+    ValueError with its message."""
+    s = str(path)
+    root = s[:-4] if len(s) > 4 and s[-4:].lower() == ".sma" else s
+    try:
+        with open(root + ".sma", "rb") as f:
+            data = f.read()
+    except OSError:
+        raise ValueError(f"Could not open smudge file {root}.sma") from None
+    pix = np.zeros((_lib.SMAX + 1, _lib.PLOT_W), dtype=np.uint16)
+    labels = []
+    lines = _fgets_lines(data)
+    next(lines, None)                                   # the header
+    for raw in lines:
+        line = raw.decode("latin-1")
+        m = _SMA_LINE.match(line)
+        if m is None:
+            raise ValueError(f"Cannot parse line '{line}'")
+        covb, cova, a, b = (_c_int(g) for g in m.groups())
+        if a <= 0 or b <= 0 or a < b:
+            raise ValueError(f"{a}A{b}B is not a valid smudge label")
+        if covb < 0 or covb > _lib.FMAX or cova < covb or covb + cova > _lib.SMAX:
+            raise ValueError(f"({covb},{cova}) is not a valid pixel coordinate")
+        if (a, b) not in labels:
+            labels.append((a, b))
+        pix[covb + cova, covb] = labels.index((a, b)) + 1
+    return pix, labels
+
+
+def _c_int(text: str) -> int:
+    """a %d conversion's value as a 32-bit int (glibc saturates what strtol cannot hold, then truncates to int)"""
+    v = max(min(int(text), (1 << 63) - 1), -(1 << 63))
+    v &= 0xFFFFFFFF
+    return v - (1 << 32) if v >= (1 << 31) else v
 
 
 # ------------------------------------------------------------------ in-process (C ABI layer B) --
