@@ -101,12 +101,14 @@ struct SymmView
     unsigned long long pend_cap, q_cap;
   };
 
-/* Bloom slot of key (hi,lo).  The WORD is chosen by the key's last k/2 bases, the two BITS inside it by
+/* Bloom slot of key (hi,lo).  The 64-bit WORD is chosen by the key's last k/2 bases, the three BITS inside it by
  * the bases before them: rc x and rc y of a candidate pair differ at one base of the front part only, so
- * both of pass 2's look-ups for a pair fall into the same word -- one load (when one shard owns both). */
+ * both of pass 2's look-ups for a pair fall into the same word -- one load (when one shard owns both).  At the
+ * filter's ~6 bits per element of S that is 7.1 % false positives per look-up, against 9.1 % for 2 bits in a
+ * 32-bit word, with the same one atomic per insert (DESIGN.md §4a, tools/bloom_layout_model.py).            */
 template <int KW>
 __device__ __forceinline__ void bloom_slot(const SymmView &W, int seg, int kmer, uint64_t hi, uint64_t lo,
-                                           uint32_t *&word, uint32_t &mask)
+                                           uint64_t *&word, uint64_t &mask)
 { const int Pr = kmer >> 1, pup = kmer-Pr;
   uint64_t sfx;                                                /* the last Pr bases, right aligned */
   if (KW == 1)
@@ -121,16 +123,16 @@ __device__ __forceinline__ void bloom_slot(const SymmView &W, int seg, int kmer,
   uint32_t h = ((uint32_t) sfx ^ (uint32_t) (sfx >> 32) * 0x85EBCA6Bu) * 0x9E3779B1u;     /* 32-bit mixing is plenty here */
   uint32_t g = ((uint32_t) pfx ^ (uint32_t) (pfx >> 32) * 0xC2B2AE35u) * 0x27D4EB2Fu;
   h ^= h >> 15;
-  word = W.bloom + (size_t) seg * W.seg_words + __umulhi(h * 0x2C1B3C6Du,W.seg_words);
-  mask = (1u << (g >> 27)) | (1u << ((g >> 22) & 31));
+  word = (uint64_t *) (W.bloom + (size_t) seg * W.seg_words) + __umulhi(h * 0x2C1B3C6Du,W.seg_words >> 1);
+  mask = (1ull << (g >> 26)) | (1ull << ((g >> 20) & 63)) | (1ull << ((g >> 14) & 63));
 }
 
 /* L2 residency: the Bloom segments (tens of MB) are what pass 2 hits at random, the candidate records
  * stream through once                                                                             */
-__device__ __forceinline__ uint32_t ld_keep(const uint32_t *p)
-{ uint32_t v; uint64_t pol;
+__device__ __forceinline__ uint64_t ld_keep(const uint64_t *p)
+{ uint64_t v, pol;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol));
   return v;
 }
 
@@ -252,8 +254,8 @@ extern "C" void hm_symm_seeds(uint64_t seed[2])
 extern "C" int hm_symm_plan(int64_t n, int64_t range, int kmer, int n_seg, hm_symm_layout *out)
 { if (out == NULL || n < 0 || range < 0 || range > n || n_seg < 1 || n_seg > HM_MAX_SHARDS)
     return hm_set_error(HM_EINVAL,"hm_symm_plan: bad arguments");
-  int bits = 1;                                  /* Bloom bits per table entry (S is ~1/6 of the table; two bits set per
-                                                  *   element): 25 MB at 2e8 entries, which the access-policy window
+  int bits = 1;                                  /* Bloom bits per table entry (S is ~1/6 of the table; three bits of one
+                                                  *   64-bit word set per element, bloom_slot): 25 MB at 2e8 entries, which the access-policy window
                                                   *   (bloom_window) can keep in the H100's 50 MB L2.  2 bits (50 MB) halve
                                                   *   the exact checks of pass 2 but no longer fit: on one H100 SXM
                                                   *   (400 W) pass 1 took 2.98 ms with 2 bits against 1.53 ms with 1,
@@ -424,9 +426,9 @@ __device__ __forceinline__ void s_push(const SymmView &W, uint64_t x, uint64_t x
 
 template <int KW, bool SL>
 __device__ __forceinline__ void bloom_insert(const SymmView &W, int kmer, uint64_t x, uint64_t xl)
-{ uint32_t *word, mask;
+{ uint64_t *word, mask;
   bloom_slot<KW>(W,W.self,kmer,x,xl,word,mask);
-  atomicOr(word,mask);
+  atomicOr((unsigned long long *) word,(unsigned long long) mask);
   if (SL)
     s_push<KW>(W,x,xl);
 }
@@ -1705,7 +1707,7 @@ __device__ __forceinline__ void sweep(const uint64_t *__restrict__ keys, const u
   const int64_t first  = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
   for (uint32_t it = 0; first-lane + (int64_t) it*RV_ILP*stride < nc; it++)
     { uint64_t x[RV_ILP], xl[RV_ILP], meta[RV_ILP];
-      uint32_t *wa[RV_ILP], *wb[RV_ILP], ba[RV_ILP], bb[RV_ILP], va[RV_ILP], vb[RV_ILP];
+      uint64_t *wa[RV_ILP], *wb[RV_ILP], ba[RV_ILP], bb[RV_ILP], va[RV_ILP], vb[RV_ILP];
       bool     ok[RV_ILP];
 #pragma unroll
       for (int u = 0; u < RV_ILP; u++)
