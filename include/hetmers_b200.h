@@ -324,6 +324,45 @@ int  hm_scan_is_symmetric(const hm_scan *s);
  * candidates pass through it in slices.  A streamed scan refuses (HM_EUNSUPPORTED).                          */
 #define HM_EXTRACT_MIN_BYTES (2ll*HM_PLOT_CELLS + (1ll << 16))   /* device pixmap + 64 KiB of records */
 int  hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec **out, int64_t *n_out);
+/* ---- extract_kmer_pairs' pair files from an in-core scan on 1..G GPUs (DESIGN.md §6c) ----------------------
+ * hm_scan_write_pairs writes what extract_kmer_pairs writes -- hm_scan_extract's list, one print_het line per
+ * record, label s's lines in the file paths[s-1] -- without the records leaving the GPUs: a histogram sweep
+ * counts the records per key prefix (the top min(HM_COND_HIST_BITS, 2k) bits of key_hi) on every GPU, the
+ * prefixes are cut into windows as dist.pair_windows cuts them for world = G under the smallest room of the GPUs
+ * (window j: pass j / G, GPU j mod G), and per pass every GPU lists its share of each window again from the scan
+ * (into the owner's buffer, peer-copied at the offset the histograms give), the owner sorts, counts lines per
+ * label and formats them, and one writer thread pwrites the text at its offsets.  The route follows
+ * hm_scan_extract's rule.  The room of a GPU is the device budget (hm_set_device_budget, else the scan's) less
+ * what the scan holds, the pixmap and counters, in records of hm_pairs_bytes' sort and format terms.  HM_ENOMEM
+ * with the sizes when that room is below the fixed part or one prefix alone exceeds it: then no file has been
+ * touched and st->planned is 0.  After the plan every label file is created or truncated; on any later failure
+ * all of them are removed.  A streamed scan refuses (HM_EUNSUPPORTED), a scan left invalid by a failed
+ * conditioning too (HM_EINVAL).  st is optional.                                                              */
+typedef struct hm_pairs_stats
+  { int64_t records;                        /* lines written, over every label                                */
+    int64_t passes, windows;
+    int64_t room;                           /* records one window may hold (the smallest room of the GPUs)    */
+    int64_t peak_bytes;                     /* most device bytes held on one GPU beyond the scan's at the start */
+    int64_t budget;                         /* device bytes the call may hold on a GPU beside the scan (least) */
+    int32_t path;                           /* HM_PATH_SYMM or HM_PATH_DIRECT: the route the pairs came from   */
+    int32_t planned;                        /* 1 once the plan fitted: an HM_ENOMEM is then not the plan's     */
+    double  ms_hist;                        /* route, histogram sweep and plan                                */
+    double  ms_list, ms_sort, ms_format;    /* window sweeps (with peer copies); sort + label bounds; format  */
+    double  ms_d2h;                         /* the text to the pinned pieces                                  */
+    double  ms_write;                       /* waiting for the writer thread (a piece, or the last ones)      */
+    double  ms_writer_busy;                 /* the writer thread's pwrite time                                */
+    double  ms_total;
+  } hm_pairs_stats;
+int  hm_scan_write_pairs(hm_scan *s, const uint16_t *pixmap, int n_labels, const char *const *paths,
+                         hm_pairs_stats *st);
+/* the histogram sweep alone, summed over the GPUs: hist (host uint64[2^min(HM_COND_HIST_BITS, 2k)]) = the
+ * records of hm_scan_extract's list per key prefix, as hm_k_pairs_hist would count them                       */
+int  hm_scan_pairs_hist(hm_scan *s, const uint16_t *pixmap, uint64_t *hist);
+/* the plan of the pair files: the fewest passes P such that the prefixes of hist[0..np) cut into P * world
+ * windows of near-equal record counts (cut r of W: the prefix boundary nearest to r/W of the total, the lower
+ * one on a tie) leave every window within `room` records; cuts (NULL: only *passes) receives the P * world + 1
+ * bounds.  HM_ENOMEM when one prefix alone holds more than room.  dist.pair_windows restates it in Python.      */
+int  hm_pair_windows(const int64_t *hist, int64_t np, int world, int64_t room, int64_t *passes, int64_t *cuts);
 /* ---- device budget and the streamed symmetric scan (DESIGN.md §4c) --------------------------------
  * hm_scan_create computes the bytes the in-core scan would allocate per GPU (table arrays, bucket index,
  * plot, fingerprint, hm_symm_plan(...).bytes).  When they exceed the device budget the scan is STREAMED:

@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "hm_rank_condition_cut",
     "hm_rank_scan_extract_records", "hm_k_pairs_hist", "hm_k_pairs_route_count", "hm_k_pairs_route_scatter",
     "hm_pairs_sort_scratch_bytes", "hm_k_pairs_sort", "hm_k_pairs_label_bounds", "hm_k_pairs_format", "hm_pairs_bytes",
+    "hm_scan_write_pairs", "hm_scan_pairs_hist", "hm_pair_windows",
 ]
 
 
@@ -110,6 +111,18 @@ class PairRec(C.Structure):
     """hm_pair_rec: one line of extract_kmer_pairs' output"""
     _fields_ = [("key_hi", C.c_uint64), ("key_lo", C.c_uint64), ("smudge", C.c_uint32),
                 ("pos", C.c_uint8), ("alt", C.c_uint8), ("pad", C.c_uint16)]
+
+
+class PairsStats(C.Structure):
+    """hm_pairs_stats: what hm_scan_write_pairs did"""
+    _fields_ = [("records", C.c_int64), ("passes", C.c_int64), ("windows", C.c_int64), ("room", C.c_int64),
+                ("peak_bytes", C.c_int64), ("budget", C.c_int64), ("path", C.c_int32), ("planned", C.c_int32),
+                ("ms_hist", C.c_double), ("ms_list", C.c_double), ("ms_sort", C.c_double), ("ms_format", C.c_double),
+                ("ms_d2h", C.c_double), ("ms_write", C.c_double), ("ms_writer_busy", C.c_double),
+                ("ms_total", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 class ScanStats(C.Structure):
@@ -255,6 +268,9 @@ def lib():
     L.hm_k_pairs_format.argtypes = [vp, i64, i32, vp, vp]
     L.hm_pairs_bytes.argtypes = [i32, i64]
     L.hm_pairs_bytes.restype = i64
+    L.hm_scan_write_pairs.argtypes = [vp, vp, i32, C.POINTER(C.c_char_p), C.POINTER(PairsStats)]
+    L.hm_scan_pairs_hist.argtypes = [vp, vp, vp]
+    L.hm_pair_windows.argtypes = [vp, i64, i32, i64, i64p, vp]
     _lib = L
     return L
 

@@ -98,6 +98,24 @@ int hm_symm_route_list(int kmer, const hm_route_bufs *B, const uint8_t *d_ans, i
                        const uint16_t *d_pixmap, hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count,
                        void *stream);
 
+/* the pair files' sweeps over one GPU's share of the pairs (hm_scan_write_pairs, DESIGN.md §6c): the records that
+ * hm_k_symm_extract (every candidate of the work area) or hm_k_pass2_extract ([lo, hi)) would list, none of them
+ * stored in full.  d_hist != NULL: histogram sweep, d_hist[top hb bits of key_hi] += 1 per record (hb <= 32;
+ * zeroed by the caller).  Else window sweep: the records with p0 <= prefix < p1 go to d_out, *d_count (zeroed by
+ * the caller) counting all of them, also those beyond cap.                                                      */
+int hm_symm_pairs_sweep(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
+                        const void *d_bucket, int bits, int idx64, int kmer, void *d_work,
+                        const hm_symm_layout *layout, const hm_symm_shards *shards, const uint16_t *d_pixmap,
+                        int hb, unsigned long long *d_hist, uint64_t p0, uint64_t p1, hm_pair_rec *d_out,
+                        int64_t cap, unsigned long long *d_count, void *stream);
+int hm_pass2_pairs_sweep(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                         const uint8_t *d_deg, const void *d_up, int idx64, int64_t lo, int64_t hi,
+                         const uint16_t *d_pixmap, int hb, unsigned long long *d_hist, uint64_t p0, uint64_t p1,
+                         hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count, const hm_shards *shards,
+                         void *stream);
+/* device bytes of one pair-file window of `records` records: hm_pairs_bytes without its route term */
+int64_t hm_pairs_window_bytes(int kmer, int64_t records);
+
 #include <cuda_runtime.h>
 int hm_cuda_fail(cudaError_t e, const char *what);
 /* sort n packed keys (two words for k > 32) in place, in scratch of hm_sort_keys_bytes (hm_condition.cu) */

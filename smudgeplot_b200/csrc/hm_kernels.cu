@@ -953,6 +953,39 @@ extern "C" int hm_k_pass2_plot(const uint16_t *d_cnt, const uint8_t *d_deg, cons
  * (PLOT[x][min] > 0, PloidyList.c:433-447,688-702).  The k-mer printed is the one with the HIGHER
  * count (on a tie the one with the smaller base), annotated with the other one's base at the
  * varying position -- print_het(seq,len,half,alt), PloidyList.c:128-165.                       */
+/* entry i's record, if it has one (an isolated pair whose pixel carries a label) */
+template <typename IdxT>
+__device__ __forceinline__ bool pass2_pair(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+                                           const uint16_t *__restrict__ cnt, const DegView &dv,
+                                           const IdxT *__restrict__ up, int64_t lo, int64_t i,
+                                           const uint16_t *__restrict__ pixmap, hm_pair_rec &r)
+{ if (((const uint8_t *) dv.self)[i] != 1)
+    return false;
+  IdxT j = up[i-lo];
+  if (j == IdxNone<IdxT>::value)
+    return false;
+  const uint8_t *dj = (const uint8_t *) deg_words(dv,(int64_t) j);
+  if ((dj == (const uint8_t *) dv.self ? __ldg(dj+j) : __ldcv(dj+j)) > 1)
+    return false;
+  int ci = cnt[i], cj = __ldg(cnt+j);
+  int s  = ci+cj;
+  int m  = ci < cj ? ci : cj;
+  unsigned pix = pixmap[s*HM_PLOT_W + m];
+  if (pix == 0)
+    return false;
+  uint64_t xh = keys[i], yh = __ldg(keys+j);
+  uint64_t xl = keys_lo ? keys_lo[i] : 0, yl = keys_lo ? __ldg(keys_lo+j) : 0;
+  int pos = (xh != yh) ? (__clzll((long long) (xh ^ yh)) >> 1)
+                       : 32 + (__clzll((long long) (xl ^ yl)) >> 1);
+  int sh  = 62-2*(pos&31);
+  int bi  = (int) (((pos < 32 ? xh : xl) >> sh) & 3);      /* i < j: bi < bj */
+  int bj  = (int) (((pos < 32 ? yh : yl) >> sh) & 3);
+  if (ci < cj) { r.key_hi = yh; r.key_lo = yl; r.alt = (uint8_t) bi; }   /* PloidyList.c:433-439 */
+  else         { r.key_hi = xh; r.key_lo = xl; r.alt = (uint8_t) bj; }   /*              :441-447 */
+  r.smudge = pix; r.pos = (uint8_t) pos; r.pad = 0;
+  return true;
+}
+
 template <typename IdxT>
 __global__ void __launch_bounds__(256)
 pass2_extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
@@ -962,33 +995,48 @@ pass2_extract_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
                      unsigned long long cap, unsigned long long *__restrict__ count)
 { int64_t stride = (int64_t) gridDim.x * blockDim.x;
   for (int64_t i = lo + (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += stride)
-    { if (((const uint8_t *) dv.self)[i] != 1)
+    { hm_pair_rec r;
+      if (!pass2_pair<IdxT>(keys,keys_lo,cnt,dv,up,lo,i,pixmap,r))
         continue;
-      IdxT j = up[i-lo];
-      if (j == IdxNone<IdxT>::value)
-        continue;
-      const uint8_t *dj = (const uint8_t *) deg_words(dv,(int64_t) j);
-      if ((dj == (const uint8_t *) dv.self ? __ldg(dj+j) : __ldcv(dj+j)) > 1)
-        continue;
-      int ci = cnt[i], cj = __ldg(cnt+j);
-      int s  = ci+cj;
-      int m  = ci < cj ? ci : cj;
-      unsigned pix = pixmap[s*HM_PLOT_W + m];
-      if (pix == 0)
-        continue;
-      uint64_t xh = keys[i], yh = __ldg(keys+j);
-      uint64_t xl = keys_lo ? keys_lo[i] : 0, yl = keys_lo ? __ldg(keys_lo+j) : 0;
-      int pos = (xh != yh) ? (__clzll((long long) (xh ^ yh)) >> 1)
-                           : 32 + (__clzll((long long) (xl ^ yl)) >> 1);
-      int sh  = 62-2*(pos&31);
-      int bi  = (int) (((pos < 32 ? xh : xl) >> sh) & 3);      /* i < j: bi < bj */
-      int bj  = (int) (((pos < 32 ? yh : yl) >> sh) & 3);
-      hm_pair_rec r;
-      if (ci < cj) { r.key_hi = yh; r.key_lo = yl; r.alt = (uint8_t) bi; }   /* PloidyList.c:433-439 */
-      else         { r.key_hi = xh; r.key_lo = xl; r.alt = (uint8_t) bj; }   /*              :441-447 */
-      r.smudge = pix; r.pos = (uint8_t) pos; r.pad = 0;
       unsigned long long at = atomicAdd(count,1ull);
       if (at < cap)
+        out[at] = r;
+    }
+}
+
+/* pass2_extract_kernel's records by key prefix (the top hb bits of key_hi), as PrefixSink takes the symmetric
+ * route's: HIST = true adds each to hist[prefix]; HIST = false stores those with p0 <= prefix < p1 into out, one
+ * atomic per warp on the counter, which counts past cap.  The warps stride together so that every lane of a
+ * warp reaches the warp-wide steps.                                                                           */
+template <typename IdxT, bool HIST>
+__global__ void __launch_bounds__(256)
+pass2_pairs_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+                   const uint16_t *__restrict__ cnt, const DegView dv,
+                   const IdxT *__restrict__ up, int64_t lo, int64_t hi,
+                   const uint16_t *__restrict__ pixmap, int hb, unsigned long long *__restrict__ hist,
+                   uint64_t p0, uint64_t p1, hm_pair_rec *__restrict__ out,
+                   unsigned long long cap, unsigned long long *__restrict__ count)
+{ const int      lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1;
+  int64_t stride = (int64_t) gridDim.x * blockDim.x;
+  for (int64_t w = lo + (int64_t) blockIdx.x * blockDim.x + (threadIdx.x & ~31); w < hi; w += stride)
+    { const int64_t i = w + lane;
+      hm_pair_rec   r;
+      const bool    has = i < hi && pass2_pair<IdxT>(keys,keys_lo,cnt,dv,up,lo,i,pixmap,r);
+      const uint64_t f  = has ? r.key_hi >> (64-hb) : 0;
+      if (HIST)
+        { warp_count(hist,has,f);
+          continue;
+        }
+      const bool     in = has && f >= p0 && f < p1;
+      const unsigned b  = __ballot_sync(0xffffffffu,in);
+      if (b == 0)
+        continue;
+      unsigned long long at = 0;
+      if (lane == 0)
+        at = atomicAdd(count,(unsigned long long) __popc(b));
+      at = __shfl_sync(0xffffffffu,at,0) + (unsigned long long) __popc(b & lt);
+      if (in && at < cap)
         out[at] = r;
     }
 }
@@ -1017,6 +1065,42 @@ extern "C" int hm_k_pass2_extract(const uint64_t *d_keys, const uint64_t *d_keys
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"pass2_extract_kernel");
+  return HM_OK;
+}
+
+int hm_pass2_pairs_sweep(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt,
+                         const uint8_t *d_deg, const void *d_up, int idx64, int64_t lo, int64_t hi,
+                         const uint16_t *d_pixmap, int hb, unsigned long long *d_hist, uint64_t p0,
+                         uint64_t p1, hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count,
+                         const hm_shards *shards, void *stream)
+{ if (lo > hi || cap < 0 || hb < 1 || hb > 32 || d_pixmap == NULL ||
+      (d_hist == NULL && (d_count == NULL || (cap > 0 && d_out == NULL))))
+    return hm_set_error(HM_EINVAL,"pass2_pairs_sweep: bad arguments");
+  if (hi == lo)
+    return HM_OK;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
+  int64_t want = (hi-lo+255)/256;
+  int     grid = (int) (want < sms*8 ? want : sms*8);
+  DegView dv   = make_deg_view((uint8_t *) d_deg,lo,hi,shards);
+  cudaStream_t st = (cudaStream_t) stream;
+  const unsigned long long c = (unsigned long long) cap;
+  if (idx64 && d_hist != NULL)
+    pass2_pairs_kernel<uint64_t,true><<<grid,256,0,st>>>
+        (d_keys,d_keys_lo,d_cnt,dv,(const uint64_t *) d_up,lo,hi,d_pixmap,hb,d_hist,p0,p1,d_out,c,d_count);
+  else if (idx64)
+    pass2_pairs_kernel<uint64_t,false><<<grid,256,0,st>>>
+        (d_keys,d_keys_lo,d_cnt,dv,(const uint64_t *) d_up,lo,hi,d_pixmap,hb,d_hist,p0,p1,d_out,c,d_count);
+  else if (d_hist != NULL)
+    pass2_pairs_kernel<uint32_t,true><<<grid,256,0,st>>>
+        (d_keys,d_keys_lo,d_cnt,dv,(const uint32_t *) d_up,lo,hi,d_pixmap,hb,d_hist,p0,p1,d_out,c,d_count);
+  else
+    pass2_pairs_kernel<uint32_t,false><<<grid,256,0,st>>>
+        (d_keys,d_keys_lo,d_cnt,dv,(const uint32_t *) d_up,lo,hi,d_pixmap,hb,d_hist,p0,p1,d_out,c,d_count);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"pass2_pairs_kernel");
   return HM_OK;
 }
 

@@ -15,6 +15,7 @@
  *******************************************************************************************/
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -157,6 +158,79 @@ extern "C" int64_t hm_pairs_bytes(int kmer, int64_t records)
   const int64_t fmt   = rec + a512((int64_t) (kmer+5)*r);
   int64_t m = route > sort ? route : sort;
   return fixed + (m > fmt ? m : fmt);
+}
+
+int64_t hm_pairs_window_bytes(int kmer, int64_t records)
+{ if (kmer < 1 || kmer > HM_MAX_KMER || records < 0)
+    return -1;
+  const int64_t r = records, rec = a512(24*r);
+  const int64_t fixed = a512(8ll << hist_bits_of(kmer)) + a512(2ll << hist_bits_of(kmer)) + (2ll << 20);
+  const int64_t sort  = 2*rec + sort_scratch_model(r);
+  const int64_t fmt   = rec + a512((int64_t) (kmer+5)*r);
+  return fixed + (sort > fmt ? sort : fmt);
+}
+
+/* The plan of the pair files (DESIGN.md §6b, §6c): the key prefixes cut into windows of near-equal record counts
+ * on prefix boundaries -- cut r of W is the boundary nearest to r/W of the total, the lower one on a tie -- with
+ * the fewest passes P such that no window of the P * world holds more than `room` records.  dist.pair_windows
+ * and dist.condition_cuts are the same rule in Python; a CPU test holds the two together.                      */
+static void nearest_cuts(const int64_t *before, int64_t np, int64_t W, int64_t *cuts)
+{ const int64_t total = before[np];
+  cuts[0] = 0;
+  for (int64_t r = 1; r < W; r++)
+    { const int64_t want = (int64_t) (((__int128) total * r) / W);
+      int64_t lo = 0, hi = np;                                  /* the largest p with before[p] <= want */
+      while (lo < hi)
+        { const int64_t m = (lo+hi+1) >> 1;
+          if (before[m] <= want) lo = m; else hi = m-1;
+        }
+      int64_t p = lo;
+      if (p < np && before[p+1] - want < want - before[p])
+        p += 1;
+      cuts[r] = p > cuts[r-1] ? p : cuts[r-1];
+    }
+  cuts[W] = np;
+}
+
+extern "C" int hm_pair_windows(const int64_t *hist, int64_t np, int world, int64_t room, int64_t *passes,
+                               int64_t *cuts)
+{ if (hist == NULL || np < 1 || world < 1 || passes == NULL)
+    return hm_set_error(HM_EINVAL,"hm_pair_windows: bad arguments");
+  int64_t *before = (int64_t *) malloc(sizeof(int64_t)*(size_t) (np+1));
+  if (before == NULL)
+    return hm_set_error(HM_ENOMEM,"out of host memory");
+  int64_t big = 0, at = 0;
+  before[0] = 0;
+  for (int64_t p = 0; p < np; p++)
+    { if (hist[p] > big) { big = hist[p]; at = p; }
+      before[p+1] = before[p] + hist[p];
+    }
+  if (big > room)
+    { free(before);
+      return hm_set_error(HM_ENOMEM,"writing the pair files: key prefix %lld holds %lld records, beyond the %lld "
+                          "records one window has room for",(long long) at,(long long) big,(long long) room);
+    }
+  const int64_t total = before[np], per = (room > 1 ? room : 1) * (int64_t) world;
+  int64_t P = (total + per - 1) / per;
+  if (P < 1) P = 1;
+  int64_t *c = NULL;
+  for (;; P++)                                 /* ends: with a window per record every window fits */
+    { int64_t *c2 = (int64_t *) realloc(c,sizeof(int64_t)*(size_t) (P*world+1));
+      if (c2 == NULL)
+        { free(c); free(before); return hm_set_error(HM_ENOMEM,"out of host memory"); }
+      c = c2;
+      nearest_cuts(before,np,P*world,c);
+      int64_t most = 0;
+      for (int64_t j = 0; j < P*world; j++)
+        if (before[c[j+1]] - before[c[j]] > most) most = before[c[j+1]] - before[c[j]];
+      if (most <= room)
+        break;
+    }
+  *passes = P;
+  if (cuts != NULL)
+    memcpy(cuts,c,sizeof(int64_t)*(size_t) (P*world+1));
+  free(c); free(before);
+  return HM_OK;
 }
 
 extern "C" int hm_k_pairs_sort(hm_pair_rec *d_rec, hm_pair_rec *d_alt, int64_t n, void *d_scratch,

@@ -30,6 +30,7 @@
 #include <unistd.h>
 #include <errno.h>
 #include <sys/stat.h>
+#include <fcntl.h>
 
 #include "hetmers_b200.h"
 #include "hm_internal.h"
@@ -2548,6 +2549,529 @@ extern "C" int hm_scan_extract(hm_scan *s, const uint16_t *pixmap, hm_pair_rec *
   sort_records(host,total);                                       /* deterministic order */
   *out = host; *n_out = total;
   return HM_OK;
+}
+
+/* ------------------------------------------------------------------ pair files (DESIGN.md §6c) ---- */
+
+/* what a pair-file call holds on each GPU: the pixmap, counters (one per window of a pass), the histogram, the
+ * label bounds of a window, and the window buffers a (records) and b (the sort's other buffer and scratch, then
+ * the window's text)                                                                                         */
+typedef struct
+  { uint16_t           *pix;
+    unsigned long long *ctr, *hist, *bounds;
+    hm_pair_rec        *a, *b;
+    int64_t             held0, peak0;
+  } PairBufs;
+
+#define PAIR_SMALL_BYTES (2*(int64_t) HM_PLOT_CELLS + 256)    /* pixmap and counters, beside the window model */
+
+static int pairs_hist_bits(int kmer) { return 2*kmer < HM_COND_HIST_BITS ? 2*kmer : HM_COND_HIST_BITS; }
+
+static void pairs_free(hm_scan *s, PairBufs *B)
+{ for (int g = 0; g < s->ngpu; g++)
+    { DevTable *D = s->d+g;
+      cudaSetDevice(D->dev);
+      dev_free(D,B[g].pix); dev_free(D,B[g].ctr); dev_free(D,B[g].hist); dev_free(D,B[g].bounds);
+      dev_free(D,B[g].a); dev_free(D,B[g].b);
+      B[g].pix = NULL; B[g].ctr = NULL; B[g].hist = NULL; B[g].bounds = NULL; B[g].a = NULL; B[g].b = NULL;
+    }
+}
+
+/* the device budget of the call, per GPU: the explicit one (hm_set_device_budget) or the scan's */
+static int64_t pairs_budget(const hm_scan *s) { return g_budget > 0 ? g_budget : s->budget; }
+
+/* The histogram sweep over each GPU's own candidates (symmetric route) or range (direct route), the route chosen
+ * as hm_scan_extract chooses it: a symmetric run first when the work areas hold no clean one, and the direct route
+ * when that run or the sweep ends with a dirty status word.  Allocates B[g].pix / ctr / hist / bounds (n_labels
+ * + 1 label bounds).  hg: host int64[G][2^hb], each GPU's histogram; *symm_out: the route taken.                */
+static int pairs_histogram(hm_scan *s, const uint16_t *pixmap, int n_labels, PairBufs *B, int64_t *hg,
+                           int *symm_out)
+{ int symm = 0, forced = 0, rc, G = s->ngpu;
+  const int     hb = pairs_hist_bits(s->kmer);
+  const int64_t np = (int64_t) 1 << hb;
+  uint64_t      status = 0;
+  if ((rc = choose_route(s,HM_PATH_AUTO,&symm,&forced)) != HM_OK)
+    return rc;
+  if (symm && !s->symm_ready)
+    { int64_t *tmp = (int64_t *) malloc(sizeof(int64_t)*HM_PLOT_CELLS);
+      if (tmp == NULL)
+        return hm_set_error(HM_ENOMEM,"out of host memory");
+      rc = run_symm(s,tmp,NULL,&status);
+      free(tmp);
+      if (rc != HM_OK)
+        return rc;
+    }
+  cudaError_t e;
+  rc = HM_OK;
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    { DevTable *D = s->d+g;
+      TRY(cudaSetDevice(D->dev));
+      TRY(dev_alloc(D,&B[g].pix,sizeof(uint16_t)*HM_PLOT_CELLS));
+      TRY(dev_alloc(D,&B[g].ctr,256));
+      TRY(dev_alloc(D,&B[g].hist,sizeof(unsigned long long)*np));
+      TRY(dev_alloc(D,&B[g].bounds,sizeof(unsigned long long)*2*(n_labels+1)));
+      TRY(cudaMemcpyAsync(B[g].pix,pixmap,sizeof(uint16_t)*HM_PLOT_CELLS,cudaMemcpyHostToDevice,D->st));
+      TRY(cudaMemsetAsync(B[g].hist,0,sizeof(unsigned long long)*np,D->st));
+    }
+  if (rc != HM_OK)
+    return rc;
+  if (symm && status == 0)
+    { for (int g = 0; g < G && rc == HM_OK; g++)
+        { DevTable *D = s->d+g;
+          TRY(cudaSetDevice(D->dev));
+          if (rc == HM_OK)
+            rc = hm_symm_pairs_sweep(D->keys,D->keys_lo,D->cnt,s->n,D->bucket,s->bits,s->idx64,s->kmer,D->symm_work,
+                                     &D->symm_layout,G > 1 ? &s->ssh[g] : NULL,B[g].pix,hb,B[g].hist,0,0,NULL,0,
+                                     NULL,D->st);
+          s->launches += 1;
+        }
+      for (int g = 0; g < G && rc == HM_OK; g++)
+        { uint64_t st = 0;
+          TRY(cudaSetDevice(s->d[g].dev));
+          if (rc == HM_OK && (rc = hm_symm_status(s->d[g].symm_work,&s->d[g].symm_layout,NULL,&st,s->d[g].st)) == HM_OK)
+            status |= st;
+        }
+      if (rc != HM_OK)
+        return rc;
+    }
+  if (symm && status != 0)
+    { if ((rc = symm_failed(s,forced,status)) != HM_OK)
+        return rc;
+      symm = 0;
+    }
+  if (!symm)
+    { if ((rc = need_direct_results(s)) != HM_OK)
+        return rc;
+      for (int g = 0; g < G && rc == HM_OK; g++)
+        { DevTable *D = s->d+g;
+          TRY(cudaSetDevice(D->dev));
+          TRY(cudaMemsetAsync(B[g].hist,0,sizeof(unsigned long long)*np,D->st));
+          if (rc == HM_OK)
+            rc = hm_pass2_pairs_sweep(D->keys,D->keys_lo,D->cnt,D->deg,D->up,s->idx64,D->lo,D->hi,B[g].pix,hb,
+                                      B[g].hist,0,0,NULL,0,NULL,s->peer_mode ? &s->sh[g] : NULL,D->st);
+          s->launches += (D->hi > D->lo);
+        }
+    }
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    { TRY(cudaSetDevice(s->d[g].dev));
+      TRY(cudaMemcpyAsync(hg+g*np,B[g].hist,sizeof(int64_t)*np,cudaMemcpyDeviceToHost,s->d[g].st));
+      TRY(cudaStreamSynchronize(s->d[g].st));
+    }
+  *symm_out = symm;
+  return rc;
+}
+
+/* the records of one window a pass lists on GPU g, into out (cap records), counted in *ctr */
+static int pairs_window_sweep(hm_scan *s, int symm, int g, const PairBufs *B, uint64_t p0, uint64_t p1,
+                              hm_pair_rec *out, int64_t cap, unsigned long long *ctr)
+{ DevTable *D = s->d+g;
+  const int hb = pairs_hist_bits(s->kmer);
+  s->launches += 1;
+  if (symm)
+    return hm_symm_pairs_sweep(D->keys,D->keys_lo,D->cnt,s->n,D->bucket,s->bits,s->idx64,s->kmer,D->symm_work,
+                               &D->symm_layout,s->ngpu > 1 ? &s->ssh[g] : NULL,B[g].pix,hb,NULL,p0,p1,out,cap,ctr,
+                               D->st);
+  return hm_pass2_pairs_sweep(D->keys,D->keys_lo,D->cnt,D->deg,D->up,s->idx64,D->lo,D->hi,B[g].pix,hb,NULL,p0,p1,
+                              out,cap,ctr,s->peer_mode ? &s->sh[g] : NULL,D->st);
+}
+
+/* The writer thread: the text of a window reaches the host in pieces (two pinned buffers, alternating); each
+ * piece's part of every label segment of its window is pwritten at its offset in the label's file.           */
+typedef struct { int s; int64_t text_off, bytes, file_off; } PairSeg;
+
+typedef struct
+  { pthread_mutex_t mu;
+    pthread_cond_t  cv;
+    const int      *fd;
+    char           *buf[2];
+    int             full[2], quit, err;
+    int64_t         t0[2], n[2];              /* the piece holds text bytes [t0, t0 + n) of its window */
+    PairSeg        *seg[2];
+    int             nseg[2];
+    double          busy_ms;
+  } PairWriter;
+
+static void *pairs_writer_main(void *arg)
+{ PairWriter *W = (PairWriter *) arg;
+  for (int i = 0; ; i ^= 1)
+    { pthread_mutex_lock(&W->mu);
+      while (!W->full[i] && !W->quit)
+        pthread_cond_wait(&W->cv,&W->mu);
+      if (!W->full[i])
+        { pthread_mutex_unlock(&W->mu); return NULL; }
+      pthread_mutex_unlock(&W->mu);
+      const double t = now_ms();
+      for (int k = 0; k < W->nseg[i] && !W->err; k++)
+        { const PairSeg *q = W->seg[i]+k;
+          int64_t a = q->text_off > W->t0[i] ? q->text_off : W->t0[i];
+          int64_t b = q->text_off+q->bytes < W->t0[i]+W->n[i] ? q->text_off+q->bytes : W->t0[i]+W->n[i];
+          while (a < b && !W->err)
+            { ssize_t w = pwrite(W->fd[q->s-1],W->buf[i]+(a-W->t0[i]),(size_t) (b-a),(off_t) (q->file_off+a-q->text_off));
+              if (w < 0 && errno == EINTR) continue;
+              if (w <= 0) { W->err = w < 0 ? errno : EIO; break; }
+              a += w;
+            }
+        }
+      pthread_mutex_lock(&W->mu);
+      W->busy_ms += now_ms()-t;
+      W->full[i] = 0;
+      pthread_cond_broadcast(&W->cv);
+      pthread_mutex_unlock(&W->mu);
+    }
+}
+
+/* waits until piece i is free; the time waited goes to *ms */
+static void pairs_writer_wait(PairWriter *W, int i, double *ms)
+{ const double t = now_ms();
+  pthread_mutex_lock(&W->mu);
+  while (W->full[i])
+    pthread_cond_wait(&W->cv,&W->mu);
+  pthread_mutex_unlock(&W->mu);
+  *ms += now_ms()-t;
+}
+
+static void pairs_remove(int n_labels, const char *const *paths)
+{ for (int s = 0; s < n_labels; s++)
+    unlink(paths[s]);
+}
+
+/* the most records one window may hold in `bytes` (hm_pairs_window_bytes, bisection); -1 below the fixed part */
+static int64_t pairs_room(int kmer, int64_t bytes)
+{ if (hm_pairs_window_bytes(kmer,0) > bytes)
+    return -1;
+  int64_t lo = 0, hi = bytes/24 > 1 ? bytes/24 : 1;
+  while (lo < hi)
+    { const int64_t m = lo + (hi-lo+1)/2;
+      if (hm_pairs_window_bytes(kmer,m) <= bytes) lo = m; else hi = m-1;
+    }
+  return lo;
+}
+
+/* the room of the call on every GPU: the smallest, in records (-1 if some GPU cannot hold the fixed part);
+ * *budget_out: the smallest device bytes the call may hold beside the scan                               */
+static int64_t pairs_min_room(hm_scan *s, const PairBufs *B, int64_t *budget_out)
+{ int64_t room = -2, budget = 0;
+  for (int g = 0; g < s->ngpu; g++)
+    { const DevTable *D = s->d+g;
+      const int64_t own  = B != NULL ? dev_bytes(D,B[g].pix) + dev_bytes(D,B[g].ctr) + dev_bytes(D,B[g].hist) +
+                                       dev_bytes(D,B[g].bounds) : 0;
+      const int64_t left = pairs_budget(s) - (D->held - own);
+      const int64_t r    = pairs_room(s->kmer,left - PAIR_SMALL_BYTES);
+      if (room == -2 || r < room) room = r;
+      if (g == 0 || left < budget) budget = left;
+    }
+  *budget_out = budget;
+  return room;
+}
+
+extern "C" int hm_scan_pairs_hist(hm_scan *s, const uint16_t *pixmap, uint64_t *hist)
+{ if (s == NULL || pixmap == NULL || hist == NULL)
+    return hm_set_error(HM_EINVAL,"hm_scan_pairs_hist: NULL argument");
+  if (s->streamed)
+    return hm_set_error(HM_EUNSUPPORTED,"listing k-mer pairs needs the direct passes' arrays, and this table does not "
+                                        "fit in device memory (budget %lld bytes)",(long long) s->budget);
+  if (s->invalid)
+    return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
+  const int64_t np = (int64_t) 1 << pairs_hist_bits(s->kmer);
+  PairBufs B[HM_MAX_GPUS];
+  memset(B,0,sizeof(B));
+  int64_t *hg = (int64_t *) malloc(sizeof(int64_t)*(size_t) (np*s->ngpu));
+  if (hg == NULL)
+    return hm_set_error(HM_ENOMEM,"out of host memory");
+  int symm = 0, rc = pairs_histogram(s,pixmap,0,B,hg,&symm);
+  pairs_free(s,B);
+  if (rc == HM_OK)
+    for (int64_t p = 0; p < np; p++)
+      { uint64_t t = 0;
+        for (int g = 0; g < s->ngpu; g++) t += (uint64_t) hg[g*np+p];
+        hist[p] = t;
+      }
+  free(hg);
+  return rc;
+}
+
+extern "C" int hm_scan_write_pairs(hm_scan *s, const uint16_t *pixmap, int n_labels, const char *const *paths,
+                                   hm_pairs_stats *st)
+{ hm_pairs_stats S;
+  memset(&S,0,sizeof(S));
+  if (st != NULL) *st = S;
+  if (s == NULL || pixmap == NULL || n_labels < 0 || (n_labels > 0 && paths == NULL))
+    return hm_set_error(HM_EINVAL,"hm_scan_write_pairs: bad arguments");
+  for (int l = 0; l < n_labels; l++)
+    if (paths[l] == NULL)
+      return hm_set_error(HM_EINVAL,"hm_scan_write_pairs: label %d has no path",l+1);
+  if (s->streamed)
+    return hm_set_error(HM_EUNSUPPORTED,"listing k-mer pairs needs the direct passes' arrays, and this table does not "
+                                        "fit in device memory (budget %lld bytes)",(long long) s->budget);
+  if (s->invalid)
+    return hm_set_error(HM_EINVAL,"this scan was left unusable by a failed conditioning");
+  const double  t_all = now_ms();
+  const int     G = s->ngpu, kmer = s->kmer, hb = pairs_hist_bits(kmer);
+  const int64_t np = (int64_t) 1 << hb, line = kmer+5;
+  int64_t       budget = 0, room = pairs_min_room(s,NULL,&budget);
+  if (room < 0)
+    return hm_set_error(HM_ENOMEM,"writing the pair files needs %lld device bytes per GPU before any record beside the "
+                        "scan's own; the device budget of %lld bytes leaves %lld",
+                        (long long) (hm_pairs_window_bytes(kmer,0)+PAIR_SMALL_BYTES),(long long) pairs_budget(s),
+                        (long long) (budget > 0 ? budget : 0));
+
+  PairBufs B[HM_MAX_GPUS];
+  memset(B,0,sizeof(B));
+  for (int g = 0; g < G; g++)
+    { B[g].held0 = s->d[g].held; B[g].peak0 = s->d[g].peak; s->d[g].peak = s->d[g].held; }
+  int64_t *hg = (int64_t *) malloc(sizeof(int64_t)*(size_t) (np*G));
+  int64_t *hsum = (int64_t *) malloc(sizeof(int64_t)*(size_t) np);
+  int64_t *cuts = NULL, *before = (int64_t *) calloc((size_t) n_labels+1,sizeof(int64_t));
+  int64_t *bh = (int64_t *) malloc(sizeof(int64_t)*(size_t) ((np+1)*G));      /* per GPU: records below prefix p */
+  int     *fd = (int *) malloc(sizeof(int)*(size_t) (n_labels > 0 ? n_labels : 1));
+  uint64_t *bounds = (uint64_t *) malloc(sizeof(uint64_t)*2*(size_t) (n_labels+1));
+  PairSeg  *segs = (PairSeg *) malloc(sizeof(PairSeg)*3*(size_t) (n_labels+1));   /* the two pieces', a window's */
+  char     *pin = NULL;
+  int       rc = HM_OK, symm = 0, files = 0, writer = 0;
+  int64_t   P = 0, piece = 0, ra = 0;
+  PairWriter W;
+  pthread_t  th;
+  cudaError_t e;
+  memset(&W,0,sizeof(W));
+  if (hg == NULL || hsum == NULL || before == NULL || bh == NULL || fd == NULL || bounds == NULL || segs == NULL)
+    rc = hm_set_error(HM_ENOMEM,"out of host memory");
+
+  double t = now_ms();
+  if (rc == HM_OK)
+    rc = pairs_histogram(s,pixmap,n_labels,B,hg,&symm);
+  S.path = symm ? HM_PATH_SYMM : HM_PATH_DIRECT;
+  if (rc == HM_OK)
+    { for (int64_t p = 0; p < np; p++)
+        { int64_t c = 0;
+          for (int g = 0; g < G; g++) c += hg[g*np+p];
+          hsum[p] = c;
+        }
+      for (int g = 0; g < G; g++)
+        { bh[g*(np+1)] = 0;
+          for (int64_t p = 0; p < np; p++) bh[g*(np+1)+p+1] = bh[g*(np+1)+p] + hg[g*np+p];
+        }
+      room = pairs_min_room(s,B,&budget);            /* (the direct passes may have been run for the route) */
+      S.room = room; S.budget = budget;
+      if (room < 0)
+        rc = hm_set_error(HM_ENOMEM,"writing the pair files needs %lld device bytes per GPU before any record beside "
+                          "the scan's own; the device budget of %lld bytes leaves %lld",
+                          (long long) (hm_pairs_window_bytes(kmer,0)+PAIR_SMALL_BYTES),(long long) pairs_budget(s),
+                          (long long) (budget > 0 ? budget : 0));
+    }
+  if (rc == HM_OK && (rc = hm_pair_windows(hsum,np,G,room,&P,NULL)) == HM_OK)
+    { if ((cuts = (int64_t *) malloc(sizeof(int64_t)*(size_t) (P*G+1))) == NULL)
+        rc = hm_set_error(HM_ENOMEM,"out of host memory");
+      else
+        rc = hm_pair_windows(hsum,np,G,room,&P,cuts);
+    }
+  S.ms_hist = now_ms()-t;
+  if (rc != HM_OK)                                     /* nothing written: HM_ENOMEM here is the plan's refusal */
+    goto done;
+  S.planned = 1;
+  S.passes = P; S.windows = P*G;
+
+  /* the window buffers, for the largest window (at most room records): a = records, b = the sort's other buffer
+   * and its scratch, then the window's text                                                                  */
+  { int64_t most = 0, text = 0, scratch = 0, rb = 0;
+    for (int64_t j = 0; j < P*G; j++)
+      { int64_t c = 0;
+        for (int64_t p = cuts[j]; p < cuts[j+1]; p++) c += hsum[p];
+        if (c > most) most = c;
+        S.records += c;
+      }
+    scratch = hm_pairs_sort_scratch_bytes(most);
+    text    = most*line;
+    piece   = text < (64ll << 20) ? (text > 0 ? text : 1) : (64ll << 20);
+    ra      = (24*most + 511) & ~511ll;
+    rb      = ra + scratch > text ? ra + scratch : text;
+    for (int g = 0; g < G && rc == HM_OK; g++)
+      { DevTable *D = s->d+g;
+        TRY(cudaSetDevice(D->dev));
+        TRY(dev_alloc(D,&B[g].a,ra > 0 ? ra : 512));
+        TRY(dev_alloc(D,&B[g].b,rb > 0 ? rb : 512));
+      }
+    if (rc == HM_OK)
+      rc = sync_all(s,"pair-file buffers");
+    if (rc == HM_OK && (e = cudaHostAlloc((void **) &pin,(size_t) (2*piece),cudaHostAllocDefault)) != cudaSuccess)
+      rc = hm_cuda_fail(e,"cudaHostAlloc(pair-file pieces)");
+    if (rc != HM_OK)
+      goto done;
+  }
+
+  /* every label file created (or truncated) before pass 0, so that a label with no pair gets an empty file */
+  for (int l = 0; l < n_labels && rc == HM_OK; l++)
+    { fd[l] = open(paths[l],O_WRONLY | O_CREAT | O_TRUNC,0666);
+      if (fd[l] < 0)
+        rc = hm_set_error(HM_EIO,"cannot create the pair file %s: %s",paths[l],strerror(errno));
+      else
+        files = l+1;
+    }
+  if (rc != HM_OK)
+    goto done;
+  pthread_mutex_init(&W.mu,NULL);
+  pthread_cond_init(&W.cv,NULL);
+  W.fd = fd; W.buf[0] = pin; W.buf[1] = pin+piece; W.seg[0] = segs; W.seg[1] = segs+(n_labels+1);
+  if (pthread_create(&th,NULL,pairs_writer_main,&W) != 0)
+    { rc = hm_set_error(HM_EIO,"cannot start the pair-file writer thread");
+      goto done;
+    }
+  writer = 1;
+
+  { int side = 0;
+    for (int64_t p = 0; p < P && rc == HM_OK; p++)
+      { int64_t share[HM_MAX_GPUS][HM_MAX_GPUS], nwin[HM_MAX_GPUS];   /* [owner][lister] */
+        unsigned long long got[HM_MAX_GPUS][HM_MAX_GPUS];
+        t = now_ms();
+        for (int o = 0; o < G; o++)
+          { const int64_t j = p*G + o;
+            nwin[o] = 0;
+            for (int h = 0; h < G; h++)
+              { share[o][h] = bh[h*(np+1)+cuts[j+1]] - bh[h*(np+1)+cuts[j]];
+                nwin[o] += share[o][h];
+              }
+          }
+        /* each GPU lists its share of every window of the pass: its own window's straight into its buffer, the
+         * others' into b and from there to the owner, after the shares of the GPUs before it                    */
+        for (int h = 0; h < G && rc == HM_OK; h++)
+          { DevTable *D = s->d+h;
+            TRY(cudaSetDevice(D->dev));
+            TRY(cudaMemsetAsync(B[h].ctr,0,sizeof(unsigned long long)*G,D->st));
+            for (int o = 0; o < G && rc == HM_OK; o++)
+              { const int64_t j = p*G + o;
+                int64_t off = 0;
+                for (int q = 0; q < h; q++) off += share[o][q];
+                if (share[o][h] == 0)
+                  continue;
+                rc = pairs_window_sweep(s,symm,h,B,(uint64_t) cuts[j],(uint64_t) cuts[j+1],o == h ? B[o].a+off : B[h].b,
+                                        share[o][h],B[h].ctr+o);
+                if (o != h)
+                  TRY(cudaMemcpyPeerAsync(B[o].a+off,s->d[o].dev,B[h].b,D->dev,sizeof(hm_pair_rec)*share[o][h],D->st));
+              }
+            TRY(cudaMemcpyAsync(got[h],B[h].ctr,sizeof(unsigned long long)*G,cudaMemcpyDeviceToHost,D->st));
+          }
+        if (rc == HM_OK)
+          rc = sync_all(s,"pair-file window sweep");
+        for (int h = 0; h < G && rc == HM_OK; h++)
+          { uint64_t stw = 0;
+            if (symm && (rc = hm_symm_status(s->d[h].symm_work,&s->d[h].symm_layout,NULL,&stw,s->d[h].st)) != HM_OK)
+              break;
+            if (stw != 0)
+              rc = hm_set_error(HM_ECUDA,"the symmetric scan failed its own checks while listing the pairs of pass "
+                                "%lld (status %llu)",(long long) p,(unsigned long long) stw);
+            for (int o = 0; o < G && rc == HM_OK; o++)
+              if ((int64_t) got[h][o] != share[o][h])
+                rc = hm_set_error(HM_ECUDA,"window %lld: GPU %d listed %llu records, its histogram %lld",
+                                  (long long) (p*G+o),s->d[h].dev,got[h][o],(long long) share[o][h]);
+          }
+        S.ms_list += now_ms()-t;
+        if (rc != HM_OK)
+          break;
+
+        t = now_ms();
+        for (int o = 0; o < G && rc == HM_OK; o++)
+          { DevTable *D = s->d+o;
+            const int64_t n = nwin[o];
+            int in_alt = 0;
+            TRY(cudaSetDevice(D->dev));
+            if (rc == HM_OK && n > 0)
+              rc = hm_k_pairs_sort(B[o].a,B[o].b,n,(char *) B[o].b + ra,dev_bytes(D,B[o].b)-ra,&in_alt,D->st);
+            if (in_alt)
+              TRY(cudaMemcpyAsync(B[o].a,B[o].b,sizeof(hm_pair_rec)*n,cudaMemcpyDeviceToDevice,D->st));
+            TRY(cudaMemsetAsync(B[o].bounds,0,sizeof(unsigned long long)*2*(n_labels+1),D->st));
+            if (rc == HM_OK)
+              rc = hm_k_pairs_label_bounds(B[o].a,n,n_labels,(uint64_t *) B[o].bounds,D->st);
+            s->launches += (n > 0) ? 2 : 0;
+          }
+        if (rc == HM_OK)
+          rc = sync_all(s,"pair-file sort");
+        S.ms_sort += now_ms()-t;
+        t = now_ms();
+        for (int o = 0; o < G && rc == HM_OK; o++)
+          { TRY(cudaSetDevice(s->d[o].dev));
+            if (rc == HM_OK)
+              rc = hm_k_pairs_format(B[o].a,nwin[o],kmer,(char *) B[o].b,s->d[o].st);
+            s->launches += (nwin[o] > 0);
+          }
+        if (rc == HM_OK)
+          rc = sync_all(s,"pair-file format");
+        S.ms_format += now_ms()-t;
+
+        /* window by window, in file order: the label segments, and the text through the pinned pieces */
+        for (int o = 0; o < G && rc == HM_OK; o++)
+          { DevTable *D = s->d+o;
+            const int64_t n = nwin[o];
+            int           nseg = 0;
+            int64_t       lines = 0;
+            TRY(cudaSetDevice(D->dev));
+            TRY(cudaMemcpy(bounds,B[o].bounds,sizeof(uint64_t)*2*(n_labels+1),cudaMemcpyDeviceToHost));
+            if (rc != HM_OK)
+              break;
+            PairSeg *ws = segs + 2*(n_labels+1);
+            for (int l = 1; l <= n_labels; l++)
+              { const int64_t c = (int64_t) (bounds[2*l+1] - bounds[2*l]);
+                if (c <= 0)
+                  continue;
+                ws[nseg].s = l; ws[nseg].text_off = (int64_t) bounds[2*l]*line; ws[nseg].bytes = c*line;
+                ws[nseg].file_off = before[l]*line;
+                before[l] += c; lines += c; nseg += 1;
+              }
+            if (lines != n)
+              { rc = hm_set_error(HM_EINVAL,"window %lld holds %lld records with a label beyond the %d labels",
+                                  (long long) (p*G+o),(long long) (n-lines),n_labels);
+                break;
+              }
+            for (int64_t t0 = 0; t0 < n*line && rc == HM_OK; t0 += piece)
+              { const int64_t m = n*line - t0 < piece ? n*line - t0 : piece;
+                pairs_writer_wait(&W,side,&S.ms_write);
+                t = now_ms();
+                TRY(cudaMemcpyAsync(W.buf[side],(char *) B[o].b + t0,(size_t) m,cudaMemcpyDeviceToHost,D->st));
+                TRY(cudaStreamSynchronize(D->st));
+                S.ms_d2h += now_ms()-t;
+                if (rc != HM_OK)
+                  break;
+                memcpy(W.seg[side],ws,sizeof(PairSeg)*(size_t) nseg);
+                pthread_mutex_lock(&W.mu);
+                W.t0[side] = t0; W.n[side] = m; W.nseg[side] = nseg; W.full[side] = 1;
+                pthread_cond_broadcast(&W.cv);
+                pthread_mutex_unlock(&W.mu);
+                side ^= 1;
+              }
+          }
+      }
+  }
+
+done:
+  if (writer)
+    { pairs_writer_wait(&W,0,&S.ms_write);
+      pairs_writer_wait(&W,1,&S.ms_write);
+      pthread_mutex_lock(&W.mu);
+      W.quit = 1;
+      pthread_cond_broadcast(&W.cv);
+      pthread_mutex_unlock(&W.mu);
+      pthread_join(th,NULL);
+      S.ms_writer_busy = W.busy_ms;
+      if (rc == HM_OK && W.err != 0)
+        rc = hm_set_error(HM_EIO,"writing the pair files: %s",strerror(W.err));
+    }
+  if (W.fd != NULL)
+    { pthread_mutex_destroy(&W.mu); pthread_cond_destroy(&W.cv); }
+  for (int l = 0; l < files; l++)
+    if (close(fd[l]) != 0 && rc == HM_OK)
+      rc = hm_set_error(HM_EIO,"closing the pair file %s: %s",paths[l],strerror(errno));
+  if (rc != HM_OK && files > 0)                  /* no partial output is left looking complete */
+    pairs_remove(n_labels,paths);
+  if (pin != NULL)
+    cudaFreeHost(pin);
+  pairs_free(s,B);
+  for (int g = 0; g < G; g++)
+    { DevTable *D = s->d+g;
+      if (D->peak - B[g].held0 > S.peak_bytes) S.peak_bytes = D->peak - B[g].held0;
+      if (B[g].peak0 > D->peak) D->peak = B[g].peak0;
+    }
+  free(hg); free(hsum); free(cuts); free(before); free(bh); free(fd); free(bounds); free(segs);
+  S.ms_total = now_ms()-t_all;
+  if (st != NULL) *st = S;
+  return rc;
 }
 
 extern "C" int hm_hetmers_host(const hm_host_table *t, const int *dev, int n_gpus,

@@ -1584,6 +1584,47 @@ __device__ __forceinline__ void count_pair(uint32_t *tile, unsigned long long *_
  * -- a pair of its own that the direct passes find from u.  Each is listed as pass2_extract_kernel lists it: the
  * member with the higher count (the lower one on a tie), the other member's base at the varying position.
  * One atomic per warp on the counter, which counts every record, also those beyond cap.                    */
+/* list_pairs' records one at a time, for PrefixSink: how many a candidate lists, and the candidate's own record
+ * (mirror = false) or its mirror image's (mirror = true).  list_pairs keeps its own inline copy, so that the
+ * listing kernels compile as they did; the pair-file tests compare the two byte for byte.                      */
+template <int KW>
+__device__ __forceinline__ int pair_records(uint64_t meta, unsigned lab, int kmer)
+{ const int p = (int) ((meta >> 32) & 0xff);
+  return lab == 0 ? 0 : (2*p == kmer-1 ? 1 : 2);
+}
+
+template <int KW>
+__device__ __forceinline__ hm_pair_rec pair_record(uint64_t x, uint64_t xl, uint64_t meta, unsigned lab, int kmer,
+                                                   bool mirror)
+{ const int cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
+  const int p  = (int) ((meta >> 32) & 0xff), by = (int) ((meta >> 40) & 3);
+  const int bx = base_at<KW>(x,xl,p);
+  hm_pair_rec r;
+  r.smudge = lab; r.pad = 0;
+  if (!mirror)
+    { r.pos = (uint8_t) p;
+      if (cx < cy)                                         /* y, alt bx */
+        { uint64_t y = x, yl = xl;
+          set_base<KW>(y,yl,p,by);
+          r.key_hi = y; r.key_lo = yl; r.alt = (uint8_t) bx;
+        }
+      else                                                 /* x, alt by */
+        { r.key_hi = x; r.key_lo = xl; r.alt = (uint8_t) by; }
+      return r;
+    }
+  const int q = kmer-1-p;
+  uint64_t  rx, rxl;
+  revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
+  r.pos = (uint8_t) q;
+  if (cy < cx)                                             /* v = rc x, alt = u's base 3-by */
+    { r.key_hi = rx; r.key_lo = rxl; r.alt = (uint8_t) (3-by); }
+  else                                                     /* u = rc y, alt = v's base 3-bx */
+    { set_base<KW>(rx,rxl,q,3-by);
+      r.key_hi = rx; r.key_lo = rxl; r.alt = (uint8_t) (3-bx);
+    }
+  return r;
+}
+
 template <int KW>
 __device__ __forceinline__ void list_pairs(uint64_t x, uint64_t xl, uint64_t meta, unsigned lab, int kmer,
                                            hm_pair_rec *__restrict__ out, unsigned long long cap,
@@ -1678,6 +1719,55 @@ struct ListSink                                  /* extract_kmer_pairs' records:
           lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
         }
       list_pairs<KW>(x,xl,meta,lab,kmer,out,cap,count,lane,(1u << lane) - 1);
+    }
+  };
+
+/* The records ListSink would list, by key prefix (the top hb bits of key_hi, as pairs_hist_kernel bins them):
+ * HIST = true adds each to hist[prefix] (one atomic per distinct prefix of a warp); HIST = false stores only
+ * those with p0 <= prefix < p1 into out, one atomic per warp on the counter, which counts past cap          */
+template <int KW, bool HIST>
+struct PrefixSink
+  { const uint16_t *pixmap;
+    unsigned long long *hist;
+    hm_pair_rec *out;
+    unsigned long long cap, *count;
+    uint64_t p0, p1;
+    int kmer, hb;
+    static constexpr bool NEEDS_KEY = true;
+    static constexpr int  QUEUES = 0;
+    __device__ __forceinline__ void begin() const {}
+    __device__ __forceinline__ void end() const {}
+    __device__ __forceinline__ void take(bool iso, uint64_t x, uint64_t xl, uint64_t meta) const
+    { const int lane = threadIdx.x & 31;
+      unsigned  lab = 0;
+      if (iso)
+        { const int cx = (int) (meta & 0xffff), cy = (int) ((meta >> 16) & 0xffff);
+          lab = __ldg(pixmap + (cx+cy)*HM_PLOT_W + (cx < cy ? cx : cy));
+        }
+      const int   nr = pair_records<KW>(meta,lab,kmer);
+      hm_pair_rec r0, r1;
+      uint64_t    f0 = 0, f1 = 0;
+      if (nr >= 1) { r0 = pair_record<KW>(x,xl,meta,lab,kmer,false); f0 = r0.key_hi >> (64-hb); }
+      if (nr == 2) { r1 = pair_record<KW>(x,xl,meta,lab,kmer,true);  f1 = r1.key_hi >> (64-hb); }
+      if (HIST)
+        { warp_count(hist,nr >= 1,f0);
+          warp_count(hist,nr == 2,f1);
+          return;
+        }
+      const bool     in0 = nr >= 1 && f0 >= p0 && f0 < p1, in1 = nr == 2 && f1 >= p0 && f1 < p1;
+      const unsigned b0 = __ballot_sync(0xffffffffu,in0), b1 = __ballot_sync(0xffffffffu,in1);
+      if ((b0 | b1) == 0)
+        return;
+      const unsigned lt = (1u << lane) - 1;
+      unsigned long long at = 0;
+      if (lane == 0)
+        at = atomicAdd(count,(unsigned long long) (__popc(b0)+__popc(b1)));
+      at = __shfl_sync(0xffffffffu,at,0) + (unsigned long long) (__popc(b0 & lt)+__popc(b1 & lt));
+      if (in0 && at < cap)
+        out[at] = r0;
+      at += in0;
+      if (in1 && at < cap)
+        out[at] = r1;
     }
   };
 
@@ -1924,6 +2014,67 @@ extern "C" int hm_k_symm_extract(const uint64_t *d_keys, const uint64_t *d_keys_
                                                                        d_pixmap,d_out,cap,d_count,st); });
   if (e != cudaSuccess)
     return hm_cuda_fail(e,"extract_kernel");
+  return HM_OK;
+}
+
+/* extract_kernel's sweep with a PrefixSink: the pair files' histogram (HIST) and window sweeps (DESIGN.md §6c).
+ * The window sweep at k <= 32 spills at 64 registers (2 CTAs per SM): it runs 1 CTA per SM, as k > 32 does.  */
+template <typename IdxT, int KW, bool HIST>
+__global__ void __launch_bounds__(EX_THREADS,KW == 1 && HIST ? 2 : 1)
+pairs_sweep_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ keys_lo,
+                   const uint16_t *__restrict__ cnt, int64_t n, const IdxT *__restrict__ bucket, int bshift,
+                   int kmer, const SymmView W, const PrefixSink<KW,HIST> sink)
+{ sweep<IdxT,KW,LK_TABLE>(keys,keys_lo,cnt,n,bucket,bshift,kmer,W,sink); }
+
+template <typename IdxT, int KW, bool HIST>
+static cudaError_t launch_pairs_sweep(const uint64_t *keys, const uint64_t *keys_lo, const uint16_t *cnt, int64_t n,
+                                      const void *bucket, int bits, int kmer, const SymmView &W,
+                                      const PrefixSink<KW,HIST> &sink, cudaStream_t st)
+{ static int per_sm[64] = {0};                                /* per instantiation */
+  size_t smem = (size_t) (EX_THREADS/32)*RV_QCAP*8*(KW+1);
+  int dev = 0, sms = 132, occ = 1;
+  cudaGetDevice(&dev);
+  if (dev >= 64 || per_sm[dev] == 0)
+    { cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ,pairs_sweep_kernel<IdxT,KW,HIST>,EX_THREADS,smem);
+      if (e != cudaSuccess) return e;
+      if (occ < 1) occ = 1;
+      if (dev < 64) per_sm[dev] = occ;
+    }
+  else
+    occ = per_sm[dev];
+  cudaDeviceGetAttribute(&sms,cudaDevAttrMultiProcessorCount,dev);
+  int64_t want = ((int64_t) W.cand_cap+EX_THREADS*RV_ILP-1)/(EX_THREADS*RV_ILP);
+  int     grid = rv_grid(want,(int64_t) sms*occ);
+  pairs_sweep_kernel<IdxT,KW,HIST><<<grid,EX_THREADS,smem,st>>>(keys,keys_lo,cnt,n,(const IdxT *) bucket,64-bits,kmer,
+                                                                W,sink);
+  return cudaGetLastError();
+}
+
+int hm_symm_pairs_sweep(const uint64_t *d_keys, const uint64_t *d_keys_lo, const uint16_t *d_cnt, int64_t n,
+                        const void *d_bucket, int bits, int idx64, int kmer, void *d_work,
+                        const hm_symm_layout *layout, const hm_symm_shards *shards,
+                        const uint16_t *d_pixmap, int hb, unsigned long long *d_hist, uint64_t p0,
+                        uint64_t p1, hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count,
+                        void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || d_work == NULL || layout == NULL || d_pixmap == NULL ||
+      hb < 1 || hb > 2*kmer || hb > 32 || cap < 0 || (d_hist == NULL && (d_count == NULL || (cap > 0 && d_out == NULL))))
+    return hm_set_error(HM_EINVAL,"symm_pairs_sweep: bad arguments");
+  if ((kmer > 32) != (d_keys_lo != NULL))
+    return hm_set_error(HM_EINVAL,"symm_pairs_sweep: second key word array %s for k=%d",
+                        d_keys_lo ? "given" : "missing",kmer);
+  cudaStream_t st = (cudaStream_t) stream;
+  SymmView W = make_view(d_work,layout,shards);
+  cudaError_t e = dispatch(kmer,idx64,[&](auto I)
+    { using IdxT = typename decltype(I)::IdxT;
+      constexpr int KW = decltype(I)::KW;
+      if (d_hist != NULL)
+        { const PrefixSink<KW,true> sink = { d_pixmap, d_hist, NULL, 0, NULL, 0, 0, kmer, hb };
+          return launch_pairs_sweep<IdxT,KW,true>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,sink,st);
+        }
+      const PrefixSink<KW,false> sink = { d_pixmap, NULL, d_out, (unsigned long long) cap, d_count, p0, p1, kmer, hb };
+      return launch_pairs_sweep<IdxT,KW,false>(d_keys,d_keys_lo,d_cnt,n,d_bucket,bits,kmer,W,sink,st); });
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"pairs_sweep_kernel");
   return HM_OK;
 }
 

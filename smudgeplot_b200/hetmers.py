@@ -250,6 +250,36 @@ class Scan:
         libc.free(out)
         return arr
 
+    def pairs_hist(self, pixmap: np.ndarray):
+        """the records of extract()'s list per key prefix (the top min(20, 2k) bits of key_hi), counted by the
+        histogram sweep that write_pairs plans with (hm_scan_pairs_hist) -> uint64[2^min(20, 2k)]"""
+        pm = np.ascontiguousarray(pixmap, dtype=np.uint16).reshape(-1)
+        assert pm.size == _lib.PLOT_CELLS
+        h = np.zeros(1 << min(_lib.COND_HIST_BITS, 2 * self.kt.kmer), dtype=np.uint64)
+        _lib.check(self._L.hm_scan_pairs_hist(self._h, pm.ctypes.data, h.ctypes.data))
+        return h
+
+    def write_pairs(self, sma, out, device_budget: int | None = None):
+        """extract_kmer_pairs' files for the smudges of `sma` (parsed as read_sma parses it): <out>.<a>A<b>B.txt per
+        label, byte for byte what the executable writes, sorted and formatted on the GPUs (hm_scan_write_pairs,
+        DESIGN.md §6c).  device_budget sets the process-wide device budget (bytes per GPU, as Scan's does) for this
+        and later calls.  A plan that does not fit raises HetmersError -3 before any file is touched.
+        -> stats dict: records, passes, windows, room, lines per label name, peak_bytes (device bytes beyond the
+        scan's), budget (device bytes the call may hold beside the scan), path, and the phase times"""
+        pix, labels = read_sma(sma)
+        if device_budget is not None:
+            self._L.hm_set_device_budget(int(device_budget))
+        names = [f"{a}A{b}B" for a, b in labels]
+        paths = [f"{out}.{n}.txt" for n in names]
+        arr = (C.c_char_p * max(len(paths), 1))(*[p.encode() for p in paths])
+        st = _lib.PairsStats()
+        pm = np.ascontiguousarray(pix, dtype=np.uint16).reshape(-1)
+        _lib.check(self._L.hm_scan_write_pairs(self._h, pm.ctypes.data, len(paths), arr, C.byref(st)))
+        d = st.as_dict()
+        line = self.kt.kmer + 5
+        d["lines"] = {n: os.path.getsize(p) // line for n, p in zip(names, paths)}
+        return d
+
     def download(self, deg: bool = True):
         n = getattr(self, "nels", self.kt.nels)
         keys = np.empty(n, dtype=np.uint64)

@@ -40,7 +40,7 @@ static const char *Usage[] = { " [-v] [-T<int(4)>] [-P<dir(/tmp)>]",
                                " [-o<output>] [-e<int(4)>] <source>[.ktab] <smudges>[.sma]" };
 #define NPOSITIONAL 3
 
-typedef struct { int a, b; FILE *f; } Smudge;
+typedef struct { int a, b; FILE *f; char *name; } Smudge;
 #else
 static const char *Prog_Name = "hetmers";
 
@@ -118,7 +118,7 @@ static int smudge_label(SmudgeSet *set, int a, int b, const char *out_root)
     set->v[s].a = a;
     set->v[s].b = b;
     set->v[s].f = fopen(name,"w");                  /* created even if no pair ends up in it */
-    free(name);
+    set->v[s].name = name;
   }
   if (set->v[s].f == NULL)
     { fprintf(stderr,"%s: Cannot open smudge file %s.%dA%dB.txt\n",Prog_Name,out_root,a,b);
@@ -480,11 +480,39 @@ int main(int argc, char *argv[])
     die_hm();
   t_scan = wall_ms();
 #ifdef EXTRACT_PAIRS
-  hm_pair_rec *REC = NULL;
-  int64_t      NREC = 0;
-  int          KMER = hm_table_view(T)->kmer;
-  if (hm_scan_extract(S,PIXMAP,&REC,&NREC) != HM_OK)
-    die_hm();
+  //  The pair files are sorted and formatted on the GPUs and written by hm_scan_write_pairs.  Only when its plan
+  //  does not fit the device budget (HM_ENOMEM before any file is touched) is the list brought to the host
+  //  (hm_scan_extract) and written here line by line.
+  hm_pair_rec   *REC = NULL;
+  int64_t        NREC = 0;
+  int            KMER = hm_table_view(T)->kmer, HOST_WRITER = 0;
+  hm_pairs_stats PST;
+  double         t_pairs = wall_ms();
+  { const char **paths = malloc(sizeof(char *)*(SM.n > 0 ? SM.n : 1));
+    int          rc;
+    if (paths == NULL)
+      exit (1);
+    for (i = 0; i < SM.n; i++)
+      { fclose(SM.v[i].f);
+        SM.v[i].f = NULL;
+        paths[i] = SM.v[i].name;
+      }
+    rc = hm_scan_write_pairs(S,PIXMAP,SM.n,paths,&PST);
+    free(paths);
+    if (rc == HM_ENOMEM && !PST.planned)
+      { HOST_WRITER = 1;
+        for (i = 0; i < SM.n; i++)
+          if ((SM.v[i].f = fopen(SM.v[i].name,"w")) == NULL)
+            { fprintf(stderr,"%s: Cannot open smudge file %s\n",Prog_Name,SM.v[i].name);
+              exit (1);
+            }
+        if (hm_scan_extract(S,PIXMAP,&REC,&NREC) != HM_OK)
+          die_hm();
+      }
+    else if (rc != HM_OK)
+      die_hm();
+  }
+  t_pairs = wall_ms() - t_pairs;
 #endif
   //  (the device-resident table is not torn down: the process is about to end, and destroying the CUDA
   //   context by hand costs ~0.1 s of wall clock for nothing)
@@ -496,13 +524,24 @@ int main(int argc, char *argv[])
                    "\"ms_pass1\": %.3f, \"ms_pass2\": %.3f, \"ms_scan\": %.3f, \"kernel_launches\": %lld, "
                    "\"streamed\": %s, \"chunks\": %lld, \"device_bytes\": %lld, "
                    "\"wall_ms\": {\"open\": %.1f, \"cuda_init_load\": %.1f, \"examine\": %.1f, \"scan\": %.1f}, "
-                   "\"load_ms\": {\"alloc\": %.1f, \"records\": %.1f, \"index\": %.1f}}\n",
+                   "\"load_ms\": {\"alloc\": %.1f, \"records\": %.1f, \"index\": %.1f}",
             (long long) stats.nels,stats.n_gpus,stats.path == HM_PATH_SYMM ? "symmetric" : "direct",
             stats.bucket_bits,stats.ms_h2d_unpack,
             stats.ms_pass1,stats.ms_pass2,stats.ms_scan,(long long) stats.kernel_launches,
             streamed ? "true" : "false",(long long) chunks,(long long) dev_bytes,
             t_open-t_start,t_load-t_open,t_exam-t_load,t_scan-t_exam,
             stats.ms_alloc,stats.ms_records,stats.ms_index);
+#ifdef EXTRACT_PAIRS
+      fprintf(stderr,", \"pairs\": {\"writer\": \"%s\", \"wall_ms\": %.1f, \"records\": %lld, \"passes\": %lld, "
+                   "\"windows\": %lld, \"room\": %lld, \"peak_bytes\": %lld, \"budget\": %lld, \"ms_hist\": %.3f, "
+                   "\"ms_list\": %.3f, \"ms_sort\": %.3f, \"ms_format\": %.3f, \"ms_d2h\": %.3f, \"ms_write\": %.3f, "
+                   "\"ms_writer_busy\": %.3f, \"ms_total\": %.3f}",
+              HOST_WRITER ? "host" : "gpu",t_pairs,(long long) (HOST_WRITER ? NREC : PST.records),
+              (long long) PST.passes,(long long) PST.windows,(long long) PST.room,(long long) PST.peak_bytes,
+              (long long) PST.budget,PST.ms_hist,PST.ms_list,PST.ms_sort,PST.ms_format,PST.ms_d2h,PST.ms_write,
+              PST.ms_writer_busy,PST.ms_total);
+#endif
+      fprintf(stderr,"}\n");
     }
 
   if (input != NULL)                                              /* PloidyPlot.c:1584-1592 */
@@ -518,6 +557,7 @@ int main(int argc, char *argv[])
 #ifdef EXTRACT_PAIRS
   //  The pair list comes back sorted by (smudge, k-mer); one line per pair in print_het's format
   //  (PloidyList.c:128-165): lower-case bases with "(x/y)" at the varying position
+  if (HOST_WRITER)
   { static const char dna[4] = { 'a', 'c', 'g', 't' };
     char   line[160];
     int64_t r;
@@ -539,6 +579,8 @@ int main(int argc, char *argv[])
       fclose(SM.v[i].f);
     free(REC);
   }
+  for (i = 0; i < SM.n; i++)
+    free(SM.v[i].name);
 #else
   if (VERBOSE)
     { fprintf(stderr,"\n  Count complete, outputting table\n");
