@@ -143,6 +143,12 @@ __device__ __forceinline__ uint64_t ld_stream(const uint64_t *p)
   return v;
 }
 
+/* *p |= v as a reduction (SASS REDG), which returns nothing to the SM.  atomicOr with its result unused
+ * compiled to an ATOMG into RZ in the pass-1 kernels, whose old word L2 still sends back: the Bloom inserts
+ * as ATOMGs cost runscan_kernel 0.05 ms at 2e8 entries, as REDGs nothing measurable (DESIGN.md §8)      */
+__device__ __forceinline__ void red_or64(uint64_t *p, uint64_t v)
+{ asm volatile("red.global.relaxed.gpu.or.b64 [%0], %1;" :: "l"(__cvta_generic_to_global(p)), "l"(v) : "memory"); }
+
 __device__ __forceinline__ int owner_of(const SymmView &W, uint64_t hi)
 { int r = 0;
   for (int s = 1; s < W.n_seg; s++)
@@ -367,6 +373,15 @@ template <int KW> struct RsSmem
 __device__ __forceinline__ uint64_t pack_meta(int cx, int cy, int pos, int yb)
 { return (uint64_t) cx | ((uint64_t) cy << 16) | ((uint64_t) pos << 32) | ((uint64_t) yb << 40); }
 
+/* Probe build only: the mode tools/time_runscan_phases.py sets (see the probe block before runscan_kernel).
+ * RS_PROBE_IS(m) is a constant false in the default build, so the hooks below compile to nothing there. */
+#ifdef RS_PROBE
+__device__ int rs_probe_mode;
+#define RS_PROBE_IS(m) (rs_probe_mode == (m))
+#else
+#define RS_PROBE_IS(m) false
+#endif
+
 /* candidate records into the CTA's staging area (warp-wide call; `emit` per lane): one shared atomic for
  * all the lanes that emit; lanes that find the staging area full
  * go to the list directly, again with one (global) atomic for all of them                              */
@@ -375,7 +390,7 @@ __device__ __forceinline__ void stage_candidates(const RsSmem<KW> &S, unsigned *
                                                  bool emit, uint64_t x, uint64_t xl, uint64_t meta,
                                                  int lane, unsigned lt)
 { const unsigned bal = __ballot_sync(0xffffffffu,emit);
-  if (bal == 0)
+  if (bal == 0 || RS_PROBE_IS(4))                      /* probe no-stage: nothing is staged */
     return;
   unsigned base = 0;
   if (lane == 0)
@@ -428,7 +443,8 @@ template <int KW, bool SL>
 __device__ __forceinline__ void bloom_insert(const SymmView &W, int kmer, uint64_t x, uint64_t xl)
 { uint64_t *word, mask;
   bloom_slot<KW>(W,W.self,kmer,x,xl,word,mask);
-  atomicOr((unsigned long long *) word,(unsigned long long) mask);
+  if (!RS_PROBE_IS(3) || mask == (uint64_t) (uintptr_t) word)   /* probe no-RED: the slot is computed (the test reads */
+    red_or64(word,mask);                                        /*   it and never holds), the RED not issued */
   if (SL)
     s_push<KW>(W,x,xl);
 }
@@ -638,11 +654,12 @@ __device__ __forceinline__ bool settle_members(const RsSmem<KW> &S, const SymmVi
  * atomic per warp and phase -- into one of RS_PROBE_SLOTS rows by CTA, as a few hundred thousand atomics on
  * six addresses would serialise in L2 and time themselves -- and a mode: 0 the full kernel, 1 stage the
  * window and return (load-only bound), 2 every CTA stages tile blockIdx.x % 64, which stays in L2, and does
- * the full work (compute-only bound).                                                                   */
+ * the full work (compute-only bound); each of the next three takes one part out of the full kernel, so its
+ * gap to mode 0 is the price of that part: 3 no-RED (bloom_insert computes the slot but issues no atomic),
+ * 4 no-stage (stage_candidates and the step-5 flush do nothing), 5 no-long (step 4 is skipped).          */
 #define RS_PHASES 6
 #define RS_PROBE_SLOTS 1024
 __device__ unsigned long long rs_probe_cycles[RS_PROBE_SLOTS*RS_PHASES];
-__device__ int rs_probe_mode;
 #define RS_PROBE_TILE(b)  (rs_probe_mode == 2 ? (b) % 64 : (b))
 #define RS_PROBE_START    long long rs_t = clock64(); unsigned long long rs_acc[RS_PHASES] = {0, 0, 0, 0, 0, 0};
 #define RS_PROBE_MARK(ph) { const long long t_ = clock64(); rs_acc[ph] += (unsigned long long) (t_ - rs_t); rs_t = t_; }
@@ -815,6 +832,8 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
       }
   }
   __syncwarp();
+  if (RS_PROBE_IS(5))                                  /* probe no-long: step 4 is skipped */
+    n3 = 0;
   RS_PROBE_MARK(2)
 
   /* ---- 3. runs of two: one comparison settles both members ---- */
@@ -920,7 +939,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
       last = (atomicAdd(&s_done,1u) == RS_THREADS/32-1);
     }
   last = __shfl_sync(FULL,last,0);
-  if (!last)
+  if (!last || RS_PROBE_IS(4))                         /* (probe no-stage: no flush either) */
     { RS_PROBE_MARK(5) RS_PROBE_FLUSH() return; }
   __threadfence_block();
   const unsigned nr = s_nr;

@@ -11,10 +11,15 @@ process runs the bench table through that build (HETMERS_LIB):
   load_only     every CTA stages its window, then returns: the bound set by the table's bytes
   compute_only  every CTA stages tile blockIdx.x % 64 (which stays in L2) and does the full work: the bound
                 set by the kernel's own instructions and latencies
+  no_red        the full kernel, but bloom_insert computes the Bloom slot and issues no atomic
+  no_stage      the full kernel, but no candidate record is staged or flushed (step 5)
+  no_long       the full kernel without step 4 (runs of three or more)
+The gap between `full` and each of the last three is the price of the part that mode takes out.
 
 Times are CUDA events around hm_k_symm_runscan (the header and Bloom clears included, as in bench.py's
-roofline.ms_per_launch), the median of `rounds` rounds of `reps` launches, the three modes alternated round by
-round.  Prints one JSON line with the card name and power limit.  Writes nothing to the trees.
+roofline.ms_per_launch), the median of `rounds` rounds of `reps` launches, the modes alternated round by round.
+`phases` holds every mode's cycles.  Prints one JSON line with the card name and power limit.  Writes nothing
+to the trees.
 
     python tools/time_runscan_phases.py [--tree NAME=DIR ...] [--reps 20] [--rounds 5] [--nels 2e8]
 
@@ -33,7 +38,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 PHASES = ["stage", "adjacency", "classify", "runs_of_two", "longer_runs", "flush"]
-MODES = {"full": 0, "load_only": 1, "compute_only": 2}
+MODES = {"full": 0, "load_only": 1, "compute_only": 2, "no_red": 3, "no_stage": 4, "no_long": 5}
 
 
 def card():
@@ -95,22 +100,24 @@ def child(args):
     for m in MODES.values():                                 # warm-up, every mode
         timed(m)
     ms = {name: [] for name in MODES}
-    cyc = [0] * len(PHASES)
+    cyc = {name: [0] * len(PHASES) for name in MODES}
     for _ in range(args.rounds):
         for name, m in MODES.items():
             ms[name].append(timed(m))
-            if name == "full":
-                _lib.check(L.hm_probe_runscan(0, cycles))
-                cyc = [a + int(b) for a, b in zip(cyc, cycles)]
+            _lib.check(L.hm_probe_runscan(0, cycles))
+            cyc[name] = [a + int(b) for a, b in zip(cyc[name], cycles)]
     _lib.check(L.hm_probe_runscan(0, None))
-    nc, st = t.symm_status()
-    tot = sum(cyc) or 1
     warps = args.rounds * args.reps * tiles * 8
+
+    def split(c):
+        tot = sum(c) or 1
+        return {"cycles_per_warp": round(tot / warps, 1),
+                **{p: {"share": round(x / tot, 4), "per_warp": round(x / warps, 1)} for p, x in zip(PHASES, c)}}
+
     out = {"nels": t.n, "tiles": tiles, "reps": args.reps, "rounds": args.rounds,
            "ms": {name: round(statistics.median(v), 4) for name, v in ms.items()},
            "ms_range": {name: [round(min(v), 4), round(max(v), 4)] for name, v in ms.items()},
-           "phases": {p: {"share": round(c / tot, 4), "per_warp": round(c / warps, 1)} for p, c in zip(PHASES, cyc)},
-           "cycles_per_warp": round(tot / warps, 1)}
+           "phases": {name: split(c) for name, c in cyc.items()}}
     print(json.dumps(out), flush=True)
 
 
