@@ -59,9 +59,12 @@
                                                 *   a run whose head lies in the tile is then inside the window  */
 #define RS_LONGRUN 32                          /* dense kernel: runs of more entries go to runs_kernel */
 #ifndef RS_MINBLOCKS
-#define RS_MINBLOCKS 5                         /* resident CTAs per SM the register budget must allow (48 regs, no
-                                                *   spills).  runscan_kernel at 2e8 entries on one H100 SXM (400 W):
-                                                *   4: 1.18 ms, 5: 1.12, 6 (40 regs): 1.14                          */
+#define RS_MINBLOCKS 6                         /* resident CTAs per SM the register budget must allow (40 regs, no
+                                                *   spills; at k <= 32 six 34 KB windows fit in shared memory).  Each
+                                                *   CTA waits on its window and on its step-5 atomic with all its
+                                                *   warps, and a sixth CTA covers those waits: runscan_kernel at 2e8
+                                                *   entries on one H100 SXM (700 W), 5: 1.027-1.032 ms, 6: 0.977-0.983
+                                                *   (DESIGN.md §8)                                                    */
 #endif
 #ifndef RS_STAGE
 #define RS_STAGE   384                         /* candidate records staged per CTA before they leave (a 2048-entry
@@ -449,6 +452,58 @@ __device__ __forceinline__ void bloom_insert(const SymmView &W, int kmer, uint64
     s_push<KW>(W,x,xl);
 }
 
+/* Step 5 of the pass-1 kernels, after a CTA barrier: the staged records leave with one global atomic per CTA
+ * and list (one per record, or per warp, on the one list counter serialises in L2), and every thread moves
+ * at most RS_FLUSH of them.  flush_reserve issues thread 0's atomics and, while they are under way, reads
+ * the thread's records from shared memory into F; after a second barrier flush_store writes them and the
+ * run heads (rare) to the lists.                                                                           */
+#define RS_FLUSH ((RS_STAGE+RS_THREADS-1)/RS_THREADS)
+struct RsFlush { uint64_t key[RS_FLUSH], lo[RS_FLUSH], meta[RS_FLUSH]; };
+
+template <int KW>
+__device__ __forceinline__ void flush_reserve(const RsSmem<KW> &S, unsigned long long *s_cb,
+                                              unsigned long long *s_rb, const SymmView &W,
+                                              unsigned nc, unsigned nr, RsFlush &F)
+{ if (threadIdx.x == 0)
+    { if (nc > 0) *s_cb = atomicAdd(W.cand_n,(unsigned long long) nc);
+      if (nr > 0) *s_rb = atomicAdd(W.runs_n,(unsigned long long) nr);
+    }
+#pragma unroll
+  for (int j = 0; j < RS_FLUSH; j++)
+    { const unsigned i = threadIdx.x + j*RS_THREADS;
+      if (i < nc)
+        { F.key[j] = S.ckey[i];
+          if (KW == 2) F.lo[j] = S.clo[i];
+          F.meta[j] = S.cmeta[i];
+        }
+    }
+}
+
+template <int KW>
+__device__ __forceinline__ void flush_store(const RsSmem<KW> &S, unsigned long long cb, unsigned long long rb,
+                                            const SymmView &W, unsigned nc, unsigned nr, int64_t T0,
+                                            const RsFlush &F)
+{
+#pragma unroll
+  for (int j = 0; j < RS_FLUSH; j++)
+    { const unsigned i = threadIdx.x + j*RS_THREADS;
+      if (i < nc)
+        { if (cb+i < W.cand_cap)
+            { W.cand_key[cb+i] = F.key[j];
+              if (KW == 2) W.cand_lo[cb+i] = F.lo[j];
+              W.cand_meta[cb+i] = F.meta[j];
+            }
+          else
+            atomicOr(W.status,SY_STATUS_OVERFLOW);
+        }
+    }
+  for (unsigned i = threadIdx.x; i < nr; i += RS_THREADS)
+    if (rb+i < W.runs_cap)
+      W.runs[rb+i] = (uint64_t) (T0 + ((int) S.t2r[i] - RS_HALO));
+    else
+      atomicOr(W.status,SY_STATUS_OVERFLOW);
+}
+
 /* Pass 1b: the runs runscan_kernel only lists -- more than RS_RUNCAP entries (or runs that may reach
  * past its window), and on crowded tables the runs runscan_dense_kernel leaves (more than RS_LONGRUN):
  * repeats, low-complexity sequence, tiny k.  The listed count is only known on the device, so the grid
@@ -642,41 +697,58 @@ __device__ __forceinline__ bool settle_members(const RsSmem<KW> &S, const SymmVi
  *      H100 SXM at 400 W when it settled them all)
  *   Pair tests in steps 3 and 4 look at the bases after the run prefix only, one 32-bit word for k <= 32
  *   and one 64-bit word for k <= 64 (run_sfx, one_base_in_run).
- *   5. candidate records and run heads are staged in shared memory; the LAST warp to finish moves
- *      them out with one global atomic per CTA and list (one per record, or per warp, on the one
- *      list counter serialises in L2)
+ *   5. candidate records and run heads are staged in shared memory; after a CTA barrier thread 0
+ *      reserves their ranges with one global atomic per CTA and list (one per record, or per warp, on
+ *      the one list counter serialises in L2) while every thread reads its at most RS_FLUSH records
+ *      from shared memory, and after a second barrier every thread stores them (flush_reserve,
+ *      flush_store): the CTA ends one atomic round trip and one store after its last warp is done
  * (The alternatives -- every entry scanning its run in place, per-entry classification with predicated
  * list writes, CTA-wide task lists with a barrier per phase -- need more instructions, leave more lanes
  * idle or wait at the barriers.)                                                                      */
 #ifdef RS_PROBE
 /* Probe build only (make EXTRA=-DRS_PROBE=1, tools/time_runscan_phases.py): the clock64() cycles every warp
- * spends in each phase (0 staging / TMA wait, 1..5 as numbered in the kernel), summed over all warps with one
- * atomic per warp and phase -- into one of RS_PROBE_SLOTS rows by CTA, as a few hundred thousand atomics on
- * six addresses would serialise in L2 and time themselves -- and a mode: 0 the full kernel, 1 stage the
- * window and return (load-only bound), 2 every CTA stages tile blockIdx.x % 64, which stays in L2, and does
- * the full work (compute-only bound); each of the next three takes one part out of the full kernel, so its
- * gap to mode 0 is the price of that part: 3 no-RED (bloom_insert computes the slot but issues no atomic),
- * 4 no-stage (stage_candidates and the step-5 flush do nothing), 5 no-long (step 4 is skipped).          */
-#define RS_PHASES 6
+ * spends in each phase (0 staging / TMA wait, 1..4 as numbered in the kernel, then step 5 in three: 5 the
+ * hand-off between the warps, 6 the global atomics on the list counters until their results are back, 7 the
+ * copy of the staged records), summed over all warps with one atomic per warp and phase -- into one of
+ * RS_PROBE_SLOTS rows by CTA, as a few hundred thousand atomics on a few addresses would serialise in L2 and
+ * time themselves.  Columns RS_PHASES.. hold each CTA's lifetime by thread 0's clock, added once per CTA:
+ * 8 start to window landed, 9 landed to every warp done with step 4 (the barrier that opens step 5), 10 from
+ * then to thread 0's end (the tail).  And a mode: 0 the full kernel, 1 stage the window and return (load-only bound),
+ * 2 every CTA stages tile blockIdx.x % 64, which stays in L2, and does the full work (compute-only bound);
+ * each of the next four takes one part out of the full kernel, so its gap to mode 0 is the price of that
+ * part: 3 no-RED (bloom_insert computes the slot but issues no atomic), 4 no-stage (stage_candidates and the
+ * step-5 flush do nothing), 5 no-long (step 4 is skipped), 6 no-tail (every warp returns after step 4).   */
+#define RS_PHASES 8
+#define RS_COLS   (RS_PHASES+3)
 #define RS_PROBE_SLOTS 1024
-__device__ unsigned long long rs_probe_cycles[RS_PROBE_SLOTS*RS_PHASES];
+__device__ unsigned long long rs_probe_cycles[RS_PROBE_SLOTS*RS_COLS];
 #define RS_PROBE_TILE(b)  (rs_probe_mode == 2 ? (b) % 64 : (b))
-#define RS_PROBE_START    long long rs_t = clock64(); unsigned long long rs_acc[RS_PHASES] = {0, 0, 0, 0, 0, 0};
+#define RS_PROBE_START    __shared__ long long rs_t0, rs_t1; \
+                          long long rs_t = clock64(); unsigned long long rs_acc[RS_PHASES] = {0, 0, 0, 0, 0, 0, 0, 0}; \
+                          if (threadIdx.x == 0) rs_t0 = rs_t;
 #define RS_PROBE_MARK(ph) { const long long t_ = clock64(); rs_acc[ph] += (unsigned long long) (t_ - rs_t); rs_t = t_; }
+#define RS_PROBE_LANDED() if (threadIdx.x == 0) rs_t1 = clock64();
+#define RS_PROBE_ALLDONE  const long long rs_t2 = clock64();
+#define RS_PROBE_ROW      (rs_probe_cycles + (blockIdx.x % RS_PROBE_SLOTS)*RS_COLS)
 #define RS_PROBE_FLUSH()  { if (lane == 0) _Pragma("unroll") for (int p_ = 0; p_ < RS_PHASES; p_++) \
-                              atomicAdd(rs_probe_cycles + (blockIdx.x % RS_PROBE_SLOTS)*RS_PHASES + p_,rs_acc[p_]); }
+                              atomicAdd(RS_PROBE_ROW + p_,rs_acc[p_]); }
+#define RS_PROBE_LIFE()   { const long long t3_ = clock64(); \
+                            if (threadIdx.x == 0) { atomicAdd(RS_PROBE_ROW + RS_PHASES,  (unsigned long long) (rs_t1 - rs_t0)); \
+                                             atomicAdd(RS_PROBE_ROW + RS_PHASES+1,(unsigned long long) (rs_t2 - rs_t1)); \
+                                             atomicAdd(RS_PROBE_ROW + RS_PHASES+2,(unsigned long long) (t3_ - rs_t2)); } }
 #define RS_PROBE_LOADONLY() if (rs_probe_mode == 1) { RS_PROBE_FLUSH(); return; }
+#define RS_PROBE_NOTAIL()   if (rs_probe_mode == 6) { RS_PROBE_FLUSH(); return; }
 
-/* cycles != NULL: the sums since the last call into cycles[RS_PHASES]; then clear them and set the mode */
+/* cycles != NULL: the sums since the last call into cycles[RS_PHASES+3]; then clear them and set the mode */
 extern "C" int hm_probe_runscan(int mode, unsigned long long *cycles)
-{ static unsigned long long rows[RS_PROBE_SLOTS*RS_PHASES];
+{ static unsigned long long rows[RS_PROBE_SLOTS*RS_COLS];
   cudaError_t e = cudaDeviceSynchronize();
   if (e == cudaSuccess && cycles != NULL)
     { e = cudaMemcpyFromSymbol(rows,rs_probe_cycles,sizeof(rows));
-      for (int p = 0; p < RS_PHASES; p++)
+      for (int p = 0; p < RS_COLS; p++)
         { cycles[p] = 0;
           for (int r = 0; r < RS_PROBE_SLOTS; r++)
-            cycles[p] += rows[r*RS_PHASES+p];
+            cycles[p] += rows[r*RS_COLS+p];
         }
     }
   memset(rows,0,sizeof(rows));
@@ -690,8 +762,12 @@ extern "C" int hm_probe_runscan(int mode, unsigned long long *cycles)
 #define RS_PROBE_TILE(b)  (b)
 #define RS_PROBE_START
 #define RS_PROBE_MARK(ph)
+#define RS_PROBE_LANDED()
+#define RS_PROBE_ALLDONE
 #define RS_PROBE_FLUSH()
+#define RS_PROBE_LIFE()
 #define RS_PROBE_LOADONLY()
+#define RS_PROBE_NOTAIL()
 #endif
 
 template <typename IdxT, int KW, bool SL>
@@ -701,7 +777,8 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
                int kmer, int64_t lo, int64_t hi, int64_t tile0, int use_tma, const SymmView W)
 { extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t s_bar;
-  __shared__ unsigned s_nc, s_nr, s_done;
+  __shared__ unsigned s_nc, s_nr;
+  __shared__ unsigned long long s_base[2];
   RsSmem<KW> S;
   S.key   = (uint64_t *) smem;
   S.klo   = S.key + (KW == 2 ? RS_WIN : 0);
@@ -732,7 +809,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
   const int m   = v1-v0;
   const int mt  = use_tma ? (m & ~7) : 0;
   if (threadIdx.x == 0)
-    { s_nc = 0; s_nr = 0; s_done = 0;
+    { s_nc = 0; s_nr = 0;
       if (mt > 0)
         { mbar_init(&s_bar,1);
           fence_proxy_async_smem();
@@ -766,6 +843,7 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
   else
     mbar_wait(&s_bar,0);
   RS_PROBE_MARK(0)
+  RS_PROBE_LANDED()
   RS_PROBE_LOADONLY()
 
   /* ---- 1. adjacency bits of this warp's words wd0-1 .. wd0+RS_EPT, word t in lane t ---- */
@@ -930,48 +1008,24 @@ runscan_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ k
         }
     }
   RS_PROBE_MARK(4)
+  RS_PROBE_NOTAIL()
 
-  /* ---- 5. the last warp to get here moves the staged records out ---- */
-  __syncwarp();
-  unsigned last = 0;
-  if (lane == 0)
-    { __threadfence_block();
-      last = (atomicAdd(&s_done,1u) == RS_THREADS/32-1);
-    }
-  last = __shfl_sync(FULL,last,0);
-  if (!last || RS_PROBE_IS(4))                         /* (probe no-stage: no flush either) */
-    { RS_PROBE_MARK(5) RS_PROBE_FLUSH() return; }
-  __threadfence_block();
-  const unsigned nr = s_nr;
-  if (nr > 0)
-    { unsigned long long rb = 0;
-      if (lane == 0)
-        rb = atomicAdd(W.runs_n,(unsigned long long) nr);
-      rb = __shfl_sync(FULL,rb,0);
-      for (unsigned i = lane; i < nr; i += 32)
-        if (rb+i < W.runs_cap)
-          W.runs[rb+i] = (uint64_t) (T0 + ((int) S.t2r[i] - RS_HALO));
-        else
-          atomicOr(W.status,SY_STATUS_OVERFLOW);
-    }
-  const unsigned nc = s_nc < RS_STAGE ? s_nc : RS_STAGE;
-  if (nc == 0)
-    { RS_PROBE_MARK(5) RS_PROBE_FLUSH() return; }
-  unsigned long long base = 0;
-  if (lane == 0)
-    base = atomicAdd(W.cand_n,(unsigned long long) nc);
-  base = __shfl_sync(FULL,base,0);
-  for (unsigned i = lane; i < nc; i += 32)
-    { unsigned long long at = base + i;
-      if (at < W.cand_cap)
-        { W.cand_key[at] = S.ckey[i];
-          if (KW == 2) W.cand_lo[at] = S.clo[i];
-          W.cand_meta[at] = S.cmeta[i];
-        }
-      else
-        atomicOr(W.status,SY_STATUS_OVERFLOW);
-    }
+  /* ---- 5. every warp moves its share of the staged records out ---- */
+  __syncthreads();
   RS_PROBE_MARK(5)
+  RS_PROBE_ALLDONE
+  if (RS_PROBE_IS(4))                                  /* (probe no-stage: no flush either) */
+    { RS_PROBE_FLUSH() return; }
+  const unsigned nc = s_nc < RS_STAGE ? s_nc : RS_STAGE, nr = s_nr;
+  if (nc == 0 && nr == 0)                              /* (CTA-uniform) */
+    { RS_PROBE_MARK(6) RS_PROBE_LIFE() RS_PROBE_FLUSH() return; }
+  RsFlush F;
+  flush_reserve<KW>(S,&s_base[0],&s_base[1],W,nc,nr,F);
+  __syncthreads();
+  RS_PROBE_MARK(6)
+  flush_store<KW>(S,s_base[0],s_base[1],W,nc,nr,T0,F);
+  RS_PROBE_MARK(7)
+  RS_PROBE_LIFE()
   RS_PROBE_FLUSH()
 }
 
@@ -993,7 +1047,8 @@ runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
                      int64_t tile0, int use_tma, const SymmView W)
 { extern __shared__ __align__(128) uint8_t smem[];
   __shared__ __align__(8) uint64_t s_bar;
-  __shared__ unsigned s_nc, s_nl, s_done;
+  __shared__ unsigned s_nc, s_nl;
+  __shared__ unsigned long long s_base[2];
   __shared__ unsigned s_eq[RS_WIN/32+1];
   RsSmem<KW> S;
   S.key   = (uint64_t *) smem;
@@ -1024,7 +1079,7 @@ runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
   const int m   = v1-v0;
   const int mt  = use_tma ? (m & ~7) : 0;
   if (threadIdx.x == 0)
-    { s_nc = 0; s_nl = 0; s_done = 0;
+    { s_nc = 0; s_nl = 0;
       if (mt > 0)
         { mbar_init(&s_bar,1);
           fence_proxy_async_smem();
@@ -1164,46 +1219,15 @@ runscan_dense_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restri
       stage_candidates<KW>(S,&s_nc,W,emit,x,xl,meta,lane,lt);
     }
 
-  /* ---- the last warp to get here moves the staged records and the long-run heads out ---- */
-  __syncwarp();
-  unsigned last = 0;
-  if (lane == 0)
-    { __threadfence_block();
-      last = (atomicAdd(&s_done,1u) == RS_THREADS/32-1);
-    }
-  last = __shfl_sync(FULL,last,0);
-  if (!last)
+  /* ---- every warp moves its share of the staged records and the long-run heads out ---- */
+  __syncthreads();
+  const unsigned nc = s_nc < RS_STAGE ? s_nc : RS_STAGE, nr = s_nl;
+  if (nc == 0 && nr == 0)                              /* (CTA-uniform) */
     return;
-  __threadfence_block();
-  const unsigned nr = s_nl;
-  if (nr > 0)
-    { unsigned long long rb = 0;
-      if (lane == 0)
-        rb = atomicAdd(W.runs_n,(unsigned long long) nr);
-      rb = __shfl_sync(FULL,rb,0);
-      for (unsigned i = lane; i < nr; i += 32)
-        if (rb+i < W.runs_cap)
-          W.runs[rb+i] = (uint64_t) (T0 + ((int) S.t2r[i] - RS_HALO));
-        else
-          atomicOr(W.status,SY_STATUS_OVERFLOW);
-    }
-  const unsigned nc = s_nc < RS_STAGE ? s_nc : RS_STAGE;
-  if (nc == 0)
-    return;
-  unsigned long long base = 0;
-  if (lane == 0)
-    base = atomicAdd(W.cand_n,(unsigned long long) nc);
-  base = __shfl_sync(FULL,base,0);
-  for (unsigned i = lane; i < nc; i += 32)
-    { unsigned long long at = base + i;
-      if (at < W.cand_cap)
-        { W.cand_key[at] = S.ckey[i];
-          if (KW == 2) W.cand_lo[at] = S.clo[i];
-          W.cand_meta[at] = S.cmeta[i];
-        }
-      else
-        atomicOr(W.status,SY_STATUS_OVERFLOW);
-    }
+  RsFlush F;
+  flush_reserve<KW>(S,&s_base[0],&s_base[1],W,nc,nr,F);
+  __syncthreads();
+  flush_store<KW>(S,s_base[0],s_base[1],W,nc,nr,T0,F);
 }
 
 /* f(Inst<IdxT,KW>()) for the instantiation that serves (kmer, idx64): KW key words, IdxT bucket offsets */

@@ -6,15 +6,23 @@ directory (make EXTRA=-DRS_PROBE=1 OBJDIR=... LIBDIR=...; the tree's own build i
 process runs the bench table through that build (HETMERS_LIB):
 
   full          runscan_kernel as it is, and the clock64() cycles its warps spend per phase (0 staging / TMA
-                wait, 1 adjacency bits, 2 classification + task lists, 3 runs of two, 4 longer runs, 5 flush),
-                summed over all warps; `per_warp` is cycles per warp and tile
+                wait, 1 adjacency bits, 2 classification + task lists, 3 runs of two, 4 longer runs, then step 5:
+                5 hand-off between the warps, 6 the global atomics on the list counters until their results
+                are back, 7 the copy of the staged records), summed over all warps; `per_warp` is cycles per
+                warp and tile.  `cta` is each CTA's lifetime in cycles, split at the moments its window has
+                landed and every warp is done with step 4: `to_window`, `steps_1_4` (two or more warps
+                running) and `tail` (from then to the CTA's end)
   load_only     every CTA stages its window, then returns: the bound set by the table's bytes
   compute_only  every CTA stages tile blockIdx.x % 64 (which stays in L2) and does the full work: the bound
                 set by the kernel's own instructions and latencies
   no_red        the full kernel, but bloom_insert computes the Bloom slot and issues no atomic
   no_stage      the full kernel, but no candidate record is staged or flushed (step 5)
   no_long       the full kernel without step 4 (runs of three or more)
-The gap between `full` and each of the last three is the price of the part that mode takes out.
+  no_tail       the full kernel, but every warp returns after step 4: nothing is moved out
+The gap between `full` and each of the last four is the price of the part that mode takes out.
+
+`records` are sha256 digests of the full kernel's candidate records (key, lo, meta; sorted) and of its listed
+run heads (sorted), with their counts: equal digests across trees mean the same records as a multiset.
 
 Times are CUDA events around hm_k_symm_runscan (the header and Bloom clears included, as in bench.py's
 roofline.ms_per_launch), the median of `rounds` rounds of `reps` launches, the modes alternated round by round.
@@ -37,8 +45,9 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-PHASES = ["stage", "adjacency", "classify", "runs_of_two", "longer_runs", "flush"]
-MODES = {"full": 0, "load_only": 1, "compute_only": 2, "no_red": 3, "no_stage": 4, "no_long": 5}
+PHASES = ["stage", "adjacency", "classify", "runs_of_two", "longer_runs", "handoff", "list_atomics", "copy"]
+LIFE = ["to_window", "steps_1_4", "tail"]
+MODES = {"full": 0, "load_only": 1, "compute_only": 2, "no_red": 3, "no_stage": 4, "no_long": 5, "no_tail": 6}
 
 
 def card():
@@ -78,7 +87,7 @@ def child(args):
     if not hasattr(L, "hm_probe_runscan"):
         raise SystemExit(f"{_lib.LIB_PATH} is not a probe build (no hm_probe_runscan)")
     L.hm_probe_runscan.argtypes = [C.c_int, C.POINTER(C.c_uint64)]
-    cycles = (C.c_uint64 * len(PHASES))()
+    cycles = (C.c_uint64 * (len(PHASES) + len(LIFE)))()
     dev = torch.device("cuda", 0)
     G = synth.calibrate_G(K, int(args.nels), PLOIDY, HET, COV, LCUT)
     keys, cnt = synth.synth_table(K, G, PLOIDY, HET, COV, LCUT, SEED, device=dev)
@@ -99,8 +108,10 @@ def child(args):
 
     for m in MODES.values():                                 # warm-up, every mode
         timed(m)
+    _lib.check(L.hm_probe_runscan(0, None))                 # the full kernel
+    records = digests(t, torch)
     ms = {name: [] for name in MODES}
-    cyc = {name: [0] * len(PHASES) for name in MODES}
+    cyc = {name: [0] * (len(PHASES) + len(LIFE)) for name in MODES}
     for _ in range(args.rounds):
         for name, m in MODES.items():
             ms[name].append(timed(m))
@@ -109,16 +120,43 @@ def child(args):
     _lib.check(L.hm_probe_runscan(0, None))
     warps = args.rounds * args.reps * tiles * 8
 
-    def split(c):
-        tot = sum(c) or 1
-        return {"cycles_per_warp": round(tot / warps, 1),
-                **{p: {"share": round(x / tot, 4), "per_warp": round(x / warps, 1)} for p, x in zip(PHASES, c)}}
+    ctas = args.rounds * args.reps * tiles
 
-    out = {"nels": t.n, "tiles": tiles, "reps": args.reps, "rounds": args.rounds,
+    def split(c):
+        ph, life = c[:len(PHASES)], c[len(PHASES):]
+        tot = sum(ph) or 1
+        return {"cycles_per_warp": round(tot / warps, 1),
+                **{p: {"share": round(x / tot, 4), "per_warp": round(x / warps, 1)} for p, x in zip(PHASES, ph)},
+                "cta": {p: round(x / ctas, 1) for p, x in zip(LIFE, life)}}
+
+    out = {"nels": t.n, "tiles": tiles, "reps": args.reps, "rounds": args.rounds, "records": records,
            "ms": {name: round(statistics.median(v), 4) for name, v in ms.items()},
            "ms_range": {name: [round(min(v), 4), round(max(v), 4)] for name, v in ms.items()},
            "phases": {name: split(c) for name, c in cyc.items()}}
     print(json.dumps(out), flush=True)
+
+
+def digests(t, torch):
+    """one full-kernel pass 1 -> sha256 of its sorted candidate records and of its sorted run heads"""
+    import hashlib
+
+    import numpy as np
+    t.runscan()
+    torch.cuda.synchronize()
+    lay, w = t.symm_layout, t.symm_work
+    hdr = w[lay.off_header: lay.off_header + 24].view(torch.int64).cpu().numpy()
+    nc, nr = min(int(hdr[0]), lay.cand_cap), min(int(hdr[2]), lay.runs_cap)
+
+    def words(off, n):
+        return w[off: off + 8 * n].view(torch.int64).cpu().numpy().view(np.uint64)
+    key = words(lay.off_cand_key, nc)
+    lo = words(lay.off_cand_lo, nc) if t.kmer > 32 else np.zeros(nc, np.uint64)
+    meta = words(lay.off_cand_meta, nc)
+    rec = np.stack([key, lo, meta], axis=1)
+    rec = rec[np.lexsort((meta, lo, key))]
+    runs = np.sort(words(lay.off_runs, nr))
+    return {"cand_n": nc, "cand_sha256": hashlib.sha256(np.ascontiguousarray(rec).tobytes()).hexdigest(),
+            "runs_n": nr, "runs_sha256": hashlib.sha256(runs.tobytes()).hexdigest(), "status": int(hdr[1])}
 
 
 def main():
