@@ -502,7 +502,8 @@ int64_t hm_pairs_bytes(int kmer, int64_t records);
  * with count >= ethresh (do_trim), plus every kept k-mer's reverse complement with the same count (do_symm),
  * sorted, the original winning where both are present -- as the FastK table `dst` (same kmer, ibyte and parts
  * as the source, parts cut on stub-index buckets).  It reads the table the scan was created from (that
- * hm_host_table must still be valid), in or out of core alike, on dev[0], and leaves the scan as it was.  The
+ * hm_host_table must still be valid), in or out of core alike, on dev[0] (on several of the scan's GPUs: see
+ * hm_set_condition_gpus), and leaves the scan as it was.  The
  * source passes through the GPU once to histogram the output by key prefix (HM_COND_HIST_BITS bits of the
  * first word), then once per key range of hm_condition_plan: each pass gathers the range's kept originals and
  * reverse complements, sorts the latter, merges (the steps hm_scan_condition takes in place), packs FastK
@@ -513,18 +514,34 @@ int64_t hm_pairs_bytes(int kmer, int64_t records);
  * written: a scan conditioned in place (HM_EINVAL), a dst one of whose files is one of the source's part files
  * (HM_EINVAL; seen through the part descriptors hm_table_open keeps open -- smudgeplot_b200.hetmers.Scan checks
  * by name for the tables it reads), a budget below one range's smallest working set (HM_ENOMEM).                                                                */
+/* GPUs hm_scan_condition_files runs on (process-wide; default 1: dev[0] alone, with one writer thread).  With
+ * n > 1 it uses the first min(n, G) devices of the scan, dev[0..]: each histograms a contiguous slice of the source
+ * (a streamed scan's through its own loader, an in-core scan's from its resident replica, so nothing crosses PCIe),
+ * the plan is made once under the smallest budget of those GPUs, range r runs on GPU r mod G' (from the replica in
+ * core, from the host table streamed), and each GPU's writer thread pwrites the range's records at their final
+ * offsets (hm_table_write_place / _at) while later ranges are settled.  The files are byte-identical to n = 1's.
+ * A device repeated in dev[] (a streamed scan) runs several of these shares, each under its own budget.  A
+ * failure on any GPU stops them all; every thread is joined, every allocation freed, every file removed.     */
+int  hm_set_condition_gpus(int n);         /* -> the value it replaces */
+#define HM_COND_MAX_GPUS  16                /* hm_condition_stats.gpu_peak_bytes entries             */
 #define HM_COND_HIST_BITS 20                /* output histogram: 2^min(20, 2k) key prefixes         */
 #define HM_COND_MAX_RANGE (1ll << 31)       /* entries one range may hold                           */
 
 typedef struct hm_condition_stats
   { int64_t nels_in, nels_out;
     int32_t ranges, passes;                 /* key ranges; passes over the source (ranges + 1)      */
-    int64_t peak_bytes;                     /* most device bytes the call held                       */
+    int64_t peak_bytes;                     /* most device bytes the call held (on one GPU)          */
     int64_t bytes_read, bytes_written;      /* source bytes sent H2D; table bytes written            */
     double  ms_hist, ms_ranges, ms_write, ms_total;   /* histogram pass; range passes (gather to pack); */
-                                            /*   host time writing (overlaps the next range); call  */
+                                            /*   host time writing (overlaps the next range; summed */
+                                            /*   over the writer threads); call                     */
     int64_t budget_bytes;                   /* the budget the call planned with: the one set less what */
-  } hm_condition_stats;                     /*   the scan holds, or free memory less the reserve      */
+                                            /*   the scan holds, or free memory less the reserve      */
+                                            /*   (several GPUs: the smallest)                         */
+    int32_t gpus, pad;                      /* GPUs the call ran on                                  */
+    double  ms_write_max;                   /* the busiest writer thread's time                      */
+    int64_t gpu_peak_bytes[HM_COND_MAX_GPUS];  /* peak_bytes of each GPU the call ran on             */
+  } hm_condition_stats;
 
 typedef struct hm_condition_layout         /* what hm_condition_plan chooses                            */
   { int64_t budget;
@@ -659,6 +676,18 @@ int  hm_table_write_buckets(hm_table_writer *w, int64_t b0, int64_t nb, const in
 int  hm_table_write_append(hm_table_writer *w, const uint8_t *rec, int64_t n);
 int  hm_table_write_close(hm_table_writer *w);
 void hm_table_write_abort(hm_table_writer *w);
+/* Positional mode, instead of write_buckets + append (a writer takes one or the other): ranges of the table are
+ * announced in table order with hm_table_write_place (counts[i] records for bucket b0+i, as write_buckets takes
+ * them; *first = the range's first ordinal), and their records -- any slice, in any order, from any thread --
+ * are written at their final offsets with hm_table_write_at(w, ordinal of rec[0], rec, n), a slice that crosses
+ * a part cut going to both parts.  The parts are cut exactly as the append path cuts them, so the files are
+ * byte-identical.  A cut is fixed once the bucket holding its ordinal is announced; records of the last bucket
+ * announced can still belong to either side of a cut, so hm_table_write_at copies those (at most one bucket's)
+ * and the place or hm_table_write_seal (no range follows; close seals too) that settles them writes them.  No
+ * call waits for another.  Records not yet placed are an error (HM_EINVAL).                                  */
+int  hm_table_write_place(hm_table_writer *w, int64_t b0, int64_t nb, const int64_t *counts, int64_t *first);
+int  hm_table_write_at(hm_table_writer *w, int64_t first, const uint8_t *rec, int64_t n);
+void hm_table_write_seal(hm_table_writer *w);
 
 /* .smu writer: "min\t(sum-min)\tcount\n", sum-major, min < FMAX (PloidyPlot.c:1603-1617) */
 int  hm_write_smu(const char *path, const int64_t *plot);

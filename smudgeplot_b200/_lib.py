@@ -33,7 +33,8 @@ ABI_SYMBOLS = [
     "hm_rank_scan_extract_settle", "hm_rank_scan_extract_result", "hm_sort_pair_records",
     "hm_condition_range_bytes", "hm_condition_plan", "hm_scan_condition_files",
     "hm_table_write_open", "hm_table_write_buckets", "hm_table_write_append", "hm_table_write_close",
-    "hm_table_write_abort",
+    "hm_table_write_abort", "hm_table_write_place", "hm_table_write_at", "hm_table_write_seal",
+    "hm_set_condition_gpus",
     "hm_k_cond_hist", "hm_k_shard_route_count", "hm_k_shard_route_scatter", "hm_k_shard_settle_bytes",
     "hm_k_shard_settle", "hm_shard_condition_bytes",
     "hm_k_shard_route_count_window", "hm_k_shard_route_scatter_window", "hm_k_cond_pack", "hm_rank_condition_bytes",
@@ -84,6 +85,7 @@ class StreamLayout(C.Structure):
 
 
 COND_HIST_BITS = 20
+COND_MAX_GPUS = 16
 
 
 class ConditionStats(C.Structure):
@@ -91,10 +93,13 @@ class ConditionStats(C.Structure):
     _fields_ = [("nels_in", C.c_int64), ("nels_out", C.c_int64), ("ranges", C.c_int32), ("passes", C.c_int32),
                 ("peak_bytes", C.c_int64), ("bytes_read", C.c_int64), ("bytes_written", C.c_int64),
                 ("ms_hist", C.c_double), ("ms_ranges", C.c_double), ("ms_write", C.c_double), ("ms_total", C.c_double),
-                ("budget_bytes", C.c_int64)]
+                ("budget_bytes", C.c_int64), ("gpus", C.c_int32), ("pad", C.c_int32), ("ms_write_max", C.c_double),
+                ("gpu_peak_bytes", C.c_int64 * COND_MAX_GPUS)]
 
     def as_dict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_}
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k not in ("pad", "gpu_peak_bytes")}
+        d["gpu_peak_bytes"] = list(self.gpu_peak_bytes)[:max(self.gpus, 1)]
+        return d
 
 
 class ConditionLayout(C.Structure):
@@ -243,6 +248,11 @@ def lib():
     L.hm_table_write_close.argtypes = [vp]
     L.hm_table_write_abort.argtypes = [vp]
     L.hm_table_write_abort.restype = None
+    L.hm_table_write_place.argtypes = [vp, i64, i64, vp, C.POINTER(i64)]
+    L.hm_table_write_at.argtypes = [vp, i64, vp, i64]
+    L.hm_table_write_seal.argtypes = [vp]
+    L.hm_table_write_seal.restype = None
+    L.hm_set_condition_gpus.argtypes = [i32]
     L.hm_k_cond_hist.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp]
     L.hm_k_shard_route_count.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, i32, vp, vp, vp]
     L.hm_k_shard_route_scatter.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]

@@ -1021,14 +1021,16 @@ static int cond_fetch(const CondSrc *S, int64_t o, int64_t m, const uint64_t **k
   return load_into(S->s,S->D,S->t,S->d_index,o,m,S->keys,S->klo,S->cnt,0,S->G);
 }
 
-/* pass 0: kept originals (+ their reverse complements) per key prefix -> hist (host, 2^hb entries) */
-static int cond_histogram(const CondSrc *S, int ethr, int do_symm, int hb, unsigned long long *d_hist, int64_t *hist)
+/* pass 0 over source ordinals [first, end): kept originals (+ their reverse complements) per key prefix -> hist
+ * (host, 2^hb entries)                                                                                        */
+static int cond_histogram(const CondSrc *S, int64_t first, int64_t end, int ethr, int do_symm, int hb,
+                          unsigned long long *d_hist, int64_t *hist)
 { cudaStream_t  st = S->D->st;
   const int64_t np = (int64_t) 1 << hb;
   int           rc = HM_OK;
   HM_CUDA(cudaMemsetAsync(d_hist,0,8*(size_t) np,st));
-  for (int64_t o = 0; o < S->n && rc == HM_OK; o += S->chunk)
-    { const int64_t   m = S->n-o < S->chunk ? S->n-o : S->chunk;
+  for (int64_t o = first; o < end && rc == HM_OK; o += S->chunk)
+    { const int64_t   m = end-o < S->chunk ? end-o : S->chunk;
       const uint64_t *k, *l;
       const uint16_t *c;
       rc = cond_fetch(S,o,m,&k,&l,&c);
@@ -1177,7 +1179,7 @@ extern "C" int hm_scan_condition(hm_scan *s, int ethresh, int do_trim, int do_sy
       S.s = s; S.D = D; S.keys = D->keys; S.klo = D->keys_lo; S.cnt = D->cnt; S.n = s->n; S.chunk = s->n > 0 ? s->n : 1;
       TRY(cudaSetDevice(D->dev));
       TRY(dev_alloc(D,&d_hist,8*np));
-      if (rc == HM_OK) rc = cond_histogram(&S,P.ethr,1,P.hb,d_hist,hist);
+      if (rc == HM_OK) rc = cond_histogram(&S,0,s->n,P.ethr,1,P.hb,d_hist,hist);
       dev_free(D,d_hist);
       s->launches += 1;
       total = 0;
@@ -1296,12 +1298,13 @@ static int names_source(const hm_host_table *t, const char *dst)
 }
 
 /* one range's records, from the device to the table files on a host thread: pinned pieces, the copy of the next
- * piece overlapping the write of this one                                                                  */
+ * piece overlapping the write of this one.  Appended (one GPU: the thread announces the buckets first), or
+ * written at the ordinal the range was placed at (several GPUs)                                             */
 typedef struct
-  { int             dev, pbyte, rc;
+  { int             dev, pbyte, rc, positional;
     hm_table_writer *w;
     const uint8_t  *d_rec;
-    int64_t         n, b0, nb, *counts, pin_bytes;
+    int64_t         n, b0, nb, *counts, pin_bytes, first;
     uint8_t        *pin[2];
     cudaStream_t    st;
     double          ms;
@@ -1313,7 +1316,8 @@ static void *write_worker(void *p)
   double    t0 = now_ms();
   int64_t   per = J->pin_bytes/J->pbyte;
   cudaError_t e = cudaSetDevice(J->dev);
-  J->rc = e != cudaSuccess ? hm_cuda_fail(e,"writer thread") : hm_table_write_buckets(J->w,J->b0,J->nb,J->counts);
+  J->rc = e != cudaSuccess ? hm_cuda_fail(e,"writer thread")
+                           : J->positional ? HM_OK : hm_table_write_buckets(J->w,J->b0,J->nb,J->counts);
   if (J->rc == HM_OK && J->n > 0)
     { e = cudaMemcpyAsync(J->pin[0],J->d_rec,(size_t) ((J->n < per ? J->n : per)*J->pbyte),cudaMemcpyDeviceToHost,J->st);
       for (int64_t o = 0, i = 0; o < J->n && J->rc == HM_OK; o += per, i++)
@@ -1324,7 +1328,8 @@ static void *write_worker(void *p)
               e = cudaMemcpyAsync(J->pin[(i+1)&1],J->d_rec+(o+per)*J->pbyte,(size_t) (m2*J->pbyte),cudaMemcpyDeviceToHost,J->st);
             }
           if (e != cudaSuccess) { J->rc = hm_cuda_fail(e,"records to the host"); break; }
-          J->rc = hm_table_write_append(J->w,J->pin[i&1],m);
+          J->rc = J->positional ? hm_table_write_at(J->w,J->first+o,J->pin[i&1],m)
+                                : hm_table_write_append(J->w,J->pin[i&1],m);
         }
       cudaStreamSynchronize(J->st);
     }
@@ -1332,6 +1337,260 @@ static void *write_worker(void *p)
     { strncpy(J->msg,hm_last_error(),sizeof(J->msg)-1); J->msg[sizeof(J->msg)-1] = 0; }
   J->ms += now_ms()-t0;
   return NULL;
+}
+
+static int g_cond_gpus = 1;
+
+extern "C" int hm_set_condition_gpus(int n)
+{ const int was = g_cond_gpus;
+  g_cond_gpus = n > 1 ? n : 1;
+  return was;
+}
+
+/* what one GPU of hm_scan_condition_files holds: its source (the host table through its own loader, or its
+ * resident replica), the fixed part and the range buffers, and its writer thread                           */
+typedef struct
+  { DevTable           *D;
+    CondSrc             src;
+    hm_cond_bufs        B;
+    int64_t            *d_index;
+    uint64_t           *ck, *cl;
+    uint16_t           *cc;
+    unsigned long long *d_hist, *tiles;
+    Stager              G;
+    WriteJob            J;
+    pthread_t           th;
+    int                 writing;
+    int64_t            *hist, *hcnt;      /* host: this GPU's share of the histogram; a range's bucket counts */
+    int64_t             held0, peak0, out, ranges;
+    int                 rc;
+    char                msg[512];
+  } CondGpu;
+
+typedef struct
+  { CondGpu        *gpu;
+    int             n_gpus, ethr, do_symm, hb, ibyte;
+    int64_t         n, n_ranges, *cuts;
+    hm_table_writer *w;
+    pthread_mutex_t mu;                    /* (several GPUs) ranges are placed in order: `next` is due       */
+    pthread_cond_t  cv;
+    int64_t         next;
+    volatile int    stop;                  /* a GPU failed: the others leave at their next range             */
+  } CondRun;
+
+/* GPU g's share of the source: the fixed part (stub index, bucket counts, histogram, counters) and the chunk
+ * buffers + loader, or (resident) tile counts for chunks of its replica                                      */
+static int cond_gpu_open(hm_scan *s, CondGpu *C, DevTable *D, const hm_host_table *t, int resident, int64_t chunk,
+                         int np_bits, int ethr, int do_symm)
+{ const int64_t ixlen = (int64_t) 1 << (8*t->ibyte), np = (int64_t) 1 << np_bits;
+  int rc = HM_OK;
+  cudaError_t e;
+  C->D = D;
+  HM_CUDA(cudaSetDevice(D->dev));
+  C->held0 = D->held; C->peak0 = D->peak;
+  D->peak = D->held;
+  C->B.kmer = s->kmer; C->B.ibyte = t->ibyte; C->B.hb = np_bits; C->B.ethresh = ethr; C->B.do_symm = do_symm;
+  C->hist = (int64_t *) calloc((size_t) np,sizeof(int64_t));
+  C->hcnt = (int64_t *) malloc(sizeof(int64_t)*(size_t) ixlen);
+  if (C->hist == NULL || C->hcnt == NULL)
+    return hm_set_error(HM_ENOMEM,"out of host memory");
+  if (!resident) TRY(dev_alloc(D,&C->d_index,8*ixlen));
+  TRY(dev_alloc(D,&C->B.bcount,8*ixlen));
+  TRY(dev_alloc(D,&C->d_hist,8*np));
+  TRY(dev_alloc(D,&C->B.ctr,256));
+  if (!resident)
+    { TRY(dev_alloc(D,&C->ck,8*(chunk+1)));
+      if (s->kmer > 32) TRY(dev_alloc(D,&C->cl,8*(chunk+1)));
+      TRY(dev_alloc(D,&C->cc,2*(chunk+8)));
+    }
+  TRY(dev_alloc(D,&C->tiles,hm_cond_tiles_bytes(chunk)));
+  if (!resident)
+    { TRY(cudaMemcpyAsync(C->d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,D->st));
+      if (rc == HM_OK)
+        rc = stager_open(s,D,t,chunk,&C->G);
+      C->src.t = t; C->src.d_index = C->d_index; C->src.G = &C->G;
+      C->src.keys = C->ck; C->src.klo = C->cl; C->src.cnt = C->cc;
+    }
+  else
+    { C->src.keys = D->keys; C->src.klo = D->keys_lo; C->src.cnt = D->cnt; }
+  C->src.s = s; C->src.D = D; C->src.n = t->nels; C->src.chunk = chunk;
+  return rc;
+}
+
+/* the range buffers, sized for the largest range */
+static int cond_gpu_range_bufs(CondGpu *C, int64_t T, int pbyte)
+{ DevTable *D = C->D;
+  hm_cond_bufs *B = &C->B;
+  const int two = B->kmer > 32;
+  int rc = HM_OK;
+  cudaError_t e;
+  B->cap = T;
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&B->key,8*T));
+  if (two) TRY(dev_alloc(D,&B->lo,8*T));
+  TRY(dev_alloc(D,&B->cnt,2*T));
+  TRY(dev_alloc(D,&B->rec,pbyte*T));
+  if (B->do_symm)
+    { TRY(dev_alloc(D,&B->alt_key,8*T));
+      TRY(dev_alloc(D,&B->alt_cnt,2*T));
+      TRY(dev_alloc(D,&B->m_key,8*T));
+      TRY(dev_alloc(D,&B->m_cnt,2*T));
+      if (two)
+        { TRY(dev_alloc(D,&B->alt_lo,8*T));
+          TRY(dev_alloc(D,&B->m_lo,8*T));
+          TRY(dev_alloc(D,&B->idx[0],4*T));
+          TRY(dev_alloc(D,&B->idx[1],4*T));
+        }
+      TRY(dev_alloc(D,&B->mtiles,2*hm_cond_tiles_bytes(T)));
+      B->sort_bytes = hm_cond_sort_room(T);
+      TRY(dev_alloc(D,&B->sort_tmp,B->sort_bytes));
+    }
+  if (rc == HM_OK)
+    { C->J.dev = D->dev; C->J.pbyte = pbyte; C->J.d_rec = B->rec;
+      C->J.pin_bytes = (int64_t) pbyte*((64ll << 20)/pbyte);
+      TRY(cudaStreamCreateWithFlags(&C->J.st,cudaStreamNonBlocking));
+      TRY(cudaHostAlloc(&C->J.pin[0],(size_t) C->J.pin_bytes,cudaHostAllocDefault));
+      TRY(cudaHostAlloc(&C->J.pin[1],(size_t) C->J.pin_bytes,cudaHostAllocDefault));
+    }
+  return rc;
+}
+
+/* everything GPU C allocated goes; the scan's own residency report is left as it was */
+static void cond_gpu_close(CondGpu *C)
+{ DevTable *D = C->D;
+  hm_cond_bufs *B = &C->B;
+  if (D == NULL)
+    return;
+  cudaSetDevice(D->dev);
+  stager_close(D,&C->G);
+  cudaStreamSynchronize(D->st);
+  void *mine[] = { C->d_index, B->bcount, C->d_hist, B->ctr, C->ck, C->cl, C->cc, C->tiles, B->key, B->lo, B->cnt,
+                   B->rec, B->alt_key, B->alt_cnt, B->m_key, B->m_cnt, B->alt_lo, B->m_lo, B->idx[0], B->idx[1],
+                   B->mtiles, B->sort_tmp };
+  for (size_t k = 0; k < sizeof(mine)/sizeof(mine[0]); k++)
+    dev_free(D,mine[k]);
+  cudaStreamSynchronize(D->st);
+  if (C->J.st) cudaStreamDestroy(C->J.st);
+  if (C->J.pin[0]) cudaFreeHost(C->J.pin[0]);
+  if (C->J.pin[1]) cudaFreeHost(C->J.pin[1]);
+  D->peak = C->peak0 > D->held ? C->peak0 : D->held;
+  free(C->hist); free(C->hcnt);
+}
+
+/* pass 0 on GPU g: its contiguous slice of the source ordinals */
+static int cond_gpu_hist(CondRun *R, int g)
+{ CondGpu *C = R->gpu+g;
+  HM_CUDA(cudaSetDevice(C->D->dev));
+  return cond_histogram(&C->src,R->n*g/R->n_gpus,R->n*(g+1)/R->n_gpus,R->ethr,R->do_symm,R->hb,C->d_hist,C->hist);
+}
+
+static int writer_join(CondGpu *C)
+{ if (!C->writing)
+    return HM_OK;
+  pthread_join(C->th,NULL);
+  C->writing = 0;
+  return C->J.rc != HM_OK ? hm_set_error(C->J.rc,"%s",C->J.msg) : HM_OK;
+}
+
+/* the other GPUs stop at their next range; those waiting to place theirs are let go */
+static void cond_stop(CondRun *R)
+{ pthread_mutex_lock(&R->mu);
+  R->stop = 1;
+  pthread_cond_broadcast(&R->cv);
+  pthread_mutex_unlock(&R->mu);
+}
+
+/* passes 1..R on GPU g: ranges g, g + G, ...  One GPU appends; several place each range once every earlier one is
+ * placed (placing waits only for the placing of the range before, never for a write), then write it at its
+ * offsets                                                                                                     */
+static int cond_gpu_ranges(CondRun *R, int g)
+{ CondGpu      *C = R->gpu+g;
+  DevTable     *D = C->D;
+  const int     hb = R->hb, ibyte = R->ibyte, several = R->n_gpus > 1;
+  int           rc = HM_OK;
+  cudaError_t   e;
+  TRY(cudaSetDevice(D->dev));
+  for (int64_t r = g; r < R->n_ranges && rc == HM_OK && !R->stop; r += R->n_gpus)
+    { const uint64_t p0 = (uint64_t) R->cuts[r], p1 = (uint64_t) R->cuts[r+1];
+      int64_t n_r = 0;
+      rc = cond_range(&C->src,&C->B,p0,p1,C->tiles,&n_r);
+      /* the stub buckets the range's keys fall in */
+      const uint64_t b0 = 8*ibyte >= hb ? p0 << (8*ibyte-hb) : p0 >> (hb-8*ibyte);
+      const uint64_t b1 = 8*ibyte >= hb ? p1 << (8*ibyte-hb) : ((p1-1) >> (hb-8*ibyte)) + 1;
+      const int rw = writer_join(C);                            /* the last range's records have left B.rec */
+      if (rc == HM_OK) rc = rw;
+      if (rc == HM_OK) rc = hm_cond_pack(&C->B,n_r,b0,(int64_t) (b1-b0),D->st);
+      TRY(cudaMemcpyAsync(C->hcnt,C->B.bcount,8*(size_t) (b1-b0),cudaMemcpyDeviceToHost,D->st));
+      TRY(cudaStreamSynchronize(D->st));
+      C->J.n = n_r; C->J.b0 = (int64_t) b0; C->J.nb = (int64_t) (b1-b0); C->J.counts = C->hcnt;
+      if (rc == HM_OK && several)
+        { pthread_mutex_lock(&R->mu);
+          while (R->next != r && !R->stop)
+            pthread_cond_wait(&R->cv,&R->mu);
+          if (!R->stop)
+            { rc = hm_table_write_place(R->w,C->J.b0,C->J.nb,C->hcnt,&C->J.first);
+              R->next = r+1;
+            }
+          pthread_cond_broadcast(&R->cv);
+          pthread_mutex_unlock(&R->mu);
+          if (R->stop && rc == HM_OK)
+            break;
+        }
+      if (rc == HM_OK)
+        { C->J.positional = several;
+          C->out += n_r;
+          if (pthread_create(&C->th,NULL,write_worker,&C->J) == 0) C->writing = 1;
+          else                                                  write_worker(&C->J);
+          if (!C->writing && C->J.rc != HM_OK) rc = hm_set_error(C->J.rc,"%s",C->J.msg);
+        }
+      C->ranges++;
+    }
+  if (rc != HM_OK && several)
+    cond_stop(R);
+  const int rw = writer_join(C);
+  return rc != HM_OK ? rc : rw;
+}
+
+typedef int (*CondFn)(CondRun *R, int g);
+typedef struct { CondRun *R; CondFn fn; int g; } CondTask;
+
+static void *cond_worker(void *p)
+{ CondTask *T = (CondTask *) p;
+  CondGpu  *C = T->R->gpu+T->g;
+  C->rc = T->fn(T->R,T->g);
+  if (C->rc != HM_OK)
+    { strncpy(C->msg,hm_last_error(),sizeof(C->msg)-1); C->msg[sizeof(C->msg)-1] = 0; }
+  return NULL;
+}
+
+/* fn on every GPU of the call at once, a host thread each (the calling thread takes the last); the first
+ * failing GPU's error, naming it when there are several.  The GPUs wait for each other (ranges are placed in
+ * order), so one cannot run after another: a thread that cannot be started stops the call.                  */
+static int cond_on_gpus(CondRun *R, CondFn fn)
+{ const int G = R->n_gpus;
+  CondTask  task[HM_MAX_GPUS];
+  pthread_t th[HM_MAX_GPUS];
+  int       made = 0, rc = HM_OK;
+  if (G == 1)
+    return fn(R,0);
+  for (int g = 0; g < G; g++)
+    { task[g].R = R; task[g].fn = fn; task[g].g = g;
+      R->gpu[g].rc = HM_OK;
+    }
+  while (made < G-1 && pthread_create(th+made,NULL,cond_worker,task+made) == 0)
+    made++;
+  if (made == G-1)
+    cond_worker(task+G-1);
+  else
+    { cond_stop(R);
+      rc = hm_set_error(HM_ENOMEM,"conditioning on %d GPUs: cannot start the host thread of GPU %d",G,made);
+    }
+  for (int g = 0; g < made; g++)
+    pthread_join(th[g],NULL);
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    if (R->gpu[g].rc != HM_OK)
+      rc = hm_set_error(R->gpu[g].rc,"conditioning on GPU %d (%d of %d): %s",R->gpu[g].D->dev,g,G,R->gpu[g].msg);
+  return rc;
 }
 
 extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
@@ -1348,157 +1607,98 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
   if (names_source(t,dst))
     return hm_set_error(HM_EINVAL,"%s names the source table: conditioning writes a new table",dst);
 
-  DevTable *D = s->d;
-  const int kmer = s->kmer, ibyte = t->ibyte, KW = kmer > 32 ? 2 : 1;
+  const int G = g_cond_gpus < s->ngpu ? g_cond_gpus : s->ngpu;
+  const int resident = G > 1 && !s->streamed;     /* several GPUs of an in-core scan read their replicas */
+  const int kmer = s->kmer, ibyte = t->ibyte;
   const int pbyte = ((kmer+3)>>2) - ibyte + 2;
   const int hb = cond_hist_bits(kmer);
   const int64_t n = t->nels, np = (int64_t) 1 << hb, ixlen = (int64_t) 1 << (8*ibyte);
   const int ethr = do_trim ? ethresh : 0;
   int       rc = HM_OK;
-  cudaError_t e;
-  HM_CUDA(cudaSetDevice(D->dev));
-  /* what the call may hold: an explicit budget covers the scan too (as hm_scan_condition counts its table), so
-   * the scan's resident arrays come off it; the default one is free memory, which already excludes them       */
-  const int64_t budget = g_budget > 0 ? g_budget - D->held : device_budget(&D->dev,1);
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  /* what the call may hold on each GPU: an explicit budget covers the scan too (as hm_scan_condition counts its
+   * table), so the scan's resident arrays come off it; the default one is free memory, which already excludes
+   * them.  The plan takes the smallest.                                                                      */
+  int dev[HM_MAX_GPUS] = { 0 };
+  for (int g = 0; g < G; g++) dev[g] = s->d[g].dev;
+  int64_t budget = g_budget > 0 ? g_budget - s->d[0].held : device_budget(dev,G);
+  for (int g = 1; g < G && g_budget > 0; g++)
+    if (g_budget - s->d[g].held < budget) budget = g_budget - s->d[g].held;
 
   hm_condition_stats S;
   memset(&S,0,sizeof(S));
   S.nels_in = n;
   S.budget_bytes = budget;
+  S.gpus = G;
   hm_condition_layout lay;
   int64_t *hist = (int64_t *) calloc((size_t) np,sizeof(int64_t));
   int64_t *cuts = (int64_t *) malloc(sizeof(int64_t)*(size_t) (np+1));
-  int64_t *hcnt = (int64_t *) malloc(sizeof(int64_t)*(size_t) ixlen);
-  if (hist == NULL || cuts == NULL || hcnt == NULL)
-    { free(hist); free(cuts); free(hcnt); return hm_set_error(HM_ENOMEM,"out of host memory"); }
+  CondGpu *gpu  = (CondGpu *) calloc((size_t) G,sizeof(CondGpu));
+  if (hist == NULL || cuts == NULL || gpu == NULL)
+    { free(hist); free(cuts); free(gpu); return hm_set_error(HM_ENOMEM,"out of host memory"); }
   /* the fixed part and a chunk must fit before the source is read (an empty histogram asks nothing more) */
   if ((rc = hm_condition_plan(n,kmer,ibyte,budget,do_symm,hist,hb,cuts,&lay)) != HM_OK)
-    { free(hist); free(cuts); free(hcnt); return rc; }
-  const int64_t chunk = lay.chunk;
+    { free(hist); free(cuts); free(gpu); return rc; }
 
-  const int64_t held0 = D->held, peak0 = D->peak;
-  D->peak = D->held;
-  hm_cond_bufs B;
-  memset(&B,0,sizeof(B));
-  B.kmer = kmer; B.ibyte = ibyte; B.hb = hb; B.ethresh = ethr; B.do_symm = do_symm;
-  int64_t *d_index = NULL;
-  uint64_t *ck = NULL, *cl = NULL;
-  uint16_t *cc = NULL;
-  unsigned long long *d_hist = NULL, *tiles = NULL;
-  Stager    G;
-  memset(&G,0,sizeof(G));
-  hm_table_writer *w = NULL;
-  WriteJob  J;
-  memset(&J,0,sizeof(J));
-  pthread_t th;
-  int       writing = 0;
-  TRY(dev_alloc(D,&d_index,8*ixlen));
-  TRY(dev_alloc(D,&B.bcount,8*ixlen));
-  TRY(dev_alloc(D,&d_hist,8*np));
-  TRY(dev_alloc(D,&B.ctr,256));
-  TRY(dev_alloc(D,&ck,8*(chunk+1)));
-  if (KW == 2) TRY(dev_alloc(D,&cl,8*(chunk+1)));
-  TRY(dev_alloc(D,&cc,2*(chunk+8)));
-  TRY(dev_alloc(D,&tiles,hm_cond_tiles_bytes(chunk)));
-  TRY(cudaMemcpyAsync(d_index,t->index,8*(size_t) ixlen,cudaMemcpyHostToDevice,D->st));
-  if (rc == HM_OK)
-    rc = stager_open(s,D,t,chunk,&G);
-  CondSrc src = { s, D, t, d_index, &G, ck, cl, cc, n, chunk };
+  CondRun R;
+  memset(&R,0,sizeof(R));
+  R.gpu = gpu; R.n_gpus = G; R.ethr = ethr; R.do_symm = do_symm; R.hb = hb; R.ibyte = ibyte; R.n = n;
+  R.cuts = cuts;
+  pthread_mutex_init(&R.mu,NULL);
+  pthread_cond_init(&R.cv,NULL);
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    rc = cond_gpu_open(s,gpu+g,s->d+g,t,resident,lay.chunk,hb,ethr,do_symm);
 
-  /* pass 0: the output histogram */
+  /* pass 0: the output histogram, a slice of the source per GPU */
   if (rc == HM_OK)
-    rc = cond_histogram(&src,ethr,do_symm,hb,d_hist,hist);
+    rc = cond_on_gpus(&R,cond_gpu_hist);
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    for (int64_t p = 0; p < np; p++) hist[p] += gpu[g].hist[p];
   S.ms_hist = now_ms()-t0;
   if (rc == HM_OK)
     rc = hm_condition_plan(n,kmer,ibyte,budget,do_symm,hist,hb,cuts,&lay);
   int64_t hint = 0;
   for (int64_t p = 0; p < np; p++) hint += hist[p];
 
-  /* the range buffers, sized for the largest range */
   const int64_t T = lay.range_cap > 0 ? lay.range_cap : 1;
-  B.cap = T;
-  TRY(dev_alloc(D,&B.key,8*T));
-  if (KW == 2) TRY(dev_alloc(D,&B.lo,8*T));
-  TRY(dev_alloc(D,&B.cnt,2*T));
-  TRY(dev_alloc(D,&B.rec,pbyte*T));
-  if (do_symm)
-    { TRY(dev_alloc(D,&B.alt_key,8*T));
-      TRY(dev_alloc(D,&B.alt_cnt,2*T));
-      TRY(dev_alloc(D,&B.m_key,8*T));
-      TRY(dev_alloc(D,&B.m_cnt,2*T));
-      if (KW == 2)
-        { TRY(dev_alloc(D,&B.alt_lo,8*T));
-          TRY(dev_alloc(D,&B.m_lo,8*T));
-          TRY(dev_alloc(D,&B.idx[0],4*T));
-          TRY(dev_alloc(D,&B.idx[1],4*T));
-        }
-      TRY(dev_alloc(D,&B.mtiles,2*hm_cond_tiles_bytes(T)));
-      B.sort_bytes = hm_cond_sort_room(T);
-      TRY(dev_alloc(D,&B.sort_tmp,B.sort_bytes));
-    }
+  for (int g = 0; g < G && rc == HM_OK; g++)
+    rc = cond_gpu_range_bufs(gpu+g,T,pbyte);
   if (rc == HM_OK)
     rc = hm_table_write_open(dst,kmer,ibyte,do_trim && ethresh > t->minval ? ethresh : t->minval,
-                             t->nparts > 0 ? t->nparts : 1,hint,&w);
-  if (rc == HM_OK)
-    { J.dev = D->dev; J.pbyte = pbyte; J.w = w; J.d_rec = B.rec;
-      J.pin_bytes = (int64_t) pbyte*((64ll << 20)/pbyte);
-      TRY(cudaStreamCreateWithFlags(&J.st,cudaStreamNonBlocking));
-      TRY(cudaHostAlloc(&J.pin[0],(size_t) J.pin_bytes,cudaHostAllocDefault));
-      TRY(cudaHostAlloc(&J.pin[1],(size_t) J.pin_bytes,cudaHostAllocDefault));
-    }
+                             t->nparts > 0 ? t->nparts : 1,hint,&R.w);
+  for (int g = 0; g < G; g++)
+    gpu[g].J.w = R.w;
 
   /* passes 1..R: a key range each */
   double t_ranges = now_ms();
-  for (int r = 0; r < lay.n_ranges && rc == HM_OK; r++)
-    { const uint64_t p0 = (uint64_t) cuts[r], p1 = (uint64_t) cuts[r+1];
-      int64_t n_r = 0;
-      rc = cond_range(&src,&B,p0,p1,tiles,&n_r);
-      /* the stub buckets the range's keys fall in */
-      const uint64_t b0 = 8*ibyte >= hb ? p0 << (8*ibyte-hb) : p0 >> (hb-8*ibyte);
-      const uint64_t b1 = 8*ibyte >= hb ? p1 << (8*ibyte-hb) : ((p1-1) >> (hb-8*ibyte)) + 1;
-      if (writing)                                             /* the last range's records have left B.rec */
-        { pthread_join(th,NULL); writing = 0;
-          if (J.rc != HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
-        }
-      if (rc == HM_OK) rc = hm_cond_pack(&B,n_r,b0,(int64_t) (b1-b0),D->st);
-      TRY(cudaMemcpy(hcnt,B.bcount,8*(size_t) (b1-b0),cudaMemcpyDeviceToHost));
-      if (rc == HM_OK)
-        { J.n = n_r; J.b0 = (int64_t) b0; J.nb = (int64_t) (b1-b0); J.counts = hcnt;
-          S.nels_out += n_r;
-          if (pthread_create(&th,NULL,write_worker,&J) == 0) writing = 1;
-          else                                                write_worker(&J);
-          if (!writing && J.rc != HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
-        }
-      S.ranges++;
-    }
-  if (writing)
-    { pthread_join(th,NULL);
-      if (J.rc != HM_OK && rc == HM_OK) rc = hm_set_error(J.rc,"%s",J.msg);
-    }
+  R.n_ranges = lay.n_ranges;
+  if (rc == HM_OK)
+    rc = cond_on_gpus(&R,cond_gpu_ranges);
   S.ms_ranges = now_ms()-t_ranges;
-  if (w != NULL)
-    { int rw = rc == HM_OK ? hm_table_write_close(w) : (hm_table_write_abort(w), HM_OK);
+  if (R.w != NULL)
+    { int rw = rc == HM_OK ? hm_table_write_close(R.w) : (hm_table_write_abort(R.w), HM_OK);
       if (rc == HM_OK) rc = rw;
     }
 
-  /* everything the call allocated goes; the scan's own residency report is left as it was */
-  stager_close(D,&G);
-  cudaStreamSynchronize(D->st);
-  void *mine[] = { d_index, B.bcount, d_hist, B.ctr, ck, cl, cc, tiles, B.key, B.lo, B.cnt, B.rec, B.alt_key, B.alt_cnt,
-                   B.m_key, B.m_cnt, B.alt_lo, B.m_lo, B.idx[0], B.idx[1], B.mtiles, B.sort_tmp };
-  for (size_t k = 0; k < sizeof(mine)/sizeof(mine[0]); k++)
-    dev_free(D,mine[k]);
-  cudaStreamSynchronize(D->st);
-  if (J.st) cudaStreamDestroy(J.st);
-  if (J.pin[0]) cudaFreeHost(J.pin[0]);
-  if (J.pin[1]) cudaFreeHost(J.pin[1]);
-  S.peak_bytes = D->peak-held0;
-  D->peak = peak0 > D->held ? peak0 : D->held;
-  free(hist); free(cuts); free(hcnt);
+  for (int g = 0; g < G; g++)
+    { CondGpu *C = gpu+g;
+      if (C->D != NULL)
+        { const int64_t peak = C->D->peak - C->held0;
+          if (peak > S.peak_bytes) S.peak_bytes = peak;
+          if (g < HM_COND_MAX_GPUS) S.gpu_peak_bytes[g] = peak;
+        }
+      S.nels_out += C->out;
+      S.ranges += (int32_t) C->ranges;
+      S.ms_write += C->J.ms;
+      if (C->J.ms > S.ms_write_max) S.ms_write_max = C->J.ms;
+      cond_gpu_close(C);
+    }
+  pthread_mutex_destroy(&R.mu);
+  pthread_cond_destroy(&R.cv);
+  free(hist); free(cuts); free(gpu);
   S.passes = S.ranges+1;
-  S.bytes_read = (int64_t) S.passes*n*pbyte;
+  S.bytes_read = resident ? 0 : (int64_t) S.passes*n*pbyte;
   S.bytes_written = 16 + 8*ixlen + 12ll*(t->nparts > 0 ? t->nparts : 1) + S.nels_out*pbyte;
-  S.ms_write = J.ms;
   S.ms_total = now_ms()-t0;
   if (st != NULL) *st = S;
   return rc;

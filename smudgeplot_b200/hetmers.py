@@ -194,21 +194,29 @@ class Scan:
         self.nels = n.value
         return n.value
 
-    def condition_files(self, dst: str, ethresh: int, trim: bool, symm: bool, device_budget: int | None = None):
+    def condition_files(self, dst: str, ethresh: int, trim: bool, symm: bool, device_budget: int | None = None,
+                        gpus: int | None = None):
         """write the trimmed (count >= ethresh) and / or symmetrised table as the FastK table `dst`, one key range
         at a time on the first GPU, for a table of any size (hm_scan_condition_files); the scan itself is left as
         it was.  A `dst` whose files are the source's (kt.name) is refused (HM_EINVAL) before anything is written.
         device_budget sets the process-wide device budget (bytes per GPU, as Scan's does) for this and later calls;
-        an explicit budget counts what the scan already holds on the device.
-        -> stats dict (entries in / out, ranges, passes, peak device bytes, bytes read / written, times)"""
+        an explicit budget counts what the scan already holds on the device.  gpus=n runs this call on the scan's
+        first min(n, its GPUs) devices, the ranges dealt round-robin and written at their offsets by a thread per
+        GPU (hm_set_condition_gpus; the files are the same); None keeps the process-wide setting (default 1).
+        -> stats dict (entries in / out, ranges, passes, peak device bytes, bytes read / written, times, gpus)"""
         from .fastk import same_table_files
         if self.kt.name is not None and same_table_files(self.kt.name, self.kt.nparts, str(dst)):
             raise _lib.HetmersError(-1, f"{dst} names the source table: conditioning writes a new table")
         if device_budget is not None:
             self._L.hm_set_device_budget(int(device_budget))
         st = _lib.ConditionStats()
-        _lib.check(self._L.hm_scan_condition_files(self._h, int(ethresh), int(trim), int(symm), str(dst).encode(),
-                                                   C.byref(st)))
+        was = self._L.hm_set_condition_gpus(int(gpus)) if gpus is not None else None
+        try:
+            _lib.check(self._L.hm_scan_condition_files(self._h, int(ethresh), int(trim), int(symm), str(dst).encode(),
+                                                       C.byref(st)))
+        finally:
+            if was is not None:
+                self._L.hm_set_condition_gpus(was)
         return st.as_dict()
 
     PATHS = {"auto": 0, "direct": 1, "symm": 2}
@@ -322,18 +330,19 @@ def scan_table(kt: KtabFiles, gpus: int = 1):
     return plot.reshape(_lib.SMAX + 1, _lib.PLOT_W), st.as_dict()
 
 
-def condition_table(src, dst, L: int, device_budget: int | None = None):
+def condition_table(src, dst, L: int, device_budget: int | None = None, gpus: int | None = None):
     """`condition_kmer_table` in process: examine `src` as hetmers does (-e L) and write it trimmed and / or
     symmetrised as needed to `dst`, streaming it through the GPU if it is larger.  device_budget sets the
-    process-wide device budget, as Scan's does.  -> stats dict, or None when the table needs neither step
-    (nothing is written).  A `dst` naming `src` is refused (HM_EINVAL) before anything is written."""
+    process-wide device budget, as Scan's does.  gpus=n scans and conditions on devices 0..n-1 (what
+    HETMERS_GPUS=n does for the executable); None keeps one GPU.  -> stats dict, or None when the table needs
+    neither step (nothing is written).  A `dst` naming `src` is refused (HM_EINVAL) before anything is written."""
     if device_budget is not None:
         _lib.lib().hm_set_device_budget(int(device_budget))
-    with Scan(read_ktab(str(src), mmap=True)) as sc:
+    with Scan(read_ktab(str(src), mmap=True), gpus=1 if gpus is None else int(gpus)) as sc:
         trim, symm = sc.examine(int(L))
         if trim and symm:
             return None
-        return sc.condition_files(dst, int(L), not trim, not symm)
+        return sc.condition_files(dst, int(L), not trim, not symm, gpus=gpus)
 
 
 def smu_text(plot: np.ndarray) -> str:

@@ -8,12 +8,15 @@
  * It takes hetmers' decisions (hm_scan_examine with the same -e): trim if the table is untrimmed,
  * symmetrise if the probe finds it not symmetric; -v prints hetmers' verdict and step lines.  A table
  * that needs neither is left alone: nothing is written and the exit code is 0.  Tables larger than the
- * GPU are streamed (HETMERS_DEVICE_BUDGET and HETMERS_STREAM as for hetmers); one GPU (device 0).
+ * GPU are streamed (HETMERS_DEVICE_BUDGET and HETMERS_STREAM as for hetmers).  HETMERS_GPUS=<n>|all (default 1,
+ * as for hetmers) scans on devices 0..n-1 and conditions on all of them: the key ranges are dealt round-robin and
+ * each GPU's writer thread writes its ranges' records at their offsets; the files are those of one GPU.
  * Then `hetmers <target>` finds the table trimmed and symmetric and scans it, streamed if it must.
  *******************************************************************************************/
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <strings.h>
 
 #include "hetmers_b200.h"
 
@@ -31,6 +34,29 @@ static int positive_arg(const char *arg, const char *what)
       exit (1);
     }
   return ((int) v);
+}
+
+/* HETMERS_GPUS as hetmers reads it: <n> or "all", default 1, at most the visible devices (with a warning) and 16;
+ * main has already refused a machine with no visible device                                                  */
+static int pick_gpus(int *devs)
+{ int ngpu = 1, navail = hm_device_count(), i;
+  const char *g = getenv("HETMERS_GPUS");
+
+  if (g != NULL && *g != '\0')
+    { if (strcasecmp(g,"all") == 0)
+        ngpu = navail;
+      else
+        ngpu = atoi(g);
+      if (ngpu < 1) ngpu = 1;
+      if (ngpu > navail)
+        { fprintf(stderr,"%s: Warning, only %d GPUs are visible\n",Prog_Name,navail);
+          ngpu = navail;
+        }
+    }
+  if (ngpu > 16) ngpu = 16;
+  for (i = 0; i < ngpu; i++)
+    devs[i] = i;
+  return (ngpu);
 }
 
 static void die_hm(void)
@@ -81,7 +107,7 @@ int main(int argc, char *argv[])
 
   hm_table *T;
   hm_scan  *S;
-  int       dev = 0, trim, symm;
+  int       dev[16], ngpu, trim, symm;
 
   if (hm_table_open(argv[1],&T) != HM_OK)
     { if (strncmp(hm_last_error(),"Cannot open",11) == 0)
@@ -99,8 +125,10 @@ int main(int argc, char *argv[])
     if (b != NULL && *b != '\0')
       hm_set_device_budget(strtoll(b,NULL,10));
   }
-  if (hm_scan_create(hm_table_view(T),&dev,1,&S) != HM_OK)
+  ngpu = pick_gpus(dev);
+  if (hm_scan_create(hm_table_view(T),dev,ngpu,&S) != HM_OK)
     die_hm();
+  hm_set_condition_gpus(ngpu);
   if (hm_scan_examine(S,ETHRESH,&trim,&symm) != HM_OK)
     die_hm();
 
@@ -126,7 +154,10 @@ int main(int argc, char *argv[])
   hm_condition_stats st;
   if (hm_scan_condition_files(S,ETHRESH,!trim,!symm,argv[2],&st) != HM_OK)
     die_hm();
-  if (VERBOSE)
+  if (VERBOSE && st.gpus > 1)
+    fprintf(stderr,"\n  Wrote %lld k-mers to %s (%d key ranges, %d passes over the source, %d GPUs)\n",
+            (long long) st.nels_out,argv[2],st.ranges,st.passes,st.gpus);
+  else if (VERBOSE)
     fprintf(stderr,"\n  Wrote %lld k-mers to %s (%d key ranges, %d passes over the source)\n",
             (long long) st.nels_out,argv[2],st.ranges,st.passes);
 

@@ -12,10 +12,12 @@
 #define _GNU_SOURCE
 #include <errno.h>
 #include <fcntl.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <strings.h>
+#include <pthread.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -196,7 +198,16 @@ fail:
  * bucket's start when there are fewer entries).  That bucket may have begun before the ordinal is
  * reached, so a cut moves the bucket's records written so far from the old part to the new one --
  * at most one bucket's worth per part.  Everything is written under temporary names and renamed into
- * place by hm_table_write_close; any failure removes the temporaries.                             */
+ * place by hm_table_write_close; any failure removes the temporaries.
+ *
+ * Positional mode (hm_table_write_place / _at / _seal): ranges are announced in table order, each getting its
+ * first ordinal, and their records are written at their final offsets by any thread in any order.  A cut is
+ * fixed the moment the bucket holding its ordinal is announced (at that bucket's start, as the append path
+ * cuts); until then it lies at or after the start of the last bucket announced, so only records of that bucket
+ * can be in doubt.  hm_table_write_at never waits: it copies those records and the place or seal that settles
+ * them writes them (at most one bucket's records are held).  Nothing written is ever moved.                 */
+typedef struct pending { int64_t first, n; struct pending *next; uint8_t rec[]; } pending;
+
 struct hm_table_writer
   { int      kmer, ibyte, minval, nparts, pbyte, part;   /* part: the one being written (0-based)  */
     int64_t  hint, ixlen;
@@ -207,6 +218,11 @@ struct hm_table_writer
     int     *fd;                       /* [nparts] temporary part files                            */
     char    *dir, *root, *tmp_tag;
     int      failed;
+    int      positional, sealed, known;/* (positional) part_first[0, known) is fixed               */
+    int64_t  last_start;               /* (positional) first ordinal of the last bucket announced  */
+    struct pending *held;              /* (positional) records written while their part was open  */
+    int64_t  held_from;                /*   the open ordinal they wait on (the last bucket's start)*/
+    pthread_mutex_t mu;                /* (positional) guards the above, declared and written      */
   };
 
 static char *writer_path(const hm_table_writer *w, int part, int tmp)   /* part 0 = the stub */
@@ -244,6 +260,12 @@ static void writer_free(hm_table_writer *w, int unlink_tmp)
       if (q != NULL) { unlink(q); free(q); }
     }
   free(w->count); free(w->part_first); free(w->fd); free(w->dir); free(w->root); free(w->tmp_tag);
+  while (w->held != NULL)
+    { pending *nx = w->held->next;
+      free(w->held);
+      w->held = nx;
+    }
+  pthread_mutex_destroy(&w->mu);
   free(w);
 }
 
@@ -263,6 +285,8 @@ int hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int n
   w->pbyte = ((kmer+3)>>2) - ibyte + 2;
   w->ixlen = (int64_t) 1 << (8*ibyte);
   w->cur = -1;
+  w->known = 1;
+  pthread_mutex_init(&w->mu,NULL);
   w->count      = calloc((size_t) w->ixlen,sizeof(int64_t));
   w->part_first = calloc((size_t) nparts,sizeof(int64_t));
   w->fd         = malloc(sizeof(int)*(size_t) nparts);
@@ -296,7 +320,7 @@ int hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int n
 }
 
 int hm_table_write_buckets(hm_table_writer *w, int64_t b0, int64_t nb, const int64_t *counts)
-{ if (w == NULL || w->failed)
+{ if (w == NULL || w->failed || w->positional)
     return hm_set_error(HM_EINVAL,"hm_table_write_buckets: no usable writer");
   for (int64_t i = 0; i < nb; i++)
     { int64_t b = b0+i;
@@ -351,7 +375,7 @@ static int writer_flush(hm_table_writer *w, const uint8_t *rec, int64_t from)
 }
 
 int hm_table_write_append(hm_table_writer *w, const uint8_t *rec, int64_t n)
-{ if (w == NULL || w->failed)
+{ if (w == NULL || w->failed || w->positional)
     return hm_set_error(HM_EINVAL,"hm_table_write_append: no usable writer");
   if (w->written+n > w->declared)
     { w->failed = 1;
@@ -380,10 +404,163 @@ int hm_table_write_append(hm_table_writer *w, const uint8_t *rec, int64_t n)
   return HM_OK;
 }
 
+/* ---- positional mode ---- */
+
+/* records [first, first+n) at rec into their parts; pf[0, known): the fixed part starts, every cut not yet fixed
+ * lying at or beyond first+n -- the part of ordinal o is the last p with pf[p] <= o                          */
+static int writer_put(const hm_table_writer *w, const int64_t *pf, int known, int64_t first, const uint8_t *rec,
+                      int64_t n)
+{ const int64_t end = first+n;
+  int p = 0;
+  for (int64_t o = first; o < end; )
+    { while (p+1 < known && pf[p+1] <= o) p++;
+      int64_t e = p+1 < known && pf[p+1] < end ? pf[p+1] : end;
+      if (pwrite_all(w->fd[p],rec+(o-first)*w->pbyte,(size_t) (e-o)*w->pbyte,
+                     PART_HEADER + (off_t) (o-pf[p])*w->pbyte) != 0)
+        return hm_set_error(HM_EIO,"writing table part %d: %s",p+1,strerror(errno));
+      o = e;
+    }
+  return HM_OK;
+}
+
+/* the first ordinal whose part may still change: the last bucket's start while a cut is open, else none */
+static int64_t writer_open_from(const hm_table_writer *w)
+{ return w->known < w->nparts && w->hint > 0 ? w->last_start : INT64_MAX; }
+
+/* (mutex held) the part starts fixed so far, copied to *pf (cut or malloc'ed); 0 when out of memory */
+static int writer_cuts(hm_table_writer *w, int64_t *cut, int64_t **pf)
+{ *pf = cut;
+  if (w->known > 64 && (*pf = malloc(sizeof(int64_t)*(size_t) w->known)) == NULL)
+    return 0;
+  memcpy(*pf,w->part_first,sizeof(int64_t)*(size_t) w->known);
+  return 1;
+}
+
+/* (mutex held, released on return) the held records are written once nothing held can change part any more */
+static int writer_release(hm_table_writer *w)
+{ pending *q = NULL;
+  int64_t  cut[64], *pf = cut;
+  int      known = w->known, rc = HM_OK;
+  if (w->held != NULL && !w->failed && writer_open_from(w) > w->held_from)
+    { q = w->held; w->held = NULL;
+      if (!writer_cuts(w,cut,&pf))
+        { w->failed = 1; rc = hm_set_error(HM_ENOMEM,"Out of memory (table writer)"); }
+    }
+  pthread_mutex_unlock(&w->mu);
+  while (q != NULL)
+    { pending *nx = q->next;
+      if (rc == HM_OK) rc = writer_put(w,pf,known,q->first,q->rec,q->n);
+      free(q);
+      q = nx;
+    }
+  if (pf != cut) free(pf);
+  if (rc != HM_OK)
+    { pthread_mutex_lock(&w->mu); w->failed = 1; pthread_mutex_unlock(&w->mu); }
+  return rc;
+}
+
+int hm_table_write_place(hm_table_writer *w, int64_t b0, int64_t nb, const int64_t *counts, int64_t *first)
+{ int rc = HM_OK;
+  if (w == NULL || first == NULL || nb < 0 || (nb > 0 && counts == NULL))
+    return hm_set_error(HM_EINVAL,"hm_table_write_place: bad arguments");
+  pthread_mutex_lock(&w->mu);
+  if (w->failed || w->sealed || (!w->positional && w->declared > 0))
+    rc = hm_set_error(HM_EINVAL,"hm_table_write_place: no usable writer");
+  else
+    w->positional = 1;
+  *first = w->declared;
+  for (int64_t i = 0; i < nb && rc == HM_OK; i++)
+    { int64_t b = b0+i;
+      if (counts[i] == 0)
+        continue;
+      if (b < 0 || b >= w->ixlen || counts[i] < 0 || b < w->last)
+        { w->failed = 1;
+          rc = hm_set_error(HM_EINVAL,"hm_table_write_place: bucket %lld announced out of order",(long long) b);
+          break;
+        }
+      if (w->declared == 0 || b != w->last)                 /* a new bucket starts here */
+        w->last_start = w->declared;
+      w->count[b] += counts[i];
+      w->declared += counts[i];
+      w->last = b;
+      while (w->known < w->nparts && w->hint > 0 && writer_target(w,w->known) < w->declared)
+        w->part_first[w->known++] = w->last_start;          /* the bucket holding the cut's ordinal */
+    }
+  if (rc != HM_OK)
+    { pthread_mutex_unlock(&w->mu);
+      return rc;
+    }
+  return writer_release(w);
+}
+
+static int writer_seal(hm_table_writer *w)
+{ pthread_mutex_lock(&w->mu);
+  w->sealed = 1;
+  while (w->known < w->nparts)
+    w->part_first[w->known++] = w->hint > 0 && w->declared > 0 ? w->last_start : w->declared;
+  return writer_release(w);
+}
+
+void hm_table_write_seal(hm_table_writer *w)
+{ if (w != NULL)
+    writer_seal(w);
+}
+
+int hm_table_write_at(hm_table_writer *w, int64_t first, const uint8_t *rec, int64_t n)
+{ if (w == NULL || first < 0 || n < 0 || (n > 0 && rec == NULL))
+    return hm_set_error(HM_EINVAL,"hm_table_write_at: bad arguments");
+  const int64_t end = first+n;
+  int64_t cut[64], *pf = cut;
+  pthread_mutex_lock(&w->mu);
+  if (w->failed || !w->positional || end > w->declared)
+    { if (w->positional && !w->failed && end > w->declared) w->failed = 1;
+      pthread_mutex_unlock(&w->mu);
+      return hm_set_error(HM_EINVAL,"hm_table_write_at: no usable writer or records %lld..%lld not placed",
+                          (long long) first,(long long) end);
+    }
+  /* records from the last bucket's start on may still fall on either side of an open cut: held (copied) until
+   * a later place or the seal fixes it; the rest go to their files now                                      */
+  const int64_t open = writer_open_from(w);
+  const int64_t mid = end < open ? end : (first > open ? first : open);
+  int rc = HM_OK;
+  if (mid < end)
+    { pending *q = malloc(sizeof(pending) + (size_t) (end-mid)*w->pbyte);
+      if (q == NULL)
+        rc = hm_set_error(HM_ENOMEM,"Out of memory (table writer)");
+      else
+        { q->first = mid; q->n = end-mid;
+          memcpy(q->rec,rec+(mid-first)*w->pbyte,(size_t) (end-mid)*w->pbyte);
+          if (w->held == NULL) w->held_from = open;
+          q->next = w->held; w->held = q;
+        }
+    }
+  const int known = w->known;
+  if (rc == HM_OK && !writer_cuts(w,cut,&pf))
+    rc = hm_set_error(HM_ENOMEM,"Out of memory (table writer)");
+  if (rc != HM_OK)
+    { w->failed = 1;
+      pthread_mutex_unlock(&w->mu);
+      return rc;
+    }
+  pthread_mutex_unlock(&w->mu);
+  rc = writer_put(w,pf,known,first,rec,mid-first);
+  if (pf != cut) free(pf);
+  pthread_mutex_lock(&w->mu);
+  if (rc == HM_OK) w->written += n;
+  else             w->failed = 1;
+  pthread_mutex_unlock(&w->mu);
+  return rc;
+}
+
 int hm_table_write_close(hm_table_writer *w)
 { int rc = HM_OK;
   if (w == NULL)
     return hm_set_error(HM_EINVAL,"hm_table_write_close: no writer");
+  /* positional: the cuts not reached are fixed (as below) and the records still held written */
+  if (w->positional && writer_seal(w) != HM_OK)
+    { writer_free(w,1);
+      return HM_EIO;
+    }
   if (w->failed || w->written != w->declared)
     { rc = w->failed ? hm_set_error(HM_EINVAL,"hm_table_write_close: an earlier call failed")
                      : hm_set_error(HM_EINVAL,"hm_table_write_close: %lld announced records were not appended",
@@ -392,7 +569,7 @@ int hm_table_write_close(hm_table_writer *w)
       return rc;
     }
   /* cuts not reached (fewer entries than the hint): at the last bucket's start, as write_ktab cuts */
-  while (rc == HM_OK && w->part+1 < w->nparts)
+  while (rc == HM_OK && !w->positional && w->part+1 < w->nparts)
     rc = writer_cut(w,w->hint > 0 && w->written > 0 ? w->cur_start : w->written);
   for (int p = 0; p < w->nparts && rc == HM_OK; p++)
     { int64_t end = p+1 < w->nparts ? w->part_first[p+1] : w->written;
