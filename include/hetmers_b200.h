@@ -432,6 +432,14 @@ int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks)
 typedef struct hm_rank_scan hm_rank_scan;
 int  hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
                          hm_rank_scan **out);
+/* create from the rank's share alone: `share` holds the entries [cuts[rank], cuts[rank+1]) of a table of n_total
+ * entries (its ordinals start at 0, its stub index counts only them), and the caller gives every rank's cuts
+ * (int64[world+1], 0 .. n_total, each on a run boundary) and first_keys (uint64[world]: word 0 of entry cuts[r],
+ * ~0 when cuts[r] = n_total).  The scan is sized by the whole table, as create sizes it; hm_rank_scan_cuts
+ * returns these cuts.                                                                                        */
+int  hm_rank_scan_create_share(const hm_host_table *share, int64_t n_total, const int64_t *cuts,
+                               const uint64_t *first_keys, int device, int rank, int world, const uint64_t seed[2],
+                               hm_rank_scan **out);
 void hm_rank_scan_destroy(hm_rank_scan *r);
 /* cuts: int64[world+1]; first_keys (optional): uint64[world], word 0 of the first entry of each share */
 int  hm_rank_scan_cuts(const hm_rank_scan *r, int64_t *cuts, uint64_t *first_keys);

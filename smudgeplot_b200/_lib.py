@@ -26,7 +26,7 @@ ABI_SYMBOLS = [
     "hm_k_symm_extract",
     "hm_symm_status", "hm_symm_align_cut",
     "hm_scan_download", "hm_set_device_budget", "hm_stream_plan", "hm_stream_plan_shards", "hm_scan_residency", "hm_table_open", "hm_table_close", "hm_table_view", "hm_write_smu",
-    "hm_rank_scan_create", "hm_rank_scan_destroy", "hm_rank_scan_cuts", "hm_rank_scan_pass1", "hm_rank_scan_bloom",
+    "hm_rank_scan_create", "hm_rank_scan_create_share", "hm_rank_scan_destroy", "hm_rank_scan_cuts", "hm_rank_scan_pass1", "hm_rank_scan_bloom",
     "hm_rank_scan_prepare", "hm_rank_scan_slices", "hm_rank_scan_route", "hm_rank_scan_answer", "hm_rank_scan_settle",
     "hm_rank_scan_result", "hm_rank_scan_residency",
     "hm_rank_scan_extract_prepare", "hm_rank_scan_extract_slices", "hm_rank_scan_extract_route",
@@ -214,6 +214,7 @@ def lib():
     L.hm_scan_residency.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     u64p, i64p = C.POINTER(C.c_uint64), C.POINTER(i64)
     L.hm_rank_scan_create.argtypes = [C.POINTER(HostTable), i32, i32, i32, u64p, C.POINTER(vp)]
+    L.hm_rank_scan_create_share.argtypes = [C.POINTER(HostTable), i64, i64p, u64p, i32, i32, i32, u64p, C.POINTER(vp)]
     L.hm_rank_scan_destroy.argtypes = [vp]
     L.hm_rank_scan_destroy.restype = None
     L.hm_rank_scan_cuts.argtypes = [vp, i64p, u64p]

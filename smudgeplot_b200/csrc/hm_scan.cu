@@ -3382,10 +3382,12 @@ extern "C" void hm_rank_scan_destroy(hm_rank_scan *r)
   free(r);
 }
 
-extern "C" int hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
-                                   hm_rank_scan **out)
+/* a rank scan of a table of n entries streaming the host table t (the whole table, or the rank's share of it:
+ * [0, t->nels) either way) through `device`; its cuts are set by the caller                                   */
+static int rank_scan_open(const hm_host_table *t, int64_t n, int device, int rank, int world, const uint64_t seed[2],
+                          hm_rank_scan **out)
 { if (t == NULL || out == NULL || seed == NULL || world < 1 || world > HM_MAX_GPUS || rank < 0 || rank >= world ||
-      device < 0)
+      device < 0 || n < t->nels)
     return hm_set_error(HM_EINVAL,"hm_rank_scan_create: bad arguments");
   if (t->kmer < HM_SYMM_MIN_KMER || t->kmer > HM_MAX_KMER)
     return hm_set_error(HM_EUNSUPPORTED,"the table does not fit in device memory and k = %d has no strand-symmetric "
@@ -3400,7 +3402,7 @@ extern "C" int hm_rank_scan_create(const hm_host_table *t, int device, int rank,
   if (r == NULL || s == NULL)
     { free(r); free(s); return hm_set_error(HM_ENOMEM,"out of host memory"); }
   r->s = s;
-  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = t->nels; s->ngpu = 1; s->nshard = world; s->rank = rank;
+  s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = n; s->ngpu = 1; s->nshard = world; s->rank = rank;
   s->bits = hm_pick_bucket_bits(s->n); s->fpos = hm_pick_filter_bits(s->n); s->idx64 = (s->n >= 0xFFFFFFF0ll);
   s->seed[0] = seed[0]; s->seed[1] = seed[1];               /* the same on every rank: the sums are added */
   s->budget = device_budget(&device,1);
@@ -3411,13 +3413,50 @@ extern "C" int hm_rank_scan_create(const hm_host_table *t, int device, int rank,
   if (rc == HM_OK) rc = open_device(D,device,1);
   TRY(dev_alloc(D,&D->plot,sizeof(unsigned long long)*HM_PLOT_CELLS));
   TRY(dev_alloc(D,&D->fp_acc,4*sizeof(uint64_t)));
-  D->lo = 0; D->hi = s->n;
-  if (rc == HM_OK && world > 1)
-    rc = stream_cuts(s);
+  D->lo = 0; D->hi = t->nels;
   if (rc != HM_OK)
     { r->s = NULL; free(r);
       hm_scan_destroy(s);
       return rc;
+    }
+  *out = r;
+  return HM_OK;
+}
+
+extern "C" int hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
+                                   hm_rank_scan **out)
+{ hm_rank_scan *r = NULL;
+  int rc = rank_scan_open(t,t != NULL ? t->nels : 0,device,rank,world,seed,&r);
+  if (rc == HM_OK && world > 1 && (rc = stream_cuts(r->s)) != HM_OK)
+    hm_rank_scan_destroy(r);
+  else if (rc == HM_OK)
+    *out = r;
+  return rc;
+}
+
+extern "C" int hm_rank_scan_create_share(const hm_host_table *share, int64_t n_total, const int64_t *cuts,
+                                         const uint64_t *first_keys, int device, int rank, int world,
+                                         const uint64_t seed[2], hm_rank_scan **out)
+{ int ok = share != NULL && cuts != NULL && first_keys != NULL && world >= 1 && world <= HM_MAX_GPUS && rank >= 0 &&
+           rank < world && cuts[0] == 0 && cuts[world] == n_total;
+  for (int q = 0; ok && q < world; q++)
+    ok = cuts[q] <= cuts[q+1];
+  if (!ok || cuts[rank+1]-cuts[rank] != share->nels)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_create_share: bad arguments (the share must hold entries "
+                        "[cuts[rank], cuts[rank+1]) of cuts rising from 0 to n_total)");
+  hm_rank_scan *r = NULL;
+  int rc = rank_scan_open(share,n_total,device,rank,world,seed,&r);
+  if (rc != HM_OK)
+    return rc;
+  if (world > 1)                              /* stream_cuts' descriptor, from the given cuts */
+    { hm_symm_shards *sh = r->s->ssh;
+      int live = 1;
+      for (int q = 1; q < world; q++)
+        if (cuts[q] < n_total) live = q+1;
+      memset(sh,0,sizeof(*sh));
+      sh->n_seg = live; sh->self = rank;
+      for (int q = 0; q <= world; q++) sh->off[q] = cuts[q];
+      for (int q = 0; q < world; q++)  sh->first_key[q] = first_keys[q];
     }
   *out = r;
   return HM_OK;

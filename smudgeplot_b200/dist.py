@@ -1154,8 +1154,21 @@ def bucket_condition_cuts(hist, world: int, hb: int, ibyte: int):
     (the reference bisects a table on disk by its buckets).  hist: output entries per hb-bit key prefix; a bucket
     holds the first 8*ibyte bits.  Where buckets are coarser than prefixes (8*ibyte < hb) the cut is made over the
     histogram summed per bucket and scaled back to prefixes.  -> [0, c_1, ..., c_{world-1}, 2^hb]"""
+    return _coarse_condition_cuts(hist, world, hb, 8 * ibyte)
+
+
+def run_condition_cuts(hist, world: int, hb: int, ibyte: int, kmer: int):
+    """bucket_condition_cuts coarsened to run boundaries, so that every rank's part of the table starts on a run (the
+    entries sharing their first kmer//2 bases) as pass 1 of the streamed scan needs: cuts on prefixes of min(hb,
+    8*ibyte, 2*(kmer//2)) bits, made over the histogram summed per such prefix.  Where runs are no finer than
+    buckets (2*(kmer//2) >= 8*ibyte) these are bucket_condition_cuts.  -> [0, c_1, ..., c_{world-1}, 2^hb]"""
+    return _coarse_condition_cuts(hist, world, hb, min(8 * ibyte, 2 * (kmer >> 1)))
+
+
+def _coarse_condition_cuts(hist, world: int, hb: int, bits: int):
+    """condition_cuts on the boundaries of `bits`-bit key prefixes, hist counting per hb-bit prefix"""
     import numpy as np
-    sh = hb - 8 * ibyte
+    sh = hb - bits
     if sh <= 0:
         return condition_cuts(hist, world)
     h = np.asarray(hist, dtype=np.int64).reshape(-1, 1 << sh).sum(axis=1)
@@ -1241,6 +1254,144 @@ def _write_atomic(path: str, data: bytes):
         raise
 
 
+class _RankConditioning:
+    """One rank's part of trimming and symmetrising the FastK table kt across the ranks (condition_ktab,
+    StreamedShardedScan.from_ktab).  The constructor loads the rank's share of the source onto dev and takes
+    hetmers' decisions on the whole table (job_examine); needed() tells whether a step is.  plan() cuts the key
+    prefixes into the ranks' ranges (cut_rule(hist, world, hb)) and every range into the passes its
+    budget allows beside the resident share; run(take) conditions them, handing each pass's packed records to
+    take.  close() frees the share.  st: the stats both callers report; ms: ms per phase."""
+
+    def __init__(self, kt, ethresh, group, dev, coll, budget, ms):
+        from . import _lib
+        from .device import _ptr, _stream
+        self.group, self.dev, self.coll, self.budget, self.ms = group, dev, coll, budget, ms
+        self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
+        self.lap = _lapper(ms)
+        self.k, self.n, self.ibyte, self.ethresh = kt.kmer, kt.nels, kt.ibyte, ethresh
+        t = time.perf_counter()
+        lo, hi = share_range(self.n, self.world, self.rank)
+        self.m = hi - lo
+        self.share = list(_load_share(kt, lo, hi, dev))
+        t = self.done("load", t)
+        Lb, share = _lib.lib(), self.share
+
+        def share_min(a, b):
+            out = torch.full((1,), 0x8000, dtype=torch.int32, device=dev)
+            _lib.check(Lb.hm_k_min_count(_ptr(share[1]), a, b, _ptr(out), _stream()))
+            return int(out.item())
+
+        self.trimmed, self.symmetric = job_examine(ethresh, self.k, self.n, share[0], share[2], share_min, group,
+                                                   coll)
+        self.do_trim, self.do_symm = not self.trimmed, not self.symmetric
+        self.lap("examine", t)
+        self.st = {"trimmed": self.trimmed, "symmetric": self.symmetric,
+                   "steps": (["trim"] if self.do_trim else []) + (["symmetrise"] if self.do_symm else []),
+                   "entries_in": self.n}
+
+    def done(self, phase, t):                              # the phase's kernels have finished
+        torch.cuda.synchronize(self.dev)
+        return self.lap(phase, t)
+
+    def needed(self) -> bool:
+        return self.do_trim or self.do_symm
+
+    def close(self):
+        self.share.clear()
+
+    def plan(self, cut_rule, what: str):
+        """histograms, the rank cuts, every rank's sub-ranges and every pass's counts.  HM_ENOMEM on every rank
+        (the share freed) when a rank's share and one pass do not fit its budget; what: the job, for the message"""
+        import numpy as np
+        from . import _lib
+        from .device import _ptr, _stream
+        Lb, k, world, rank, share = _lib.lib(), self.k, self.world, self.rank, self.share
+        t = time.perf_counter()
+        self.ethr = self.ethresh if self.do_trim else 0
+        self.hb = hb = min(_lib.COND_HIST_BITS, 2 * k)
+        hist = torch.zeros((2, 1 << hb), dtype=torch.int64, device=self.dev)
+        for row, symm in ((0, 0), (1, self.do_symm)):
+            _lib.check(Lb.hm_k_cond_hist(_ptr(share[0]), _ptr(share[2]), _ptr(share[1]), self.m, k, self.ethr, symm,
+                                         _ptr(hist[row]), _stream()))
+        h_loc = hist.cpu().numpy()
+        _in_place(lambda x: dist.all_reduce(x, group=self.group), hist, self.group)
+        self.h_all = h_all = hist.cpu().numpy()
+        del hist
+        self.cuts = cuts = cut_rule(h_all[1], world, hb)
+        budgets = _reduce([self.budget if d == rank else 0 for d in range(world)], self.coll, self.group)
+        shares = [b - a for a, b in (share_range(self.n, world, d) for d in range(world))]
+        try:
+            self.subs = subs = rank_sub_cuts(k, self.ibyte, shares, self.do_symm, budgets, h_all[1], cuts)
+        except _lib.HetmersError:
+            self.close()
+            raise
+        self.passes = rank_pass_counts(h_loc, h_all, subs, rank)
+        need = max(Lb.hm_rank_condition_bytes(k, self.ibyte, world, self.m, *c[:3], int(self.do_symm))
+                   for c in self.passes)
+        needs = _reduce([need if d == rank else 0 for d in range(world)], self.coll, self.group)
+        short = [d for d in range(world) if needs[d] > budgets[d]]
+        if short:
+            self.close()
+            raise _lib.HetmersError(-3, f"rank {rank}: conditioning {what} across {world} ranks needs {needs} "
+                                        f"device bytes per rank, beyond the budgets {budgets} of ranks {short}; use "
+                                        f"more ranks, or condition_kmer_table")
+        self.span = prefix_buckets(cuts[rank], cuts[rank + 1], hb, self.ibyte) if cuts[rank] < cuts[rank + 1] \
+            else (0, 0)
+        self.bcounts = np.zeros(self.span[1] - self.span[0], dtype=np.int64)
+        self.st.update(passes=len(self.passes), prefix_cuts=cuts, sub_ranges=subs[rank], sent=[], received=[],
+                       budget=self.budget, working_set_bytes=need)
+        self.done("hist_and_plan", t)
+
+    def rank_entries(self, d: int) -> int:
+        """the conditioned entries rank d receives, from the summed histogram"""
+        a, b = self.cuts[d], self.cuts[d + 1]
+        return int(self.h_all[1][a:b].sum())
+
+    def run(self, take):
+        """the passes: this rank's sub-range p conditioned and packed (its records' stub-bucket counts added to
+        self.bcounts over self.span), then take(records, keys) with the pass's device records (uint8, in key
+        order) and keys (their first words, int64); take must not keep either.  The share is freed at the end."""
+        import numpy as np
+        from . import _lib
+        from .device import _ptr, _stream
+        Lb, k, ibyte, hb, world, rank = _lib.lib(), self.k, self.ibyte, self.hb, self.world, self.rank
+        pbyte = ((k + 3) >> 2) - ibyte + 2
+        subs, span = self.subs, self.span
+        self.ms["passes"] = []
+        for p, expect in enumerate(self.passes):
+            pm = {}
+            self.ms["passes"].append(pm)
+            plap = _lapper(pm)
+
+            def pdone(phase, t0):
+                torch.cuda.synchronize(self.dev)
+                return plap("settle" if phase == "sort_and_merge" else phase, t0)
+            dest = np.full(1 << hb, -1, dtype=np.int16)
+            for d in range(world):
+                if p < len(subs[d]) - 1:
+                    dest[subs[d][p]:subs[d][p + 1]] = d
+            (ok, oc, ol), sent_to, got_from = _route_exchange_settle(
+                k, self.m, self.share, self.ethr, self.do_symm, torch.from_numpy(dest).to(self.dev), True, expect,
+                self.group, self.coll, pdone, time.perf_counter())
+            self.st["sent"].append(sum(sent_to))
+            self.st["received"].append(sum(got_from))
+            t = time.perf_counter()
+            e = ok.numel()
+            if e:
+                b0, b1 = prefix_buckets(subs[rank][p], subs[rank][p + 1], hb, ibyte)
+                rec = torch.empty(e * pbyte, dtype=torch.uint8, device=self.dev)
+                bc = torch.empty(b1 - b0, dtype=torch.int64, device=self.dev)
+                _lib.check(Lb.hm_k_cond_pack(k, ibyte, _ptr(ok), _ptr(ol), _ptr(oc), e, b0, b1 - b0, _ptr(rec),
+                                             _ptr(bc), _stream()))
+                self.bcounts[b0 - span[0]:b1 - span[0]] += bc.cpu().numpy()
+                del bc
+                take(rec, ok)
+                del rec
+            del ok, oc, ol
+            pdone("pack", t)
+        self.close()
+
+
 def condition_ktab(src, dst, L, group=None, device=None, budget=None):
     """Trim and / or symmetrise the FastK table `src` into the new FastK table `dst` across the ranks of the group,
     every rank calling this (DESIGN.md §4f).  hetmers' decisions are taken on the whole table as from_ktab(L=...)
@@ -1265,93 +1416,45 @@ def condition_ktab(src, dst, L, group=None, device=None, budget=None):
     import tempfile
     import numpy as np
     from . import _lib, fastk
-    from .device import _ptr, _stream
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     dev = torch.device(device if device is not None else "cuda")
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     coll = dev if _nccl(group) else torch.device("cpu")
-    Lb = _lib.lib()
     ethresh = int(L)
     src, dst = str(src), str(dst)
     ms = {}
     lap = _lapper(ms)
-
-    def done(phase, t):                                    # the phase's kernels have finished
-        torch.cuda.synchronize(dev)
-        return lap(phase, t)
 
     with torch.cuda.device(dev):
         if budget is None:
             budget = torch.cuda.mem_get_info(dev)[0] - _lib.BUDGET_RESERVE
         torch.cuda.reset_peak_memory_stats(dev)
         base = torch.cuda.memory_allocated(dev)
-        t = time.perf_counter()
         kt = fastk.read_ktab(src, mmap=True)
-        k, n, ibyte, src_parts = kt.kmer, kt.nels, kt.ibyte, kt.nparts
+        k, ibyte, src_parts = kt.kmer, kt.ibyte, kt.nparts
         if max(_reduce([int(fastk.same_table_files(src, src_parts, dst))], coll, group, dist.ReduceOp.MAX)):
             raise _lib.HetmersError(-1, f"rank {rank}: {dst} names the source table: conditioning writes a new table")
         minval_src = kt.minval
-        lo, hi = share_range(n, world, rank)
-        m = hi - lo
-        share = list(_load_share(kt, lo, hi, dev))
+        job = _RankConditioning(kt, ethresh, group, dev, coll, budget, ms)
         del kt
-        t = done("load", t)
-
-        def share_min(a, b):
-            out = torch.full((1,), 0x8000, dtype=torch.int32, device=dev)
-            _lib.check(Lb.hm_k_min_count(_ptr(share[1]), a, b, _ptr(out), _stream()))
-            return int(out.item())
-
-        trimmed, symmetric = job_examine(ethresh, k, n, share[0], share[2], share_min, group, coll)
-        do_trim, do_symm = not trimmed, not symmetric
-        t = lap("examine", t)
-        if not (do_trim or do_symm):
-            share.clear()
+        if not job.needed():
+            job.close()
             return None
-        ethr = ethresh if do_trim else 0
-        hb = min(_lib.COND_HIST_BITS, 2 * k)
-
-        # histograms, the rank cuts on buckets, every rank's sub-ranges, and every pass's counts
-        hist = torch.zeros((2, 1 << hb), dtype=torch.int64, device=dev)
-        for row, symm in ((0, 0), (1, do_symm)):
-            _lib.check(Lb.hm_k_cond_hist(_ptr(share[0]), _ptr(share[2]), _ptr(share[1]), m, k, ethr, symm,
-                                         _ptr(hist[row]), _stream()))
-        h_loc = hist.cpu().numpy()
-        _in_place(lambda x: dist.all_reduce(x, group=group), hist, group)
-        h_all = hist.cpu().numpy()
-        del hist
-        cuts = bucket_condition_cuts(h_all[1], world, hb, ibyte)
-        budgets = _reduce([budget if d == rank else 0 for d in range(world)], coll, group)
-        shares = [b - a for a, b in (share_range(n, world, d) for d in range(world))]
-        try:
-            subs = rank_sub_cuts(k, ibyte, shares, do_symm, budgets, h_all[1], cuts)
-        except _lib.HetmersError:
-            share.clear()
-            raise
-        plan = rank_pass_counts(h_loc, h_all, subs, rank)
-        need = max(Lb.hm_rank_condition_bytes(k, ibyte, world, m, *c[:3], int(do_symm)) for c in plan)
-        needs = _reduce([need if d == rank else 0 for d in range(world)], coll, group)
-        short = [d for d in range(world) if needs[d] > budgets[d]]
-        if short:
-            share.clear()
-            raise _lib.HetmersError(-3, f"rank {rank}: conditioning {src} into files across {world} ranks needs "
-                                        f"{needs} device bytes per rank, beyond the budgets {budgets} of ranks {short}; "
-                                        f"use more ranks, or condition_kmer_table")
-        t = done("hist_and_plan", t)
+        do_trim = job.do_trim
+        job.plan(lambda h, w, hb: bucket_condition_cuts(h, w, hb, ibyte), f"{src} into files")
 
         # the passes: this rank's sub-range p conditioned, packed and appended to its temporary part
         ddir, root = fastk.split_name(dst)
         pbyte = ((k + 3) >> 2) - ibyte + 2
-        span = prefix_buckets(cuts[rank], cuts[rank + 1], hb, ibyte) if cuts[rank] < cuts[rank + 1] else (0, 0)
-        bcounts = np.zeros(span[1] - span[0], dtype=np.int64)
+        span, bcounts = job.span, job.bcounts
         fd, tmp, err = -1, "", None
         try:
             fd, tmp = tempfile.mkstemp(prefix=f".{root}.ktab.", suffix=f".rank{rank}.tmp", dir=ddir)
         except OSError as x:
             err = f"{ddir}: {x}"
         if max(_reduce([int(err is not None)], coll, group, dist.ReduceOp.MAX)):
-            share.clear()
+            job.close()
             if fd >= 0:
                 os.close(fd)
                 os.unlink(tmp)
@@ -1367,52 +1470,23 @@ def condition_ktab(src, dst, L, group=None, device=None, budget=None):
 
         writer = cf.ThreadPoolExecutor(1)
         pending, n_out, part, nparts, total = None, 0, None, 0, 0
-        st = {"trimmed": trimmed, "symmetric": symmetric,
-              "steps": (["trim"] if do_trim else []) + (["symmetrise"] if do_symm else []),
-              "entries_in": n, "passes": len(plan), "prefix_cuts": cuts, "sub_ranges": subs[rank],
-              "sent": [], "received": [], "budget": budget, "working_set_bytes": need}
-        ms["passes"] = []
+        st = job.st
+
+        def take(rec, keys):
+            nonlocal pending, err, n_out
+            host = rec.cpu().numpy()
+            if pending is not None and err is None:        # the last pass's records have been written
+                try:
+                    pending.result()
+                except OSError as x:
+                    err = f"{tmp}: {x}"
+            if err is None:
+                pending = writer.submit(append, host)
+            n_out += keys.numel()
+
         try:
             os.write(fd, struct.pack("<iq", k, 0))         # the count is set once every pass is written
-            for p, expect in enumerate(plan):
-                pm = {}
-                ms["passes"].append(pm)
-                plap = _lapper(pm)
-
-                def pdone(phase, t0):
-                    torch.cuda.synchronize(dev)
-                    return plap("settle" if phase == "sort_and_merge" else phase, t0)
-                dest = np.full(1 << hb, -1, dtype=np.int16)
-                for d in range(world):
-                    if p < len(subs[d]) - 1:
-                        dest[subs[d][p]:subs[d][p + 1]] = d
-                (ok, oc, ol), sent_to, got_from = _route_exchange_settle(
-                    k, m, share, ethr, do_symm, torch.from_numpy(dest).to(dev), True, expect, group, coll, pdone,
-                    time.perf_counter())
-                st["sent"].append(sum(sent_to))
-                st["received"].append(sum(got_from))
-                t = time.perf_counter()
-                e = ok.numel()
-                if e:
-                    b0, b1 = prefix_buckets(subs[rank][p], subs[rank][p + 1], hb, ibyte)
-                    rec = torch.empty(e * pbyte, dtype=torch.uint8, device=dev)
-                    bc = torch.empty(b1 - b0, dtype=torch.int64, device=dev)
-                    _lib.check(Lb.hm_k_cond_pack(k, ibyte, _ptr(ok), _ptr(ol), _ptr(oc), e, b0, b1 - b0, _ptr(rec),
-                                                 _ptr(bc), _stream()))
-                    bcounts[b0 - span[0]:b1 - span[0]] += bc.cpu().numpy()
-                    host = rec.cpu().numpy()
-                    del rec, bc
-                    if pending is not None and err is None:    # the last pass's records have been written
-                        try:
-                            pending.result()
-                        except OSError as x:
-                            err = f"{tmp}: {x}"
-                    if err is None:
-                        pending = writer.submit(append, host)
-                    n_out += e
-                del ok, oc, ol
-                pdone("pack", t)
-            share.clear()
+            job.run(take)
             t = time.perf_counter()
             if pending is not None and err is None:
                 try:
@@ -1483,7 +1557,7 @@ def condition_ktab(src, dst, L, group=None, device=None, budget=None):
                         os.unlink(fastk.part_path(dst, q))
             lap("commit", t)
         finally:
-            share.clear()
+            job.close()
             writer.shutdown(wait=True)
             if fd >= 0:
                 os.close(fd)
@@ -1903,14 +1977,15 @@ def write_pair_files(recs, kmer: int, labels, out, group, dev, budget=None, lap=
 
 class StreamedShardedScan:
     """The streamed counterpart of ShardedScan: rank r of the group streams its run-aligned share of the FastK
-    table at the path `table` (or the `_lib.HostTable` `table`, whose buffers must outlive the scan) through
-    `device` under the device budget (`budget` bytes, else free memory minus a reserve);
-    no rank holds the table.  Pass 2 settles a Bloom hit on a key another rank owns by asking that rank: the keys
-    go to their owners with all_to_all_single, one byte per key comes back (hm_rank_scan_*, DESIGN.md §4c).
+    table at the path `table` (or the `_lib.HostTable` `table`, whose buffers must outlive the scan, or the
+    in-memory fastk.KtabFiles `table`) through `device` under the device budget (`budget` bytes, else free memory
+    minus a reserve); no rank holds the table.  from_ktab(L=...) conditions a raw table on the way in.  Pass 2
+    settles a Bloom hit on a key another rank owns by asking that rank: the keys go to their owners with
+    all_to_all_single, one byte per key comes back (hm_rank_scan_*, DESIGN.md §4c).
     scan() -> the plot (int64[SMAX+1, FMAX+1] on every rank), equal to the in-core scan's; extract(pixmap, dst) ->
     extract_kmer_pairs' records on rank dst, equal to the in-core list."""
 
-    def __init__(self, table, group=None, device=None, budget: int | None = None):
+    def __init__(self, table, group=None, device=None, budget: int | None = None, _share=None):
         import ctypes as C
         from . import _lib, fastk
         from .hetmers import _host_table
@@ -1922,6 +1997,8 @@ class StreamedShardedScan:
         self.L = L = _lib.lib()
         if isinstance(table, _lib.HostTable):
             self._ht, self._keep = table, None
+        elif isinstance(table, fastk.KtabFiles):
+            self._ht, self._keep = _host_table(table)
         else:
             self._ht, self._keep = _host_table(fastk.read_ktab(table, mmap=True))   # read again by every scan
         self.kmer = self._ht.kmer
@@ -1931,7 +2008,15 @@ class StreamedShardedScan:
             L.hm_set_device_budget(int(budget))
         h = C.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(L.hm_rank_scan_create(C.byref(self._ht), self.device.index, self.rank, self.world, sd, C.byref(h)))
+            if _share is None:
+                _lib.check(L.hm_rank_scan_create(C.byref(self._ht), self.device.index, self.rank, self.world, sd,
+                                                 C.byref(h)))
+            else:                                               # table: this rank's share of _share's cuts
+                n_total, cuts, first = _share
+                _lib.check(L.hm_rank_scan_create_share(C.byref(self._ht), n_total,
+                                                       (C.c_int64 * (self.world + 1))(*cuts),
+                                                       (C.c_uint64 * self.world)(*first), self.device.index,
+                                                       self.rank, self.world, sd, C.byref(h)))
         self._h = h
         cuts = (C.c_int64 * (self.world + 1))()
         _lib.check(L.hm_rank_scan_cuts(h, cuts, None))
@@ -1943,9 +2028,129 @@ class StreamedShardedScan:
             self.close()
             raise RuntimeError(f"rank {self.rank}: the ranks computed different shard cuts from the table files "
                                f"({[e.tolist() for e in every]})")
+        self.share = None                                       # (from_ktab) this rank's conditioned share
         self.status = 0
+        self._base_stats = {}                                   # what every stats dict starts with (from_ktab)
         self.stats = {}
         self._pass1_done = False                                # candidates, S list and Bloom filter resident
+
+    @classmethod
+    def from_ktab(cls, src, group=None, device=None, L=None, budget=None, host_budget=None):
+        """The streamed scan of the FastK table `src` as hetmers -e<L> scans it; every rank calls this.  With L the
+        table is trimmed and / or symmetrised on the way in, as hm_scan_examine(L) decides on the whole table
+        (job_examine), without writing a conditioned copy: each rank conditions one range of key prefixes, cut on
+        run boundaries (run_condition_cuts), in the passes of condition_ktab that its device budget allows beside
+        its share of the source; it keeps the packed records of its range in host memory as a one-part table
+        (self.share: its stub index counts only them) and streams that share on every scan.  A table that needs
+        neither step, and L None, give StreamedShardedScan(src): the source files are streamed, no host copy held.
+        budget: device bytes per rank, for the conditioning and the scan (default: free memory minus
+        _lib.BUDGET_RESERVE); host_budget: host bytes per rank (default: no cap).  HM_ENOMEM on every rank, with the
+        sizes and before the first pass, when a rank's share of the source and one pass do not fit its budget, when
+        a rank's conditioned share (records and stub index) exceeds its host_budget, or when a rank cannot allocate
+        it.  stats["condition"]: condition_ktab's stats (verdicts, steps, entries in / out, passes, prefix cuts and
+        sub-ranges, entries sent / received per pass, peak device bytes, ms per phase), the entry cuts of the
+        shares, and host_bytes, what this rank holds once its share is settled (the host budget is checked
+        against the histograms' count, which may exceed it by the keys that equal their reverse complement or
+        were held on both strands)."""
+        import numpy as np
+        from . import _lib, fastk
+        if L is None:
+            out = cls(src, group, device, budget)
+            out._base_stats = {"condition": {"steps": [], "host_bytes": 0}}
+            out.stats = dict(out._base_stats)
+            return out
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        dev = torch.device(device if device is not None else "cuda")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        coll = dev if _nccl(group) else torch.device("cpu")
+        src, ms = str(src), {}
+        lap = _lapper(ms)
+        with torch.cuda.device(dev):
+            cond_budget = budget if budget is not None else torch.cuda.mem_get_info(dev)[0] - _lib.BUDGET_RESERVE
+            torch.cuda.reset_peak_memory_stats(dev)
+            base = torch.cuda.memory_allocated(dev)
+            kt = fastk.read_ktab(src, mmap=True)
+            k, n, ibyte, minval = kt.kmer, kt.nels, kt.ibyte, kt.minval
+            job = _RankConditioning(kt, int(L), group, dev, coll, cond_budget, ms)
+            del kt
+            st = job.st
+            if not job.needed():
+                job.close()
+                torch.cuda.empty_cache()                        # the scan allocates outside torch's cache
+                st.update(entries_out=n, host_bytes=0, peak_bytes=torch.cuda.max_memory_allocated(dev) - base, ms=ms)
+                out = cls(src, group, device, budget)
+                out._base_stats = {"condition": st}
+                out.stats = dict(out._base_stats)
+                return out
+            job.plan(lambda h, w, hb: run_condition_cuts(h, w, hb, ibyte, k), f"{src} into host shares")
+
+            # the host share, sized by the histograms before the first pass (a bound: settling merges a reverse
+            # complement with an equal original, a palindrome with itself)
+            t = time.perf_counter()
+            pbyte = ((k + 3) >> 2) - ibyte + 2
+            ixlen = 1 << (8 * ibyte)
+            needs = [job.rank_entries(d) * pbyte + 8 * ixlen for d in range(world)]
+            caps = _reduce([(-1 if host_budget is None else int(host_budget)) if d == rank else 0
+                            for d in range(world)], coll, group)
+            over = [d for d in range(world) if 0 <= caps[d] < needs[d]]
+            buf = index = None
+            if not over:
+                try:
+                    buf = np.empty(needs[rank] - 8 * ixlen, dtype=np.uint8)
+                    index = np.zeros(ixlen, dtype=np.int64)
+                except MemoryError:
+                    buf = index = None
+            failed = [d for d, f in enumerate(_reduce([int(d == rank and not over and buf is None)
+                                                       for d in range(world)], coll, group)) if f]
+            if over or failed:
+                job.close()
+                if over:
+                    raise _lib.HetmersError(-3, f"rank {rank}: conditioning {src} into host shares across {world} "
+                                                f"ranks holds {needs} host bytes per rank, beyond the host budgets "
+                                                f"{caps} of ranks {over} (-1: no cap)")
+                raise _lib.HetmersError(-3, f"rank {rank}: conditioning {src} into host shares across {world} "
+                                            f"ranks: ranks {failed} cannot allocate their "
+                                            f"{[needs[d] for d in failed]} host bytes")
+            t = lap("host_alloc", t)
+            at, first = 0, None
+
+            def take(rec, keys):
+                nonlocal at, first
+                if first is None:
+                    first = int(keys[0]) & _U64
+                torch.from_numpy(buf[at:at + rec.numel()]).copy_(rec)
+                at += rec.numel()
+
+            try:
+                job.run(take)
+            finally:
+                job.close()
+            torch.cuda.empty_cache()
+            t = time.perf_counter()
+            m_out = at // pbyte
+            buf.resize(at, refcheck=False)         # the histograms count a merged pair of equal keys twice
+            s0, s1 = job.span
+            index[s0:s1] = job.bcounts
+            np.cumsum(index, out=index)
+
+            # every rank's entry cut and first key: an empty rank's first key is the next non-empty rank's, so that
+            # it owns no key (~0 past the last)
+            got = _reduce(sum(([m_out, _signed(first) if first is not None else 0] if d == rank else [0, 0]
+                               for d in range(world)), []), coll, group)
+            outs, firsts = got[0::2], [x & _U64 for x in got[1::2]]
+            cuts = [0] + np.cumsum(outs).tolist()
+            first_keys = [next((firsts[q] for q in range(r, world) if outs[q] > 0), _U64) for r in range(world)]
+            lap("host_share", t)
+            st.update(entries_out=cuts[-1], rank_entries_out=m_out, cuts=cuts, host_bytes=buf.nbytes + index.nbytes,
+                      peak_bytes=torch.cuda.max_memory_allocated(dev) - base, ms=ms)
+            share = fastk.KtabFiles(kmer=k, nparts=1, minval=max(minval, int(L)) if job.do_trim else minval,
+                                    ibyte=ibyte, index=index, part_nels=[m_out], records=[buf])
+        out = cls(share, group, device, budget, _share=(cuts[-1], cuts, first_keys))
+        out.share = share
+        out._base_stats = {"condition": st}
+        out.stats = dict(out._base_stats)
+        return out
 
     def _view(self, ptr: int, nbytes: int) -> torch.Tensor:
         return _cuda_view(ptr, max(nbytes, 1), self.device)[:nbytes]
@@ -2052,7 +2257,7 @@ class StreamedShardedScan:
             out = plot.clone().view(_lib.SMAX + 1, _lib.PLOT_W)
             lap("plot_allreduce", t)
         self.status = int(st.value)
-        self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms, "candidates": nc,
+        self.stats = {**self._base_stats, "rounds": n_rounds, "slice": slice_, "max_slice": ms, "candidates": nc,
                       "queries_sent_to": sent_to}
         return out
 
@@ -2119,8 +2324,9 @@ class StreamedShardedScan:
             _libc_free(out)
             lap("rank_sort" if sort else "rank_records", t)
         self.status = int(st.value)
-        self.stats = {"rounds": n_rounds, "slice": slice_, "max_slice": ms.value, "candidates": nc.value,
-                      "queries_sent_to": sent_to, "pass1_reused": reuse, "records": int(n.value)}
+        self.stats = {**self._base_stats, "rounds": n_rounds, "slice": slice_, "max_slice": ms.value,
+                      "candidates": nc.value, "queries_sent_to": sent_to, "pass1_reused": reuse,
+                      "records": int(n.value)}
         if not self.symm_ok():
             raise RuntimeError(f"rank {self.rank}: the routed pair listing ended with a non-zero status word on some "
                                f"rank (here {self.status:#x}); its records must not be used")
@@ -2146,3 +2352,4 @@ class StreamedShardedScan:
             with torch.cuda.device(self.device):
                 self.L.hm_rank_scan_destroy(self._h)
         self._h = None
+        self._keep = self.share = None                         # the host buffers the scan streamed
