@@ -279,6 +279,10 @@ typedef struct hm_scan hm_scan;   /* opaque: device-resident table + work buffer
  * work is sharded by contiguous index range, DESIGN.md §6).  Replaces Open_Kmer_Stream +
  * Clone_Kmer_Stream + the 4 GiB cache fill (libfastk.c:786-951; PloidyPlot.c:954-964).       */
 int  hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out);
+/* hm_scan_create, streamed whatever the table's size (what HETMERS_STREAM=1 does, for this call): nothing of the
+ * table is resident, so a call that reads the host table itself (hm_scan_condition_host) has the device budget
+ * to itself.  Scan.from_ktab conditions through such a scan when in-place conditioning does not fit.          */
+int  hm_scan_create_streamed(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out);
 /* Optional: start CUDA (driver + primary contexts of the first n_gpus visible devices, 0 = all) and
  * the pinned staging buffers on a background thread and return at once; hm_scan_create waits for
  * it.  Lets a short-lived process overlap CUDA start-up with opening its table files.             */
@@ -574,6 +578,17 @@ int hm_condition_plan(int64_t n, int kmer, int ibyte, int64_t budget, int do_sym
                       int hist_bits, int64_t *cuts, hm_condition_layout *out);
 int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
                             hm_condition_stats *st);
+/* hm_scan_condition_files into host memory instead of files: the same plan, the same range passes on the same
+ * GPUs (hm_set_condition_gpus), and the table writer's memory target (hm_table_write_open_host), so *out holds
+ * the records and stub index the files would hold, as one part (free it with hm_host_table_free; hm_scan_create
+ * scans it in or out of core).  The buffer is sized by the output histogram, a bound on the records, and checked
+ * against host_budget (-1: no cap) before the first range pass: HM_ENOMEM with both sizes when it does not fit,
+ * or when it cannot be allocated.  The refusals of hm_scan_condition_files that concern no file stand (a scan
+ * conditioned in place: HM_EINVAL; a device budget below one range's working set: HM_ENOMEM); on any failure
+ * *out is NULL and nothing stays allocated.  st->bytes_written counts the host bytes (records and index).  The
+ * scan is left as it was.                                                                                    */
+int hm_scan_condition_host(hm_scan *s, int ethresh, int do_trim, int do_symm, int64_t host_budget,
+                           hm_host_table **out, hm_condition_stats *st);
 
 /* ---- conditioning across the ranks of a one-process-per-GPU job (csrc/hm_shard_condition.cu, DESIGN.md §4e) ----
  * Each rank holds a sorted share of the source (m entries; d_keys_lo only for k > 32) and the caller runs the
@@ -696,6 +711,17 @@ void hm_table_write_abort(hm_table_writer *w);
 int  hm_table_write_place(hm_table_writer *w, int64_t b0, int64_t nb, const int64_t *counts, int64_t *first);
 int  hm_table_write_at(hm_table_writer *w, int64_t first, const uint8_t *rec, int64_t n);
 void hm_table_write_seal(hm_table_writer *w);
+/* The same writer with host memory as its target: a one-part table of at most nels_cap records (HM_ENOMEM when
+ * that buffer cannot be allocated; announcing more is an error, HM_EINVAL).  write_buckets / append, place / at /
+ * seal and abort behave as they do for files; records are copied into one buffer at their final offsets and the
+ * stub index is counted in memory.  hm_table_write_close_host closes it (hm_table_write_close refuses a memory
+ * writer, and close_host a file writer; both free the writer either way): *out is a one-part table with the
+ * given kmer, ibyte and minval whose records are the part files' payloads concatenated and whose index is the
+ * stub's, byte for byte, for the same calls.  Free it with hm_host_table_free; on abort or failure nothing stays
+ * allocated.                                                                                                  */
+int  hm_table_write_open_host(int kmer, int ibyte, int minval, int64_t nels_cap, hm_table_writer **out);
+int  hm_table_write_close_host(hm_table_writer *w, hm_host_table **out);
+void hm_host_table_free(hm_host_table *t);     /* a table hm_table_write_close_host or hm_scan_condition_host made */
 
 /* .smu writer: "min\t(sum-min)\tcount\n", sum-major, min < FMAX (PloidyPlot.c:1603-1617) */
 int  hm_write_smu(const char *path, const int64_t *plot);

@@ -34,7 +34,8 @@ ABI_SYMBOLS = [
     "hm_condition_range_bytes", "hm_condition_plan", "hm_scan_condition_files",
     "hm_table_write_open", "hm_table_write_buckets", "hm_table_write_append", "hm_table_write_close",
     "hm_table_write_abort", "hm_table_write_place", "hm_table_write_at", "hm_table_write_seal",
-    "hm_set_condition_gpus",
+    "hm_set_condition_gpus", "hm_scan_condition_host", "hm_table_write_open_host", "hm_table_write_close_host",
+    "hm_host_table_free", "hm_scan_create_streamed",
     "hm_k_cond_hist", "hm_k_shard_route_count", "hm_k_shard_route_scatter", "hm_k_shard_settle_bytes",
     "hm_k_shard_settle", "hm_shard_condition_bytes",
     "hm_k_shard_route_count_window", "hm_k_shard_route_scatter_window", "hm_k_cond_pack", "hm_rank_condition_bytes",
@@ -89,7 +90,7 @@ COND_MAX_GPUS = 16
 
 
 class ConditionStats(C.Structure):
-    """hm_condition_stats: what hm_scan_condition_files did"""
+    """hm_condition_stats: what hm_scan_condition_files / hm_scan_condition_host did"""
     _fields_ = [("nels_in", C.c_int64), ("nels_out", C.c_int64), ("ranges", C.c_int32), ("passes", C.c_int32),
                 ("peak_bytes", C.c_int64), ("bytes_read", C.c_int64), ("bytes_written", C.c_int64),
                 ("ms_hist", C.c_double), ("ms_ranges", C.c_double), ("ms_write", C.c_double), ("ms_total", C.c_double),
@@ -197,6 +198,7 @@ def lib():
     L.hm_symm_status.argtypes = [vp, C.POINTER(SymmLayout), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), vp]
     L.hm_symm_align_cut.argtypes = [vp, i64, i32, i64, C.POINTER(i64)]
     L.hm_scan_create.argtypes = [C.POINTER(HostTable), C.POINTER(i32), i32, C.POINTER(vp)]
+    L.hm_scan_create_streamed.argtypes = L.hm_scan_create.argtypes
     L.hm_scan_destroy.argtypes = [vp]
     L.hm_scan_destroy.restype = None
     L.hm_scan_examine.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32)]
@@ -254,6 +256,12 @@ def lib():
     L.hm_table_write_seal.argtypes = [vp]
     L.hm_table_write_seal.restype = None
     L.hm_set_condition_gpus.argtypes = [i32]
+    L.hm_scan_condition_host.argtypes = [vp, i32, i32, i32, i64, C.POINTER(C.POINTER(HostTable)),
+                                         C.POINTER(ConditionStats)]
+    L.hm_table_write_open_host.argtypes = [i32, i32, i32, i64, C.POINTER(vp)]
+    L.hm_table_write_close_host.argtypes = [vp, C.POINTER(C.POINTER(HostTable))]
+    L.hm_host_table_free.argtypes = [C.POINTER(HostTable)]
+    L.hm_host_table_free.restype = None
     L.hm_k_cond_hist.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp]
     L.hm_k_shard_route_count.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, i32, vp, vp, vp]
     L.hm_k_shard_route_scatter.argtypes = [vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, vp, i64, i64, vp, vp, vp]

@@ -810,7 +810,8 @@ static int open_device(DevTable *D, int dev, int pool)
   return rc;
 }
 
-extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out)
+/* stream: 1 streams the scan whatever its size */
+static int scan_create(const hm_host_table *t, const int *dev, int n_gpus, int stream, hm_scan **out)
 { double t0 = now_ms();
   if (t == NULL || out == NULL || n_gpus < 1 || n_gpus > HM_MAX_GPUS)
     return hm_set_error(HM_EINVAL,"hm_scan_create: bad arguments");
@@ -838,8 +839,7 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
 
   s->budget = device_budget(dev,n_gpus);
   s->incore_bytes = incore_bytes(n,t->kmer,n_gpus,s->bits,s->idx64);
-  const char *force = getenv("HETMERS_STREAM");            /* =1: stream whatever the budget (tests, capping) */
-  if (s->incore_bytes > s->budget || (force != NULL && strcmp(force,"1") == 0))
+  if (s->incore_bytes > s->budget || stream)
     { /* streamed: only the plot and the fingerprint sums are allocated now; the table stays on the host.
        * Several GPUs: shard r streams its run-aligned share [c_r, c_r+1) through dev[r] (DESIGN.md §4c) */
       if ((rc = stream_setup(s,t)) != HM_OK)
@@ -928,6 +928,15 @@ extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus
   s->ms_alloc = t_alloc-t0; s->ms_records = t_rec-t_alloc; s->ms_index = now_ms()-t_rec;
   *out = s;
   return HM_OK;
+}
+
+extern "C" int hm_scan_create(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out)
+{ const char *force = getenv("HETMERS_STREAM");            /* =1: stream whatever the budget (tests, capping) */
+  return scan_create(t,dev,n_gpus,force != NULL && strcmp(force,"1") == 0,out);
+}
+
+extern "C" int hm_scan_create_streamed(const hm_host_table *t, const int *dev, int n_gpus, hm_scan **out)
+{ return scan_create(t,dev,n_gpus,1,out);
 }
 
 /* work buffers of the direct passes (hm_kernels.cu): incidence array, recorded partners, prefix filter */
@@ -1593,18 +1602,23 @@ static int cond_on_gpus(CondRun *R, CondFn fn)
   return rc;
 }
 
-extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
-                                       hm_condition_stats *st)
+/* hm_scan_condition_files (dst) and hm_scan_condition_host (out, dst NULL): one plan and one set of range passes,
+ * the writer's target the only difference                                                                      */
+static int condition_into(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst, int64_t host_budget,
+                          hm_host_table **out, hm_condition_stats *st)
 { double t0 = now_ms();
-  if (s == NULL || dst == NULL)
-    return hm_set_error(HM_EINVAL,"hm_scan_condition_files: NULL argument");
+  const char *who = dst != NULL ? "hm_scan_condition_files" : "hm_scan_condition_host";
+  if (s == NULL || (dst == NULL && out == NULL))
+    return hm_set_error(HM_EINVAL,"%s: NULL argument",who);
+  if (out != NULL)
+    *out = NULL;
   if (s->conditioned || s->invalid)
     return hm_set_error(HM_EINVAL,"this scan's table was conditioned in place: the files it was created from no longer "
                         "describe it");
   if (!do_trim && !do_symm)
-    return hm_set_error(HM_EINVAL,"hm_scan_condition_files: neither trimming nor symmetrising was asked for");
+    return hm_set_error(HM_EINVAL,"%s: neither trimming nor symmetrising was asked for",who);
   const hm_host_table *t = s->src;
-  if (names_source(t,dst))
+  if (dst != NULL && names_source(t,dst))
     return hm_set_error(HM_EINVAL,"%s names the source table: conditioning writes a new table",dst);
 
   const int G = g_cond_gpus < s->ngpu ? g_cond_gpus : s->ngpu;
@@ -1660,12 +1674,21 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
   int64_t hint = 0;
   for (int64_t p = 0; p < np; p++) hint += hist[p];
 
+  /* into host memory: the histogram bounds the records (settling merges an original with an equal reverse
+   * complement, a palindrome with itself), and the buffer is checked and allocated before the first range pass */
+  const int64_t host_need = hint*pbyte + 8*ixlen;
+  if (rc == HM_OK && dst == NULL && host_budget >= 0 && host_need > host_budget)
+    rc = hm_set_error(HM_ENOMEM,"conditioning into host memory needs %lld host bytes (%lld records of %d bytes and a "
+                      "stub index of %lld), beyond the host budget of %lld",(long long) host_need,(long long) hint,
+                      pbyte,(long long) (8*ixlen),(long long) host_budget);
+  const int minval = do_trim && ethresh > t->minval ? ethresh : t->minval;
+  if (rc == HM_OK && dst == NULL)
+    rc = hm_table_write_open_host(kmer,ibyte,minval,hint,&R.w);
   const int64_t T = lay.range_cap > 0 ? lay.range_cap : 1;
   for (int g = 0; g < G && rc == HM_OK; g++)
     rc = cond_gpu_range_bufs(gpu+g,T,pbyte);
-  if (rc == HM_OK)
-    rc = hm_table_write_open(dst,kmer,ibyte,do_trim && ethresh > t->minval ? ethresh : t->minval,
-                             t->nparts > 0 ? t->nparts : 1,hint,&R.w);
+  if (rc == HM_OK && dst != NULL)
+    rc = hm_table_write_open(dst,kmer,ibyte,minval,t->nparts > 0 ? t->nparts : 1,hint,&R.w);
   for (int g = 0; g < G; g++)
     gpu[g].J.w = R.w;
 
@@ -1676,7 +1699,8 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
     rc = cond_on_gpus(&R,cond_gpu_ranges);
   S.ms_ranges = now_ms()-t_ranges;
   if (R.w != NULL)
-    { int rw = rc == HM_OK ? hm_table_write_close(R.w) : (hm_table_write_abort(R.w), HM_OK);
+    { int rw = rc != HM_OK ? (hm_table_write_abort(R.w), HM_OK)
+             : dst != NULL ? hm_table_write_close(R.w) : hm_table_write_close_host(R.w,out);
       if (rc == HM_OK) rc = rw;
     }
 
@@ -1698,10 +1722,25 @@ extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int
   free(hist); free(cuts); free(gpu);
   S.passes = S.ranges+1;
   S.bytes_read = resident ? 0 : (int64_t) S.passes*n*pbyte;
-  S.bytes_written = 16 + 8*ixlen + 12ll*(t->nparts > 0 ? t->nparts : 1) + S.nels_out*pbyte;
+  S.bytes_written = dst != NULL ? 16 + 8*ixlen + 12ll*(t->nparts > 0 ? t->nparts : 1) + S.nels_out*pbyte
+                                 : rc == HM_OK ? 8*ixlen + S.nels_out*pbyte : 0;   /* host bytes held */
   S.ms_total = now_ms()-t0;
   if (st != NULL) *st = S;
   return rc;
+}
+
+extern "C" int hm_scan_condition_files(hm_scan *s, int ethresh, int do_trim, int do_symm, const char *dst,
+                                       hm_condition_stats *st)
+{ if (dst == NULL)
+    return hm_set_error(HM_EINVAL,"hm_scan_condition_files: NULL argument");
+  return condition_into(s,ethresh,do_trim,do_symm,dst,-1,NULL,st);
+}
+
+extern "C" int hm_scan_condition_host(hm_scan *s, int ethresh, int do_trim, int do_symm, int64_t host_budget,
+                                      hm_host_table **out, hm_condition_stats *st)
+{ if (out == NULL)
+    return hm_set_error(HM_EINVAL,"hm_scan_condition_host: NULL argument");
+  return condition_into(s,ethresh,do_trim,do_symm,NULL,host_budget,out,st);
 }
 
 /* reverse complement of a left-aligned packed k-mer (k <= 32) */

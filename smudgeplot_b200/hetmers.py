@@ -161,24 +161,126 @@ def _host_table(kt: KtabFiles):
     return ht, (index, recs, part_nels, part_rec)
 
 
+class _OwnedTable:
+    """The one-part host table hm_scan_condition_host made.  Every array viewing it holds this object, and it is
+    freed (hm_host_table_free) when the last of them and the Scan that owns it have let it go."""
+
+    def __init__(self, ptr):
+        self.ptr = ptr
+        self._free = _lib.lib().hm_host_table_free
+
+    def _array(self, addr, shape, typestr):
+        holder = type("_View", (), {})()
+        holder.owner = self
+        holder.__array_interface__ = {"shape": shape, "typestr": typestr, "data": (addr, False), "version": 3}
+        return np.asarray(holder)
+
+    def ktab(self) -> KtabFiles:
+        v = self.ptr.contents
+        n, pbyte = int(v.nels), ((v.kmer + 3) >> 2) - v.ibyte + 2
+        index = self._array(C.cast(v.index, C.c_void_p).value, (1 << (8 * v.ibyte),), "<i8")
+        rec = self._array(v.part_rec[0], (n * pbyte,), "|u1") if n else np.empty(0, dtype=np.uint8)
+        return KtabFiles(kmer=v.kmer, nparts=1, minval=v.minval, ibyte=v.ibyte, index=index, part_nels=[n],
+                         records=[rec])
+
+    def __del__(self):
+        if self.ptr:
+            self._free(self.ptr)
+            self.ptr = None
+
+
 class Scan:
     """Device-resident table + both passes (hm_scan_*).  A table whose in-core scan does not fit the device
     budget is streamed through the GPU on every run() instead (residency()); device_budget (bytes per GPU)
-    sets that budget for this and later scans of the process (0: free device memory minus a reserve)."""
+    sets that budget for this and later scans of the process (0: free device memory minus a reserve).
+    from_ktab(src, L) scans a raw FastK table as hetmers -e<L> does, conditioning it on the way in."""
 
-    def __init__(self, kt: KtabFiles, gpus: int = 1, devices=None, device_budget: int | None = None):
+    def __init__(self, kt: KtabFiles, gpus: int = 1, devices=None, device_budget: int | None = None, _owned=None,
+                 _stream=False):
         L = _lib.lib()
         self._L = L
-        self.kt = kt
+        self._h = None
+        self._owned = _owned                      # (from_ktab) the conditioned host table (_OwnedTable)
+        self.kt = _owned.ktab() if _owned else kt
+        self.stats = {}
         if device_budget is not None:
             L.hm_set_device_budget(int(device_budget))
-        ht, self._keep = _host_table(kt)          # a streamed scan reads these buffers on every run
+        if _owned:
+            ht, self._keep = _owned.ptr.contents, None
+        else:
+            ht, self._keep = _host_table(kt)      # a streamed scan reads these buffers on every run
         self._ht = ht
-        devs = list(devices) if devices is not None else list(range(gpus))
-        arr = (C.c_int * len(devs))(*devs)
+        self.devices = list(devices) if devices is not None else list(range(gpus))
+        arr = (C.c_int * len(self.devices))(*self.devices)
         h = C.c_void_p()
-        _lib.check(L.hm_scan_create(C.byref(ht), arr, len(devs), C.byref(h)))
+        create = L.hm_scan_create_streamed if _stream else L.hm_scan_create
+        rc = create(C.byref(ht), arr, len(self.devices), C.byref(h))
+        if rc != 0:
+            self.close()
+            _lib.check(rc)
         self._h = h
+
+    @classmethod
+    def from_ktab(cls, src, L=None, gpus: int = 1, devices=None, device_budget: int | None = None,
+                  host_budget: int | None = None):
+        """The scan of the FastK table `src` as hetmers -e<L> scans it, in one process on `gpus` GPUs (or the
+        device ids `devices`), for a table of any size, without writing a conditioned copy.  L None, or a table
+        hm_scan_examine(L) finds trimmed and symmetric, gives Scan over the source files.  Otherwise the table is
+        trimmed and / or symmetrised on the way in, by the one route the sizes allow: in place on the devices
+        (hm_scan_condition) when the source is in core and that fits the device budget, else into host memory
+        (hm_scan_condition_host on the same devices; an in-core source is first reopened streamed, so that the
+        conditioning has the device budget to itself; the source scan is destroyed afterwards) and a scan created
+        over that table, in core if it fits, streamed if not.  The scan owns the host table: close() destroys the
+        scan, then frees the table unless arrays of self.kt (its records and index) are still held elsewhere, in
+        which case they keep it alive.  device_budget: device bytes per GPU, as Scan's; host_budget: host bytes the
+        conditioned table may take (None: no cap), checked against the output histogram's bound before the first
+        range pass (HetmersError -3 with both sizes).  stats["condition"] differs by route: always route ("none",
+        "in_place" or "host"), steps ("trim", "symmetrise") and host_bytes (the host table's records and index, 0
+        but on the host route); "in_place" adds nels_in, nels_out and ms_total; "host" adds every
+        hm_condition_stats field (ranges, passes, peak_bytes, budget_bytes, ...)."""
+        import time
+        lib = _lib.lib()
+        sc = cls(read_ktab(str(src), mmap=True), gpus, devices, device_budget)
+        st = {"route": "none", "steps": [], "host_bytes": 0}
+        sc.stats = {"condition": st}
+        try:
+            if L is None:
+                return sc
+            trim, symm = sc.examine(int(L))
+            st["steps"] = [name for name, done in (("trim", trim), ("symmetrise", symm)) if not done]
+            if not st["steps"]:
+                return sc
+            if not sc.residency()[0]:
+                t0 = time.perf_counter()
+                try:                                    # refused (HM_ENOMEM) before the table is touched
+                    n = sc.condition(int(L), not trim, not symm)
+                    st.update(route="in_place", nels_in=sc.kt.nels, nels_out=n,
+                              ms_total=(time.perf_counter() - t0) * 1e3)
+                    return sc
+                except _lib.HetmersError as e:
+                    if e.code != -3:
+                        raise
+                src_kt, devs = sc.kt, sc.devices        # the resident source goes: conditioning reads the host table
+                sc.close()
+                sc = cls(src_kt, devices=devs, _stream=True)
+            ht = C.POINTER(_lib.HostTable)()
+            cs = _lib.ConditionStats()
+            was = lib.hm_set_condition_gpus(len(sc.devices))
+            try:
+                _lib.check(lib.hm_scan_condition_host(sc._h, int(L), int(not trim), int(not symm),
+                                                      -1 if host_budget is None else int(host_budget), C.byref(ht),
+                                                      C.byref(cs)))
+            finally:
+                lib.hm_set_condition_gpus(was)
+            sc.close()
+            out = cls(None, devices=sc.devices, _owned=_OwnedTable(ht))
+        except BaseException:
+            sc.close()
+            raise
+        st.update(route="host", **cs.as_dict())
+        st["host_bytes"] = cs.bytes_written
+        out.stats = {"condition": st}
+        return out
 
     def examine(self, ethresh: int):
         """(trimmed?, symmetric?) as examine_table decides them (PloidyPlot.c:1167-1230)."""
@@ -301,9 +403,12 @@ class Scan:
         return keys, cnt, d
 
     def close(self):
-        if self._h:
+        if getattr(self, "_h", None):
             self._L.hm_scan_destroy(self._h)
             self._h = None
+        if getattr(self, "_owned", None):               # after the scan that reads it
+            self._owned = self._ht = None
+            self.kt = None
 
     def __enter__(self):
         return self

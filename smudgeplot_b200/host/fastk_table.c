@@ -206,6 +206,16 @@ fail:
  * cuts); until then it lies at or after the start of the last bucket announced, so only records of that bucket
  * can be in doubt.  hm_table_write_at never waits: it copies those records and the place or seal that settles
  * them writes them (at most one bucket's records are held).  Nothing written is ever moved.                 */
+static int pwrite_all(int fd, const void *buf, size_t len, off_t off)
+{ const char *b = (const char *) buf;
+  while (len > 0)
+    { ssize_t r = pwrite(fd,b,len,off);
+      if (r <= 0) return -1;
+      b += r; len -= (size_t) r; off += r;
+    }
+  return 0;
+}
+
 typedef struct pending { int64_t first, n; struct pending *next; uint8_t rec[]; } pending;
 
 struct hm_table_writer
@@ -223,7 +233,23 @@ struct hm_table_writer
     struct pending *held;              /* (positional) records written while their part was open  */
     int64_t  held_from;                /*   the open ordinal they wait on (the last bucket's start)*/
     pthread_mutex_t mu;                /* (positional) guards the above, declared and written      */
+    uint8_t *mem;                      /* memory target (one part): room for mem_cap records, else */
+    int64_t  mem_cap;                  /*   NULL and the records go to the part files             */
   };
+
+/* n bytes at byte offset off of part p's payload: into the part file, or the memory target's buffer */
+static int writer_sink(const hm_table_writer *w, int p, const void *buf, size_t n, off_t off)
+{ if (w->mem != NULL)
+    { memcpy(w->mem+off,buf,n);
+      return 0;
+    }
+  return pwrite_all(w->fd[p],buf,n,PART_HEADER+off);
+}
+
+/* records to announce beyond the memory target's room (the records every later call assumes placed) */
+static int writer_over(const hm_table_writer *w, int64_t more)
+{ return w->mem != NULL && w->declared+more > w->mem_cap;
+}
 
 static char *writer_path(const hm_table_writer *w, int part, int tmp)   /* part 0 = the stub */
 { size_t len = strlen(w->dir)+strlen(w->root)+strlen(w->tmp_tag)+48;
@@ -233,16 +259,6 @@ static char *writer_path(const hm_table_writer *w, int part, int tmp)   /* part 
   if (part == 0) snprintf(p,len,"%s/%s.ktab%s",w->dir,w->root,tmp ? w->tmp_tag : "");
   else           snprintf(p,len,"%s/.%s.ktab.%d%s",w->dir,w->root,part,tmp ? w->tmp_tag : "");
   return p;
-}
-
-static int pwrite_all(int fd, const void *buf, size_t len, off_t off)
-{ const char *b = (const char *) buf;
-  while (len > 0)
-    { ssize_t r = pwrite(fd,b,len,off);
-      if (r <= 0) return -1;
-      b += r; len -= (size_t) r; off += r;
-    }
-  return 0;
 }
 
 static void writer_free(hm_table_writer *w, int unlink_tmp)
@@ -259,7 +275,7 @@ static void writer_free(hm_table_writer *w, int unlink_tmp)
     { char *q = writer_path(w,0,1);
       if (q != NULL) { unlink(q); free(q); }
     }
-  free(w->count); free(w->part_first); free(w->fd); free(w->dir); free(w->root); free(w->tmp_tag);
+  free(w->count); free(w->part_first); free(w->fd); free(w->dir); free(w->root); free(w->tmp_tag); free(w->mem);
   while (w->held != NULL)
     { pending *nx = w->held->next;
       free(w->held);
@@ -271,14 +287,10 @@ static void writer_free(hm_table_writer *w, int unlink_tmp)
 
 void hm_table_write_abort(hm_table_writer *w) { writer_free(w,1); }
 
-int hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int nparts, int64_t nels_hint,
-                        hm_table_writer **out)
-{ hm_table_writer *w;
-  if (name == NULL || out == NULL || kmer < 1 || ibyte < 1 || ibyte > 3 || ibyte > ((kmer+3)>>2) ||
-      nparts < 1 || nels_hint < 0)
-    return hm_set_error(HM_EINVAL,"hm_table_write_open: bad arguments");
+/* the writer's state shared by both targets (*out = NULL on failure) */
+static int writer_new(int kmer, int ibyte, int minval, int nparts, int64_t nels_hint, hm_table_writer **out)
+{ hm_table_writer *w = calloc(1,sizeof(*w));
   *out = NULL;
-  w = calloc(1,sizeof(*w));
   if (w == NULL)
     return hm_set_error(HM_ENOMEM,"Out of memory (table writer)");
   w->kmer = kmer; w->ibyte = ibyte; w->minval = minval; w->nparts = nparts; w->hint = nels_hint;
@@ -289,14 +301,47 @@ int hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int n
   pthread_mutex_init(&w->mu,NULL);
   w->count      = calloc((size_t) w->ixlen,sizeof(int64_t));
   w->part_first = calloc((size_t) nparts,sizeof(int64_t));
+  if (w->count == NULL || w->part_first == NULL)
+    { writer_free(w,0); return hm_set_error(HM_ENOMEM,"Out of memory (table writer)"); }
+  *out = w;
+  return HM_OK;
+}
+
+int hm_table_write_open_host(int kmer, int ibyte, int minval, int64_t nels_cap, hm_table_writer **out)
+{ hm_table_writer *w;
+  if (out == NULL || kmer < 1 || ibyte < 1 || ibyte > 3 || ibyte > ((kmer+3)>>2) || nels_cap < 0)
+    return hm_set_error(HM_EINVAL,"hm_table_write_open_host: bad arguments");
+  int rc = writer_new(kmer,ibyte,minval,1,0,&w);
+  if (rc != HM_OK)
+    return rc;
+  w->mem_cap = nels_cap;
+  w->mem     = malloc(nels_cap > 0 ? (size_t) (nels_cap*w->pbyte) : 1);
+  if (w->mem == NULL)
+    { rc = hm_set_error(HM_ENOMEM,"Out of memory (a table of %lld records: %lld host bytes)",(long long) nels_cap,
+                        (long long) (nels_cap*w->pbyte));
+      writer_free(w,0);
+      return rc;
+    }
+  *out = w;
+  return HM_OK;
+}
+
+int hm_table_write_open(const char *name, int kmer, int ibyte, int minval, int nparts, int64_t nels_hint,
+                        hm_table_writer **out)
+{ hm_table_writer *w;
+  if (name == NULL || out == NULL || kmer < 1 || ibyte < 1 || ibyte > 3 || ibyte > ((kmer+3)>>2) ||
+      nparts < 1 || nels_hint < 0)
+    return hm_set_error(HM_EINVAL,"hm_table_write_open: bad arguments");
+  int rc = writer_new(kmer,ibyte,minval,nparts,nels_hint,&w);
+  if (rc != HM_OK)
+    return rc;
   w->fd         = malloc(sizeof(int)*(size_t) nparts);
   w->dir        = malloc(strlen(name)+8);
   w->root       = malloc(strlen(name)+8);
   w->tmp_tag    = malloc(64);
-  if (w->count == NULL || w->part_first == NULL || w->fd == NULL || w->dir == NULL || w->root == NULL ||
-      w->tmp_tag == NULL)
+  for (int p = 0; p < nparts && w->fd != NULL; p++) w->fd[p] = -1;
+  if (w->fd == NULL || w->dir == NULL || w->root == NULL || w->tmp_tag == NULL)
     { writer_free(w,0); return hm_set_error(HM_ENOMEM,"Out of memory (table writer)"); }
-  for (int p = 0; p < nparts; p++) w->fd[p] = -1;
   split_name(name,w->dir,w->root);
   snprintf(w->tmp_tag,64,".tmp%ld",(long) getpid());
   for (int p = 0; p < nparts; p++)
@@ -329,6 +374,11 @@ int hm_table_write_buckets(hm_table_writer *w, int64_t b0, int64_t nb, const int
       if (b < 0 || b >= w->ixlen || counts[i] < 0 || b < w->last)
         { w->failed = 1;
           return hm_set_error(HM_EINVAL,"hm_table_write_buckets: bucket %lld announced out of order",(long long) b);
+        }
+      if (writer_over(w,counts[i]))
+        { w->failed = 1;
+          return hm_set_error(HM_EINVAL,"hm_table_write_buckets: more than the %lld records the table has room for",
+                              (long long) w->mem_cap);
         }
       w->count[b] += counts[i];
       w->declared += counts[i];
@@ -368,8 +418,7 @@ static int64_t writer_target(const hm_table_writer *w, int q)
 /* records [from, w->written) of the current part, held at rec, go to its file in one write */
 static int writer_flush(hm_table_writer *w, const uint8_t *rec, int64_t from)
 { if (w->written > from &&
-      pwrite_all(w->fd[w->part],rec,(size_t) (w->written-from)*w->pbyte,
-                 PART_HEADER + (off_t) (from-w->part_first[w->part])*w->pbyte) != 0)
+      writer_sink(w,w->part,rec,(size_t) (w->written-from)*w->pbyte,(off_t) (from-w->part_first[w->part])*w->pbyte) != 0)
     return hm_set_error(HM_EIO,"writing table part %d: %s",w->part+1,strerror(errno));
   return HM_OK;
 }
@@ -415,8 +464,7 @@ static int writer_put(const hm_table_writer *w, const int64_t *pf, int known, in
   for (int64_t o = first; o < end; )
     { while (p+1 < known && pf[p+1] <= o) p++;
       int64_t e = p+1 < known && pf[p+1] < end ? pf[p+1] : end;
-      if (pwrite_all(w->fd[p],rec+(o-first)*w->pbyte,(size_t) (e-o)*w->pbyte,
-                     PART_HEADER + (off_t) (o-pf[p])*w->pbyte) != 0)
+      if (writer_sink(w,p,rec+(o-first)*w->pbyte,(size_t) (e-o)*w->pbyte,(off_t) (o-pf[p])*w->pbyte) != 0)
         return hm_set_error(HM_EIO,"writing table part %d: %s",p+1,strerror(errno));
       o = e;
     }
@@ -476,6 +524,12 @@ int hm_table_write_place(hm_table_writer *w, int64_t b0, int64_t nb, const int64
       if (b < 0 || b >= w->ixlen || counts[i] < 0 || b < w->last)
         { w->failed = 1;
           rc = hm_set_error(HM_EINVAL,"hm_table_write_place: bucket %lld announced out of order",(long long) b);
+          break;
+        }
+      if (writer_over(w,counts[i]))
+        { w->failed = 1;
+          rc = hm_set_error(HM_EINVAL,"hm_table_write_place: more than the %lld records the table has room for",
+                            (long long) w->mem_cap);
           break;
         }
       if (w->declared == 0 || b != w->last)                 /* a new bucket starts here */
@@ -552,22 +606,84 @@ int hm_table_write_at(hm_table_writer *w, int64_t first, const uint8_t *rec, int
   return rc;
 }
 
-int hm_table_write_close(hm_table_writer *w)
-{ int rc = HM_OK;
-  if (w == NULL)
-    return hm_set_error(HM_EINVAL,"hm_table_write_close: no writer");
-  /* positional: the cuts not reached are fixed (as below) and the records still held written */
+/* what closing takes on either target: positional, the cuts not reached are fixed (as hm_table_write_close fixes
+ * them) and the records still held written; then every announced record must have been written.  w is freed on
+ * failure.                                                                                                    */
+static int writer_finish(hm_table_writer *w, const char *who)
+{ int rc;
   if (w->positional && writer_seal(w) != HM_OK)
     { writer_free(w,1);
       return HM_EIO;
     }
   if (w->failed || w->written != w->declared)
-    { rc = w->failed ? hm_set_error(HM_EINVAL,"hm_table_write_close: an earlier call failed")
-                     : hm_set_error(HM_EINVAL,"hm_table_write_close: %lld announced records were not appended",
+    { rc = w->failed ? hm_set_error(HM_EINVAL,"%s: an earlier call failed",who)
+                     : hm_set_error(HM_EINVAL,"%s: %lld announced records were not appended",who,
                                     (long long) (w->declared-w->written));
       writer_free(w,1);
       return rc;
     }
+  return HM_OK;
+}
+
+/* the memory target's table: its records and index leave the writer with it */
+typedef struct
+  { hm_host_table  view;
+    int64_t        part_nels[1];
+    const uint8_t *part_rec[1];
+  } host_table;
+
+int hm_table_write_close_host(hm_table_writer *w, hm_host_table **out)
+{ int rc;
+  if (w == NULL || out == NULL || w->mem == NULL)
+    { writer_free(w,1);
+      return hm_set_error(HM_EINVAL,"hm_table_write_close_host: no memory writer");
+    }
+  *out = NULL;
+  if ((rc = writer_finish(w,"hm_table_write_close_host")) != HM_OK)
+    return rc;
+  host_table *h = calloc(1,sizeof(*h));
+  if (h == NULL)
+    { writer_free(w,1);
+      return hm_set_error(HM_ENOMEM,"Out of memory (table record)");
+    }
+  int64_t acc = 0;
+  for (int64_t b = 0; b < w->ixlen; b++)                    /* counts -> bucket END offsets, as the stub holds */
+    { acc += w->count[b]; w->count[b] = acc; }
+  if (w->written > 0 && w->written < w->mem_cap)            /* the room was a bound: give back what was not used */
+    { uint8_t *m = realloc(w->mem,(size_t) (w->written*w->pbyte));
+      if (m != NULL) w->mem = m;
+    }
+  h->part_nels[0] = w->written;
+  h->part_rec[0]  = w->mem;
+  h->view.kmer = w->kmer; h->view.ibyte = w->ibyte; h->view.nparts = 1; h->view.minval = w->minval;
+  h->view.nels = w->written;
+  h->view.index = w->count;
+  h->view.part_nels = h->part_nels;
+  h->view.part_rec  = h->part_rec;
+  w->count = NULL; w->mem = NULL;
+  writer_free(w,1);
+  *out = &h->view;
+  return HM_OK;
+}
+
+void hm_host_table_free(hm_host_table *t)
+{ if (t == NULL)
+    return;
+  free((void *) t->index);
+  free((void *) t->part_rec[0]);
+  free(t);
+}
+
+int hm_table_write_close(hm_table_writer *w)
+{ int rc = HM_OK;
+  if (w == NULL)
+    return hm_set_error(HM_EINVAL,"hm_table_write_close: no writer");
+  if (w->mem != NULL)
+    { writer_free(w,1);
+      return hm_set_error(HM_EINVAL,"hm_table_write_close: a memory writer closes with hm_table_write_close_host");
+    }
+  if ((rc = writer_finish(w,"hm_table_write_close")) != HM_OK)
+    return rc;
   /* cuts not reached (fewer entries than the hint): at the last bucket's start, as write_ktab cuts */
   while (rc == HM_OK && !w->positional && w->part+1 < w->nparts)
     rc = writer_cut(w,w->hint > 0 && w->written > 0 ? w->cur_start : w->written);
