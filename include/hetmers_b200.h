@@ -414,6 +414,57 @@ int  hm_stream_plan_shards(int64_t n, int kmer, int ibyte, int64_t budget, int n
  * over the shards (0 in core).  Either pointer may be NULL.                                           */
 int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks);
 
+/* ---- lists in host memory (DESIGN.md §4c, *Lists in host memory*) ----
+ * A streamed run keeps its candidate records and S list on the device.  With a list host budget set (process-wide,
+ * bytes; 0, the default, is off) a run whose lists cannot grow within the device budget moves them to host memory
+ * instead of refusing: pass 1 flushes them to host arrays whenever they run out of room (and once more at its end),
+ * and pass 2 uploads the candidates a slice at a time, parks every Bloom hit, and answers the round's queries
+ * against the S list uploaded a partition at a time.  The device then holds the Bloom filter, one chunk and pass
+ * 2's plan (hm_spill_plan); the lists' host bytes must stay within the budget (else HM_ENOMEM naming both sizes).
+ * A run whose lists fit is unchanged.  With several shards in one process, one shard spilling makes every shard
+ * spill.  The one-process-per-GPU ranks (hm_rank_scan_*) never spill.  HETMERS_LIST_HOST_BUDGET=<bytes> sets it
+ * for the executables.                                                                                          */
+void hm_set_list_host_budget(int64_t bytes);
+
+typedef struct hm_spill_stats               /* what the last run of a scan did with its lists                   */
+  { int32_t spilled;                        /* 1 if the lists went to host memory                              */
+    int32_t pad;
+    int64_t flushes;                        /* pass 1 flushes, over the shards                                 */
+    int64_t d2h_bytes;                      /* list bytes moved device -> host in pass 1                       */
+    int64_t host_peak_bytes;                /* host bytes the lists held at most (every shard's)               */
+    int64_t partitions;                     /* S partitions pass 2 walks                                       */
+    int64_t rounds;                         /* pass 2 rounds, over the shards                                  */
+    int64_t h2d_bytes;                      /* candidate slices and S partitions moved host -> device in pass 2 */
+    int64_t slice, part;                    /* candidates per slice, S keys per partition (hm_spill_plan)      */
+    int64_t first_key_queries;              /* partitions whose first key was queried, over rounds and shards  */
+    double  ms_pass1, ms_flush, ms_pass2;   /* pass 1 (the slowest shard's chunk loop); its flushes (the slowest
+                                               shard's); pass 2 (the slowest shard's rounds)                   */
+  } hm_spill_stats;
+int  hm_scan_spill_stats(const hm_scan *s, hm_spill_stats *out);
+
+typedef struct hm_spill_layout              /* pass 2 of host lists in `room` device bytes                      */
+  { int64_t room;
+    int64_t slice;                          /* candidates per uploaded slice, and the round's pending slots     */
+    int64_t queries;                        /* query slots: 2 per pending slot                                 */
+    int64_t part;                           /* S keys per partition                                            */
+    int32_t part_bits, pad;                 /* bucket index bits of a partition (hm_pick_bucket_bits(part))    */
+    int64_t slice_bytes, part_bytes;        /* device bytes of the slice side and of the partition side        */
+  } hm_spill_layout;
+/* Pass 2's room arithmetic for n_cand candidates (the most of any shard) and an S list of n_s keys (every shard's).
+ * Per slot of a slice: its record (8 KW + 8), a pending slot (8), two queries of 2 (8 KW + 8) + 1 bytes each and
+ * their sort scratch (HM_SPILL_SORT_Q per query + HM_SPILL_SORT_FIXED); per partition key 8 KW, plus its uint32
+ * bucket index.  Everything at full size if it fits; else the slice side takes at most half the room, the
+ * partitions the most the rest holds, and the slice what they leave.  A slice holds at most HM_SPILL_MAX_SLICE
+ * candidates (its 2 x that queries are sorted with 32-bit indices) and a partition at most HM_SPILL_MAX_PART keys
+ * (its bucket index has 32-bit offsets).  HM_ENOMEM, with the sizes, when the room holds less than
+ * min(n, HM_SPILL_MIN) of either.                                                                               */
+#define HM_SPILL_MIN        1024
+#define HM_SPILL_SORT_Q     32
+#define HM_SPILL_SORT_FIXED (64ll << 10)
+#define HM_SPILL_MAX_SLICE  0x3FFFFFF0ll
+#define HM_SPILL_MAX_PART   0xFFFFFFEFll
+int  hm_spill_plan(int64_t n_cand, int64_t n_s, int kmer, int64_t room, hm_spill_layout *out);
+
 /* ---- one rank of a one-process-per-GPU job streaming a strand-symmetric table (DESIGN.md §4c, *Ranks*) ----
  * Rank `rank` of `world` streams its run-aligned share [c_rank, c_rank+1) (the cuts of the in-process shards)
  * through `device` under the device budget; no rank holds the table, and no call reads another rank's memory.

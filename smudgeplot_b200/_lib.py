@@ -43,6 +43,7 @@ ABI_SYMBOLS = [
     "hm_rank_scan_extract_records", "hm_k_pairs_hist", "hm_k_pairs_route_count", "hm_k_pairs_route_scatter",
     "hm_pairs_sort_scratch_bytes", "hm_k_pairs_sort", "hm_k_pairs_label_bounds", "hm_k_pairs_format", "hm_pairs_bytes",
     "hm_scan_write_pairs", "hm_scan_pairs_hist", "hm_pair_windows",
+    "hm_set_list_host_budget", "hm_scan_spill_stats", "hm_spill_plan",
 ]
 
 
@@ -84,6 +85,28 @@ class StreamLayout(C.Structure):
     _fields_ = [("budget", C.c_int64), ("chunk", C.c_int64), ("fixed_bytes", C.c_int64), ("chunk_bytes", C.c_int64),
                 ("list_bytes", C.c_int64), ("chunk_list_bytes", C.c_int64)]
 
+
+class SpillStats(C.Structure):
+    """hm_spill_stats: what the last streamed run did with its lists (host memory when spilled)"""
+    _fields_ = [("spilled", C.c_int32), ("pad", C.c_int32), ("flushes", C.c_int64), ("d2h_bytes", C.c_int64),
+                ("host_peak_bytes", C.c_int64), ("partitions", C.c_int64), ("rounds", C.c_int64),
+                ("h2d_bytes", C.c_int64), ("slice", C.c_int64), ("part", C.c_int64),
+                ("first_key_queries", C.c_int64), ("ms_pass1", C.c_double), ("ms_flush", C.c_double), ("ms_pass2", C.c_double)]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k != "pad"}
+        d["spilled"] = bool(d["spilled"])
+        return d
+
+
+class SpillLayout(C.Structure):
+    """hm_spill_layout: pass 2's slices and S partitions for lists in host memory"""
+    _fields_ = [("room", C.c_int64), ("slice", C.c_int64), ("queries", C.c_int64), ("part", C.c_int64),
+                ("part_bits", C.c_int32), ("pad", C.c_int32), ("slice_bytes", C.c_int64), ("part_bytes", C.c_int64)]
+
+
+SPILL_MIN, SPILL_SORT_Q, SPILL_SORT_FIXED = 1024, 32, 64 << 10
+SPILL_MAX_SLICE, SPILL_MAX_PART = 0x3FFFFFF0, 0xFFFFFFEF   # 32-bit query indices; 32-bit partition bucket index
 
 COND_HIST_BITS = 20
 COND_MAX_GPUS = 16
@@ -214,6 +237,10 @@ def lib():
     L.hm_stream_plan.argtypes = [i64, i32, i32, i64, C.POINTER(StreamLayout)]
     L.hm_stream_plan_shards.argtypes = [i64, i32, i32, i64, i32, C.POINTER(StreamLayout)]
     L.hm_scan_residency.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
+    L.hm_set_list_host_budget.argtypes = [i64]
+    L.hm_set_list_host_budget.restype = None
+    L.hm_scan_spill_stats.argtypes = [vp, C.POINTER(SpillStats)]
+    L.hm_spill_plan.argtypes = [i64, i64, i32, i64, C.POINTER(SpillLayout)]
     u64p, i64p = C.POINTER(C.c_uint64), C.POINTER(i64)
     L.hm_rank_scan_create.argtypes = [C.POINTER(HostTable), i32, i32, i32, u64p, C.POINTER(vp)]
     L.hm_rank_scan_create_share.argtypes = [C.POINTER(HostTable), i64, i64p, u64p, i32, i32, i32, u64p, C.POINTER(vp)]

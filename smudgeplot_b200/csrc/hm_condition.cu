@@ -531,3 +531,22 @@ int hm_sort_keys(uint64_t *keys, uint64_t *lo, int64_t n, int kmer, void *scratc
     }
   return HM_OK;
 }
+
+/* CUB's temporary storage for hm_sort_perm of up to n keys */
+int64_t hm_sort_perm_bytes(int64_t n)
+{ size_t need = 0;
+  if (n < 1) n = 1;
+  cub::DeviceRadixSort::SortPairs(NULL,need,(const uint64_t *) NULL,(uint64_t *) NULL,(const uint32_t *) NULL,
+                                  (uint32_t *) NULL,n,0,64);
+  return (int64_t) need + 256;
+}
+
+/* one stable radix sort of n keys k_in -> k_out carrying v_in -> v_out, enqueued on st */
+int hm_sort_perm(const uint64_t *k_in, uint64_t *k_out, const uint32_t *v_in, uint32_t *v_out, int64_t n,
+                 void *tmp, int64_t tmp_bytes, cudaStream_t st)
+{ size_t tb = (size_t) tmp_bytes;
+  if (tmp_bytes < hm_sort_perm_bytes(n))
+    return hm_set_error(HM_EINVAL,"hm_sort_perm: %lld bytes of scratch for %lld keys",(long long) tmp_bytes,(long long) n);
+  HM_CUDA(cub::DeviceRadixSort::SortPairs(tmp,tb,k_in,k_out,v_in,v_out,n,0,64,st));
+  return HM_OK;
+}

@@ -52,6 +52,7 @@ int hm_symm_stream_chunk(const uint64_t *d_keys, const uint64_t *d_keys_lo, cons
                          const hm_symm_shards *shards, void *stream);
 int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t *n_cand,
                           uint64_t *status, uint64_t *n_s, void *stream);
+int hm_symm_stream_reset_lists(void *d_work, const hm_symm_layout *L, void *stream);
 /* one shard: the exact checks look up this shard's S list (d_s_key ...); several: the owner's, through
  * d_views[owner] (device array of shards->n_seg views)                                                 */
 int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
@@ -122,6 +123,22 @@ int hm_cuda_fail(cudaError_t e, const char *what);
 int64_t hm_sort_keys_bytes(int64_t n, int kmer);
 int     hm_sort_keys(uint64_t *keys, uint64_t *lo, int64_t n, int kmer, void *scratch, int64_t scratch_bytes,
                      cudaStream_t st);
+/* a stable radix sort of n one-word keys carrying uint32 values, in CUB scratch of hm_sort_perm_bytes (hm_condition.cu) */
+int64_t hm_sort_perm_bytes(int64_t n);
+int     hm_sort_perm(const uint64_t *k_in, uint64_t *k_out, const uint32_t *v_in, uint32_t *v_out, int64_t n,
+                     void *tmp, int64_t tmp_bytes, cudaStream_t st);
+/* lists in host memory (DESIGN.md §4c): a slice of n candidates (R's cand arrays, R->cand_cap >= n) swept by
+ * resolve_kernel<..., LK_PARK> into B's pending list and queries (reset: the slice opens a round); the round's
+ * counts (synchronises); its queries sorted by key into B->send, their slots into perm_a or perm_b (B->send_slot
+ * is set to it; at k > 32 B->send has 2 q_cap words); then hm_symm_route_answer per S partition and
+ * hm_symm_route_settle                                                                                      */
+int hm_symm_park_resolve(int kmer, int64_t n, int reset, void *d_work, const hm_symm_layout *L,
+                         const hm_stream_lists *R, const hm_symm_shards *shards, const hm_route_bufs *B,
+                         unsigned long long *d_plot, void *stream);
+int hm_symm_park_counts(const void *d_work, const hm_symm_layout *L, int64_t *n_pend, int64_t *n_q, uint64_t *status,
+                        void *stream);
+int hm_symm_park_sort(int kmer, hm_route_bufs *B, int64_t n_q, uint32_t *perm_a, uint32_t *perm_b,
+                      void *tmp, int64_t tmp_bytes, void *stream);
 /* conditioning, a key range at a time (hm_condition.cu; driven by hm_scan_condition and hm_scan_condition_files
  * in hm_scan.cu and by hm_k_shard_settle): the device buffers of one range of at most `cap` output entries.
  * key / lo / cnt: the region the kept originals fill from the front and the reverse complements from the back;

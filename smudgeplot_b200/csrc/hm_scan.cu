@@ -92,6 +92,9 @@ struct hm_scan
     volatile int stop;                    /* (streamed) a shard failed: the others leave their chunk loops     */
     int      nshard, rank;                /* (streamed) shards of the table, and the one d[0] streams: n_gpus and 0  */
                                           /*   in one process, (world, rank) for one rank of a job (hm_rank_scan)  */
+    hm_spill_stats spill;                 /* (streamed) what the last run did with its lists (hm_scan_spill_stats) */
+    int64_t  list_cap;                    /* (streamed) the run's list host budget (0: the lists stay on the device) */
+    int64_t  host_held;                   /* (streamed) host bytes the lists of every shard hold                     */
   };
 
 static double now_ms(void)
@@ -566,6 +569,59 @@ static int fingerprint_verdict(hm_scan *s)
 static int64_t g_budget = 0;
 
 extern "C" void hm_set_device_budget(int64_t bytes) { g_budget = bytes > 0 ? bytes : 0; }
+
+/* host bytes a streamed run's lists may take in host memory (0: they stay on the device or the run refuses) */
+static int64_t g_list_host_budget = 0;
+
+extern "C" void hm_set_list_host_budget(int64_t bytes) { g_list_host_budget = bytes > 0 ? bytes : 0; }
+
+/* pass 2 of lists in host memory: device bytes of a slice of c candidates with its pending slots, queries and
+ * their sort scratch, and of a partition of p S keys with its bucket index                                  */
+static int64_t spill_slice_bytes(int64_t c, int KW)
+{ return c*(8*KW+8) + 8*c + 2*c*(2*(8*KW+8)+1) + 2*c*HM_SPILL_SORT_Q + HM_SPILL_SORT_FIXED; }
+
+static int64_t spill_part_bytes(int64_t p, int KW)
+{ return p*8*KW + 4*((1ll << hm_pick_bucket_bits(p))+1); }
+
+/* the largest x <= most with f(x) <= room (f increasing), 0 if none */
+static int64_t spill_largest(int64_t most, int64_t room, int KW, int64_t (*f)(int64_t, int))
+{ int64_t lo = 0, hi = most;
+  while (lo < hi)
+    { int64_t mid = lo + (hi-lo+1)/2;
+      if (f(mid,KW) <= room) lo = mid; else hi = mid-1;
+    }
+  return lo;
+}
+
+extern "C" int hm_spill_plan(int64_t n_cand, int64_t n_s, int kmer, int64_t room, hm_spill_layout *out)
+{ if (n_cand < 0 || n_s < 0 || kmer < 1 || kmer > HM_MAX_KMER || out == NULL)
+    return hm_set_error(HM_EINVAL,"hm_spill_plan: bad arguments");
+  int     KW = kmer > 32 ? 2 : 1;
+  int64_t nc = n_cand > 1 ? n_cand : 1, np = n_s > 1 ? n_s : 1, slice, part;
+  if (nc > HM_SPILL_MAX_SLICE) nc = HM_SPILL_MAX_SLICE;      /* query indices and slots are 32-bit        */
+  if (np > HM_SPILL_MAX_PART)  np = HM_SPILL_MAX_PART;       /* a partition's bucket index is 32-bit      */
+  if (spill_slice_bytes(nc,KW) + spill_part_bytes(np,KW) <= room)
+    { slice = nc; part = np; }
+  else
+    { slice = spill_largest(nc,room/2,KW,spill_slice_bytes);
+      part  = spill_largest(np,room-spill_slice_bytes(slice,KW),KW,spill_part_bytes);
+      slice = spill_largest(nc,room-spill_part_bytes(part,KW),KW,spill_slice_bytes);
+    }
+  int64_t min_c = nc < HM_SPILL_MIN ? nc : HM_SPILL_MIN, min_p = np < HM_SPILL_MIN ? np : HM_SPILL_MIN;
+  if (slice < min_c || part < min_p)
+    return hm_set_error(HM_ENOMEM,"pass 2 of the streamed scan's lists in host memory has %lld bytes of device room, "
+                        "and slices of %lld candidates (%lld bytes) beside partitions of %lld S keys (%lld bytes) need "
+                        "%lld; give the scan a larger device budget (HETMERS_DEVICE_BUDGET)",(long long) room,
+                        (long long) min_c,(long long) spill_slice_bytes(min_c,KW),(long long) min_p,
+                        (long long) spill_part_bytes(min_p,KW),
+                        (long long) (spill_slice_bytes(min_c,KW) + spill_part_bytes(min_p,KW)));
+  memset(out,0,sizeof(*out));
+  out->room = room;
+  out->slice = slice; out->queries = 2*slice;
+  out->part = part; out->part_bits = hm_pick_bucket_bits(part);
+  out->slice_bytes = spill_slice_bytes(slice,KW); out->part_bytes = spill_part_bytes(part,KW);
+  return HM_OK;
+}
 
 /* the budget per GPU: the one set, or the smallest free memory of the devices (counting what an idle
  * stream-ordered pool keeps reserved for us) minus a reserve for the CUDA runtime and library code; a device
@@ -2042,6 +2098,43 @@ static int last_run_start(const uint64_t *d_keys, int64_t m, int kmer, int64_t *
   return HM_OK;
 }
 
+/* lists in host memory: blocks of pageable host memory, each one flush's entries -- nw arrays of n words one after
+ * another (candidates: key, meta and at k > 32 lo; S: key and at k > 32 lo).  They move to and from the device
+ * through a shard's two pinned staging halves (stage_copy), so the pinned memory stays 2 SPILL_STAGE_BYTES per
+ * shard whatever the lists' size.                                                                             */
+typedef struct { uint64_t *w; int64_t n; } HostBlock;
+typedef struct { HostBlock *b; int nb, cap; } HostList;
+
+/* a new block of n entries of nw words at the end of L (*out: its words) */
+static int host_list_add(HostList *L, int64_t n, int nw, uint64_t **out)
+{ if (L->nb == L->cap)
+    { int        cap = L->cap ? 2*L->cap : 16;
+      HostBlock *b = (HostBlock *) realloc(L->b,sizeof(HostBlock)*(size_t) cap);
+      if (b == NULL) return hm_set_error(HM_ENOMEM,"out of host memory");
+      L->b = b; L->cap = cap;
+    }
+  void *p = malloc(8*(size_t) n*(size_t) nw);
+  if (p == NULL)
+    return hm_set_error(HM_ENOMEM,"out of host memory for the streamed scan's host lists (%lld bytes)",
+                        (long long) (8*n*nw));
+  L->b[L->nb].w = (uint64_t *) p; L->b[L->nb].n = n;
+  L->nb += 1;
+  *out = (uint64_t *) p;
+  return HM_OK;
+}
+
+static int64_t host_list_entries(const HostList *L)
+{ int64_t n = 0;
+  for (int i = 0; i < L->nb; i++) n += L->b[i].n;
+  return n;
+}
+
+static void host_list_free(HostList *L)
+{ for (int i = 0; i < L->nb; i++) free(L->b[i].w);
+  free(L->b);
+  memset(L,0,sizeof(*L));
+}
+
 /* everything one streamed run allocates */
 typedef struct
   { int64_t   cap;                                     /* entries per chunk buffer */
@@ -2060,6 +2153,13 @@ typedef struct
     cudaStream_t sc;                                   /* the chunks' kernels: overlap the next chunk's load */
     hm_stream_sview *views;                            /* several shards: every shard's S view, on this device */
     double    ms_loop;                                 /* the chunk loop, wall clock */
+    int       spill, spilled;                          /* the lists may go to host memory; they have        */
+    int64_t   list_room;                               /* (tests) HETMERS_LIST_ROOM: flush above this many list bytes */
+    HostList  hc, hs;                                  /* there: the candidate records, the S list          */
+    uint8_t  *stage[2];                                /* pinned staging halves (stage_copy)                */
+    cudaEvent_t stage_ev[2];
+    int64_t   flushes, d2h_bytes, rounds, h2d_bytes, first_key_queries;
+    double    ms_flush, ms_pass2;
   } StreamRun;
 
 static void stream_free_chunks(DevTable *D, StreamRun *R)
@@ -2133,11 +2233,103 @@ static int stream_grow(hm_scan *s, DevTable *D, cudaStream_t st, uint64_t **arr[
   return HM_OK;
 }
 
+#define SPILL_STAGE_BYTES (16ll << 20)            /* one pinned staging half */
+
+/* the shard's staging halves and their events, once per run (freed by stream_release) */
+static int stage_open(StreamRun *R)
+{ if (R->stage[0] != NULL)
+    return HM_OK;
+  for (int i = 0; i < 2; i++)
+    { HM_CUDA(cudaHostAlloc((void **) &R->stage[i],(size_t) SPILL_STAGE_BYTES,cudaHostAllocPortable));
+      HM_CUDA(cudaEventCreateWithFlags(&R->stage_ev[i],cudaEventDisableTiming));
+    }
+  return HM_OK;
+}
+
+static void stage_close(StreamRun *R)
+{ for (int i = 0; i < 2; i++)
+    { if (R->stage_ev[i]) { cudaEventSynchronize(R->stage_ev[i]); cudaEventDestroy(R->stage_ev[i]); }
+      if (R->stage[i]) cudaFreeHost(R->stage[i]);
+      R->stage[i] = NULL; R->stage_ev[i] = NULL;
+    }
+}
+
+/* `bytes` from device memory to a pageable host array (to_host) or back, on R->sc, a staging half per piece: the
+ * DMA of one piece overlaps the host copy of the other.  Returns with the host array written (to_host), or with
+ * the host array read and the copies to the device enqueued on R->sc (the halves are waited for before reuse). */
+static int stage_copy(StreamRun *R, void *dst, const void *src, int64_t bytes, int to_host)
+{ const int64_t P = SPILL_STAGE_BYTES, n = (bytes+P-1)/P;
+  int rc;
+  if ((rc = stage_open(R)) != HM_OK)
+    return rc;
+  for (int64_t i = 0; i <= n; i++)
+    { const int h = (int) (i & 1);
+      const int64_t off = i*P, len = i < n ? (bytes-off < P ? bytes-off : P) : 0;
+      if (to_host)
+        { if (i < n)
+            { HM_CUDA(cudaMemcpyAsync(R->stage[h],(const uint8_t *) src+off,(size_t) len,cudaMemcpyDeviceToHost,R->sc));
+              HM_CUDA(cudaEventRecord(R->stage_ev[h],R->sc));
+            }
+          if (i >= 1)
+            { const int64_t o1 = off-P, l1 = bytes-o1 < P ? bytes-o1 : P;
+              HM_CUDA(cudaEventSynchronize(R->stage_ev[h^1]));
+              memcpy((uint8_t *) dst+o1,R->stage[h^1],(size_t) l1);
+            }
+        }
+      else if (i < n)
+        { HM_CUDA(cudaEventSynchronize(R->stage_ev[h]));        /* the half's previous piece has left it */
+          memcpy(R->stage[h],(const uint8_t *) src+off,(size_t) len);
+          HM_CUDA(cudaMemcpyAsync((uint8_t *) dst+off,R->stage[h],(size_t) len,cudaMemcpyHostToDevice,R->sc));
+          HM_CUDA(cudaEventRecord(R->stage_ev[h],R->sc));
+        }
+    }
+  return HM_OK;
+}
+
+/* The nc candidate records and ns S keys on the device (the S keys sorted) appended to the host lists, the list
+ * counts reset and the device lists freed: the next chunk grows them again from nothing.  HM_ENOMEM when the
+ * host lists of every shard would pass the list host budget.                                                */
+static int stream_flush(hm_scan *s, DevTable *D, StreamRun *R, uint64_t nc, uint64_t ns)
+{ int     KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
+  double  t0 = now_ms();
+  int64_t bytes = (int64_t) nc*(8*KW+8) + (int64_t) ns*8*KW;
+  int64_t held = __sync_add_and_fetch(&s->host_held,bytes), pk;
+  if (held > s->list_cap)
+    return hm_set_error(HM_ENOMEM,"the streamed scan's lists need %lld bytes of host memory (%lld of them in this flush) "
+                        "but the list host budget is %lld bytes; give the scan a larger one (HETMERS_LIST_HOST_BUDGET)",
+                        (long long) held,(long long) bytes,(long long) s->list_cap);
+  while ((pk = s->spill.host_peak_bytes) < held && !__sync_bool_compare_and_swap(&s->spill.host_peak_bytes,pk,held))
+    ;
+  uint64_t *h = NULL;
+  if (nc > 0 && (rc = host_list_add(&R->hc,(int64_t) nc,KW+1,&h)) == HM_OK)
+    { rc = stage_copy(R,h,R->R.cand_key,8*(int64_t) nc,1);
+      if (rc == HM_OK) rc = stage_copy(R,h+nc,R->R.cand_meta,8*(int64_t) nc,1);
+      if (rc == HM_OK && KW == 2) rc = stage_copy(R,h+2*nc,R->R.cand_lo,8*(int64_t) nc,1);
+    }
+  if (rc == HM_OK && ns > 0 && (rc = host_list_add(&R->hs,(int64_t) ns,KW,&h)) == HM_OK)
+    { rc = stage_copy(R,h,R->R.s_key,8*(int64_t) ns,1);
+      if (rc == HM_OK && KW == 2) rc = stage_copy(R,h+ns,R->R.s_lo,8*(int64_t) ns,1);
+    }
+  if (rc == HM_OK) rc = hm_symm_stream_reset_lists(R->work,&R->L,R->sc);
+  if (rc != HM_OK) return rc;
+  HM_CUDA(cudaStreamSynchronize(R->sc));
+  dev_free(D,R->R.cand_key); dev_free(D,R->R.cand_meta); dev_free(D,R->R.cand_lo);
+  dev_free(D,R->R.s_key);    dev_free(D,R->R.s_lo);
+  R->R.cand_key = R->R.cand_meta = R->R.cand_lo = R->R.s_key = R->R.s_lo = NULL;
+  R->R.cand_cap = R->R.s_cap = 0;
+  R->spilled = 1;
+  R->flushes += 1;
+  R->d2h_bytes += bytes;
+  R->ms_flush += now_ms()-t0;
+  return HM_OK;
+}
+
 /* pass 1 of one shard: its range [D->lo, D->hi) chunk by chunk (leaves early, with HM_OK, once s->stop is set) */
 static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shards *sh)
 { const hm_host_table *t = s->host;
   int      KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
   int64_t  lo = D->lo, hi = D->hi, c0 = lo, chunks = 0;
+  int64_t  from = lo;                                /* where the lists on the device began: lo, or the last flush */
   int      b = 0;
   uint64_t nc = 0, status = 0, ns = 0, ns0 = 0;     /* ns0: S keys before the chunk in flight */
   HM_CUDA(cudaEventRecord(D->ev[0],R->sc));
@@ -2168,14 +2360,26 @@ static int stream_pass(hm_scan *s, DevTable *D, StreamRun *R, const hm_symm_shar
                              R->sort_tmp,R->sort_bytes,R->sc)) != HM_OK)
         break;
       ns0 = ns;
-      { uint64_t **ca[3] = { &R->R.cand_key, &R->R.cand_meta, &R->R.cand_lo };
-        uint64_t **sa[2] = { &R->R.s_key, &R->R.s_lo };
-        rc = stream_grow(s,D,R->sc,ca,KW == 2 ? 3 : 2,&R->R.cand_cap,(int64_t) nc,(int64_t) nc + cut/2 + 1024,
-                         c0-lo,hi-lo,"candidate");
-        if (rc == HM_OK)
-          rc = stream_grow(s,D,R->sc,sa,KW,&R->R.s_cap,(int64_t) ns,(int64_t) ns + cut + 1024,c0-lo,hi-lo,"S");
-        if (rc != HM_OK) break;
-      }
+      for (int flushed = 0; ; flushed = 1)        /* no room left: with a list host budget, flush and grow again */
+        { uint64_t **ca[3] = { &R->R.cand_key, &R->R.cand_meta, &R->R.cand_lo };
+          uint64_t **sa[2] = { &R->R.s_key, &R->R.s_lo };
+          int64_t    want = ((int64_t) nc + cut/2 + 1024)*(8*KW+8) + ((int64_t) ns + cut + 1024)*8*KW;
+          if (R->spill && R->list_room > 0 && !flushed && want > R->list_room)
+            rc = HM_ENOMEM;
+          else
+            { rc = stream_grow(s,D,R->sc,ca,KW == 2 ? 3 : 2,&R->R.cand_cap,(int64_t) nc,(int64_t) nc + cut/2 + 1024,
+                               c0-from,hi-from,"candidate");
+              if (rc == HM_OK)
+                rc = stream_grow(s,D,R->sc,sa,KW,&R->R.s_cap,(int64_t) ns,(int64_t) ns + cut + 1024,c0-from,hi-from,"S");
+            }
+          if (rc != HM_ENOMEM || !R->spill || flushed)
+            break;
+          if ((rc = stream_flush(s,D,R,nc,ns)) != HM_OK)
+            break;
+          nc = ns = ns0 = 0;
+          from = c0;
+        }
+      if (rc != HM_OK) break;
       rc = hm_k_build_bucket_index(R->keys[b],m,R->bits,R->bucket,0,R->sc);
       if (rc == HM_OK)
         rc = hm_k_symm_fingerprint(R->keys[b],KW == 2 ? R->klo[b] : NULL,R->cnt[b],0,cut,s->kmer,s->seed,D->fp_acc,R->sc);
@@ -2227,6 +2431,8 @@ static int shard_pass1(hm_scan *s, int g, void *arg)
   if ((rc = hm_symm_stream_counts(R->work,&R->L,&nc,&status,&ns,R->sc)) != HM_OK) return rc;
   if (status != 0)
     return hm_set_error(HM_ECUDA,"streamed scan: list overflow in pass 1 (status %llu)",(unsigned long long) status);
+  if (R->spilled)                               /* the rest of the lists joins what went to host memory */
+    return stream_flush(s,D,R,nc,ns);
   return HM_OK;
 }
 
@@ -2268,46 +2474,229 @@ static void stream_release(hm_scan *s, int g, StreamRun *R)
   dev_free(D,R->R.cand_key); dev_free(D,R->R.cand_meta); dev_free(D,R->R.cand_lo);
   dev_free(D,R->R.s_key);    dev_free(D,R->R.s_lo);
   if (D->st) cudaStreamSynchronize(D->st);
+  if (R->sc) cudaStreamSynchronize(R->sc);
+  host_list_free(&R->hc); host_list_free(&R->hs);
+  stage_close(R);
   if (R->sc) cudaStreamDestroy(R->sc);
   cudaCtxResetPersistingL2Cache();
   cudaGetLastError();
   memset(R,0,sizeof(*R));
 }
 
-/* Pass 1 of every shard at once; the verdict over all shards' fingerprints; the Bloom segments all-gathered; the
- * chunk buffers and stub index freed, to make room for each shard's S index; pass 2 of every shard, whose exact
- * checks look keys up in the S list of their owner (peer memory); the plots summed on the host.              */
-static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_stats *stats)
-{ int       G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
-  double    t0 = now_ms();
-  double    ms_loop = 0;
-  cudaError_t e;
-  s->stop = 0;
-  if ((rc = on_every_gpu(s,shard_pass1,RR)) != HM_OK)
-    return rc;
-  for (int g = 0; g < G; g++)
-    if (RR[g].ms_loop > ms_loop) ms_loop = RR[g].ms_loop;
-  float  ms1 = slowest_ms(s,0,1);
-  double t_pass1 = now_ms();
-  if ((rc = fingerprint_verdict(s)) != HM_OK) return rc;
-  if (!s->symmetric)
-    return refuse_asymmetric(s);
+/* ---- pass 2 of lists in host memory (DESIGN.md §4c, *Lists in host memory*) ---- */
 
-  uint64_t ns[HM_MAX_GPUS];
-  int      sbits[HM_MAX_GPUS], sidx64 = 0;
+/* one S partition: n keys (and at k > 32 their second words) in a host block; partitions cut the concatenated S
+ * lists of the shards -- the whole table's S, sorted -- into pieces of at most plan.part keys                   */
+typedef struct { const uint64_t *key, *lo; int64_t n; } SpillPart;
+
+typedef struct
+  { StreamRun      *RR;
+    hm_spill_layout P;
+    SpillPart      *parts;
+    int64_t         nparts;
+  } SpillRun;
+
+/* the first index in [lo, hi) of the sorted queries q (KW words each) whose key is >= (kh, kl) */
+static int64_t query_lower_bound(const uint64_t *q, int KW, int64_t lo, int64_t hi, uint64_t kh, uint64_t kl)
+{ while (lo < hi)
+    { int64_t  m = lo + (hi-lo)/2;
+      uint64_t h = q[KW*m], l = KW == 2 ? q[KW*m+1] : 0;
+      if (h < kh || (h == kh && l < kl)) lo = m+1; else hi = m;
+    }
+  return lo;
+}
+
+/* the device buffers of one shard's pass 2 over host lists */
+typedef struct
+  { hm_stream_lists L;                            /* cand_key / cand_meta / cand_lo: one slice */
+    hm_route_bufs   B;
+    uint32_t       *perm[2];
+    uint8_t        *ans;
+    void           *tmp;
+    int64_t         tmp_bytes;
+    uint64_t       *pkey, *plo;                   /* one partition and its bucket index */
+    void           *pbucket;
+    uint64_t       *hq;                           /* (host) the round's sorted queries */
+  } SpillBufs;
+
+static void spill_free(DevTable *D, StreamRun *R, SpillBufs *X)
+{ if (R->sc) cudaStreamSynchronize(R->sc);
+  dev_free(D,X->L.cand_key); dev_free(D,X->L.cand_meta); dev_free(D,X->L.cand_lo);
+  dev_free(D,X->B.pend); dev_free(D,X->B.q_key); dev_free(D,X->B.q_lo); dev_free(D,X->B.q_tag); dev_free(D,X->B.send);
+  dev_free(D,X->perm[0]); dev_free(D,X->perm[1]); dev_free(D,X->ans); dev_free(D,X->tmp);
+  dev_free(D,X->pkey); dev_free(D,X->plo); dev_free(D,X->pbucket);
+  free(X->hq);
+  memset(X,0,sizeof(*X));
+}
+
+/* the round's parked candidates settled: its queries sorted by key, each S partition some query falls in uploaded
+ * and indexed, the queries in it answered; then every parked candidate none of whose queries was found counted */
+static int spill_settle(hm_scan *s, int g, const SpillRun *S, StreamRun *R, SpillBufs *X, int64_t n_pend, int64_t n_q)
+{ DevTable *D = s->d+g;
+  const int KW = s->kmer > 32 ? 2 : 1, bits = S->P.part_bits;
+  int rc;
+  if ((rc = hm_symm_park_sort(s->kmer,&X->B,n_q,X->perm[0],X->perm[1],X->tmp,X->tmp_bytes,R->sc)) != HM_OK)
+    return rc;
+  if (n_q > 0)
+    { HM_CUDA(cudaMemcpyAsync(X->hq,X->B.send,8*(size_t) KW*(size_t) n_q,cudaMemcpyDeviceToHost,R->sc));
+      HM_CUDA(cudaMemsetAsync(X->ans,0,(size_t) n_q,R->sc));
+      HM_CUDA(cudaStreamSynchronize(R->sc));
+    }
+  int64_t lo = 0;
+  for (int64_t p = 0; p < S->nparts && lo < n_q && rc == HM_OK; p++)
+    { const SpillPart *P = S->parts+p;
+      int64_t hi = n_q;
+      if (p+1 < S->nparts)
+        hi = query_lower_bound(X->hq,KW,lo,n_q,P[1].key[0],KW == 2 ? P[1].lo[0] : 0);
+      if (hi == lo)
+        continue;                               /* no query falls in this partition: nothing uploaded */
+      R->first_key_queries += (X->hq[KW*lo] == P->key[0] && (KW == 1 || X->hq[KW*lo+1] == P->lo[0]));
+      rc = stage_copy(R,X->pkey,P->key,8*P->n,0);
+      if (rc == HM_OK && KW == 2) rc = stage_copy(R,X->plo,P->lo,8*P->n,0);
+      if (rc == HM_OK) rc = hm_k_build_bucket_index(X->pkey,P->n,bits,X->pbucket,0,R->sc);
+      if (rc == HM_OK)
+        rc = hm_symm_route_answer(X->pkey,X->plo,X->pbucket,bits,0,s->kmer,X->B.send+KW*lo,hi-lo,X->ans+lo,R->sc);
+      R->h2d_bytes += 8*KW*P->n;
+      __sync_fetch_and_add(&s->launches,2);
+      lo = hi;
+    }
+  if (rc == HM_OK)
+    rc = hm_symm_route_settle(s->kmer,&X->B,X->ans,n_q,n_pend,D->plot,R->sc);
+  __sync_fetch_and_add(&s->launches,2);
+  R->rounds += 1;
+  return rc;
+}
+
+/* on_every_gpu: shard g's pass 2 over its candidates in host memory, in rounds of slices (arg: the SpillRun) */
+static int shard_spill_pass2(hm_scan *s, int g, void *arg)
+{ const SpillRun *S = (const SpillRun *) arg;
+  DevTable  *D = s->d+g;
+  StreamRun *R = S->RR+g;
+  const hm_symm_shards *sh = s->nshard > 1 ? s->ssh+g : NULL;
+  const int  KW = s->kmer > 32 ? 2 : 1;
+  const int64_t C = S->P.slice, Q = S->P.queries;
+  SpillBufs  X;
+  int        rc = HM_OK;
+  cudaError_t e;
+  memset(&X,0,sizeof(X));
+  X.L = R->R;
+  X.L.cand_cap = C;
+  X.tmp_bytes = hm_sort_perm_bytes(Q);
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&X.L.cand_key,8*C));
+  TRY(dev_alloc(D,&X.L.cand_meta,8*C));
+  X.L.cand_lo = NULL;
+  if (KW == 2) TRY(dev_alloc(D,&X.L.cand_lo,8*C));
+  TRY(dev_alloc(D,&X.B.pend,8*C));
+  TRY(dev_alloc(D,&X.B.q_key,8*Q));
+  if (KW == 2) TRY(dev_alloc(D,&X.B.q_lo,8*Q));
+  TRY(dev_alloc(D,&X.B.q_tag,8*Q));
+  TRY(dev_alloc(D,&X.B.send,8*KW*Q));
+  TRY(dev_alloc(D,&X.perm[0],4*Q));
+  TRY(dev_alloc(D,&X.perm[1],4*Q));
+  TRY(dev_alloc(D,&X.ans,Q));
+  TRY(dev_alloc(D,&X.tmp,X.tmp_bytes));
+  TRY(dev_alloc(D,&X.pkey,8*S->P.part));
+  if (KW == 2) TRY(dev_alloc(D,&X.plo,8*S->P.part));
+  TRY(dev_alloc(D,&X.pbucket,4*((1ll << S->P.part_bits)+1)));
+  X.B.pend_cap = C; X.B.q_cap = Q;
+  if (rc == HM_OK && D->held > s->budget)
+    rc = hm_set_error(HM_ENOMEM,"pass 2 of the streamed scan's lists in host memory holds %lld device bytes, more than "
+                      "the budget of %lld (the plan counted %lld)",(long long) D->held,(long long) s->budget,
+                      (long long) (S->P.slice_bytes+S->P.part_bytes));
+  if (rc == HM_OK && (X.hq = (uint64_t *) malloc(8*(size_t) KW*(size_t) Q)) == NULL)
+    rc = hm_set_error(HM_ENOMEM,"out of host memory");
+  double  t0 = now_ms();
+  int64_t in_round = 0, n_pend = 0, n_q = 0;
+  uint64_t status = 0;
+  if (rc == HM_OK) cudaEventRecord(D->ev[2],R->sc);
+  for (int b = 0; b < R->hc.nb && rc == HM_OK && !s->stop; b++)
+    { const HostBlock *hb = R->hc.b+b;
+      for (int64_t c = 0; c < hb->n && rc == HM_OK; c += C)
+        { int64_t m = hb->n-c < C ? hb->n-c : C;
+          if (in_round > 0 && n_pend + m > C)           /* the next slice might not find a pending slot for each hit */
+            { rc = spill_settle(s,g,S,R,&X,n_pend,n_q);
+              in_round = 0;
+              if (rc != HM_OK) break;
+            }
+          rc = stage_copy(R,X.L.cand_key,hb->w+c,8*m,0);
+          if (rc == HM_OK) rc = stage_copy(R,X.L.cand_meta,hb->w+hb->n+c,8*m,0);
+          if (rc == HM_OK && KW == 2) rc = stage_copy(R,X.L.cand_lo,hb->w+2*hb->n+c,8*m,0);
+          R->h2d_bytes += m*(8*KW+8);
+          if (rc == HM_OK)
+            rc = hm_symm_park_resolve(s->kmer,m,in_round == 0,R->work,&R->L,&X.L,sh,&X.B,D->plot,R->sc);
+          __sync_fetch_and_add(&s->launches,1);
+          if (rc == HM_OK)
+            rc = hm_symm_park_counts(R->work,&R->L,&n_pend,&n_q,&status,R->sc);
+          if (rc == HM_OK && (status != 0 || n_pend > C || n_q > Q))   /* the round rule keeps both within the buffers */
+            rc = hm_set_error(HM_ECUDA,"streamed scan: pass 2 of the host lists overflowed (status %llu, %lld parked "
+                              "of %lld slots, %lld queries of %lld)",(unsigned long long) status,(long long) n_pend,
+                              (long long) C,(long long) n_q,(long long) Q);
+          in_round += 1;
+        }
+    }
+  if (rc == HM_OK && in_round > 0)
+    rc = spill_settle(s,g,S,R,&X,n_pend,n_q);
+  cudaEventRecord(D->ev[3],R->sc);
+  R->ms_pass2 = now_ms()-t0;
+  spill_free(D,R,&X);
+  return rc;
+}
+
+/* pass 2 of every shard whose lists went to host memory: the chunk buffers and stub index freed, one plan for the
+ * room that leaves on every shard, the S partitions cut, the rounds of every shard at once                   */
+static int spill_pass2(hm_scan *s, StreamRun *RR)
+{ int      G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc;
+  int64_t  ncmax = 0, ns = 0, room = -1;
+  SpillRun S;
+  memset(&S,0,sizeof(S));
+  S.RR = RR;
   for (int g = 0; g < G; g++)
-    { uint64_t nc = 0, status = 0;
-      HM_CUDA(cudaSetDevice(s->d[g].dev));
-      if ((rc = hm_symm_stream_counts(RR[g].work,&RR[g].L,&nc,&status,&ns[g],RR[g].sc)) != HM_OK) return rc;
-      if ((int64_t) ns[g] >= 0xFFFFFFF0ll) sidx64 = 1;    /* one offset width for every shard's index */
+    { DevTable *D = s->d+g;
+      HM_CUDA(cudaSetDevice(D->dev));
+      stream_free_chunks(D,RR+g);
+      dev_free(D,RR[g].d_index); RR[g].d_index = NULL;
+      int64_t nc = host_list_entries(&RR[g].hc);
+      if (nc > ncmax) ncmax = nc;
+      ns += host_list_entries(&RR[g].hs);
+      if (room < 0 || s->budget - D->held < room) room = s->budget - D->held;
     }
-  if (G > 1)                                    /* every shard pulls the other shards' Bloom segments */
-    { void *work[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
-      for (int g = 0; g < G; g++)
-        { work[g] = RR[g].work; st[g] = RR[g].sc; }
-      if ((rc = gather_bloom(s,work,&RR[0].L,st,1)) != HM_OK)
-        return rc;
+  const char *e = getenv("HETMERS_SPILL_ROOM");              /* smaller slices and partitions than the room allows */
+  if (e != NULL && atoll(e) > 0 && atoll(e) < room)
+    room = atoll(e);
+  if ((rc = hm_spill_plan(ncmax,ns,s->kmer,room,&S.P)) != HM_OK)
+    return rc;
+  if ((e = getenv("HETMERS_SPILL_PART")) != NULL && atoll(e) > 0 && atoll(e) < S.P.part)   /* smaller partitions */
+    { S.P.part = atoll(e);
+      S.P.part_bits = hm_pick_bucket_bits(S.P.part);
     }
+  int64_t np = 0;
+  for (int g = 0; g < G; g++)
+    for (int b = 0; b < RR[g].hs.nb; b++)
+      np += (RR[g].hs.b[b].n + S.P.part-1)/S.P.part;
+  if ((S.parts = (SpillPart *) malloc(sizeof(SpillPart)*(size_t) (np > 0 ? np : 1))) == NULL)
+    return hm_set_error(HM_ENOMEM,"out of host memory");
+  for (int g = 0; g < G; g++)                                  /* shards in key order, blocks in key order */
+    for (int b = 0; b < RR[g].hs.nb; b++)
+      { const HostBlock *hb = RR[g].hs.b+b;
+        for (int64_t o = 0; o < hb->n; o += S.P.part)
+          { SpillPart *P = S.parts + S.nparts++;
+            P->key = hb->w+o; P->lo = KW == 2 ? hb->w+hb->n+o : NULL;
+            P->n = hb->n-o < S.P.part ? hb->n-o : S.P.part;
+          }
+      }
+  rc = on_every_gpu(s,shard_spill_pass2,&S);
+  free(S.parts);
+  s->spill.partitions = S.nparts;
+  s->spill.slice = S.P.slice; s->spill.part = S.P.part;
+  return rc;
+}
+
+/* pass 2 of every shard with its lists on the device: the chunk buffers and stub index freed, to make room for
+ * each shard's S index; the exact checks look keys up in the S list of their owner (peer memory)            */
+static int stream_lists_pass2(hm_scan *s, StreamRun *RR, const uint64_t *ns, int *sbits, int sidx64)
+{ int G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
+  cudaError_t e;
   for (int g = 0; g < G; g++)
     if ((rc = stream_s_index(s,g,RR+g,ns[g],sidx64,G > 1,&sbits[g])) != HM_OK)
       return rc;
@@ -2341,6 +2730,60 @@ static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_sta
       __sync_fetch_and_add(&s->launches,3);
       if (rc != HM_OK) return rc;
     }
+  return HM_OK;
+}
+
+/* Pass 1 of every shard at once; the verdict over all shards' fingerprints; the Bloom segments all-gathered; the
+ * chunk buffers and stub index freed, to make room for each shard's S index; pass 2 of every shard, whose exact
+ * checks look keys up in the S list of their owner (peer memory); the plots summed on the host.              */
+static int run_stream_body(hm_scan *s, StreamRun *RR, int64_t *plot, hm_scan_stats *stats)
+{ int       G = s->ngpu, KW = s->kmer > 32 ? 2 : 1, rc = HM_OK;
+  double    t0 = now_ms();
+  double    ms_loop = 0;
+  cudaError_t e;
+  s->stop = 0;
+  if ((rc = on_every_gpu(s,shard_pass1,RR)) != HM_OK)
+    return rc;
+  for (int g = 0; g < G; g++)
+    if (RR[g].ms_loop > ms_loop) ms_loop = RR[g].ms_loop;
+  float  ms1 = slowest_ms(s,0,1);
+  double t_pass1 = now_ms();
+  if ((rc = fingerprint_verdict(s)) != HM_OK) return rc;
+  if (!s->symmetric)
+    return refuse_asymmetric(s);
+  int spilled = 0;
+  for (int g = 0; g < G; g++)
+    spilled |= RR[g].spilled;
+  for (int g = 0; g < G && spilled; g++)        /* one pass 2 for every shard: every shard's lists to host memory */
+    if (!RR[g].spilled)
+      { uint64_t nc = 0, status = 0, nsg = 0;
+        HM_CUDA(cudaSetDevice(s->d[g].dev));
+        if ((rc = hm_symm_stream_counts(RR[g].work,&RR[g].L,&nc,&status,&nsg,RR[g].sc)) != HM_OK ||
+            (rc = stream_flush(s,s->d+g,RR+g,nc,nsg)) != HM_OK)
+          return rc;
+      }
+
+  uint64_t ns[HM_MAX_GPUS];
+  int      sbits[HM_MAX_GPUS], sidx64 = 0;
+  for (int g = 0; g < G; g++)
+    { uint64_t nc = 0, status = 0;
+      HM_CUDA(cudaSetDevice(s->d[g].dev));
+      if ((rc = hm_symm_stream_counts(RR[g].work,&RR[g].L,&nc,&status,&ns[g],RR[g].sc)) != HM_OK) return rc;
+      if ((int64_t) ns[g] >= 0xFFFFFFF0ll) sidx64 = 1;    /* one offset width for every shard's index */
+    }
+  if (G > 1)                                    /* every shard pulls the other shards' Bloom segments */
+    { void *work[HM_MAX_GPUS]; cudaStream_t st[HM_MAX_GPUS];
+      for (int g = 0; g < G; g++)
+        { work[g] = RR[g].work; st[g] = RR[g].sc; }
+      if ((rc = gather_bloom(s,work,&RR[0].L,st,1)) != HM_OK)
+        return rc;
+    }
+  if (spilled)
+    { if ((rc = spill_pass2(s,RR)) != HM_OK)
+        return rc;
+    }
+  else if ((rc = stream_lists_pass2(s,RR,ns,sbits,sidx64)) != HM_OK)
+    return rc;
   int64_t *tmp = NULL;
   if (G > 1)
     { if ((tmp = (int64_t *) malloc(sizeof(int64_t)*HM_PLOT_CELLS)) == NULL)
@@ -2380,14 +2823,37 @@ static int run_stream(hm_scan *s, int64_t *plot, hm_scan_stats *stats)
     return hm_set_error(HM_EUNSUPPORTED,"the table does not fit in device memory and k = %d has no strand-symmetric "
                         "scan; the direct passes need it resident",s->kmer);
   memset(R,0,sizeof(R));
+  memset(&s->spill,0,sizeof(s->spill));
+  s->list_cap = g_list_host_budget;
+  s->host_held = 0;
   for (int g = 0; g < G; g++)
     { s->d[g].peak = s->d[g].held;
       s->d[g].chunks = 0;
+      R[g].spill = (s->list_cap > 0);
+      if (R[g].spill && getenv("HETMERS_LIST_ROOM") != NULL)    /* smaller device lists than the budget allows */
+        R[g].list_room = atoll(getenv("HETMERS_LIST_ROOM"));
     }
   int rc = run_stream_body(s,R,plot,stats);
+  hm_spill_stats *X = &s->spill;
+  for (int g = 0; g < G; g++)
+    { X->spilled |= R[g].spilled;
+      X->flushes += R[g].flushes; X->d2h_bytes += R[g].d2h_bytes;
+      X->rounds += R[g].rounds;   X->h2d_bytes += R[g].h2d_bytes;
+      X->first_key_queries += R[g].first_key_queries;
+      if (R[g].ms_loop > X->ms_pass1)  X->ms_pass1 = R[g].ms_loop;
+      if (R[g].ms_flush > X->ms_flush) X->ms_flush = R[g].ms_flush;
+      if (R[g].ms_pass2 > X->ms_pass2) X->ms_pass2 = R[g].ms_pass2;
+    }
   for (int g = 0; g < G; g++)                  /* every shard's thread has been joined: free it all */
     stream_release(s,g,R+g);
   return rc;
+}
+
+extern "C" int hm_scan_spill_stats(const hm_scan *s, hm_spill_stats *out)
+{ if (s == NULL || out == NULL)
+    return hm_set_error(HM_EINVAL,"hm_scan_spill_stats: bad arguments");
+  *out = s->spill;
+  return HM_OK;
 }
 
 /* examine_table's decisions on a streamed scan: the trim minimum over the same middle entries, chunk by

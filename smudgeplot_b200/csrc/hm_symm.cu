@@ -1497,9 +1497,11 @@ __device__ __noinline__ bool has_upper_partner(const uint64_t *__restrict__ keys
 enum Lookup
   { LK_TABLE,        /* in core: is there an upper partner of the key in its run of the table                     */
     LK_SLIST,        /* streamed: is the key in the sorted S list (several shards: the owner's, through W.sviews) */
-    LK_ROUTED        /* one rank of a one-process-per-GPU job: keys it owns in its own S list; a candidate left
+    LK_ROUTED,       /* one rank of a one-process-per-GPU job: keys it owns in its own S list; a candidate left
                       *   with a hit on a key owned elsewhere is parked (route_push) and settled once the owners
                       *   have answered                                                                         */
+    LK_PARK          /* streamed, S list in host memory: no look-up at all; every candidate with a hit is parked
+                      *   (route_push, no owner) and settled once the S partitions have answered its queries   */
   };
 
 /* Routed pass 2 (DESIGN.md §4c, *Ranks*): a parked candidate goes to the view's pending list -- its meta, and its
@@ -1547,6 +1549,10 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
   revcomp_kmer<KW>(x,xl,kmer,rx,rxl);
   ry = rx; ryl = rxl;
   set_base<KW>(ry,ryl,kmer-1-p,3-yb);                      /* rc y = rc x with the mirrored base swapped */
+  if (LK == LK_PARK)
+    { route_push<KW,false>(W,x,xl,meta,ha,0,rx,rxl,hb,0,ry,ryl);
+      return false;
+    }
   if (LK == LK_ROUTED)
     { const int  oa = (ha && W.n_seg > 1) ? owner_of(W,rx) : W.self, ob = (hb && W.n_seg > 1) ? owner_of(W,ry) : W.self;
       if ((ha && oa == W.self && bucket_find<IdxT,KW>(keys,keys_lo,bucket,bshift,rx,rxl) >= 0) ||
@@ -2228,6 +2234,14 @@ int hm_symm_stream_counts(const void *d_work, const hm_symm_layout *L, uint64_t 
   return HM_OK;
 }
 
+/* the candidate and S counts back to 0 once their entries have been copied out (status and Bloom filter stay) */
+int hm_symm_stream_reset_lists(void *d_work, const hm_symm_layout *L, void *stream)
+{ unsigned long long *h = (unsigned long long *) ((uint8_t *) d_work + L->off_header);
+  HM_CUDA(cudaMemsetAsync(h+SY_HDR_CAND,0,sizeof(uint64_t),(cudaStream_t) stream));
+  HM_CUDA(cudaMemsetAsync(h+SY_HDR_S,0,sizeof(uint64_t),(cudaStream_t) stream));
+  return HM_OK;
+}
+
 /* pass 2 of the streamed scan: the exact check of a Bloom hit is a look-up in the sorted S list (several shards:
  * the S list of the key's owner, reached through the view's d_views)                                          */
 int hm_symm_stream_resolve(const uint64_t *d_s_key, const uint64_t *d_s_lo, int64_t n_s,
@@ -2411,6 +2425,107 @@ int hm_symm_route_settle(int kmer, const hm_route_bufs *B, const uint8_t *d_ans,
     route_settle_kernel<<<route_grid(n_pend),256,0,st>>>(B->pend,n_pend,kmer,d_plot);
   HM_CUDA(cudaGetLastError());
   HM_CUDA(cudaStreamSynchronize(st));
+  return HM_OK;
+}
+
+/* ------------------------------------------------------------------ lists in host memory ---- */
+/* The streamed scan whose candidate records and S list went to host memory in pass 1 (hm_scan.cu, DESIGN.md §4c,
+ * *Lists in host memory*).  A round sweeps candidate slices with resolve_kernel<..., LK_PARK>: a Bloom miss is
+ * counted at once, a hit parked with a query per key that hit (q_tag = pending slot).  The round's queries are
+ * then sorted by key into B->send (KW words each) and B->send_slot, so that the queries falling in one S partition
+ * are one contiguous range; route_answer_kernel answers each range against its uploaded partition, and
+ * hm_symm_route_settle counts the parked candidates none of whose queries was found.                          */
+
+/* one slice of n candidates (R's cand_key / cand_lo / cand_meta) swept into the round's pending list and queries;
+ * reset: the slice opens a round (its pending and query counts start at 0)                                     */
+int hm_symm_park_resolve(int kmer, int64_t n, int reset, void *d_work, const hm_symm_layout *L,
+                         const hm_stream_lists *R, const hm_symm_shards *shards, const hm_route_bufs *B,
+                         unsigned long long *d_plot, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || d_plot == NULL || B == NULL || n < 0 || n > R->cand_cap ||
+      (kmer > 32) != (R->cand_lo != NULL))
+    return hm_set_error(HM_EINVAL,"symm_park_resolve: bad arguments");
+  cudaStream_t st = (cudaStream_t) stream;
+  hm_stream_lists S = *R;
+  S.cand_cap = n;
+  SymmView W = route_view(d_work,L,&S,shards,B,0,n);
+  if (reset)
+    HM_CUDA(cudaMemsetAsync(W.cand_n+SY_HDR_PEND,0,2*sizeof(uint64_t),st));
+  HM_CUDA(cudaMemsetAsync(W.cand_n,0xff,sizeof(uint64_t),st));      /* the sweep reads min(header, cand_cap) = n */
+  if (n == 0)
+    return HM_OK;
+  cudaError_t e = kmer > 32
+    ? launch_resolve<uint32_t,2,LK_PARK>(NULL,NULL,NULL,0,NULL,2,kmer,W,d_plot,8*n,st)
+    : launch_resolve<uint32_t,1,LK_PARK>(NULL,NULL,NULL,0,NULL,2,kmer,W,d_plot,8*n,st);
+  if (l2_persist())
+    bloom_window(st,NULL,0,0);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"resolve_kernel (parked)");
+  return HM_OK;
+}
+
+/* the round's parked candidates and queries so far, and the status word (synchronises) */
+int hm_symm_park_counts(const void *d_work, const hm_symm_layout *L, int64_t *n_pend, int64_t *n_q, uint64_t *status,
+                        void *stream)
+{ uint64_t h[SY_HDR_QUERY+1];
+  HM_CUDA(cudaMemcpyAsync(h,(const uint8_t *) d_work + L->off_header,sizeof(h),cudaMemcpyDeviceToHost,
+                          (cudaStream_t) stream));
+  HM_CUDA(cudaStreamSynchronize((cudaStream_t) stream));
+  *n_pend = (int64_t) h[SY_HDR_PEND]; *n_q = (int64_t) h[SY_HDR_QUERY]; *status = h[SY_HDR_STATUS];
+  return HM_OK;
+}
+
+__global__ void park_iota_kernel(uint32_t *__restrict__ v, int64_t n)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    v[i] = (uint32_t) i;
+}
+
+__global__ void park_gather_kernel(const uint64_t *__restrict__ src, const uint32_t *__restrict__ perm, int64_t n,
+                                   uint64_t *__restrict__ dst)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    dst[i] = src[perm[i]];
+}
+
+/* the queries in key order: KW words each into send, their pending slots into slot */
+template <int KW>
+__global__ void park_pack_kernel(const uint64_t *__restrict__ qk, const uint64_t *__restrict__ ql,
+                                 const uint64_t *__restrict__ tag, const uint32_t *__restrict__ perm, int64_t n,
+                                 uint64_t *__restrict__ send, uint32_t *__restrict__ slot)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    { const uint32_t j = perm[i];
+      send[KW*i] = qk[j];
+      if (KW == 2) send[KW*i+1] = ql[j];
+      slot[i] = (uint32_t) tag[j];
+    }
+}
+
+/* Sort the n_q queries of the round by key: a radix sort of key -> query index (k > 32: by the second word, then
+ * stably by the first), the queries gathered in that order into B->send and their slots into one of perm_a /
+ * perm_b, which B->send_slot is set to.  perm_a / perm_b: uint32[q_cap]; B->send holds 2 q_cap words at k > 32
+ * (the second half is scratch there).  tmp: hm_sort_perm_bytes(q_cap) bytes.                                 */
+int hm_symm_park_sort(int kmer, hm_route_bufs *B, int64_t n_q, uint32_t *perm_a, uint32_t *perm_b,
+                      void *tmp, int64_t tmp_bytes, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (n_q <= 0)
+    return HM_OK;
+  if (n_q > B->q_cap)
+    return hm_set_error(HM_EINVAL,"symm_park_sort: %lld queries for %lld slots",(long long) n_q,(long long) B->q_cap);
+  const int g = route_grid(n_q);
+  int rc;
+  park_iota_kernel<<<g,256,0,st>>>(perm_a,n_q);
+  if (kmer <= 32)
+    { if ((rc = hm_sort_perm(B->q_key,B->send,perm_a,perm_b,n_q,tmp,tmp_bytes,st)) != HM_OK) return rc;
+      park_pack_kernel<1><<<g,256,0,st>>>(B->q_key,NULL,B->q_tag,perm_b,n_q,B->send,perm_a);
+      B->send_slot = perm_a;
+    }
+  else
+    { uint64_t *hi = B->send + B->q_cap;
+      if ((rc = hm_sort_perm(B->q_lo,B->send,perm_a,perm_b,n_q,tmp,tmp_bytes,st)) != HM_OK) return rc;
+      park_gather_kernel<<<g,256,0,st>>>(B->q_key,perm_b,n_q,hi);
+      if ((rc = hm_sort_perm(hi,B->send,perm_b,perm_a,n_q,tmp,tmp_bytes,st)) != HM_OK) return rc;
+      park_pack_kernel<2><<<g,256,0,st>>>(B->q_key,B->q_lo,B->q_tag,perm_a,n_q,B->send,perm_b);
+      B->send_slot = perm_b;
+    }
+  HM_CUDA(cudaGetLastError());
   return HM_OK;
 }
 

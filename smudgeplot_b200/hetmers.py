@@ -193,10 +193,13 @@ class Scan:
     """Device-resident table + both passes (hm_scan_*).  A table whose in-core scan does not fit the device
     budget is streamed through the GPU on every run() instead (residency()); device_budget (bytes per GPU)
     sets that budget for this and later scans of the process (0: free device memory minus a reserve).
+    list_host_budget (bytes) lets a streamed run whose candidate records and S list outgrow the device budget keep
+    them in host memory instead of refusing (hm_set_list_host_budget: for this and later runs of the process; 0,
+    the default, is off); spill_stats() tells what the last run did.
     from_ktab(src, L) scans a raw FastK table as hetmers -e<L> does, conditioning it on the way in."""
 
     def __init__(self, kt: KtabFiles, gpus: int = 1, devices=None, device_budget: int | None = None, _owned=None,
-                 _stream=False):
+                 _stream=False, list_host_budget: int | None = None):
         L = _lib.lib()
         self._L = L
         self._h = None
@@ -205,6 +208,8 @@ class Scan:
         self.stats = {}
         if device_budget is not None:
             L.hm_set_device_budget(int(device_budget))
+        if list_host_budget is not None:
+            L.hm_set_list_host_budget(int(list_host_budget))
         if _owned:
             ht, self._keep = _owned.ptr.contents, None
         else:
@@ -222,7 +227,7 @@ class Scan:
 
     @classmethod
     def from_ktab(cls, src, L=None, gpus: int = 1, devices=None, device_budget: int | None = None,
-                  host_budget: int | None = None):
+                  host_budget: int | None = None, list_host_budget: int | None = None):
         """The scan of the FastK table `src` as hetmers -e<L> scans it, in one process on `gpus` GPUs (or the
         device ids `devices`), for a table of any size, without writing a conditioned copy.  L None, or a table
         hm_scan_examine(L) finds trimmed and symmetric, gives Scan over the source files.  Otherwise the table is
@@ -234,13 +239,14 @@ class Scan:
         scan, then frees the table unless arrays of self.kt (its records and index) are still held elsewhere, in
         which case they keep it alive.  device_budget: device bytes per GPU, as Scan's; host_budget: host bytes the
         conditioned table may take (None: no cap), checked against the output histogram's bound before the first
-        range pass (HetmersError -3 with both sizes).  stats["condition"] differs by route: always route ("none",
+        range pass (HetmersError -3 with both sizes).  list_host_budget: as Scan's (host bytes of a streamed run's
+        lists), independent of host_budget.  stats["condition"] differs by route: always route ("none",
         "in_place" or "host"), steps ("trim", "symmetrise") and host_bytes (the host table's records and index, 0
         but on the host route); "in_place" adds nels_in, nels_out and ms_total; "host" adds every
         hm_condition_stats field (ranges, passes, peak_bytes, budget_bytes, ...)."""
         import time
         lib = _lib.lib()
-        sc = cls(read_ktab(str(src), mmap=True), gpus, devices, device_budget)
+        sc = cls(read_ktab(str(src), mmap=True), gpus, devices, device_budget, list_host_budget=list_host_budget)
         st = {"route": "none", "steps": [], "host_bytes": 0}
         sc.stats = {"condition": st}
         try:
@@ -328,6 +334,13 @@ class Scan:
         b, c = C.c_int64(), C.c_int64()
         r = self._L.hm_scan_residency(self._h, C.byref(b), C.byref(c))
         return bool(r), b.value, c.value
+
+    def spill_stats(self):
+        """-> dict of hm_spill_stats for the last run: spilled, flushes, d2h_bytes, host_peak_bytes, partitions,
+        rounds, h2d_bytes, slice, part, ms_pass1, ms_flush, ms_pass2"""
+        st = _lib.SpillStats()
+        _lib.check(self._L.hm_scan_spill_stats(self._h, C.byref(st)))
+        return st.as_dict()
 
     def is_symmetric(self) -> bool:
         """whole-table verdict of the symmetry fingerprint (hm_scan_create / hm_scan_condition)"""

@@ -379,6 +379,9 @@ int main(int argc, char *argv[])
     { const char *b = getenv("HETMERS_DEVICE_BUDGET");     /* device bytes the scan may hold per GPU */
       if (b != NULL && *b != '\0')
         hm_set_device_budget(strtoll(b,NULL,10));
+      b = getenv("HETMERS_LIST_HOST_BUDGET");                /* host bytes a streamed run's lists may take */
+      if (b != NULL && *b != '\0')
+        hm_set_list_host_budget(strtoll(b,NULL,10));
     }
     if (hm_table_view(T)->nels < 2)
       { fprintf(stderr,"%s: k-mer table %s has fewer than 2 entries\n",Prog_Name,SRC);
@@ -531,6 +534,14 @@ int main(int argc, char *argv[])
             streamed ? "true" : "false",(long long) chunks,(long long) dev_bytes,
             t_open-t_start,t_load-t_open,t_exam-t_load,t_scan-t_exam,
             stats.ms_alloc,stats.ms_records,stats.ms_index);
+      hm_spill_stats SP;
+      if (hm_scan_spill_stats(S,&SP) == HM_OK && SP.spilled)
+        fprintf(stderr,", \"spill\": {\"flushes\": %lld, \"d2h_bytes\": %lld, \"host_peak_bytes\": %lld, "
+                       "\"partitions\": %lld, \"rounds\": %lld, \"h2d_bytes\": %lld, \"slice\": %lld, \"part\": %lld, "
+                       "\"ms_pass1\": %.3f, \"ms_flush\": %.3f, \"ms_pass2\": %.3f}",
+                (long long) SP.flushes,(long long) SP.d2h_bytes,(long long) SP.host_peak_bytes,(long long) SP.partitions,
+                (long long) SP.rounds,(long long) SP.h2d_bytes,(long long) SP.slice,(long long) SP.part,
+                SP.ms_pass1,SP.ms_flush,SP.ms_pass2);
 #ifdef EXTRACT_PAIRS
       fprintf(stderr,", \"pairs\": {\"writer\": \"%s\", \"wall_ms\": %.1f, \"records\": %lld, \"passes\": %lld, "
                    "\"windows\": %lld, \"room\": %lld, \"peak_bytes\": %lld, \"budget\": %lld, \"ms_hist\": %.3f, "
