@@ -422,8 +422,8 @@ int  hm_scan_residency(const hm_scan *s, int64_t *device_bytes, int64_t *chunks)
  * against the S list uploaded a partition at a time.  The device then holds the Bloom filter, one chunk and pass
  * 2's plan (hm_spill_plan); the lists' host bytes must stay within the budget (else HM_ENOMEM naming both sizes).
  * A run whose lists fit is unchanged.  With several shards in one process, one shard spilling makes every shard
- * spill.  The one-process-per-GPU ranks (hm_rank_scan_*) never spill.  HETMERS_LIST_HOST_BUDGET=<bytes> sets it
- * for the executables.                                                                                          */
+ * spill.  The one-process-per-GPU ranks (hm_rank_scan_*) are not affected by it: each has its own list host budget
+ * (hm_rank_scan_set_list_host_budget).  HETMERS_LIST_HOST_BUDGET=<bytes> sets it for the executables.          */
 void hm_set_list_host_budget(int64_t bytes);
 
 typedef struct hm_spill_stats               /* what the last run of a scan did with its lists                   */
@@ -483,7 +483,16 @@ int  hm_spill_plan(int64_t n_cand, int64_t n_s, int kmer, int64_t room, hm_spill
  *   all-to-all'ed as above -> answer -> the answers all-to-all'ed back -> extract_settle; then extract_result ->
  *   the ranks' records gathered on one rank and sorted there with hm_sort_pair_records.
  * Device pointers are returned; they stay valid until the next pass1, slices / extract_slices, extract_result
- * or destroy.                                                                                              */
+ * or destroy.
+ * Lists in host memory (DESIGN.md §4c, *Lists in host memory*): with set_list_host_budget(bytes > 0) before
+ * pass1, a rank whose lists cannot grow within its device budget flushes them to host memory in pass 1 (at most
+ * `bytes` there, else HM_ENOMEM naming both sizes).  The caller then agrees one mode for the job: after pass1,
+ * spill_stats().spilled on any rank -> host_lists() on every rank that did not spill -> prepare (no S index; its
+ * max_slice from hm_rank_spill_plan) -> the Bloom all-gather; the rounds go as above with two differences: each
+ * rank's queries include those it owns itself (counts[rank]), so recv holds world * 2 * slice keys and every
+ * rank's split, its own included, is exchanged; and answer sorts the keys received, answers them against the
+ * rank's S list uploaded a partition at a time, and returns the answers in receive order.  The host lists
+ * live until the next pass1 or destroy, so a listing after a scan reuses them.                           */
 typedef struct hm_rank_scan hm_rank_scan;
 int  hm_rank_scan_create(const hm_host_table *t, int device, int rank, int world, const uint64_t seed[2],
                          hm_rank_scan **out);
@@ -527,6 +536,26 @@ int  hm_rank_scan_extract_result(hm_rank_scan *r, hm_pair_rec **records, int64_t
 int  hm_rank_scan_extract_records(hm_rank_scan *r, hm_pair_rec **records, int64_t *n, uint64_t *status);
 /* sort n records in place into hm_scan_extract's order: (smudge, key, position, alternative base) */
 int  hm_sort_pair_records(hm_pair_rec *records, int64_t n);
+/* host bytes this rank's lists may take from the next pass1 on (0, the default: they stay on the device) */
+int  hm_rank_scan_set_list_host_budget(hm_rank_scan *r, int64_t bytes);
+/* after pass1, when some rank of the job spilled and this one did not: its lists to host memory as well */
+int  hm_rank_scan_host_lists(hm_rank_scan *r);
+/* this rank's hm_spill_stats: pass 1's flushes since the last pass1, pass 2's rounds, partitions and bytes since
+ * the last slices / extract_slices (ms_pass2: the time inside its route, answer and settle calls)          */
+int  hm_rank_scan_spill_stats(const hm_rank_scan *r, hm_spill_stats *out);
+/* The device plan of a rank's parked routed rounds, for n_cand candidates and an S list of n_s keys (the rank's)
+ * in `room` bytes, world ranks, listing or counting.  Per slot of a slice: the slice side -- its record (8 KW +
+ * 8), a pending slot (8), two queries (8 KW + 8 each), their send words and slots (8 KW + 4 each) and answers
+ * (1 each), and when listing its parked key words (8 KW) and two records (2 x 24) -- and the receive side: world
+ * x 2 keys, each received, sorted (8 KW apiece), with two sort permutations (8), its answer before and after the
+ * scatter back (2) and its sort scratch (HM_SPILL_SORT_Q, plus HM_SPILL_SORT_FIXED once); HM_RANK_SPILL_FIXED
+ * for the counters and allocation rounding.  Per partition key 8 KW plus its uint32 bucket index.  Split as
+ * hm_spill_plan splits (slice and receive sides together); a slice holds at most HM_SPILL_MAX_SLICE / world
+ * candidates (the world x 2 x slice keys received are sorted with 32-bit indices).  HM_ENOMEM, with the sizes,
+ * when the room holds less than min(n, HM_SPILL_MIN) of either.  out->slice_bytes counts both sides.         */
+#define HM_RANK_SPILL_FIXED (16ll*HM_MAX_SHARDS + 32*256)
+int  hm_rank_spill_plan(int64_t n_cand, int64_t n_s, int kmer, int world, int listing, int64_t room,
+                        hm_spill_layout *out);
 
 /* ---- extract_kmer_pairs' pair files across the ranks of a one-process-per-GPU job (csrc/hm_pairs.cu, DESIGN.md
  * §6b; dist.ShardedScan / StreamedShardedScan.write_pairs).  The caller runs the collectives between the calls:

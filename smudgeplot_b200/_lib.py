@@ -44,6 +44,7 @@ ABI_SYMBOLS = [
     "hm_pairs_sort_scratch_bytes", "hm_k_pairs_sort", "hm_k_pairs_label_bounds", "hm_k_pairs_format", "hm_pairs_bytes",
     "hm_scan_write_pairs", "hm_scan_pairs_hist", "hm_pair_windows",
     "hm_set_list_host_budget", "hm_scan_spill_stats", "hm_spill_plan",
+    "hm_rank_scan_set_list_host_budget", "hm_rank_scan_host_lists", "hm_rank_scan_spill_stats", "hm_rank_spill_plan",
 ]
 
 
@@ -241,6 +242,10 @@ def lib():
     L.hm_set_list_host_budget.restype = None
     L.hm_scan_spill_stats.argtypes = [vp, C.POINTER(SpillStats)]
     L.hm_spill_plan.argtypes = [i64, i64, i32, i64, C.POINTER(SpillLayout)]
+    L.hm_rank_scan_set_list_host_budget.argtypes = [vp, i64]
+    L.hm_rank_scan_host_lists.argtypes = [vp]
+    L.hm_rank_scan_spill_stats.argtypes = [vp, C.POINTER(SpillStats)]
+    L.hm_rank_spill_plan.argtypes = [i64, i64, i32, i32, i32, i64, C.POINTER(SpillLayout)]
     u64p, i64p = C.POINTER(C.c_uint64), C.POINTER(i64)
     L.hm_rank_scan_create.argtypes = [C.POINTER(HostTable), i32, i32, i32, u64p, C.POINTER(vp)]
     L.hm_rank_scan_create_share.argtypes = [C.POINTER(HostTable), i64, i64p, u64p, i32, i32, i32, u64p, C.POINTER(vp)]

@@ -139,6 +139,16 @@ int hm_symm_park_counts(const void *d_work, const hm_symm_layout *L, int64_t *n_
                         void *stream);
 int hm_symm_park_sort(int kmer, hm_route_bufs *B, int64_t n_q, uint32_t *perm_a, uint32_t *perm_b,
                       void *tmp, int64_t tmp_bytes, void *stream);
+/* a rank's lists in host memory (hm_rank_scan_*): hm_symm_park_resolve or hm_symm_park_extract sweep a slice (the
+ * queries tagged with their owners, this rank included); the keys the rank receives sorted by key
+ * (hm_symm_recv_sort: *perm = each sorted key's receive index), answered per S partition with
+ * hm_symm_route_answer, and the answers put back in receive order (hm_symm_recv_unsort)                    */
+int hm_symm_park_extract(int kmer, int64_t n, void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                         const hm_symm_shards *shards, const hm_route_bufs *B, const uint16_t *d_pixmap,
+                         hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count, void *stream);
+int hm_symm_recv_sort(int kmer, const uint64_t *recv, int64_t n, uint64_t *sorted, uint32_t *perm_a, uint32_t *perm_b,
+                      void *tmp, int64_t tmp_bytes, uint32_t **perm, void *stream);
+int hm_symm_recv_unsort(const uint8_t *d_ans_sorted, const uint32_t *d_perm, int64_t n, uint8_t *d_ans, void *stream);
 /* conditioning, a key range at a time (hm_condition.cu; driven by hm_scan_condition and hm_scan_condition_files
  * in hm_scan.cu and by hm_k_shard_settle): the device buffers of one range of at most `cap` output entries.
  * key / lo / cnt: the region the kept originals fill from the front and the reverse complements from the back;

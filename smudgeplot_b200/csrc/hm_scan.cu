@@ -95,6 +95,7 @@ struct hm_scan
     hm_spill_stats spill;                 /* (streamed) what the last run did with its lists (hm_scan_spill_stats) */
     int64_t  list_cap;                    /* (streamed) the run's list host budget (0: the lists stay on the device) */
     int64_t  host_held;                   /* (streamed) host bytes the lists of every shard hold                     */
+    const char *list_knob;                /* (streamed) what sets list_cap, for messages (NULL: the environment's)  */
   };
 
 static double now_ms(void)
@@ -620,6 +621,57 @@ extern "C" int hm_spill_plan(int64_t n_cand, int64_t n_s, int kmer, int64_t room
   out->slice = slice; out->queries = 2*slice;
   out->part = part; out->part_bits = hm_pick_bucket_bits(part);
   out->slice_bytes = spill_slice_bytes(slice,KW); out->part_bytes = spill_part_bytes(part,KW);
+  return HM_OK;
+}
+
+/* a rank's parked routed rounds (hm_rank_spill_plan): device bytes of the slice and receive sides of a slice of c
+ * candidates, for `world` ranks, counting or listing                                                          */
+static int64_t rank_spill_slice_bytes(int64_t c, int KW, int world, int listing)
+{ int64_t send = c*(8*KW+8) + 8*c + 2*c*(8*KW+8) + 2*c*(8*KW+4) + 2*c;
+  int64_t keep = listing ? c*8*KW + 2*c*(int64_t) sizeof(hm_pair_rec) : 0;
+  int64_t recv = (int64_t) world*2*c*(2*8*KW + 8 + 2 + HM_SPILL_SORT_Q) + HM_SPILL_SORT_FIXED;
+  return send + keep + recv + HM_RANK_SPILL_FIXED;
+}
+
+/* the largest c <= most whose slice side fits room, 0 if none */
+static int64_t rank_spill_largest(int64_t most, int64_t room, int KW, int world, int listing)
+{ int64_t lo = 0, hi = most;
+  while (lo < hi)
+    { int64_t mid = lo + (hi-lo+1)/2;
+      if (rank_spill_slice_bytes(mid,KW,world,listing) <= room) lo = mid; else hi = mid-1;
+    }
+  return lo;
+}
+
+extern "C" int hm_rank_spill_plan(int64_t n_cand, int64_t n_s, int kmer, int world, int listing, int64_t room,
+                                  hm_spill_layout *out)
+{ if (n_cand < 0 || n_s < 0 || kmer < 1 || kmer > HM_MAX_KMER || world < 1 || world > HM_MAX_SHARDS || out == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_spill_plan: bad arguments");
+  int     KW = kmer > 32 ? 2 : 1, L = listing != 0;
+  int64_t nc = n_cand > 1 ? n_cand : 1, np = n_s > 1 ? n_s : 1, slice, part;
+  if (nc > HM_SPILL_MAX_SLICE/world) nc = HM_SPILL_MAX_SLICE/world;    /* received keys are sorted with 32-bit indices */
+  if (np > HM_SPILL_MAX_PART)        np = HM_SPILL_MAX_PART;           /* a partition's bucket index is 32-bit      */
+  if (rank_spill_slice_bytes(nc,KW,world,L) + spill_part_bytes(np,KW) <= room)
+    { slice = nc; part = np; }
+  else
+    { slice = rank_spill_largest(nc,room/2,KW,world,L);
+      part  = spill_largest(np,room-rank_spill_slice_bytes(slice,KW,world,L),KW,spill_part_bytes);
+      slice = rank_spill_largest(nc,room-spill_part_bytes(part,KW),KW,world,L);
+    }
+  int64_t min_c = nc < HM_SPILL_MIN ? nc : HM_SPILL_MIN, min_p = np < HM_SPILL_MIN ? np : HM_SPILL_MIN;
+  if (slice < min_c || part < min_p)
+    return hm_set_error(HM_ENOMEM,"pass 2 of a rank's lists in host memory has %lld bytes of device room, and %s slices "
+                        "of %lld candidates with what %d ranks send for them (%lld bytes) beside partitions of %lld S "
+                        "keys (%lld bytes) need %lld; give the rank a larger device budget",(long long) room,
+                        L ? "listing" : "counting",(long long) min_c,world,
+                        (long long) rank_spill_slice_bytes(min_c,KW,world,L),(long long) min_p,
+                        (long long) spill_part_bytes(min_p,KW),
+                        (long long) (rank_spill_slice_bytes(min_c,KW,world,L) + spill_part_bytes(min_p,KW)));
+  memset(out,0,sizeof(*out));
+  out->room = room;
+  out->slice = slice; out->queries = 2*slice;
+  out->part = part; out->part_bits = hm_pick_bucket_bits(part);
+  out->slice_bytes = rank_spill_slice_bytes(slice,KW,world,L); out->part_bytes = spill_part_bytes(part,KW);
   return HM_OK;
 }
 
@@ -2296,8 +2348,9 @@ static int stream_flush(hm_scan *s, DevTable *D, StreamRun *R, uint64_t nc, uint
   int64_t held = __sync_add_and_fetch(&s->host_held,bytes), pk;
   if (held > s->list_cap)
     return hm_set_error(HM_ENOMEM,"the streamed scan's lists need %lld bytes of host memory (%lld of them in this flush) "
-                        "but the list host budget is %lld bytes; give the scan a larger one (HETMERS_LIST_HOST_BUDGET)",
-                        (long long) held,(long long) bytes,(long long) s->list_cap);
+                        "but the list host budget is %lld bytes; give the scan a larger one (%s)",
+                        (long long) held,(long long) bytes,(long long) s->list_cap,
+                        s->list_knob ? s->list_knob : "HETMERS_LIST_HOST_BUDGET");
   while ((pk = s->spill.host_peak_bytes) < held && !__sync_bool_compare_and_swap(&s->spill.host_peak_bytes,pk,held))
     ;
   uint64_t *h = NULL;
@@ -2506,6 +2559,56 @@ static int64_t query_lower_bound(const uint64_t *q, int KW, int64_t lo, int64_t 
   return lo;
 }
 
+/* the S partitions of the host S list hs (blocks in key order), cut into pieces of at most `part` keys:
+ * spill_part_count how many, spill_cut_parts appends them at parts + *n                                   */
+static int64_t spill_part_count(const HostList *hs, int64_t part)
+{ int64_t np = 0;
+  for (int b = 0; b < hs->nb; b++)
+    np += (hs->b[b].n + part-1)/part;
+  return np;
+}
+
+static void spill_cut_parts(const HostList *hs, int64_t part, int KW, SpillPart *parts, int64_t *n)
+{ for (int b = 0; b < hs->nb; b++)
+    { const HostBlock *hb = hs->b+b;
+      for (int64_t o = 0; o < hb->n; o += part)
+        { SpillPart *P = parts + (*n)++;
+          P->key = hb->w+o; P->lo = KW == 2 ? hb->w+hb->n+o : NULL;
+          P->n = hb->n-o < part ? hb->n-o : part;
+        }
+    }
+}
+
+/* n sorted keys (hq on the host, d_q on the device, KW words each) answered against the partitions in key order:
+ * the keys falling in partition p are the contiguous range between the lower bounds of its first key and the
+ * next partition's; a partition no key falls in is not uploaded, the others are uploaded into pkey / plo,
+ * indexed into pbucket (`bits`) and answer their range into ans (zeroed by the caller)                       */
+static int spill_answer_parts(hm_scan *s, StreamRun *R, const SpillPart *parts, int64_t nparts, int bits,
+                              const uint64_t *hq, const uint64_t *d_q, int64_t n, uint64_t *pkey, uint64_t *plo,
+                              void *pbucket, uint8_t *ans)
+{ const int KW = s->kmer > 32 ? 2 : 1;
+  int       rc = HM_OK;
+  int64_t   lo = 0;
+  for (int64_t p = 0; p < nparts && lo < n && rc == HM_OK; p++)
+    { const SpillPart *P = parts+p;
+      int64_t hi = n;
+      if (p+1 < nparts)
+        hi = query_lower_bound(hq,KW,lo,n,P[1].key[0],KW == 2 ? P[1].lo[0] : 0);
+      if (hi == lo)
+        continue;                               /* no key falls in this partition: nothing uploaded */
+      R->first_key_queries += (hq[KW*lo] == P->key[0] && (KW == 1 || hq[KW*lo+1] == P->lo[0]));
+      rc = stage_copy(R,pkey,P->key,8*P->n,0);
+      if (rc == HM_OK && KW == 2) rc = stage_copy(R,plo,P->lo,8*P->n,0);
+      if (rc == HM_OK) rc = hm_k_build_bucket_index(pkey,P->n,bits,pbucket,0,R->sc);
+      if (rc == HM_OK)
+        rc = hm_symm_route_answer(pkey,plo,pbucket,bits,0,s->kmer,d_q+KW*lo,hi-lo,ans+lo,R->sc);
+      R->h2d_bytes += 8*KW*P->n;
+      __sync_fetch_and_add(&s->launches,2);
+      lo = hi;
+    }
+  return rc;
+}
+
 /* the device buffers of one shard's pass 2 over host lists */
 typedef struct
   { hm_stream_lists L;                            /* cand_key / cand_meta / cand_lo: one slice */
@@ -2542,24 +2645,7 @@ static int spill_settle(hm_scan *s, int g, const SpillRun *S, StreamRun *R, Spil
       HM_CUDA(cudaMemsetAsync(X->ans,0,(size_t) n_q,R->sc));
       HM_CUDA(cudaStreamSynchronize(R->sc));
     }
-  int64_t lo = 0;
-  for (int64_t p = 0; p < S->nparts && lo < n_q && rc == HM_OK; p++)
-    { const SpillPart *P = S->parts+p;
-      int64_t hi = n_q;
-      if (p+1 < S->nparts)
-        hi = query_lower_bound(X->hq,KW,lo,n_q,P[1].key[0],KW == 2 ? P[1].lo[0] : 0);
-      if (hi == lo)
-        continue;                               /* no query falls in this partition: nothing uploaded */
-      R->first_key_queries += (X->hq[KW*lo] == P->key[0] && (KW == 1 || X->hq[KW*lo+1] == P->lo[0]));
-      rc = stage_copy(R,X->pkey,P->key,8*P->n,0);
-      if (rc == HM_OK && KW == 2) rc = stage_copy(R,X->plo,P->lo,8*P->n,0);
-      if (rc == HM_OK) rc = hm_k_build_bucket_index(X->pkey,P->n,bits,X->pbucket,0,R->sc);
-      if (rc == HM_OK)
-        rc = hm_symm_route_answer(X->pkey,X->plo,X->pbucket,bits,0,s->kmer,X->B.send+KW*lo,hi-lo,X->ans+lo,R->sc);
-      R->h2d_bytes += 8*KW*P->n;
-      __sync_fetch_and_add(&s->launches,2);
-      lo = hi;
-    }
+  rc = spill_answer_parts(s,R,S->parts,S->nparts,bits,X->hq,X->B.send,n_q,X->pkey,X->plo,X->pbucket,X->ans);
   if (rc == HM_OK)
     rc = hm_symm_route_settle(s->kmer,&X->B,X->ans,n_q,n_pend,D->plot,R->sc);
   __sync_fetch_and_add(&s->launches,2);
@@ -2672,19 +2758,11 @@ static int spill_pass2(hm_scan *s, StreamRun *RR)
     }
   int64_t np = 0;
   for (int g = 0; g < G; g++)
-    for (int b = 0; b < RR[g].hs.nb; b++)
-      np += (RR[g].hs.b[b].n + S.P.part-1)/S.P.part;
+    np += spill_part_count(&RR[g].hs,S.P.part);
   if ((S.parts = (SpillPart *) malloc(sizeof(SpillPart)*(size_t) (np > 0 ? np : 1))) == NULL)
     return hm_set_error(HM_ENOMEM,"out of host memory");
   for (int g = 0; g < G; g++)                                  /* shards in key order, blocks in key order */
-    for (int b = 0; b < RR[g].hs.nb; b++)
-      { const HostBlock *hb = RR[g].hs.b+b;
-        for (int64_t o = 0; o < hb->n; o += S.P.part)
-          { SpillPart *P = S.parts + S.nparts++;
-            P->key = hb->w+o; P->lo = KW == 2 ? hb->w+hb->n+o : NULL;
-            P->n = hb->n-o < S.P.part ? hb->n-o : S.P.part;
-          }
-      }
+    spill_cut_parts(&RR[g].hs,S.P.part,KW,S.parts,&S.nparts);
   rc = on_every_gpu(s,shard_spill_pass2,&S);
   free(S.parts);
   s->spill.partitions = S.nparts;
@@ -3841,6 +3919,20 @@ struct hm_rank_scan
     hm_pair_rec  *rec;
     hm_pair_rec  *host;                      /* the records of the rounds so far                              */
     int64_t       host_n, host_cap;
+    int64_t       list_cap;                  /* host bytes the lists may take (0: they stay on the device)   */
+    int           lists_host;                /* the lists are in host memory (R.hc, R.hs): parked routed rounds */
+    int           part_bits;
+    int64_t       room, part, nparts;        /* pass 2's device room; S keys per partition, partitions       */
+    hm_stream_lists X;                       /* (lists in host memory) one uploaded candidate slice           */
+    uint64_t     *sorted;                    /* the keys received, sorted (2 words apiece at k > 32)          */
+    uint32_t     *perm[2];
+    uint8_t      *ans_sorted;
+    void         *tmp;
+    int64_t       tmp_bytes;
+    uint64_t     *pkey, *plo;                /* one S partition and its bucket index                          */
+    void         *pbucket;
+    uint64_t     *hq;                        /* (host) the sorted keys received                               */
+    SpillPart    *parts;
   };
 
 static void rank_free_route(hm_rank_scan *r)
@@ -3852,6 +3944,14 @@ static void rank_free_route(hm_rank_scan *r)
   dev_free(D,r->recv); dev_free(D,r->ans_recv); dev_free(D,r->ans_sent);
   memset(&r->B,0,sizeof(r->B));
   r->recv = NULL; r->ans_recv = NULL; r->ans_sent = NULL; r->rec = NULL;
+  if (r->R.sc) cudaStreamSynchronize(r->R.sc);           /* (lists in host memory) */
+  dev_free(D,r->X.cand_key); dev_free(D,r->X.cand_meta); dev_free(D,r->X.cand_lo);
+  dev_free(D,r->sorted); dev_free(D,r->perm[0]); dev_free(D,r->perm[1]); dev_free(D,r->ans_sorted); dev_free(D,r->tmp);
+  dev_free(D,r->pkey); dev_free(D,r->plo); dev_free(D,r->pbucket);
+  free(r->hq); free(r->parts);
+  memset(&r->X,0,sizeof(r->X));
+  r->sorted = NULL; r->perm[0] = r->perm[1] = NULL; r->ans_sorted = NULL; r->tmp = NULL; r->tmp_bytes = 0;
+  r->pkey = r->plo = NULL; r->pbucket = NULL; r->hq = NULL; r->parts = NULL;   /* (nparts stays, for the stats) */
 }
 
 static void rank_free_listing(hm_rank_scan *r)
@@ -3910,6 +4010,7 @@ static int rank_scan_open(const hm_host_table *t, int64_t n, int device, int ran
   s->kmer = t->kmer; s->ibyte = t->ibyte; s->n = n; s->ngpu = 1; s->nshard = world; s->rank = rank;
   s->bits = hm_pick_bucket_bits(s->n); s->fpos = hm_pick_filter_bits(s->n); s->idx64 = (s->n >= 0xFFFFFFF0ll);
   s->seed[0] = seed[0]; s->seed[1] = seed[1];               /* the same on every rank: the sums are added */
+  s->list_knob = "the list_host_budget argument";
   s->budget = device_budget(&device,1);
   s->incore_bytes = incore_bytes(s->n,t->kmer,1,s->bits,s->idx64);
   int rc = stream_setup(s,t);
@@ -3989,8 +4090,13 @@ extern "C" int hm_rank_scan_pass1(hm_rank_scan *r, uint64_t *fp)
   rank_free_route(r);
   rank_free_listing(r);
   stream_release(s,0,&r->R);
-  r->stage = 0; r->status = 0;
+  r->stage = 0; r->status = 0; r->nparts = 0; r->part = 0;
   D->peak = D->held; D->chunks = 0; s->stop = 0;
+  memset(&s->spill,0,sizeof(s->spill));
+  s->list_cap = r->list_cap; s->host_held = 0; r->lists_host = 0;
+  r->R.spill = (r->list_cap > 0);
+  if (r->R.spill && getenv("HETMERS_LIST_ROOM") != NULL)       /* smaller device lists than the budget allows */
+    r->R.list_room = atoll(getenv("HETMERS_LIST_ROOM"));
   int rc = shard_pass1(s,0,&r->R);
   if (rc != HM_OK)
     return rc;
@@ -3999,7 +4105,58 @@ extern "C" int hm_rank_scan_pass1(hm_rank_scan *r, uint64_t *fp)
     return rc;
   HM_CUDA(cudaMemcpy(fp,D->fp_acc,4*sizeof(uint64_t),cudaMemcpyDeviceToHost));
   r->ncand = (int64_t) nc;
+  if (r->R.spilled)                              /* shard_pass1 flushed what was left */
+    { r->lists_host = 1;
+      r->ncand = host_list_entries(&r->R.hc); r->ns = (uint64_t) host_list_entries(&r->R.hs);
+    }
   r->stage = 1;
+  return HM_OK;
+}
+
+extern "C" int hm_rank_scan_set_list_host_budget(hm_rank_scan *r, int64_t bytes)
+{ if (r == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_set_list_host_budget: bad arguments");
+  r->list_cap = bytes > 0 ? bytes : 0;
+  return HM_OK;
+}
+
+/* another rank spilled: this rank's lists (all of them on the device) go to host memory too */
+extern "C" int hm_rank_scan_host_lists(hm_rank_scan *r)
+{ if (r == NULL || r->stage != 1)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_host_lists: pass 1 first");
+  if (r->lists_host)
+    return HM_OK;
+  hm_scan  *s = r->s;
+  uint64_t nc = 0, status = 0, ns = 0;
+  int rc;
+  HM_CUDA(cudaSetDevice(s->d[0].dev));
+  if ((rc = hm_symm_stream_counts(r->R.work,&r->R.L,&nc,&status,&ns,r->R.sc)) != HM_OK ||
+      (rc = stream_flush(s,s->d,&r->R,nc,ns)) != HM_OK)
+    return rc;
+  r->lists_host = 1;
+  r->ncand = host_list_entries(&r->R.hc); r->ns = (uint64_t) host_list_entries(&r->R.hs);
+  return HM_OK;
+}
+
+/* lists in host memory: the chunk buffers and stub index freed (no S index: S is not resident), the room that
+ * leaves (HETMERS_SPILL_ROOM: less) and the largest slice the plan gives in it                              */
+static int rank_host_prepare(hm_rank_scan *r, int listing, int64_t fixed, int64_t *max_slice)
+{ hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  hm_spill_layout P;
+  HM_CUDA(cudaSetDevice(D->dev));
+  stream_free_chunks(D,&r->R);
+  dev_free(D,r->R.d_index); r->R.d_index = NULL;
+  HM_CUDA(cudaStreamSynchronize(r->R.sc));
+  int64_t room = s->budget - D->held - fixed;
+  const char *e = getenv("HETMERS_SPILL_ROOM");              /* smaller slices and partitions than the room allows */
+  if (e != NULL && atoll(e) > 0 && atoll(e) < room)
+    room = atoll(e);
+  int rc = hm_rank_spill_plan(r->ncand,(int64_t) r->ns,s->kmer,s->nshard,listing,room,&P);
+  if (rc != HM_OK)
+    return rc;
+  r->room = room;
+  *max_slice = P.slice;
   return HM_OK;
 }
 
@@ -4033,6 +4190,13 @@ extern "C" int hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_c
   if (!symmetric)
     return refuse_asymmetric(s);
   int rc;
+  if (r->lists_host)
+    { if ((rc = rank_host_prepare(r,0,0,max_slice)) != HM_OK)
+        return rc;
+      *n_cand = r->ncand;
+      r->stage = 2;
+      return HM_OK;
+    }
   r->sidx64 = ((int64_t) r->ns >= 0xFFFFFFF0ll);
   if ((rc = stream_s_index(s,0,&r->R,r->ns,r->sidx64,1,&r->sbits)) != HM_OK)
     return rc;
@@ -4054,9 +4218,14 @@ extern "C" int hm_rank_scan_prepare(hm_rank_scan *r, int symmetric, int64_t *n_c
  * send (uint64, KW words per query, grouped by owner), recv (the same for what arrives), ans_recv (a byte per
  * key that arrived) and ans_sent (a byte per query sent, in send order).                                    */
 /* the route buffers of slices of `slice` candidates (listing: with the parked keys and the records) */
+static int rank_alloc_host(hm_rank_scan *r, int64_t slice, int listing, int64_t *rounds, void **d_send, void **d_recv,
+                           void **d_ans_recv, void **d_ans_sent);
+
 static int rank_alloc_route(hm_rank_scan *r, int64_t slice, int listing, int64_t *rounds, void **d_send, void **d_recv,
                             void **d_ans_recv, void **d_ans_sent)
-{ hm_scan  *s = r->s;
+{ if (r->lists_host)
+    return rank_alloc_host(r,slice,listing,rounds,d_send,d_recv,d_ans_recv,d_ans_sent);
+  hm_scan  *s = r->s;
   DevTable *D = s->d;
   int64_t   KW = s->kmer > 32 ? 2 : 1, q = 2*slice, o = s->nshard-1;
   int64_t   need = listing ? listing_bytes(slice,s->kmer,s->nshard) : route_bytes(slice,s->kmer,s->nshard);
@@ -4096,6 +4265,168 @@ static int rank_alloc_route(hm_rank_scan *r, int64_t slice, int listing, int64_t
   return HM_OK;
 }
 
+/* ---- a rank's lists in host memory (DESIGN.md §4c, *Lists in host memory*): the parked routed rounds ---- */
+
+/* the slice of `slice` candidates, its queries and their exchange, what world ranks send for them, and one S
+ * partition in the room prepare found (hm_rank_spill_plan); *rounds = the slices this rank's candidates take.
+ * recv holds world x 2 x slice keys: every rank's queries, this rank's own among them.                       */
+static int rank_alloc_host(hm_rank_scan *r, int64_t slice, int listing, int64_t *rounds, void **d_send, void **d_recv,
+                           void **d_ans_recv, void **d_ans_sent)
+{ hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  const int KW = s->kmer > 32 ? 2 : 1, W = s->nshard;
+  int64_t   q = 2*slice, qr = (int64_t) W*q, room = r->room;
+  int       rc = HM_OK;
+  cudaError_t e;
+  rank_free_route(r);
+  int64_t need = rank_spill_slice_bytes(slice,KW,W,listing);
+  int64_t np = (int64_t) r->ns > 1 ? (int64_t) r->ns : 1;
+  if (np > HM_SPILL_MAX_PART) np = HM_SPILL_MAX_PART;
+  int64_t part = spill_largest(np,room-need,KW,spill_part_bytes);
+  const char *env = getenv("HETMERS_SPILL_PART");                   /* smaller partitions */
+  if (env != NULL && atoll(env) > 0 && atoll(env) < part)
+    part = atoll(env);
+  if (part < 1 || (part < (np < HM_SPILL_MIN ? np : HM_SPILL_MIN) && (env == NULL || atoll(env) <= 0)))
+    return hm_set_error(HM_ENOMEM,"pass 2 of a rank's lists in host memory: slices of %lld candidates need %lld device "
+                        "bytes of the %lld in the room, which leaves too little for S partitions",(long long) slice,
+                        (long long) need,(long long) room);
+  TRY(cudaSetDevice(D->dev));
+  TRY(dev_alloc(D,&r->X.cand_key,8*slice));
+  TRY(dev_alloc(D,&r->X.cand_meta,8*slice));
+  if (KW == 2) TRY(dev_alloc(D,&r->X.cand_lo,8*slice));
+  TRY(dev_alloc(D,&r->B.pend,8*slice));
+  TRY(dev_alloc(D,&r->B.q_key,8*q));
+  if (KW == 2) TRY(dev_alloc(D,&r->B.q_lo,8*q));
+  TRY(dev_alloc(D,&r->B.q_tag,8*q));
+  TRY(dev_alloc(D,&r->B.send,8*KW*q));
+  TRY(dev_alloc(D,&r->B.send_slot,4*q));
+  TRY(dev_alloc(D,&r->B.counts,16*HM_MAX_SHARDS));
+  TRY(dev_alloc(D,&r->ans_sent,q));
+  if (listing)
+    { TRY(dev_alloc(D,&r->B.pend_key,8*slice));
+      if (KW == 2) TRY(dev_alloc(D,&r->B.pend_lo,8*slice));
+      TRY(dev_alloc(D,&r->rec,2*slice*(int64_t) sizeof(hm_pair_rec)));
+    }
+  r->tmp_bytes = hm_sort_perm_bytes(qr);
+  TRY(dev_alloc(D,&r->recv,8*KW*qr));
+  TRY(dev_alloc(D,&r->sorted,8*KW*qr));
+  TRY(dev_alloc(D,&r->perm[0],4*qr));
+  TRY(dev_alloc(D,&r->perm[1],4*qr));
+  TRY(dev_alloc(D,&r->ans_recv,qr));
+  TRY(dev_alloc(D,&r->ans_sorted,qr));
+  TRY(dev_alloc(D,&r->tmp,r->tmp_bytes));
+  TRY(dev_alloc(D,&r->pkey,8*part));
+  if (KW == 2) TRY(dev_alloc(D,&r->plo,8*part));
+  r->part_bits = hm_pick_bucket_bits(part);
+  TRY(dev_alloc(D,&r->pbucket,4*((1ll << r->part_bits)+1)));
+  if (rc == HM_OK && D->held > s->budget)
+    rc = hm_set_error(HM_ENOMEM,"pass 2 of a rank's lists in host memory holds %lld device bytes, more than the budget "
+                      "of %lld (the plan counted %lld)",(long long) D->held,(long long) s->budget,
+                      (long long) (need + spill_part_bytes(part,KW)));
+  int64_t nparts = spill_part_count(&r->R.hs,part);
+  if (rc == HM_OK && ((r->hq = (uint64_t *) malloc(8*(size_t) KW*(size_t) qr)) == NULL ||
+                      (r->parts = (SpillPart *) malloc(sizeof(SpillPart)*(size_t) (nparts > 0 ? nparts : 1))) == NULL))
+    rc = hm_set_error(HM_ENOMEM,"out of host memory");
+  if (rc != HM_OK)
+    { rank_free_route(r); return rc; }
+  r->nparts = 0;
+  spill_cut_parts(&r->R.hs,part,KW,r->parts,&r->nparts);
+  r->X.cand_cap = slice;
+  r->B.pend_cap = slice; r->B.q_cap = q;
+  r->slice = slice; r->part = part;
+  r->rounds = (r->ncand + slice-1)/slice;
+  r->R.rounds = r->R.h2d_bytes = r->R.first_key_queries = 0;
+  r->R.ms_pass2 = 0;
+  *rounds = r->rounds;
+  if (d_send)     *d_send = r->B.send;
+  if (d_recv)     *d_recv = r->recv;
+  if (d_ans_recv) *d_ans_recv = r->ans_recv;
+  if (d_ans_sent) *d_ans_sent = r->ans_sent;
+  return HM_OK;
+}
+
+/* the candidates [c0, c1) of the host list uploaded into the slice buffers (they may span blocks) */
+static int rank_host_upload(hm_rank_scan *r, int64_t c0, int64_t c1)
+{ const int KW = r->s->kmer > 32 ? 2 : 1;
+  int64_t   at = 0, base = 0;
+  int       rc = HM_OK;
+  for (int b = 0; b < r->R.hc.nb && at < c1-c0 && rc == HM_OK; b++)
+    { const HostBlock *hb = r->R.hc.b+b;
+      int64_t lo = c0+at-base;                                   /* where the slice goes on in this block */
+      if (lo < hb->n)
+        { int64_t m = hb->n-lo < c1-c0-at ? hb->n-lo : c1-c0-at;
+          rc = stage_copy(&r->R,r->X.cand_key+at,hb->w+lo,8*m,0);
+          if (rc == HM_OK) rc = stage_copy(&r->R,r->X.cand_meta+at,hb->w+hb->n+lo,8*m,0);
+          if (rc == HM_OK && KW == 2) rc = stage_copy(&r->R,r->X.cand_lo+at,hb->w+2*hb->n+lo,8*m,0);
+          at += m;
+        }
+      base += hb->n;
+    }
+  r->R.h2d_bytes += (c1-c0)*(8*KW+8);
+  return rc;
+}
+
+/* a round of the parked routed pass: the slice [c0, c1) uploaded and swept (listing: extract_kernel), every Bloom
+ * hit parked with a query per key that hit, tagged with the key's owner; the queries grouped by owner         */
+static int rank_host_route(hm_rank_scan *r, int64_t c0, int64_t c1, int listing, int64_t *counts)
+{ hm_scan  *s = r->s;
+  DevTable *D = s->d;
+  uint64_t  status = 0;
+  double    t0 = now_ms();
+  int       rc = rank_host_upload(r,c0,c1);
+  const hm_symm_shards *sh = s->nshard > 1 ? s->ssh : NULL;
+  if (rc == HM_OK)
+    rc = listing
+      ? hm_symm_park_extract(s->kmer,c1-c0,r->R.work,&r->R.L,&r->X,sh,&r->B,r->pix,r->rec,2*r->slice,r->rec_n,r->R.sc)
+      : hm_symm_park_resolve(s->kmer,c1-c0,1,r->R.work,&r->R.L,&r->X,sh,&r->B,D->plot,r->R.sc);
+  __sync_fetch_and_add(&s->launches,(int64_t) (c1 > c0));
+  if (rc == HM_OK)
+    rc = hm_symm_route_group(s->kmer,s->nshard,r->R.work,&r->R.L,&r->B,counts,&r->n_sent,&r->n_pend,&status,r->R.sc);
+  r->status |= status;
+  r->R.rounds += 1;
+  r->R.ms_pass2 += now_ms()-t0;
+  return rc;
+}
+
+/* the n keys received (every rank's queries to this one, its own among them): sorted by key, answered against the
+ * rank's S list a partition at a time -- only the partitions some key falls in are uploaded and indexed -- and
+ * the answers put back in receive order into ans_recv (synchronises)                                        */
+static int rank_host_answer(hm_rank_scan *r, int64_t n)
+{ hm_scan   *s = r->s;
+  const int  KW = s->kmer > 32 ? 2 : 1;
+  double     t0 = now_ms();
+  uint32_t  *perm = NULL;
+  int        rc = hm_symm_recv_sort(s->kmer,r->recv,n,r->sorted,r->perm[0],r->perm[1],r->tmp,r->tmp_bytes,&perm,r->R.sc);
+  if (rc != HM_OK)
+    return rc;
+  if (n > 0)
+    { HM_CUDA(cudaMemcpyAsync(r->hq,r->sorted,8*(size_t) KW*(size_t) n,cudaMemcpyDeviceToHost,r->R.sc));
+      HM_CUDA(cudaMemsetAsync(r->ans_sorted,0,(size_t) n,r->R.sc));
+      HM_CUDA(cudaStreamSynchronize(r->R.sc));
+    }
+  rc = spill_answer_parts(s,&r->R,r->parts,r->nparts,r->part_bits,r->hq,r->sorted,n,r->pkey,r->plo,r->pbucket,
+                          r->ans_sorted);
+  if (rc == HM_OK)
+    rc = hm_symm_recv_unsort(r->ans_sorted,perm,n,r->ans_recv,r->R.sc);
+  r->R.ms_pass2 += now_ms()-t0;
+  return rc;
+}
+
+extern "C" int hm_rank_scan_spill_stats(const hm_rank_scan *r, hm_spill_stats *out)
+{ if (r == NULL || out == NULL)
+    return hm_set_error(HM_EINVAL,"hm_rank_scan_spill_stats: bad arguments");
+  const StreamRun *R = &r->R;
+  memset(out,0,sizeof(*out));
+  out->spilled = r->lists_host;
+  out->flushes = R->flushes; out->d2h_bytes = R->d2h_bytes;
+  out->host_peak_bytes = r->s->spill.host_peak_bytes;
+  out->partitions = r->nparts; out->rounds = R->rounds; out->h2d_bytes = R->h2d_bytes;
+  out->slice = r->lists_host ? r->slice : 0; out->part = r->part;
+  out->first_key_queries = R->first_key_queries;
+  out->ms_pass1 = R->ms_loop; out->ms_flush = R->ms_flush; out->ms_pass2 = R->ms_pass2;
+  return HM_OK;
+}
+
 extern "C" int hm_rank_scan_slices(hm_rank_scan *r, int64_t slice, int64_t *rounds, void **d_send, void **d_recv,
                                    void **d_ans_recv, void **d_ans_sent)
 { if (r == NULL || r->stage != 2 || slice < 1 || rounds == NULL)
@@ -4126,6 +4457,8 @@ extern "C" int hm_rank_scan_route(hm_rank_scan *r, int64_t round, int64_t *count
   HM_CUDA(cudaSetDevice(D->dev));
   if (round == 0)
     HM_CUDA(cudaEventRecord(D->ev[2],r->R.sc));
+  if (r->lists_host)
+    return rank_host_route(r,c0,c1,0,counts);
   if ((rc = hm_symm_route_resolve(r->R.R.s_key,KW == 2 ? r->R.R.s_lo : NULL,(int64_t) r->ns,r->R.s_bucket,r->sbits,
                                   r->sidx64,s->kmer,c0,c1,r->R.work,&r->R.L,&r->R.R,s->nshard > 1 ? s->ssh : NULL,&r->B,
                                   D->plot,r->R.sc)) != HM_OK)
@@ -4141,9 +4474,12 @@ extern "C" int hm_rank_scan_route(hm_rank_scan *r, int64_t round, int64_t *count
 /* the n keys that arrived in recv: one byte each into ans_recv (synchronises) */
 extern "C" int hm_rank_scan_answer(hm_rank_scan *r, int64_t n)
 { hm_scan *s = r ? r->s : NULL;
-  if (r == NULL || (r->stage != 3 && r->stage != 5) || n < 0 || n > (s->nshard-1)*2*r->slice)
+  if (r == NULL || (r->stage != 3 && r->stage != 5) || n < 0 ||
+      n > (s->nshard-1 + (r != NULL && r->lists_host))*2*r->slice)
     return hm_set_error(HM_EINVAL,"hm_rank_scan_answer: bad arguments");
   HM_CUDA(cudaSetDevice(s->d[0].dev));
+  if (r->lists_host)
+    return rank_host_answer(r,n);
   return hm_symm_route_answer(r->R.R.s_key,s->kmer > 32 ? r->R.R.s_lo : NULL,r->R.s_bucket,r->sbits,r->sidx64,s->kmer,
                               r->recv,n,r->ans_recv,r->R.sc);
 }
@@ -4154,8 +4490,10 @@ extern "C" int hm_rank_scan_settle(hm_rank_scan *r)
     return hm_set_error(HM_EINVAL,"hm_rank_scan_settle: bad arguments");
   hm_scan *s = r->s;
   HM_CUDA(cudaSetDevice(s->d[0].dev));
+  double t0 = now_ms();
   int rc = hm_symm_route_settle(s->kmer,&r->B,r->ans_sent,r->n_sent,r->n_pend,s->d[0].plot,r->R.sc);
   __sync_fetch_and_add(&s->launches,2);
+  if (r->lists_host) r->R.ms_pass2 += now_ms()-t0;
   return rc;
 }
 
@@ -4200,8 +4538,12 @@ extern "C" int hm_rank_scan_extract_prepare(hm_rank_scan *r, const uint16_t *pix
   cudaError_t e;
   rank_free_route(r);
   rank_free_listing(r);
-  int64_t room = s->budget - D->held - LISTING_FIXED_BYTES, lo = largest_slice(room,s->kmer,s->nshard,listing_bytes);
-  if (lo < ROUTE_MIN_SLICE)
+  int64_t room = s->budget - D->held - LISTING_FIXED_BYTES, lo = 0;
+  if (r->lists_host)
+    { if ((rc = rank_host_prepare(r,1,LISTING_FIXED_BYTES,&lo)) != HM_OK)
+        return rc;
+    }
+  else if ((lo = largest_slice(room,s->kmer,s->nshard,listing_bytes)) < ROUTE_MIN_SLICE)
     return hm_set_error(HM_ENOMEM,"a device budget of %lld bytes leaves %lld bytes beside the resident lists of this rank "
                         "(%lld held) and the pixmap (%lld), and listing k-mer pairs in slices of %d candidates needs %lld",
                         (long long) s->budget,(long long) (room > 0 ? room : 0),(long long) D->held,
@@ -4242,6 +4584,8 @@ extern "C" int hm_rank_scan_extract_route(hm_rank_scan *r, int64_t round, int64_
   uint64_t  status = 0;
   rank_round(r,round,&c0,&c1);
   HM_CUDA(cudaSetDevice(D->dev));
+  if (r->lists_host)
+    return rank_host_route(r,c0,c1,1,counts);
   if ((rc = hm_symm_route_extract(r->R.R.s_key,KW == 2 ? r->R.R.s_lo : NULL,(int64_t) r->ns,r->R.s_bucket,r->sbits,
                                   r->sidx64,s->kmer,c0,c1,r->R.work,&r->R.L,&r->R.R,s->nshard > 1 ? s->ssh : NULL,&r->B,
                                   r->pix,r->rec,2*r->slice,r->rec_n,r->R.sc)) != HM_OK)
@@ -4262,8 +4606,10 @@ extern "C" int hm_rank_scan_extract_settle(hm_rank_scan *r)
   hm_scan *s = r->s;
   unsigned long long c = 0;
   HM_CUDA(cudaSetDevice(s->d[0].dev));
+  double t0 = now_ms();
   int rc = hm_symm_route_list(s->kmer,&r->B,r->ans_sent,r->n_sent,r->n_pend,r->pix,r->rec,2*r->slice,r->rec_n,r->R.sc);
   __sync_fetch_and_add(&s->launches,2);
+  if (r->lists_host) r->R.ms_pass2 += now_ms()-t0;
   if (rc != HM_OK)
     return rc;
   HM_CUDA(cudaMemcpy(&c,r->rec_n,sizeof(c),cudaMemcpyDeviceToHost));

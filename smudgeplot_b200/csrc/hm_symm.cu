@@ -1501,7 +1501,9 @@ enum Lookup
                       *   with a hit on a key owned elsewhere is parked (route_push) and settled once the owners
                       *   have answered                                                                         */
     LK_PARK          /* streamed, S list in host memory: no look-up at all; every candidate with a hit is parked
-                      *   (route_push, no owner) and settled once the S partitions have answered its queries   */
+                      *   (route_push; each query tagged with its key's owner when the view has several shards,
+                      *   which the one-process rounds ignore and a rank's routes by) and settled once the S
+                      *   partitions have answered its queries                                                 */
   };
 
 /* Routed pass 2 (DESIGN.md §4c, *Ranks*): a parked candidate goes to the view's pending list -- its meta, and its
@@ -1550,7 +1552,8 @@ __device__ __forceinline__ bool isolated_after_all(const uint64_t *__restrict__ 
   ry = rx; ryl = rxl;
   set_base<KW>(ry,ryl,kmer-1-p,3-yb);                      /* rc y = rc x with the mirrored base swapped */
   if (LK == LK_PARK)
-    { route_push<KW,false>(W,x,xl,meta,ha,0,rx,rxl,hb,0,ry,ryl);
+    { const int oa = (ha && W.n_seg > 1) ? owner_of(W,rx) : W.self, ob = (hb && W.n_seg > 1) ? owner_of(W,ry) : W.self;
+      route_push<KW,Sink::NEEDS_KEY>(W,x,xl,meta,ha,oa,rx,rxl,hb,ob,ry,ryl);
       return false;
     }
   if (LK == LK_ROUTED)
@@ -2526,6 +2529,102 @@ int hm_symm_park_sort(int kmer, hm_route_bufs *B, int64_t n_q, uint32_t *perm_a,
       B->send_slot = perm_b;
     }
   HM_CUDA(cudaGetLastError());
+  return HM_OK;
+}
+
+/* ------------------------------------------------------------------ parked routed rounds ---- */
+/* One rank of a one-process-per-GPU job whose lists went to host memory (hm_scan.cu hm_rank_scan_*, DESIGN.md §4c,
+ * *Lists in host memory*, *Ranks*).  A round sweeps one uploaded slice with resolve_kernel or extract_kernel
+ * <..., LK_PARK>: every Bloom hit is parked, each hit key a query tagged owner << 32 | pending slot, the owner
+ * possibly this rank; route_group sends them.  The owner sorts the keys it receives (hm_symm_recv_sort), answers
+ * them against its S list a partition at a time (route_answer_kernel over each contiguous range) and puts the
+ * answers back in receive order (hm_symm_recv_unsort), so that they return in the order they were sent.      */
+
+/* the listing's sweep of one slice of n candidates: misses with a labelled pixel listed at once, hits parked with
+ * their key words (a new round: the pending and query counts, and the record counter, start at 0)             */
+int hm_symm_park_extract(int kmer, int64_t n, void *d_work, const hm_symm_layout *L, const hm_stream_lists *R,
+                         const hm_symm_shards *shards, const hm_route_bufs *B, const uint16_t *d_pixmap,
+                         hm_pair_rec *d_out, int64_t cap, unsigned long long *d_count, void *stream)
+{ if (kmer < HM_SYMM_MIN_KMER || kmer > HM_MAX_KMER || B == NULL || n < 0 || n > R->cand_cap || d_pixmap == NULL ||
+      d_count == NULL || d_out == NULL || cap < 2*n || (kmer > 32) != (R->cand_lo != NULL) || B->pend_key == NULL ||
+      (kmer > 32 && B->pend_lo == NULL))
+    return hm_set_error(HM_EINVAL,"symm_park_extract: bad arguments");
+  cudaStream_t st = (cudaStream_t) stream;
+  hm_stream_lists S = *R;
+  S.cand_cap = n;
+  SymmView W = route_view(d_work,L,&S,shards,B,0,n);
+  HM_CUDA(cudaMemsetAsync(W.cand_n+SY_HDR_PEND,0,2*sizeof(uint64_t),st));
+  HM_CUDA(cudaMemsetAsync(W.cand_n,0xff,sizeof(uint64_t),st));      /* the sweep reads min(header, cand_cap) = n */
+  HM_CUDA(cudaMemsetAsync(d_count,0,sizeof(unsigned long long),st));
+  if (n == 0)
+    return HM_OK;
+  cudaError_t e = kmer > 32
+    ? launch_extract<uint32_t,2,LK_PARK>(NULL,NULL,NULL,0,NULL,2,kmer,W,d_pixmap,d_out,cap,d_count,st)
+    : launch_extract<uint32_t,1,LK_PARK>(NULL,NULL,NULL,0,NULL,2,kmer,W,d_pixmap,d_out,cap,d_count,st);
+  if (e != cudaSuccess)
+    return hm_cuda_fail(e,"extract_kernel (parked)");
+  return HM_OK;
+}
+
+/* word `w` of each received key (kw words apiece), in the order perm gives (NULL: as received) */
+__global__ void recv_word_kernel(const uint64_t *__restrict__ recv, int kw, int w, const uint32_t *__restrict__ perm,
+                                 int64_t n, uint64_t *__restrict__ dst)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    dst[i] = recv[(int64_t) kw*(perm != NULL ? (int64_t) perm[i] : i) + w];
+}
+
+/* the received keys in key order: both words of key perm[i] to sorted[2i], sorted[2i+1] */
+__global__ void recv_pack_kernel(const uint64_t *__restrict__ recv, const uint32_t *__restrict__ perm, int64_t n,
+                                 uint64_t *__restrict__ sorted)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    { const int64_t j = perm[i];
+      sorted[2*i] = recv[2*j]; sorted[2*i+1] = recv[2*j+1];
+    }
+}
+
+/* Sort the n keys received (KW words each, in recv) by key into sorted (KW words each; 2n words at k > 32, also the
+ * scratch there): a radix sort of key -> receive index (k > 32: by the second word, then stably by the first).
+ * *perm: perm_a or perm_b, whichever holds each sorted key's receive index.  perm_a / perm_b: uint32[n];
+ * tmp: hm_sort_perm_bytes(n) bytes.                                                                         */
+int hm_symm_recv_sort(int kmer, const uint64_t *recv, int64_t n, uint64_t *sorted, uint32_t *perm_a, uint32_t *perm_b,
+                      void *tmp, int64_t tmp_bytes, uint32_t **perm, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  *perm = perm_a;
+  if (n <= 0)
+    return HM_OK;
+  const int g = route_grid(n);
+  int rc;
+  park_iota_kernel<<<g,256,0,st>>>(perm_a,n);
+  if (kmer <= 32)
+    { if ((rc = hm_sort_perm(recv,sorted,perm_a,perm_b,n,tmp,tmp_bytes,st)) != HM_OK) return rc;
+      *perm = perm_b;
+    }
+  else
+    { uint64_t *a = sorted, *b = sorted + n;
+      recv_word_kernel<<<g,256,0,st>>>(recv,2,1,NULL,n,a);
+      if ((rc = hm_sort_perm(a,b,perm_a,perm_b,n,tmp,tmp_bytes,st)) != HM_OK) return rc;
+      recv_word_kernel<<<g,256,0,st>>>(recv,2,0,perm_b,n,a);
+      if ((rc = hm_sort_perm(a,b,perm_b,perm_a,n,tmp,tmp_bytes,st)) != HM_OK) return rc;
+      recv_pack_kernel<<<g,256,0,st>>>(recv,perm_a,n,sorted);
+      *perm = perm_a;
+    }
+  HM_CUDA(cudaGetLastError());
+  return HM_OK;
+}
+
+__global__ void recv_unsort_kernel(const uint8_t *__restrict__ ans_sorted, const uint32_t *__restrict__ perm, int64_t n,
+                                   uint8_t *__restrict__ ans)
+{ for (int64_t i = (int64_t) blockIdx.x*blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x*blockDim.x)
+    ans[perm[i]] = ans_sorted[i];
+}
+
+/* the answers to the sorted keys back in receive order: ans[perm[i]] = ans_sorted[i] (synchronises) */
+int hm_symm_recv_unsort(const uint8_t *d_ans_sorted, const uint32_t *d_perm, int64_t n, uint8_t *d_ans, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (n > 0)
+    recv_unsort_kernel<<<route_grid(n),256,0,st>>>(d_ans_sorted,d_perm,n,d_ans);
+  HM_CUDA(cudaGetLastError());
+  HM_CUDA(cudaStreamSynchronize(st));
   return HM_OK;
 }
 

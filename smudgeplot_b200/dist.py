@@ -1233,6 +1233,46 @@ def rank_pass_counts(h_local, h_all, subs, rank: int):
     return out
 
 
+def raise_on_any_rank(err, what: str, coll, group=None):
+    """One flag all-reduce where a rank may have failed (a rank's lists in host memory: StreamedShardedScan with a
+    list_host_budget).  err: this rank's HetmersError, or None -> returns if no rank failed; else raises on every
+    rank: this rank's own error, or a HetmersError with the failing rank's code naming the ranks that failed, so
+    that no rank is left waiting in the next collective."""
+    from . import _lib
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    codes = _reduce([int(err.code) if err is not None and d == rank else 0 for d in range(world)], coll, group)
+    bad = [d for d, c in enumerate(codes) if c]
+    if not bad:
+        return
+    if err is not None:
+        raise err
+    raise _lib.HetmersError(codes[bad[0]], f"rank {rank}: {what} failed on rank{'s' if len(bad) > 1 else ''} "
+                                           f"{', '.join(map(str, bad))} (codes {[codes[d] for d in bad]})")
+
+
+def pass1_agreement(fp, spilled: bool, err, coll, group=None):
+    """The job-wide verdicts after pass 1 of ranks that may keep their lists in host memory, in one all-gather:
+    fp = this rank's four fingerprint sums (uint64), spilled = its lists went to host memory, err = its
+    HetmersError or None.  -> (symmetric, spilled on any rank); a rank's failure raises on every rank, as
+    raise_on_any_rank does."""
+    from . import _lib
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    mine = torch.tensor([_signed(int(v)) for v in fp] + [int(bool(spilled) and err is None),
+                                                        int(err.code) if err is not None else 0],
+                        dtype=torch.int64, device=coll)
+    parts = [torch.zeros_like(mine) for _ in range(world)]
+    dist.all_gather(parts, mine, group=group)
+    rows = [p.tolist() for p in parts]
+    bad = [d for d, r in enumerate(rows) if r[5]]
+    if bad:
+        if err is not None:
+            raise err
+        raise _lib.HetmersError(rows[bad[0]][5], f"rank {rank}: pass 1 failed on rank{'s' if len(bad) > 1 else ''} "
+                                                 f"{', '.join(map(str, bad))} (codes {[rows[d][5] for d in bad]})")
+    tot = [sum(r[i] for r in rows) & _U64 for i in range(4)]
+    return tot[0] == tot[2] and tot[1] == tot[3], any(r[4] for r in rows)
+
+
 def _reduce(vals, coll, group, op=dist.ReduceOp.SUM):
     """all_reduce of a list of integers -> the reduced list"""
     x = torch.tensor(vals, dtype=torch.int64, device=coll)
@@ -1983,9 +2023,16 @@ class StreamedShardedScan:
     settles a Bloom hit on a key another rank owns by asking that rank: the keys go to their owners with
     all_to_all_single, one byte per key comes back (hm_rank_scan_*, DESIGN.md §4c).
     scan() -> the plot (int64[SMAX+1, FMAX+1] on every rank), equal to the in-core scan's; extract(pixmap, dst) ->
-    extract_kmer_pairs' records on rank dst, equal to the in-core list."""
+    extract_kmer_pairs' records on rank dst, equal to the in-core list.
+    list_host_budget (bytes, per rank; None or 0, the default: off) lets a rank whose candidate records and S list
+    outgrow its device budget keep them in host memory instead of refusing (DESIGN.md §4c, *Lists in host
+    memory*): if any rank's lists go there, every rank's do, and pass 2 runs parked routed rounds, each rank
+    answering the queries on the keys it owns against its S list uploaded a partition at a time.  Give it on
+    every rank or on none; each rank's lists must stay within its own value (else HetmersError -3 on every rank,
+    naming both sizes).  stats["spill"]: this rank's hm_spill_stats (as hetmers.Scan.spill_stats())."""
 
-    def __init__(self, table, group=None, device=None, budget: int | None = None, _share=None):
+    def __init__(self, table, group=None, device=None, budget: int | None = None,
+                 list_host_budget: int | None = None, _share=None):
         import ctypes as C
         from . import _lib, fastk
         from .hetmers import _host_table
@@ -2018,16 +2065,24 @@ class StreamedShardedScan:
                                                        (C.c_uint64 * self.world)(*first), self.device.index,
                                                        self.rank, self.world, sd, C.byref(h)))
         self._h = h
+        self._host_lists = bool(list_host_budget) and int(list_host_budget) > 0
+        if self._host_lists:
+            _lib.check(L.hm_rank_scan_set_list_host_budget(h, int(list_host_budget)))
         cuts = (C.c_int64 * (self.world + 1))()
         _lib.check(L.hm_rank_scan_cuts(h, cuts, None))
         self.cuts = [int(c) for c in cuts]
-        mine = torch.tensor(self.cuts, dtype=torch.int64, device=self._coll_dev)
+        mine = torch.tensor(self.cuts + [int(self._host_lists)], dtype=torch.int64, device=self._coll_dev)
         every = [torch.empty_like(mine) for _ in range(self.world)]
         dist.all_gather(every, mine, group=group)
-        if any(not torch.equal(e, mine) for e in every):
+        if any(not torch.equal(e[:-1], mine[:-1]) for e in every):
             self.close()
             raise RuntimeError(f"rank {self.rank}: the ranks computed different shard cuts from the table files "
-                               f"({[e.tolist() for e in every]})")
+                               f"({[e[:-1].tolist() for e in every]})")
+        if any(int(e[-1]) != self._host_lists for e in every):
+            self.close()
+            raise ValueError(f"rank {self.rank}: list_host_budget must be given on every rank or on none (given on "
+                             f"ranks {[d for d, e in enumerate(every) if int(e[-1])]})")
+        self._lists_host = False                                # (list_host_budget) the job's lists in host memory
         self.share = None                                       # (from_ktab) this rank's conditioned share
         self.status = 0
         self._base_stats = {}                                   # what every stats dict starts with (from_ktab)
@@ -2035,7 +2090,7 @@ class StreamedShardedScan:
         self._pass1_done = False                                # candidates, S list and Bloom filter resident
 
     @classmethod
-    def from_ktab(cls, src, group=None, device=None, L=None, budget=None, host_budget=None):
+    def from_ktab(cls, src, group=None, device=None, L=None, budget=None, host_budget=None, list_host_budget=None):
         """The streamed scan of the FastK table `src` as hetmers -e<L> scans it; every rank calls this.  With L the
         table is trimmed and / or symmetrised on the way in, as hm_scan_examine(L) decides on the whole table
         (job_examine), without writing a conditioned copy: each rank conditions one range of key prefixes, cut on
@@ -2044,7 +2099,8 @@ class StreamedShardedScan:
         (self.share: its stub index counts only them) and streams that share on every scan.  A table that needs
         neither step, and L None, give StreamedShardedScan(src): the source files are streamed, no host copy held.
         budget: device bytes per rank, for the conditioning and the scan (default: free memory minus
-        _lib.BUDGET_RESERVE); host_budget: host bytes per rank (default: no cap).  HM_ENOMEM on every rank, with the
+        _lib.BUDGET_RESERVE); host_budget: host bytes per rank (default: no cap); list_host_budget: as the
+        constructor's (host bytes of this rank's lists in the scans, independent of host_budget).  HM_ENOMEM on every rank, with the
         sizes and before the first pass, when a rank's share of the source and one pass do not fit its budget, when
         a rank's conditioned share (records and stub index) exceeds its host_budget, or when a rank cannot allocate
         it.  stats["condition"]: condition_ktab's stats (verdicts, steps, entries in / out, passes, prefix cuts and
@@ -2055,7 +2111,7 @@ class StreamedShardedScan:
         import numpy as np
         from . import _lib, fastk
         if L is None:
-            out = cls(src, group, device, budget)
+            out = cls(src, group, device, budget, list_host_budget)
             out._base_stats = {"condition": {"steps": [], "host_bytes": 0}}
             out.stats = dict(out._base_stats)
             return out
@@ -2079,7 +2135,7 @@ class StreamedShardedScan:
                 job.close()
                 torch.cuda.empty_cache()                        # the scan allocates outside torch's cache
                 st.update(entries_out=n, host_bytes=0, peak_bytes=torch.cuda.max_memory_allocated(dev) - base, ms=ms)
-                out = cls(src, group, device, budget)
+                out = cls(src, group, device, budget, list_host_budget)
                 out._base_stats = {"condition": st}
                 out.stats = dict(out._base_stats)
                 return out
@@ -2146,7 +2202,7 @@ class StreamedShardedScan:
                       peak_bytes=torch.cuda.max_memory_allocated(dev) - base, ms=ms)
             share = fastk.KtabFiles(kmer=k, nparts=1, minval=max(minval, int(L)) if job.do_trim else minval,
                                     ibyte=ibyte, index=index, part_nels=[m_out], records=[buf])
-        out = cls(share, group, device, budget, _share=(cuts[-1], cuts, first_keys))
+        out = cls(share, group, device, budget, list_host_budget, _share=(cuts[-1], cuts, first_keys))
         out.share = share
         out._base_stats = {"condition": st}
         out.stats = dict(out._base_stats)
@@ -2167,6 +2223,8 @@ class StreamedShardedScan:
         import ctypes as C
         from . import _lib
         L, h, g, W = self.L, self._h, self.group, self.world
+        if self._host_lists:
+            return self._pass1_host(lap)
         self._pass1_done = False
         t = time.perf_counter()
         fp = (C.c_uint64 * 4)()
@@ -2188,6 +2246,53 @@ class StreamedShardedScan:
         self._pass1_done = True
         return nc.value, ms.value
 
+    def _pass1_host(self, lap):
+        """_pass1 of ranks with a list host budget: one mode for the job -- if any rank's lists went to host memory
+        in pass 1, every rank's go there (hm_rank_scan_host_lists) and prepare builds no S index -- with a failure
+        on any rank (its lists over its list_host_budget, a plan refusal) raised on every rank"""
+        import ctypes as C
+        from . import _lib
+        L, h, g, W = self.L, self._h, self.group, self.world
+        self._pass1_done = self._lists_host = False
+        t = time.perf_counter()
+        fp = (C.c_uint64 * 4)()
+        err = None
+        try:
+            _lib.check(L.hm_rank_scan_pass1(h, fp))
+        except _lib.HetmersError as e:
+            err = e
+        spilled = err is None and self.spill_stats()["spilled"]
+        t = lap("pass1", t)
+        symmetric, self._lists_host = pass1_agreement(list(fp), spilled, None if err is None else err,
+                                                      self._coll_dev, g)
+        nc, ms = C.c_int64(), C.c_int64()
+        err = None
+        try:
+            if self._lists_host:
+                _lib.check(L.hm_rank_scan_host_lists(h))
+            _lib.check(L.hm_rank_scan_prepare(h, int(symmetric), C.byref(nc), C.byref(ms)))
+        except _lib.HetmersError as e:
+            err = e
+        raise_on_any_rank(err, "preparing pass 2", self._coll_dev, g)
+        t = lap("verdict_and_s_index", t)
+        seg, segb = C.c_void_p(), C.c_int64()
+        _lib.check(L.hm_rank_scan_bloom(h, C.byref(seg), C.byref(segb)))
+        if W > 1:
+            view = self._view(seg.value, W * segb.value).view(W, segb.value)
+            _in_place(lambda x: exchange_segments(x, self.rank, g), view, g)
+            self._sync()
+        lap("bloom_allgather", t)
+        self._pass1_done = True
+        return nc.value, ms.value
+
+    def spill_stats(self) -> dict:
+        """this rank's hm_spill_stats (hm_rank_scan_spill_stats), as hetmers.Scan.spill_stats() gives them"""
+        import ctypes as C
+        from . import _lib
+        st = _lib.SpillStats()
+        _lib.check(self.L.hm_rank_scan_spill_stats(self._h, C.byref(st)))
+        return st.as_dict()
+
     def _rounds(self, n_cand, max_slice, slices_fn, route_fn, settle_fn, lap):
         """the slice every rank can hold, its buffers (slices_fn), then every round up to the most any rank needs:
         route_fn(round, counts) -> the query keys all-to-all'ed to their owners -> answer -> the answer bytes
@@ -2202,14 +2307,24 @@ class StreamedShardedScan:
         slice_ = max(1, min(int(lim[0]), -int(lim[1])))        # the smallest room, no more than the most candidates
         rounds = C.c_int64()
         ptr = [C.c_void_p() for _ in range(4)]
-        _lib.check(slices_fn(h, slice_, C.byref(rounds), *[C.byref(p) for p in ptr]))
+        if self._host_lists:
+            err = None
+            try:
+                _lib.check(slices_fn(h, slice_, C.byref(rounds), *[C.byref(p) for p in ptr]))
+            except _lib.HetmersError as e:
+                err = e
+            raise_on_any_rank(err, "sizing pass 2's buffers", self._coll_dev, g)
+        else:
+            _lib.check(slices_fn(h, slice_, C.byref(rounds), *[C.byref(p) for p in ptr]))
         rt = torch.tensor([rounds.value], dtype=torch.int64, device=self._coll_dev)
         dist.all_reduce(rt, op=dist.ReduceOp.MAX, group=g)
         n_rounds = int(rt.item())
         q = 2 * slice_
+        # lists in host memory: every rank's queries go to their owners, this rank's own included
+        senders = W if self._lists_host else W - 1
         send = self._view(ptr[0].value, 8 * kw * q).view(torch.int64)
-        recv = self._view(ptr[1].value, 8 * kw * q * (W - 1)).view(torch.int64)
-        ans_recv = self._view(ptr[2].value, q * (W - 1))
+        recv = self._view(ptr[1].value, 8 * kw * q * senders).view(torch.int64)
+        ans_recv = self._view(ptr[2].value, q * senders)
         ans_sent = self._view(ptr[3].value, q)
         t = lap("slices", t)
         counts = (C.c_int64 * W)()
@@ -2217,7 +2332,18 @@ class StreamedShardedScan:
         for rd in range(n_rounds):
             _lib.check(route_fn(h, rd, counts))
             t = lap("resolve", t)
-            if W > 1:
+            if W == 1 and self._lists_host:                     # the one rank answers itself
+                ns = nr = int(counts[0])
+                sent_to[0] += ns
+                recv[:kw * nr].copy_(send[:kw * ns])
+                self._sync()
+                t = lap("exchange_queries", t)
+                _lib.check(L.hm_rank_scan_answer(h, nr))
+                t = lap("answer", t)
+                ans_sent[:ns].copy_(ans_recv[:nr])
+                self._sync()
+                t = lap("exchange_answers", t)
+            elif W > 1:
                 out_c = [int(c) for c in counts]
                 sc = torch.tensor(out_c, dtype=torch.int64, device=self._coll_dev)
                 rc = torch.empty_like(sc)
@@ -2258,7 +2384,10 @@ class StreamedShardedScan:
             lap("plot_allreduce", t)
         self.status = int(st.value)
         self.stats = {**self._base_stats, "rounds": n_rounds, "slice": slice_, "max_slice": ms, "candidates": nc,
-                      "queries_sent_to": sent_to}
+                      "queries_sent_to": sent_to, "spill": self.spill_stats()}
+        if self._host_lists and not self.symm_ok():
+            raise _lib.HetmersError(-2, f"rank {self.rank}: the streamed scan ended with a non-zero status word on some "
+                                        f"rank (here {self.status:#x}); its plot must not be used")
         return out
 
     def extract(self, pixmap, dst: int = 0, timings: dict | None = None):
@@ -2310,7 +2439,15 @@ class StreamedShardedScan:
                 self._pass1(lap)
             t = time.perf_counter()
             nc, ms = C.c_int64(), C.c_int64()
-            _lib.check(L.hm_rank_scan_extract_prepare(h, pm.ctypes.data, C.byref(nc), C.byref(ms)))
+            if self._host_lists:
+                err = None
+                try:
+                    _lib.check(L.hm_rank_scan_extract_prepare(h, pm.ctypes.data, C.byref(nc), C.byref(ms)))
+                except _lib.HetmersError as e:
+                    err = e
+                raise_on_any_rank(err, "preparing the pair listing", self._coll_dev, g)
+            else:
+                _lib.check(L.hm_rank_scan_extract_prepare(h, pm.ctypes.data, C.byref(nc), C.byref(ms)))
             lap("extract_prepare", t)
             n_rounds, slice_, sent_to = self._rounds(nc.value, ms.value, L.hm_rank_scan_extract_slices,
                                                      L.hm_rank_scan_extract_route, L.hm_rank_scan_extract_settle, lap)
@@ -2326,7 +2463,10 @@ class StreamedShardedScan:
         self.status = int(st.value)
         self.stats = {**self._base_stats, "rounds": n_rounds, "slice": slice_, "max_slice": ms.value,
                       "candidates": nc.value, "queries_sent_to": sent_to, "pass1_reused": reuse,
-                      "records": int(n.value)}
+                      "records": int(n.value), "spill": self.spill_stats()}
+        if self._host_lists and not self.symm_ok():
+            raise _lib.HetmersError(-2, f"rank {self.rank}: the routed pair listing ended with a non-zero status word on "
+                                        f"some rank (here {self.status:#x}); its records must not be used")
         if not self.symm_ok():
             raise RuntimeError(f"rank {self.rank}: the routed pair listing ended with a non-zero status word on some "
                                f"rank (here {self.status:#x}); its records must not be used")
